@@ -1,8 +1,8 @@
-"""bayesianoptimization_b200 - a B200-native GP-surrogate + acquisition engine that drops in
+"""bayesianoptimization_b200 - a H100-native GP-surrogate + acquisition engine that drops in
 behind ``bayes_opt.BayesianOptimization.suggest()`` and the ``bayes_opt.acquisition`` classes.
 
 Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI (x constraint probability) ->
-argmin/top-k, in hand-written sm_100a CUDA behind the C ABI declared in include/b200bo.h.
+argmin/top-k, in hand-written sm_90a CUDA behind the C ABI declared in include/b200bo.h.
 No CPU fallback: importing the compute classes without the built library raises ImportError.
 
 Two layers:

@@ -1,5 +1,5 @@
-"""Build the C-ABI CUDA library in-tree (nvcc, sm_100a only).  No JIT cache: the .so sits next
-to this file so it travels with the repository snapshot to the GPU box."""
+"""Build the C-ABI CUDA library in-tree (nvcc, sm_90a only).  No JIT cache: the .so sits next
+to this file, so an in-tree checkout is importable once built."""
 from __future__ import annotations
 
 import os
@@ -10,9 +10,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200bo.so")
 SOURCES = ["b200bo.cu"]
-HEADERS = ["common.cuh", "select.cuh", "tc_common.cuh", "potrf_block.cuh", "fit_kernels.cuh", "predict_kernels.cuh", "predict16.cuh", "predict_tc3.cuh", os.path.join("..", "..", "include", "b200bo.h")]
+HEADERS = ["common.cuh", "select.cuh", "tc_common.cuh", "potrf_block.cuh", "fit_kernels.cuh", "predict_kernels.cuh", "predict16.cuh", os.path.join("..", "..", "include", "b200bo.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-ldl",
 ]
 
@@ -26,7 +26,7 @@ def _stale() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu -> libb200bo.so for sm_100a.  Returns the library path."""
+    """Compile csrc/*.cu -> libb200bo.so for sm_90a.  Returns the library path."""
     if not force and not _stale():
         return LIB
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"

@@ -64,7 +64,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(
-            f"{LIB_PATH} is missing: the sm_100a CUDA library has not been built. Run "
+            f"{LIB_PATH} is missing: the sm_90a CUDA library has not been built. Run "
             "`python -c 'import __graft_entry__ as g; g.build()'` (needs nvcc). "
             "bayesianoptimization_b200 has no CPU fallback."
         )

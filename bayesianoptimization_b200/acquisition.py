@@ -2,7 +2,7 @@
 
 The reference's plugin point is ``BayesianOptimization(acquisition_function=...)``: a subclass of
 ``bayes_opt.acquisition.AcquisitionFunction`` controls ``_get_acq``, ``_random_sample_minimize`` and
-``_smart_minimize`` (R/bayes_opt/acquisition.py:171-219, :274-320, :322-420).  This module plugs the B200
+``_smart_minimize`` (R/bayes_opt/acquisition.py:171-219, :274-320, :322-420).  This module plugs the device
 engine in at exactly those three hooks and nothing else: the classes below ARE the reference's classes
 (``bayes_opt`` is imported, not restated - constructors, ``suggest``, decay schedules, parameter
 get/set, ConstantLiar's dummy bookkeeping, GPHedge's portfolio logic and every error message are
@@ -53,7 +53,7 @@ def _device_kind(obj):
 
 
 class DeviceHooks(abc.ABC):
-    """Mixin: the three hooks of the acquisition seam on the B200.  Must precede the reference class in
+    """Mixin: the three hooks of the acquisition seam on the GPU.  Must precede the reference class in
     the MRO.  (Derives from abc.ABC like bayes_opt's AcquisitionFunction so that both have the same
     instance layout: a live reference object can then be re-classed in place, see ``accelerate``.)"""
 

@@ -1,4 +1,4 @@
-// b200bo.cu - C ABI (include/b200bo.h) over the sm_100a kernels.  No CPU fallback: every
+// b200bo.cu - C ABI (include/b200bo.h) over the sm_90a kernels.  No CPU fallback: every
 // compute entry point needs a CUDA device and reports B200BO_ERR_CUDA without one.
 #include <atomic>
 #include <cmath>
@@ -20,11 +20,9 @@
 #include "fit_kernels.cuh"
 #include "predict_kernels.cuh"
 #include "predict16.cuh"
-#include "predict_tc3.cuh"
 
 using namespace b200bo;
 
-constexpr int kDefaultTcVariant = 4;  // fp32 mode: 4 = N = 256 per MMA + row-block pairs (measured 115.7 ms; 3 = un-paired 124.7; 2 = 128-wide pairs 120.6, same box)
 constexpr int kDefaultPredictWarps = 16;  // measured A/B (DESIGN.md 6): 550.1 ms vs 561.7 ms per 2^20 candidates at C3
 
 // ---------------------------------------------------------------------------------------
@@ -107,7 +105,7 @@ struct b200bo_gp {
     // small-batch path scratch (per GP) + work-unit tables (rebuilt when np changes)
     DevBuf s_ksm, s_partial, s_mupart, s_unit, s_rb, s_colsq;
     int s_np = 0, s_nunits = 0;
-    // fp32 mode: L^-1 as tf32 (hi,lo) UMMA operand images (built on first use after a fit)
+    // fp32 mode: L^-1 as tf32 (hi,lo) wgmma operand images (built on first use after a fit)
     DevBuf tc_linv;
     bool tc_valid = false;
     DevBuf cov_xc, cov_kst, cov_v, cov_c, cov_out, cov_mu;  // predict(return_cov=True) scratch
@@ -199,10 +197,6 @@ static int init_handle(b200bo_gp* gp) {
                             kPredictSmemBytesTc));
     CU(cudaFuncSetAttribute(predict_acq_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             kPredictSmemBytesTc));
-    CU(cudaFuncSetAttribute(predict_acq_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            kPredictSmemBytesTc2));
-    CU(cudaFuncSetAttribute(predict_acq_tc3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesTc3));
-    CU(cudaFuncSetAttribute(predict_acq_tc4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesTc4));
     CU(cudaFuncSetAttribute(small_trsv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmallTrsvSmemBytes));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -311,7 +305,9 @@ extern "C" int b200bo_gp_set_data(b200bo_gp* gp, const double* X, const double* 
     if (!gp || !X || !y) return set_err(B200BO_ERR_ARG, "NULL argument");
     if (n <= 0 || d <= 0 || d > B200BO_MAX_DIM)
         return set_err(B200BO_ERR_ARG, "bad shape n=%lld d=%d (d <= %d)", (long long)n, d, B200BO_MAX_DIM);
-    if (n > 46000) return set_err(B200BO_ERR_ARG, "n=%lld too large", (long long)n);
+    // five np x np fp64 matrices (K, L, L^-1, its transpose, workspace) + the fp32-mode images of L^-1:
+    // about 44 np^2 bytes, 64 GB at the limit - what an 80 GB H100 holds beside the candidate batches
+    if (n > 38000) return set_err(B200BO_ERR_ARG, "n=%lld too large (n <= 38000)", (long long)n);
     if (!gp->xform.empty() && (int)gp->xform.size() != d)
         return set_err(B200BO_ERR_ARG, "transform has %zu entries, d=%d", gp->xform.size(), d);
     CU(cudaSetDevice(gp->device));
@@ -937,7 +933,7 @@ static int ensure_small(b200bo_gp* gp) {
     return B200BO_OK;
 }
 
-// Cost model (microseconds, measured orders of magnitude on B200) choosing between the tiled
+// Cost model (microseconds, orders of magnitude) choosing between the tiled
 // persistent kernel and the small-batch path.  B200BO_SMALL_PATH=0/1 forces one of them.
 // B200BO_PATH_STABLE: the decision is taken for a nominal batch of one pass (SMC rows) whatever m is,
 // so an optimiser's f(x) and its finite-difference stencil always run through the same kernels.
@@ -960,7 +956,7 @@ static bool use_small_path(long long m, int np_max, int n_gps, int sm_count, int
 static int predict_impl(int precision) {
     const char* e = getenv("B200BO_PREDICT_IMPL");
     if (e && (e[0] == 'd' || e[0] == 'D') && (e[1] == 'f' || e[1] == 'F')) return PREDICT_IMPL_DFMA;
-    if (e && (e[0] == 't' || e[0] == 'T')) return PREDICT_IMPL_TF32;  // "tf32": fp32 mode on tcgen05
+    if (e && (e[0] == 't' || e[0] == 'T')) return PREDICT_IMPL_TF32;  // "tf32": fp32 mode on wgmma
     if (e && (e[0] == 'd' || e[0] == 'D')) return PREDICT_IMPL_DMMA;
     return precision == B200BO_PRECISION_FP32 ? PREDICT_IMPL_TF32 : PREDICT_IMPL_DMMA;
 }
@@ -1154,27 +1150,7 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
                 P.gp[g].linv_tc = spec->gps[g]->tc_linv.as<uint8_t>();
             }
             CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off tiling from the kernel time
-            const char* tv = getenv("B200BO_TC_VARIANT");  // "1": non-overlapped version, "2"/"3": see kDefaultTcVariant
-            const int variant = (tv && tv[0] >= '1' && tv[0] <= '4') ? tv[0] - '0' : kDefaultTcVariant;
-            if (dreg && (variant == 3 || variant == 4)) {
-                // N = 256 per MMA: candidate tiles of 256, two K* image buffers of np x 2 KiB per CTA
-                const long long nt3 = (m + T3N - 1) / T3N;
-                if (!(sm.resume || !sm.finish)) grid = (int)(nt3 < g0->sm_count ? nt3 : g0->sm_count);
-                P.scratch_stride = (long long)np_max * 512;
-                if ((rc = g0->pscratch.reserve(sizeof(double) * (size_t)P.scratch_stride * g0->sm_count))) return rc;
-                P.scratch = g0->pscratch.as<double>();
-                if (variant == 4)
-                    predict_acq_tc4_kernel<<<grid, TC2_NT, kPredictSmemBytesTc4, stream>>>(P);
-                else
-                    predict_acq_tc3_kernel<<<grid, TC2_NT, kPredictSmemBytesTc3, stream>>>(P);
-            } else if (dreg && variant != 1) {
-                // overlapped version: two K* image buffers per CTA
-                P.scratch_stride *= 2;
-                if (const char* dbg = getenv("B200BO_TC_DEBUG")) P.pad0 = atoi(dbg);
-                if ((rc = g0->pscratch.reserve(sizeof(double) * (size_t)P.scratch_stride * g0->sm_count))) return rc;
-                P.scratch = g0->pscratch.as<double>();
-                predict_acq_tc2_kernel<<<grid, TC2_NT, kPredictSmemBytesTc2, stream>>>(P);
-            } else if (dreg) {
+            if (dreg) {
                 predict_acq_tc_kernel<true><<<grid, PNT, kPredictSmemBytesTc, stream>>>(P);
             } else {
                 predict_acq_tc_kernel<false><<<grid, PNT, kPredictSmemBytesTc, stream>>>(P);

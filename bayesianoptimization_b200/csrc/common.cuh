@@ -1,4 +1,4 @@
-// common.cuh - shared device helpers for the b200bo kernels (sm_100a).
+// common.cuh - shared device helpers for the b200bo kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <math_constants.h>

@@ -33,7 +33,7 @@ struct GpDev {
     const double* alphav;  // [np]      alpha_, zero padded
     const double* ls;      // [d]       length scales (replicated when isotropic)
     const int* xform;      // [d] or nullptr
-    const uint8_t* linv_tc;  // fp32 mode: L^-1 as tf32 (hi,lo) UMMA operand images, or nullptr
+    const uint8_t* linv_tc;  // fp32 mode: L^-1 as tf32 (hi,lo) wgmma operand images, or nullptr
     int n, np, family, nu;
     double constv, y_mean, y_std, lb, ub;
     double prior;  // prior variance kernel_.diag(x*) = constv + WhiteKernel noise_level
@@ -143,7 +143,7 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
 constexpr int PA_CHUNK = 64;  // training rows per staged chunk
 
 // TC = false: K* written as fp64 [np][128] (operand of the fp64 GEMM variants).
-// TC = true : K* written as tf32 (hi, lo) pairs in the UMMA operand-image layout of tc_common.cuh
+// TC = true : K* written as tf32 (hi, lo) pairs in the wgmma operand-image layout of tc_common.cuh
 //             ([np/32][hi|lo][16 KiB], candidate = operand row, training index = K).
 template <bool DREG, int COV, bool TC>
 __device__ __forceinline__ void predict_phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
@@ -520,23 +520,23 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_kernel(const PredictParams
 }
 
 // =======================================================================================
-// fp32 mode: the same fused kernel with the N^2 term on the 5th-generation tensor cores.
-//   V = L^-1 K*^T as 3xTF32 (a_hi*b_hi + a_hi*b_lo + a_lo*b_hi), fp32 accumulators in TMEM.
+// fp32 mode: the same fused kernel with the N^2 term on the warpgroup tensor cores (wgmma).
+//   V = L^-1 K*^T as 3xTF32 (a_hi*b_hi + a_hi*b_lo + a_lo*b_hi), fp32 accumulators in registers.
 //   K* itself, K* alpha_ (the mean) and the whole epilogue stay fp64: only the triangular product
-//   and the sum of squares run at reduced precision (north_star tolerance for this mode: 1e-3).
-// Warp roles during the GEMM phase (one CTA per SM, 256 threads, TMEM 2 x 128 columns):
+//   and the sum of squares run at reduced precision (tolerance of this mode: 1e-3).
+// Warp roles during the GEMM phase (one CTA per SM, 256 threads):
 //   warp 0 / lane 0  producer: 1-D bulk async copies (TMA engine) of pre-tiled operand images
 //                    [A_hi|A_lo] (L^-1, tiled once at fit time) and [B_hi|B_lo] (written by phase A)
-//   warp 1 / lane 0  tcgen05.mma issuer: 4 k-steps x 3 products per 32-k stage, tcgen05.commit
-//                    releases the stage / publishes the accumulator
-//   warps 4..7       epilogue: tcgen05.ld of their TMEM quadrant, per-thread sum of squares
-// The operand images use the SWIZZLE_NONE K-major core-matrix layout, so a stage is a verbatim
+//                    into a ring of TC_STAGES shared-memory stages, completion on mbarriers
+//   warps 4..7       one warpgroup: per 32-k stage 4 k-steps x 3 products x 2 row halves of
+//                    wgmma.m64n128k8 into a 128 x 128 register accumulator; after each 128-row block
+//                    of L^-1 the per-column sums of squares of the accumulator
+// The operand images use the no-swizzle K-major core-matrix layout, so a stage is a verbatim
 // 64 KiB byte copy - no tensor map, no swizzle bookkeeping.
 // =======================================================================================
 constexpr int TC_STAGES = 3;
 constexpr int TC_STAGE_BYTES = 4 * tc::kTcImgBytes;                // A_hi, A_lo, B_hi, B_lo
 constexpr int kPredictSmemBytesTc = TC_STAGES * TC_STAGE_BYTES;    // 196608
-constexpr int TC_TMEM_COLS = 256;                                  // two 128-column accumulators
 
 template <bool DREG>
 __global__ void __launch_bounds__(PNT, 1) predict_acq_tc_kernel(const PredictParams P) {
@@ -545,8 +545,7 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_tc_kernel(const PredictPar
     __shared__ double base_s[PBN];
     __shared__ double prod_s[PBN];
     __shared__ double red_s[4][PBN];
-    __shared__ uint64_t full_bar[TC_STAGES], empty_bar[TC_STAGES], accfull_bar[2], accempty_bar[2];
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full_bar[TC_STAGES], empty_bar[TC_STAGES];
     __shared__ SelShared sel_s;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -561,23 +560,13 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_tc_kernel(const PredictPar
     if (tid == 0) {
         for (int s = 0; s < TC_STAGES; ++s) {
             tc::mbar_init(&full_bar[s], 1);
-            tc::mbar_init(&empty_bar[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            tc::mbar_init(&accfull_bar[b], 1);
-            tc::mbar_init(&accempty_bar[b], 4);
+            tc::mbar_init(&empty_bar[s], 4);  // one arrival per consumer warp
         }
         tc::mbar_fence_init();
     }
-    if (warp == 1) tc::tmem_alloc(&tmem_base_s, TC_TMEM_COLS);
-    tc::tc_fence_before_sync();
     __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem_base = tmem_base_s;
-    const uint32_t idesc = tc::umma_idesc_tf32(128, 128);
 
-    uint32_t stage_it = 0;  // stages filled / consumed so far (producer and MMA thread count alike)
-    uint32_t acc_it = 0;    // accumulator buffers produced / drained so far
+    uint32_t stage_it = 0;  // stages filled / consumed so far (producer and consumers count alike)
 
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const long long c0 = tile * PBN;
@@ -606,91 +595,75 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_tc_kernel(const PredictPar
                         }
                     }
                 }
-            } else if (warp == 1) {
-                if (lane == 0) {
-                    uint32_t it = stage_it, ai = acc_it;
-                    for (int ib = 0; ib < nb; ++ib, ++ai) {
-                        const int nkt = (ib + 1) * (PBM / tc::kTcK);
-                        const uint32_t buf = ai & 1;
-                        tc::mbar_wait(&accempty_bar[buf], ((ai >> 1) & 1) ^ 1);
-                        tc::tc_fence_after_sync();
-                        const uint32_t d_tmem = tmem_base + buf * 128;
-                        for (int kt = 0; kt < nkt; ++kt, ++it) {
-                            const int s = it % TC_STAGES;
-                            tc::mbar_wait(&full_bar[s], (it / TC_STAGES) & 1);
-                            tc::tc_fence_after_sync();
-                            const uint32_t base = tc::smem_u32(stage_mem + (size_t)s * TC_STAGE_BYTES);
+            } else if (warp >= 4) {
+                const int q = warp & 3;
+                // per-thread column sums of V^2: columns 8*i + 2*(lane%4) + e
+                float csq[32];
 #pragma unroll
-                            for (int j = 0; j < tc::kTcK / 8; ++j) {
-                                const uint32_t koff = j * 2 * tc::kTcLBO;
-                                const uint64_t a_hi = tc::umma_desc_kmajor_noswz(base + koff, tc::kTcLBO, tc::kTcSBO);
-                                const uint64_t a_lo = tc::umma_desc_kmajor_noswz(base + tc::kTcImgBytes + koff,
-                                                                                 tc::kTcLBO, tc::kTcSBO);
-                                const uint64_t b_hi = tc::umma_desc_kmajor_noswz(base + 2 * tc::kTcImgBytes + koff,
-                                                                                 tc::kTcLBO, tc::kTcSBO);
-                                const uint64_t b_lo = tc::umma_desc_kmajor_noswz(base + 3 * tc::kTcImgBytes + koff,
-                                                                                 tc::kTcLBO, tc::kTcSBO);
-                                tc::umma_tf32(d_tmem, a_hi, b_hi, idesc, (kt | j) ? 1u : 0u);
-                                tc::umma_tf32(d_tmem, a_hi, b_lo, idesc, 1u);
-                                tc::umma_tf32(d_tmem, a_lo, b_hi, idesc, 1u);
+                for (int j = 0; j < 32; ++j) csq[j] = 0.f;
+                uint32_t it = stage_it;
+                for (int ib = 0; ib < nb; ++ib) {
+                    const int nkt = (ib + 1) * (PBM / tc::kTcK);
+                    float acc[2][64];
+                    int pending = -1;  // stage whose MMAs may still be reading shared memory
+                    for (int kt = 0; kt < nkt; ++kt, ++it) {
+                        const int s = it % TC_STAGES;
+                        tc::mbar_wait(&full_bar[s], (it / TC_STAGES) & 1);
+                        const uint32_t base = tc::smem_u32(stage_mem + (size_t)s * TC_STAGE_BYTES);
+                        tc::wgmma_fence();
+#pragma unroll
+                        for (int j = 0; j < tc::kTcK / 8; ++j) {
+                            const uint32_t koff = j * 2 * tc::kTcLBO;
+                            const uint64_t b_hi = tc::wgmma_desc_kmajor_noswz(base + 2 * tc::kTcImgBytes + koff,
+                                                                              tc::kTcLBO, tc::kTcSBO);
+                            const uint64_t b_lo = tc::wgmma_desc_kmajor_noswz(base + 3 * tc::kTcImgBytes + koff,
+                                                                              tc::kTcLBO, tc::kTcSBO);
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {  // rows 64h .. 64h+63 of the block: 8 core matrices
+                                const uint32_t moff = h * 8 * tc::kTcSBO;
+                                const uint64_t a_hi = tc::wgmma_desc_kmajor_noswz(base + moff + koff, tc::kTcLBO,
+                                                                                  tc::kTcSBO);
+                                const uint64_t a_lo = tc::wgmma_desc_kmajor_noswz(
+                                    base + tc::kTcImgBytes + moff + koff, tc::kTcLBO, tc::kTcSBO);
+                                tc::wgmma_m64n128k8_tf32(acc[h], a_hi, b_hi, (kt | j) ? 1u : 0u);
+                                tc::wgmma_m64n128k8_tf32(acc[h], a_hi, b_lo, 1u);
+                                tc::wgmma_m64n128k8_tf32(acc[h], a_lo, b_hi, 1u);
                             }
-                            tc::umma_commit(&empty_bar[s]);
                         }
-                        tc::umma_commit(&accfull_bar[buf]);
-                    }
-                }
-            }
-            float csq[PBN];
-            if (warp >= 4) {
-                const int q = warp & 3;
-#pragma unroll
-                for (int j = 0; j < PBN; ++j) csq[j] = 0.f;
-                uint32_t ai = acc_it;
-                for (int ib = 0; ib < nb; ++ib, ++ai) {
-                    const uint32_t buf = ai & 1;
-                    tc::mbar_wait(&accfull_bar[buf], (ai >> 1) & 1);
-                    tc::tc_fence_after_sync();
-                    const uint32_t taddr = tmem_base + buf * 128 + ((uint32_t)(q * 32) << 16);
-#pragma unroll
-                    for (int cc = 0; cc < PBN; cc += 32) {
-                        uint32_t r[32];
-                        tc::tmem_ld_32x32(taddr + cc, r);
-                        tc::tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const float v = __uint_as_float(r[j]);
-                            csq[cc + j] = fmaf(v, v, csq[cc + j]);
+                        tc::wgmma_commit();
+                        // keep this stage's MMAs in flight; the previous stage's are complete -> release it
+                        tc::wgmma_wait<1>();
+                        if (pending >= 0) {
+                            __syncwarp();
+                            if (lane == 0) tc::mbar_arrive(&empty_bar[pending]);
                         }
+                        pending = s;
                     }
-                    tc::tc_fence_before_sync();
+                    tc::wgmma_wait<0>();
                     __syncwarp();
-                    if (lane == 0) tc::mbar_arrive(&accempty_bar[buf]);
-                }
-            }
-            // every role advanced by the same amounts
-            {
-                uint32_t stages = 0;
-                for (int ib = 0; ib < nb; ++ib) stages += (ib + 1) * (PBM / tc::kTcK);
-                stage_it += stages;
-                acc_it += nb;
-            }
-            tc::tc_fence_before_sync();
-            __syncthreads();
-            tc::tc_fence_after_sync();
-            if (warp >= 4) {
-                const int q = warp & 3;
-                // sum over the 32 rows (lanes) of this quadrant; fp64 from here on
+                    if (lane == 0) tc::mbar_arrive(&empty_bar[pending]);
 #pragma unroll
-                for (int j = 0; j < PBN; ++j) {
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int i = 0; i < 16; ++i)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const float v0 = acc[h][4 * i + e], v1 = acc[h][4 * i + 2 + e];
+                                csq[2 * i + e] = fmaf(v1, v1, fmaf(v0, v0, csq[2 * i + e]));
+                            }
+                }
+                // sum over the 16 rows of this warp held by lanes with equal lane%4; fp64 from here on
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
                     double v = (double)csq[j];
-                    v += __shfl_xor_sync(0xffffffffu, v, 16);
-                    v += __shfl_xor_sync(0xffffffffu, v, 8);
                     v += __shfl_xor_sync(0xffffffffu, v, 4);
-                    v += __shfl_xor_sync(0xffffffffu, v, 2);
-                    v += __shfl_xor_sync(0xffffffffu, v, 1);
-                    if (lane == 0) red_s[q][j] = v;
+                    v += __shfl_xor_sync(0xffffffffu, v, 8);
+                    v += __shfl_xor_sync(0xffffffffu, v, 16);
+                    if (lane < 4) red_s[q][8 * (j >> 1) + 2 * lane + (j & 1)] = v;
                 }
             }
+            // every role advanced by the same amount
+            for (int ib = 0; ib < nb; ++ib) stage_it += (ib + 1) * (PBM / tc::kTcK);
             __syncthreads();
             if (tid < PBN) {
                 const int c = tid;
@@ -705,351 +678,6 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_tc_kernel(const PredictPar
         }
     }
     if (P.sel_cta && tid < PBN) runsel_store(sel_s, P.sel_cta + blockIdx.x, tid);
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, TC_TMEM_COLS);
-}
-
-// ---------------------------------------------------------------------------------------
-// fp32 mode, overlapped version (d <= 16): the K* build of the NEXT job runs on four dedicated
-// builder warps while the tensor cores work on the current one, so the fp64 front end disappears
-// behind the GEMM.  512 threads = 4 warp groups:
-//   warps 0-3   producer (warp 0, one lane), tcgen05.mma issuer (warp 1, one lane), 2 spare
-//   warps 4-7   epilogue: tcgen05.ld of their TMEM quadrant, warp transpose-reduce of v^2 over the
-//               32 rows, cross-warp sum, per-candidate acquisition epilogue
-//   warps 8-15  builders: two threads per candidate; K* in fp64 -> tf32 (hi,lo) operand images in a
-//               double-buffered global scratch, K* alpha_ in fp64
-// A job is one (candidate tile, GP).  mbarriers: full/empty (smem stages), accfull/accempty (TMEM
-// buffers), b_ready[2] (builders -> producer/epilogue), job_done[2] (epilogue -> builders).
-// ---------------------------------------------------------------------------------------
-constexpr int TC2_NT = 512;       // 16 warps: 4 (producer, MMA, 2 spare) + 4 epilogue + 8 builders
-constexpr int TC2_NB = 256;       // builder threads: two per candidate column (row halves of every chunk)
-constexpr int kPredictSmemBytesTc2 = TC_STAGES * TC_STAGE_BYTES + 2 * PA_CHUNK * kPredictMaxDimRegs * 8;  // 212992
-
-template <int COV>
-__device__ __forceinline__ void tc2_build_job(const PredictParams& P, const GpDev& G, long long c0, int btid,
-                                              uint8_t* __restrict__ Bimg, double* xs_s, double* mu_out) {
-    const int d = P.d, np = G.np;
-    const int c = btid & (PBN - 1), half = btid >> 7;
-    double xc[kPredictMaxDimRegs];
-    {
-        const long long gi = c0 + c;
-#pragma unroll
-        for (int j = 0; j < kPredictMaxDimRegs; ++j) {
-            double v = 0.0;
-            if (j < d && gi < P.m) {
-                v = candidate_coord(P, gi, j);
-                if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-                v = v / G.ls[j];
-            }
-            xc[j] = v;
-        }
-    }
-    const int chunk_pieces = PA_CHUNK * d / 2;
-    auto load_chunk = [&](int buf, int ch) {
-        const double* src = G.Xs + (size_t)ch * PA_CHUNK * d;
-        double* dst = xs_s + (size_t)buf * PA_CHUNK * kPredictMaxDimRegs;
-        for (int q = btid; q < chunk_pieces; q += TC2_NB) cp_async16_cg(dst + 2 * q, src + 2 * q);
-    };
-    const int nch = np / PA_CHUNK;
-    load_chunk(0, 0);
-    cp_async_commit();
-    double mu_acc = 0.0;
-    constexpr int R = 8;
-    for (int ch = 0; ch < nch; ++ch) {
-        if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
-        cp_async_commit();
-        cp_async_wait<1>();
-        tc::named_bar_sync(2, TC2_NB);
-        const double* xs = xs_s + (size_t)(ch & 1) * PA_CHUNK * kPredictMaxDimRegs;
-        for (int r0 = half * (PA_CHUNK / 2); r0 < (half + 1) * (PA_CHUNK / 2); r0 += R) {
-            double r2[R];
-#pragma unroll
-            for (int q = 0; q < R; ++q) r2[q] = 0.0;
-            if ((d & 1) == 0) {
-#pragma unroll
-                for (int j = 0; j < kPredictMaxDimRegs; j += 2) {
-                    if (j < d) {
-#pragma unroll
-                        for (int q = 0; q < R; ++q) {
-                            const double2 xv = *reinterpret_cast<const double2*>(xs + (r0 + q) * d + j);
-                            const double d0 = xc[j] - xv.x, d1 = xc[j + 1] - xv.y;
-                            r2[q] = fma(d0, d0, r2[q]);
-                            r2[q] = fma(d1, d1, r2[q]);
-                        }
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < kPredictMaxDimRegs; ++j) {
-                    if (j < d) {
-#pragma unroll
-                        for (int q = 0; q < R; ++q) {
-                            const double df = xc[j] - xs[(r0 + q) * d + j];
-                            r2[q] = fma(df, df, r2[q]);
-                        }
-                    }
-                }
-            }
-            float hi[R], lo[R];
-#pragma unroll
-            for (int q = 0; q < R; ++q) {
-                const int n = ch * PA_CHUNK + r0 + q;
-                double kv = G.constv * cov_eval<COV>(r2[q]);
-                if (n >= G.n) kv = 0.0;
-                hi[q] = tc::to_tf32((float)kv);
-                lo[q] = tc::to_tf32((float)(kv - (double)hi[q]));
-                mu_acc = fma(__ldg(G.alphav + n), kv, mu_acc);
-            }
-            const int n0 = ch * PA_CHUNK + r0;
-            uint8_t* img = Bimg + (size_t)(n0 >> 5) * (2 * tc::kTcImgBytes);
-#pragma unroll
-            for (int h4 = 0; h4 < 2; ++h4) {
-                const int off = tc::tc_img_offset(c, (n0 & 31) + 4 * h4);
-                *reinterpret_cast<float4*>(img + off) =
-                    make_float4(hi[4 * h4], hi[4 * h4 + 1], hi[4 * h4 + 2], hi[4 * h4 + 3]);
-                *reinterpret_cast<float4*>(img + tc::kTcImgBytes + off) =
-                    make_float4(lo[4 * h4], lo[4 * h4 + 1], lo[4 * h4 + 2], lo[4 * h4 + 3]);
-            }
-        }
-        tc::named_bar_sync(2, TC2_NB);
-    }
-    cp_async_wait<0>();
-    *mu_out = mu_acc;
-}
-
-// Row blocks are processed in PAIRS against each K* stage (two TMEM accumulators per buffer), which
-// halves the HBM traffic of the K* images (their 0.6 GB working set cannot live in L2).  A stage
-// holds HALF a k-tile (16 k) of every operand image: [A(ib0) hi|lo][A(ib1) hi|lo][B hi|lo], 6 x 8 KiB;
-// four stages keep three loads in flight behind the MMAs (the 2-stage/32-k version was latency bound).
-constexpr int TC2_STAGES = 4;
-constexpr int TC2_HALF = tc::kTcImgBytes / 2;         // 8192: k 0..15 or 16..31 of an image
-constexpr int TC2_STAGE_BYTES = 6 * TC2_HALF;         // 49152
-constexpr int TC2_TMEM_COLS = 512;                    // 2 buffers x 2 row blocks x 128 columns
-static_assert(TC2_STAGES * TC2_STAGE_BYTES + 2 * PA_CHUNK * kPredictMaxDimRegs * 8 == kPredictSmemBytesTc2, "smem");
-
-__global__ void __launch_bounds__(TC2_NT, 1) predict_acq_tc2_kernel(const PredictParams P) {
-    extern __shared__ __align__(16) double smem[];
-    __shared__ double mu_s[2][2][PBN];  // [job parity][row half][candidate]
-    __shared__ float red_s[4][PBN];
-    __shared__ uint64_t full_bar[TC2_STAGES], empty_bar[TC2_STAGES], accfull_bar[2], accempty_bar[2];
-    __shared__ uint64_t bready_bar[2], jobdone_bar[2];
-    __shared__ uint32_t tmem_base_s;
-    __shared__ SelShared sel_s;
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    uint8_t* stage_mem = reinterpret_cast<uint8_t*>(smem);
-    double* xs_s = reinterpret_cast<double*>(stage_mem + TC2_STAGES * TC2_STAGE_BYTES);
-    uint8_t* scratch = reinterpret_cast<uint8_t*>(P.scratch + (long long)blockIdx.x * P.scratch_stride);
-    const size_t buf_bytes = (size_t)P.scratch_stride * 4;  // two buffers of scratch_stride*4 bytes each
-    const long long ntiles = (P.m + PBN - 1) / PBN;
-    const long long my_tiles = (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
-    const long long njobs = my_tiles * P.n_gps;
-    constexpr int KT_PER_BLOCK = PBM / tc::kTcK;  // 4 k-tiles per 128 rows
-    constexpr uint32_t IMG2 = 2 * tc::kTcImgBytes;
-
-    if (tid == 0) {
-        for (int s = 0; s < TC2_STAGES; ++s) {
-            tc::mbar_init(&full_bar[s], 1);
-            tc::mbar_init(&empty_bar[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            tc::mbar_init(&accfull_bar[b], 1);
-            tc::mbar_init(&accempty_bar[b], 4);
-            tc::mbar_init(&bready_bar[b], TC2_NB / 32);
-            tc::mbar_init(&jobdone_bar[b], 4);
-        }
-        tc::mbar_fence_init();
-    }
-    if (warp == 1) tc::tmem_alloc(&tmem_base_s, TC2_TMEM_COLS);
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    tc::tc_fence_after_sync();
-    const uint32_t tmem_base = tmem_base_s;
-
-    // measurement hooks (B200BO_TC_DEBUG): bit 0 = builders only, bit 1 = GEMM only (results invalid)
-    const bool dbg_no_gemm = (P.pad0 & 1) != 0, dbg_no_build = (P.pad0 & 2) != 0;
-    if (warp == 0) {
-        // ------------------------------ producer -------------------------------------------
-        if (lane == 0 && !dbg_no_gemm) {
-            uint32_t it = 0;
-            for (long long j = 0; j < njobs; ++j) {
-                const GpDev& G = P.gp[j % P.n_gps];
-                const int nb = G.np / PBM, nkt_row = G.np / tc::kTcK;
-                const uint8_t* Bimg = scratch + (size_t)(j & 1) * buf_bytes;
-                tc::mbar_wait(&bready_bar[j & 1], (uint32_t)((j >> 1) & 1));
-                for (int ib0 = 0; ib0 < nb; ib0 += 2) {
-                    const bool two = ib0 + 1 < nb;
-                    const int nkt0 = (ib0 + 1) * KT_PER_BLOCK, nkt = two ? nkt0 + KT_PER_BLOCK : nkt0;
-                    const uint8_t* A0 = G.linv_tc + (size_t)ib0 * nkt_row * IMG2;
-                    const uint8_t* A1 = A0 + (size_t)nkt_row * IMG2;
-                    for (int ht = 0; ht < 2 * nkt; ++ht, ++it) {
-                        const int kt = ht >> 1;
-                        const size_t hoff = (size_t)(ht & 1) * TC2_HALF;  // which 16-k half of the images
-                        const int s = it % TC2_STAGES;
-                        tc::mbar_wait(&empty_bar[s], ((it / TC2_STAGES) & 1) ^ 1);
-                        const bool a0 = kt < nkt0;
-                        tc::mbar_arrive_expect_tx(&full_bar[s], (1u + (a0 ? 1u : 0u) + (two ? 1u : 0u)) * 2u * TC2_HALF);
-                        uint8_t* dst = stage_mem + (size_t)s * TC2_STAGE_BYTES;
-                        const uint8_t* a0p = A0 + (size_t)kt * IMG2 + hoff;
-                        const uint8_t* a1p = A1 + (size_t)kt * IMG2 + hoff;
-                        const uint8_t* bp = Bimg + (size_t)kt * IMG2 + hoff;
-                        if (a0) {
-                            tc::bulk_g2s(dst, a0p, TC2_HALF, &full_bar[s]);
-                            tc::bulk_g2s(dst + TC2_HALF, a0p + tc::kTcImgBytes, TC2_HALF, &full_bar[s]);
-                        }
-                        if (two) {
-                            tc::bulk_g2s(dst + 2 * TC2_HALF, a1p, TC2_HALF, &full_bar[s]);
-                            tc::bulk_g2s(dst + 3 * TC2_HALF, a1p + tc::kTcImgBytes, TC2_HALF, &full_bar[s]);
-                        }
-                        tc::bulk_g2s(dst + 4 * TC2_HALF, bp, TC2_HALF, &full_bar[s]);
-                        tc::bulk_g2s(dst + 5 * TC2_HALF, bp + tc::kTcImgBytes, TC2_HALF, &full_bar[s]);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------ tcgen05.mma issuer ---------------------------------
-        if (lane == 0 && !dbg_no_gemm) {
-            const uint32_t idesc = tc::umma_idesc_tf32(128, 128);
-            uint32_t it = 0, ai = 0;
-            for (long long j = 0; j < njobs; ++j) {
-                const GpDev& G = P.gp[j % P.n_gps];
-                const int nb = G.np / PBM;
-                for (int ib0 = 0; ib0 < nb; ib0 += 2, ++ai) {
-                    const bool two = ib0 + 1 < nb;
-                    const int nkt0 = (ib0 + 1) * KT_PER_BLOCK, nkt = two ? nkt0 + KT_PER_BLOCK : nkt0;
-                    const uint32_t buf = ai & 1;
-                    tc::mbar_wait(&accempty_bar[buf], ((ai >> 1) & 1) ^ 1);
-                    tc::tc_fence_after_sync();
-                    const uint32_t d0 = tmem_base + buf * 256, d1 = d0 + 128;
-                    for (int ht = 0; ht < 2 * nkt; ++ht, ++it) {
-                        const int kt = ht >> 1;
-                        const int s = it % TC2_STAGES;
-                        tc::mbar_wait(&full_bar[s], (it / TC2_STAGES) & 1);
-                        tc::tc_fence_after_sync();
-                        const uint32_t base = tc::smem_u32(stage_mem + (size_t)s * TC2_STAGE_BYTES);
-                        const bool a0 = kt < nkt0;
-#pragma unroll
-                        for (int k8 = 0; k8 < 2; ++k8) {
-                            const uint32_t koff = k8 * 2 * tc::kTcLBO;
-                            const uint64_t b_hi = tc::umma_desc_kmajor_noswz(base + 4 * TC2_HALF + koff, tc::kTcLBO, tc::kTcSBO);
-                            const uint64_t b_lo = tc::umma_desc_kmajor_noswz(base + 5 * TC2_HALF + koff, tc::kTcLBO, tc::kTcSBO);
-                            if (a0) {
-                                const uint64_t a_hi = tc::umma_desc_kmajor_noswz(base + koff, tc::kTcLBO, tc::kTcSBO);
-                                const uint64_t a_lo = tc::umma_desc_kmajor_noswz(base + TC2_HALF + koff, tc::kTcLBO, tc::kTcSBO);
-                                tc::umma_tf32(d0, a_hi, b_hi, idesc, (ht | k8) ? 1u : 0u);
-                                tc::umma_tf32(d0, a_hi, b_lo, idesc, 1u);
-                                tc::umma_tf32(d0, a_lo, b_hi, idesc, 1u);
-                            }
-                            if (two) {
-                                const uint64_t a_hi = tc::umma_desc_kmajor_noswz(base + 2 * TC2_HALF + koff, tc::kTcLBO, tc::kTcSBO);
-                                const uint64_t a_lo = tc::umma_desc_kmajor_noswz(base + 3 * TC2_HALF + koff, tc::kTcLBO, tc::kTcSBO);
-                                tc::umma_tf32(d1, a_hi, b_hi, idesc, (ht | k8) ? 1u : 0u);
-                                tc::umma_tf32(d1, a_hi, b_lo, idesc, 1u);
-                                tc::umma_tf32(d1, a_lo, b_hi, idesc, 1u);
-                            }
-                        }
-                        tc::umma_commit(&empty_bar[s]);
-                    }
-                    tc::umma_commit(&accfull_bar[buf]);
-                }
-            }
-        }
-    } else if (warp >= 4 && warp < 8) {
-        // ------------------------------ epilogue --------------------------------------------
-        const int q = warp & 3, etid = tid - 128;
-        uint32_t ai = 0;
-        double base_neg = 0.0, prod = 1.0;
-        if (P.sel_cta) {
-            runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, etid);
-            tc::named_bar_sync(1, 128);
-        }
-        for (long long j = 0; j < njobs; ++j) {
-            const int g = (int)(j % P.n_gps);
-            const GpDev& G = P.gp[g];
-            const long long tile = blockIdx.x + (j / P.n_gps) * gridDim.x;
-            const int nb = G.np / PBM;
-            float csum[4] = {0.f, 0.f, 0.f, 0.f};  // columns lane, lane+32, lane+64, lane+96
-            for (int ib0 = 0; ib0 < nb && !dbg_no_gemm; ib0 += 2, ++ai) {
-                const bool two = ib0 + 1 < nb;
-                const uint32_t buf = ai & 1;
-                tc::mbar_wait(&accfull_bar[buf], (ai >> 1) & 1);
-                tc::tc_fence_after_sync();
-                const uint32_t taddr = tmem_base + buf * 256 + ((uint32_t)(q * 32) << 16);
-                const int nchunk = two ? 8 : 4;
-                for (int cc = 0; cc < nchunk; ++cc) {
-                    uint32_t r[32];
-                    tc::tmem_ld_32x32(taddr + cc * 32, r);
-                    tc::tmem_ld_wait();
-                    float v[32];
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const float x = __uint_as_float(r[i]);
-                        v[i] = x * x;
-                    }
-                    // warp transpose-reduce: afterwards lane L holds the sum over the 32 rows of column L
-#pragma unroll
-                    for (int s = 16; s >= 1; s >>= 1) {
-#pragma unroll
-                        for (int i = 0; i < s; ++i) {
-                            const bool up = (lane & s) != 0;
-                            const float send = up ? v[i] : v[i + s];
-                            const float recv = __shfl_xor_sync(0xffffffffu, send, s);
-                            v[i] = (up ? v[i + s] : v[i]) + recv;
-                        }
-                    }
-                    const int c4 = cc & 3;
-                    csum[0] += (c4 == 0) ? v[0] : 0.f;
-                    csum[1] += (c4 == 1) ? v[0] : 0.f;
-                    csum[2] += (c4 == 2) ? v[0] : 0.f;
-                    csum[3] += (c4 == 3) ? v[0] : 0.f;
-                }
-                tc::tc_fence_before_sync();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(&accempty_bar[buf]);
-            }
-#pragma unroll
-            for (int cc = 0; cc < 4; ++cc) red_s[q][cc * 32 + lane] = csum[cc];
-            tc::named_bar_sync(1, 128);
-            const double colsq =
-                (((double)red_s[0][etid] + (double)red_s[1][etid]) + (double)red_s[2][etid]) + (double)red_s[3][etid];
-            tc::mbar_wait(&bready_bar[j & 1], (uint32_t)((j >> 1) & 1));  // acquire the builders' mean
-            double val = 0.0;
-            candidate_epilogue(P, G, g, mu_s[j & 1][0][etid] + mu_s[j & 1][1][etid], colsq, tile * PBN + etid,
-                               base_neg, prod, &val);
-            if (P.sel_cta && g == P.n_gps - 1)
-                runsel_update<1>(sel_s, P.sel_k, etid, val, tile * PBN + etid + P.index_base, tile * PBN + etid < P.m);
-            tc::named_bar_sync(1, 128);
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&jobdone_bar[j & 1]);
-        }
-        if (P.sel_cta) runsel_store(sel_s, P.sel_cta + blockIdx.x, etid);
-    } else if (warp >= 8) {
-        // ------------------------------ builders ---------------------------------------------
-        const int btid = tid - 256;
-        for (long long j = 0; j < njobs; ++j) {
-            const int g = (int)(j % P.n_gps);
-            const GpDev& G = P.gp[g];
-            const long long tile = blockIdx.x + (j / P.n_gps) * gridDim.x;
-            tc::mbar_wait(&jobdone_bar[j & 1], (uint32_t)(((j >> 1) & 1) ^ 1));  // buffer j&1 free again
-            uint8_t* Bimg = scratch + (size_t)(j & 1) * buf_bytes;
-            double mu = 0.0;
-            if (!dbg_no_build) switch (cov_code(G.family, G.nu)) {
-                case 0: tc2_build_job<0>(P, G, tile * PBN, btid, Bimg, xs_s, &mu); break;
-                case 1: tc2_build_job<1>(P, G, tile * PBN, btid, Bimg, xs_s, &mu); break;
-                case 2: tc2_build_job<2>(P, G, tile * PBN, btid, Bimg, xs_s, &mu); break;
-                default: tc2_build_job<3>(P, G, tile * PBN, btid, Bimg, xs_s, &mu); break;
-            }
-            mu_s[j & 1][btid >> 7][btid & (PBN - 1)] = mu;
-            tc::fence_proxy_async_global();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&bready_bar[j & 1]);
-        }
-    }
-    tc::tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc(tmem_base, TC2_TMEM_COLS);
 }
 
 // L^-1 (fp64, row-major) -> tf32 (hi, lo) operand images [ib][kt][hi|lo][16 KiB] (lower k-tiles only)

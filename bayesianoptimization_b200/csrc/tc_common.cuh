@@ -1,8 +1,6 @@
-// tc_common.cuh - thin inline-PTX layer for the sm_100a tensor-core path: mbarriers, 1-D bulk
-// async copies (TMA engine, no tensor map), tcgen05 (UMMA) issue/commit, TMEM allocation and
-// tcgen05.ld.  Descriptor bit layouts follow the PTX ISA "tcgen05 shared memory descriptor" /
-// "instruction descriptor" tables (the same fields CUTLASS names UMMA::SmemDescriptor /
-// UMMA::InstrDescriptor).
+// tc_common.cuh - thin inline-PTX layer for the sm_90a tensor-core path: mbarriers, 1-D bulk
+// async copies (TMA engine, no tensor map) and wgmma issue/commit/wait.  The descriptor bit layout
+// follows the PTX ISA "matrix descriptor" table of the warpgroup-level MMA instructions.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -63,74 +61,47 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
 
-// ---- TMEM ----------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::);
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // same warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols));
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-
-// 32 lanes (this warp's TMEM quadrant) x 32 consecutive 32-bit columns -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-
-// ---- UMMA descriptors ------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand, SWIZZLE_NONE ("interleaved" core matrices):
-// a core matrix is 8 rows x 16 bytes stored as 128 contiguous bytes; SBO = byte distance between
-// core matrices adjacent in the M/N direction, LBO = between core matrices adjacent in K.
-__device__ __forceinline__ uint64_t umma_desc_kmajor_noswz(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                           uint32_t sbo_bytes) {
+// ---- wgmma (warpgroup MMA) ------------------------------------------------------------------
+// Shared-memory matrix descriptor, K-major operand, no swizzle ("interleaved" core matrices): a core
+// matrix is 8 rows x 16 bytes stored as 128 contiguous bytes; LBO = byte distance between core
+// matrices adjacent in K, SBO = between core matrices adjacent in the M/N direction.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_noswz(uint32_t smem_addr, uint32_t lbo_bytes,
+                                                            uint32_t sbo_bytes) {
     uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);    // [0,14)  start address >> 4
+    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);       // [0,14)  start address >> 4
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;  // [16,30) leading byte offset >> 4
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;  // [32,46) stride byte offset >> 4
-    d |= (uint64_t)1 << 46;                              // [46,48) descriptor version (sm_100)
-    return d;                                            // base_offset 0, lbo_mode 0, layout NONE
+    return d;                                           // base offset 0, layout type 0 (no swizzle)
 }
 
-// Instruction descriptor for kind::tf32, fp32 accumulate, A and B K-major, dense.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4)      // c_format  = F32
-           | (2u << 7)    // a_format  = TF32
-           | (2u << 10)   // b_format  = TF32
-           | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; one thread issues
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D(64x128, fp32 registers of the warpgroup) (+)= A(64x8 tf32, smem) * B(128x8 tf32, smem)^T.
+// Thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8*i + 2*(t%4) (+1):
+// d[4i + 0/1] = (row, col/col+1), d[4i + 2/3] = (row + 8, col/col+1), i = 0..15.
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc,
+                                                     uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued MMAs of this thread complete -> one arrival on the mbarrier
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-                 : "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
 // fp32 -> tf32 (round to nearest, ties away), result kept in a 32-bit container

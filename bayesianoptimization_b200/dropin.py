@@ -1,4 +1,4 @@
-"""``enable(optimizer)``: switch an existing ``bayes_opt.BayesianOptimization`` onto the B200 engine.
+"""``enable(optimizer)``: switch an existing ``bayes_opt.BayesianOptimization`` onto the device engine.
 The reference constructs its GP objects privately (R/bayes_opt/bayesian_optimization.py:124-130,
 R/bayes_opt/constraint.py:72-81) and offers no constructor injection, so the swap happens on the three
 attributes the hot path reads:
@@ -22,7 +22,7 @@ def accelerate_acquisition(acq, candidate_source=None):
 
 
 def enable(optimizer, device=0, devices=None, precision="fp64", candidate_source="host_rng"):
-    """Make ``optimizer.suggest()`` / ``maximize()`` / ``predict()`` run on the B200.
+    """Make ``optimizer.suggest()`` / ``maximize()`` / ``predict()`` run on the GPU.
 
     candidate_source  "host_rng" (default): the random candidates of every suggest() are the reference's own
                       MT19937 stream (parity mode); "device_philox": generated inside the fused kernel

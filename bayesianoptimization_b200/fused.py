@@ -2,7 +2,7 @@
 
 ``FusedAcquisition`` is what replaces the closure built by ``AcquisitionFunction._get_acq``
 (R/bayes_opt/acquisition.py:171-219): x (M,d)|(d,) -> (M,) values of  -base_acq(mu, sigma) [* p_constraint]
-evaluated for the whole batch by ONE fused sm_100a launch (``b200bo_acq_eval``), plus the selection
+evaluated for the whole batch by ONE fused sm_90a launch (``b200bo_acq_eval``), plus the selection
 step of ``_random_sample_minimize`` (:311-317) on the device (``b200bo_acq_argmin_topk``).  With more than
 one device (``B200GaussianProcessRegressor(devices=[...])``) the candidate rows are sharded over the
 replicas and the per-device (argmin, top-k) records are merged by one NCCL all-gather
@@ -42,7 +42,7 @@ class FusedAcquisition:
 
     kind      B.ACQ_UCB / ACQ_EI / ACQ_POI
     gp        fitted B200GaussianProcessRegressor (target)
-    constraint  object with .model (list of B200 GPs), .lb, .ub  (bayes_opt ConstraintModel) or None
+    constraint  object with .model (list of device GPs), .lb, .ub  (bayes_opt ConstraintModel) or None
     params    either fixed ``kappa``/``xi``/``y_max`` values or ``owner``: an acquisition object whose
               current kappa / xi / y_max are read at every call, as the reference closure does
               (it calls self.base_acq at call time, R/bayes_opt/acquisition.py:207,217).

@@ -2,10 +2,10 @@
 
 A subclass of sklearn's ``GaussianProcessRegressor`` (the object the reference constructs at
 R/bayes_opt/bayesian_optimization.py:124-130 and R/bayes_opt/constraint.py:72-81) whose
-``fit`` / ``predict`` / ``log_marginal_likelihood`` run on the B200 through the C ABI in
+``fit`` / ``predict`` / ``log_marginal_likelihood`` run on the GPU through the C ABI in
 ``include/b200bo.h``.  Host logic (hyper-parameter search driver, RNG consumption, attribute
 names, error types) mirrors SK/gaussian_process/_gpr.py so the reference's callers cannot tell
-the difference; every matrix operation runs in hand-written sm_100a kernels.  There is no CPU
+the difference; every matrix operation runs in hand-written sm_90a kernels.  There is no CPU
 fallback: unsupported kernels raise NotImplementedError, a missing CUDA library raises
 ImportError, a missing device raises B200Error.
 """
@@ -114,12 +114,12 @@ def _parse_base(k):
     if isinstance(k, Matern):  # also matches WrappedKernel subclasses of Matern
         if k.nu not in _NU_CODES:
             raise NotImplementedError(
-                f"Matern(nu={k.nu}) is not supported by the B200 engine (nu in 0.5, 1.5, 2.5, inf)")
+                f"Matern(nu={k.nu}) is not supported by the device engine (nu in 0.5, 1.5, 2.5, inf)")
         return B.KERNEL_MATERN, _NU_CODES[k.nu], k.length_scale, k.hyperparameter_length_scale.fixed
     if isinstance(k, RBF):
         return B.KERNEL_RBF, B.NU_INF, k.length_scale, k.hyperparameter_length_scale.fixed
     raise NotImplementedError(
-        f"kernel {type(k).__name__} is not supported by the B200 engine; supported: Matern, RBF, "
+        f"kernel {type(k).__name__} is not supported by the device engine; supported: Matern, RBF, "
         "optionally multiplied by a ConstantKernel, optionally wrapped by bayes_opt wrap_kernel")
 
 
@@ -133,7 +133,7 @@ def parse_kernel(kernel) -> EngineKernel:
             raise NotImplementedError("only {Matern, RBF}[* ConstantKernel] + WhiteKernel sums are supported")
         white, other, first = (k1, k2, True) if isinstance(k1, WhiteKernel) else (k2, k1, False)
         if isinstance(other, Sum):
-            raise NotImplementedError("nested kernel sums are not supported by the B200 engine")
+            raise NotImplementedError("nested kernel sums are not supported by the device engine")
         ek = parse_kernel(other)
         ek.noise = float(white.noise_level)
         ek.noise_free = not white.hyperparameter_noise_level.fixed
@@ -174,7 +174,7 @@ def probe_transform(kernel, d):
     if out.shape != probe.shape:
         raise NotImplementedError(
             "kernel input transform changes the dimension (categorical one-hot) - not supported "
-            "by the B200 engine yet")
+            "by the device engine yet")
     codes = np.zeros(d, dtype=np.int32)
     for j in range(d):
         if np.array_equal(out[:, j], probe[:, j]):
@@ -246,12 +246,12 @@ class _Handle:
 
 
 class B200GaussianProcessRegressor(GaussianProcessRegressor):
-    """GaussianProcessRegressor whose numerics run on a B200 (fp64).
+    """GaussianProcessRegressor whose numerics run on an H100 (fp64).
 
     Same constructor as sklearn's plus ``device`` (CUDA ordinal of the fit), ``devices`` (optional list of
     ordinals: the fitted state is replicated there and large acquisition batches / the L-BFGS-B seeds are
     sharded over them, SURVEY.md 8e) and ``precision``: "fp64" (exact,
-    parity 1e-5, default) or "fp32" (the N^2 term of predict on tcgen05 tensor cores as 3xTF32 with
+    parity 1e-5, default) or "fp32" (the N^2 term of predict on wgmma tensor cores as 3xTF32 with
     fp32 accumulation; fit, K*, the mean and the acquisition epilogue stay fp64; tolerance 1e-3).  ``fit`` mirrors
     SK/gaussian_process/_gpr.py:233-368 (incl. the 1 + n_restarts_optimizer L-BFGS-B runs and the
     exact RandomState draws at :328-333); ``predict`` mirrors :370-500 for return_std;
@@ -393,13 +393,13 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         if y.ndim == 2 and y.shape[1] == 1:
             y = y[:, 0]
         if y.ndim != 1:
-            raise NotImplementedError("multi-output targets are not supported by the B200 engine")
+            raise NotImplementedError("multi-output targets are not supported by the device engine")
         if X.shape[0] != y.shape[0]:
             raise ValueError("X and y have inconsistent numbers of samples")
         if not (np.all(np.isfinite(X)) and np.all(np.isfinite(y))):
             raise ValueError("Input contains NaN or infinity.")
         if np.iterable(self.alpha):
-            raise NotImplementedError("per-sample alpha is not supported by the B200 engine")
+            raise NotImplementedError("per-sample alpha is not supported by the device engine")
         self.n_features_in_ = X.shape[1]
         ek = parse_kernel(self.kernel_)  # raises NotImplementedError for unsupported kernels
         if ek.length_scale.size not in (1, X.shape[1]):

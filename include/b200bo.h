@@ -1,12 +1,12 @@
 /*
- * b200bo.h - C ABI of the B200-native GP-surrogate + acquisition engine.
+ * b200bo.h - C ABI of the H100-native GP-surrogate + acquisition engine.
  *
  * This is the drop-in boundary for ONE hot path of bayesian-optimization/BayesianOptimization
  * (v3.3.0): GP fit at given hyper-parameters -> batched posterior predict -> acquisition ->
  * argmin/top-k.  The reference has no FFI; its plugin surface is Python duck-typing on
  * sklearn's GaussianProcessRegressor and bayes_opt.acquisition.AcquisitionFunction
  * (SURVEY.md section 8b).  Every entry point below names the reference code it replaces
- * (R/ = /root/reference/, SK/ = site-packages/sklearn/).  INTEGRATION.md shows the ctypes
+ * (R/ = R/, SK/ = site-packages/sklearn/).  INTEGRATION.md shows the ctypes
  * binding a maintainer of the reference would add.
  *
  * Conventions
@@ -114,7 +114,7 @@ void b200bo_gp_destroy(b200bo_gp* gp);
 
 /* Arithmetic of the N^2 term (V = L^-1 K*^T and sum V^2) in the fused predict/acquisition kernel:
  *   B200BO_PRECISION_FP64  exact fp64 (mma.sync f64 / DFMA); parity bar 1e-5 (default)
- *   B200BO_PRECISION_FP32  "fp32 mode": 3xTF32 on tcgen05 tensor cores, fp32 accumulate in TMEM;
+ *   B200BO_PRECISION_FP32  "fp32 mode": 3xTF32 on wgmma tensor cores, fp32 accumulate in registers;
  *                          K*, the mean and the acquisition epilogue stay fp64; tolerance 1e-3.
  * A call uses the precision of gps[0].  (BASELINE configs[2]: fp32 vs fp64 tolerance.) */
 #define B200BO_PRECISION_FP64 0

@@ -8,13 +8,13 @@ It is the checker the CUDA path is compared with; it is never the product.  Only
 
 Pinning: the restatement is checked (tests/test_oracle_golden.py) against
   * fixtures in tests/golden/*.npz produced by ``oracle/make_golden.py`` from the UNMODIFIED
-    reference (``/root/reference/bayes_opt``) driving the live sklearn/scipy stack, and
+    reference (``R/bayes_opt``) driving the live sklearn/scipy stack, and
   * the live ``sklearn.gaussian_process.GaussianProcessRegressor`` (a dependency of the
-    reference that is installed in this image and on the GPU box).
+    reference that is installed in this image and on the GPU machine).
 The reference's own tests hold no golden vectors for K, L, alpha, mu, sigma or acquisition
 values (SURVEY.md section 8c) - the live computation is the oracle of record.
 
-Citations:  R/ = /root/reference/,  SK/ = site-packages/sklearn/,  SP/ = site-packages/scipy/.
+Citations:  R/ = R/,  SK/ = site-packages/sklearn/,  SP/ = site-packages/scipy/.
 """
 from __future__ import annotations
 

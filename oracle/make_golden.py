@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.npz from the UNMODIFIED reference + the live sklearn/scipy stack.
 
-Run in the build container only (needs /root/reference):
+Run in the build container only (needs the reference checkout):
 
-    PYTHONPATH=oracle/shims:/root/reference python oracle/make_golden.py
+    PYTHONPATH=oracle/shims:the reference checkout python oracle/make_golden.py
 
 The fixtures pin the oracle (oracle/gp_oracle.py) and, through it, the CUDA path.  Every value
 below comes out of reference code paths:

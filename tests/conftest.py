@@ -9,22 +9,16 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 
-# The reference package (bayes_opt) drives the drop-in tests.  It is vendored, unmodified, into the
-# git-ignored oracle/_ref by tools/vendor_ref.py (here, where /root/reference exists) and travels to the GPU
-# box with the snapshot; the product package imports `bayes_opt` from sys.path like any user environment.
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-try:
-    import vendor_ref
-
-    _REF = vendor_ref.vendor()
-except Exception:  # pragma: no cover
-    _REF = None
-if _REF and _REF not in sys.path:
+# The reference package (bayes_opt) drives the drop-in tests.  build() vendors it, unmodified, into the
+# git-ignored oracle/_ref (oracle/vendor_ref.py) when the reference checkout is available; the product package
+# imports `bayes_opt` from sys.path like any user environment.
+_REF = os.path.join(ROOT, "oracle", "_ref")
+if os.path.isdir(os.path.join(_REF, "bayes_opt")) and _REF not in sys.path:
     sys.path.insert(0, _REF)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 _NEEDS_REF = ("ExpectedImprovement", "UpperConfidenceBound", "ProbabilityOfImprovement", "ConstantLiar", "GPHedge",
@@ -43,8 +37,8 @@ def _skip_without_reference(items):
         pass
     import inspect
 
-    skip = pytest.mark.skip(reason="bayes_opt not importable: run tools/vendor_ref.py where /root/reference exists "
-                                   "(oracle/_ref ships with the repository snapshot)")
+    skip = pytest.mark.skip(reason="bayes_opt not importable: build() vendors it into oracle/_ref from the reference "
+                                   "checkout (oracle/vendor_ref.py)")
     for item in items:
         try:
             src = inspect.getsource(item.function)
@@ -90,5 +84,5 @@ def ref():
     try:
         import bayes_opt
     except ImportError:
-        pytest.skip("reference package bayes_opt not importable (run tools/vendor_ref.py where /root/reference exists)")
+        pytest.skip("reference package bayes_opt not importable (build() vendors it: oracle/vendor_ref.py)")
     return bayes_opt

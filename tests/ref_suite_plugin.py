@@ -2,10 +2,10 @@
 
     python -m pytest -p tests.ref_suite_plugin oracle/_ref/ref_tests
 
-The reference's tests (vendored, unmodified, into the git-ignored oracle/_ref/ref_tests by tools/vendor_ref.py)
+The reference's tests (vendored, unmodified, into the git-ignored oracle/_ref/ref_tests by oracle/vendor_ref.py)
 build their objects from three names: ``sklearn.gaussian_process.GaussianProcessRegressor``, the classes of
 ``bayes_opt.acquisition`` and ``bayes_opt.constraint.ConstraintModel``.  Before those modules are collected this
-plugin rebinds the names to the B200 classes (which ARE the reference's classes + the device hooks), so every
+plugin rebinds the names to the device classes (which ARE the reference's classes + the device hooks), so every
 ``acq.suggest(gp, target_space)``, ``BayesianOptimization.suggest()/maximize()``, ``ConstraintModel.predict`` of
 the reference's suite runs on the device, and the reference's own assertions judge the result.  Nothing under
 oracle/_ref is edited.  Used by tests/test_gpu_reference_suite.py (GPU) and, with B200BO_REF_SUITE_DRYRUN=1, by a

@@ -5,11 +5,11 @@ suggest()/register() side by side (R/bayes_opt/bayesian_optimization.py:323-333,
   * the caller-owned RandomState is in the SAME state (the hooks consume the stream exactly like the
     reference: restarts of gp.fit, the candidate batch, GPHedge's softmax draw),
   * theta* of the hyper-parameter fit agrees to optimiser tolerance (two-tier parity, SURVEY.md section 7),
-  * the B200 suggestion is the reference's suggestion to optimiser tolerance, and it is as good as the
+  * the device suggestion is the reference's suggestion to optimiser tolerance, and it is as good as the
     reference's under the REFERENCE's own acquisition closure (sklearn/scipy on the host).
 
 Both optimizers then register the reference's point, so the trajectories stay comparable.  The vendored
-package (oracle/_ref, tools/vendor_ref.py) is the unmodified reference."""
+package (oracle/_ref, oracle/vendor_ref.py) is the unmodified reference."""
 import warnings
 
 import numpy as np

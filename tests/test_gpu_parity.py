@@ -792,11 +792,13 @@ def test_mixed_int_space_round_transform_and_de_branch(bo, golden, TS):
     assert_allclose(sug, g["suggestion"], rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("variant", ["overlapped", "sequential", "n256", "n256pair"])
-@pytest.mark.parametrize("n,d,m", [(300, 4, 1000), (1024, 8, 20_000), (4096, 16, 40_000), (500, 20, 3000)])
-def test_fp32_mode_tcgen05_vs_oracle(bo, O, n, d, m, variant, monkeypatch):
-    """fp32 mode (precision="fp32"): the N^2 term on tcgen05 tensor cores (3xTF32, fp32 accumulate
-    in TMEM); K*, the mean and the epilogue stay fp64.  north_star tolerance for this mode: 1e-3
+@pytest.mark.parametrize("n,d,m", [(300, 4, 1000), (1024, 8, 20_000), (4096, 16, 40_000), (500, 20, 3000),
+                                   (128, 1, 500), (129, 2, 777), (640, 3, 5000), (2000, 24, 10_000),
+                                   (1500, 12, 4096), (3000, 16, 30_000), (700, 17, 2500), (256, 32, 4000),
+                                   (1200, 64, 1500), (2048, 10, 65_536), (900, 5, 129), (4100, 16, 20_000)])
+def test_fp32_mode_wgmma_vs_oracle(bo, O, n, d, m, monkeypatch):
+    """fp32 mode (precision="fp32"): the N^2 term on the wgmma tensor cores (3xTF32, fp32 accumulate
+    in registers); K*, the mean and the epilogue stay fp64.  Tolerance for this mode: 1e-3
     relative, stated on the quantity the reduced precision touches - the predictive VARIANCE:
     |d var| <= 1e-3*var + 1e-4*s_y^2 (sigma^2 is a difference of O(1) numbers; SURVEY section 7)."""
     X, y = _synth(n, d)
@@ -809,7 +811,6 @@ def test_fp32_mode_tcgen05_vs_oracle(bo, O, n, d, m, variant, monkeypatch):
     a.y_max = float(y.max())
     f = a._get_acq(gp=gp)
     monkeypatch.setenv("B200BO_SMALL_PATH", "0")
-    monkeypatch.setenv("B200BO_TC_VARIANT", {"sequential": "1", "overlapped": "2", "n256": "3", "n256pair": "4"}[variant])
     mu, sd = gp.predict(xt, return_std=True)
     ys = f(xt)
     idx, val, top = f.argmin_topk(xt, 10)

@@ -2,7 +2,7 @@
 test_bayesian_optimization.py, test_target_space.py, test_seq_domain_red.py, test_parameter.py, test_util.py and
 test_logger.py of the reference (everything but the notebook runner) - vendored unmodified
 into the git-ignored oracle/_ref/ref_tests - collected with tests/ref_suite_plugin.py, which rebinds
-GaussianProcessRegressor, the bayes_opt.acquisition classes and ConstraintModel to the B200 classes.  Every
+GaussianProcessRegressor, the bayes_opt.acquisition classes and ConstraintModel to the device classes.  Every
 suggest()/maximize()/predict() of that suite then runs on the device; the assertions are the reference's."""
 import os
 import re
@@ -16,7 +16,7 @@ pytestmark = pytest.mark.gpu
 
 def test_reference_test_suite_passes_on_the_drop_in():
     if not os.path.isdir(SUITE):
-        pytest.skip("reference tests not vendored (tools/vendor_ref.py needs /root/reference)")
+        pytest.skip("reference tests not vendored (oracle/vendor_ref.py needs the reference checkout)")
     r = run_reference_suite(("--tb=short",))
     tail = r.stdout[-6000:]
     m = re.search(r"(\d+) passed", r.stdout)

@@ -44,7 +44,7 @@ def _np_select(ys, k):
 
 
 @pytest.mark.parametrize("precision", ["fp64", "fp32"])
-@pytest.mark.parametrize("m,k", [(129, 5), (5000, 10), (148 * 128 * 3 + 77, 64), (40_000, 1)])
+@pytest.mark.parametrize("m,k", [(129, 5), (5000, 10), (132 * 128 * 3 + 77, 64), (40_000, 1)])
 def test_fused_selection_equals_numpy_on_the_same_values(bo, monkeypatch, precision, m, k):
     """argmin/top-k from the running per-CTA lists + k-way merge == np.argmin / stable argsort of the values
     the same kernel writes when asked to materialise them (ties, many CTAs, k up to 64)."""

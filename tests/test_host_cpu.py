@@ -218,7 +218,7 @@ def test_acq_min_machinery_on_analytic_bowl(bo, ref):
 
 
 def test_constraint_model_host_logic(bo, ref):
-    """The device ConstraintModel IS the reference's class with B200 GPs inside."""
+    """The device ConstraintModel IS the reference's class with device GPs inside."""
     assert issubclass(bo.ConstraintModel, ref.constraint.ConstraintModel)
     cm = bo.ConstraintModel(lambda x: x, np.array([-1.0, 0.0]), np.array([1.0, 2.0]))
     assert len(cm.model) == 2

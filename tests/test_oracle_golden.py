@@ -111,7 +111,7 @@ def test_c4s_constrained(golden):
     (ConstantKernel(1.7) * RBF(length_scale=1.1), dict(kind=O.KIND_RBF, length_scale=1.1, const=1.7)),
 ])
 def test_oracle_vs_live_sklearn(kern, kw):
-    """Runs anywhere sklearn is installed (this image, incl. the GPU box)."""
+    """Runs anywhere sklearn is installed (this image, incl. the GPU machine)."""
     rs = np.random.RandomState(11)
     X = rs.uniform(size=(200, 6))
     y = np.cos(X.sum(1)) + 0.05 * rs.randn(200)
