@@ -6,10 +6,11 @@ argmin/top-k, in hand-written sm_90a CUDA behind the C ABI declared in include/b
 No CPU fallback: importing the compute classes without the built library raises ImportError.
 
 Two layers:
-  * GP seam / C ABI (needs numpy, scipy, sklearn):  B200GaussianProcessRegressor, FusedAcquisition
+  * GP seam / C ABI (needs numpy, scipy, sklearn):  B200GaussianProcessRegressor, FusedAcquisition,
+    PosteriorPaths (posterior sample paths, resolved lazily)
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
-    UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ConstantLiar, GPHedge,
-    AcquisitionFunction, ConstraintModel, enable(optimizer) - resolved lazily on first access.
+    UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ThompsonSampling, ConstantLiar,
+    GPHedge, AcquisitionFunction, ConstraintModel, enable(optimizer) - resolved lazily on first access.
 """
 from . import _lib
 from ._build import build_library
@@ -23,7 +24,7 @@ _PLUGIN = {
     "AcquisitionFunction": "acquisition", "UpperConfidenceBound": "acquisition",
     "ExpectedImprovement": "acquisition", "ProbabilityOfImprovement": "acquisition",
     "ConstantLiar": "acquisition", "GPHedge": "acquisition", "DeviceHooks": "acquisition",
-    "ConstraintModel": "constraint",
+    "ThompsonSampling": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths",
 }
 
 

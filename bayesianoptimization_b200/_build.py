@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200bo.so")
 SOURCES = ["b200bo.cu"]
-HEADERS = ["common.cuh", "select.cuh", "tc_common.cuh", "potrf_block.cuh", "fit_kernels.cuh", "predict_kernels.cuh", "predict16.cuh", os.path.join("..", "..", "include", "b200bo.h")]
+HEADERS = ["common.cuh", "select.cuh", "tc_common.cuh", "potrf_block.cuh", "fit_kernels.cuh", "predict_kernels.cuh", "predict16.cuh", "paths.cuh", os.path.join("..", "..", "include", "b200bo.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-ldl",

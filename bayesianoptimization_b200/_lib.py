@@ -14,7 +14,7 @@ OK, ERR_CUDA, ERR_ARG, ERR_NOT_PD, ERR_UNSUPPORTED, ERR_STATE = 0, -1, -2, -3, -
 KERNEL_MATERN, KERNEL_RBF = 0, 1
 NU_05, NU_15, NU_25, NU_INF = 0, 1, 2, 3
 ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE = 0, 1, 2, 3
-MAX_GPS, MAX_DIM, MAX_TOPK = 8, 64, 64
+MAX_GPS, MAX_DIM, MAX_TOPK, MAX_PATHS = 8, 64, 64, 16
 XFORM_IDENTITY, XFORM_ROUND = 0, 1
 GET_L, GET_ALPHA, GET_YSTATS, GET_K, GET_LINV = 0, 1, 2, 3, 4
 PRECISION_FP64, PRECISION_FP32 = 0, 1
@@ -30,6 +30,8 @@ EXPORTS = [
     "b200bo_acq_argmin_topk_philox", "b200bo_acq_select_philox_dev", "b200bo_philox_rows",
     "b200bo_gp_replicate", "b200bo_multi_gpu_acq_argmin_topk", "b200bo_multi_gpu_acq_argmin_topk_philox",
     "b200bo_multi_gpu_acq_eval",
+    "b200bo_paths_create", "b200bo_paths_destroy", "b200bo_paths_eval", "b200bo_paths_argmin_topk",
+    "b200bo_paths_argmin_topk_philox",
 ]
 
 
@@ -111,6 +113,13 @@ def lib():
     L.b200bo_multi_gpu_acq_argmin_topk_philox.argtypes = [C.POINTER(AcqSpec), C.c_int, C.c_uint64, dp, dp,
                                                           C.c_int64, C.c_int64, C.c_int, *philox_outs]
     L.b200bo_multi_gpu_acq_eval.argtypes = [C.POINTER(AcqSpec), C.c_int, dp, C.c_int64, i64p, dp]
+    L.b200bo_paths_create.argtypes = [C.c_void_p, C.c_int, C.c_int, dp, dp, dp, dp, C.POINTER(C.c_void_p)]
+    L.b200bo_paths_destroy.argtypes = [C.c_void_p]
+    L.b200bo_paths_destroy.restype = None
+    L.b200bo_paths_eval.argtypes = [C.c_void_p, dp, C.c_int64, dp]
+    L.b200bo_paths_argmin_topk.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int, dp, i64p, dp, i64p]
+    L.b200bo_paths_argmin_topk_philox.argtypes = [C.c_void_p, C.c_uint64, dp, dp, C.c_int64, C.c_int64, C.c_int,
+                                                  *philox_outs]
     _lib = L
     return L
 

@@ -15,6 +15,9 @@ inherited), with ``DeviceHooks`` mixed in:
                               (mixed-integer spaces: the reference's own DE branch, unchanged, calling
                               the device closure)
 
+``ThompsonSampling`` is the one policy defined here rather than inherited: a posterior sample path per
+``suggest()``, ranked and refined through the same three hooks.
+
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
 (gpr.B200GaussianProcessRegressor), ``fused.FusedAcquisition`` and the C ABI do not need it.
 """
@@ -26,6 +29,8 @@ import numpy as np
 
 try:
     from bayes_opt import acquisition as _ref
+    from bayes_opt.exception import ConstraintNotSupportedError as _ConstraintNotSupportedError
+    from bayes_opt.util import ensure_rng as _ensure_rng
 except ImportError as e:  # pragma: no cover - depends on the environment
     raise ImportError(
         "bayesianoptimization_b200.acquisition plugs into the bayes_opt package "
@@ -52,6 +57,13 @@ def _device_kind(obj):
     return None
 
 
+def _device_closure(acq):
+    """True for closures that select and refine on the device: they map (M,d) -> (M,) and offer
+    ``argmin_topk`` and ``argmin_topk_philox`` (optionally ``refine_mode``) - FusedAcquisition and the
+    Thompson-sampling path closure (paths.PathAcquisition)."""
+    return callable(getattr(acq, "argmin_topk", None)) and callable(getattr(acq, "argmin_topk_philox", None))
+
+
 class DeviceHooks(abc.ABC):
     """Mixin: the three hooks of the acquisition seam on the GPU.  Must precede the reference class in
     the MRO.  (Derives from abc.ABC like bayes_opt's AcquisitionFunction so that both have the same
@@ -72,7 +84,7 @@ class DeviceHooks(abc.ABC):
     b200_candidate_source = "host_rng"
 
     def _random_sample_minimize(self, acq, space, random_state, n_random, n_x_seeds=0):
-        if n_random == 0 or not isinstance(acq, FusedAcquisition) or n_x_seeds > B.MAX_TOPK:
+        if n_random == 0 or not _device_closure(acq) or n_x_seeds > B.MAX_TOPK:
             # (n_smart beyond the device's top-k capacity: evaluate on the device, select with numpy)
             return super()._random_sample_minimize(acq, space, random_state, n_random, n_x_seeds)
         if self.b200_candidate_source == "device_philox" and all(space.continuous_dimensions):
@@ -84,8 +96,8 @@ class DeviceHooks(abc.ABC):
         return x_tries[idx], min_acq, (x_tries[top] if n_x_seeds != 0 else [])
 
     def _smart_minimize(self, acq, space, x_seeds, random_state):
-        batched = isinstance(acq, FusedAcquisition) or getattr(acq, "b200_vectorized", False)
-        refine = acq.refine_mode() if isinstance(acq, FusedAcquisition) else _null()
+        batched = _device_closure(acq) or getattr(acq, "b200_vectorized", False)
+        refine = acq.refine_mode() if _device_closure(acq) and hasattr(acq, "refine_mode") else _null()
         with refine:
             if not batched or len(x_seeds) == 0 or not all(space.continuous_dimensions):
                 return super()._smart_minimize(acq, space, x_seeds, random_state)
@@ -118,6 +130,55 @@ class ProbabilityOfImprovement(DeviceHooks, _ref.ProbabilityOfImprovement):
 
 class ExpectedImprovement(DeviceHooks, _ref.ExpectedImprovement):
     """bayes_opt.acquisition.ExpectedImprovement with the device hooks."""
+
+
+class ThompsonSampling(DeviceHooks, _ref.AcquisitionFunction):
+    """Thompson sampling: every ``suggest()`` draws ONE function from the GP posterior and proposes its maximiser.
+
+    The function is a posterior sample path (``B200GaussianProcessRegressor.sample_paths``, n_paths=1) drawn from
+    the RandomState ``suggest`` receives, before the random candidates are drawn from it.  A path is a fixed smooth
+    function, so the random stage ranks it on the device and the L-BFGS-B refinement runs on it like on any other
+    closure.  The reference ships no such class (its tutorial's version samples multivariate_normal(mean, cov) on
+    the host, which is O(M^3) in the candidates and drops the refinement).
+
+    n_features  random Fourier features of the prior part of each path (the data update is exact).
+    Constraints are not supported (ConstraintNotSupportedError)."""
+
+    def __init__(self, n_features=4096, random_state=None):
+        super().__init__(random_state=random_state)
+        if isinstance(n_features, bool) or not isinstance(n_features, (int, np.integer)) or n_features < 1:
+            raise ValueError(f"n_features must be a positive integer, got {n_features!r}")
+        self.n_features = int(n_features)
+        self._path_rng = None
+
+    def base_acq(self, *args, **kwargs):
+        raise NotImplementedError(
+            "ThompsonSampling has no base_acq(mean, std): it ranks candidates by one posterior sample path drawn "
+            "per suggest() (B200GaussianProcessRegressor.sample_paths), not by a formula of mean and std")
+
+    def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        # the path of this call is drawn from the caller's stream: remember it for _get_acq
+        self._path_rng = _ensure_rng(random_state)
+        try:
+            return super().suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
+                                   random_state=self._path_rng)
+        finally:
+            self._path_rng = None
+
+    def _get_acq(self, gp, constraint=None):
+        if constraint is not None:
+            raise _ConstraintNotSupportedError(
+                f"{type(self).__name__} does not support constrained optimization: a constraint model was given")
+        from .paths import PathAcquisition
+
+        rs = self._path_rng if self._path_rng is not None else _ensure_rng(None)
+        return PathAcquisition(_as_b200_gp(gp).sample_paths(1, self.n_features, random_state=rs))
+
+    def get_acquisition_params(self):
+        return {"n_features": self.n_features}
+
+    def set_acquisition_params(self, params):
+        self.n_features = int(params["n_features"])
 
 
 _HOOKED = {
@@ -168,6 +229,7 @@ class GPHedge(_ref.GPHedge):
 # isinstance(x, b200.AcquisitionFunction) holds for every acquisition of this module, as
 # isinstance(x, bayes_opt.acquisition.AcquisitionFunction) does in the reference (abc virtual subclasses:
 # the concrete classes keep the reference's MRO).
-for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, ConstantLiar, GPHedge):
+for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, ConstantLiar, GPHedge,
+             ThompsonSampling):
     AcquisitionFunction.register(_cls)
 del _cls

@@ -18,6 +18,7 @@
 #include <nvtx3/nvToolsExt.h>
 
 #include "fit_kernels.cuh"
+#include "paths.cuh"
 #include "predict_kernels.cuh"
 #include "predict16.cuh"
 
@@ -84,6 +85,28 @@ struct DevBuf {
     }
 };
 
+// Streamed upload of a host candidate matrix: chunk i+1 goes up on `copy` while chunk i is evaluated on `exec`
+// (double-buffered device chunks, ordered by events).  Shared by the acquisition and the sample-path entry points.
+struct ChunkedUpload {
+    cudaStream_t copy = nullptr, exec = nullptr;
+    cudaEvent_t up[2] = {nullptr, nullptr}, done[2] = {nullptr, nullptr};
+    int ensure();
+    void release() {
+        if (copy) cudaStreamDestroy(copy);
+        if (exec) cudaStreamDestroy(exec);
+        for (int i = 0; i < 2; ++i) {
+            if (up[i]) cudaEventDestroy(up[i]);
+            if (done[i]) cudaEventDestroy(done[i]);
+        }
+        copy = exec = nullptr;
+        up[0] = up[1] = done[0] = done[1] = nullptr;
+    }
+    // launch(d_chunk, rows, first_row, chunk_number, is_last) issues the work of one chunk on `exec`;
+    // buf: two device buffers of chunk x d doubles.  Returns with the work enqueued, not finished.
+    template <class Launch>
+    int run(const double* Xc, long long m, int d, long long chunk, double* const buf[2], Launch launch);
+};
+
 struct b200bo_gp {
     int device = 0;
     int sm_count = 0;
@@ -122,8 +145,7 @@ struct b200bo_gp {
     unsigned long long fgraph_key[16] = {0};
     long long fgraph_nodes = 0;
     // streamed host batches: copy / execute streams and the double-buffer events
-    cudaStream_t copy_stream = nullptr, exec_stream = nullptr;
-    cudaEvent_t chunk_up[2] = {nullptr, nullptr}, chunk_done[2] = {nullptr, nullptr};
+    ChunkedUpload upload;
     int precision = B200BO_PRECISION_FP64;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     // fit-side work (set_data / fit / lml) of this handle is issued on this stream: the legacy default
@@ -246,12 +268,7 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
     if (gp->bulk_stream) cudaStreamDestroy(gp->bulk_stream);
     if (gp->ev_chain) cudaEventDestroy(gp->ev_chain);
     if (gp->ev_bulk) cudaEventDestroy(gp->ev_bulk);
-    if (gp->copy_stream) cudaStreamDestroy(gp->copy_stream);
-    if (gp->exec_stream) cudaStreamDestroy(gp->exec_stream);
-    for (int i = 0; i < 2; ++i) {
-        if (gp->chunk_up[i]) cudaEventDestroy(gp->chunk_up[i]);
-        if (gp->chunk_done[i]) cudaEventDestroy(gp->chunk_done[i]);
-    }
+    gp->upload.release();
     if (gp->ev0) cudaEventDestroy(gp->ev0);
     if (gp->ev1) cudaEventDestroy(gp->ev1);
     if (g_last_timed == gp) g_last_timed = nullptr;
@@ -663,15 +680,12 @@ static int transpose_W(b200bo_gp* gp) {
     return B200BO_OK;
 }
 
-// alpha_ = K^-1 y via the explicit inverse factors + one step of iterative refinement
-static int solve_alpha(b200bo_gp* gp) {
+// a = K^-1 y via the explicit inverse factors + one step of iterative refinement.  y, a: np entries (y zero
+// padded); v1, v2: np-entry scratch.  alpha_ (solve_alpha) and the per-path solves of b200bo_paths_create.
+static int solve_spd(b200bo_gp* gp, const double* y, double* a, double* v1, double* v2) {
     const int np = gp->np;
     const int wpb = 8;  // warps per block
     dim3 blk(32 * wpb), grd((np + wpb - 1) / wpb);
-    double* a = gp->alphav.as<double>();
-    double* v1 = gp->v1.as<double>();
-    double* v2 = gp->v2.as<double>();
-    const double* y = gp->y.as<double>();
     // z = W y ; a = W^T z
     gemv_rows_kernel<<<grd, blk, 0, g_st>>>(gp->W.as<double>(), np, y, v1, np, np, 1);
     gemv_rows_kernel<<<grd, blk, 0, g_st>>>(gp->WT.as<double>(), np, v1, a, np, np, 2);
@@ -684,6 +698,11 @@ static int solve_alpha(b200bo_gp* gp) {
     for (int i = 0; i < 7; ++i) LAUNCHED();
     CU(cudaGetLastError());
     return B200BO_OK;
+}
+
+// alpha_ = K^-1 y
+static int solve_alpha(b200bo_gp* gp) {
+    return solve_spd(gp, gp->y.as<double>(), gp->alphav.as<double>(), gp->v1.as<double>(), gp->v2.as<double>());
 }
 
 extern "C" int b200bo_gp_fit(b200bo_gp* gp, const double* X, const double* y, int64_t n, int d,
@@ -1228,14 +1247,30 @@ extern "C" int b200bo_last_kernel_ms(float* ms) {
 // from launch to launch and are merged once - the H2D copy disappears behind the kernel.
 constexpr long long kChunkTilesPerSm = 8;
 
-static int ensure_copy_stream(b200bo_gp* g0) {
-    if (!g0->copy_stream) {
-        CU(cudaStreamCreateWithFlags(&g0->copy_stream, cudaStreamNonBlocking));
-        CU(cudaStreamCreateWithFlags(&g0->exec_stream, cudaStreamNonBlocking));
+int ChunkedUpload::ensure() {
+    if (!copy) {
+        CU(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+        CU(cudaStreamCreateWithFlags(&exec, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
-            CU(cudaEventCreateWithFlags(&g0->chunk_up[i], cudaEventDisableTiming));
-            CU(cudaEventCreateWithFlags(&g0->chunk_done[i], cudaEventDisableTiming));
+            CU(cudaEventCreateWithFlags(&up[i], cudaEventDisableTiming));
+            CU(cudaEventCreateWithFlags(&done[i], cudaEventDisableTiming));
         }
+    }
+    return B200BO_OK;
+}
+
+template <class Launch>
+int ChunkedUpload::run(const double* Xc, long long m, int d, long long chunk, double* const buf[2], Launch launch) {
+    int rc, i = 0;
+    for (long long c0 = 0; c0 < m; c0 += chunk, ++i) {
+        const long long mc = (m - c0) < chunk ? (m - c0) : chunk;
+        const int b = i & 1;
+        if (i >= 2) CU(cudaStreamWaitEvent(copy, done[b], 0));  // buffer b consumed
+        CU(cudaMemcpyAsync(buf[b], Xc + (size_t)c0 * d, sizeof(double) * (size_t)mc * d, cudaMemcpyHostToDevice, copy));
+        CU(cudaEventRecord(up[b], copy));
+        CU(cudaStreamWaitEvent(exec, up[b], 0));
+        if ((rc = launch(buf[b], mc, c0, i, c0 + chunk >= m))) return rc;
+        CU(cudaEventRecord(done[b], exec));
     }
     return B200BO_OK;
 }
@@ -1251,31 +1286,23 @@ static int check_nonfinite(b200bo_gp* g0) {
 static int run_host_chunked(const b200bo_acq* spec, const double* Xc, int64_t m, int k, SelRecord* sel_host) {
     b200bo_gp* g0 = spec->gps[0];
     int rc;
-    if ((rc = ensure_copy_stream(g0))) return rc;
+    ChunkedUpload& U = g0->upload;
+    if ((rc = U.ensure())) return rc;
     const int d = g0->d;
     const long long chunk = kChunkTilesPerSm * PBN * g0->sm_count;
     if ((rc = g0->xc.reserve(sizeof(double) * (size_t)2 * chunk * d))) return rc;
     if ((rc = g0->sel.reserve(sizeof(SelRecord) * (B200BO_MAX_TOPK + 1)))) return rc;
-    double* buf[2] = {g0->xc.as<double>(), g0->xc.as<double>() + (size_t)chunk * d};
-    int i = 0;
-    for (long long c0 = 0; c0 < m; c0 += chunk, ++i) {
-        const long long mc = (m - c0) < chunk ? (m - c0) : chunk;
-        const int b = i & 1;
-        if (i >= 2) CU(cudaStreamWaitEvent(g0->copy_stream, g0->chunk_done[b], 0));  // buffer b consumed
-        CU(cudaMemcpyAsync(buf[b], Xc + (size_t)c0 * d, sizeof(double) * (size_t)mc * d, cudaMemcpyHostToDevice,
-                           g0->copy_stream));
-        CU(cudaEventRecord(g0->chunk_up[b], g0->copy_stream));
-        CU(cudaStreamWaitEvent(g0->exec_stream, g0->chunk_up[b], 0));
+    double* const buf[2] = {g0->xc.as<double>(), g0->xc.as<double>() + (size_t)chunk * d};
+    rc = U.run(Xc, m, d, chunk, buf, [&](const double* dx, long long mc, long long c0, int i, bool last) {
         CandSrc src;
-        src.d_Xc = buf[b];
+        src.d_Xc = dx;
         SelMode sm;
         sm.resume = i > 0;
-        sm.finish = (c0 + chunk >= m);
-        if ((rc = eval_core(spec, src, mc, nullptr, nullptr, nullptr, k, g0->sel.p, c0, g0->exec_stream, sm)))
-            return rc;
-        CU(cudaEventRecord(g0->chunk_done[b], g0->exec_stream));
-    }
-    CU(cudaStreamSynchronize(g0->exec_stream));
+        sm.finish = last;
+        return eval_core(spec, src, mc, nullptr, nullptr, nullptr, k, g0->sel.p, c0, U.exec, sm);
+    });
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(U.exec));
     CU(cudaMemcpy(sel_host, g0->sel.p, sizeof(SelRecord) * (k + 1), cudaMemcpyDeviceToHost));
     return check_nonfinite(g0);
 }
@@ -1489,6 +1516,336 @@ extern "C" int b200bo_philox_rows(int device, uint64_t seed, const double* lo, c
     cudaFree(d_pb);
     cudaFree(d_out);
     if (e != cudaSuccess) return set_err(B200BO_ERR_CUDA, "philox_rows: %s", cudaGetErrorString(e));
+    return B200BO_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// posterior sample paths (Thompson sampling): paths.cuh
+// ---------------------------------------------------------------------------------------
+// Everything a path evaluates is a copy owned by the path: a later fit, append or LML evaluation on the GP
+// handle (which overwrite its factor buffers) does not change a path drawn earlier.
+struct b200bo_paths {
+    int device = 0, sm_count = 0, grid_cap = 0;
+    int n = 0, np = 0, d = 0, q = 0, L = 0, Lp = 0, cov = 0;
+    double constv = 1.0, feat_scale = 0.0, y_mean = 0.0, y_std = 1.0;
+    bool has_xf = false;
+    DevBuf Xs, V, omega, bias, W, ls, xf, xc, out, sel_cta, sel, pbounds, prow, bad;
+    ChunkedUpload upload;
+};
+
+// register slots per thread for the q sums: 1, 4 or 16 (q = 1, 2..4, 5..16)
+static int paths_qt(int q) { return q <= 1 ? 1 : (q <= 4 ? 4 : B200BO_MAX_PATHS); }
+
+using PathsKernel = void (*)(const PathsParams);
+static PathsKernel paths_kernel(int cov, int q) {
+    static const PathsKernel tab[4][3] = {
+        {paths_eval_kernel<0, 1>, paths_eval_kernel<0, 4>, paths_eval_kernel<0, B200BO_MAX_PATHS>},
+        {paths_eval_kernel<1, 1>, paths_eval_kernel<1, 4>, paths_eval_kernel<1, B200BO_MAX_PATHS>},
+        {paths_eval_kernel<2, 1>, paths_eval_kernel<2, 4>, paths_eval_kernel<2, B200BO_MAX_PATHS>},
+        {paths_eval_kernel<3, 1>, paths_eval_kernel<3, 4>, paths_eval_kernel<3, B200BO_MAX_PATHS>},
+    };
+    const int qt = paths_qt(q);
+    return tab[cov][qt == 1 ? 0 : (qt == 4 ? 1 : 2)];
+}
+
+static PathsParams paths_params(const b200bo_paths* ps) {
+    PathsParams P;
+    memset(&P, 0, sizeof(P));
+    P.Xs = ps->Xs.as<double>();
+    P.V = ps->V.as<double>();
+    P.omega = ps->omega.as<double>();
+    P.bias = ps->bias.as<double>();
+    P.W = ps->W.as<double>();
+    P.ls = ps->ls.as<double>();
+    P.xform = ps->has_xf ? ps->xf.as<int>() : nullptr;
+    P.n = ps->n;
+    P.np = ps->np;
+    P.d = ps->d;
+    P.q = ps->q;
+    P.Lp = ps->Lp;
+    P.constv = ps->constv;
+    P.feat_scale = ps->feat_scale;
+    P.y_mean = ps->y_mean;
+    P.y_std = ps->y_std;
+    P.clamp_count = ps->bad.as<unsigned long long>();
+    return P;
+}
+
+static int paths_grid(const b200bo_paths* ps, int64_t m) {
+    const long long ntiles = (m + PBN - 1) / PBN;
+    return (int)(ntiles < ps->grid_cap ? ntiles : ps->grid_cap);
+}
+
+static int paths_launch(const b200bo_paths* ps, const PathsParams& P, int grid, cudaStream_t st) {
+    if (grid <= 0) return B200BO_OK;
+    void* args[] = {(void*)&P};
+    CU(cudaLaunchKernel((const void*)paths_kernel(ps->cov, P.q), dim3(grid), dim3(PT_NT), args,
+                        paths_smem_bytes(P.d, P.q, P.sel_cta != nullptr), st));
+    LAUNCHED();
+    return B200BO_OK;
+}
+
+// one k-way merge per path: (k+1) records of path p at sel[p * (k+1)]
+static int paths_merge(b200bo_paths* ps, int grid, int k, cudaStream_t st) {
+    NvtxRange nvtx_sel("b200bo:select");
+    for (int p = 0; p < ps->q; ++p) {
+        merge_sel_kernel<<<1, 256, 0, st>>>(ps->sel_cta.as<SelList>() + (size_t)p * grid, grid, k,
+                                            ps->sel.as<SelRecord>() + (size_t)p * (k + 1));
+        LAUNCHED();
+    }
+    CU(cudaGetLastError());
+    return B200BO_OK;
+}
+
+static int paths_check_nonfinite(b200bo_paths* ps) {
+    unsigned long long c[2] = {0, 0};
+    CU(cudaMemcpy(c, ps->bad.p, sizeof(c), cudaMemcpyDeviceToHost));
+    if (c[1] != 0) return set_err(B200BO_ERR_ARG, "Input X contains NaN or infinity.");
+    return B200BO_OK;
+}
+
+static void paths_unpack(const std::vector<SelRecord>& rec, int q, int k, double* best_val, int64_t* best_idx,
+                         double* topk_val, int64_t* topk_idx) {
+    const int kk = k > 0 ? k : 1;
+    for (int p = 0; p < q; ++p)
+        unpack_records(rec.data() + (size_t)p * (kk + 1), k, best_val ? best_val + p : nullptr,
+                       best_idx ? best_idx + p : nullptr, topk_val ? topk_val + (size_t)p * k : nullptr,
+                       topk_idx ? topk_idx + (size_t)p * k : nullptr);
+}
+
+struct ScopedBufs {
+    DevBuf b[4];
+    ~ScopedBufs() {
+        for (DevBuf& x : b) x.release();
+    }
+};
+
+// copies of the GP's evaluation state, the draws, and V = K^-1 (y_norm - Phi(Xs) W - eps) column by column
+static int paths_setup(b200bo_gp* gp, b200bo_paths* ps, const double* omega, const double* bv, const double* w,
+                       const double* eps) {
+    const int n = ps->n, np = ps->np, d = ps->d, q = ps->q, L = ps->L, Lp = ps->Lp;
+    const void* fn = (const void*)paths_kernel(ps->cov, q);
+    // One instantiation serves every (d, q) of its class and every path alive on the device: its opt-in limit is
+    // the largest size any of them can need (d = B200BO_MAX_DIM, q = its QT: 230 784 B for QT = 16), so creating
+    // a smaller path never lowers the limit below what a path drawn earlier launches with.
+    CU(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)paths_smem_bytes(B200BO_MAX_DIM, paths_qt(q), true)));
+    const size_t smem = paths_smem_bytes(d, q, true);
+    int bps = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, fn, PT_NT, smem));
+    ps->grid_cap = ps->sm_count * (bps < 1 ? 1 : (bps > 2 ? 2 : bps));
+    int rc;
+    if ((rc = ps->Xs.reserve(sizeof(double) * (size_t)np * d))) return rc;
+    if ((rc = ps->V.reserve(sizeof(double) * (size_t)np * q))) return rc;
+    if ((rc = ps->omega.reserve(sizeof(double) * (size_t)Lp * d))) return rc;
+    if ((rc = ps->bias.reserve(sizeof(double) * (size_t)Lp))) return rc;
+    if ((rc = ps->W.reserve(sizeof(double) * (size_t)Lp * q))) return rc;
+    if ((rc = ps->ls.reserve(sizeof(double) * B200BO_MAX_DIM))) return rc;
+    if ((rc = ps->xf.reserve(sizeof(int) * B200BO_MAX_DIM))) return rc;
+    if ((rc = ps->bad.reserve(2 * sizeof(unsigned long long)))) return rc;
+    if ((rc = ps->out.reserve(sizeof(double) * (size_t)n * q))) return rc;
+    CU(cudaMemcpy(ps->Xs.p, gp->Xs.p, sizeof(double) * (size_t)np * d, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(ps->ls.p, gp->ls.p, sizeof(double) * d, cudaMemcpyDeviceToDevice));
+    if (ps->has_xf) CU(cudaMemcpy(ps->xf.p, gp->xf.p, sizeof(int) * d, cudaMemcpyDeviceToDevice));
+    {
+        std::vector<double> om((size_t)Lp * d, 0.0), bb((size_t)Lp, 0.0), ww((size_t)Lp * q, 0.0);
+        memcpy(om.data(), omega, sizeof(double) * (size_t)L * d);
+        memcpy(bb.data(), bv, sizeof(double) * (size_t)L);
+        memcpy(ww.data(), w, sizeof(double) * (size_t)L * q);
+        CU(cudaMemcpy(ps->omega.p, om.data(), sizeof(double) * om.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(ps->bias.p, bb.data(), sizeof(double) * bb.size(), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(ps->W.p, ww.data(), sizeof(double) * ww.size(), cudaMemcpyHostToDevice));
+    }
+    CU(cudaMemset(ps->V.p, 0, sizeof(double) * (size_t)np * q));
+    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
+    // prior part at the training rows: the candidate kernel itself on the training inputs, with V = 0 and unit
+    // output scaling, so r and every later candidate share one feature code
+    PathsParams P = paths_params(ps);
+    P.Xc = gp->X.as<double>();
+    P.m = n;
+    P.out = ps->out.as<double>();
+    P.y_mean = 0.0;
+    P.y_std = 1.0;
+    if ((rc = paths_launch(ps, P, paths_grid(ps, n), nullptr))) return rc;
+    std::vector<double> prior((size_t)n * q);
+    CU(cudaMemcpy(prior.data(), ps->out.p, sizeof(double) * prior.size(), cudaMemcpyDeviceToHost));
+    std::vector<double> R((size_t)q * np, 0.0);
+    for (int i = 0; i < n; ++i)
+        for (int p = 0; p < q; ++p)
+            R[(size_t)p * np + i] = gp->y_norm[i] - prior[(size_t)i * q + p] - eps[(size_t)i * q + p];
+    ScopedBufs s;
+    DevBuf &r = s.b[0], &x = s.b[1], &t1 = s.b[2], &t2 = s.b[3];
+    if ((rc = r.reserve(sizeof(double) * R.size()))) return rc;
+    if ((rc = x.reserve(sizeof(double) * R.size()))) return rc;
+    if ((rc = t1.reserve(sizeof(double) * np))) return rc;
+    if ((rc = t2.reserve(sizeof(double) * np))) return rc;
+    CU(cudaMemcpy(r.p, R.data(), sizeof(double) * R.size(), cudaMemcpyHostToDevice));
+    for (int p = 0; p < q; ++p)
+        if ((rc = solve_spd(gp, r.as<double>() + (size_t)p * np, x.as<double>() + (size_t)p * np, t1.as<double>(),
+                            t2.as<double>())))
+            return rc;
+    CU(cudaMemcpy(R.data(), x.p, sizeof(double) * R.size(), cudaMemcpyDeviceToHost));
+    std::vector<double> Vrow((size_t)np * q, 0.0);
+    for (int i = 0; i < n; ++i)
+        for (int p = 0; p < q; ++p) Vrow[(size_t)i * q + p] = R[(size_t)p * np + i];
+    CU(cudaMemcpy(ps->V.p, Vrow.data(), sizeof(double) * Vrow.size(), cudaMemcpyHostToDevice));
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_paths_create(b200bo_gp* gp, int q, int L, const double* omega, const double* b,
+                                   const double* w, const double* eps, b200bo_paths** out) {
+    if (!gp || !omega || !b || !w || !eps || !out) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!gp->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
+    if (gp->replica) return set_err(B200BO_ERR_STATE, "a predict-only replica holds no K: draw paths from the source handle");
+    if (q < 1 || q > B200BO_MAX_PATHS) return set_err(B200BO_ERR_ARG, "q=%d out of range [1,%d]", q, B200BO_MAX_PATHS);
+    if (L < 1 || L > (1 << 24)) return set_err(B200BO_ERR_ARG, "L=%d out of range [1,2^24]", L);
+    CU(cudaSetDevice(gp->device));
+    StreamScope scope(nullptr);  // legacy default stream
+    NvtxRange nvtx_range("b200bo:paths_create");
+    b200bo_paths* ps = new b200bo_paths();
+    ps->device = gp->device;
+    ps->sm_count = gp->sm_count;
+    ps->n = (int)gp->n;
+    ps->np = gp->np;
+    ps->d = gp->d;
+    ps->q = q;
+    ps->L = L;
+    ps->Lp = round_up(L, PT_CHUNK);
+    ps->cov = cov_code(gp->family, gp->nu);
+    ps->constv = gp->constv;
+    ps->feat_scale = std::sqrt(2.0 * gp->constv / (double)L);
+    ps->y_mean = gp->y_mean;
+    ps->y_std = gp->y_std;
+    ps->has_xf = !gp->xform.empty();
+    const int rc = paths_setup(gp, ps, omega, b, w, eps);
+    if (rc != B200BO_OK) {
+        b200bo_paths_destroy(ps);
+        return rc;
+    }
+    *out = ps;
+    return B200BO_OK;
+}
+
+extern "C" void b200bo_paths_destroy(b200bo_paths* ps) {
+    if (!ps) return;
+    cudaSetDevice(ps->device);
+    DevBuf* bufs[] = {&ps->Xs, &ps->V, &ps->omega, &ps->bias, &ps->W, &ps->ls, &ps->xf, &ps->xc,
+                      &ps->out, &ps->sel_cta, &ps->sel, &ps->pbounds, &ps->prow, &ps->bad};
+    for (DevBuf* b : bufs) b->release();
+    ps->upload.release();
+    delete ps;
+}
+
+extern "C" int b200bo_paths_eval(b200bo_paths* ps, const double* Xc, int64_t m, double* out) {
+    if (!ps || m < 0 || (m > 0 && (!Xc || !out))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_eval");
+    int rc;
+    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * ps->d))) return rc;
+    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m * ps->q))) return rc;
+    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * ps->d, cudaMemcpyHostToDevice));
+    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
+    PathsParams P = paths_params(ps);
+    P.Xc = ps->xc.as<double>();
+    P.m = m;
+    P.out = ps->out.as<double>();
+    if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
+    CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m * ps->q, cudaMemcpyDeviceToHost));
+    return paths_check_nonfinite(ps);
+}
+
+// Host batches of more than one chunk (kChunkTilesPerSm tiles per SM) are streamed as in run_host_chunked
+// (ChunkedUpload): the per-CTA lists of every path carry over between launches and are merged once.
+extern "C" int b200bo_paths_argmin_topk(b200bo_paths* ps, const double* Xc, int64_t m, int k, double* best_val,
+                                        int64_t* best_idx, double* topk_val, int64_t* topk_idx) {
+    if (!ps) return set_err(B200BO_ERR_ARG, "paths is NULL");
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (m <= 0 || !Xc) return set_err(B200BO_ERR_ARG, "m must be > 0");
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_select");
+    const int kk = k > 0 ? k : 1, d = ps->d, q = ps->q;
+    const long long chunk = kChunkTilesPerSm * PBN * ps->sm_count;
+    ChunkedUpload& U = ps->upload;
+    int rc;
+    if ((rc = U.ensure())) return rc;
+    const bool one = m <= chunk;
+    const long long cm = one ? m : chunk;
+    const int grid = one ? paths_grid(ps, m) : ps->grid_cap;  // chunked: one list per CTA slot across launches
+    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)(one ? 1 : 2) * cm * d))) return rc;
+    if ((rc = ps->sel_cta.reserve(sizeof(SelList) * (size_t)q * grid))) return rc;
+    if ((rc = ps->sel.reserve(sizeof(SelRecord) * (size_t)q * (kk + 1)))) return rc;
+    double* const buf[2] = {ps->xc.as<double>(), ps->xc.as<double>() + (one ? 0 : (size_t)cm * d)};
+    CU(cudaMemsetAsync(ps->bad.p, 0, 2 * sizeof(unsigned long long), U.exec));
+    PathsParams P = paths_params(ps);
+    P.sel_cta = ps->sel_cta.as<SelList>();
+    P.sel_k = kk;
+    rc = U.run(Xc, m, d, cm, buf, [&](const double* dx, long long mc, long long c0, int i, bool) {
+        P.Xc = dx;
+        P.m = mc;
+        P.index_base = c0;
+        P.sel_resume = i > 0;
+        return paths_launch(ps, P, grid, U.exec);
+    });
+    if (rc) return rc;
+    if ((rc = paths_merge(ps, grid, kk, U.exec))) return rc;
+    CU(cudaStreamSynchronize(U.exec));
+    std::vector<SelRecord> rec((size_t)q * (kk + 1));
+    CU(cudaMemcpy(rec.data(), ps->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
+    if ((rc = paths_check_nonfinite(ps))) return rc;
+    paths_unpack(rec, q, k, best_val, best_idx, topk_val, topk_idx);
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_paths_argmin_topk_philox(b200bo_paths* ps, uint64_t seed, const double* lo, const double* hi,
+                                               int64_t m, int64_t index_base, int k, double* best_val,
+                                               int64_t* best_idx, double* best_x, double* topk_val,
+                                               int64_t* topk_idx, double* topk_x) {
+    if (!ps || !lo || !hi) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (m <= 0) return set_err(B200BO_ERR_ARG, "m must be > 0");
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_select");
+    const int kk = k > 0 ? k : 1, d = ps->d, q = ps->q;
+    double pb[2 * B200BO_MAX_DIM];
+    for (int j = 0; j < d; ++j) {
+        if (!(lo[j] <= hi[j])) return set_err(B200BO_ERR_ARG, "Philox bounds: lo > hi in column %d", j);
+        pb[j] = lo[j];
+        pb[d + j] = hi[j] - lo[j];
+    }
+    const int grid = paths_grid(ps, m);
+    int rc;
+    if ((rc = ps->pbounds.reserve(sizeof(double) * 2 * B200BO_MAX_DIM))) return rc;
+    if ((rc = ps->sel_cta.reserve(sizeof(SelList) * (size_t)q * grid))) return rc;
+    if ((rc = ps->sel.reserve(sizeof(SelRecord) * (size_t)q * (kk + 1)))) return rc;
+    CU(cudaMemcpy(ps->pbounds.p, pb, sizeof(double) * 2 * d, cudaMemcpyHostToDevice));
+    PathsParams P = paths_params(ps);
+    P.pbounds = ps->pbounds.as<double>();
+    P.seed = seed;
+    P.index_base = index_base;
+    P.m = m;
+    P.sel_cta = ps->sel_cta.as<SelList>();
+    P.sel_k = kk;
+    if ((rc = paths_launch(ps, P, grid, nullptr))) return rc;
+    if ((rc = paths_merge(ps, grid, kk, nullptr))) return rc;
+    const int nrec = q * (kk + 1);
+    std::vector<SelRecord> rec((size_t)nrec);
+    CU(cudaMemcpy(rec.data(), ps->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
+    paths_unpack(rec, q, k, best_val, best_idx, topk_val, topk_idx);
+    if (best_x || (topk_x && k > 0)) {
+        if ((rc = ps->prow.reserve(sizeof(double) * (size_t)nrec * d))) return rc;
+        philox_rows_kernel<<<nrec, 64>>>(seed, ps->pbounds.as<double>(), d, ps->sel.as<SelRecord>(), nrec,
+                                         ps->prow.as<double>());
+        LAUNCHED();
+        CU(cudaGetLastError());
+        std::vector<double> rows((size_t)nrec * d);
+        CU(cudaMemcpy(rows.data(), ps->prow.p, sizeof(double) * rows.size(), cudaMemcpyDeviceToHost));
+        for (int p = 0; p < q; ++p) {
+            const double* rp = rows.data() + (size_t)p * (kk + 1) * d;
+            if (best_x) memcpy(best_x + (size_t)p * d, rp, sizeof(double) * d);
+            if (topk_x && k > 0) memcpy(topk_x + (size_t)p * k * d, rp + d, sizeof(double) * (size_t)k * d);
+        }
+    }
     return B200BO_OK;
 }
 

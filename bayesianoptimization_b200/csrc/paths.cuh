@@ -1,0 +1,186 @@
+// paths.cuh - posterior sample paths of a fitted GP (Thompson sampling), evaluated and ranked on the device.
+//
+// Pathwise conditioning (Wilson et al., ICML 2020, "Efficiently sampling functions from Gaussian process
+// posteriors"), in the normalised target units of the fitted state:
+//   path_p(x) = s_y * ( sum_l W[l][p] phi_l(xs) + sum_i V[i][p] k(xs, Xs_i) ) + y_mean,   xs = transform(x)/ls
+//   phi_l(xs) = sqrt(2c/L) cos(omega_l . xs + b_l)        (random Fourier features of the prior, L of them)
+//   V = K^-1 (y_norm - Phi(Xs) W - eps)                   (exact update, solved once per path at creation)
+// The reference has no counterpart: its tutorial draws multivariate_normal(mean, cov) from
+// predict(return_cov=True) on the host, O(M^3) in the number of candidates.  Here a candidate costs
+// O(N d + L d) whatever M is, and q <= B200BO_MAX_PATHS paths share one candidate tile.
+//
+// Decomposition: a persistent grid of 256-thread CTAs, 128-candidate tiles, two threads per candidate (each
+// takes half of every staged chunk).  Training rows (Xs, V) and then features (omega, W, b) stream through
+// shared memory in double-buffered cp.async chunks of 64; the q sums live in registers.  The two halves are
+// added in a fixed order, so a candidate's value depends on its coordinates only - not on the batch size, its
+// position in the batch or the grid size (the finite-difference stencil of the L-BFGS-B refinement relies on
+// that).  Output: f (m x q), and/or -f folded into one running selection list per path (select.cuh).
+#pragma once
+#include "common.cuh"
+#include "predict_kernels.cuh"
+#include "select.cuh"
+
+namespace b200bo {
+
+constexpr int PT_CHUNK = 64;  // training rows / features per staged chunk
+constexpr int PT_NT = 256;
+constexpr int PT_R = 4;       // rows per inner step (independent chains for the fp64 pipe)
+
+struct PathsParams {
+    const double* Xs;     // [np][d]  transform(X)/ls of the training rows (path-owned copy), zero padded
+    const double* V;      // [np][q]  K^-1 r, zero padded
+    const double* omega;  // [Lp][d]  spectral draws, zero padded
+    const double* bias;   // [Lp]     phases
+    const double* W;      // [Lp][q]  feature weights, zero padded
+    const double* ls;     // [d]      length scales (replicated when isotropic)
+    const int* xform;     // [d] or nullptr
+    int n, np, d, q, Lp, sel_k, sel_resume, pad0;
+    double constv, feat_scale, y_mean, y_std;
+    // candidate source: the fields candidate_coord reads (predict_kernels.cuh)
+    const double* Xc;         // [m][d] or nullptr (Philox)
+    const double* pbounds;    // Philox: [2][d] = lo_j, hi_j - lo_j
+    unsigned long long seed;  // Philox key
+    long long index_base;     // global index of this launch's candidate 0
+    long long m;
+    unsigned long long* clamp_count;  // [1]: non-finite candidate coordinates (slot [0] unused)
+    double* out;              // [m][q] or nullptr
+    SelList* sel_cta;         // [q][gridDim.x] per-CTA running selections, or nullptr
+};
+
+// dynamic shared memory: 2 stage buffers [64][d + q + 1] | xc [d][128] | red [2][q][128] | SelShared [q]
+__host__ __device__ inline size_t paths_smem_bytes(int d, int q, bool sel) {
+    return sizeof(double) * ((size_t)2 * PT_CHUNK * (d + q + 1) + (size_t)d * PBN + (size_t)2 * q * PBN) +
+           (sel ? sizeof(SelShared) * (size_t)q : 0);
+}
+
+// QT: register slots of the q sums (1, 4 or 16).  QT = 1, 4: 2 CTAs per SM (<= 128 registers, no spills).  QT = 16:
+// one CTA per SM and 176 registers - at 128 it spilled, and on an H100 (400 W) it took 147 ms instead of 127 ms for
+// 16 paths x 2^20 candidates at C3.
+template <int COV, int QT>
+__global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(const PathsParams P) {
+    extern __shared__ __align__(16) double smem[];
+    const int tid = threadIdx.x, d = P.d, q = P.q;
+    const int c = tid & (PBN - 1), half = tid >> 7;
+    const int bufsz = PT_CHUNK * (d + q + 1);
+    double* stage = smem;
+    double* xc_s = smem + 2 * bufsz;                // [d][PBN]
+    double* red = xc_s + (size_t)d * PBN;           // [2][q][PBN]
+    SelShared* sel = reinterpret_cast<SelShared*>(red + (size_t)2 * q * PBN);
+    if (P.sel_cta) {
+        if (tid < PBN)
+            for (int p = 0; p < q; ++p)
+                runsel_begin(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, P.sel_resume, tid);
+        __syncthreads();
+    }
+    const long long ntiles = (P.m + PBN - 1) / PBN;
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long c0 = tile * PBN;
+        // candidate coordinates, scaled exactly as scale_x_kernel scales the training rows
+        for (int idx = tid; idx < PBN * d; idx += PT_NT) {
+            const int cc = idx / d, j = idx - cc * d;
+            const long long gi = c0 + cc;
+            double v = 0.0;
+            if (gi < P.m) {
+                v = candidate_coord(P, gi, j);
+                if (P.xform && P.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
+                v = v / P.ls[j];
+            }
+            xc_s[j * PBN + cc] = v;
+        }
+        double ak[QT], af[QT];
+#pragma unroll
+        for (int p = 0; p < QT; ++p) ak[p] = af[p] = 0.0;
+        // pass 0: training rows (Xs, V) -> sum_i V[i][p] k(xs, Xs_i); pass 1: features (omega, W, b)
+        for (int pass = 0; pass < 2; ++pass) {
+            const double* A = pass ? P.omega : P.Xs;
+            const double* B = pass ? P.W : P.V;
+            const int nch = (pass ? P.Lp : P.np) / PT_CHUNK;
+            auto load = [&](int buf, int ch) {
+                double* dst = stage + buf * bufsz;
+                const double* a = A + (size_t)ch * PT_CHUNK * d;
+                for (int i = tid; i < PT_CHUNK * d / 2; i += PT_NT) cp_async16_cg(dst + 2 * i, a + 2 * i);
+                const double* b = B + (size_t)ch * PT_CHUNK * q;
+                for (int i = tid; i < PT_CHUNK * q / 2; i += PT_NT)
+                    cp_async16_cg(dst + PT_CHUNK * d + 2 * i, b + 2 * i);
+                if (pass && tid < PT_CHUNK / 2)
+                    cp_async16_cg(dst + PT_CHUNK * (d + q) + 2 * tid, P.bias + (size_t)ch * PT_CHUNK + 2 * tid);
+            };
+            load(0, 0);
+            cp_async_commit();
+            for (int ch = 0; ch < nch; ++ch) {
+                if (ch + 1 < nch) load((ch + 1) & 1, ch + 1);
+                cp_async_commit();
+                cp_async_wait<1>();
+                __syncthreads();  // chunk ch (and, on the first chunk, xc_s) visible
+                const double* a = stage + (ch & 1) * bufsz;
+                const double* b = a + PT_CHUNK * d;
+                const double* ph = b + PT_CHUNK * q;
+                for (int r0 = half * (PT_CHUNK / 2); r0 < (half + 1) * (PT_CHUNK / 2); r0 += PT_R) {
+                    double s[PT_R];
+#pragma unroll
+                    for (int t = 0; t < PT_R; ++t) s[t] = 0.0;
+                    for (int j = 0; j < d; ++j) {
+                        const double xv = xc_s[j * PBN + c];
+#pragma unroll
+                        for (int t = 0; t < PT_R; ++t) {
+                            const double av = a[(r0 + t) * d + j];
+                            if (pass) {
+                                s[t] = fma(av, xv, s[t]);
+                            } else {
+                                const double df = xv - av;
+                                s[t] = fma(df, df, s[t]);
+                            }
+                        }
+                    }
+#pragma unroll
+                    for (int t = 0; t < PT_R; ++t) {
+                        const int r = r0 + t;
+                        if (pass) {
+                            const double phi = cos(s[t] + ph[r]);
+#pragma unroll
+                            for (int p = 0; p < QT; ++p)
+                                if (p < q) af[p] = fma(b[r * q + p], phi, af[p]);
+                        } else {
+                            double kv = P.constv * cov_eval<COV>(s[t]);
+                            if (ch * PT_CHUNK + r >= P.n) kv = 0.0;
+#pragma unroll
+                            for (int p = 0; p < QT; ++p)
+                                if (p < q) ak[p] = fma(b[r * q + p], kv, ak[p]);
+                        }
+                    }
+                }
+                __syncthreads();  // buffer (ch & 1) free for the prefetch of chunk ch + 2
+            }
+            cp_async_wait<0>();
+        }
+        // the two halves of every sum, always added in the same order
+        if (half == 1) {
+#pragma unroll
+            for (int p = 0; p < QT; ++p)
+                if (p < q) {
+                    red[p * PBN + c] = ak[p];
+                    red[(q + p) * PBN + c] = af[p];
+                }
+        }
+        __syncthreads();
+        if (half == 0) {
+            const long long gi = c0 + c;
+            const bool valid = gi < P.m;
+#pragma unroll
+            for (int p = 0; p < QT; ++p) {
+                if (p < q) {
+                    const double kp = ak[p] + red[p * PBN + c];
+                    const double fp = af[p] + red[(q + p) * PBN + c];
+                    const double f = P.y_std * fma(P.feat_scale, fp, kp) + P.y_mean;
+                    if (P.out && valid) P.out[gi * q + p] = f;
+                    if (P.sel_cta) runsel_update<1>(sel[p], P.sel_k, tid, -f, gi + P.index_base, valid);
+                }
+            }
+        }
+        __syncthreads();  // xc_s / red reused by the next tile
+    }
+    if (P.sel_cta && tid < PBN)
+        for (int p = 0; p < q; ++p) runsel_store(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, tid);
+}
+
+}  // namespace b200bo

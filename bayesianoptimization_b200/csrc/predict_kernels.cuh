@@ -62,7 +62,9 @@ struct PredictParams {
 // A non-finite coordinate is counted in clamp_count[1]: the host entry points turn it into the ValueError
 // ("Input X contains NaN or infinity") sklearn's validate_data raises - checked where the data is read anyway instead
 // of a separate pass over the batch on the host (10 ms per 2^20 x 16 batch).
-__device__ __forceinline__ double candidate_coord(const PredictParams& P, long long gi, int j) {
+// Params: PredictParams or any launch-parameter struct with the same candidate-source fields (paths.cuh).
+template <class Params>
+__device__ __forceinline__ double candidate_coord(const Params& P, long long gi, int j) {
     if (P.Xc) {
         const double v = P.Xc[gi * P.d + j];
         if (!isfinite(v) && P.clamp_count) atomicAdd(P.clamp_count + 1, 1ull);

@@ -700,3 +700,13 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
 
     # sample_y (SK/gaussian_process/_gpr.py:502-539) is inherited: it only calls
     # self.predict(X, return_cov=True), which runs on the device.
+
+    def sample_paths(self, n_paths=1, n_features=4096, random_state=None):
+        """``n_paths`` (1..16) posterior sample paths of the latent function, as smooth functions that can be
+        evaluated anywhere (paths.PosteriorPaths): the prior part is a random-Fourier-feature draw with
+        ``n_features`` features, the data update is exact.  The draws come from ``random_state``
+        (``check_random_state``) in the order of ``paths.draw_path_inputs``.  The reference has no counterpart;
+        unlike ``sample_y`` the cost per evaluated point does not grow with the number of points."""
+        from .paths import PosteriorPaths
+
+        return PosteriorPaths(self, n_paths, n_features, random_state)

@@ -1,0 +1,170 @@
+"""Posterior sample paths of a fitted device GP - the function draws behind Thompson sampling.
+
+``B200GaussianProcessRegressor.sample_paths(n_paths, n_features, random_state)`` returns a ``PosteriorPaths``:
+q fixed, smooth functions drawn from the GP posterior by pathwise conditioning (Wilson et al., ICML 2020),
+
+    path_p(x) = s_y * ( sum_l W[l, p] phi_l(xs) + sum_i V[i, p] k(xs, Xs_i) ) + y_mean,    xs = transform(x) / ls
+    phi_l(xs) = sqrt(2 c / L) cos(omega_l . xs + b_l)
+    V = K^-1 (y_norm - Phi(Xs) W - eps)
+
+The first sum is a random-Fourier-feature draw from the prior (an approximation with L features), the second an
+exact data-dependent update.  A path samples the latent function: the WhiteKernel term is observation noise, it
+enters eps and K's diagonal and not the path.  Evaluating a path costs O(N d + L d) per candidate, with no N^2
+term, and q paths share one candidate tile (``csrc/paths.cuh``).
+
+Every random number comes from the caller's RandomState, drawn on the host in the order of ``draw_path_inputs``;
+the arrays cross the C ABI as they are.  This module needs numpy/sklearn and the CUDA library, not ``bayes_opt``.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+from sklearn.utils import check_random_state
+
+from . import _lib as B
+
+_NU = {B.NU_05: 0.5, B.NU_15: 1.5, B.NU_25: 2.5, B.NU_INF: np.inf}
+
+
+def draw_path_inputs(rs, n_paths, n_features, d, nu, n, noise_var):
+    """The draws of q = n_paths paths with L = n_features features, consumed from ``rs`` in exactly this order:
+
+        z     = rs.standard_normal((L, d))
+        u     = rs.chisquare(2 nu, L)                 (Matern nu in {0.5, 1.5, 2.5} only)
+        omega = z * sqrt(2 nu / u)[:, None]           (multivariate t, 2 nu dof; omega = z for RBF / nu = inf)
+        b     = rs.uniform(0, 2 pi, L)
+        w     = rs.standard_normal((L, q))
+        eps   = rs.standard_normal((n, q)) * sqrt(noise_var)
+
+    omega is the spectral draw of the unit-length-scale kernel: the length scales are already divided out of xs."""
+    L, q = int(n_features), int(n_paths)
+    z = rs.standard_normal((L, d))
+    if np.isinf(nu):
+        omega = z
+    else:
+        u = rs.chisquare(2.0 * nu, L)
+        omega = z * np.sqrt(2.0 * nu / u)[:, None]
+    b = rs.uniform(0.0, 2.0 * np.pi, L)
+    w = rs.standard_normal((L, q))
+    eps = rs.standard_normal((n, q)) * np.sqrt(noise_var)
+    return omega, b, w, eps
+
+
+class _PathsHandle:
+    """Owns one b200bo_paths*."""
+
+    def __init__(self):
+        self.ptr = C.c_void_p()
+
+    def __del__(self):
+        try:
+            if self.ptr:
+                B.lib().b200bo_paths_destroy(self.ptr)
+                self.ptr = C.c_void_p()
+        except Exception:  # interpreter shutdown
+            pass
+
+
+class PosteriorPaths:
+    """q posterior sample paths of a fitted B200GaussianProcessRegressor, evaluated on the GP's fit device.
+
+    ``paths(X)`` -> (M, q) values in data units; ``argmin_topk`` / ``argmin_topk_philox`` rank -path_p per path
+    on the device.  The paths own copies of the GP state they evaluate: refitting the GP afterwards does not
+    change them."""
+
+    def __init__(self, gp, n_paths=1, n_features=4096, random_state=None):
+        from .gpr import parse_kernel
+
+        if isinstance(n_paths, bool) or not isinstance(n_paths, (int, np.integer)) or not 1 <= n_paths <= B.MAX_PATHS:
+            raise ValueError(f"n_paths must be an integer in [1, {B.MAX_PATHS}], got {n_paths!r}")
+        if isinstance(n_features, bool) or not isinstance(n_features, (int, np.integer)) or n_features < 1:
+            raise ValueError(f"n_features must be a positive integer, got {n_features!r}")
+        gp._ensure_device_fit()  # "GP is not fitted" when it is not
+        ek = parse_kernel(gp.kernel_)
+        h = gp._handle()
+        L = B.lib()
+        self.n_paths = int(n_paths)
+        self.n_features = int(n_features)
+        self.dim = gp.X_train_.shape[1]
+        self.device = int(gp.device)
+        self.devices = [self.device]
+        self._xform = gp.__dict__.get("_b200_xform", ("device", None))
+        self._d = int(L.b200bo_gp_dim(h.ptr))  # after a host-side transform (one-hot): the transformed width
+        n = int(L.b200bo_gp_n(h.ptr))
+        rs = check_random_state(random_state)
+        omega, b, w, eps = draw_path_inputs(rs, self.n_paths, self.n_features, self._d, _NU[ek.nu],
+                                            n, float(gp.alpha) + ek.noise)
+        self._handle = _PathsHandle()
+        B.check(L.b200bo_paths_create(h.ptr, self.n_paths, self.n_features, B.as_dp(B.c_f64(omega)),
+                                      B.as_dp(B.c_f64(b)), B.as_dp(B.c_f64(w)), B.as_dp(B.c_f64(eps)),
+                                      C.byref(self._handle.ptr)))
+
+    def _candidates(self, X):
+        X = B.c_f64(np.asarray(X, dtype=np.float64).reshape(-1, self.dim))
+        mode, arg = self._xform
+        if mode == "host":  # the batch-dependent transform (categorical one-hot), as FusedAcquisition applies it
+            X = B.c_f64(np.asarray(arg(X), dtype=np.float64))
+        return X
+
+    def __call__(self, X):
+        """(M, q) path values at the rows of X (data units)."""
+        X = self._candidates(X)
+        out = np.empty((X.shape[0], self.n_paths))
+        B.check(B.lib().b200bo_paths_eval(self._handle.ptr, B.as_dp(X), X.shape[0], B.as_dp(out)))
+        return out
+
+    def argmin_topk(self, X, k):
+        """Per path p: np.argmin and the k smallest (np.argsort order) of -path_p over the rows of X.
+        Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
+        X = self._candidates(X)
+        k = int(k)
+        q = self.n_paths
+        bv, bi = np.empty(q), np.empty(q, dtype=np.int64)
+        tv, ti = np.empty(q * max(k, 1)), np.empty(q * max(k, 1), dtype=np.int64)
+        B.check(B.lib().b200bo_paths_argmin_topk(self._handle.ptr, B.as_dp(X), X.shape[0], k, B.as_dp(bv),
+                                                 bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tv),
+                                                 ti.ctypes.data_as(C.POINTER(C.c_int64))))
+        tops = [t[t >= 0] for t in ti[:q * k].reshape(q, k)]
+        return bi, bv, tops
+
+    def argmin_topk_philox(self, seed, bounds, m, k, index_base=0):
+        """Throughput mode: per path, the selection over m candidates generated inside the kernel (Philox4x32-10
+        keyed by (seed, global row index), the layout of FusedAcquisition.argmin_topk_philox).
+        Returns (idx (q,), values (q,), x_best (q, d), [top-k indices], [top-k rows])."""
+        if self._xform[0] == "host":
+            raise NotImplementedError("device candidate generation with a host-side kernel transform")
+        bounds = B.c_f64(np.asarray(bounds, dtype=np.float64).reshape(self.dim, 2))
+        lo, hi = B.c_f64(bounds[:, 0]), B.c_f64(bounds[:, 1])
+        k, q, d = int(k), self.n_paths, self.dim
+        kk = max(k, 1)
+        bv, bi, bx = np.empty(q), np.empty(q, dtype=np.int64), np.empty((q, d))
+        tv, ti, tx = np.empty(q * kk), np.empty(q * kk, dtype=np.int64), np.empty((q * kk, d))
+        B.check(B.lib().b200bo_paths_argmin_topk_philox(
+            self._handle.ptr, int(seed) & 0xFFFFFFFFFFFFFFFF, B.as_dp(lo), B.as_dp(hi), int(m), int(index_base), k,
+            B.as_dp(bv), bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(bx), B.as_dp(tv),
+            ti.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tx)))
+        ti, tx = ti[:q * k].reshape(q, k), tx[:q * k].reshape(q, k, d)
+        keep = ti >= 0
+        return bi, bv, bx, [ti[p][keep[p]] for p in range(q)], [tx[p][keep[p]] for p in range(q)]
+
+
+class PathAcquisition:
+    """Acquisition closure over path 0 of a PosteriorPaths: x (M,d)|(d,) -> (M,) values of -path(x), with the
+    device selection of the random stage (``argmin_topk``, ``argmin_topk_philox``) in the signatures of
+    ``FusedAcquisition``, so the hooks of the acquisition seam rank and refine it on the device."""
+
+    def __init__(self, paths):
+        self.paths = paths
+        self.devices = paths.devices
+
+    def __call__(self, x):
+        return -self.paths(x)[:, 0]
+
+    def argmin_topk(self, x, k):
+        idx, val, tops = self.paths.argmin_topk(x, k)
+        return int(idx[0]), float(val[0]), tops[0]
+
+    def argmin_topk_philox(self, seed, bounds, m, k, index_base=0):
+        idx, val, bx, ti, tx = self.paths.argmin_topk_philox(seed, bounds, m, k, index_base)
+        return int(idx[0]), float(val[0]), bx[0], ti[0], tx[0]

@@ -251,6 +251,42 @@ int b200bo_multi_gpu_acq_argmin_topk_philox(const b200bo_acq* specs, int n_dev, 
 int b200bo_multi_gpu_acq_eval(const b200bo_acq* specs, int n_dev, const double* Xc, int64_t m,
                               const int64_t* offsets, double* acq_neg);
 
+/* ---- posterior sample paths (Thompson sampling) ------------------------------------------ */
+/* The reference has no counterpart in the package; its tutorial's custom ThompsonSampling
+ * (R/examples/acquisition_functions.ipynb) draws multivariate_normal(mean, cov) on the host from
+ * predict(X, return_cov=True), O(M^3) in the number of candidates.  A path here is a fixed smooth function
+ * (pathwise conditioning, Wilson et al. ICML 2020), in the normalised units of the fitted state:
+ *   path_p(x) = y_std * ( sum_l w[l][p] phi_l(xs) + sum_i v[i][p] k(xs, Xs_i) ) + y_mean,  xs = transform(x)/ls
+ *   phi_l(xs) = sqrt(2 const_value / L) cos(omega_l . xs + b_l)
+ *   v = K^-1 (y_norm - Phi(Xs) w - eps)      (K incl. alpha + noise_level on the diagonal, as in fit)
+ * A path samples the latent function: the WhiteKernel term enters eps and K's diagonal, not the path.
+ * Every draw crosses the ABI as an array, so the caller's RNG stays the only source of randomness:
+ *   omega: (L,d) unit-length-scale spectral draws (standard normal for RBF; multivariate t with 2 nu degrees of
+ *          freedom for Matern nu), b: (L,) phases in [0, 2 pi), w: (L,q) N(0,1) weights, eps: (n,q) noise draws
+ *          with variance alpha + noise_level.  All row-major host arrays; d = b200bo_gp_dim(gp), n = b200bo_gp_n(gp).
+ * A path owns copies of everything it evaluates: a later fit / append / lml on `gp` does not change it.  It lives
+ * on gp's device and evaluates in fp64 whatever gp's precision. */
+#define B200BO_MAX_PATHS 16
+
+typedef struct b200bo_paths b200bo_paths; /* opaque: q posterior sample paths of one fitted GP */
+
+/* 1 <= q <= B200BO_MAX_PATHS, L >= 1.  One solve of K v = r per path, O(N^2 q). */
+int b200bo_paths_create(b200bo_gp* gp, int q, int L, const double* omega, const double* b, const double* w,
+                        const double* eps, b200bo_paths** out);
+void b200bo_paths_destroy(b200bo_paths* paths);
+/* out: (m,q) host, path values at the rows of Xc (m,d) host, in data units.  A row's value depends on its
+ * coordinates only (not on m, its position or the launch geometry). */
+int b200bo_paths_eval(b200bo_paths* paths, const double* Xc, int64_t m, double* out);
+/* Per path p, ranks -path_p on the rows of Xc with the semantics of b200bo_acq_argmin_topk: best_val[p], best_idx[p]
+ * (np.argmin), topk_val[p*k + i], topk_idx[p*k + i] (np.argsort order).  Large batches are streamed in chunks. */
+int b200bo_paths_argmin_topk(b200bo_paths* paths, const double* Xc, int64_t m, int k, double* best_val,
+                             int64_t* best_idx, double* topk_val, int64_t* topk_idx);
+/* Throughput mode as b200bo_acq_argmin_topk_philox: candidates generated in the kernel from (seed, global index);
+ * best_x: (q,d), topk_x: (q,k,d) host - the winners' rows. */
+int b200bo_paths_argmin_topk_philox(b200bo_paths* paths, uint64_t seed, const double* lo, const double* hi, int64_t m,
+                                    int64_t index_base, int k, double* best_val, int64_t* best_idx, double* best_x,
+                                    double* topk_val, int64_t* topk_idx, double* topk_x);
+
 /* Duration (ms) of the most recent fused predict+acquisition kernel launched through a
  * device or host entry point on this thread, measured with CUDA events on its stream.
  * Synchronises on the stop event. */
