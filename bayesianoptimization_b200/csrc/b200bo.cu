@@ -25,6 +25,7 @@
 using namespace b200bo;
 
 constexpr int kDefaultPredictWarps = 16;  // measured A/B (DESIGN.md 6): 550.1 ms vs 561.7 ms per 2^20 candidates at C3
+constexpr float kDefaultLinvL2Last = 1.0f;  // evict_last fraction of the L^-1 loads (DESIGN.md 6)
 
 // ---------------------------------------------------------------------------------------
 // error plumbing
@@ -220,8 +221,10 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             kPredictSmemBytesTc));
     CU(cudaFuncSetAttribute(small_trsv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmallTrsvSmemBytes));
-    CU(cudaFuncSetAttribute(predict_acq16_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_acq16_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 884>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 884>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
@@ -969,7 +972,7 @@ static bool use_small_path(long long m, int np_max, int n_gps, int sm_count, int
     return t_small < t_big;
 }
 
-// GEMM inner-loop variant of the fused predict kernel: "dmma" (mma.sync m8n8k4 f64, default) or
+// GEMM inner-loop variant of the fused predict kernel: "dmma" (mma.sync f64, default; shape: predict_mma) or
 // "dfma" (8x8 register tiles).  Both are exact fp64 with fixed-order reductions; the environment
 // variable B200BO_PREDICT_IMPL selects one for A/B measurements.
 static int predict_impl(int precision) {
@@ -987,6 +990,33 @@ static int predict_warps() {
     if (e && e[0] == '1' && e[1] == '6') return 16;
     if (e && e[0] == '8') return 8;
     return kDefaultPredictWarps;
+}
+
+// MMA shape of phase B of predict_acq16_kernel: 1684 (mma.sync m16n8k4 f64, sm_90, default) or, with
+// B200BO_PREDICT_MMA=884, the sm_80 shape m8n8k4 for A/B measurements
+static int predict_mma() {
+    const char* e = getenv("B200BO_PREDICT_MMA");
+    return (e && strcmp(e, "884") == 0) ? 884 : 1684;
+}
+
+template <int MMA>
+static void launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
+    if (dreg)
+        predict_acq16_kernel<true, MMA><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P);
+    else
+        predict_acq16_kernel<false, MMA><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P);
+}
+
+// evict_last fraction of predict_acq16_kernel's L^-1 loads; B200BO_PREDICT_L2=<fraction in (0,1]> or "none"
+// (evict_normal) overrides the measured default for A/B measurements
+static float predict_linv_l2_last() {
+    const char* e = getenv("B200BO_PREDICT_L2");
+    if (e && strcmp(e, "none") == 0) return 0.f;
+    if (e && *e) {
+        const float f = strtof(e, nullptr);
+        if (f > 0.f && f <= 1.f) return f;
+    }
+    return kDefaultLinvL2Last;
 }
 
 // fp32 mode operand images of L^-1 (once per fit)
@@ -1175,10 +1205,11 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
                 predict_acq_tc_kernel<false><<<grid, PNT, kPredictSmemBytesTc, stream>>>(P);
             }
         } else if (predict_impl(g0->precision) == PREDICT_IMPL_DMMA && predict_warps() == 16) {
-            if (dreg)
-                predict_acq16_kernel<true><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P);
+            P.linv_l2_last = predict_linv_l2_last();
+            if (predict_mma() == 884)
+                launch_predict16<884>(dreg, grid, stream, P);
             else
-                predict_acq16_kernel<false><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P);
+                launch_predict16<1684>(dreg, grid, stream, P);
         } else if (predict_impl(g0->precision) == PREDICT_IMPL_DMMA) {
             if (dreg)
                 predict_acq_kernel<PREDICT_IMPL_DMMA, true><<<grid, PNT, kPredictSmemBytesDmma, stream>>>(P);

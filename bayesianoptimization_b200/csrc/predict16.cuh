@@ -8,9 +8,13 @@
 //     DMMA loop, stalled_wait 4.8 / math_pipe_throttle 3.2 per issue);
 //   * phase A (K* build, DFMA + sqrt/exp latency chains) runs with 16 warps, four row-quarters per candidate
 //     column, so its latency-bound part shrinks;
-//   * L2 policy hints: L^-1 (67 MB triangle at N=4096, re-read by every CTA for every tile) is loaded
-//     evict_last, the CTA-private K* scratch (written once, swept cyclically: LRU-hostile) evict_first, so the
-//     0.6 GB scratch stream stops evicting the factor from the 126 MB L2.
+//   * phase B runs on the sm_90 shape mma.sync m16n8k4 f64 (MMA = 1684, the default: twice the fp64 tensor rate of
+//     the sm_80 shape m8n8k4 per SM and clock on H100); m8n8k4 (MMA = 884) stays selectable with
+//     B200BO_PREDICT_MMA=884 for A/B measurements (DESIGN.md 4.1, 6, 6.1);
+//   * L2 policy hints: the CTA-private K* scratch (written once, swept cyclically: LRU-hostile) is stored and
+//     loaded evict_first; L^-1 (re-read by every CTA for every tile) is loaded evict_last on a fraction
+//     P.linv_l2_last of its lines.  At N=4096 the L^-1 triangle is 67 MB, more than the 50 MB L2 of an H100, so
+//     the fraction is a measured choice (DESIGN.md 6), not "keep it all".
 // Selected with B200BO_PREDICT_WARPS=16 (A/B measurements decide the default, see DESIGN.md).
 #pragma once
 #include "predict_kernels.cuh"
@@ -20,9 +24,13 @@ namespace b200bo {
 constexpr int P16_NT = 512;
 constexpr int P16_SPLIT = P16_NT / PBN;  // row quarters of every staged chunk in phase A
 
-__device__ __forceinline__ unsigned long long l2_policy_evict_last() {
+// evict_last on a fraction `frac` of the lines (the rest evict_unchanged); frac <= 0: evict_normal, i.e. no hint
+__device__ __forceinline__ unsigned long long l2_policy_evict_last(float frac) {
     unsigned long long p;
-    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;\n" : "=l"(p));
+    if (frac > 0.f)
+        asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, %1;\n" : "=l"(p) : "f"(frac));
+    else
+        asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;\n" : "=l"(p));
     return p;
 }
 __device__ __forceinline__ unsigned long long l2_policy_evict_first() {
@@ -169,9 +177,16 @@ __device__ __forceinline__ void predict16_load_stage(double* as, double* bs, con
     }
 }
 
-// ---- phase B: mma.sync m8n8k4 f64; 16 warps, warp tile 32(m) x 32(n); red[4][PBN] ----------------
+// ---- phase B: mma.sync f64; 16 warps, warp tile 32(m) x 32(n); red[4][PBN] ------------------------
+// MMA = 1684: m16n8k4 (sm_90, DMMA.16x8x4), the default; MMA = 884: m8n8k4 (sm_80, DMMA.8x8x4) for A/B.
+// Both load the same fragments: a[i] = A(row wm*32 + i*8 + g, k-row t4), b[j] = B(k-row t4, column wn*32 + j*8 + g),
+// conflict-free (PSTR_DMMA).  m16n8k4 tile mi takes a[2mi] (rows g) and a[2mi+1] (rows g+8) as its a0/a1, so its
+// c0..c3 are acc[2mi][j][0..1] and acc[2mi+1][j][0..1]: acc[i][j][e] is V row wm*32 + i*8 + g, candidate
+// wn*32 + j*8 + 2*t4 + e for both shapes and the epilogue is shared.
+template <int MMA>
 __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* __restrict__ Ks, double* smem,
                                                   unsigned long long pol_last, unsigned long long pol_first) {
+    static_assert(MMA == 884 || MMA == 1684, "phase B shape");
     constexpr int STR = PSTR_DMMA, BK = PBK_DMMA;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // the four warps of an SM sub-partition (equal warp & 3) own the four different row slabs, so skipping the
@@ -224,10 +239,19 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
                     for (int i = 0; i < 4; ++i) a[i] = as[krow + i * 8];
 #pragma unroll
                     for (int j = 0; j < 4; ++j) b[j] = bs[krow + j * 8];
+                    if constexpr (MMA == 1684) {
 #pragma unroll
-                    for (int i = 0; i < 4; ++i)
+                        for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+                            for (int j = 0; j < 4; ++j)
+                                dmma1684(acc[2 * mi][j][0], acc[2 * mi][j][1], acc[2 * mi + 1][j][0],
+                                         acc[2 * mi + 1][j][1], a[2 * mi], a[2 * mi + 1], b[j]);
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+                    }
                 }
             }
         }
@@ -266,7 +290,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
     __syncthreads();
 }
 
-template <bool DREG>
+template <bool DREG, int MMA>
 __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictParams P) {
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
@@ -277,7 +301,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
     const int tid = threadIdx.x;
     double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
     const long long ntiles = (P.m + PBN - 1) / PBN;
-    const unsigned long long pol_last = l2_policy_evict_last(), pol_first = l2_policy_evict_first();
+    const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last), pol_first = l2_policy_evict_first();
     if (P.sel_cta) {
         if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
         __syncthreads();
@@ -287,7 +311,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
             predict16_phase_a<DREG>(P, G, c0, Ks, smem, mu_s, pol_first);
-            predict16_phase_b(G, Ks, smem, pol_last, pol_first);
+            predict16_phase_b<MMA>(G, Ks, smem, pol_last, pol_first);
             const double* red = smem;
             if (tid < PBN) {
                 const int c = tid;

@@ -56,6 +56,7 @@ struct PredictParams {
     double* scratch;   // gridDim.x * scratch_stride doubles
     long long scratch_stride;
     unsigned long long* clamp_count;  // nullable; [0] negative variances clamped to 0, [1] non-finite candidate coordinates
+    float linv_l2_last;  // predict_acq16_kernel: evict_last fraction of the L^-1 loads; <= 0: evict_normal
 };
 
 // coordinate j of candidate gi (local index) as the reference's x_tries[gi, j]
@@ -91,6 +92,18 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
                  : "+d"(c0), "+d"(c1)
                  : "d"(a), "d"(b));
+}
+
+// sm_90 shape (SASS DMMA.16x8x4): twice the fp64 tensor rate of m8n8k4 per SM and clock on H100, the same rate as
+// m16n8k8 / m16n8k16 (tools/dmma_shapes.cu, DESIGN.md 6) with the fragment registers of m8n8k4.
+// Fragments (PTX ISA, .f64), g = lane/4, t4 = lane%4:
+//   A 16x4: a0 (g, t4), a1 (g+8, t4)    B 4x8: b0 (t4, g)
+//   C 16x8: c0 (g, 2t4), c1 (g, 2t4+1), c2 (g+8, 2t4), c3 (g+8, 2t4+1)
+__device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, double& c3, double a0, double a1,
+                                         double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+                 : "d"(a0), "d"(a1), "d"(b));
 }
 
 // ---- per-candidate epilogue shared by the tiled and the small-batch kernels ---------------------
