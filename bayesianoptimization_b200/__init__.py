@@ -7,10 +7,11 @@ No CPU fallback: importing the compute classes without the built library raises 
 
 Two layers:
   * GP seam / C ABI (needs numpy, scipy, sklearn):  B200GaussianProcessRegressor, FusedAcquisition,
-    PosteriorPaths (posterior sample paths, resolved lazily)
+    PosteriorPaths, ConstrainedPaths (posterior sample paths, resolved lazily)
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
-    UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ThompsonSampling, ConstantLiar,
-    GPHedge, AcquisitionFunction, ConstraintModel, enable(optimizer) - resolved lazily on first access.
+    UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ThompsonSampling,
+    ConstrainedThompsonSampling, ConstantLiar, GPHedge, AcquisitionFunction, ConstraintModel, enable(optimizer) -
+    resolved lazily on first access.
 """
 from . import _lib
 from ._build import build_library
@@ -24,7 +25,8 @@ _PLUGIN = {
     "AcquisitionFunction": "acquisition", "UpperConfidenceBound": "acquisition",
     "ExpectedImprovement": "acquisition", "ProbabilityOfImprovement": "acquisition",
     "ConstantLiar": "acquisition", "GPHedge": "acquisition", "DeviceHooks": "acquisition",
-    "ThompsonSampling": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths",
+    "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
+    "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
 }
 
 

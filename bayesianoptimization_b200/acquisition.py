@@ -16,7 +16,8 @@ inherited), with ``DeviceHooks`` mixed in:
                               the device closure)
 
 ``ThompsonSampling`` is the one policy defined here rather than inherited: a posterior sample path per
-``suggest()``, ranked and refined through the same three hooks.
+``suggest()``, ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`` extends it to
+constrained problems (the paths of the target and the constraint GPs, ranked feasible-first).
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
 (gpr.B200GaussianProcessRegressor), ``fused.FusedAcquisition`` and the C ABI do not need it.
@@ -181,6 +182,32 @@ class ThompsonSampling(DeviceHooks, _ref.AcquisitionFunction):
         self.n_features = int(params["n_features"])
 
 
+class ConstrainedThompsonSampling(ThompsonSampling):
+    """Thompson sampling that also serves constrained problems (the SCBO rule: Eriksson & Poloczek, "Scalable
+    Constrained Bayesian Optimization", AISTATS 2021).
+
+    Every ``suggest()`` draws one posterior path of the target GP and one of each constraint GP, in that order, from
+    the RandomState ``suggest`` receives (each with ``draw_path_inputs`` of its own GP and the same n_features).
+    Among the candidates the sampled constraints call feasible it proposes the one with the largest sampled target;
+    when none is feasible, the one with the smallest total violation (``paths.ConstrainedPaths``).  Unlike EI / PoI
+    it needs no feasible registered point, so it does not raise NoValidPointRegisteredError.  Without a constraint
+    it is ThompsonSampling.  The constraint GPs must be device GPs (``enable(optimizer)`` makes them so)."""
+
+    def _get_acq(self, gp, constraint=None):
+        if constraint is None:
+            return super()._get_acq(gp, constraint=None)
+        from .paths import ConstrainedPaths, PathAcquisition
+
+        gp = _as_b200_gp(gp)
+        models = [_as_b200_gp(m) for m in constraint.model]  # before any draw: a refusal consumes no random numbers
+        if len(models) + 1 > B.MAX_GPS:
+            raise NotImplementedError(f"at most {B.MAX_GPS - 1} constraint GPs are supported")
+        rs = self._path_rng if self._path_rng is not None else _ensure_rng(None)
+        target = gp.sample_paths(1, self.n_features, random_state=rs)
+        paths = [m.sample_paths(1, self.n_features, random_state=rs) for m in models]
+        return PathAcquisition(ConstrainedPaths(target, paths, constraint.lb, constraint.ub))
+
+
 _HOOKED = {
     _ref.UpperConfidenceBound: UpperConfidenceBound,
     _ref.ProbabilityOfImprovement: ProbabilityOfImprovement,
@@ -230,6 +257,6 @@ class GPHedge(_ref.GPHedge):
 # isinstance(x, bayes_opt.acquisition.AcquisitionFunction) does in the reference (abc virtual subclasses:
 # the concrete classes keep the reference's MRO).
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, ConstantLiar, GPHedge,
-             ThompsonSampling):
+             ThompsonSampling, ConstrainedThompsonSampling):
     AcquisitionFunction.register(_cls)
 del _cls

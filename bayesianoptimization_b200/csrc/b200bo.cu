@@ -1,5 +1,6 @@
 // b200bo.cu - C ABI (include/b200bo.h) over the sm_90a kernels.  No CPU fallback: every
 // compute entry point needs a CUDA device and reports B200BO_ERR_CUDA without one.
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
@@ -1560,7 +1561,9 @@ struct b200bo_paths {
     int n = 0, np = 0, d = 0, q = 0, L = 0, Lp = 0, cov = 0;
     double constv = 1.0, feat_scale = 0.0, y_mean = 0.0, y_std = 1.0;
     bool has_xf = false;
+    std::vector<double> bound;  // (q,) B_p >= |path_p(x)| everywhere (b200bo_paths_bound)
     DevBuf Xs, V, omega, bias, W, ls, xf, xc, out, sel_cta, sel, pbounds, prow, bad;
+    DevBuf cvals, cmerit, craw;  // constrained calls with this handle as set 0: [G][chunk][q] values, outputs
     ChunkedUpload upload;
 };
 
@@ -1661,6 +1664,8 @@ static int paths_setup(b200bo_gp* gp, b200bo_paths* ps, const double* omega, con
     // a smaller path never lowers the limit below what a path drawn earlier launches with.
     CU(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)paths_smem_bytes(B200BO_MAX_DIM, paths_qt(q), true)));
+    CU(cudaFuncSetAttribute(cpaths_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)cpaths_smem_bytes(B200BO_MAX_PATHS)));
     const size_t smem = paths_smem_bytes(d, q, true);
     int bps = 0;
     CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, fn, PT_NT, smem));
@@ -1720,6 +1725,14 @@ static int paths_setup(b200bo_gp* gp, b200bo_paths* ps, const double* omega, con
     for (int i = 0; i < n; ++i)
         for (int p = 0; p < q; ++p) Vrow[(size_t)i * q + p] = R[(size_t)p * np + i];
     CU(cudaMemcpy(ps->V.p, Vrow.data(), sizeof(double) * Vrow.size(), cudaMemcpyHostToDevice));
+    // |cos| <= 1 and 0 <= c k <= c: B_p = |y_mean| + y_std (feat_scale sum_l |w_lp| + c sum_i |v_ip|) bounds |path_p|
+    ps->bound.assign(q, 0.0);
+    for (int p = 0; p < q; ++p) {
+        double sw = 0.0, sv = 0.0;
+        for (int l = 0; l < L; ++l) sw += std::fabs(w[(size_t)l * q + p]);
+        for (int i = 0; i < n; ++i) sv += std::fabs(Vrow[(size_t)i * q + p]);
+        ps->bound[p] = std::fabs(ps->y_mean) + ps->y_std * (ps->feat_scale * sw + ps->constv * sv);
+    }
     return B200BO_OK;
 }
 
@@ -1761,7 +1774,8 @@ extern "C" void b200bo_paths_destroy(b200bo_paths* ps) {
     if (!ps) return;
     cudaSetDevice(ps->device);
     DevBuf* bufs[] = {&ps->Xs, &ps->V, &ps->omega, &ps->bias, &ps->W, &ps->ls, &ps->xf, &ps->xc,
-                      &ps->out, &ps->sel_cta, &ps->sel, &ps->pbounds, &ps->prow, &ps->bad};
+                      &ps->out, &ps->sel_cta, &ps->sel, &ps->pbounds, &ps->prow, &ps->bad,
+                      &ps->cvals, &ps->cmerit, &ps->craw};
     for (DevBuf* b : bufs) b->release();
     ps->upload.release();
     delete ps;
@@ -1828,6 +1842,41 @@ extern "C" int b200bo_paths_argmin_topk(b200bo_paths* ps, const double* Xc, int6
     return B200BO_OK;
 }
 
+// Philox bounds (lo_j, hi_j - lo_j) of the throughput mode into ps->pbounds
+static int paths_set_pbounds(b200bo_paths* ps, const double* lo, const double* hi) {
+    const int d = ps->d;
+    double pb[2 * B200BO_MAX_DIM];
+    for (int j = 0; j < d; ++j) {
+        if (!(lo[j] <= hi[j])) return set_err(B200BO_ERR_ARG, "Philox bounds: lo > hi in column %d", j);
+        pb[j] = lo[j];
+        pb[d + j] = hi[j] - lo[j];
+    }
+    int rc;
+    if ((rc = ps->pbounds.reserve(sizeof(double) * 2 * B200BO_MAX_DIM))) return rc;
+    CU(cudaMemcpy(ps->pbounds.p, pb, sizeof(double) * 2 * d, cudaMemcpyHostToDevice));
+    return B200BO_OK;
+}
+
+// the Philox rows of the q (k+1) merged records in ps->sel: best_x (q,d), topk_x (q,k,d) host, either nullable
+static int paths_winner_rows(b200bo_paths* ps, uint64_t seed, int k, double* best_x, double* topk_x) {
+    if (!best_x && !(topk_x && k > 0)) return B200BO_OK;
+    const int kk = k > 0 ? k : 1, d = ps->d, q = ps->q, nrec = q * (kk + 1);
+    int rc;
+    if ((rc = ps->prow.reserve(sizeof(double) * (size_t)nrec * d))) return rc;
+    philox_rows_kernel<<<nrec, 64>>>(seed, ps->pbounds.as<double>(), d, ps->sel.as<SelRecord>(), nrec,
+                                     ps->prow.as<double>());
+    LAUNCHED();
+    CU(cudaGetLastError());
+    std::vector<double> rows((size_t)nrec * d);
+    CU(cudaMemcpy(rows.data(), ps->prow.p, sizeof(double) * rows.size(), cudaMemcpyDeviceToHost));
+    for (int p = 0; p < q; ++p) {
+        const double* rp = rows.data() + (size_t)p * (kk + 1) * d;
+        if (best_x) memcpy(best_x + (size_t)p * d, rp, sizeof(double) * d);
+        if (topk_x && k > 0) memcpy(topk_x + (size_t)p * k * d, rp + d, sizeof(double) * (size_t)k * d);
+    }
+    return B200BO_OK;
+}
+
 extern "C" int b200bo_paths_argmin_topk_philox(b200bo_paths* ps, uint64_t seed, const double* lo, const double* hi,
                                                int64_t m, int64_t index_base, int k, double* best_val,
                                                int64_t* best_idx, double* best_x, double* topk_val,
@@ -1837,19 +1886,12 @@ extern "C" int b200bo_paths_argmin_topk_philox(b200bo_paths* ps, uint64_t seed, 
     if (m <= 0) return set_err(B200BO_ERR_ARG, "m must be > 0");
     CU(cudaSetDevice(ps->device));
     NvtxRange nvtx_range("b200bo:paths_select");
-    const int kk = k > 0 ? k : 1, d = ps->d, q = ps->q;
-    double pb[2 * B200BO_MAX_DIM];
-    for (int j = 0; j < d; ++j) {
-        if (!(lo[j] <= hi[j])) return set_err(B200BO_ERR_ARG, "Philox bounds: lo > hi in column %d", j);
-        pb[j] = lo[j];
-        pb[d + j] = hi[j] - lo[j];
-    }
+    const int kk = k > 0 ? k : 1, q = ps->q;
     const int grid = paths_grid(ps, m);
     int rc;
-    if ((rc = ps->pbounds.reserve(sizeof(double) * 2 * B200BO_MAX_DIM))) return rc;
+    if ((rc = paths_set_pbounds(ps, lo, hi))) return rc;
     if ((rc = ps->sel_cta.reserve(sizeof(SelList) * (size_t)q * grid))) return rc;
     if ((rc = ps->sel.reserve(sizeof(SelRecord) * (size_t)q * (kk + 1)))) return rc;
-    CU(cudaMemcpy(ps->pbounds.p, pb, sizeof(double) * 2 * d, cudaMemcpyHostToDevice));
     PathsParams P = paths_params(ps);
     P.pbounds = ps->pbounds.as<double>();
     P.seed = seed;
@@ -1859,25 +1901,172 @@ extern "C" int b200bo_paths_argmin_topk_philox(b200bo_paths* ps, uint64_t seed, 
     P.sel_k = kk;
     if ((rc = paths_launch(ps, P, grid, nullptr))) return rc;
     if ((rc = paths_merge(ps, grid, kk, nullptr))) return rc;
-    const int nrec = q * (kk + 1);
-    std::vector<SelRecord> rec((size_t)nrec);
+    std::vector<SelRecord> rec((size_t)q * (kk + 1));
     CU(cudaMemcpy(rec.data(), ps->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
     paths_unpack(rec, q, k, best_val, best_idx, topk_val, topk_idx);
-    if (best_x || (topk_x && k > 0)) {
-        if ((rc = ps->prow.reserve(sizeof(double) * (size_t)nrec * d))) return rc;
-        philox_rows_kernel<<<nrec, 64>>>(seed, ps->pbounds.as<double>(), d, ps->sel.as<SelRecord>(), nrec,
-                                         ps->prow.as<double>());
+    return paths_winner_rows(ps, seed, k, best_x, topk_x);
+}
+
+// ---------------------------------------------------------------------------------------
+// constrained Thompson sampling: the target's and the constraint GPs' paths ranked jointly (paths.cuh,
+// cpaths_select_kernel).  Per chunk of candidates every set's paths_eval_kernel writes its (chunk x q) values into
+// set 0's [G][chunk][q] scratch, then cpaths_select_kernel combines them; one merge per path at the end.
+// ---------------------------------------------------------------------------------------
+extern "C" int b200bo_paths_bound(const b200bo_paths* ps, double* bound) {
+    if (!ps || !bound) return set_err(B200BO_ERR_ARG, "NULL argument");
+    memcpy(bound, ps->bound.data(), sizeof(double) * ps->q);
+    return B200BO_OK;
+}
+
+static int cpaths_check(b200bo_paths* const* sets, int G, const double* lb, const double* ub, CPathsParams& C) {
+    if (!sets || !lb || !ub) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (G < 2 || G > B200BO_MAX_GPS)
+        return set_err(B200BO_ERR_ARG, "G=%d out of range [2,%d] (the target and 1..%d constraints)", G,
+                       B200BO_MAX_GPS, B200BO_MAX_GPS - 1);
+    for (int g = 0; g < G; ++g)
+        if (!sets[g]) return set_err(B200BO_ERR_ARG, "sets[%d] is NULL", g);
+    const b200bo_paths* s0 = sets[0];
+    for (int g = 1; g < G; ++g) {
+        if (sets[g]->device != s0->device) return set_err(B200BO_ERR_ARG, "sets[%d] lives on another device", g);
+        if (sets[g]->d != s0->d) return set_err(B200BO_ERR_ARG, "sets[%d]: d=%d, target d=%d", g, sets[g]->d, s0->d);
+        if (sets[g]->q != s0->q) return set_err(B200BO_ERR_ARG, "sets[%d]: q=%d, target q=%d", g, sets[g]->q, s0->q);
+    }
+    memset(&C, 0, sizeof(C));
+    for (int j = 1; j < G; ++j) {
+        if (!(lb[j - 1] <= ub[j - 1])) return set_err(B200BO_ERR_ARG, "constraint %d: lb > ub", j - 1);
+        C.lb[j] = lb[j - 1];
+        C.ub[j] = ub[j - 1];
+    }
+    for (int p = 0; p < s0->q; ++p) C.T[p] = 2.0 * s0->bound[p] + 1.0;
+    C.G = G;
+    C.q = s0->q;
+    return B200BO_OK;
+}
+
+// Xc: host rows, streamed through set 0's ChunkedUpload; nullptr: the Philox source of set 0's pbounds and `seed`,
+// generated chunk by chunk.  k > 0: -g folded into the per-path lists (merged into set 0's sel); merit / raw (host,
+// nullable): the (m,q) merit and the (m,G,q) values.  Returns with the work finished and the inputs checked.
+static int cpaths_run(b200bo_paths* const* sets, CPathsParams& C, const double* Xc, uint64_t seed, int64_t m,
+                      int64_t index_base, int k, double* merit, double* raw) {
+    b200bo_paths* s0 = sets[0];
+    const int G = C.G, q = C.q, d = s0->d;
+    const long long chunk = kChunkTilesPerSm * PBN * s0->sm_count;
+    const bool one = m <= chunk;
+    const long long cm = one ? m : chunk;
+    const int sgrid = (int)std::min<long long>((cm + CP_NT - 1) / CP_NT, 2LL * s0->sm_count);
+    ChunkedUpload& U = s0->upload;
+    int rc;
+    if ((rc = U.ensure())) return rc;
+    if ((rc = s0->cvals.reserve(sizeof(double) * (size_t)G * cm * q))) return rc;
+    if (merit && (rc = s0->cmerit.reserve(sizeof(double) * (size_t)cm * q))) return rc;
+    if (raw && (rc = s0->craw.reserve(sizeof(double) * (size_t)cm * G * q))) return rc;
+    if (k > 0) {
+        if ((rc = s0->sel_cta.reserve(sizeof(SelList) * (size_t)q * sgrid))) return rc;
+        if ((rc = s0->sel.reserve(sizeof(SelRecord) * (size_t)q * (k + 1)))) return rc;
+    }
+    CU(cudaMemsetAsync(s0->bad.p, 0, 2 * sizeof(unsigned long long), U.exec));
+    C.vals = s0->cvals.as<double>();
+    C.stride = cm;
+    C.sel_k = k;
+    C.merit = merit ? s0->cmerit.as<double>() : nullptr;
+    C.raw = raw ? s0->craw.as<double>() : nullptr;
+    C.sel_cta = k > 0 ? s0->sel_cta.as<SelList>() : nullptr;
+    auto work = [&](const double* dx, long long mc, long long c0, int i) -> int {
+        int r;
+        for (int g = 0; g < G; ++g) {
+            PathsParams P = paths_params(sets[g]);
+            P.Xc = dx;
+            P.pbounds = s0->pbounds.as<double>();
+            P.seed = seed;
+            P.index_base = index_base + c0;
+            P.m = mc;
+            P.clamp_count = s0->bad.as<unsigned long long>();
+            P.out = s0->cvals.as<double>() + (size_t)g * cm * q;
+            if ((r = paths_launch(sets[g], P, paths_grid(sets[g], mc), U.exec))) return r;
+        }
+        C.m = mc;
+        C.index_base = index_base + c0;
+        C.sel_resume = i > 0;
+        cpaths_select_kernel<<<sgrid, CP_NT, cpaths_smem_bytes(k > 0 ? q : 0), U.exec>>>(C);
         LAUNCHED();
         CU(cudaGetLastError());
-        std::vector<double> rows((size_t)nrec * d);
-        CU(cudaMemcpy(rows.data(), ps->prow.p, sizeof(double) * rows.size(), cudaMemcpyDeviceToHost));
-        for (int p = 0; p < q; ++p) {
-            const double* rp = rows.data() + (size_t)p * (kk + 1) * d;
-            if (best_x) memcpy(best_x + (size_t)p * d, rp, sizeof(double) * d);
-            if (topk_x && k > 0) memcpy(topk_x + (size_t)p * k * d, rp + d, sizeof(double) * (size_t)k * d);
-        }
+        // pageable host memory: each copy returns once it is done, in stream order behind the kernels
+        if (merit)
+            CU(cudaMemcpyAsync(merit + (size_t)c0 * q, C.merit, sizeof(double) * (size_t)mc * q,
+                               cudaMemcpyDeviceToHost, U.exec));
+        if (raw)
+            CU(cudaMemcpyAsync(raw + (size_t)c0 * G * q, C.raw, sizeof(double) * (size_t)mc * G * q,
+                               cudaMemcpyDeviceToHost, U.exec));
+        return B200BO_OK;
+    };
+    if (Xc) {
+        if ((rc = s0->xc.reserve(sizeof(double) * (size_t)(one ? 1 : 2) * cm * d))) return rc;
+        double* const buf[2] = {s0->xc.as<double>(), s0->xc.as<double>() + (one ? 0 : (size_t)cm * d)};
+        rc = U.run(Xc, m, d, cm, buf, [&](const double* dx, long long mc, long long c0, int i, bool) {
+            return work(dx, mc, c0, i);
+        });
+    } else {
+        int i = 0;
+        for (long long c0 = 0; c0 < m && rc == B200BO_OK; c0 += cm, ++i) rc = work(nullptr, std::min(cm, m - c0), c0, i);
     }
+    if (rc) return rc;
+    if (k > 0 && (rc = paths_merge(s0, sgrid, k, U.exec))) return rc;
+    CU(cudaStreamSynchronize(U.exec));
+    return Xc ? paths_check_nonfinite(s0) : B200BO_OK;
+}
+
+extern "C" int b200bo_cpaths_eval(b200bo_paths* const* sets, int G, const double* lb, const double* ub,
+                                  const double* Xc, int64_t m, double* merit, double* raw) {
+    CPathsParams C;
+    int rc;
+    if ((rc = cpaths_check(sets, G, lb, ub, C))) return rc;
+    if (m < 0 || (m > 0 && (!Xc || !merit))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    CU(cudaSetDevice(sets[0]->device));
+    NvtxRange nvtx_range("b200bo:cpaths_eval");
+    return cpaths_run(sets, C, Xc, 0, m, 0, 0, merit, raw);
+}
+
+extern "C" int b200bo_cpaths_argmin_topk(b200bo_paths* const* sets, int G, const double* lb, const double* ub,
+                                         const double* Xc, int64_t m, int k, double* best_val, int64_t* best_idx,
+                                         double* topk_val, int64_t* topk_idx) {
+    CPathsParams C;
+    int rc;
+    if ((rc = cpaths_check(sets, G, lb, ub, C))) return rc;
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (m <= 0 || !Xc) return set_err(B200BO_ERR_ARG, "m must be > 0");
+    b200bo_paths* s0 = sets[0];
+    CU(cudaSetDevice(s0->device));
+    NvtxRange nvtx_range("b200bo:cpaths_select");
+    const int kk = k > 0 ? k : 1;
+    if ((rc = cpaths_run(sets, C, Xc, 0, m, 0, kk, nullptr, nullptr))) return rc;
+    std::vector<SelRecord> rec((size_t)C.q * (kk + 1));
+    CU(cudaMemcpy(rec.data(), s0->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
+    paths_unpack(rec, C.q, k, best_val, best_idx, topk_val, topk_idx);
     return B200BO_OK;
+}
+
+extern "C" int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G, const double* lb,
+                                                const double* ub, uint64_t seed, const double* lo, const double* hi,
+                                                int64_t m, int64_t index_base, int k, double* best_val,
+                                                int64_t* best_idx, double* best_x, double* topk_val,
+                                                int64_t* topk_idx, double* topk_x) {
+    CPathsParams C;
+    int rc;
+    if ((rc = cpaths_check(sets, G, lb, ub, C))) return rc;
+    if (!lo || !hi) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (m <= 0) return set_err(B200BO_ERR_ARG, "m must be > 0");
+    b200bo_paths* s0 = sets[0];
+    CU(cudaSetDevice(s0->device));
+    NvtxRange nvtx_range("b200bo:cpaths_select");
+    const int kk = k > 0 ? k : 1;
+    if ((rc = paths_set_pbounds(s0, lo, hi))) return rc;
+    if ((rc = cpaths_run(sets, C, nullptr, seed, m, index_base, kk, nullptr, nullptr))) return rc;
+    std::vector<SelRecord> rec((size_t)C.q * (kk + 1));
+    CU(cudaMemcpy(rec.data(), s0->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
+    paths_unpack(rec, C.q, k, best_val, best_idx, topk_val, topk_idx);
+    return paths_winner_rows(s0, seed, k, best_x, topk_x);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -183,4 +183,77 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
         for (int p = 0; p < q; ++p) runsel_store(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, tid);
 }
 
+// ---------------------------------------------------------------------------------------
+// Constrained Thompson sampling (SCBO rule: Eriksson & Poloczek, AISTATS 2021).  G = 1 + J sets of q paths: set 0
+// the target, set j >= 1 constraint GP j with bounds [lb_j, ub_j].  Path p of every set is one joint draw.  Per
+// candidate and path, from the values paths_eval_kernel left in vals[g][i][p] (data units):
+//   viol = sum_{j=1..J} (max(0, lb_j - c_j) + max(0, c_j - ub_j))         in j order
+//   g    = f                       if viol == 0
+//        = -T_p (1 + viol)         otherwise,   T_p = 2 B_p + 1 > 2 max|f_p|
+// so every infeasible merit lies below every feasible one, and the infeasible tier still resolves viol to relative
+// round-off (an additive offset T + viol would resolve it only to ulp(T)).  Explicit _rn intrinsics: no FMA
+// contraction, so a numpy restatement on the raw values reproduces g bit for bit.  max() propagates NaN, as
+// np.maximum does.  Output: g (m x q), the raw values (m x G x q), and/or -g folded into one list per path.
+// ---------------------------------------------------------------------------------------
+constexpr int CP_NT = 128;
+
+struct CPathsParams {
+    const double* vals;  // [G][stride][q]
+    long long stride;    // rows per set in vals
+    long long m;         // rows of this launch
+    long long index_base;
+    int G, q, sel_k, sel_resume;
+    double lb[B200BO_MAX_GPS], ub[B200BO_MAX_GPS];  // [j], j >= 1
+    double T[B200BO_MAX_PATHS];
+    double* merit;      // [m][q] or nullptr
+    double* raw;        // [m][G][q] or nullptr
+    SelList* sel_cta;   // [q][gridDim.x] or nullptr
+};
+
+__host__ __device__ inline size_t cpaths_smem_bytes(int q) { return sizeof(SelShared) * (size_t)q; }
+
+__device__ __forceinline__ double cp_pos(double x) { return (x > 0.0 || x != x) ? x : 0.0; }
+
+__global__ void __launch_bounds__(CP_NT) cpaths_select_kernel(const CPathsParams P) {
+    extern __shared__ __align__(16) unsigned char cp_smem[];
+    SelShared* sel = reinterpret_cast<SelShared*>(cp_smem);
+    __shared__ double lb_s[B200BO_MAX_GPS], ub_s[B200BO_MAX_GPS], T_s[B200BO_MAX_PATHS];
+    const int t = threadIdx.x, q = P.q, G = P.G;
+    if (t == 0) {  // constant indices: the parameter arrays stay in the constant bank
+#pragma unroll
+        for (int j = 0; j < B200BO_MAX_GPS; ++j) {
+            lb_s[j] = P.lb[j];
+            ub_s[j] = P.ub[j];
+        }
+#pragma unroll
+        for (int p = 0; p < B200BO_MAX_PATHS; ++p) T_s[p] = P.T[p];
+    }
+    if (P.sel_cta)
+        for (int p = 0; p < q; ++p) runsel_begin(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, P.sel_resume, t);
+    __syncthreads();
+    const long long ntiles = (P.m + CP_NT - 1) / CP_NT;
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long gi = tile * CP_NT + t;
+        const bool valid = gi < P.m;
+        for (int p = 0; p < q; ++p) {
+            double g = 0.0;
+            if (valid) {
+                const double f = P.vals[gi * q + p];
+                double viol = 0.0;
+                for (int j = 1; j < G; ++j) {
+                    const double c = P.vals[((size_t)j * P.stride + gi) * q + p];
+                    viol = __dadd_rn(viol, __dadd_rn(cp_pos(__dsub_rn(lb_s[j], c)), cp_pos(__dsub_rn(c, ub_s[j]))));
+                    if (P.raw) P.raw[((size_t)gi * G + j) * q + p] = c;
+                }
+                g = viol == 0.0 ? f : __dmul_rn(-T_s[p], __dadd_rn(1.0, viol));
+                if (P.raw) P.raw[(size_t)gi * G * q + p] = f;
+                if (P.merit) P.merit[gi * q + p] = g;
+            }
+            if (P.sel_cta) runsel_update<1>(sel[p], P.sel_k, t, -g, gi + P.index_base, valid);
+        }
+    }
+    if (P.sel_cta)
+        for (int p = 0; p < q; ++p) runsel_store(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, t);
+}
+
 }  // namespace b200bo

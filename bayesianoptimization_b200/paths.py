@@ -149,6 +149,117 @@ class PosteriorPaths:
         return bi, bv, bx, [ti[p][keep[p]] for p in range(q)], [tx[p][keep[p]] for p in range(q)]
 
 
+    def bound(self):
+        """(q,) B_p >= |path_p(x)| for every x (computed at creation from the path's own weights)."""
+        out = np.empty(self.n_paths)
+        B.check(B.lib().b200bo_paths_bound(self._handle.ptr, B.as_dp(out)))
+        return out
+
+
+class ConstrainedPaths:
+    """Joint posterior paths of a target GP and J constraint GPs, ranked feasible-first (SCBO: Eriksson & Poloczek,
+    "Scalable Constrained Bayesian Optimization", AISTATS 2021).  Path p of every set is one joint draw; per
+    candidate x and path p, with f the target path and c_j constraint path j (data units):
+
+        viol_p(x)  = sum_j (max(0, lb_j - c_j) + max(0, c_j - ub_j))            (0 iff every lb_j <= c_j <= ub_j)
+        merit_p(x) = f  if viol_p(x) == 0,  else  -T_p (1 + viol_p(x)),    T_p = 2 B_p + 1 (target.bound())
+
+    Every infeasible merit lies below every feasible one, and among infeasible candidates the smallest violation
+    ranks first, so no feasible point needs to be registered.  The interface is PosteriorPaths': ``paths(X)`` ->
+    (M, q) merit, ``raw(X)`` -> (M, G, q) values, ``argmin_topk`` / ``argmin_topk_philox`` rank -merit_p on the
+    device (``b200bo_cpaths_*``), so ``PathAcquisition(ConstrainedPaths(...))`` is a device closure."""
+
+    def __init__(self, target, constraints, lb, ub):
+        sets = [target, *constraints]
+        if not constraints:
+            raise ValueError("ConstrainedPaths needs at least one constraint set (use PosteriorPaths without)")
+        if len(sets) > B.MAX_GPS:
+            raise ValueError(f"at most {B.MAX_GPS - 1} constraint sets are supported, got {len(constraints)}")
+        lb = np.asarray(lb, dtype=np.float64).reshape(-1)
+        ub = np.asarray(ub, dtype=np.float64).reshape(-1)
+        if lb.shape != (len(constraints),) or ub.shape != (len(constraints),):
+            raise ValueError(f"lb and ub need one entry per constraint set ({len(constraints)})")
+        if not np.all(lb <= ub):
+            raise ValueError("constraint bounds: lb > ub")
+        for j, s in enumerate(constraints):
+            if s.n_paths != target.n_paths:
+                raise ValueError(f"constraint set {j} has {s.n_paths} paths, the target {target.n_paths}")
+            if s.dim != target.dim:
+                raise ValueError(f"constraint set {j} has d={s.dim}, the target d={target.dim}")
+            if s.device != target.device:
+                raise ValueError(f"constraint set {j} lives on device {s.device}, the target on {target.device}")
+        modes = [s._xform for s in sets]
+        host = [a for m, a in modes if m == "host"]
+        # `==`, not `is`: the reference hands every GP `space.kernel_transform`, a new bound method per access
+        if host and (len(host) != len(modes) or any(h != host[0] for h in host)):
+            raise NotImplementedError("the sets use different host-side input transforms")
+        self.target, self.constraints = target, list(constraints)
+        self._sets = sets  # keeps every handle alive as long as this object
+        self._ptrs = (C.c_void_p * len(sets))(*[s._handle.ptr.value for s in sets])
+        self._lb, self._ub = B.c_f64(lb), B.c_f64(ub)
+        self._xform = modes[0]
+        self.n_paths = target.n_paths
+        self.n_sets = len(sets)
+        self.dim = target.dim
+        self.device = target.device
+        self.devices = [self.device]
+
+    def _args(self):
+        return self._ptrs, self.n_sets, B.as_dp(self._lb), B.as_dp(self._ub)
+
+    def _candidates(self, X):
+        return PosteriorPaths._candidates(self, X)  # the host-side transform, once for every set
+
+    def _eval(self, X, raw):
+        X = self._candidates(X)
+        m, q = X.shape[0], self.n_paths
+        merit = np.empty((m, q))
+        out = np.empty((m, self.n_sets, q)) if raw else None
+        B.check(B.lib().b200bo_cpaths_eval(*self._args(), B.as_dp(X), m, B.as_dp(merit),
+                                           B.as_dp(out) if raw else None))
+        return out if raw else merit
+
+    def __call__(self, X):
+        """(M, q) merit at the rows of X."""
+        return self._eval(X, raw=False)
+
+    def raw(self, X):
+        """(M, G, q) path values at the rows of X: [:, 0] the target's, [:, j] constraint set j's (data units)."""
+        return self._eval(X, raw=True)
+
+    def argmin_topk(self, X, k):
+        """Per path p: np.argmin and the k smallest (np.argsort order) of -merit_p over the rows of X.
+        Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
+        X = self._candidates(X)
+        k, q = int(k), self.n_paths
+        bv, bi = np.empty(q), np.empty(q, dtype=np.int64)
+        tv, ti = np.empty(q * max(k, 1)), np.empty(q * max(k, 1), dtype=np.int64)
+        B.check(B.lib().b200bo_cpaths_argmin_topk(*self._args(), B.as_dp(X), X.shape[0], k, B.as_dp(bv),
+                                                  bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tv),
+                                                  ti.ctypes.data_as(C.POINTER(C.c_int64))))
+        tops = [t[t >= 0] for t in ti[:q * k].reshape(q, k)]
+        return bi, bv, tops
+
+    def argmin_topk_philox(self, seed, bounds, m, k, index_base=0):
+        """Throughput mode as PosteriorPaths.argmin_topk_philox, ranking -merit_p.
+        Returns (idx (q,), values (q,), x_best (q, d), [top-k indices], [top-k rows])."""
+        if self._xform[0] == "host":
+            raise NotImplementedError("device candidate generation with a host-side kernel transform")
+        bounds = B.c_f64(np.asarray(bounds, dtype=np.float64).reshape(self.dim, 2))
+        lo, hi = B.c_f64(bounds[:, 0]), B.c_f64(bounds[:, 1])
+        k, q, d = int(k), self.n_paths, self.dim
+        kk = max(k, 1)
+        bv, bi, bx = np.empty(q), np.empty(q, dtype=np.int64), np.empty((q, d))
+        tv, ti, tx = np.empty(q * kk), np.empty(q * kk, dtype=np.int64), np.empty((q * kk, d))
+        B.check(B.lib().b200bo_cpaths_argmin_topk_philox(
+            *self._args(), int(seed) & 0xFFFFFFFFFFFFFFFF, B.as_dp(lo), B.as_dp(hi), int(m), int(index_base), k,
+            B.as_dp(bv), bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(bx), B.as_dp(tv),
+            ti.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tx)))
+        ti, tx = ti[:q * k].reshape(q, k), tx[:q * k].reshape(q, k, d)
+        keep = ti >= 0
+        return bi, bv, bx, [ti[p][keep[p]] for p in range(q)], [tx[p][keep[p]] for p in range(q)]
+
+
 class PathAcquisition:
     """Acquisition closure over path 0 of a PosteriorPaths: x (M,d)|(d,) -> (M,) values of -path(x), with the
     device selection of the random stage (``argmin_topk``, ``argmin_topk_philox``) in the signatures of

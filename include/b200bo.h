@@ -286,6 +286,32 @@ int b200bo_paths_argmin_topk(b200bo_paths* paths, const double* Xc, int64_t m, i
 int b200bo_paths_argmin_topk_philox(b200bo_paths* paths, uint64_t seed, const double* lo, const double* hi, int64_t m,
                                     int64_t index_base, int k, double* best_val, int64_t* best_idx, double* best_x,
                                     double* topk_val, int64_t* topk_idx, double* topk_x);
+/* bound: (q,) host.  B_p = |y_mean| + y_std (sqrt(2 const_value / L) sum_l |w[l][p]| + const_value sum_i |v[i][p]|),
+ * computed at creation: |path_p(x)| <= B_p for every x, since |cos| <= 1 and 0 <= const_value k <= const_value. */
+int b200bo_paths_bound(const b200bo_paths* paths, double* bound);
+
+/* ---- constrained Thompson sampling (SCBO rule: Eriksson & Poloczek, AISTATS 2021) ------------------------------
+ * The reference raises NoValidPointRegisteredError in EI / PoI until a registered point is feasible
+ * (R/bayes_opt/acquisition.py:888-896); this rule needs no feasible point.  sets[0] = paths of the target GP,
+ * sets[j] (1 <= j < G) = paths of constraint GP j with bounds lb[j-1] <= ub[j-1] (+-inf allowed); path p of every set
+ * is one joint draw.  Per candidate x and path p, with f = sets[0] path p at x and c_j = sets[j] path p at x:
+ *   viol_p(x)  = sum_{j=1..G-1}, in j order, of (max(0, lb_j - c_j) + max(0, c_j - ub_j))   (0 iff lb_j <= c_j <= ub_j)
+ *   merit_p(x) = f                              if viol_p(x) == 0
+ *              = -T_p (1 + viol_p(x))           otherwise,  T_p = 2 B_p + 1 (B_p of sets[0], b200bo_paths_bound)
+ * so every infeasible merit lies below every feasible one.  Adds, subtracts, max (NaN-propagating, as np.maximum)
+ * and one multiply, in this order and without FMA contraction.  The selection entries rank -merit_p with the
+ * semantics of b200bo_paths_argmin_topk.  G <= B200BO_MAX_GPS; every set on the same device with the same d and q,
+ * else B200BO_ERR_ARG.  The scratch lives in sets[0]; the handles are not thread-safe. */
+/* merit: (m,q) host; raw: (m,G,q) host or NULL - raw[i][g][p] = path p of sets[g] at row i. */
+int b200bo_cpaths_eval(b200bo_paths* const* sets, int G, const double* lb, const double* ub, const double* Xc,
+                       int64_t m, double* merit, double* raw);
+int b200bo_cpaths_argmin_topk(b200bo_paths* const* sets, int G, const double* lb, const double* ub, const double* Xc,
+                              int64_t m, int k, double* best_val, int64_t* best_idx, double* topk_val,
+                              int64_t* topk_idx);
+int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G, const double* lb, const double* ub,
+                                     uint64_t seed, const double* lo, const double* hi, int64_t m, int64_t index_base,
+                                     int k, double* best_val, int64_t* best_idx, double* best_x, double* topk_val,
+                                     int64_t* topk_idx, double* topk_x);
 
 /* Duration (ms) of the most recent fused predict+acquisition kernel launched through a
  * device or host entry point on this thread, measured with CUDA events on its stream.

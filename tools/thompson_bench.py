@@ -8,6 +8,11 @@ For C3 (N = 4096, d = 16) and C5 (N = 8192, d = 32), fixed hyper-parameters, it 
   * ei               FusedAcquisition.argmin_topk (b200bo_acq_argmin_topk, k = 10),
 on the same M host candidates: CUDA events on the default stream around each call (the calls return with their
 results on the host, so a window includes the streamed H2D copy of the batch), after warm-up, mean over the steps.
+The C4 leg (N = 2048, d = 16, two constraint GPs, --m-c4 = 2^19 candidates) times
+  * cts_q1           ConstrainedPaths.argmin_topk (b200bo_cpaths_argmin_topk, k = 10): one path of the target and one of
+                     each constraint GP, ranked feasible-first,
+  * ts_q1            the target's path alone (PosteriorPaths.argmin_topk), for the cost of the joint ranking,
+  * poi_constrained  FusedAcquisition PoI x probability of feasibility (b200bo_acq_argmin_topk, k = 10).
 Also reported: the one-off path creation (draws on the host + one O(N^2) solve per path).  Rates: cand/s = M / time,
 path*cand/s = q M / time.  The GPU name and power limit are read in the same run.
 """
@@ -27,6 +32,7 @@ if ROOT not in sys.path:
 import numpy as np  # noqa: E402
 
 CONFIGS = {"C3": (4096, 16), "C5": (8192, 32)}
+C4 = (2048, 16, 2)  # N, d, constraint GPs
 
 
 def device_info():
@@ -58,13 +64,54 @@ def timed(fn, steps, warmup):
     return float(np.mean(ms)), float(np.min(ms))
 
 
+def c4_leg(bo, args):
+    from types import SimpleNamespace
+
+    from sklearn.gaussian_process.kernels import Matern
+
+    from bayesianoptimization_b200.paths import ConstrainedPaths
+
+    n, d, J = C4
+    m = args.m_c4
+    rs = np.random.RandomState(0)
+    X = rs.uniform(size=(n, d))
+    Xc = rs.uniform(size=(m, d))
+    mk = lambda y: bo.B200GaussianProcessRegressor(kernel=Matern(0.5 * np.sqrt(d), nu=2.5), alpha=1e-6,  # noqa: E731
+                                                   normalize_y=True, optimizer=None).fit(X, y)
+    y = np.sin(X.sum(1)) + 0.1 * rs.randn(n)
+    gp = mk(y)
+    cgps = [mk(np.cos(X[:, j::J].sum(1)) + 0.1 * rs.randn(n)) for j in range(J)]
+    lb, ub = np.array([-np.inf, -0.5]), np.array([0.3, np.inf])
+    res = {"N": n, "d": d, "constraint_gps": J, "m": m}
+    t = time.perf_counter()
+    path_rs = np.random.RandomState(1)
+    target = gp.sample_paths(1, args.features, random_state=path_rs)
+    cp = ConstrainedPaths(target, [g.sample_paths(1, args.features, random_state=path_rs) for g in cgps], lb, ub)
+    res["cts_q1_create_ms"] = 1e3 * (time.perf_counter() - t)
+    mean, best = timed(lambda: cp.argmin_topk(Xc, 10), args.steps, args.warmup)
+    res["cts_q1_ms"], res["cts_q1_min_ms"], res["cts_q1_cand_per_s"] = mean, best, m / (mean * 1e-3)
+    mean, best = timed(lambda: target.argmin_topk(Xc, 10), args.steps, args.warmup)
+    res["ts_q1_ms"], res["ts_q1_min_ms"] = mean, best
+    acq = bo.FusedAcquisition(bo._lib.ACQ_POI, gp, SimpleNamespace(model=cgps, lb=lb, ub=ub), xi=0.01,
+                              y_max=float(y.max()))
+    mean, best = timed(lambda: acq.argmin_topk(Xc, 10), args.steps, args.warmup)
+    res["poi_constrained_ms"], res["poi_constrained_min_ms"] = mean, best
+    res["poi_constrained_cand_per_s"] = m / (mean * 1e-3)
+    res["cts_q1_vs_ts_q1"] = res["cts_q1_ms"] / res["ts_q1_ms"]
+    res["cts_q1_speedup_vs_poi_constrained"] = res["poi_constrained_ms"] / res["cts_q1_ms"]
+    feas = np.mean(cp(Xc[:65536])[:, 0] == cp.raw(Xc[:65536])[:, 0, 0])
+    res["cts_feasible_fraction_first_65536"] = float(feas)
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--m", type=int, default=1 << 20)
     ap.add_argument("--features", type=int, default=4096)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
-    ap.add_argument("--configs", default="C3,C5")
+    ap.add_argument("--m-c4", type=int, default=1 << 19)
+    ap.add_argument("--configs", default="C3,C5,C4")
     args = ap.parse_args()
     import torch
 
@@ -77,6 +124,9 @@ def main():
     out = {"bench": "thompson_vs_ei", "device": device_info(), "m": args.m, "n_features": args.features, "k": 10,
            "steps": args.steps, "warmup": args.warmup, "configs": {}}
     for name in args.configs.split(","):
+        if name == "C4":
+            out["configs"][name] = c4_leg(bo, args)
+            continue
         n, d = CONFIGS[name]
         rs = np.random.RandomState(0)
         X = rs.uniform(size=(n, d))
