@@ -27,6 +27,8 @@ using namespace b200bo;
 
 constexpr int kDefaultPredictWarps = 16;  // measured A/B (DESIGN.md 6): 550.1 ms vs 561.7 ms per 2^20 candidates at C3
 constexpr float kDefaultLinvL2Last = 1.0f;  // evict_last fraction of the L^-1 loads (DESIGN.md 6)
+// phase B data path of predict_acq16_kernel: bulk copies without clusters, 4-5 % above cp.async at C3 (DESIGN.md 6)
+constexpr int kDefaultPredictPipe = PIPE_BULK;
 
 // ---------------------------------------------------------------------------------------
 // error plumbing
@@ -112,6 +114,8 @@ struct ChunkedUpload {
 struct b200bo_gp {
     int device = 0;
     int sm_count = 0;
+    int pair_grid = 0;  // CTAs of predict_acq16_kernel's clustered launch: 2 x max active clusters (0: not queried yet)
+    bool pipe_armed = false;  // a bulk-copy phase B ran on this handle: its timeout flag is worth reading
     long long n = 0;
     int np = 0, d = 0;
     bool has_data = false, fitted = false;
@@ -133,6 +137,9 @@ struct b200bo_gp {
     // fp32 mode: L^-1 as tf32 (hi,lo) wgmma operand images (built on first use after a fit)
     DevBuf tc_linv;
     bool tc_valid = false;
+    // bulk-copy phase B of the fp64 kernel: L^-1 as padded stage images (built on first use after a fit)
+    DevBuf pad_linv;
+    bool pad_valid = false;
     DevBuf cov_xc, cov_kst, cov_v, cov_c, cov_out, cov_mu;  // predict(return_cov=True) scratch
     DevBuf sel_cta;         // per-CTA running selection lists of the fused kernels
     DevBuf pbounds, prow;   // throughput mode: Philox bounds (lo, span) / regenerated winner rows
@@ -222,10 +229,14 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             kPredictSmemBytesTc));
     CU(cudaFuncSetAttribute(small_trsv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmallTrsvSmemBytes));
-    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 884>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 884>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 884, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 884, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
@@ -263,7 +274,7 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
                       &gp->alphav, &gp->v1, &gp->v2, &gp->ls, &gp->xf, &gp->info, &gp->part,
                       &gp->pscratch, &gp->xc, &gp->out_acq, &gp->out_mu, &gp->out_sd, &gp->sel,
                       &gp->clamp, &gp->s_ksm, &gp->s_partial, &gp->s_mupart, &gp->s_unit, &gp->s_rb, &gp->s_colsq,
-                      &gp->tc_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
+                      &gp->tc_linv, &gp->pad_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
                       &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside};
     for (DevBuf* b : bufs) b->release();
     if (gp->stream) cudaStreamDestroy(gp->stream);
@@ -336,6 +347,7 @@ extern "C" int b200bo_gp_set_data(b200bo_gp* gp, const double* X, const double* 
     gp->fitted = false;
     gp->replica = false;
     gp->tc_valid = false;
+    gp->pad_valid = false;
     gp->n = n;
     gp->d = d;
     gp->np = round_up(n, kPad);
@@ -795,6 +807,7 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     CU(cudaMemcpy(gp->y.p, gp->y_norm.data(), sizeof(double) * nn, cudaMemcpyHostToDevice));
     gp->n = nn;
     gp->tc_valid = false;
+    gp->pad_valid = false;
     if ((rc = solve_alpha(gp))) return rc;
     CU(cudaDeviceSynchronize());
     return B200BO_OK;
@@ -811,6 +824,7 @@ extern "C" int b200bo_gp_lml(b200bo_gp* gp, const b200bo_kernel* kern, double al
     NvtxRange nvtx_range("b200bo:lml");
     gp->fitted = false;  // buffers are being overwritten
     gp->tc_valid = false;
+    gp->pad_valid = false;
     const int n = (int)gp->n, np = gp->np, d = gp->d;
     const int aniso = kern->n_length_scale > 1;
     const int want_noise = (has_const & 2) ? 1 : 0;
@@ -1000,12 +1014,70 @@ static int predict_mma() {
     return (e && strcmp(e, "884") == 0) ? 884 : 1684;
 }
 
-template <int MMA>
-static void launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
-    if (dreg)
-        predict_acq16_kernel<true, MMA><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P);
-    else
-        predict_acq16_kernel<false, MMA><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P);
+// phase B data path of predict_acq16_kernel (m16n8k4 only; m8n8k4 keeps cp.async): B200BO_PREDICT_PIPE=bulk (bulk
+// copies on an mbarrier ring, L^-1 multicast across CTA pairs), bulk_nomc (the same without clusters) or cpasync
+// (per-thread cp.async under CTA barriers) overrides the default for A/B measurements
+static int predict_pipe() {
+    const char* e = getenv("B200BO_PREDICT_PIPE");
+    if (e && strcmp(e, "bulk") == 0) return PIPE_BULK_MC;
+    if (e && strcmp(e, "bulk_nomc") == 0) return PIPE_BULK;
+    if (e && strcmp(e, "cpasync") == 0) return PIPE_CPASYNC;
+    return kDefaultPredictPipe;
+}
+
+template <int MMA, int PIPE>
+static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
+    auto fn = dreg ? predict_acq16_kernel<true, MMA, PIPE> : predict_acq16_kernel<false, MMA, PIPE>;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(P16_NT);
+    cfg.dynamicSmemBytes = kPredictSmemBytesDmma;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    if (PIPE == PIPE_BULK_MC) {
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2;
+        attr[0].val.clusterDim.y = 1;
+        attr[0].val.clusterDim.z = 1;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+    }
+    CU(cudaLaunchKernelEx(&cfg, fn, P));
+    return B200BO_OK;
+}
+
+// grid of the clustered launch: two CTAs per cluster that can be resident at once, never more than one per SM
+static int predict_pair_grid(b200bo_gp* g0) {
+    if (g0->pair_grid > 0) return B200BO_OK;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(2);
+    cfg.blockDim = dim3(P16_NT);
+    cfg.dynamicSmemBytes = kPredictSmemBytesDmma;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    CU(cudaOccupancyMaxActiveClusters(&clusters, predict_acq16_kernel<true, 1684, PIPE_BULK_MC>, &cfg));
+    int nodreg = 0;
+    CU(cudaOccupancyMaxActiveClusters(&nodreg, predict_acq16_kernel<false, 1684, PIPE_BULK_MC>, &cfg));
+    clusters = nodreg < clusters ? nodreg : clusters;
+    if (clusters < 1) return set_err(B200BO_ERR_CUDA, "predict_acq16_kernel: no CTA pair fits on the device");
+    g0->pair_grid = 2 * clusters < g0->sm_count ? 2 * clusters : g0->sm_count & ~1;
+    return B200BO_OK;
+}
+
+// predict_acq16_kernel's bulk-copy phase B flags an mbarrier wait that ran out of its budget (a protocol error)
+static int check_pipe_timeout(b200bo_gp* g0) {
+    if (!g0->pipe_armed) return B200BO_OK;
+    unsigned long long f = 0;
+    CU(cudaSetDevice(g0->device));
+    CU(cudaMemcpyFromSymbol(&f, g_pipe_timeout, sizeof(f)));
+    if (f != 0) return set_err(B200BO_ERR_CUDA, "predict_acq16_kernel: a phase B pipeline wait timed out");
+    return B200BO_OK;
 }
 
 // evict_last fraction of predict_acq16_kernel's L^-1 loads; B200BO_PREDICT_L2=<fraction in (0,1]> or "none"
@@ -1018,6 +1090,20 @@ static float predict_linv_l2_last() {
         if (f > 0.f && f <= 1.f) return f;
     }
     return kDefaultLinvL2Last;
+}
+
+// padded stage images of L^-1 for the bulk-copy phase B of the fp64 kernel (once per fit)
+static int ensure_pad(b200bo_gp* gp, cudaStream_t stream) {
+    if (gp->pad_valid) return B200BO_OK;
+    const int np = gp->np;
+    int rc;
+    if ((rc = gp->pad_linv.reserve(sizeof(double) * pad_linv_doubles(np)))) return rc;
+    dim3 grid(np / PBK_DMMA, np / PBM);
+    pad_linv_stages_kernel<<<grid, 256, 0, stream>>>(gp->WT.as<double>(), np, gp->pad_linv.as<double>());
+    LAUNCHED();
+    CU(cudaGetLastError());
+    gp->pad_valid = true;
+    return B200BO_OK;
 }
 
 // fp32 mode operand images of L^-1 (once per fit)
@@ -1189,7 +1275,10 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
             P.sel_resume = sm.resume;
             fused_sel = true;
         }
-        P.scratch_stride = (long long)np_max * PBN;
+        // phase B path of the 16-warp fp64 kernel; the bulk-copy paths read K* in the padded stage layout
+        const bool fp64_16 = predict_impl(g0->precision) == PREDICT_IMPL_DMMA && predict_warps() == 16;
+        const int pipe = fp64_16 && predict_mma() != 884 ? predict_pipe() : PIPE_CPASYNC;
+        P.scratch_stride = (long long)np_max * (pipe == PIPE_CPASYNC ? PBN : PSTR_DMMA);
         if ((rc = g0->pscratch.reserve(sizeof(double) * (size_t)P.scratch_stride * g0->sm_count))) return rc;
         P.scratch = g0->pscratch.as<double>();
         CU(cudaEventRecord(g0->ev0, stream));
@@ -1205,12 +1294,35 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
             } else {
                 predict_acq_tc_kernel<false><<<grid, PNT, kPredictSmemBytesTc, stream>>>(P);
             }
-        } else if (predict_impl(g0->precision) == PREDICT_IMPL_DMMA && predict_warps() == 16) {
+        } else if (fp64_16) {
             P.linv_l2_last = predict_linv_l2_last();
-            if (predict_mma() == 884)
-                launch_predict16<884>(dreg, grid, stream, P);
-            else
-                launch_predict16<1684>(dreg, grid, stream, P);
+            if (pipe != PIPE_CPASYNC) {
+                for (int g = 0; g < spec->n_gps; ++g) {
+                    if ((rc = ensure_pad(spec->gps[g], stream))) return rc;
+                    P.gp[g].linv_pad = spec->gps[g]->pad_linv.as<double>();
+                }
+                if (!sm.resume) {
+                    void* flag = nullptr;
+                    CU(cudaGetSymbolAddress(&flag, g_pipe_timeout));
+                    CU(cudaMemsetAsync(flag, 0, sizeof(unsigned long long), stream));
+                    g0->pipe_armed = true;
+                }
+                CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off staging from the kernel time
+            }
+            if (predict_mma() == 884) {
+                rc = launch_predict16<884, PIPE_CPASYNC>(dreg, grid, stream, P);
+            } else if (pipe == PIPE_BULK_MC) {
+                // whole CTA pairs, each pair running the same number of tiles (see predict_acq16_kernel)
+                if ((rc = predict_pair_grid(g0))) return rc;
+                const long long pairs = (ntiles + 1) / 2;
+                grid = (sm.resume || !sm.finish || pairs >= g0->pair_grid / 2) ? g0->pair_grid : (int)(2 * pairs);
+                rc = launch_predict16<1684, PIPE_BULK_MC>(dreg, grid, stream, P);
+            } else if (pipe == PIPE_BULK) {
+                rc = launch_predict16<1684, PIPE_BULK>(dreg, grid, stream, P);
+            } else {
+                rc = launch_predict16<1684, PIPE_CPASYNC>(dreg, grid, stream, P);
+            }
+            if (rc) return rc;
         } else if (predict_impl(g0->precision) == PREDICT_IMPL_DMMA) {
             if (dreg)
                 predict_acq_kernel<PREDICT_IMPL_DMMA, true><<<grid, PNT, kPredictSmemBytesDmma, stream>>>(P);
@@ -1270,7 +1382,7 @@ extern "C" int b200bo_last_kernel_ms(float* ms) {
     CU(cudaSetDevice(g_last_timed->device));
     CU(cudaEventSynchronize(g_last_timed->ev1));
     CU(cudaEventElapsedTime(ms, g_last_timed->ev0, g_last_timed->ev1));
-    return B200BO_OK;
+    return check_pipe_timeout(g_last_timed);
 }
 
 // Host-buffer front end shared by predict / acq_eval / argmin_topk.  Large selection-only batches are
@@ -1312,7 +1424,7 @@ static int check_nonfinite(b200bo_gp* g0) {
     unsigned long long c[2] = {0, 0};
     CU(cudaMemcpy(c, g0->clamp.p, sizeof(c), cudaMemcpyDeviceToHost));
     if (c[1] != 0) return set_err(B200BO_ERR_ARG, "Input X contains NaN or infinity.");
-    return B200BO_OK;
+    return check_pipe_timeout(g0);
 }
 
 static int run_host_chunked(const b200bo_acq* spec, const double* Xc, int64_t m, int k, SelRecord* sel_host) {

@@ -11,6 +11,9 @@
 //   * phase B runs on the sm_90 shape mma.sync m16n8k4 f64 (MMA = 1684, the default: twice the fp64 tensor rate of
 //     the sm_80 shape m8n8k4 per SM and clock on H100); m8n8k4 (MMA = 884) stays selectable with
 //     B200BO_PREDICT_MMA=884 for A/B measurements (DESIGN.md 4.1, 6, 6.1);
+//   * phase B operands reach shared memory either by per-thread cp.async under CTA barriers (PIPE_CPASYNC) or by
+//     bulk copies on an mbarrier ring (PIPE_BULK), with the L^-1 stages multicast across CTA pairs (PIPE_BULK_MC);
+//     B200BO_PREDICT_PIPE selects (DESIGN.md 4.1, 6.1);
 //   * L2 policy hints: the CTA-private K* scratch (written once, swept cyclically: LRU-hostile) is stored and
 //     loaded evict_first; L^-1 (re-read by every CTA for every tile) is loaded evict_last on a fraction
 //     P.linv_l2_last of its lines.  At N=4096 the L^-1 triangle is 67 MB, more than the 50 MB L2 of an H100, so
@@ -47,7 +50,9 @@ __device__ __forceinline__ void st_global_hint(double* p, double v, unsigned lon
 }
 
 // ---- phase A: K*^T tile (np x 128) into the CTA's scratch + K* alpha_ -----------------------------
-template <bool DREG, int COV>
+// KSTR: row stride of the K* scratch in doubles: PBN (cp.async phase B) or PSTR_DMMA (bulk-copy phase B: the rows
+// of a stage are then contiguous in global memory exactly as in shared memory, one copy per stage)
+template <bool DREG, int COV, int KSTR>
 __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
                                                        double* __restrict__ Ks, double* smem,
                                                        double (*mu_s)[PBN], unsigned long long pol_first) {
@@ -138,7 +143,7 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
                 const int n = ch * PA_CHUNK + r0 + q;
                 double kv = G.constv * cov_eval<COV>(r2[q]);
                 if (n >= G.n) kv = 0.0;
-                st_global_hint(Ks + (size_t)n * PBN + c, kv, pol_first);
+                st_global_hint(Ks + (size_t)n * KSTR + c, kv, pol_first);
                 mu_acc = fma(al[r0 + q], kv, mu_acc);
             }
         }
@@ -150,15 +155,15 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
     __syncthreads();
 }
 
-template <bool DREG>
+template <bool DREG, int KSTR>
 __device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const GpDev& G, long long c0,
                                                   double* __restrict__ Ks, double* smem, double (*mu_s)[PBN],
                                                   unsigned long long pol_first) {
     switch (cov_code(G.family, G.nu)) {
-        case 0: predict16_phase_a_impl<DREG, 0>(P, G, c0, Ks, smem, mu_s, pol_first); break;
-        case 1: predict16_phase_a_impl<DREG, 1>(P, G, c0, Ks, smem, mu_s, pol_first); break;
-        case 2: predict16_phase_a_impl<DREG, 2>(P, G, c0, Ks, smem, mu_s, pol_first); break;
-        default: predict16_phase_a_impl<DREG, 3>(P, G, c0, Ks, smem, mu_s, pol_first); break;
+        case 0: predict16_phase_a_impl<DREG, 0, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
+        case 1: predict16_phase_a_impl<DREG, 1, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
+        case 2: predict16_phase_a_impl<DREG, 2, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
+        default: predict16_phase_a_impl<DREG, 3, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
     }
 }
 
@@ -290,28 +295,261 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
     __syncthreads();
 }
 
-template <bool DREG, int MMA>
+// ---- phase B fed by bulk copies on an mbarrier ring (PIPE_BULK, PIPE_BULK_MC) -------------------------------
+// Same stages (PSTAGES x BK k-rows of L^-1 and of K*, rows padded to PSTR_DMMA), fragments, MMAs and summation order
+// as predict16_phase_b<1684>, so V, and everything computed from it, is bit-equal.  Only the way the operands reach
+// shared memory differs:
+//   * both operands sit in global memory in the padded stage layout: L^-1 as stage images built once per fit
+//     (pad_linv_stages_kernel), K* written by phase A with row stride PSTR_DMMA.  A stage is then TWO cp.async.bulk
+//     of 33 KiB issued by one thread (per-row copies, 64 per stage, made the issuing warp the critical path);
+//   * full[s] (one arrival + 66 KiB of transactions) replaces the CTA barrier of every k-tile.  PIPE_BULK: every
+//     warp counts its consumption of a stage in done[s] (shared-memory atomic), and the last of the 16 refills the
+//     slot at once with the stage three ahead, so no warp ever waits for a free slot.  The ring runs straight across
+//     row blocks, so the first stages of block ib+1 load while the warps fold block ib into csq;
+//   * PIPE_BULK_MC: the two CTAs of a cluster run the same L^-1 stages; each copies half of the L^-1 image of a
+//     stage and multicasts it to both, so L^-1 leaves L2 once per pair.  A refill then needs both CTAs: warp 0
+//     issues stage ks + 2 behind the first MMA batch of k-tile ks after waiting on empty[s], which counts the warps
+//     of both CTAs (every warp arrives on its own and on the partner's barrier).
+// Every warp waits on full[s] even for the k-tiles it skips (diagonal block): a count or an arrival that is not
+// bounded by the fill it releases could be counted against an earlier fill.
+// The ring belongs to phase B only: a CTA (MC: cluster) barrier at entry and exit keeps the copies away from the
+// shared memory that phase A and the epilogue use, and `it` (stages used so far) carries the ring's phase.
+// doubles before the stage image (row block ib, k-tile kt) of L^-1: row block j holds (j + 1) * PBM / PBK_DMMA k-tiles
+__host__ __device__ inline size_t pad_stage_offset(int ib, int kt) {
+    return ((size_t)(PBM / PBK_DMMA) * ib * (ib + 1) / 2 + kt) * PBK_DMMA * PSTR_DMMA;
+}
+__host__ __device__ inline size_t pad_linv_doubles(int np) { return pad_stage_offset(np / PBM, 0); }
+
+// L^-1 (as linvT, row-major np x np) -> the stage images of the bulk-copy phase B: for row block ib (blockIdx.y) and
+// k-tile kt (blockIdx.x), k-rows kt*BK .. +BK of linvT, columns ib*PBM .. +PBM, rows padded to PSTR_DMMA with zeros
+__global__ void __launch_bounds__(256) pad_linv_stages_kernel(const double* __restrict__ WT, int np,
+                                                              double* __restrict__ out) {
+    const int kt = blockIdx.x, ib = blockIdx.y;
+    if (kt >= (ib + 1) * (PBM / PBK_DMMA)) return;
+    double* img = out + pad_stage_offset(ib, kt);
+    for (int idx = threadIdx.x; idx < PBK_DMMA * PSTR_DMMA; idx += 256) {
+        const int r = idx / PSTR_DMMA, c = idx - r * PSTR_DMMA;
+        img[idx] = c < PBM ? WT[(size_t)(kt * PBK_DMMA + r) * np + (size_t)ib * PBM + c] : 0.0;
+    }
+}
+
+enum { PIPE_CPASYNC = 0, PIPE_BULK = 1, PIPE_BULK_MC = 2 };
+// failed polls before a wait gives up: seconds, against microseconds for a stage to arrive from L2 or HBM
+constexpr uint32_t kPipeWaitBudget = 1u << 28;
+// set by a wait of the bulk-copy phase B that ran out of its budget; the host reports it as an error and clears it
+// before every launch.  A global, not a launch parameter, so that the k-loop holds no register for it.
+__device__ unsigned long long g_pipe_timeout;
+
+template <bool MC>
+__device__ __forceinline__ void pipe_barrier() {
+    if constexpr (MC)
+        tc::cluster_sync();
+    else
+        __syncthreads();
+}
+
+// The producer re-derives its operands (policies, K* scratch, cluster rank) from the kernel parameters at every issue
+// instead of holding them in registers across the k-loop: the kernel sits at 128 registers per thread.
+template <bool MC>
+__device__ __forceinline__ void predict16_phase_b_bulk(const PredictParams& P, const GpDev& G, double* smem,
+                                                       uint64_t* full, uint64_t* empty, unsigned* done,
+                                                       uint32_t& it) {
+    constexpr int STR = PSTR_DMMA, BK = PBK_DMMA;
+    constexpr uint32_t kStageBytes = 2 * BK * STR * sizeof(double);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int wn = warp >> 2;
+    const int wm = (warp + wn) & 3;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int nb = G.np / PBM;
+    double* As = smem;
+    double* Bs = smem + PSTAGES * BK * STR;
+    // K* (phase A's global stores) and the stage memory (phase A / epilogue) are read / overwritten by the async proxy
+    tc::fence_proxy_async_global();
+    tc::fence_proxy_async_smem();
+    pipe_barrier<MC>();
+    // one thread: stage (pib, pks) of this phase B into the free slot s
+    auto copy = [&](int pib, int pks, int s) {
+        {
+            tc::mbar_arrive_expect_tx(&full[s], kStageBytes);
+            const double* ag = G.linv_pad + pad_stage_offset(pib, pks);
+            const double* bg = P.scratch + (long long)blockIdx.x * P.scratch_stride + (size_t)pks * BK * STR;
+            const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last);
+            if constexpr (MC) {
+                constexpr int HALF = BK / 2 * STR;
+                const int r = (int)tc::cluster_ctarank();
+                tc::bulk_g2s_multicast_hint(As + s * BK * STR + r * HALF, ag + r * HALF, HALF * 8, &full[s], 0x3,
+                                            pol_last);
+            } else {
+                tc::bulk_g2s_hint(As + s * BK * STR, ag, BK * STR * 8, &full[s], pol_last);
+            }
+            tc::bulk_g2s_hint(Bs + s * BK * STR, bg, BK * STR * 8, &full[s], l2_policy_evict_first());
+        }
+    };
+    // MC producer (warp 0): stage (pib, pks) into slot s once both CTAs have consumed its previous fill (parity ph ^ 1)
+    auto issue = [&](int pib, int pks, int s, uint32_t ph) {
+        tc::mbar_wait_budget(&empty[s], ph ^ 1, &g_pipe_timeout, kPipeWaitBudget);
+        if (lane == 0) copy(pib, pks, s);
+        __syncwarp();
+    };
+    // ring position of the next stage to consume: slot s, fill parity ph
+    int s = it % PSTAGES;
+    uint32_t ph = (it / PSTAGES) & 1;
+    it += 2 * nb * (nb + 1);  // stages of this phase B: sum over ib of (ib + 1) * PBM / BK
+    static_assert(PBM / BK == 4 && PSTAGES == 3, "ring bookkeeping");
+    if constexpr (MC) {
+        if (warp == 0) {  // block 0 has PBM / BK >= PSTAGES - 1 k-tiles
+            issue(0, 0, s, ph);
+            issue(0, 1, s == 2 ? 0 : s + 1, s == 2 ? ph ^ 1 : ph);
+        }
+    } else if (tid == 0) {  // every slot is free at entry; block 0 has PBM / BK >= PSTAGES k-tiles
+        for (int q = 0; q < PSTAGES; ++q) copy(0, q, (s + q) % PSTAGES);
+    }
+    double csq[4][2];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) csq[j][0] = csq[j][1] = 0.0;
+    for (int ib = 0; ib < nb; ++ib) {
+        double acc[4][4][2];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+        const int nks = (ib + 1) * (PBM / BK);
+        for (int ks = 0; ks < nks; ++ks) {
+            tc::mbar_wait_budget(&full[s], ph, &g_pipe_timeout, kPipeWaitBudget);
+            // the fragment offsets are re-derived from a fresh %tid.x read: holding them across the loop spilled them
+            const int tx = tc::tid_x(), wx = tx >> 5, wmx = (wx + (wx >> 2)) & 3, gx = (tx & 31) >> 2;
+            const bool live = ks * BK < ib * PBM + (wmx + 1) * 32;
+            const double* as = As + s * BK * STR + wmx * 32 + gx;
+            const double* bs = Bs + s * BK * STR + (wx >> 2) * 32 + gx;
+#pragma unroll
+            for (int k4 = 0; k4 < BK / 4; ++k4) {
+                if (MC && k4 == 1 && warp == 0) {  // stage ks + 2 goes into the slot stage ks - 1 left
+                    int pib = ib, pks = ks + PSTAGES - 1;
+                    if (pks >= nks) {
+                        pks -= nks;
+                        ++pib;
+                    }
+                    if (pib < nb) issue(pib, pks, s == 0 ? 2 : s - 1, s == 0 ? ph : ph ^ 1);
+                }
+                if (live) {
+                    double a[4], b[4];
+                    const int krow = (k4 * 4 + t4) * STR;
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) a[i] = as[krow + i * 8];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) b[j] = bs[krow + j * 8];
+#pragma unroll
+                    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                        for (int j = 0; j < 4; ++j)
+                            dmma1684(acc[2 * mi][j][0], acc[2 * mi][j][1], acc[2 * mi + 1][j][0],
+                                     acc[2 * mi + 1][j][1], a[2 * mi], a[2 * mi + 1], b[j]);
+                }
+            }
+            __syncwarp();
+            if (lane == 0) {
+                if constexpr (MC) {
+                    tc::mbar_arrive_cluster(&empty[s], 0);
+                    tc::mbar_arrive_cluster(&empty[s], 1);
+                } else {
+                    __threadfence_block();  // this warp's reads of slot s happen before its count
+                    if ((atomicAdd(&done[s], 1u) & 15u) == 15u) {  // last of the 16 warps: refill with stage ks + 3
+                        __threadfence_block();
+                        tc::fence_proxy_async_smem();
+                        int pib = ib, pks = ks + PSTAGES;
+                        if (pks >= nks) {
+                            pks -= nks;
+                            ++pib;
+                        }
+                        if (pib < nb) copy(pib, pks, s);
+                    }
+                }
+            }
+            if (++s == PSTAGES) {
+                s = 0;
+                ph ^= 1;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            double s0 = 0.0, s1 = 0.0;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                s0 = fma(acc[i][j][0], acc[i][j][0], s0);
+                s1 = fma(acc[i][j][1], acc[i][j][1], s1);
+            }
+            csq[j][0] += s0;
+            csq[j][1] += s1;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            double v = csq[j][e];
+            v += __shfl_xor_sync(0xffffffffu, v, 4);
+            v += __shfl_xor_sync(0xffffffffu, v, 8);
+            v += __shfl_xor_sync(0xffffffffu, v, 16);
+            csq[j][e] = v;
+        }
+    pipe_barrier<MC>();  // every stage consumed in this CTA (MC: and in the partner) before red overwrites stage 0
+    double* red = smem;  // [4][PBN]: row slab wm, every column produced by exactly one warp
+    if (g == 0) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            red[wm * PBN + wn * 32 + j * 8 + t4 * 2] = csq[j][0];
+            red[wm * PBN + wn * 32 + j * 8 + t4 * 2 + 1] = csq[j][1];
+        }
+    }
+    __syncthreads();
+}
+
+// PIPE: phase B data path; PIPE_BULK_MC is launched in clusters of 2 CTAs, and the two CTAs of a cluster run the
+// same number of tiles: when the pair's second tile lies past the batch (odd tile count), the second CTA runs it
+// with every column masked (c0 >= m: zero coordinates, no output, no selection entry).
+template <bool DREG, int MMA, int PIPE>
 __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictParams P) {
+    static_assert(PIPE == PIPE_CPASYNC || MMA == 1684, "the bulk-copy phase B runs on m16n8k4");
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
     __shared__ double base_s[PBN];
     __shared__ double prod_s[PBN];
     __shared__ SelShared sel_s;
+    __shared__ uint64_t full_bar[PSTAGES], empty_bar[PSTAGES];
+    __shared__ unsigned done_cnt[PSTAGES];
 
     const int tid = threadIdx.x;
     double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
     const long long ntiles = (P.m + PBN - 1) / PBN;
     const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last), pol_first = l2_policy_evict_first();
+    uint32_t rank = 0, it = 0;
+    if constexpr (PIPE != PIPE_CPASYNC) {
+        if constexpr (PIPE == PIPE_BULK_MC) rank = tc::cluster_ctarank();
+        if (tid == 0) {
+            for (int s = 0; s < PSTAGES; ++s) {
+                tc::mbar_init(&full_bar[s], 1);
+                tc::mbar_init(&empty_bar[s], (P16_NT / 32) * 2);
+                done_cnt[s] = 0;
+            }
+            tc::mbar_fence_init();
+        }
+        pipe_barrier<PIPE == PIPE_BULK_MC>();  // MC: the partner's barriers exist before the first remote arrival
+    }
     if (P.sel_cta) {
         if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
         __syncthreads();
     }
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    for (long long tile = blockIdx.x; tile - rank < ntiles; tile += gridDim.x) {
         const long long c0 = tile * PBN;
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
-            predict16_phase_a<DREG>(P, G, c0, Ks, smem, mu_s, pol_first);
-            predict16_phase_b<MMA>(G, Ks, smem, pol_last, pol_first);
+            if constexpr (PIPE == PIPE_CPASYNC) {
+                predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first);
+                predict16_phase_b<MMA>(G, Ks, smem, pol_last, pol_first);
+            } else {  // policies made where they are used: nothing extra stays live across phase B
+                predict16_phase_a<DREG, PSTR_DMMA>(P, G, c0, Ks, smem, mu_s, l2_policy_evict_first());
+                predict16_phase_b_bulk<PIPE == PIPE_BULK_MC>(P, G, smem, full_bar, empty_bar, done_cnt, it);
+            }
             const double* red = smem;
             if (tid < PBN) {
                 const int c = tid;

@@ -1,5 +1,5 @@
-// tc_common.cuh - thin inline-PTX layer for the sm_90a tensor-core path: mbarriers, 1-D bulk
-// async copies (TMA engine, no tensor map) and wgmma issue/commit/wait.  The descriptor bit layout
+// tc_common.cuh - thin inline-PTX layer for the sm_90a kernels: mbarriers, 1-D bulk async copies
+// (TMA engine, no tensor map, optionally multicast in a thread-block cluster) and wgmma issue/commit/wait.  The descriptor bit layout
 // follows the PTX ISA "matrix descriptor" table of the warpgroup-level MMA instructions.
 #pragma once
 #include <cuda_runtime.h>
@@ -40,6 +40,62 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
 }
 
+__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t"
+        "}\n"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return ok != 0;
+}
+// mbar_wait with a budget of `budget` failed polls (each try_wait may also suspend the thread for a while): on expiry
+// *err is set and the wait gives up, as does every later wait that sees *err set, so a protocol error ends the
+// kernel with a reported error instead of a hang
+__device__ __forceinline__ void mbar_wait_budget(uint64_t* bar, uint32_t parity, unsigned long long* err,
+                                                 uint32_t budget) {
+    for (uint32_t n = 0; !mbar_try_wait(bar, parity); ++n) {
+        if (*reinterpret_cast<volatile unsigned long long*>(err)) return;
+        if (n == budget) {
+            atomicExch(err, 1ull);
+            return;
+        }
+    }
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster (this CTA included)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    asm volatile(
+        "{\n\t"
+        ".reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t"
+        "}\n" ::"r"(smem_u32(bar)),
+        "r"(rank)
+        : "memory");
+}
+
+// %tid.x through a volatile read: the compiler re-reads it where it is used instead of keeping values derived from
+// it live in registers (or spilled) across a long loop
+__device__ __forceinline__ int tid_x() {
+    int t;
+    asm volatile("mov.u32 %0, %%tid.x;\n" : "=r"(t));
+    return t;
+}
+
+// ---- thread-block clusters ------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+}
+
 // named barrier among a subset of the CTA's warps (id 1..15; nthreads multiple of 32)
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
@@ -51,6 +107,24 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
             smem_u32(smem_dst)),
         "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
+        : "memory");
+}
+// the same with an L2 cache policy (createpolicy), and multicast to the CTAs of `cta_mask` in the cluster: the data
+// and the complete_tx land at the same shared-memory offsets in every destination CTA
+__device__ __forceinline__ void bulk_g2s_hint(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar,
+                                              unsigned long long pol) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], "
+        "%4;\n" ::"r"(smem_u32(smem_dst)),
+        "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+        : "memory");
+}
+__device__ __forceinline__ void bulk_g2s_multicast_hint(void* smem_dst, const void* gmem_src, uint32_t bytes,
+                                                        uint64_t* bar, uint16_t cta_mask, unsigned long long pol) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint "
+        "[%0], [%1], %2, [%3], %4, %5;\n" ::"r"(smem_u32(smem_dst)),
+        "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask), "l"(pol)
         : "memory");
 }
 // generic-proxy writes to global memory -> visible to the async proxy (bulk copies)
