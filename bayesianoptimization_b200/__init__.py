@@ -1,7 +1,7 @@
 """bayesianoptimization_b200 - a H100-native GP-surrogate + acquisition engine that drops in
 behind ``bayes_opt.BayesianOptimization.suggest()`` and the ``bayes_opt.acquisition`` classes.
 
-Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI (x constraint probability) ->
+Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI/MES (x constraint probability) ->
 argmin/top-k, in hand-written sm_90a CUDA behind the C ABI declared in include/b200bo.h.
 No CPU fallback: importing the compute classes without the built library raises ImportError.
 
@@ -10,8 +10,8 @@ Two layers:
     PosteriorPaths, ConstrainedPaths (posterior sample paths, resolved lazily)
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ThompsonSampling,
-    ConstrainedThompsonSampling, ConstantLiar, GPHedge, AcquisitionFunction, ConstraintModel, enable(optimizer) -
-    resolved lazily on first access.
+    ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, GPHedge, AcquisitionFunction,
+    ConstraintModel, enable(optimizer) - resolved lazily on first access.
 """
 from . import _lib
 from ._build import build_library
@@ -26,6 +26,7 @@ _PLUGIN = {
     "ExpectedImprovement": "acquisition", "ProbabilityOfImprovement": "acquisition",
     "ConstantLiar": "acquisition", "GPHedge": "acquisition", "DeviceHooks": "acquisition",
     "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
+    "MaxValueEntropySearch": "acquisition",
     "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
 }
 

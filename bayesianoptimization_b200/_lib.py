@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(HERE, "libb200bo.so")
 OK, ERR_CUDA, ERR_ARG, ERR_NOT_PD, ERR_UNSUPPORTED, ERR_STATE = 0, -1, -2, -3, -4, -5
 KERNEL_MATERN, KERNEL_RBF = 0, 1
 NU_05, NU_15, NU_25, NU_INF = 0, 1, 2, 3
-ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE = 0, 1, 2, 3
+ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE, ACQ_MES = 0, 1, 2, 3, 4
 MAX_GPS, MAX_DIM, MAX_TOPK, MAX_PATHS = 8, 64, 64, 16
 XFORM_IDENTITY, XFORM_ROUND = 0, 1
 GET_L, GET_ALPHA, GET_YSTATS, GET_K, GET_LINV = 0, 1, 2, 3, 4
@@ -23,7 +23,7 @@ PATH_AUTO, PATH_STABLE = 0, 1
 EXPORTS = [
     "b200bo_version", "b200bo_last_error", "b200bo_device_count", "b200bo_launch_count",
     "b200bo_gp_create", "b200bo_gp_destroy", "b200bo_gp_set_precision", "b200bo_gp_set_private_stream",
-    "b200bo_gp_set_transform", "b200bo_gp_fit",
+    "b200bo_gp_set_transform", "b200bo_gp_set_max_values", "b200bo_gp_fit",
     "b200bo_gp_set_data", "b200bo_gp_append", "b200bo_gp_lml", "b200bo_gp_get", "b200bo_gp_n", "b200bo_gp_dim",
     "b200bo_gp_predict", "b200bo_gp_predict_cov", "b200bo_acq_eval", "b200bo_acq_argmin_topk", "b200bo_acq_eval_dev",
     "b200bo_last_kernel_ms",
@@ -84,6 +84,7 @@ def lib():
     L.b200bo_gp_set_precision.argtypes = [C.c_void_p, C.c_int]
     L.b200bo_gp_set_private_stream.argtypes = [C.c_void_p, C.c_int]
     L.b200bo_gp_set_transform.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
+    L.b200bo_gp_set_max_values.argtypes = [C.c_void_p, dp, C.c_int]
     L.b200bo_gp_fit.argtypes = [C.c_void_p, dp, dp, C.c_int64, C.c_int, C.POINTER(KernelSpec),
                                 C.c_double, C.c_int, i64p]
     L.b200bo_gp_set_data.argtypes = [C.c_void_p, dp, dp, C.c_int64, C.c_int, C.c_int]

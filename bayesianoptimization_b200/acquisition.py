@@ -15,9 +15,10 @@ inherited), with ``DeviceHooks`` mixed in:
                               (mixed-integer spaces: the reference's own DE branch, unchanged, calling
                               the device closure)
 
-``ThompsonSampling`` is the one policy defined here rather than inherited: a posterior sample path per
-``suggest()``, ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`` extends it to
-constrained problems (the paths of the target and the constraint GPs, ranked feasible-first).
+``ThompsonSampling`` is a policy defined here rather than inherited: a posterior sample path per ``suggest()``,
+ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`` extends it to constrained problems
+(the paths of the target and the constraint GPs, ranked feasible-first).  ``MaxValueEntropySearch`` is the
+information-based policy: samples of the maximum from posterior paths, then a fused-kernel epilogue of mu and sigma.
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
 (gpr.B200GaussianProcessRegressor), ``fused.FusedAcquisition`` and the C ABI do not need it.
@@ -58,6 +59,13 @@ def _device_kind(obj):
     return None
 
 
+def _philox_seed(random_state):
+    """The ONE 64-bit Philox key a device-generated candidate batch takes from the caller's RandomState: two 32-bit
+    draws, the first the high word."""
+    hi = int(random_state.randint(0, 2**32, dtype=np.uint64))
+    return hi << 32 | int(random_state.randint(0, 2**32, dtype=np.uint64))
+
+
 def _device_closure(acq):
     """True for closures that select and refine on the device: they map (M,d) -> (M,) and offer
     ``argmin_topk`` and ``argmin_topk_philox`` (optionally ``refine_mode``) - FusedAcquisition and the
@@ -89,7 +97,7 @@ class DeviceHooks(abc.ABC):
             # (n_smart beyond the device's top-k capacity: evaluate on the device, select with numpy)
             return super()._random_sample_minimize(acq, space, random_state, n_random, n_x_seeds)
         if self.b200_candidate_source == "device_philox" and all(space.continuous_dimensions):
-            seed = int(random_state.randint(0, 2**32, dtype=np.uint64)) << 32 | int(random_state.randint(0, 2**32, dtype=np.uint64))
+            seed = _philox_seed(random_state)
             _, min_acq, x_min, _, x_seeds = acq.argmin_topk_philox(seed, space.bounds, n_random, n_x_seeds)
             return x_min, min_acq, (x_seeds if n_x_seeds != 0 else [])
         x_tries = space.random_sample(n_random, random_state=random_state)  # the reference's RNG stream
@@ -133,7 +141,36 @@ class ExpectedImprovement(DeviceHooks, _ref.ExpectedImprovement):
     """bayes_opt.acquisition.ExpectedImprovement with the device hooks."""
 
 
-class ThompsonSampling(DeviceHooks, _ref.AcquisitionFunction):
+class _SuggestStream:
+    """Mixin for policies whose closure draws random numbers: ``suggest`` keeps its RandomState (and target space)
+    for ``_get_acq``, which the reference's suggest calls before the random candidates are drawn from that same
+    stream.  Outside suggest(), ``_get_acq`` gets a fresh unseeded stream and no space."""
+
+    _path_rng = None
+    _suggest_space = None
+
+    def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        self._path_rng = _ensure_rng(random_state)
+        self._suggest_space = target_space
+        try:
+            return super().suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
+                                   random_state=self._path_rng)
+        finally:
+            self._path_rng = None
+            self._suggest_space = None
+
+    def _suggest_rng(self):
+        return self._path_rng if self._path_rng is not None else _ensure_rng(None)
+
+
+def _check_int(name, v, lo, hi=None):
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v > hi):
+        rng = f"an integer in [{lo}, {hi}]" if hi is not None else f"an integer >= {lo}"
+        raise ValueError(f"{name} must be {rng}, got {v!r}")
+    return int(v)
+
+
+class ThompsonSampling(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
     """Thompson sampling: every ``suggest()`` draws ONE function from the GP posterior and proposes its maximiser.
 
     The function is a posterior sample path (``B200GaussianProcessRegressor.sample_paths``, n_paths=1) drawn from
@@ -150,21 +187,11 @@ class ThompsonSampling(DeviceHooks, _ref.AcquisitionFunction):
         if isinstance(n_features, bool) or not isinstance(n_features, (int, np.integer)) or n_features < 1:
             raise ValueError(f"n_features must be a positive integer, got {n_features!r}")
         self.n_features = int(n_features)
-        self._path_rng = None
 
     def base_acq(self, *args, **kwargs):
         raise NotImplementedError(
             "ThompsonSampling has no base_acq(mean, std): it ranks candidates by one posterior sample path drawn "
             "per suggest() (B200GaussianProcessRegressor.sample_paths), not by a formula of mean and std")
-
-    def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
-        # the path of this call is drawn from the caller's stream: remember it for _get_acq
-        self._path_rng = _ensure_rng(random_state)
-        try:
-            return super().suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
-                                   random_state=self._path_rng)
-        finally:
-            self._path_rng = None
 
     def _get_acq(self, gp, constraint=None):
         if constraint is not None:
@@ -172,7 +199,7 @@ class ThompsonSampling(DeviceHooks, _ref.AcquisitionFunction):
                 f"{type(self).__name__} does not support constrained optimization: a constraint model was given")
         from .paths import PathAcquisition
 
-        rs = self._path_rng if self._path_rng is not None else _ensure_rng(None)
+        rs = self._suggest_rng()  # the path of this call is drawn from the caller's stream
         return PathAcquisition(_as_b200_gp(gp).sample_paths(1, self.n_features, random_state=rs))
 
     def get_acquisition_params(self):
@@ -202,10 +229,89 @@ class ConstrainedThompsonSampling(ThompsonSampling):
         models = [_as_b200_gp(m) for m in constraint.model]  # before any draw: a refusal consumes no random numbers
         if len(models) + 1 > B.MAX_GPS:
             raise NotImplementedError(f"at most {B.MAX_GPS - 1} constraint GPs are supported")
-        rs = self._path_rng if self._path_rng is not None else _ensure_rng(None)
+        rs = self._suggest_rng()
         target = gp.sample_paths(1, self.n_features, random_state=rs)
         paths = [m.sample_paths(1, self.n_features, random_state=rs) for m in models]
         return PathAcquisition(ConstrainedPaths(target, paths, constraint.lb, constraint.ub))
+
+
+# Default size of the candidate set over which the maxima of the MES sample paths are taken (DESIGN.md 4.8).
+MES_MAX_CANDIDATES = 2**16
+
+
+def mes_max_values(gp, paths, space, random_state, n_candidates, candidate_source="host_rng"):
+    """Samples y*_k of the maximum of the target: per path k of ``paths`` (a PosteriorPaths of ``gp``),
+    y*_k = max(max of path k over n_candidates random points and X_train_, the largest registered target).
+    The floor keeps every sample consistent with the data: the maximum is at least what has been observed.
+    The candidates are ``space.random_sample(n_candidates, random_state)``, or in device_philox mode on a continuous
+    space one 64-bit seed drawn as DeviceHooks._random_sample_minimize draws it (rows generated in the kernel)."""
+    if candidate_source == "device_philox" and all(space.continuous_dimensions):
+        _, neg_max, *_ = paths.argmin_topk_philox(_philox_seed(random_state), space.bounds, n_candidates, 0)
+    else:
+        _, neg_max, _ = paths.argmin_topk(space.random_sample(n_candidates, random_state=random_state), 0)
+    best = np.maximum(-np.asarray(neg_max, dtype=np.float64), paths(gp.X_train_).max(axis=0))
+    return np.maximum(best, float(np.max(gp._y_raw)))
+
+
+class MaxValueEntropySearch(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
+    """Max-value entropy search (MES: Wang & Jegelka, "Max-value Entropy Search for Efficient Bayesian
+    Optimization", ICML 2017): proposes the point whose observation is expected to tell the most about the value of
+    the maximum, y*.  With K samples y*_k and the GP's posterior mean mu(x) and standard deviation sigma(x),
+
+        alpha(x) = (1/K) sum_k [ g_k psi(g_k) / (2 Psi(g_k)) - log Psi(g_k) ],    g_k = (y*_k - mu(x)) / sigma(x)
+
+    (psi, Psi: standard normal pdf and cdf; alpha = 0 where sigma = 0), evaluated in the epilogue of the fused
+    predict kernel like EI.  Every ``suggest()`` draws from the RandomState it receives, in this order:
+
+      1. ``draw_path_inputs`` of n_samples posterior sample paths of the target GP (``sample_paths``);
+      2. the candidate set of the maxima: ``space.random_sample(n_max_candidates, rs)``, or with
+         candidate_source="device_philox" on a continuous space one 64-bit Philox seed (``mes_max_values``);
+      3. then the reference's random stage and L-BFGS-B refinement, as for every acquisition.
+
+    y*_k is path k's maximum over those candidates and the training inputs, floored at the largest registered
+    target.  With a constraint the closure is MES times the probability of feasibility; y* is sampled from the
+    unconstrained target, and no feasible registered point is needed (EI / PoI raise NoValidPointRegisteredError).
+
+    n_samples         K, 1..16 sample paths (one per y* sample)
+    n_features        random Fourier features of each path's prior part
+    n_max_candidates  size of the candidate set of step 2 (default MES_MAX_CANDIDATES)"""
+
+    def __init__(self, n_samples=10, n_features=4096, n_max_candidates=MES_MAX_CANDIDATES, random_state=None):
+        super().__init__(random_state=random_state)
+        self.n_samples = _check_int("n_samples", n_samples, 1, B.MAX_PATHS)
+        self.n_features = _check_int("n_features", n_features, 1)
+        self.n_max_candidates = _check_int("n_max_candidates", n_max_candidates, 1)
+        self.max_values = None  # the y* samples of the latest closure
+
+    def base_acq(self, *args, **kwargs):
+        raise NotImplementedError(
+            "MaxValueEntropySearch has no base_acq(mean, std): its formula also needs the samples of the maximum "
+            "drawn per suggest(), and it runs in the fused device kernel")
+
+    def _get_acq(self, gp, constraint=None):
+        gp = _as_b200_gp(gp)
+        if constraint is not None:  # before any draw: a refusal consumes no random numbers
+            models = [_as_b200_gp(m) for m in constraint.model]
+            if len(models) + 1 > B.MAX_GPS:
+                raise NotImplementedError(f"at most {B.MAX_GPS - 1} constraint GPs are supported")
+        space = self._suggest_space
+        if space is None:
+            raise RuntimeError("MaxValueEntropySearch samples the maximum over the target space of suggest(): "
+                               "build its closure through suggest()")
+        rs = self._suggest_rng()
+        paths = gp.sample_paths(self.n_samples, self.n_features, random_state=rs)
+        ystar = mes_max_values(gp, paths, space, rs, self.n_max_candidates, self.b200_candidate_source)
+        self.max_values = ystar
+        return FusedAcquisition(B.ACQ_MES, gp, constraint, owner=self, max_values=ystar)
+
+    def get_acquisition_params(self):
+        return {"n_samples": self.n_samples, "n_features": self.n_features,
+                "n_max_candidates": self.n_max_candidates}
+
+    def set_acquisition_params(self, params):
+        self.n_samples = _check_int("n_samples", params["n_samples"], 1, B.MAX_PATHS)
+        self.n_features = _check_int("n_features", params["n_features"], 1)
+        self.n_max_candidates = _check_int("n_max_candidates", params["n_max_candidates"], 1)
 
 
 _HOOKED = {
@@ -257,6 +363,6 @@ class GPHedge(_ref.GPHedge):
 # isinstance(x, bayes_opt.acquisition.AcquisitionFunction) does in the reference (abc virtual subclasses:
 # the concrete classes keep the reference's MRO).
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, ConstantLiar, GPHedge,
-             ThompsonSampling, ConstrainedThompsonSampling):
+             ThompsonSampling, ConstrainedThompsonSampling, MaxValueEntropySearch):
     AcquisitionFunction.register(_cls)
 del _cls

@@ -128,6 +128,7 @@ struct b200bo_gp {
     std::vector<double> y_raw;   // host copy of the raw targets (n)
     bool normalize = false;
     std::vector<int> xform;      // host copy (d) or empty
+    std::vector<double> ystar;   // MES samples of the maximum (b200bo_gp_set_max_values), or empty
     DevBuf X, Xs, y, K, L, W, WT, T, alphav, v1, v2, ls, xf, info, part;
     // predict-side scratch (used when this handle is gps[0] of a call)
     DevBuf pscratch, xc, out_acq, out_mu, out_sd, sel, clamp;
@@ -326,6 +327,16 @@ extern "C" int b200bo_gp_set_transform(b200bo_gp* gp, const int32_t* xform, int 
         }
     }
     gp->fitted = false;
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_gp_set_max_values(b200bo_gp* gp, const double* ystar, int K) {
+    if (!gp) return set_err(B200BO_ERR_ARG, "gp is NULL");
+    if (K < 0 || K > B200BO_MAX_PATHS) return set_err(B200BO_ERR_ARG, "K=%d out of range [0,%d]", K, B200BO_MAX_PATHS);
+    if (K > 0 && !ystar) return set_err(B200BO_ERR_ARG, "ystar is NULL");
+    for (int k = 0; k < K; ++k)
+        if (!std::isfinite(ystar[k])) return set_err(B200BO_ERR_ARG, "ystar[%d] is not finite", k);
+    gp->ystar.assign(ystar, ystar + K);
     return B200BO_OK;
 }
 
@@ -1124,7 +1135,7 @@ static int check_spec(const b200bo_acq* spec) {
     if (!spec) return set_err(B200BO_ERR_ARG, "spec is NULL");
     if (spec->n_gps < 1 || spec->n_gps > B200BO_MAX_GPS)
         return set_err(B200BO_ERR_ARG, "n_gps=%d out of range [1,%d]", spec->n_gps, B200BO_MAX_GPS);
-    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_NONE)
+    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_MES)
         return set_err(B200BO_ERR_ARG, "unknown acquisition kind %d", spec->kind);
     if (spec->path != B200BO_PATH_AUTO && spec->path != B200BO_PATH_STABLE)
         return set_err(B200BO_ERR_ARG, "unknown path policy %d", spec->path);
@@ -1138,6 +1149,8 @@ static int check_spec(const b200bo_acq* spec) {
         if (g >= 1 && !(spec->lb[g] < spec->ub[g]))
             return set_err(B200BO_ERR_ARG, "constraint %d: lb must be < ub", g);
     }
+    if (spec->kind == B200BO_ACQ_MES && spec->gps[0]->ystar.empty())
+        return set_err(B200BO_ERR_STATE, "MES: gps[0] holds no samples of the maximum (b200bo_gp_set_max_values)");
     return B200BO_OK;
 }
 
@@ -1200,6 +1213,10 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
     P.kappa = spec->kappa;
     P.xi = spec->xi;
     P.y_max = spec->y_max;
+    if (spec->kind == B200BO_ACQ_MES) {
+        P.n_ystar = (int)g0->ystar.size();
+        for (int k = 0; k < P.n_ystar; ++k) P.ystar[k] = g0->ystar[k];
+    }
     P.Xc = src.philox ? nullptr : src.d_Xc;
     P.index_base = index_base;
     if (src.philox) {

@@ -108,6 +108,20 @@ __device__ __forceinline__ double norm_pdf(double x) {
     return exp(-(x * x) / 2.0) / 2.50662827463100050242;
 }
 
+// log Psi(g) and the inverse Mills ratio psi(g) / Psi(g) of the standard normal (psi: pdf, Psi: cdf), finite and
+// accurate for every finite g.  Naive log(ndtr(g)) is -inf below g ~ -38 and psi/Psi is 0/0 there, so below 0 both
+// come from the scaled complementary error function: Psi(g) = erfcx(-g/sqrt2) exp(-g^2/2) / 2, hence
+//   log Psi(g) = log(erfcx(-g/sqrt2) / 2) - g^2/2,    psi(g) / Psi(g) = sqrt(2/pi) / erfcx(-g/sqrt2).
+// At and above 0, Psi = ndtr(g) >= 1/2 and log Psi = log1p(-ndtr(-g)) keeps the digits of a Psi close to 1.
+__device__ __forceinline__ double log_ndtr(double g) {
+    if (g < 0.0) return log(0.5 * erfcx(-g * 0.70710678118654752440)) - 0.5 * (g * g);
+    return log1p(-ndtr(-g));
+}
+__device__ __forceinline__ double inv_mills(double g) {
+    if (g < 0.0) return 0.79788456080286535588 / erfcx(-g * 0.70710678118654752440);
+    return norm_pdf(g) / ndtr(g);
+}
+
 // frozen norm(loc, scale).cdf(b) as scipy evaluates it: NaN unless scale > 0
 // (rv_continuous.cdf argcheck), else ndtr((b - loc)/scale).
 __device__ __forceinline__ double norm_cdf_loc_scale(double b, double loc, double scale) {

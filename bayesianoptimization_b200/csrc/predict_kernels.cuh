@@ -44,6 +44,8 @@ struct PredictParams {
     GpDev gp[B200BO_MAX_GPS];
     int n_gps, d, acq_kind, pad0;
     double kappa, xi, y_max;
+    double ystar[B200BO_MAX_PATHS];  // MES: the samples y*_k of the maximum (data units), k < n_ystar
+    int n_ystar, pad1;
     const double* Xc;  // [m][d], or nullptr: candidates generated in-kernel (Philox, select.cuh)
     const double* pbounds;  // Philox mode: [2][d] = lo_j, (hi_j - lo_j)
     unsigned long long seed;  // Philox key
@@ -107,9 +109,23 @@ __device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, dou
                  : "d"(a0), "d"(a1), "d"(b));
 }
 
+// One sample's term of max-value entropy search (Wang & Jegelka, ICML 2017, eq. 6) at g = (y*_k - mu) / sigma:
+//   g psi(g) / (2 Psi(g)) - log Psi(g)
+// Out of line (DESIGN.md 4.8): inlined into the 16-warp kernel, which runs at its 128-register cap, the term's
+// libdevice code made ptxas place spill code in the clustered kernel's phase-B k-loop; as a call, the spill code the
+// MES branch adds in every predict kernel lies outside the phase-B k-loops.  For finite g the product is finite (psi
+// underflows to 0 above g ~ 38.6); the guard keeps g = +inf (sigma underflowing against y* - mu) at its limit 0.
+__device__ __noinline__ double mes_term(double g) {
+    const double r = inv_mills(g);
+    const double a = (r == 0.0) ? 0.0 : 0.5 * g * r;
+    return a - log_ndtr(g);
+}
+
 // ---- per-candidate epilogue shared by the tiled and the small-batch kernels ---------------------
 // mu_n: K* alpha_ (normalised units); colsq: sum_i V_i^2.  g = 0: target GP -> base acquisition;
 // g >= 1: constraint GP -> probability factor.  The last GP writes -base * prod.
+// MES: base = (1/K) sum_k, in k order, mes_term((y*_k - mean) / sd); base = 0 when sd == 0 (a clamped variance:
+// the predictive distribution is a point mass, an observation there teaches nothing).
 __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const GpDev& G, int g,
                                                    double mu_n, double colsq, long long gi,
                                                    double& base_neg, double& prod, double* final_val = nullptr) {
@@ -131,6 +147,12 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
         } else if (P.acq_kind == B200BO_ACQ_POI) {
             const double z = (mean - P.y_max - P.xi) / sd;
             base = ndtr(z);
+        } else if (P.acq_kind == B200BO_ACQ_MES) {
+            if (sd > 0.0) {
+                double s = 0.0;
+                for (int k = 0; k < P.n_ystar; ++k) s += mes_term((P.ystar[k] - mean) / sd);
+                base = s / (double)P.n_ystar;
+            }
         }
         base_neg = -1.0 * base;
         prod = 1.0;

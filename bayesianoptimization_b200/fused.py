@@ -40,17 +40,28 @@ def _as_b200_gp(gp):
 class FusedAcquisition:
     """Callable closure over fitted device GPs.
 
-    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI
+    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES
     gp        fitted B200GaussianProcessRegressor (target)
     constraint  object with .model (list of device GPs), .lb, .ub  (bayes_opt ConstraintModel) or None
     params    either fixed ``kappa``/``xi``/``y_max`` values or ``owner``: an acquisition object whose
               current kappa / xi / y_max are read at every call, as the reference closure does
               (it calls self.base_acq at call time, R/bayes_opt/acquisition.py:207,217).
+    max_values  ACQ_MES only: the K (1..16) samples y* of the maximum, data units (include/b200bo.h).  They are
+              set on every device handle of the target GP each time the specs are built, so several MES closures
+              over one GP, called alternately, each see their own samples.
     """
 
-    def __init__(self, kind, gp, constraint=None, kappa=0.0, xi=0.0, y_max=None, owner=None):
+    def __init__(self, kind, gp, constraint=None, kappa=0.0, xi=0.0, y_max=None, owner=None, max_values=None):
         gp = _as_b200_gp(gp)
         self.kind = int(kind)
+        self._ystar = None
+        if self.kind == B.ACQ_MES:
+            ys = B.c_f64(np.asarray(max_values if max_values is not None else [], dtype=np.float64).reshape(-1))
+            if not 1 <= ys.size <= B.MAX_PATHS or not np.all(np.isfinite(ys)):
+                raise ValueError(f"MES needs 1..{B.MAX_PATHS} finite max_values, got {max_values!r}")
+            self._ystar = ys
+        elif max_values is not None:
+            raise ValueError("max_values belong to ACQ_MES only")
         self.dim = gp.X_train_.shape[1]
         self._gps = [gp]
         self._bounds = [(0.0, 0.0)]
@@ -100,6 +111,9 @@ class FusedAcquisition:
                     sp.gps[g] = handles[g][dv].ptr.value
                     sp.lb[g], sp.ub[g] = self._bounds[g]
             self._specs, self._sig, self._keep = specs, sig, handles
+        if self._ystar is not None:
+            for h in handles[0]:
+                B.check(B.lib().b200bo_gp_set_max_values(h.ptr, B.as_dp(self._ystar), self._ystar.size))
         for sp in self._specs:
             sp.kappa, sp.xi = kappa, xi
             sp.y_max = 0.0 if y_max is None else float(y_max)

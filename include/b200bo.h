@@ -52,6 +52,16 @@ extern "C" {
 #define B200BO_ACQ_EI 1
 #define B200BO_ACQ_POI 2
 #define B200BO_ACQ_NONE 3 /* predict only: no acquisition epilogue */
+/* Max-value entropy search (Wang & Jegelka, "Max-value Entropy Search for Efficient Bayesian Optimization",
+ * ICML 2017).  No counterpart in the reference.  With mu, sigma the target GP's posterior (data units, as for EI)
+ * and y*_0 .. y*_{K-1} the samples of the maximum set on gps[0] by b200bo_gp_set_max_values:
+ *   g_k   = (y*_k - mu) / sigma
+ *   alpha = (1/K) sum_{k=0..K-1}, in k order, [ g_k psi(g_k) / (2 Psi(g_k)) - log Psi(g_k) ]   (psi, Psi: N(0,1) pdf, cdf)
+ *   acq_neg = -alpha [* prod_j p_j]  (the constraint factors of EI / PoI)
+ * sigma = 0 (a clamped variance): alpha = 0 - the predictive distribution is a point mass.  log Psi and psi / Psi are
+ * evaluated through erfcx below g = 0 and through ndtr / log1p at and above it: finite for every finite g.
+ * Without a feasible registered point the constrained form still ranks candidates (EI / PoI raise there). */
+#define B200BO_ACQ_MES 4
 
 #define B200BO_MAX_GPS 8   /* 1 target GP + up to 7 constraint GPs per call */
 #define B200BO_MAX_DIM 64  /* max input dimension d */
@@ -131,6 +141,12 @@ int b200bo_gp_set_private_stream(b200bo_gp* gp, int enable);
 /* Optional per-dimension input transform (wrap_kernel); xform has d entries or NULL. Must be
  * set before fit.  Replaces R/bayes_opt/parameter.py:484-487 for float/int parameters. */
 int b200bo_gp_set_transform(b200bo_gp* gp, const int32_t* xform, int d);
+
+/* Samples y*_0 .. y*_{K-1} of the maximum for B200BO_ACQ_MES (data units), stored as a host copy on this handle and
+ * passed to the kernel by value when the handle is gps[0] of an MES call.  0 <= K <= B200BO_MAX_PATHS; K = 0 clears
+ * them.  Non-finite values or K out of range: B200BO_ERR_ARG.  An MES call whose gps[0] holds none returns
+ * B200BO_ERR_STATE.  Fits keep them; a replica (b200bo_gp_replicate) is a handle of its own and needs its own call. */
+int b200bo_gp_set_max_values(b200bo_gp* gp, const double* ystar, int K);
 
 /* Replaces the tail of GaussianProcessRegressor.fit (SK/gaussian_process/_gpr.py:275-285,
  * :349-367): y normalisation, K = k(X,X), K_ii += alpha, L = chol(K), alpha_ = K^-1 y, plus
