@@ -14,6 +14,7 @@
 #include <thread>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <dlfcn.h>
 #include <nccl.h>
 #include <nvtx3/nvToolsExt.h>
@@ -143,6 +144,13 @@ struct b200bo_gp {
     bool pad_valid = false;
     DevBuf cov_xc, cov_kst, cov_v, cov_c, cov_out, cov_mu;  // predict(return_cov=True) scratch
     DevBuf sel_cta;         // per-CTA running selection lists of the fused kernels
+    // selection-only pruning: bound keys / local indices (two buffers each for the radix sort), its temp storage and
+    // the control words of predict_acq16_kernel's prune mode
+    DevBuf prune_key, prune_idx, prune_tmp, prune_ctl;
+    // candidates of the last call (chunked: all chunks) and those of them evaluated outside the prune mode; the
+    // prune mode counts its own in prune_ctl[2] (prune_counted)
+    long long stat_total = 0, stat_direct = 0;
+    bool prune_counted = false;
     DevBuf pbounds, prow;   // throughput mode: Philox bounds (lo, span) / regenerated winner rows
     bool replica = false;   // predict-only copy made by b200bo_gp_replicate
     // look-ahead Cholesky: bulk stream, chain/bulk events, copy of the next diagonal step's panel block
@@ -238,6 +246,8 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
+    CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
@@ -276,7 +286,8 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
                       &gp->pscratch, &gp->xc, &gp->out_acq, &gp->out_mu, &gp->out_sd, &gp->sel,
                       &gp->clamp, &gp->s_ksm, &gp->s_partial, &gp->s_mupart, &gp->s_unit, &gp->s_rb, &gp->s_colsq,
                       &gp->tc_linv, &gp->pad_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
-                      &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside};
+                      &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside, &gp->prune_key, &gp->prune_idx,
+                      &gp->prune_tmp, &gp->prune_ctl};
     for (DevBuf* b : bufs) b->release();
     if (gp->stream) cudaStreamDestroy(gp->stream);
     if (gp->fgraph_exec) cudaGraphExecDestroy(gp->fgraph_exec);
@@ -1103,6 +1114,49 @@ static float predict_linv_l2_last() {
     return kDefaultLinvL2Last;
 }
 
+// selection-only pruning (DESIGN.md 4.9) of selection-only calls of the 16-warp fp64 kernel; B200BO_PRUNE=0 turns it
+// off (read per call) for A/B measurements
+static bool prune_enabled() {
+    const char* e = getenv("B200BO_PRUNE");
+    return !(e && e[0] == '0');
+}
+
+// Bound pass + radix sort of (bound key, local index): fills P.perm / P.perm_key / P.prune_ctl for predict_acq16_kernel.
+// The k-th key word and the evaluated count carry over from launch to launch of a chunked batch (resume).
+static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool dreg, bool resume, cudaStream_t stream) {
+    const long long m = P.m, ntiles = (m + PBN - 1) / PBN;
+    int rc;
+    if ((rc = g0->prune_key.reserve(sizeof(unsigned long long) * 2 * (size_t)m))) return rc;
+    if ((rc = g0->prune_idx.reserve(sizeof(int) * 2 * (size_t)m))) return rc;
+    if ((rc = g0->prune_ctl.reserve(sizeof(unsigned long long) * 3))) return rc;
+    unsigned long long* keys = g0->prune_key.as<unsigned long long>();
+    int* idx = g0->prune_idx.as<int>();
+    unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
+    const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
+    if (dreg)
+        predict_bound_kernel<true><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr);
+    else
+        predict_bound_kernel<false><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    cub::DoubleBuffer<unsigned long long> kb(keys, keys + m);
+    cub::DoubleBuffer<int> ib(idx, idx + m);
+    size_t tmp = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, kb, ib, (int)m, 0, 64, stream));
+    if ((rc = g0->prune_tmp.reserve(tmp))) return rc;
+    CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, kb, ib, (int)m, 0, 64, stream));
+    LAUNCHED();
+    CU(cudaMemsetAsync(ctl, 0, sizeof(unsigned long long), stream));
+    if (!resume) {
+        CU(cudaMemsetAsync(ctl + 1, 0xFF, sizeof(unsigned long long), stream));
+        CU(cudaMemsetAsync(ctl + 2, 0, sizeof(unsigned long long), stream));
+    }
+    P.perm = ib.Current();
+    P.perm_key = kb.Current();
+    P.prune_ctl = ctl;
+    return B200BO_OK;
+}
+
 // padded stage images of L^-1 for the bulk-copy phase B of the fp64 kernel (once per fit)
 static int ensure_pad(b200bo_gp* gp, cudaStream_t stream) {
     if (gp->pad_valid) return B200BO_OK;
@@ -1171,21 +1225,14 @@ struct SelMode {
     int finish = 1;
 };
 
-static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, double* d_acq_neg, double* d_mu,
-                     double* d_sd, int k, void* d_sel, int64_t index_base, cudaStream_t stream,
-                     SelMode sm = SelMode()) {
+// launch parameters of the predict kernels for spec over the candidates of src (everything but outputs and scratch);
+// np_max: the largest padded training size of the spec's GPs
+static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, int64_t index_base, cudaStream_t stream,
+                       PredictParams& P, int& np_max) {
     int rc;
-    if ((rc = check_spec(spec))) return rc;
-    if (m < 0 || (m > 0 && !src.philox && !src.d_Xc)) return set_err(B200BO_ERR_ARG, "bad candidates");
-    if (src.philox && (!src.lo || !src.hi)) return set_err(B200BO_ERR_ARG, "Philox mode needs lo/hi");
-    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
-    if (k > 0 && !d_sel) return set_err(B200BO_ERR_ARG, "d_sel is NULL");
     b200bo_gp* g0 = spec->gps[0];
-    CU(cudaSetDevice(g0->device));
-    NvtxRange nvtx_range("b200bo:predict_acq");
-    PredictParams P;
     memset(&P, 0, sizeof(P));
-    int np_max = 0;
+    np_max = 0;
     for (int g = 0; g < spec->n_gps; ++g) {
         b200bo_gp* gp = spec->gps[g];
         GpDev& G = P.gp[g];
@@ -1201,6 +1248,7 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
         G.nu = gp->nu;
         G.constv = gp->constv;
         G.prior = gp->constv + gp->noise;
+        G.kdiag = gp->constv + gp->jitter;
         G.y_mean = gp->y_mean;
         G.y_std = gp->y_std;
         G.lb = spec->lb[g];
@@ -1232,6 +1280,50 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
         P.seed = src.seed;
     }
     P.m = m;
+    return B200BO_OK;
+}
+
+// Pruned selection batches are cut into launches of at most this many candidates: the bound keys, indices and sort
+// buffers take 24 bytes per candidate (about 100 MB here), whatever the size of a Philox batch.
+constexpr long long kPruneMaxBatch = 1ll << 22;
+
+static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, double* d_acq_neg, double* d_mu,
+                       double* d_sd, int k, void* d_sel, int64_t index_base, cudaStream_t stream, SelMode sm);
+
+static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, double* d_acq_neg, double* d_mu,
+                     double* d_sd, int k, void* d_sel, int64_t index_base, cudaStream_t stream,
+                     SelMode sm = SelMode()) {
+    const bool split = k > 0 && !d_acq_neg && !d_mu && !d_sd && m > kPruneMaxBatch && prune_enabled() && spec &&
+                       spec->gps[0];
+    if (!split) return eval_launch(spec, src, m, d_acq_neg, d_mu, d_sd, k, d_sel, index_base, stream, sm);
+    // consecutive launches continue the per-CTA selection lists (and the pruning's k-th key), one merge at the end
+    for (long long c0 = 0; c0 < m; c0 += kPruneMaxBatch) {
+        const long long mc = m - c0 < kPruneMaxBatch ? m - c0 : kPruneMaxBatch;
+        CandSrc s = src;
+        if (!s.philox && s.d_Xc) s.d_Xc += (size_t)c0 * spec->gps[0]->d;
+        SelMode part;
+        part.resume = sm.resume || c0 > 0;
+        part.finish = sm.finish && c0 + mc >= m;
+        const int rc = eval_launch(spec, s, mc, nullptr, nullptr, nullptr, k, d_sel, index_base + c0, stream, part);
+        if (rc) return rc;
+    }
+    return B200BO_OK;
+}
+
+static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, double* d_acq_neg, double* d_mu,
+                       double* d_sd, int k, void* d_sel, int64_t index_base, cudaStream_t stream, SelMode sm) {
+    int rc;
+    if ((rc = check_spec(spec))) return rc;
+    if (m < 0 || (m > 0 && !src.philox && !src.d_Xc)) return set_err(B200BO_ERR_ARG, "bad candidates");
+    if (src.philox && (!src.lo || !src.hi)) return set_err(B200BO_ERR_ARG, "Philox mode needs lo/hi");
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (k > 0 && !d_sel) return set_err(B200BO_ERR_ARG, "d_sel is NULL");
+    b200bo_gp* g0 = spec->gps[0];
+    CU(cudaSetDevice(g0->device));
+    NvtxRange nvtx_range("b200bo:predict_acq");
+    PredictParams P;
+    int np_max = 0;
+    if ((rc = fill_params(spec, src, m, index_base, stream, P, np_max))) return rc;
     P.acq_out = d_acq_neg;
     P.mu_out = d_mu;
     P.sd_out = d_sd;
@@ -1243,7 +1335,7 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
     if (sm.resume || !sm.finish) grid = g0->sm_count;  // chunked batches keep one list per SM across launches
     const bool small = grid > 0 && !sm.resume && sm.finish &&
                        use_small_path(m, np_max, spec->n_gps, g0->sm_count, spec->path);
-    bool fused_sel = false;
+    bool fused_sel = false, prune = false;
     if (small) {
         if (k > 0 && !P.acq_out) {  // the small path selects from the materialised values
             if ((rc = g0->out_acq.reserve(sizeof(double) * (size_t)(m > 0 ? m : 1)))) return rc;
@@ -1326,6 +1418,11 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
                 }
                 CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off staging from the kernel time
             }
+            const int kind = spec->kind;
+            prune = fused_sel && !P.acq_out && !P.mu_out && !P.sd_out && P.n_gps == 1 && pipe != PIPE_BULK_MC &&
+                    (kind == B200BO_ACQ_EI || kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_POI) &&
+                    m <= std::numeric_limits<int>::max() && prune_enabled();
+            if (prune && (rc = prune_prepare(g0, P, dreg, sm.resume, stream))) return rc;
             if (predict_mma() == 884) {
                 rc = launch_predict16<884, PIPE_CPASYNC>(dreg, grid, stream, P);
             } else if (pipe == PIPE_BULK_MC) {
@@ -1356,6 +1453,15 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
         CU(cudaEventRecord(g0->ev1, stream));
         g_last_timed = g0;
     }
+    if (!sm.resume) {
+        g0->stat_total = g0->stat_direct = 0;
+        g0->prune_counted = false;
+    }
+    g0->stat_total += m;
+    if (prune)
+        g0->prune_counted = true;
+    else
+        g0->stat_direct += m;
     if (k > 0 && sm.finish) {
         NvtxRange nvtx_sel("b200bo:select");
         if (fused_sel) {
@@ -1380,6 +1486,35 @@ extern "C" int b200bo_acq_eval_dev(const b200bo_acq* spec, const double* d_Xc, i
     return eval_core(spec, src, m, d_acq_neg, d_mu, d_sd, k, d_sel, index_base, (cudaStream_t)stream_);
 }
 
+extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
+                                          double* d_kmax, void* stream_) {
+    int rc;
+    if ((rc = check_spec(spec))) return rc;
+    if (spec->n_gps != 1 ||
+        (spec->kind != B200BO_ACQ_EI && spec->kind != B200BO_ACQ_UCB && spec->kind != B200BO_ACQ_POI))
+        return set_err(B200BO_ERR_ARG, "the pruning bound covers EI, UCB and PoI on one GP");
+    if (m <= 0 || m > std::numeric_limits<int>::max() || !d_Xc || !d_key)
+        return set_err(B200BO_ERR_ARG, "bad candidates or key buffer");
+    b200bo_gp* g0 = spec->gps[0];
+    CU(cudaSetDevice(g0->device));
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    CandSrc src;
+    src.d_Xc = d_Xc;
+    PredictParams P;
+    int np_max = 0;
+    if ((rc = fill_params(spec, src, m, 0, stream, P, np_max))) return rc;
+    const unsigned ntiles = (unsigned)((m + PBN - 1) / PBN);
+    const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
+    auto keys = reinterpret_cast<unsigned long long*>(d_key);
+    if (P.d <= kPredictMaxDimRegs)
+        predict_bound_kernel<true><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax);
+    else
+        predict_bound_kernel<false><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    return B200BO_OK;
+}
+
 extern "C" int b200bo_acq_select_philox_dev(const b200bo_acq* spec, uint64_t seed, const double* lo,
                                             const double* hi, int64_t m, int64_t index_base, int k, void* d_sel,
                                             void* stream_) {
@@ -1400,6 +1535,20 @@ extern "C" int b200bo_last_kernel_ms(float* ms) {
     CU(cudaEventSynchronize(g_last_timed->ev1));
     CU(cudaEventElapsedTime(ms, g_last_timed->ev0, g_last_timed->ev1));
     return check_pipe_timeout(g_last_timed);
+}
+
+extern "C" int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total) {
+    if (!evaluated || !total) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!g_last_timed) return set_err(B200BO_ERR_STATE, "no timed kernel on this thread");
+    b200bo_gp* g0 = g_last_timed;
+    CU(cudaSetDevice(g0->device));
+    CU(cudaEventSynchronize(g0->ev1));
+    unsigned long long pruned_eval = 0;
+    if (g0->prune_counted) CU(cudaMemcpy(&pruned_eval, g0->prune_ctl.as<unsigned long long>() + 2, sizeof(pruned_eval),
+                                         cudaMemcpyDeviceToHost));
+    *evaluated = g0->stat_direct + (int64_t)pruned_eval;
+    *total = g0->stat_total;
+    return B200BO_OK;
 }
 
 // Host-buffer front end shared by predict / acq_eval / argmin_topk.  Large selection-only batches are

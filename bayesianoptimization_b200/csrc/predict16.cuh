@@ -51,11 +51,15 @@ __device__ __forceinline__ void st_global_hint(double* p, double v, unsigned lon
 
 // ---- phase A: K*^T tile (np x 128) into the CTA's scratch + K* alpha_ -----------------------------
 // KSTR: row stride of the K* scratch in doubles: PBN (cp.async phase B) or PSTR_DMMA (bulk-copy phase B: the rows
-// of a stage are then contiguous in global memory exactly as in shared memory, one copy per stage)
+// of a stage are then contiguous in global memory exactly as in shared memory, one copy per stage).
+// KSTR = 0: the bound pass of pruning (predict_bound_kernel): no K* is stored; each thread keeps the largest |K*_i| of
+// its rows in kmax_s[part][c] instead.
+// Column c is candidate c0 + c, or perm[c0 + c] when P.perm is set (tiles in bound order).
 template <bool DREG, int COV, int KSTR>
 __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
                                                        double* __restrict__ Ks, double* smem,
-                                                       double (*mu_s)[PBN], unsigned long long pol_first) {
+                                                       double (*mu_s)[PBN], unsigned long long pol_first,
+                                                       double (*kmax_s)[PBN]) {
     const int tid = threadIdx.x;
     const int d = P.d, np = G.np;
     double* xc_s = smem;                              // [d][PBN]
@@ -66,7 +70,7 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
         const long long gi = c0 + c;
         double v = 0.0;
         if (gi < P.m) {
-            v = candidate_coord(P, gi, j);
+            v = candidate_coord(P, P.perm ? (long long)P.perm[gi] : gi, j);
             if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
             v = v / G.ls[j];
         }
@@ -90,7 +94,7 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
 #pragma unroll
         for (int j = 0; j < kPredictMaxDimRegs; ++j) xc[j] = (j < d) ? xc_s[j * PBN + c] : 0.0;
     }
-    double mu_acc = 0.0;
+    double mu_acc = 0.0, kmax = 0.0;
     constexpr int R = 8;
     constexpr int ROWS = PA_CHUNK / P16_SPLIT;  // 16 rows of every chunk per thread
     for (int ch = 0; ch < nch; ++ch) {
@@ -143,7 +147,10 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
                 const int n = ch * PA_CHUNK + r0 + q;
                 double kv = G.constv * cov_eval<COV>(r2[q]);
                 if (n >= G.n) kv = 0.0;
-                st_global_hint(Ks + (size_t)n * KSTR + c, kv, pol_first);
+                if constexpr (KSTR == 0)
+                    kmax = fmax(kmax, fabs(kv));
+                else
+                    st_global_hint(Ks + (size_t)n * KSTR + c, kv, pol_first);
                 mu_acc = fma(al[r0 + q], kv, mu_acc);
             }
         }
@@ -151,6 +158,7 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
     }
     cp_async_wait<0>();
     mu_s[part][c] = mu_acc;
+    if constexpr (KSTR == 0) kmax_s[part][c] = kmax;
     __threadfence_block();
     __syncthreads();
 }
@@ -158,13 +166,85 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
 template <bool DREG, int KSTR>
 __device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const GpDev& G, long long c0,
                                                   double* __restrict__ Ks, double* smem, double (*mu_s)[PBN],
-                                                  unsigned long long pol_first) {
+                                                  unsigned long long pol_first, double (*kmax_s)[PBN] = nullptr) {
     switch (cov_code(G.family, G.nu)) {
-        case 0: predict16_phase_a_impl<DREG, 0, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
-        case 1: predict16_phase_a_impl<DREG, 1, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
-        case 2: predict16_phase_a_impl<DREG, 2, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
-        default: predict16_phase_a_impl<DREG, 3, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first); break;
+        case 0: predict16_phase_a_impl<DREG, 0, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
+        case 1: predict16_phase_a_impl<DREG, 1, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
+        case 2: predict16_phase_a_impl<DREG, 2, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
+        default: predict16_phase_a_impl<DREG, 3, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
     }
+}
+
+// ---- selection-only pruning: the bound pass ------------------------------------------------------------------
+// For the selection of the k smallest closure values -acq (EI, UCB, PoI on one GP; DESIGN.md 4.9), a key per candidate
+// that no candidate's exact key can be below: key_nan_last(v_lb) with v_lb <= -acq(mu, sigma).
+//   sigma^2 = prior - k*^T K^-1 k* <= prior - max_i k*_i^2 / K_ii (Cauchy-Schwarz in the K^-1 inner product) = var_ub;
+//   eps * prior absorbs the rounding of the explicit-inverse sum of squares the exact value is computed from;
+//   EI and UCB (as max(mu, mu + kappa sigma)) do not decrease with sigma, nor does PoI while a = mu - y_max - xi < 0
+//   (PoI <= 1 otherwise); v_lb is lowered by a relative and an absolute margin against the rounding of ndtr / pdf.
+// Key 0 (never pruned): mu or v_lb non-finite, or a within a few ulps of 0 (sigma = 0 with a = 0 gives the NaN that
+// np.argmin reports first).  mu is bit-equal to the epilogue's: the same phase A, the same order of sums.
+constexpr double kPruneVarEps = 1e-8, kPruneRelMargin = 1e-9, kPruneAbsMargin = 1e-300;
+
+__device__ __forceinline__ unsigned long long prune_bound_key(const PredictParams& P, const GpDev& G, double mu_n,
+                                                              double kmax) {
+    const double mean = G.y_std * mu_n + G.y_mean;
+    const double var_ub = fmax(0.0, fmin(G.prior, G.prior - kmax * kmax / G.kdiag + kPruneVarEps * G.prior));
+    const double sd = sqrt(var_ub * (G.y_std * G.y_std));
+    const double a = mean - P.y_max - P.xi;
+    double base, scale;
+    if (P.acq_kind == B200BO_ACQ_UCB) {
+        base = fmax(mean, mean + P.kappa * sd);
+        scale = fabs(mean) + fabs(P.kappa * sd);
+    } else if (P.acq_kind == B200BO_ACQ_EI) {
+        const double z = a / sd;
+        base = a * ndtr(z) + sd * norm_pdf(z);
+        scale = fabs(base);
+    } else {
+        base = a < 0.0 ? ndtr(a / sd) : 1.0;
+        scale = fabs(base);
+    }
+    const double v_lb = -base - (kPruneRelMargin * scale + kPruneAbsMargin);
+    const bool a_near_0 = P.acq_kind != B200BO_ACQ_UCB &&
+                          fabs(a) <= 8.0 * 2.220446049250313e-16 * (fabs(mean) + fabs(P.y_max) + fabs(P.xi));
+    if (!isfinite(mean) || !isfinite(v_lb) || a_near_0) return 0ull;
+    return key_nan_last(v_lb);
+}
+
+// One CTA per tile of PBN candidates: phase A without the K* stores, then (key, local index) per candidate; idx and
+// kmax_out (max_i |K*_i|, for b200bo_acq_prune_bound_dev) may be nullptr.
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictParams P, unsigned long long* keys,
+                                                               int* idx, double* kmax_out) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    __shared__ double kmax_s[P16_SPLIT][PBN];
+    const long long c0 = (long long)blockIdx.x * PBN;
+    const GpDev& G = P.gp[0];
+    predict16_phase_a<DREG, 0>(P, G, c0, nullptr, smem, mu_s, 0ull, kmax_s);
+    const int c = threadIdx.x;
+    if (c < PBN && c0 + c < P.m) {
+        const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
+        const double kmax = fmax(fmax(kmax_s[0][c], kmax_s[1][c]), fmax(kmax_s[2][c], kmax_s[3][c]));
+        keys[c0 + c] = prune_bound_key(P, G, mu_n, kmax);
+        if (idx) idx[c0 + c] = (int)(c0 + c);
+        if (kmax_out) kmax_out[c0 + c] = kmax;
+    }
+}
+
+// Prune mode of predict_acq16_kernel: thread 0 claims the next tile in bound order and stops the CTA (returns ntiles)
+// once the tile's best bound key is above the least k-th key any CTA has published: every later tile's keys are
+// larger still, and a CTA's k-th key bounds the global k-th key from above.  Counts the candidates it lets through.
+__device__ __forceinline__ long long prune_claim(const PredictParams& P, long long ntiles, long long& tile_s) {
+    if (threadIdx.x == 0) {
+        long long t = (long long)atomicAdd(P.prune_ctl, 1ull);
+        if (t < ntiles && P.perm_key[t * PBN] > *reinterpret_cast<volatile unsigned long long*>(P.prune_ctl + 1))
+            t = ntiles;
+        if (t < ntiles) atomicAdd(P.prune_ctl + 2, (unsigned long long)min((long long)PBN, P.m - t * PBN));
+        tile_s = t;
+    }
+    __syncthreads();
+    return tile_s;
 }
 
 // stage loader: BK k-rows x 128 doubles of LinvT (evict_last) and of K* (evict_first), 512 threads
@@ -539,7 +619,10 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
         if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
         __syncthreads();
     }
-    for (long long tile = blockIdx.x; tile - rank < ntiles; tile += gridDim.x) {
+    // prune mode (P.perm, never with PIPE_BULK_MC): tiles claimed in bound order; `it` only crosses tile boundaries
+    __shared__ long long tile_s;
+    for (long long tile = P.perm ? prune_claim(P, ntiles, tile_s) : blockIdx.x; tile - rank < ntiles;
+         tile = P.perm ? prune_claim(P, ntiles, tile_s) : tile + gridDim.x) {
         const long long c0 = tile * PBN;
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
@@ -555,10 +638,14 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
                 const int c = tid;
                 const double colsq = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
                 const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
+                const long long gi = (P.perm && c0 + c < P.m) ? (long long)P.perm[c0 + c] : c0 + c;
                 double val = 0.0;
-                candidate_epilogue(P, G, g, mu_n, colsq, c0 + c, base_s[c], prod_s[c], &val);
-                if (P.sel_cta && g == P.n_gps - 1)
-                    runsel_update<1>(sel_s, P.sel_k, tid, val, c0 + c + P.index_base, c0 + c < P.m);
+                candidate_epilogue(P, G, g, mu_n, colsq, gi, base_s[c], prod_s[c], &val);
+                if (P.sel_cta && g == P.n_gps - 1) {
+                    runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, c0 + c < P.m);
+                    if (P.perm && tid == 0 && sel_s.list.idx[P.sel_k - 1] != SEL_NOIDX)
+                        atomicMin(P.prune_ctl + 1, sel_s.list.key[P.sel_k - 1]);
+                }
             }
             __syncthreads();
         }

@@ -38,6 +38,7 @@ struct GpDev {
     int n, np, family, nu;
     double constv, y_mean, y_std, lb, ub;
     double prior;  // prior variance kernel_.diag(x*) = constv + WhiteKernel noise_level
+    double kdiag;  // diagonal of the factorised training covariance: constv + noise_level + alpha
 };
 
 struct PredictParams {
@@ -60,6 +61,11 @@ struct PredictParams {
     long long scratch_stride;
     unsigned long long* clamp_count;  // nullable; [0] negative variances clamped to 0, [1] non-finite candidate coordinates
     float linv_l2_last;  // predict_acq16_kernel: evict_last fraction of the L^-1 loads; <= 0: evict_normal
+    // selection-only pruning (predict16.cuh, DESIGN.md 4.9), or nullptr: tile t of predict_acq16_kernel is the
+    // candidates perm[t * PBN ..] (local indices sorted by the key of a lower bound on their value, perm_key)
+    const int* perm;
+    const unsigned long long* perm_key;
+    unsigned long long* prune_ctl;  // [0] next tile to claim, [1] least k-th key of a full CTA list, [2] evaluated
 };
 
 // coordinate j of candidate gi (local index) as the reference's x_tries[gi, j]

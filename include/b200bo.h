@@ -330,9 +330,22 @@ int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G, const dou
                                      int64_t* topk_idx, double* topk_x);
 
 /* Duration (ms) of the most recent fused predict+acquisition kernel launched through a
- * device or host entry point on this thread, measured with CUDA events on its stream.
+ * device or host entry point on this thread, measured with CUDA events on its stream.  With selection-only pruning
+ * (DESIGN.md 4.9) it includes the bound pass and the sort; the selection merge is outside it either way.
  * Synchronises on the stop event. */
 int b200bo_last_kernel_ms(float* ms);
+
+/* Candidates of the most recent fused predict+acquisition call on this thread (a streamed host batch: all its chunks)
+ * and how many of them went through the N^2 term.  Fewer than all when selection-only pruning skipped candidates whose
+ * acquisition bound cannot reach the top-k (DESIGN.md 4.9).  Synchronises on the stop event. */
+int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total);
+
+/* The bound pass of selection-only pruning alone (EI, UCB or PoI on one GP; 1 <= m <= INT_MAX device rows d_Xc):
+ * d_key[i] = the order key (key_nan_last of select.cuh) of a lower bound on candidate i's closure value -acq, 0 for a
+ * candidate that is never pruned; d_kmax[i] (nullable) = max_j |k(x_i, X_j)| in normalised units.  Enqueued on
+ * `stream`, not synchronised.  For checking the bound against exact values. */
+int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key, double* d_kmax,
+                               void* stream);
 
 #ifdef __cplusplus
 }
