@@ -503,8 +503,10 @@ static int factor_body(b200bo_gp* gp) {
     // right-looking blocked Cholesky, panel width 64.  B200BO_POTRF=legacy selects the first
     // (unblocked) diagonal-block kernel, B200BO_POTRF=serial the blocked kernel without look-ahead, for A/B
     // measurements.
+    // B200BO_GEMM=64 takes the serial loop too: the look-ahead needs the side store of A[j+2, j+1] that only the
+    // 128-tile trailing update writes, and with 64-tile GEMMs the next diagonal block read a stale copy of it.
     const bool legacy_potrf = potrf_mode() == 2, serial_potrf = potrf_mode() == 1;
-    if (legacy_potrf || serial_potrf || np <= 128) {
+    if (legacy_potrf || serial_potrf || gemm_force64() || np <= 128) {
         for (int j0 = 0; j0 < np; j0 += 64) {
             if (legacy_potrf)
                 potrf_diag_legacy_kernel<<<1, 256, kPotrfLegacySmemBytes, g_st>>>(L, np, j0, W + (size_t)j0 * np + j0, np,

@@ -14,7 +14,9 @@ constexpr int kPad = 128;  // training-set size is padded to a multiple of this
 // The kernel-matrix builders evaluate sqrt and exp for every (training point, candidate) pair
 // with only a few resident warps, so data-dependent slow-path branches (libm special cases) and
 // their code size hurt more than the arithmetic.  Both routines are within 2 ulp of libm on their
-// domain (checked against numpy over 3e5 random arguments), far inside the 1e-5 parity bar.
+// domain (checked against numpy over 3e5 random arguments), far inside the 1e-5 parity bar.  Composed into a
+// covariance, exp amplifies the relative error of its argument k by k, so cov_eval is within a few ulp times (1 + k)
+// of sklearn's formula evaluated exactly (tests/test_gpu_illcond.py holds it to 4 (1 + k) ulp up to k = 700).
 
 // Polynomial / reduction constants live in constant memory: an fp64 immediate costs two uniform
 // moves every time it is used, a constant-bank operand is free.
@@ -25,9 +27,15 @@ __constant__ double kExpC[14] = {
 __constant__ double kExpR[4] = {1.4426950408889634074, -6.93147180369123816490e-01,
                                 -1.90821492927058770002e-10, 700.0};
 
-// sqrt(x) for x >= 0 (arguments below 1e-30 are treated as 1e-30: |error| <= 1e-15 absolute).
+// sqrt(x) for x >= 0.  Arguments below about 1e-30 are treated as about 1e-30 (|error| <= 1e-15 absolute), arguments
+// above about 1e38 as about 1e38: the float seed of one above FLT_MAX is rsqrtf(inf) = 0, which made the result 0 and
+// a Matern covariance at a huge distance its maximum.  The result there, about 1e19, lies far inside exp_neg's clamp,
+// so every covariance built on it is still its limit 0 (below 1e-265).  Both clamps act on the high word of the bits
+// (an integer min/max: the order of non-negative doubles is the order of their high words), so they stay off the
+// fp64 pipe that bounds phase A; between the clamps the argument is used unchanged.
 __device__ __forceinline__ double sqrt_pos(double x) {
-    const double xc = fmax(x, 1e-30);
+    const int hi = min(max(__double2hiint(x), 0x39B4484B /* high word of 1e-30 */), 0x47D2CED3 /* of 1e38 */);
+    const double xc = __hiloint2double(hi, __double2loint(x));
     double y = (double)rsqrtf((float)xc);  // 2^-23 seed
     const double h = 0.5 * xc;
     y = y * fma(-h * y, y, 1.5);
