@@ -11,7 +11,7 @@ Two layers:
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ThompsonSampling,
     ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, GPHedge, AcquisitionFunction,
-    ConstraintModel, enable(optimizer) - resolved lazily on first access.
+    ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
 """
 from . import _lib
 from ._build import build_library
@@ -26,7 +26,7 @@ _PLUGIN = {
     "ExpectedImprovement": "acquisition", "ProbabilityOfImprovement": "acquisition",
     "ConstantLiar": "acquisition", "GPHedge": "acquisition", "DeviceHooks": "acquisition",
     "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
-    "MaxValueEntropySearch": "acquisition",
+    "MaxValueEntropySearch": "acquisition", "suggest_batch": "acquisition",
     "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
 }
 

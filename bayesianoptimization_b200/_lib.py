@@ -32,7 +32,7 @@ EXPORTS = [
     "b200bo_multi_gpu_acq_eval",
     "b200bo_paths_create", "b200bo_paths_destroy", "b200bo_paths_eval", "b200bo_paths_argmin_topk",
     "b200bo_paths_argmin_topk_philox", "b200bo_paths_bound", "b200bo_cpaths_eval", "b200bo_cpaths_argmin_topk",
-    "b200bo_cpaths_argmin_topk_philox",
+    "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
 ]
 
 
@@ -122,12 +122,14 @@ def lib():
     L.b200bo_paths_destroy.argtypes = [C.c_void_p]
     L.b200bo_paths_destroy.restype = None
     L.b200bo_paths_eval.argtypes = [C.c_void_p, dp, C.c_int64, dp]
+    L.b200bo_paths_eval_rows.argtypes = [C.c_void_p, dp, C.POINTER(C.c_int32), C.c_int64, dp]
     L.b200bo_paths_argmin_topk.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int, dp, i64p, dp, i64p]
     L.b200bo_paths_argmin_topk_philox.argtypes = [C.c_void_p, C.c_uint64, dp, dp, C.c_int64, C.c_int64, C.c_int,
                                                   *philox_outs]
     L.b200bo_paths_bound.argtypes = [C.c_void_p, dp]
     sets = [C.POINTER(C.c_void_p), C.c_int, dp, dp]  # sets, G, lb, ub
     L.b200bo_cpaths_eval.argtypes = [*sets, dp, C.c_int64, dp, dp]
+    L.b200bo_cpaths_eval_rows.argtypes = [*sets, dp, C.POINTER(C.c_int32), C.c_int64, dp]
     L.b200bo_cpaths_argmin_topk.argtypes = [*sets, dp, C.c_int64, C.c_int, dp, i64p, dp, i64p]
     L.b200bo_cpaths_argmin_topk_philox.argtypes = [*sets, C.c_uint64, dp, dp, C.c_int64, C.c_int64, C.c_int,
                                                    *philox_outs]

@@ -17,7 +17,8 @@ inherited), with ``DeviceHooks`` mixed in:
 
 ``ThompsonSampling`` is a policy defined here rather than inherited: a posterior sample path per ``suggest()``,
 ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`` extends it to constrained problems
-(the paths of the target and the constraint GPs, ranked feasible-first).  ``MaxValueEntropySearch`` is the
+(the paths of the target and the constraint GPs, ranked feasible-first); ``suggest_batch`` proposes q points at once
+from q paths (batch Thompson sampling).  ``MaxValueEntropySearch`` is the
 information-based policy: samples of the maximum from posterior paths, then a fused-kernel epilogue of mu and sigma.
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
@@ -180,7 +181,12 @@ class ThompsonSampling(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
     the host, which is O(M^3) in the candidates and drops the refinement).
 
     n_features  random Fourier features of the prior part of each path (the data update is exact).
-    Constraints are not supported (ConstraintNotSupportedError)."""
+    Constraints are not supported (ConstraintNotSupportedError).
+
+    ``suggest_batch(..., q)`` proposes q points per call for parallel evaluation: q paths, one maximiser each
+    (batch Thompson sampling, DESIGN.md 4.7)."""
+
+    _batch_q = None  # inside suggest_batch: the number of paths the closure draws
 
     def __init__(self, n_features=4096, random_state=None):
         super().__init__(random_state=random_state)
@@ -193,14 +199,91 @@ class ThompsonSampling(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
             "ThompsonSampling has no base_acq(mean, std): it ranks candidates by one posterior sample path drawn "
             "per suggest() (B200GaussianProcessRegressor.sample_paths), not by a formula of mean and std")
 
+    def suggest_batch(self, gp, target_space, q, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        """q points to probe next, as a (q, dim) array: the maximisers of q posterior sample paths drawn together.
+
+        Runs the reference's ``suggest`` (its TargetSpaceEmptyError, one ``self.i += 1``, the GP fit), with a
+        closure of q paths instead of one, and from the RandomState draws in this order:
+          1. the q target paths (one ``sample_paths(q, n_features, rs)``), then q paths of each constraint GP;
+          2. ONE candidate set shared by every path: ``space.random_sample(max(n_random, n_smart), rs)``, or one
+             Philox seed in device_philox mode, ranked per path in one device pass (top n_smart per path);
+          3. the refinement: the q x n_smart L-BFGS-B runs in lockstep, every round one device call in which each row
+             is evaluated on its own path only (mixed-integer spaces: the reference's differential evolution per
+             path, in path order, on that path's closure).
+        Per path the reference's rule picks between the random-stage best and the refined best.  Then, in path order,
+        a point bit-equal to an earlier path's is replaced by the best row of its own top-n_smart not yet taken (kept
+        when there is none).  q = 1 returns ``suggest``'s point and leaves the RandomState as ``suggest`` does.
+        1 <= q <= 16, an integer."""
+        q = _check_int("q", q, 1, B.MAX_PATHS)
+        self._batch_q = q
+        try:
+            return self.suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
+                                random_state=random_state)
+        finally:
+            self._batch_q = None
+
+    def _closure(self, paths):
+        from .paths import PathAcquisition, PathBatchAcquisition
+
+        return PathAcquisition(paths) if self._batch_q is None else PathBatchAcquisition(paths)
+
     def _get_acq(self, gp, constraint=None):
         if constraint is not None:
             raise _ConstraintNotSupportedError(
                 f"{type(self).__name__} does not support constrained optimization: a constraint model was given")
-        from .paths import PathAcquisition
-
         rs = self._suggest_rng()  # the path of this call is drawn from the caller's stream
-        return PathAcquisition(_as_b200_gp(gp).sample_paths(1, self.n_features, random_state=rs))
+        return self._closure(_as_b200_gp(gp).sample_paths(self._batch_q or 1, self.n_features, random_state=rs))
+
+    def _acq_min(self, acq, space, random_state, n_random=10_000, n_smart=10):
+        from .paths import PathBatchAcquisition
+
+        if not isinstance(acq, PathBatchAcquisition):
+            return super()._acq_min(acq, space, random_state, n_random=n_random, n_smart=n_smart)
+        if n_random == 0 and n_smart == 0:
+            raise ValueError("n_random and n_smart cannot both be 0")
+        x_r, min_r, tops = self._batch_random_stage(acq.paths, space, random_state, max(n_random, n_smart), n_smart)
+        picks = list(x_r)
+        if n_smart:
+            for p, (x_s, min_s) in enumerate(self._batch_smart_stage(acq, space, tops, random_state)):
+                if min_r[p] > min_s:  # the reference's choice (R/bayes_opt/acquisition.py:267-272), per path
+                    picks[p] = x_s
+        return np.asarray(distinct_picks(picks, tops), dtype=np.float64)
+
+    def _batch_random_stage(self, paths, space, random_state, n, k):
+        """The random stage of DeviceHooks._random_sample_minimize for q paths over ONE candidate set.
+        Returns (q, d) random-stage winners, (q,) their -path values, and per path its top-k rows, best first."""
+        q = paths.n_paths
+        if self.b200_candidate_source == "device_philox" and all(space.continuous_dimensions) and k <= B.MAX_TOPK:
+            _, vals, x_r, _, tx = paths.argmin_topk_philox(_philox_seed(random_state), space.bounds, n, k)
+            return x_r, vals, (tx if k else [[]] * q)
+        x_tries = space.random_sample(n, random_state=random_state)  # the reference's RNG stream
+        if k <= B.MAX_TOPK:
+            idx, vals, ti = paths.argmin_topk(x_tries, k)
+            tops = [x_tries[t] for t in ti]
+        else:  # more seeds than the device selection holds: numpy selection on the device values, as the reference's
+            ys = -paths(x_tries)
+            idx, vals = ys.argmin(axis=0), ys.min(axis=0)
+            tops = [x_tries[np.argsort(ys[:, p])[:k]] for p in range(q)]
+        return x_tries[idx], vals, (tops if k else [[]] * q)
+
+    def _batch_smart_stage(self, acq, space, tops, random_state):
+        """Per path (x_s, min_s) of DeviceHooks._smart_minimize from that path's seeds: continuous spaces run every
+        path's L-BFGS-B runs in one lockstep; mixed-integer spaces run the reference's branch path by path."""
+        q = acq.n_paths
+        if not all(space.continuous_dimensions):
+            return [self._smart_minimize(acq.path(p), space, tops[p], random_state) for p in range(q)]
+        seeds = [s for p in range(q) for s in tops[p]]
+        owner = [p for p in range(q) for _ in tops[p]]
+        runs = lockstep_lbfgsb(acq, seeds, space.bounds, run_paths=owner) if seeds else []
+        out = []
+        for p in range(q):
+            ok = [r for r, o in zip(runs, owner) if o == p and r.success]
+            if not ok:
+                out.append((np.full(space.bounds.shape[0], np.nan), np.inf))
+                continue
+            best = min(ok, key=lambda r: float(np.squeeze(r.fun)))  # first of equal minima, like the loop
+            out.append((np.clip(best.x, space.bounds[:, 0], space.bounds[:, 1]), np.squeeze(best.fun)))
+        return out
 
     def get_acquisition_params(self):
         return {"n_features": self.n_features}
@@ -223,16 +306,53 @@ class ConstrainedThompsonSampling(ThompsonSampling):
     def _get_acq(self, gp, constraint=None):
         if constraint is None:
             return super()._get_acq(gp, constraint=None)
-        from .paths import ConstrainedPaths, PathAcquisition
+        from .paths import ConstrainedPaths
 
         gp = _as_b200_gp(gp)
         models = [_as_b200_gp(m) for m in constraint.model]  # before any draw: a refusal consumes no random numbers
         if len(models) + 1 > B.MAX_GPS:
             raise NotImplementedError(f"at most {B.MAX_GPS - 1} constraint GPs are supported")
         rs = self._suggest_rng()
-        target = gp.sample_paths(1, self.n_features, random_state=rs)
-        paths = [m.sample_paths(1, self.n_features, random_state=rs) for m in models]
-        return PathAcquisition(ConstrainedPaths(target, paths, constraint.lb, constraint.ub))
+        q = self._batch_q or 1
+        target = gp.sample_paths(q, self.n_features, random_state=rs)
+        paths = [m.sample_paths(q, self.n_features, random_state=rs) for m in models]
+        return self._closure(ConstrainedPaths(target, paths, constraint.lb, constraint.ub))
+
+
+def distinct_picks(picks, tops):
+    """The duplicate rule of batch Thompson sampling: in path order p = 0..q-1, a pick bit-equal to an earlier pick is
+    replaced by the first row of tops[p] (path p's top-k, best first) that is bit-equal to no pick so far; with none
+    left the duplicate stays.  Late in a run several paths can share their random-stage winner."""
+    out, taken = [], set()
+    for p, x in enumerate(picks):
+        x = np.asarray(x, dtype=np.float64)
+        if x.tobytes() in taken:
+            for t in tops[p]:
+                t = np.asarray(t, dtype=np.float64)
+                if t.tobytes() not in taken:
+                    x = t
+                    break
+        out.append(x)
+        taken.add(x.tobytes())
+    return out
+
+
+def suggest_batch(optimizer, q):
+    """q parameter dicts to probe next from a ``bayes_opt.BayesianOptimization`` whose acquisition function is a
+    (Constrained)ThompsonSampling: ``BayesianOptimization.suggest`` for a batch (R/bayes_opt/bayesian_optimization.py:
+    323-333).  With no registered point it returns ``optimizer.random_sample(q)``; otherwise
+    ``ThompsonSampling.suggest_batch`` with the optimizer's GP, target space and RandomState, each row converted with
+    ``array_to_params``.  Nothing new enters ``save_state``: q is an argument, not state."""
+    acq = optimizer._acquisition_function
+    if not isinstance(acq, ThompsonSampling):
+        raise TypeError(f"suggest_batch needs a ThompsonSampling or ConstrainedThompsonSampling acquisition function, "
+                        f"got {type(acq).__name__}; for a batch of other acquisition functions use ConstantLiar")
+    q = _check_int("q", q, 1, B.MAX_PATHS)
+    space = optimizer._space
+    if len(space) == 0:
+        return optimizer.random_sample(q)
+    X = acq.suggest_batch(gp=optimizer._gp, target_space=space, q=q, fit_gp=True, random_state=optimizer._random_state)
+    return [space.array_to_params(x) for x in X]
 
 
 # Default size of the candidate set over which the maxima of the MES sample paths are taken (DESIGN.md 4.8).

@@ -1844,6 +1844,7 @@ struct b200bo_paths {
     std::vector<double> bound;  // (q,) B_p >= |path_p(x)| everywhere (b200bo_paths_bound)
     DevBuf Xs, V, omega, bias, W, ls, xf, xc, out, sel_cta, sel, pbounds, prow, bad;
     DevBuf cvals, cmerit, craw;  // constrained calls with this handle as set 0: [G][chunk][q] values, outputs
+    DevBuf pidx;                 // row-mode calls: (m,) path index per row
     ChunkedUpload upload;
 };
 
@@ -1860,6 +1861,13 @@ static PathsKernel paths_kernel(int cov, int q) {
     };
     const int qt = paths_qt(q);
     return tab[cov][qt == 1 ? 0 : (qt == 4 ? 1 : 2)];
+}
+
+// row mode (b200bo_paths_eval_rows): one sum per candidate whatever q
+static PathsKernel paths_rows_kernel(int cov) {
+    static const PathsKernel tab[4] = {paths_eval_kernel<0, 1, true>, paths_eval_kernel<1, 1, true>,
+                                       paths_eval_kernel<2, 1, true>, paths_eval_kernel<3, 1, true>};
+    return tab[cov];
 }
 
 static PathsParams paths_params(const b200bo_paths* ps) {
@@ -1893,7 +1901,8 @@ static int paths_grid(const b200bo_paths* ps, int64_t m) {
 static int paths_launch(const b200bo_paths* ps, const PathsParams& P, int grid, cudaStream_t st) {
     if (grid <= 0) return B200BO_OK;
     void* args[] = {(void*)&P};
-    CU(cudaLaunchKernel((const void*)paths_kernel(ps->cov, P.q), dim3(grid), dim3(PT_NT), args,
+    const PathsKernel fn = P.path_idx ? paths_rows_kernel(ps->cov) : paths_kernel(ps->cov, P.q);
+    CU(cudaLaunchKernel((const void*)fn, dim3(grid), dim3(PT_NT), args,
                         paths_smem_bytes(P.d, P.q, P.sel_cta != nullptr), st));
     LAUNCHED();
     return B200BO_OK;
@@ -1944,7 +1953,10 @@ static int paths_setup(b200bo_gp* gp, b200bo_paths* ps, const double* omega, con
     // a smaller path never lowers the limit below what a path drawn earlier launches with.
     CU(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)paths_smem_bytes(B200BO_MAX_DIM, paths_qt(q), true)));
-    CU(cudaFuncSetAttribute(cpaths_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    // the row-mode instantiation stages all q columns of V / W: its limit covers q = B200BO_MAX_PATHS
+    CU(cudaFuncSetAttribute((const void*)paths_rows_kernel(ps->cov), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)paths_smem_bytes(B200BO_MAX_DIM, B200BO_MAX_PATHS, false)));
+    CU(cudaFuncSetAttribute(cpaths_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)cpaths_smem_bytes(B200BO_MAX_PATHS)));
     const size_t smem = paths_smem_bytes(d, q, true);
     int bps = 0;
@@ -2055,7 +2067,7 @@ extern "C" void b200bo_paths_destroy(b200bo_paths* ps) {
     cudaSetDevice(ps->device);
     DevBuf* bufs[] = {&ps->Xs, &ps->V, &ps->omega, &ps->bias, &ps->W, &ps->ls, &ps->xf, &ps->xc,
                       &ps->out, &ps->sel_cta, &ps->sel, &ps->pbounds, &ps->prow, &ps->bad,
-                      &ps->cvals, &ps->cmerit, &ps->craw};
+                      &ps->cvals, &ps->cmerit, &ps->craw, &ps->pidx};
     for (DevBuf* b : bufs) b->release();
     ps->upload.release();
     delete ps;
@@ -2077,6 +2089,39 @@ extern "C" int b200bo_paths_eval(b200bo_paths* ps, const double* Xc, int64_t m, 
     P.out = ps->out.as<double>();
     if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
     CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m * ps->q, cudaMemcpyDeviceToHost));
+    return paths_check_nonfinite(ps);
+}
+
+// path_idx (m,) host: every entry in [0, q), then copied into dst->pidx
+static int paths_upload_rows(b200bo_paths* dst, int q, const int* path_idx, int64_t m) {
+    for (int64_t i = 0; i < m; ++i)
+        if (path_idx[i] < 0 || path_idx[i] >= q)
+            return set_err(B200BO_ERR_ARG, "path_idx[%lld]=%d out of range [0,%d)", (long long)i, path_idx[i], q);
+    int rc;
+    if ((rc = dst->pidx.reserve(sizeof(int) * (size_t)m))) return rc;
+    CU(cudaMemcpy(dst->pidx.p, path_idx, sizeof(int) * (size_t)m, cudaMemcpyHostToDevice));
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_paths_eval_rows(b200bo_paths* ps, const double* Xc, const int* path_idx, int64_t m,
+                                      double* out) {
+    if (!ps || m < 0 || (m > 0 && (!Xc || !path_idx || !out))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_eval_rows");
+    int rc;
+    if ((rc = paths_upload_rows(ps, ps->q, path_idx, m))) return rc;
+    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * ps->d))) return rc;
+    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m))) return rc;
+    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * ps->d, cudaMemcpyHostToDevice));
+    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
+    PathsParams P = paths_params(ps);
+    P.Xc = ps->xc.as<double>();
+    P.m = m;
+    P.out = ps->out.as<double>();
+    P.path_idx = ps->pidx.as<int>();
+    if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
+    CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost));
     return paths_check_nonfinite(ps);
 }
 
@@ -2225,11 +2270,12 @@ static int cpaths_check(b200bo_paths* const* sets, int G, const double* lb, cons
 
 // Xc: host rows, streamed through set 0's ChunkedUpload; nullptr: the Philox source of set 0's pbounds and `seed`,
 // generated chunk by chunk.  k > 0: -g folded into the per-path lists (merged into set 0's sel); merit / raw (host,
-// nullable): the (m,q) merit and the (m,G,q) values.  Returns with the work finished and the inputs checked.
+// nullable): the (m,q) merit and the (m,G,q) values.  pidx (device, (m,), nullable): row mode - merit is (m,), row i
+// on path pidx[i] only (host rows, k = 0, no raw).  Returns with the work finished and the inputs checked.
 static int cpaths_run(b200bo_paths* const* sets, CPathsParams& C, const double* Xc, uint64_t seed, int64_t m,
-                      int64_t index_base, int k, double* merit, double* raw) {
+                      int64_t index_base, int k, double* merit, double* raw, const int* pidx = nullptr) {
     b200bo_paths* s0 = sets[0];
-    const int G = C.G, q = C.q, d = s0->d;
+    const int G = C.G, q = pidx ? 1 : C.q, d = s0->d;  // q: values per row
     const long long chunk = kChunkTilesPerSm * PBN * s0->sm_count;
     const bool one = m <= chunk;
     const long long cm = one ? m : chunk;
@@ -2262,12 +2308,18 @@ static int cpaths_run(b200bo_paths* const* sets, CPathsParams& C, const double* 
             P.m = mc;
             P.clamp_count = s0->bad.as<unsigned long long>();
             P.out = s0->cvals.as<double>() + (size_t)g * cm * q;
+            P.path_idx = pidx ? pidx + c0 : nullptr;
             if ((r = paths_launch(sets[g], P, paths_grid(sets[g], mc), U.exec))) return r;
         }
         C.m = mc;
         C.index_base = index_base + c0;
         C.sel_resume = i > 0;
-        cpaths_select_kernel<<<sgrid, CP_NT, cpaths_smem_bytes(k > 0 ? q : 0), U.exec>>>(C);
+        if (pidx) {
+            C.path_idx = pidx + c0;
+            cpaths_select_kernel<true><<<sgrid, CP_NT, 0, U.exec>>>(C);
+        } else {
+            cpaths_select_kernel<<<sgrid, CP_NT, cpaths_smem_bytes(k > 0 ? q : 0), U.exec>>>(C);
+        }
         LAUNCHED();
         CU(cudaGetLastError());
         // pageable host memory: each copy returns once it is done, in stream order behind the kernels
@@ -2305,6 +2357,19 @@ extern "C" int b200bo_cpaths_eval(b200bo_paths* const* sets, int G, const double
     CU(cudaSetDevice(sets[0]->device));
     NvtxRange nvtx_range("b200bo:cpaths_eval");
     return cpaths_run(sets, C, Xc, 0, m, 0, 0, merit, raw);
+}
+
+extern "C" int b200bo_cpaths_eval_rows(b200bo_paths* const* sets, int G, const double* lb, const double* ub,
+                                       const double* Xc, const int* path_idx, int64_t m, double* merit) {
+    CPathsParams C;
+    int rc;
+    if ((rc = cpaths_check(sets, G, lb, ub, C))) return rc;
+    if (m < 0 || (m > 0 && (!Xc || !path_idx || !merit))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    CU(cudaSetDevice(sets[0]->device));
+    NvtxRange nvtx_range("b200bo:cpaths_eval_rows");
+    if ((rc = paths_upload_rows(sets[0], C.q, path_idx, m))) return rc;
+    return cpaths_run(sets, C, Xc, 0, m, 0, 0, merit, nullptr, sets[0]->pidx.as<int>());
 }
 
 extern "C" int b200bo_cpaths_argmin_topk(b200bo_paths* const* sets, int G, const double* lb, const double* ub,

@@ -43,8 +43,9 @@ struct PathsParams {
     long long index_base;     // global index of this launch's candidate 0
     long long m;
     unsigned long long* clamp_count;  // [1]: non-finite candidate coordinates (slot [0] unused)
-    double* out;              // [m][q] or nullptr
+    double* out;              // [m][q] ([m] with path_idx) or nullptr
     SelList* sel_cta;         // [q][gridDim.x] per-CTA running selections, or nullptr
+    const int* path_idx;      // [m]: row mode (ROWS instantiation) - row i on path path_idx[i] only
 };
 
 // dynamic shared memory: 2 stage buffers [64][d + q + 1] | xc [d][128] | red [2][q][128] | SelShared [q]
@@ -56,17 +57,23 @@ __host__ __device__ inline size_t paths_smem_bytes(int d, int q, bool sel) {
 // QT: register slots of the q sums (1, 4 or 16).  QT = 1, 4: 2 CTAs per SM (<= 128 registers, no spills).  QT = 16:
 // one CTA per SM and 176 registers - at 128 it spilled, and on an H100 (400 W) it took 147 ms instead of 127 ms for
 // 16 paths x 2^20 candidates at C3.
-template <int COV, int QT>
+// ROWS (with QT = 1): row mode of the batched refinement - candidate i keeps the one sum of path P.path_idx[i] and
+// writes out[i].  The stage still holds all q columns of V / W; only the column a candidate reads changes.  Its
+// sums take the same operations in the same order as column path_idx[i] of the full evaluation, so the values
+// are bit-equal to it.
+template <int COV, int QT, bool ROWS = false>
 __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(const PathsParams P) {
+    static_assert(!ROWS || QT == 1, "row mode keeps one sum per candidate");
     extern __shared__ __align__(16) double smem[];
     const int tid = threadIdx.x, d = P.d, q = P.q;
+    const int qs = ROWS ? 1 : q;  // sums per candidate
     const int c = tid & (PBN - 1), half = tid >> 7;
     const int bufsz = PT_CHUNK * (d + q + 1);
     double* stage = smem;
     double* xc_s = smem + 2 * bufsz;                // [d][PBN]
     double* red = xc_s + (size_t)d * PBN;           // [2][q][PBN]
     SelShared* sel = reinterpret_cast<SelShared*>(red + (size_t)2 * q * PBN);
-    if (P.sel_cta) {
+    if (!ROWS && P.sel_cta) {
         if (tid < PBN)
             for (int p = 0; p < q; ++p)
                 runsel_begin(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, P.sel_resume, tid);
@@ -87,6 +94,8 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
             }
             xc_s[j * PBN + cc] = v;
         }
+        int pc = 0;  // ROWS: the column of V / W this thread's candidate reads
+        if (ROWS && c0 + c < P.m) pc = P.path_idx[c0 + c];
         double ak[QT], af[QT];
 #pragma unroll
         for (int p = 0; p < QT; ++p) ak[p] = af[p] = 0.0;
@@ -139,13 +148,13 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
                             const double phi = cos(s[t] + ph[r]);
 #pragma unroll
                             for (int p = 0; p < QT; ++p)
-                                if (p < q) af[p] = fma(b[r * q + p], phi, af[p]);
+                                if (p < qs) af[p] = fma(b[r * q + pc + p], phi, af[p]);
                         } else {
                             double kv = P.constv * cov_eval<COV>(s[t]);
                             if (ch * PT_CHUNK + r >= P.n) kv = 0.0;
 #pragma unroll
                             for (int p = 0; p < QT; ++p)
-                                if (p < q) ak[p] = fma(b[r * q + p], kv, ak[p]);
+                                if (p < qs) ak[p] = fma(b[r * q + pc + p], kv, ak[p]);
                         }
                     }
                 }
@@ -157,7 +166,7 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
         if (half == 1) {
 #pragma unroll
             for (int p = 0; p < QT; ++p)
-                if (p < q) {
+                if (p < qs) {
                     red[p * PBN + c] = ak[p];
                     red[(q + p) * PBN + c] = af[p];
                 }
@@ -168,18 +177,18 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
             const bool valid = gi < P.m;
 #pragma unroll
             for (int p = 0; p < QT; ++p) {
-                if (p < q) {
+                if (p < qs) {
                     const double kp = ak[p] + red[p * PBN + c];
                     const double fp = af[p] + red[(q + p) * PBN + c];
                     const double f = P.y_std * fma(P.feat_scale, fp, kp) + P.y_mean;
-                    if (P.out && valid) P.out[gi * q + p] = f;
-                    if (P.sel_cta) runsel_update<1>(sel[p], P.sel_k, tid, -f, gi + P.index_base, valid);
+                    if (P.out && valid) P.out[gi * qs + p] = f;
+                    if (!ROWS && P.sel_cta) runsel_update<1>(sel[p], P.sel_k, tid, -f, gi + P.index_base, valid);
                 }
             }
         }
         __syncthreads();  // xc_s / red reused by the next tile
     }
-    if (P.sel_cta && tid < PBN)
+    if (!ROWS && P.sel_cta && tid < PBN)
         for (int p = 0; p < q; ++p) runsel_store(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, tid);
 }
 
@@ -205,20 +214,24 @@ struct CPathsParams {
     int G, q, sel_k, sel_resume;
     double lb[B200BO_MAX_GPS], ub[B200BO_MAX_GPS];  // [j], j >= 1
     double T[B200BO_MAX_PATHS];
-    double* merit;      // [m][q] or nullptr
-    double* raw;        // [m][G][q] or nullptr
-    SelList* sel_cta;   // [q][gridDim.x] or nullptr
+    double* merit;      // [m][q] ([m] in row mode) or nullptr
+    double* raw;        // [m][G][q] or nullptr (not in row mode)
+    SelList* sel_cta;   // [q][gridDim.x] or nullptr (not in row mode)
+    const int* path_idx;  // [m]: row mode - vals [G][stride] hold row i's path path_idx[i] only
 };
 
 __host__ __device__ inline size_t cpaths_smem_bytes(int q) { return sizeof(SelShared) * (size_t)q; }
 
 __device__ __forceinline__ double cp_pos(double x) { return (x > 0.0 || x != x) ? x : 0.0; }
 
+// ROWS: the merit of row i on path P.path_idx[i] only, from the values the ROWS paths_eval_kernel left; the same
+// operations as column path_idx[i] of the full combine.
+template <bool ROWS = false>
 __global__ void __launch_bounds__(CP_NT) cpaths_select_kernel(const CPathsParams P) {
     extern __shared__ __align__(16) unsigned char cp_smem[];
     SelShared* sel = reinterpret_cast<SelShared*>(cp_smem);
     __shared__ double lb_s[B200BO_MAX_GPS], ub_s[B200BO_MAX_GPS], T_s[B200BO_MAX_PATHS];
-    const int t = threadIdx.x, q = P.q, G = P.G;
+    const int t = threadIdx.x, q = ROWS ? 1 : P.q, G = P.G;
     if (t == 0) {  // constant indices: the parameter arrays stay in the constant bank
 #pragma unroll
         for (int j = 0; j < B200BO_MAX_GPS; ++j) {
@@ -228,7 +241,7 @@ __global__ void __launch_bounds__(CP_NT) cpaths_select_kernel(const CPathsParams
 #pragma unroll
         for (int p = 0; p < B200BO_MAX_PATHS; ++p) T_s[p] = P.T[p];
     }
-    if (P.sel_cta)
+    if (!ROWS && P.sel_cta)
         for (int p = 0; p < q; ++p) runsel_begin(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, P.sel_resume, t);
     __syncthreads();
     const long long ntiles = (P.m + CP_NT - 1) / CP_NT;
@@ -245,14 +258,15 @@ __global__ void __launch_bounds__(CP_NT) cpaths_select_kernel(const CPathsParams
                     viol = __dadd_rn(viol, __dadd_rn(cp_pos(__dsub_rn(lb_s[j], c)), cp_pos(__dsub_rn(c, ub_s[j]))));
                     if (P.raw) P.raw[((size_t)gi * G + j) * q + p] = c;
                 }
-                g = viol == 0.0 ? f : __dmul_rn(-T_s[p], __dadd_rn(1.0, viol));
+                const int pt = ROWS ? P.path_idx[gi] : p;  // the path whose T applies
+                g = viol == 0.0 ? f : __dmul_rn(-T_s[pt], __dadd_rn(1.0, viol));
                 if (P.raw) P.raw[(size_t)gi * G * q + p] = f;
                 if (P.merit) P.merit[gi * q + p] = g;
             }
-            if (P.sel_cta) runsel_update<1>(sel[p], P.sel_k, t, -g, gi + P.index_base, valid);
+            if (!ROWS && P.sel_cta) runsel_update<1>(sel[p], P.sel_k, t, -g, gi + P.index_base, valid);
         }
     }
-    if (P.sel_cta)
+    if (!ROWS && P.sel_cta)
         for (int p = 0; p < q; ++p) runsel_store(sel[p], P.sel_cta + (size_t)p * gridDim.x + blockIdx.x, t);
 }
 

@@ -319,25 +319,30 @@ class _LockstepEvaluator:
     else is in the batch, so each run sees exactly the values it would see alone.  With several devices
     run r's rows go to device r mod G (SURVEY.md 8e)."""
 
-    def __init__(self, acq, n_active):
+    def __init__(self, acq, n_active, run_paths=None):
         self.acq = acq
         self.cv = threading.Condition()
         self.pending, self.results = {}, {}
         self.active = n_active
         self.error = None
         self.n_dev = len(getattr(acq, "devices", [0]))
+        self.run_paths = run_paths
 
     def _flush(self):
         keys = sorted(self.pending, key=lambda k: (k % self.n_dev, k)) if self.n_dev > 1 else list(self.pending)
         xs = [self.pending[k] for k in keys]
+        kw = {}
+        if self.run_paths is not None:
+            kw["path_idx"] = np.concatenate([np.full(len(x), self.run_paths[k], dtype=np.int32)
+                                             for k, x in zip(keys, xs)])
         try:
             if self.n_dev > 1:
                 counts = np.zeros(self.n_dev + 1, dtype=np.int64)
                 for k, x in zip(keys, xs):
                     counts[(k % self.n_dev) + 1] += len(x)
-                ys = np.asarray(self.acq(np.vstack(xs), shard_offsets=np.cumsum(counts)), dtype=float)
+                ys = np.asarray(self.acq(np.vstack(xs), shard_offsets=np.cumsum(counts), **kw), dtype=float)
             else:
-                ys = np.asarray(self.acq(np.vstack(xs)), dtype=float)
+                ys = np.asarray(self.acq(np.vstack(xs), **kw), dtype=float)
             off = 0
             for k, x in zip(keys, xs):
                 self.results[k] = ys[off:off + len(x)]
@@ -368,7 +373,7 @@ class _LockstepEvaluator:
 
 
 def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, gtol=1e-5, eps=1e-8,
-                    maxfun=15000, maxiter=15000, maxls=20):
+                    maxfun=15000, maxiter=15000, maxls=20, run_paths=None):
     """All L-BFGS-B runs of ``_smart_minimize`` advanced TOGETHER by one Python thread around SciPy's own
     compiled core (``scipy.optimize._lbfgsb.setulb``): the driver loop of ``_minimize_lbfgsb``
     (SP/optimize/_lbfgsb_py.py:290-420: task handling, iteration / evaluation limits, warnflag -> success) and the
@@ -409,6 +414,7 @@ def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, 
     for k, s in enumerate(seeds):
         r = Run()
         r.dev = k % n_dev  # SURVEY.md 8e: seed r -> GPU r mod G
+        r.path = None if run_paths is None else int(run_paths[k])
         r.x = np.array(np.clip(np.asarray(s, dtype=np.float64).ravel(), lb, ub), dtype=np.float64)
         r.f = np.array(0.0, dtype=np.float64)
         r.g = np.zeros(n, dtype=np.float64)
@@ -434,13 +440,16 @@ def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, 
             pts = _predicted_stencil(x0, lb, ub, eps)
             blocks.append((x0, pts))
         rows = np.vstack([np.vstack([x0[None, :], pts]) for x0, pts in blocks])
+        kw = {}
+        if run_paths is not None:
+            kw["path_idx"] = np.repeat(np.array([r.path for r in pending], dtype=np.int32), 1 + n)
         if n_dev > 1:
             counts = np.zeros(n_dev + 1, dtype=np.int64)
             for r in pending:
                 counts[r.dev + 1] += 1 + n
-            ys = np.asarray(acq(rows, shard_offsets=np.cumsum(counts)), dtype=np.float64)
+            ys = np.asarray(acq(rows, shard_offsets=np.cumsum(counts), **kw), dtype=np.float64)
         else:
-            ys = np.asarray(acq(rows), dtype=np.float64)
+            ys = np.asarray(acq(rows, **kw), dtype=np.float64)
         off = 0
         for r, (x0, pts) in zip(pending, blocks):
             f0 = float(ys[off])
@@ -493,26 +502,42 @@ def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, 
     return out
 
 
-def lockstep_lbfgsb(acq, x_seeds, bounds, lockstep=True):
+def _on_path(acq, p, dim):
+    """The objective of a run of path p over a closure ``acq(rows, path_idx)``."""
+
+    def fun(x):
+        rows = np.asarray(x, dtype=np.float64).reshape(-1, dim)
+        return acq(rows, path_idx=np.full(rows.shape[0], p, dtype=np.int32))
+
+    return fun
+
+
+def lockstep_lbfgsb(acq, x_seeds, bounds, lockstep=True, run_paths=None):
     """``[minimize(acq, seed, bounds=bounds, method="L-BFGS-B") for seed in x_seeds]`` (the loop at
     R/bayes_opt/acquisition.py:365-366) with the runs advanced in lockstep.  B200BO_LOCKSTEP=0 (or a
-    single seed) selects the plain sequential loop."""
+    single seed) selects the plain sequential loop.
+
+    run_paths: None, or one path index per seed for a closure ``acq(rows, path_idx)`` over several sample paths
+    (paths.PathBatchAcquisition): run r minimises path run_paths[r], and every merged call passes the path of each
+    of its rows."""
     seeds = [np.asarray(s, dtype=float) for s in x_seeds]
+    dim = np.asarray(bounds).shape[0]
+    fun = [acq if run_paths is None else _on_path(acq, int(run_paths[i]), dim) for i in range(len(seeds))]
     if len(seeds) <= 1 or not lockstep or os.environ.get("B200BO_LOCKSTEP", "1") == "0":
         out = []
-        for s in seeds:
+        for s, f in zip(seeds, fun):
             if lockstep:
-                obj = _FusedObjective(lambda rows: np.asarray(acq(rows), dtype=float), bounds)
+                obj = _FusedObjective(lambda rows, f=f: np.asarray(f(rows), dtype=float), bounds)
                 out.append(minimize(obj.fun, s, bounds=bounds, method="L-BFGS-B", options=obj.options()))
             else:
-                out.append(minimize(acq, s, bounds=bounds, method="L-BFGS-B"))
+                out.append(minimize(f, s, bounds=bounds, method="L-BFGS-B"))
         return out
     if _workers_supported() and os.environ.get("B200BO_LBFGSB_DRIVER", "batched") == "batched":
         try:
-            return _batched_lbfgsb(acq, seeds, bounds)
+            return _batched_lbfgsb(acq, seeds, bounds, run_paths=run_paths)
         except (ImportError, AttributeError, KeyError, TypeError):
             pass  # SciPy's private L-BFGS-B pieces differ from the ones the batched driver restates: thread driver
-    ev = _LockstepEvaluator(acq, len(seeds))
+    ev = _LockstepEvaluator(acq, len(seeds), run_paths=run_paths)
     results, errors = [None] * len(seeds), [None] * len(seeds)
 
     def run(i):

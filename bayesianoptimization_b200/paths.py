@@ -51,6 +51,18 @@ def draw_path_inputs(rs, n_paths, n_features, d, nu, n, noise_var):
     return omega, b, w, eps
 
 
+def _row_paths(path_idx, m, q):
+    """path_idx as the (m,) int32 array of the C ABI.  Values are clipped to [-1, q] only so that the narrowing
+    cannot wrap: an index outside [0, q) stays outside and the ABI rejects it."""
+    pidx = np.asarray(path_idx)
+    if pidx.dtype.kind not in "iu":
+        raise ValueError(f"path_idx must be integers, got dtype {pidx.dtype}")
+    pidx = pidx.reshape(-1)
+    if pidx.shape[0] != m:
+        raise ValueError(f"path_idx has {pidx.shape[0]} entries for {m} rows")
+    return np.ascontiguousarray(np.where(pidx < 0, -1, np.minimum(pidx, q)), dtype=np.int32)
+
+
 class _PathsHandle:
     """Owns one b200bo_paths*."""
 
@@ -112,6 +124,16 @@ class PosteriorPaths:
         X = self._candidates(X)
         out = np.empty((X.shape[0], self.n_paths))
         B.check(B.lib().b200bo_paths_eval(self._handle.ptr, B.as_dp(X), X.shape[0], B.as_dp(out)))
+        return out
+
+    def eval_rows(self, X, path_idx):
+        """(M,) values: row i of X on path path_idx[i] only, bit-equal to ``self(X)[i, path_idx[i]]`` at 1/q of its
+        cost.  An index outside [0, q) raises ValueError."""
+        X = self._candidates(X)
+        pidx = _row_paths(path_idx, X.shape[0], self.n_paths)
+        out = np.empty(X.shape[0])
+        B.check(B.lib().b200bo_paths_eval_rows(self._handle.ptr, B.as_dp(X), pidx.ctypes.data_as(C.POINTER(C.c_int32)),
+                                               X.shape[0], B.as_dp(out)))
         return out
 
     def argmin_topk(self, X, k):
@@ -227,6 +249,15 @@ class ConstrainedPaths:
         """(M, G, q) path values at the rows of X: [:, 0] the target's, [:, j] constraint set j's (data units)."""
         return self._eval(X, raw=True)
 
+    def eval_rows(self, X, path_idx):
+        """(M,) merit: row i of X on path path_idx[i] only, bit-equal to ``self(X)[i, path_idx[i]]``."""
+        X = self._candidates(X)
+        pidx = _row_paths(path_idx, X.shape[0], self.n_paths)
+        out = np.empty(X.shape[0])
+        B.check(B.lib().b200bo_cpaths_eval_rows(*self._args(), B.as_dp(X), pidx.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                X.shape[0], B.as_dp(out)))
+        return out
+
     def argmin_topk(self, X, k):
         """Per path p: np.argmin and the k smallest (np.argsort order) of -merit_p over the rows of X.
         Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
@@ -279,3 +310,27 @@ class PathAcquisition:
     def argmin_topk_philox(self, seed, bounds, m, k, index_base=0):
         idx, val, bx, ti, tx = self.paths.argmin_topk_philox(seed, bounds, m, k, index_base)
         return int(idx[0]), float(val[0]), bx[0], ti[0], tx[0]
+
+
+class PathBatchAcquisition:
+    """Closure over ALL q paths of a PosteriorPaths / ConstrainedPaths, for batch Thompson sampling
+    (``ThompsonSampling.suggest_batch``): ``acq(x, path_idx)`` -> (M,) values of -path_{path_idx[i]}(x_i), one device
+    call whatever mix of paths the rows belong to (the lockstep refinement of q x n_smart runs).  ``path(p)`` is the
+    single-path closure x -> -path_p(x) with the same values."""
+
+    def __init__(self, paths):
+        self.paths = paths
+        self.devices = paths.devices
+        self.n_paths = paths.n_paths
+
+    def __call__(self, x, path_idx):
+        return -self.paths.eval_rows(x, path_idx)
+
+    def path(self, p):
+        p, dim = int(p), self.paths.dim
+
+        def acq(x):
+            x = np.asarray(x, dtype=np.float64).reshape(-1, dim)
+            return self(x, np.full(x.shape[0], p, dtype=np.int32))
+
+        return acq

@@ -293,6 +293,10 @@ void b200bo_paths_destroy(b200bo_paths* paths);
 /* out: (m,q) host, path values at the rows of Xc (m,d) host, in data units.  A row's value depends on its
  * coordinates only (not on m, its position or the launch geometry). */
 int b200bo_paths_eval(b200bo_paths* paths, const double* Xc, int64_t m, double* out);
+/* Row mode of the batched refinement (one L-BFGS-B run per path): out: (m,) host, out[i] = path path_idx[i] at row i,
+ * bit-equal to column path_idx[i] of b200bo_paths_eval on that row.  path_idx: (m,) host, every entry in [0, q), else
+ * B200BO_ERR_ARG.  Costs one path per row instead of q. */
+int b200bo_paths_eval_rows(b200bo_paths* paths, const double* Xc, const int* path_idx, int64_t m, double* out);
 /* Per path p, ranks -path_p on the rows of Xc with the semantics of b200bo_acq_argmin_topk: best_val[p], best_idx[p]
  * (np.argmin), topk_val[p*k + i], topk_idx[p*k + i] (np.argsort order).  Large batches are streamed in chunks. */
 int b200bo_paths_argmin_topk(b200bo_paths* paths, const double* Xc, int64_t m, int k, double* best_val,
@@ -321,6 +325,10 @@ int b200bo_paths_bound(const b200bo_paths* paths, double* bound);
 /* merit: (m,q) host; raw: (m,G,q) host or NULL - raw[i][g][p] = path p of sets[g] at row i. */
 int b200bo_cpaths_eval(b200bo_paths* const* sets, int G, const double* lb, const double* ub, const double* Xc,
                        int64_t m, double* merit, double* raw);
+/* merit: (m,) host, merit[i] = merit of path path_idx[i] at row i, bit-equal to column path_idx[i] of
+ * b200bo_cpaths_eval.  path_idx: (m,) host, every entry in [0, q), else B200BO_ERR_ARG. */
+int b200bo_cpaths_eval_rows(b200bo_paths* const* sets, int G, const double* lb, const double* ub, const double* Xc,
+                            const int* path_idx, int64_t m, double* merit);
 int b200bo_cpaths_argmin_topk(b200bo_paths* const* sets, int G, const double* lb, const double* ub, const double* Xc,
                               int64_t m, int k, double* best_val, int64_t* best_idx, double* topk_val,
                               int64_t* topk_idx);
