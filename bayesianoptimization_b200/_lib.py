@@ -33,6 +33,7 @@ EXPORTS = [
     "b200bo_paths_create", "b200bo_paths_destroy", "b200bo_paths_eval", "b200bo_paths_argmin_topk",
     "b200bo_paths_argmin_topk_philox", "b200bo_paths_bound", "b200bo_cpaths_eval", "b200bo_cpaths_argmin_topk",
     "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
+    "b200bo_acq_value_grad", "b200bo_paths_grad_rows",
 ]
 
 
@@ -97,6 +98,7 @@ def lib():
     L.b200bo_gp_predict.argtypes = [C.c_void_p, dp, C.c_int64, dp, dp, i64p]
     L.b200bo_gp_predict_cov.argtypes = [C.c_void_p, dp, C.c_int64, dp, dp]
     L.b200bo_acq_eval.argtypes = [C.POINTER(AcqSpec), dp, C.c_int64, dp]
+    L.b200bo_acq_value_grad.argtypes = [C.POINTER(AcqSpec), dp, C.c_int64, dp, dp]
     L.b200bo_acq_argmin_topk.argtypes = [C.POINTER(AcqSpec), dp, C.c_int64, C.c_int, dp, i64p, dp,
                                          i64p, dp]
     L.b200bo_acq_eval_dev.argtypes = [C.POINTER(AcqSpec), C.c_void_p, C.c_int64, C.c_void_p,
@@ -123,6 +125,7 @@ def lib():
     L.b200bo_paths_destroy.restype = None
     L.b200bo_paths_eval.argtypes = [C.c_void_p, dp, C.c_int64, dp]
     L.b200bo_paths_eval_rows.argtypes = [C.c_void_p, dp, C.POINTER(C.c_int32), C.c_int64, dp]
+    L.b200bo_paths_grad_rows.argtypes = [C.c_void_p, dp, C.POINTER(C.c_int32), C.c_int64, dp, dp]
     L.b200bo_paths_argmin_topk.argtypes = [C.c_void_p, dp, C.c_int64, C.c_int, dp, i64p, dp, i64p]
     L.b200bo_paths_argmin_topk_philox.argtypes = [C.c_void_p, C.c_uint64, dp, dp, C.c_int64, C.c_int64, C.c_int,
                                                   *philox_outs]

@@ -74,6 +74,12 @@ def _device_closure(acq):
     return callable(getattr(acq, "argmin_topk", None)) and callable(getattr(acq, "argmin_topk_philox", None))
 
 
+def _offers_grad(acq):
+    """True for device closures with an analytic gradient: ``value_and_grad(x[, path_idx]) -> (values, gradients)``
+    on one device (FusedAcquisition, the closures over unconstrained sample paths)."""
+    return callable(getattr(acq, "value_and_grad", None)) and len(getattr(acq, "devices", [0])) == 1
+
+
 class DeviceHooks(abc.ABC):
     """Mixin: the three hooks of the acquisition seam on the GPU.  Must precede the reference class in
     the MRO.  (Derives from abc.ABC like bayes_opt's AcquisitionFunction so that both have the same
@@ -93,6 +99,15 @@ class DeviceHooks(abc.ABC):
     # ONE 64-bit seed is drawn from the caller's RandomState per call).  Set by enable(candidate_source=...).
     b200_candidate_source = "host_rng"
 
+    # "stencil": the L-BFGS-B refinement differentiates the closure by SciPy's 2-point scheme, d + 1 rows per
+    # evaluation (parity with the reference); "analytic": it takes the gradient from the device, one row per
+    # evaluation (continuous spaces, closures that offer value_and_grad; anything else stays on the stencil).
+    # Set by enable(refine=...).
+    b200_refine = "stencil"
+
+    def _refine_grad(self, acq, space):
+        return self.b200_refine == "analytic" and all(space.continuous_dimensions) and _offers_grad(acq)
+
     def _random_sample_minimize(self, acq, space, random_state, n_random, n_x_seeds=0):
         if n_random == 0 or not _device_closure(acq) or n_x_seeds > B.MAX_TOPK:
             # (n_smart beyond the device's top-k capacity: evaluate on the device, select with numpy)
@@ -106,12 +121,19 @@ class DeviceHooks(abc.ABC):
         return x_tries[idx], min_acq, (x_tries[top] if n_x_seeds != 0 else [])
 
     def _smart_minimize(self, acq, space, x_seeds, random_state):
+        if len(x_seeds) != 0 and self._refine_grad(acq, space):
+            runs = [r for r in lockstep_lbfgsb(acq, x_seeds, space.bounds, grad=True) if r.success]
+            return self._best_run(runs, space)
         batched = _device_closure(acq) or getattr(acq, "b200_vectorized", False)
         refine = acq.refine_mode() if _device_closure(acq) and hasattr(acq, "refine_mode") else _null()
         with refine:
             if not batched or len(x_seeds) == 0 or not all(space.continuous_dimensions):
                 return super()._smart_minimize(acq, space, x_seeds, random_state)
             runs = [r for r in lockstep_lbfgsb(acq, x_seeds, space.bounds) if r.success]
+        return self._best_run(runs, space)
+
+    @staticmethod
+    def _best_run(runs, space):
         if not runs:
             return np.full(space.bounds.shape[0], np.nan), np.inf
         best = min(runs, key=lambda r: float(np.squeeze(r.fun)))  # first of equal minima, like the loop
@@ -274,7 +296,8 @@ class ThompsonSampling(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
             return [self._smart_minimize(acq.path(p), space, tops[p], random_state) for p in range(q)]
         seeds = [s for p in range(q) for s in tops[p]]
         owner = [p for p in range(q) for _ in tops[p]]
-        runs = lockstep_lbfgsb(acq, seeds, space.bounds, run_paths=owner) if seeds else []
+        runs = lockstep_lbfgsb(acq, seeds, space.bounds, run_paths=owner,
+                               grad=self._refine_grad(acq, space)) if seeds else []
         out = []
         for p in range(q):
             ok = [r for r, o in zip(runs, owner) if o == p and r.success]
@@ -441,20 +464,24 @@ _HOOKED = {
 }
 
 
-def accelerate(acq, candidate_source=None):
+def accelerate(acq, candidate_source=None, refine=None):
     """Give an existing reference acquisition object the device hooks IN PLACE (all state kept: kappa/xi,
     decay counters, dummies, gains).  ConstantLiar / GPHedge only orchestrate: their base acquisitions are
-    accelerated, the wrappers stay what they are."""
+    accelerated, the wrappers stay what they are.  candidate_source / refine: None leaves the object's setting."""
     if candidate_source not in (None, "host_rng", "device_philox"):
         raise ValueError("candidate_source must be 'host_rng' or 'device_philox'")
+    if refine not in (None, "stencil", "analytic"):
+        raise ValueError("refine must be 'stencil' or 'analytic'")
     if isinstance(acq, _ref.ConstantLiar):
-        acq.base_acquisition = accelerate(acq.base_acquisition, candidate_source)
+        acq.base_acquisition = accelerate(acq.base_acquisition, candidate_source, refine)
         return acq
     if isinstance(acq, _ref.GPHedge):
-        acq.base_acquisitions = [accelerate(a, candidate_source) for a in acq.base_acquisitions]
+        acq.base_acquisitions = [accelerate(a, candidate_source, refine) for a in acq.base_acquisitions]
         return acq
     if candidate_source is not None:
         acq.b200_candidate_source = candidate_source
+    if refine is not None:
+        acq.b200_refine = refine
     if isinstance(acq, DeviceHooks):
         return acq
     cls = type(acq)

@@ -136,6 +136,10 @@ struct b200bo_gp {
     // small-batch path scratch (per GP) + work-unit tables (rebuilt when np changes)
     DevBuf s_ksm, s_partial, s_mupart, s_unit, s_rb, s_colsq;
     int s_np = 0, s_nunits = 0;
+    // gradient calls (b200bo_acq_value_grad): v, u, the partials of the product with L^-T and of the gradient sums,
+    // and the upper-triangular work-unit tables (rebuilt when np or d changes)
+    DevBuf s_vsum, s_usum, s_partial_u, s_gpart, s_unit_u, s_rb_u, out_grad;
+    int s_grad_np = 0, s_grad_d = 0, s_nunits_u = 0;
     // fp32 mode: L^-1 as tf32 (hi,lo) wgmma operand images (built on first use after a fit)
     DevBuf tc_linv;
     bool tc_valid = false;
@@ -237,7 +241,8 @@ static int init_handle(b200bo_gp* gp) {
                             kPredictSmemBytesTc));
     CU(cudaFuncSetAttribute(predict_acq_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             kPredictSmemBytesTc));
-    CU(cudaFuncSetAttribute(small_trsv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmallTrsvSmemBytes));
+    CU(cudaFuncSetAttribute(small_trsv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmallTrsvSmemBytes));
+    CU(cudaFuncSetAttribute(small_trsv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmallTrsvSmemBytes));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 884, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 884, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_CPASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -285,6 +290,7 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
                       &gp->alphav, &gp->v1, &gp->v2, &gp->ls, &gp->xf, &gp->info, &gp->part,
                       &gp->pscratch, &gp->xc, &gp->out_acq, &gp->out_mu, &gp->out_sd, &gp->sel,
                       &gp->clamp, &gp->s_ksm, &gp->s_partial, &gp->s_mupart, &gp->s_unit, &gp->s_rb, &gp->s_colsq,
+                      &gp->s_vsum, &gp->s_usum, &gp->s_partial_u, &gp->s_gpart, &gp->s_unit_u, &gp->s_rb_u, &gp->out_grad,
                       &gp->tc_linv, &gp->pad_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
                       &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside, &gp->prune_key, &gp->prune_idx,
                       &gp->prune_tmp, &gp->prune_ctl};
@@ -968,8 +974,38 @@ extern "C" int b200bo_gp_get(b200bo_gp* gp, int what, double* out, int64_t len) 
 // ---------------------------------------------------------------------------------------
 // predict / acquisition
 // ---------------------------------------------------------------------------------------
+// gradient calls: the work units of u = L^-T v (row block i: k chunks of [64 i, np)) + their scratch for one GP
+static int ensure_small_grad(b200bo_gp* gp) {
+    const int np = gp->np, d = gp->d;
+    if (gp->s_grad_np == np && gp->s_grad_d == d) return B200BO_OK;
+    std::vector<int2> units, rbs;
+    const int nrb = np / SROWS;
+    for (int i = 0; i < nrb; ++i) {
+        const int nj = (np - i * SROWS + SKCH - 1) / SKCH;
+        rbs.push_back(make_int2((int)units.size(), nj));
+        for (int j = 0; j < nj; ++j) units.push_back(make_int2(i, j));
+    }
+    int rc;
+    if ((rc = gp->s_unit_u.reserve(sizeof(int2) * units.size()))) return rc;
+    if ((rc = gp->s_rb_u.reserve(sizeof(int2) * rbs.size()))) return rc;
+    if ((rc = gp->s_vsum.reserve(sizeof(double) * (size_t)SMAXP * np * SMC))) return rc;
+    if ((rc = gp->s_usum.reserve(sizeof(double) * (size_t)SMAXP * np * SMC))) return rc;
+    if ((rc = gp->s_partial_u.reserve(sizeof(double) * (size_t)SMAXP * units.size() * SROWS * SMC))) return rc;
+    if ((rc = gp->s_gpart.reserve(sizeof(double) * (size_t)SMAXP * (np / 128) * 2 * d * SMC))) return rc;
+    CU(cudaMemcpy(gp->s_unit_u.p, units.data(), sizeof(int2) * units.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(gp->s_rb_u.p, rbs.data(), sizeof(int2) * rbs.size(), cudaMemcpyHostToDevice));
+    gp->s_grad_np = np;
+    gp->s_grad_d = d;
+    gp->s_nunits_u = (int)units.size();
+    return B200BO_OK;
+}
+
 // small-batch path: work-unit tables + scratch for one GP
-static int ensure_small(b200bo_gp* gp) {
+static int ensure_small(b200bo_gp* gp, bool grad = false) {
+    if (grad) {
+        const int rc = ensure_small_grad(gp);
+        if (rc) return rc;
+    }
     const int np = gp->np;
     if (gp->s_np == np) return B200BO_OK;
     std::vector<int2> units, rbs;
@@ -1366,8 +1402,8 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             const int npass = (int)((left + SMC - 1) / SMC < SMAXP ? (left + SMC - 1) / SMC : SMAXP);
             for (int g = 0; g < spec->n_gps; ++g) {
                 small_kstar_kernel<<<dim3(spec->gps[g]->np / 128, npass), 256, 0, stream>>>(S, g);
-                small_trsv_kernel<<<dim3(spec->gps[g]->s_nunits, (npass + STPG - 1) / STPG), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
-                small_reduce_kernel<<<dim3(spec->gps[g]->np / SROWS, npass), 256, 0, stream>>>(S, g);
+                small_trsv_kernel<false><<<dim3(spec->gps[g]->s_nunits, (npass + STPG - 1) / STPG), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
+                small_reduce_kernel<0><<<dim3(spec->gps[g]->np / SROWS, npass), 256, 0, stream>>>(S, g);
                 LAUNCHED();
                 LAUNCHED();
                 LAUNCHED();
@@ -1731,6 +1767,86 @@ extern "C" int b200bo_acq_eval(const b200bo_acq* spec, const double* Xc, int64_t
     return run_host(spec, Xc, m, acq_neg, nullptr, nullptr, 0, nullptr, nullptr);
 }
 
+// Value and input gradient of the closure on the small-batch kernels (predict_kernels.cuh: small_grad_kernel,
+// small_finish_grad_kernel).  Per launch group of up to SMAXP passes and per GP: K*, v = L^-1 k* (its sums exactly
+// those of the value path), u = L^-T v, the gradient partials; then one finish for every GP.
+extern "C" int b200bo_acq_value_grad(const b200bo_acq* spec, const double* Xc, int64_t m, double* val, double* grad) {
+    int rc;
+    if ((rc = check_spec(spec))) return rc;
+    if (spec->kind == B200BO_ACQ_NONE) return set_err(B200BO_ERR_ARG, "kind NONE has no acquisition");
+    if (m < 0 || (m > 0 && (!Xc || !val || !grad))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    b200bo_gp* g0 = spec->gps[0];
+    const int d = g0->d;
+    CU(cudaSetDevice(g0->device));
+    NvtxRange nvtx_range("b200bo:acq_value_grad");
+    if ((rc = g0->xc.reserve(sizeof(double) * (size_t)m * d))) return rc;
+    if ((rc = g0->out_acq.reserve(sizeof(double) * (size_t)m))) return rc;
+    if ((rc = g0->out_grad.reserve(sizeof(double) * (size_t)m * d))) return rc;
+    CU(cudaMemcpy(g0->xc.p, Xc, sizeof(double) * (size_t)m * d, cudaMemcpyHostToDevice));
+    CandSrc src;
+    src.d_Xc = g0->xc.as<double>();
+    SmallParams S;
+    memset(&S, 0, sizeof(S));
+    int np_max = 0;
+    cudaStream_t stream = nullptr;
+    if ((rc = fill_params(spec, src, m, 0, stream, S.P, np_max))) return rc;
+    S.P.acq_out = g0->out_acq.as<double>();
+    if ((rc = g0->clamp.reserve(2 * sizeof(unsigned long long)))) return rc;
+    S.P.clamp_count = g0->clamp.as<unsigned long long>();
+    CU(cudaMemsetAsync(g0->clamp.p, 0, 2 * sizeof(unsigned long long), stream));
+    for (int g = 0; g < spec->n_gps; ++g) {
+        b200bo_gp* gp = spec->gps[g];
+        if ((rc = ensure_small(gp, true))) return rc;
+        SmallGp& Q = S.sg[g];
+        Q.W = gp->W.as<double>();
+        Q.ksm = gp->s_ksm.as<double>();
+        Q.partial = gp->s_partial.as<double>();
+        Q.mu_part = gp->s_mupart.as<double>();
+        Q.colsq_rb = gp->s_colsq.as<double>();
+        Q.unit_tab = gp->s_unit.as<int2>();
+        Q.rb_tab = gp->s_rb.as<int2>();
+        Q.vsum = gp->s_vsum.as<double>();
+        Q.usum = gp->s_usum.as<double>();
+        Q.partial_u = gp->s_partial_u.as<double>();
+        Q.gpart = gp->s_gpart.as<double>();
+        Q.unit_tab_u = gp->s_unit_u.as<int2>();
+        Q.rb_tab_u = gp->s_rb_u.as<int2>();
+        S.nunits[g] = gp->s_nunits;
+        S.nunits_u[g] = gp->s_nunits_u;
+    }
+    S.m_end = m;
+    S.grad_out = g0->out_grad.as<double>();
+    CU(cudaEventRecord(g0->ev0, stream));
+    for (long long c0 = 0; c0 < m; c0 += (long long)SMAXP * SMC) {
+        S.c0 = c0;
+        const long long left = m - c0;
+        const int npass = (int)((left + SMC - 1) / SMC < SMAXP ? (left + SMC - 1) / SMC : SMAXP);
+        const int ngrp = (npass + STPG - 1) / STPG;
+        for (int g = 0; g < spec->n_gps; ++g) {
+            const b200bo_gp* gp = spec->gps[g];
+            small_kstar_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+            small_trsv_kernel<false><<<dim3(gp->s_nunits, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
+            small_reduce_kernel<1><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
+            small_trsv_kernel<true><<<dim3(gp->s_nunits_u, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
+            small_reduce_kernel<2><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
+            small_grad_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+            for (int i = 0; i < 6; ++i) LAUNCHED();
+        }
+        small_finish_grad_kernel<<<npass, 256, 0, stream>>>(S);
+        LAUNCHED();
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(g0->ev1, stream));
+    g_last_timed = g0;
+    g0->stat_total = g0->stat_direct = m;
+    g0->prune_counted = false;
+    CU(cudaDeviceSynchronize());
+    CU(cudaMemcpy(val, g0->out_acq.p, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(grad, g0->out_grad.p, sizeof(double) * (size_t)m * d, cudaMemcpyDeviceToHost));
+    return check_nonfinite(g0);
+}
+
 static void unpack_records(const SelRecord* sel, int k, double* best_val, int64_t* best_idx, double* topk_val,
                            int64_t* topk_idx) {
     if (best_val) *best_val = sel[0].value;
@@ -1845,6 +1961,7 @@ struct b200bo_paths {
     DevBuf Xs, V, omega, bias, W, ls, xf, xc, out, sel_cta, sel, pbounds, prow, bad;
     DevBuf cvals, cmerit, craw;  // constrained calls with this handle as set 0: [G][chunk][q] values, outputs
     DevBuf pidx;                 // row-mode calls: (m,) path index per row
+    DevBuf grad;                 // b200bo_paths_grad_rows: (m, d) gradients
     ChunkedUpload upload;
 };
 
@@ -2067,7 +2184,7 @@ extern "C" void b200bo_paths_destroy(b200bo_paths* ps) {
     cudaSetDevice(ps->device);
     DevBuf* bufs[] = {&ps->Xs, &ps->V, &ps->omega, &ps->bias, &ps->W, &ps->ls, &ps->xf, &ps->xc,
                       &ps->out, &ps->sel_cta, &ps->sel, &ps->pbounds, &ps->prow, &ps->bad,
-                      &ps->cvals, &ps->cmerit, &ps->craw, &ps->pidx};
+                      &ps->cvals, &ps->cmerit, &ps->craw, &ps->pidx, &ps->grad};
     for (DevBuf* b : bufs) b->release();
     ps->upload.release();
     delete ps;
@@ -2122,6 +2239,43 @@ extern "C" int b200bo_paths_eval_rows(b200bo_paths* ps, const double* Xc, const 
     P.path_idx = ps->pidx.as<int>();
     if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
     CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost));
+    return paths_check_nonfinite(ps);
+}
+
+// Value and input gradient of row i on path path_idx[i]: the value from the row-mode evaluation kernel (bit-equal
+// to b200bo_paths_eval_rows), the gradient from paths_grad_kernel on the same device rows.
+extern "C" int b200bo_paths_grad_rows(b200bo_paths* ps, const double* Xc, const int* path_idx, int64_t m, double* val,
+                                      double* grad) {
+    if (!ps || m < 0 || (m > 0 && (!Xc || !path_idx || !val || !grad))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    if (m > std::numeric_limits<int>::max()) return set_err(B200BO_ERR_ARG, "m=%lld too large", (long long)m);
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_grad_rows");
+    const int d = ps->d;
+    int rc;
+    if ((rc = paths_upload_rows(ps, ps->q, path_idx, m))) return rc;
+    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * d))) return rc;
+    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m))) return rc;
+    if ((rc = ps->grad.reserve(sizeof(double) * (size_t)m * d))) return rc;
+    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * d, cudaMemcpyHostToDevice));
+    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
+    PathsParams P = paths_params(ps);
+    P.Xc = ps->xc.as<double>();
+    P.m = m;
+    P.out = ps->out.as<double>();
+    P.path_idx = ps->pidx.as<int>();
+    if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
+    double* dg = ps->grad.as<double>();
+    switch (ps->cov) {
+        case 0: paths_grad_kernel<0><<<(unsigned)m, PG_NT>>>(P, dg); break;
+        case 1: paths_grad_kernel<1><<<(unsigned)m, PG_NT>>>(P, dg); break;
+        case 2: paths_grad_kernel<2><<<(unsigned)m, PG_NT>>>(P, dg); break;
+        default: paths_grad_kernel<3><<<(unsigned)m, PG_NT>>>(P, dg); break;
+    }
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(val, ps->out.p, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(grad, ps->grad.p, sizeof(double) * (size_t)m * d, cudaMemcpyDeviceToHost));
     return paths_check_nonfinite(ps);
 }
 

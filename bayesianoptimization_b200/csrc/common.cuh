@@ -99,6 +99,31 @@ __device__ __forceinline__ double cov_from_r2(double r2, int family, int nu) {
     }
 }
 
+// h(r) = -(1/r) dk/dr of the unit covariance k(r), from r^2: the input gradient of k(|xs - Xs_n|) is
+// -h(r) (xs - Xs_n).  RBF: k; Matern 2.5: (5/3)(1 + sqrt5 r) exp(-sqrt5 r); 1.5: 3 exp(-sqrt3 r); 0.5: exp(-r)/r.
+// Matern 0.5 has a kink at a training input (h unbounded as r -> 0, the gradient's direction undefined at 0):
+// h := 0 at r = 0, so that row contributes nothing.
+template <int COV>
+__device__ __forceinline__ double cov_dh_eval(double r2) {
+    if (COV == 3) return exp_neg(0.5 * r2);
+    const double dist = sqrt_pos(r2);
+    if (COV == 2) {
+        const double k = dist * 2.23606797749978969641;
+        return (5.0 / 3.0) * (1.0 + k) * exp_neg(k);
+    }
+    if (COV == 1) return 3.0 * exp_neg(dist * 1.73205080756887729353);
+    return r2 == 0.0 ? 0.0 : exp_neg(dist) / dist;
+}
+
+__device__ __forceinline__ double cov_dh_from_r2(double r2, int family, int nu) {
+    switch (cov_code(family, nu)) {
+        case 0: return cov_dh_eval<0>(r2);
+        case 1: return cov_dh_eval<1>(r2);
+        case 2: return cov_dh_eval<2>(r2);
+        default: return cov_dh_eval<3>(r2);
+    }
+}
+
 // scipy.special.ndtr (cephes ndtr.c), which scipy.stats.norm.cdf evaluates
 // (SP/stats/_continuous_distns.py:370-371).
 __device__ __forceinline__ double ndtr(double a) {

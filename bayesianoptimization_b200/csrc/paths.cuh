@@ -193,6 +193,81 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
 }
 
 // ---------------------------------------------------------------------------------------
+// Input gradient of a path in row mode (b200bo_paths_grad_rows): one CTA per row i, path p = path_idx[i],
+//   d path_p / d x_j = s_y ( -feat_scale sum_l W[l][p] sin(omega_l . xs + b_l) omega_lj
+//                            - sum_n V[n][p] c h(r_n) (xs_j - Xs_nj) ) / ls_j          (h: cov_dh_eval)
+// and 0 for a rounded dimension.  Items (training rows, then features) go through in chunks of 256: each thread
+// forms the scalar coefficient of one item, then thread (j, slice s) adds its contiguous share of the chunk's items
+// in index order; the slices are added in s order at the end.  No atomics: a row's gradient depends on its
+// coordinates and its path only.  The value of the same row comes from the ROWS paths_eval_kernel.
+// ---------------------------------------------------------------------------------------
+constexpr int PG_NT = 256;
+
+template <int COV>
+__global__ void __launch_bounds__(PG_NT) paths_grad_kernel(const PathsParams P, double* __restrict__ grad) {
+    __shared__ double xs_s[B200BO_MAX_DIM];
+    __shared__ double coef[PG_NT];
+    __shared__ double red[PG_NT];
+    const int tid = threadIdx.x, d = P.d, q = P.q;
+    const long long gi = blockIdx.x;
+    const int p = P.path_idx[gi];
+    if (tid < d) {
+        double v = P.Xc[gi * d + tid];
+        if (P.xform && P.xform[tid] == B200BO_XFORM_ROUND) v = rint(v);
+        xs_s[tid] = v / P.ls[tid];
+    }
+    __syncthreads();
+    const int nsl = PG_NT / d, per = PG_NT / nsl;  // slices per dimension, items of a chunk per slice (the last
+    const int j = tid % d, sl = tid / d;           // slice also takes the remainder)
+    const bool worker = sl < nsl;
+    const int i0 = sl * per, i1 = (sl == nsl - 1) ? PG_NT : i0 + per;
+    double acc = 0.0;
+    for (int pass = 0; pass < 2; ++pass) {
+        const double* A = pass ? P.omega : P.Xs;
+        const double* B = pass ? P.W : P.V;
+        const int cnt = pass ? P.Lp : P.np;
+        for (int c0 = 0; c0 < cnt; c0 += PG_NT) {
+            const int it = c0 + tid;
+            double cf = 0.0;
+            if (it < cnt) {
+                const double* a = A + (size_t)it * d;
+                double s = 0.0;
+                for (int jj = 0; jj < d; ++jj) {
+                    if (pass) {
+                        s = fma(a[jj], xs_s[jj], s);
+                    } else {
+                        const double df = xs_s[jj] - a[jj];
+                        s = fma(df, df, s);
+                    }
+                }
+                if (pass)
+                    cf = -P.feat_scale * B[(size_t)it * q + p] * sin(s + P.bias[it]);
+                else if (it < P.n)
+                    cf = -P.constv * B[(size_t)it * q + p] * cov_dh_eval<COV>(s);
+            }
+            coef[tid] = cf;
+            __syncthreads();
+            if (worker) {
+                const int e = min(i1, cnt - c0);
+                for (int i = i0; i < e; ++i) {
+                    const double av = A[(size_t)(c0 + i) * d + j];
+                    acc = fma(coef[i], pass ? av : xs_s[j] - av, acc);
+                }
+            }
+            __syncthreads();
+        }
+    }
+    red[tid] = acc;
+    __syncthreads();
+    if (tid < d) {
+        double t = 0.0;
+        for (int s2 = 0; s2 < nsl; ++s2) t += red[s2 * d + tid];
+        const bool rounded = P.xform && P.xform[tid] == B200BO_XFORM_ROUND;
+        grad[gi * d + tid] = rounded ? 0.0 : P.y_std * t / P.ls[tid];
+    }
+}
+
+// ---------------------------------------------------------------------------------------
 // Constrained Thompson sampling (SCBO rule: Eriksson & Poloczek, AISTATS 2021).  G = 1 + J sets of q paths: set 0
 // the target, set j >= 1 constraint GP j with bounds [lb_j, ub_j].  Path p of every set is one joint draw.  Per
 // candidate and path, from the values paths_eval_kernel left in vals[g][i][p] (data units):

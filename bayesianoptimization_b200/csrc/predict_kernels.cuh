@@ -765,6 +765,14 @@ struct SmallGp {
     double* colsq_rb;       // [np/SROWS][SMC] per pass: sum over the rows of a row block of V^2
     const int2* unit_tab;   // [nunits] (row-block, k-chunk)
     const int2* rb_tab;     // [np/SROWS] (first unit, number of units)
+    // gradient calls only (b200bo_acq_value_grad), else unset: v = L^-1 k*, u = L^-T v and the work units of the
+    // upper-triangular product against linvT (row block i covers k in [64 i, np))
+    double* vsum;           // [np][SMC] per pass
+    double* usum;           // [np][SMC] per pass
+    double* partial_u;      // [nunits_u][SROWS][SMC]
+    double* gpart;          // [np/128][2][d][SMC] per pass: partials of sum_n {alpha_n, u_n} c h(r_n) (xs_j - Xs_nj)
+    const int2* unit_tab_u; // [nunits_u] (row-block, k-chunk counted from the block's first row)
+    const int2* rb_tab_u;   // [np/SROWS]
 };
 
 // One launch group covers up to SMAXP passes (blockIdx.y / blockIdx.x of the finish kernel = pass): the
@@ -778,6 +786,8 @@ struct SmallParams {
     long long c0;  // first candidate of pass 0 of this launch group
     long long m_end;  // one past the last candidate of the batch
     int nunits[B200BO_MAX_GPS];  // work units per pass (stride of `partial` between passes)
+    int nunits_u[B200BO_MAX_GPS];  // gradient calls: work units per pass of the product with linvT
+    double* grad_out;  // gradient calls: [m][d]
 };
 
 __device__ __forceinline__ long long small_pass_c0(const SmallParams& S, int pass) { return S.c0 + (long long)pass * SMC; }
@@ -844,6 +854,9 @@ small_kstar_kernel(const SmallParams S, int g) {
 // of four: ~100 registers, 49 KB -> two to three resident CTAs per SM.)
 constexpr int STPG = 4;
 constexpr int kSmallTrsvSmemBytes = (SROWS * SWSTR + STPG * SKT * SMC) * 8;  // 50176
+// UPPER (gradient calls): the same product against linvT = L^-T, u = L^-T v: the unit's k range starts at its row
+// block (k in [r0 + 512 j, min(.. + 512, np))), the right-hand side is vsum and the partials go to partial_u.
+template <bool UPPER>
 __global__ void __launch_bounds__(256, 2)
 small_trsv_kernel(const SmallParams S, int g, int npass) {
     const GpDev& G = S.P.gp[g];
@@ -853,11 +866,11 @@ small_trsv_kernel(const SmallParams S, int g, int npass) {
     double* Kt = strsv_smem + SROWS * SWSTR;  // [STPG][SKT][SMC]
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int p0 = blockIdx.y * STPG, pn = min(STPG, npass - p0);
-    const int2 u = Q.unit_tab[blockIdx.x];
+    const int2 u = UPPER ? Q.unit_tab_u[blockIdx.x] : Q.unit_tab[blockIdx.x];
     const int r0 = u.x * SROWS;
-    const int kbeg = u.y * SKCH;
-    const int kend = min(kbeg + SKCH, r0 + SROWS);
     const int np = G.np;
+    const int kbeg = UPPER ? r0 + u.y * SKCH : u.y * SKCH;
+    const int kend = UPPER ? min(kbeg + SKCH, np) : min(kbeg + SKCH, r0 + SROWS);
     double acc[STPG][8];
 #pragma unroll
     for (int p = 0; p < STPG; ++p)
@@ -866,10 +879,10 @@ small_trsv_kernel(const SmallParams S, int g, int npass) {
     for (int k0 = kbeg; k0 < kend; k0 += SKT) {
         for (int idx = tid; idx < SROWS * SKT; idx += 256) {
             const int r = idx / SKT, kk = idx % SKT;
-            Wt[r * SWSTR + kk] = Q.W[(size_t)(r0 + r) * np + k0 + kk];
+            Wt[r * SWSTR + kk] = (UPPER ? G.linvT : Q.W)[(size_t)(r0 + r) * np + k0 + kk];
         }
         for (int p = 0; p < pn; ++p) {
-            const double* ksm = Q.ksm + (size_t)(p0 + p) * np * SMC + (size_t)k0 * SMC;
+            const double* ksm = (UPPER ? Q.vsum : Q.ksm) + (size_t)(p0 + p) * np * SMC + (size_t)k0 * SMC;
             for (int idx = tid; idx < SKT * SMC; idx += 256) Kt[p * SKT * SMC + idx] = ksm[idx];
         }
         __syncthreads();
@@ -895,7 +908,8 @@ small_trsv_kernel(const SmallParams S, int g, int npass) {
 #pragma unroll
     for (int p = 0; p < STPG; ++p) {
         if (p < pn) {
-            double* out = Q.partial + ((size_t)(p0 + p) * S.nunits[g] + blockIdx.x) * SROWS * SMC;
+            double* out = (UPPER ? Q.partial_u : Q.partial) +
+                          ((size_t)(p0 + p) * (UPPER ? S.nunits_u[g] : S.nunits[g]) + blockIdx.x) * SROWS * SMC;
 #pragma unroll
             for (int q = 0; q < 8; ++q) out[(warp * 8 + q) * SMC + lane] = acc[p][q];
         }
@@ -904,6 +918,9 @@ small_trsv_kernel(const SmallParams S, int g, int npass) {
 
 // Per (row block of 64 rows, pass): sum the k-chunk partials of every row in a fixed order, square, and reduce the
 // 64 rows -> colsq_rb[pass][row block][candidate].  grid (np / 64, npass).
+// MODE (gradient calls): 1 also writes the summed v[n][c] to vsum (the same sums, so colsq is unchanged); 2 sums the
+// partials of the product with linvT in index order into usum and forms no squares.
+template <int MODE>
 __global__ void __launch_bounds__(256)
 small_reduce_kernel(const SmallParams S, int g) {
     const GpDev& G = S.P.gp[g];
@@ -911,15 +928,19 @@ small_reduce_kernel(const SmallParams S, int g) {
     __shared__ double red[8][SMC];
     const int tid = threadIdx.x, c = tid & 31, rg = tid >> 5;
     const int pass = blockIdx.y;
-    const int2 rb = Q.rb_tab[blockIdx.x];
-    const double* partial = Q.partial + (size_t)pass * S.nunits[g] * SROWS * SMC;
+    const int2 rb = MODE == 2 ? Q.rb_tab_u[blockIdx.x] : Q.rb_tab[blockIdx.x];
+    const double* partial = MODE == 2 ? Q.partial_u + (size_t)pass * S.nunits_u[g] * SROWS * SMC
+                                      : Q.partial + (size_t)pass * S.nunits[g] * SROWS * SMC;
     double s = 0.0;
     for (int q = 0; q < 8; ++q) {
         const int r = rg * 8 + q;
         double v = 0.0;
         for (int j = 0; j < rb.y; ++j) v += partial[((size_t)(rb.x + j) * SROWS + r) * SMC + c];
+        if (MODE != 0)
+            (MODE == 2 ? Q.usum : Q.vsum)[((size_t)pass * G.np + blockIdx.x * SROWS + r) * SMC + c] = v;
         s = fma(v, v, s);
     }
+    if (MODE == 2) return;
     red[rg][c] = s;
     __syncthreads();
     if (tid < SMC) {
@@ -930,16 +951,11 @@ small_reduce_kernel(const SmallParams S, int g) {
     }
 }
 
-// Per pass (blockIdx.x): sum the row-block and K* alpha_ partials in index order, then the per-candidate epilogue
-// of every GP.  256 threads = 32 candidates x 8 slices of the partial lists (fixed-order two-level sum).
-__global__ void __launch_bounds__(256)
-small_finish_kernel(const SmallParams S) {
-    __shared__ double red[8][SMC];
-    __shared__ double colsq_s[B200BO_MAX_GPS][SMC];
-    __shared__ double mu_s[B200BO_MAX_GPS][SMC];
+// Per pass: the row-block and K* alpha_ partials of every GP summed in index order into colsq_s / mu_s.  256 threads
+// = 32 candidates x 8 slices of the partial lists (fixed-order two-level sum).
+__device__ __forceinline__ void small_finish_sums(const SmallParams& S, int pass, double (*red)[SMC],
+                                                  double (*colsq_s)[SMC], double (*mu_s)[SMC]) {
     const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
-    const int pass = blockIdx.x, mc = small_pass_mc(S, pass);
-    const long long pc0 = small_pass_c0(S, pass);
     for (int g = 0; g < S.P.n_gps; ++g) {
         const GpDev& G = S.P.gp[g];
         const SmallGp& Q = S.sg[g];
@@ -970,10 +986,245 @@ small_finish_kernel(const SmallParams S) {
         }
         __syncthreads();
     }
+}
+
+// Per pass (blockIdx.x): the sums above, then the per-candidate epilogue of every GP.
+__global__ void __launch_bounds__(256)
+small_finish_kernel(const SmallParams S) {
+    __shared__ double red[8][SMC];
+    __shared__ double colsq_s[B200BO_MAX_GPS][SMC];
+    __shared__ double mu_s[B200BO_MAX_GPS][SMC];
+    const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
+    const int pass = blockIdx.x, mc = small_pass_mc(S, pass);
+    const long long pc0 = small_pass_c0(S, pass);
+    small_finish_sums(S, pass, red, colsq_s, mu_s);
     if (sl == 0 && c < mc) {
         double base_neg = 0.0, prod = 1.0;
         for (int g = 0; g < S.P.n_gps; ++g)
             candidate_epilogue(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod);
+    }
+}
+
+// ---- input gradient of the closure value (b200bo_acq_value_grad, DESIGN.md 4.10) ------------------------------
+// With xs = transform(x)/ls, k*_n = c k(|xs - Xs_n|), v = L^-1 k*, u = L^-T v = K^-1 k* (normalised units):
+//   d k*_n / d x_j = -c h(r_n) (xs_j - Xs_nj) / ls_j          (h: cov_dh_from_r2)
+//   d mu / d x_j   = sum_n alpha_n d k*_n / d x_j,    d var / d x_j = -2 sum_n u_n d k*_n / d x_j
+// small_grad_kernel: per (block of 128 training rows, pass) the partial sums
+//   gpart[0][j][c] = sum_n alpha_n c h(r_n) (xs_j - Xs_nj),   gpart[1][j][c] = the same with u_n,
+// by direct differences, rows in index order.  Sub-chunks of 32 rows: first thread = (candidate, 4 rows) forms the two
+// coefficients of each row, then thread = (candidate, dimensions j = jg, jg + 8, ..) adds the 32 rows in order.
+constexpr int SGR = 32;  // rows per sub-chunk
+__global__ void __launch_bounds__(256)
+small_grad_kernel(const SmallParams S, int g) {
+    const GpDev& G = S.P.gp[g];
+    const SmallGp& Q = S.sg[g];
+    __shared__ double xc_s[SMC][B200BO_MAX_DIM + 1];
+    __shared__ double coef[2][SGR][SMC];
+    const int tid = threadIdx.x, d = S.P.d;
+    const int pass = blockIdx.y, mc = small_pass_mc(S, pass);
+    const long long pc0 = small_pass_c0(S, pass);
+    for (int idx = tid; idx < SMC * d; idx += 256) {
+        const int c = idx / d, j = idx - c * d;
+        double v = 0.0;
+        if (c < mc) {
+            v = S.P.Xc[(pc0 + c) * d + j];
+            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
+            v = v / G.ls[j];
+        }
+        xc_s[c][j] = v;
+    }
+    __syncthreads();
+    const int c = tid & 31, rg = tid >> 5;
+    constexpr int JT = B200BO_MAX_DIM / 8;
+    double sa[JT], su[JT];
+#pragma unroll
+    for (int t = 0; t < JT; ++t) sa[t] = su[t] = 0.0;
+    const double* usum = Q.usum + (size_t)pass * G.np * SMC;
+    for (int sub = 0; sub < 128 / SGR; ++sub) {
+        const int n0 = blockIdx.x * 128 + sub * SGR;
+        for (int q = 0; q < SGR / 8; ++q) {
+            const int rl = rg * (SGR / 8) + q, n = n0 + rl;
+            double ca = 0.0, cu = 0.0;
+            if (c < mc && n < G.n) {
+                const double* xr = G.Xs + (size_t)n * d;
+                double r2 = 0.0;
+                for (int j = 0; j < d; ++j) {
+                    const double df = xc_s[c][j] - xr[j];
+                    r2 = fma(df, df, r2);
+                }
+                const double ch = G.constv * cov_dh_from_r2(r2, G.family, G.nu);
+                ca = G.alphav[n] * ch;
+                cu = usum[(size_t)n * SMC + c] * ch;
+            }
+            coef[0][rl][c] = ca;
+            coef[1][rl][c] = cu;
+        }
+        __syncthreads();
+        for (int rl = 0; rl < SGR; ++rl) {
+            const double* xr = G.Xs + (size_t)(n0 + rl) * d;
+            const double ca = coef[0][rl][c], cu = coef[1][rl][c];
+#pragma unroll
+            for (int t = 0; t < JT; ++t) {
+                const int j = rg + 8 * t;
+                if (j < d) {
+                    const double df = xc_s[c][j] - xr[j];
+                    sa[t] = fma(ca, df, sa[t]);
+                    su[t] = fma(cu, df, su[t]);
+                }
+            }
+        }
+        __syncthreads();
+    }
+    double* out = Q.gpart + ((size_t)pass * (G.np / 128) + blockIdx.x) * 2 * d * SMC;
+#pragma unroll
+    for (int t = 0; t < JT; ++t) {
+        const int j = rg + 8 * t;
+        if (j < d) {
+            out[(size_t)j * SMC + c] = sa[t];
+            out[(size_t)(d + j) * SMC + c] = su[t];
+        }
+    }
+}
+
+// t'(g) of one MES sample's term t(g) = g lambda / 2 - log Psi(g), lambda = psi / Psi (inv_mills):
+// lambda' = -lambda (g + lambda), so t' = -lambda/2 - g lambda (g + lambda)/2.  Out of line like mes_term;
+// lambda = 0 (g above ~38.6) is the limit 0.
+__device__ __noinline__ double mes_term_deriv(double g) {
+    const double r = inv_mills(g);
+    if (r == 0.0) return 0.0;
+    return -0.5 * r - 0.5 * g * r * (g + r);
+}
+
+// Chain rule of one GP's factor in data units, as the coefficients of d mean and d sd:
+//   d term = cm d mean + cs d sd,   term = the base acquisition (g = 0) or the probability factor p (g >= 1).
+// Returns the term itself in `term`.  sd == 0 (a clamped or vanished variance): the caller sets d sd := 0, and the
+// coefficients that divide by sd (PoI, MES) are 0 - the value there is a step or constant in x.
+__device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, const GpDev& G, int g, double mean,
+                                                        double sd, double& term, double& cm, double& cs) {
+    cm = cs = 0.0;
+    if (g == 0) {
+        term = 0.0;
+        if (P.acq_kind == B200BO_ACQ_UCB) {
+            term = mean + P.kappa * sd;
+            cm = 1.0;
+            cs = P.kappa;
+        } else if (P.acq_kind == B200BO_ACQ_EI) {
+            const double a = mean - P.y_max - P.xi;
+            const double z = a / sd;
+            term = a * ndtr(z) + sd * norm_pdf(z);
+            cm = ndtr(z);
+            cs = norm_pdf(z);
+        } else if (P.acq_kind == B200BO_ACQ_POI) {
+            const double z = (mean - P.y_max - P.xi) / sd;
+            term = ndtr(z);
+            if (sd > 0.0) {
+                const double pz = norm_pdf(z);
+                cm = pz / sd;
+                cs = pz == 0.0 ? 0.0 : -z * pz / sd;
+            }
+        } else if (P.acq_kind == B200BO_ACQ_MES) {
+            if (sd > 0.0) {
+                double s = 0.0, sm = 0.0, ss = 0.0;
+                for (int k = 0; k < P.n_ystar; ++k) {
+                    const double gk = (P.ystar[k] - mean) / sd;
+                    s += mes_term(gk);
+                    const double td = mes_term_deriv(gk);
+                    sm += td;
+                    ss += td == 0.0 ? 0.0 : td * gk;
+                }
+                term = s / (double)P.n_ystar;
+                cm = -sm / ((double)P.n_ystar * sd);
+                cs = -ss / ((double)P.n_ystar * sd);
+            }
+        }
+    } else {
+        const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
+        const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
+        term = p_hi - p_lo;
+        if (sd > 0.0) {
+            if (G.lb != -CUDART_INF) {
+                const double z = (G.lb - mean) / sd, pz = norm_pdf(z);
+                cm += pz / sd;
+                cs += pz == 0.0 ? 0.0 : z * pz / sd;
+            }
+            if (G.ub != CUDART_INF) {
+                const double z = (G.ub - mean) / sd, pz = norm_pdf(z);
+                cm -= pz / sd;
+                cs -= pz == 0.0 ? 0.0 : z * pz / sd;
+            }
+        }
+    }
+}
+
+// Gradient finish, per pass (blockIdx.x): the value exactly as small_finish_kernel forms it (same sums, same
+// epilogue), then per candidate and GP the weights of the two partial-sum lists,
+//   grad_j = sum_g ( wa_g sum_b gpart_g[b][0][j] + wu_g sum_b gpart_g[b][1][j] ) / ls_gj      (blocks b in index order)
+//   wa_g = -w_g cm_g s_y,   wu_g = w_g cs_g s_y / sqrt(var_g)   (0 where var_g <= 0: d sd := 0)
+//   w_0 = -prod_i p_i,   w_g = -base prod_{i != g} p_i           (product rule over the GPs, g order)
+// A rounded dimension has gradient 0; a NaN value gives a NaN row.
+__global__ void __launch_bounds__(256)
+small_finish_grad_kernel(const SmallParams S) {
+    __shared__ double red[8][SMC];
+    __shared__ double colsq_s[B200BO_MAX_GPS][SMC];
+    __shared__ double mu_s[B200BO_MAX_GPS][SMC];
+    __shared__ double wa_s[B200BO_MAX_GPS][SMC], wu_s[B200BO_MAX_GPS][SMC];
+    __shared__ double val_s[SMC];
+    const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
+    const int pass = blockIdx.x, mc = small_pass_mc(S, pass), d = S.P.d, ng = S.P.n_gps;
+    const long long pc0 = small_pass_c0(S, pass);
+    small_finish_sums(S, pass, red, colsq_s, mu_s);
+    if (sl == 0 && c < mc) {
+        double base_neg = 0.0, prod = 1.0, val = 0.0;
+        for (int g = 0; g < ng; ++g)
+            candidate_epilogue(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, &val);
+        val_s[c] = val;
+        // term_g, then w_g from the terms of the other GPs; wa_s / wu_s hold cm / cs until the second loop
+        double term[B200BO_MAX_GPS];
+#pragma unroll
+        for (int g = 0; g < B200BO_MAX_GPS; ++g) {
+            term[g] = 1.0;
+            if (g < ng) {
+                const GpDev& G = S.P.gp[g];
+                const double mean = G.y_std * mu_s[g][c] + G.y_mean;
+                const double var = fmax(G.prior - colsq_s[g][c], 0.0);
+                const double sd = sqrt(var * (G.y_std * G.y_std));
+                double cm, cs;
+                candidate_epilogue_grad(S.P, G, g, mean, sd, term[g], cm, cs);
+                wa_s[g][c] = -cm * G.y_std;
+                wu_s[g][c] = var > 0.0 ? cs * G.y_std / sqrt(var) : 0.0;
+            }
+        }
+#pragma unroll
+        for (int g = 0; g < B200BO_MAX_GPS; ++g) {
+            if (g < ng) {
+                double w = -1.0;
+#pragma unroll
+                for (int i = 0; i < B200BO_MAX_GPS; ++i)
+                    if (i < ng && i != g) w *= term[i];
+                wa_s[g][c] = wa_s[g][c] == 0.0 ? 0.0 : w * wa_s[g][c];
+                wu_s[g][c] = wu_s[g][c] == 0.0 ? 0.0 : w * wu_s[g][c];
+            }
+        }
+    }
+    __syncthreads();
+    for (int idx = tid; idx < SMC * d; idx += 256) {
+        const int cc = idx & 31, j = idx >> 5;
+        if (cc >= mc) continue;
+        double gr = 0.0;
+        for (int g = 0; g < ng; ++g) {
+            const GpDev& G = S.P.gp[g];
+            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) continue;
+            const int nb = G.np / 128;
+            const double* gp = S.sg[g].gpart + (size_t)pass * nb * 2 * d * SMC;
+            double a = 0.0, u = 0.0;
+            for (int b = 0; b < nb; ++b) {
+                a += gp[((size_t)b * 2 * d + j) * SMC + cc];
+                u += gp[((size_t)b * 2 * d + d + j) * SMC + cc];
+            }
+            const double wa = wa_s[g][cc], wu = wu_s[g][cc];
+            gr += ((wa == 0.0 ? 0.0 : wa * a) + (wu == 0.0 ? 0.0 : wu * u)) / G.ls[j];
+        }
+        S.grad_out[(pc0 + cc) * d + j] = isnan(val_s[cc]) ? CUDART_NAN : gr;
     }
 }
 

@@ -175,6 +175,22 @@ class FusedAcquisition:
                 off.ctypes.data_as(C.POINTER(C.c_int64)) if off is not None else None, B.as_dp(out)))
         return out
 
+    def value_and_grad(self, x):
+        """(vals (M,), grads (M, d)): the closure value and its analytic gradient with respect to x
+        (``b200bo_acq_value_grad``, DESIGN.md 4.10).  One device; host-side input transforms are not differentiated."""
+        if len(self.devices) != 1:
+            raise NotImplementedError("value_and_grad runs on one device (multi-device gradient sharding is not built)")
+        for g in self._gps:
+            g._ensure_device_fit()
+            if g.__dict__.get("_b200_xform", ("device", None))[0] == "host":
+                raise NotImplementedError("analytic gradients with a host-side kernel transform")
+        x = B.c_f64(np.asarray(x, dtype=np.float64).reshape(-1, self.dim))
+        specs = self._build_specs()
+        m = x.shape[0]
+        vals, grads = np.empty(m), np.empty((m, self.dim))
+        B.check(B.lib().b200bo_acq_value_grad(C.byref(specs[0]), B.as_dp(x), m, B.as_dp(vals), B.as_dp(grads)))
+        return vals, grads
+
     def argmin_topk(self, x, k):
         """Evaluate + np.argmin + k smallest (value, index) on the device(s)
         (R/bayes_opt/acquisition.py:312-317).  Returns (argmin index, min value, top-k indices)."""
@@ -373,7 +389,7 @@ class _LockstepEvaluator:
 
 
 def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, gtol=1e-5, eps=1e-8,
-                    maxfun=15000, maxiter=15000, maxls=20, run_paths=None):
+                    maxfun=15000, maxiter=15000, maxls=20, run_paths=None, grad=False):
     """All L-BFGS-B runs of ``_smart_minimize`` advanced TOGETHER by one Python thread around SciPy's own
     compiled core (``scipy.optimize._lbfgsb.setulb``): the driver loop of ``_minimize_lbfgsb``
     (SP/optimize/_lbfgsb_py.py:290-420: task handling, iteration / evaluation limits, warnflag -> success) and the
@@ -383,7 +399,11 @@ def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, 
     (measured: 2.4 ms per round for 10 runs).  Same core, same arithmetic, same iterates: x, fun, nit, nfev, status
     and success equal ``scipy.optimize.minimize(..., method="L-BFGS-B")`` bit for bit (tests/test_host_cpu.py).
     Raises ImportError / AttributeError when SciPy's private pieces are not the ones this was written against
-    (the caller then uses the thread-per-run driver)."""
+    (the caller then uses the thread-per-run driver).
+
+    grad=True: ``acq.value_and_grad(rows[, path_idx])`` supplies f and its analytic gradient, so a round is ONE row
+    per pending run and nfev counts one per evaluation; the driver is otherwise the same, and the results equal
+    ``scipy.optimize.minimize(fun, jac=True, method="L-BFGS-B")`` bit for bit."""
     from scipy.optimize import OptimizeResult
     from scipy.optimize import _lbfgsb_py as _sp
 
@@ -430,8 +450,24 @@ def _batched_lbfgsb(acq, seeds, bounds, maxcor=10, ftol=2.2204460492503131e-09, 
         r.done = False
         runs.append(r)
 
+    def evaluate_pending_grad(pending):
+        """f and the analytic gradient at r.x for every pending run: one row per run."""
+        kw = {}
+        if run_paths is not None:
+            kw["path_idx"] = np.array([r.path for r in pending], dtype=np.int32)
+        rows = np.vstack([r.x for r in pending])
+        fs, gs = acq.value_and_grad(rows, **kw)
+        for i, r in enumerate(pending):
+            r.f = float(fs[i])
+            r.g = np.array(gs[i], dtype=np.float64)
+            r.xe = rows[i].copy()
+            r.nfev += 1
+            r.njev += 1
+
     def evaluate_pending(pending):
         """f and the 2-point gradient at r.x for every pending run: one batch of (d+1) rows per run."""
+        if grad:
+            return evaluate_pending_grad(pending)
         if n_dev > 1:
             pending = sorted(pending, key=lambda r: r.dev)  # stable: rows of one device are contiguous
         blocks = []
@@ -512,16 +548,39 @@ def _on_path(acq, p, dim):
     return fun
 
 
-def lockstep_lbfgsb(acq, x_seeds, bounds, lockstep=True, run_paths=None):
+def _with_grad(acq, p, dim):
+    """``fun(x) -> (f, g)`` for scipy's jac=True over ``acq.value_and_grad`` (path p when given)."""
+
+    def fun(x):
+        rows = np.asarray(x, dtype=np.float64).reshape(1, dim)
+        kw = {} if p is None else {"path_idx": np.full(1, p, dtype=np.int32)}
+        f, g = acq.value_and_grad(rows, **kw)
+        return float(f[0]), np.array(g[0], dtype=np.float64)
+
+    return fun
+
+
+def lockstep_lbfgsb(acq, x_seeds, bounds, lockstep=True, run_paths=None, grad=False):
     """``[minimize(acq, seed, bounds=bounds, method="L-BFGS-B") for seed in x_seeds]`` (the loop at
     R/bayes_opt/acquisition.py:365-366) with the runs advanced in lockstep.  B200BO_LOCKSTEP=0 (or a
     single seed) selects the plain sequential loop.
 
     run_paths: None, or one path index per seed for a closure ``acq(rows, path_idx)`` over several sample paths
     (paths.PathBatchAcquisition): run r minimises path run_paths[r], and every merged call passes the path of each
-    of its rows."""
+    of its rows.
+
+    grad=True: the runs use the analytic gradient of ``acq.value_and_grad`` instead of the 2-point stencil (one row
+    per run and round); a single seed or B200BO_LOCKSTEP=0 runs ``minimize(fun, jac=True)`` on the same method."""
     seeds = [np.asarray(s, dtype=float) for s in x_seeds]
     dim = np.asarray(bounds).shape[0]
+    if grad:
+        if len(seeds) > 1 and lockstep and os.environ.get("B200BO_LOCKSTEP", "1") != "0":
+            try:
+                return _batched_lbfgsb(acq, seeds, bounds, run_paths=run_paths, grad=True)
+            except (ImportError, AttributeError, KeyError, TypeError):
+                pass  # SciPy's private L-BFGS-B pieces differ: one minimize(jac=True) per run
+        return [minimize(_with_grad(acq, None if run_paths is None else int(run_paths[i]), dim), s, jac=True,
+                         bounds=bounds, method="L-BFGS-B") for i, s in enumerate(seeds)]
     fun = [acq if run_paths is None else _on_path(acq, int(run_paths[i]), dim) for i in range(len(seeds))]
     if len(seeds) <= 1 or not lockstep or os.environ.get("B200BO_LOCKSTEP", "1") == "0":
         out = []

@@ -136,6 +136,19 @@ class PosteriorPaths:
                                                X.shape[0], B.as_dp(out)))
         return out
 
+    def grad_rows(self, X, path_idx):
+        """(vals (M,), grads (M, d)): row i of X on path path_idx[i], the value bit-equal to ``eval_rows`` and its
+        analytic gradient with respect to the row (``b200bo_paths_grad_rows``).  Host-side input transforms are not
+        differentiated."""
+        if self._xform[0] == "host":
+            raise NotImplementedError("analytic gradients with a host-side kernel transform")
+        X = self._candidates(X)
+        pidx = _row_paths(path_idx, X.shape[0], self.n_paths)
+        vals, grads = np.empty(X.shape[0]), np.empty((X.shape[0], self.dim))
+        B.check(B.lib().b200bo_paths_grad_rows(self._handle.ptr, B.as_dp(X), pidx.ctypes.data_as(C.POINTER(C.c_int32)),
+                                               X.shape[0], B.as_dp(vals), B.as_dp(grads)))
+        return vals, grads
+
     def argmin_topk(self, X, k):
         """Per path p: np.argmin and the k smallest (np.argsort order) of -path_p over the rows of X.
         Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
@@ -299,9 +312,18 @@ class PathAcquisition:
     def __init__(self, paths):
         self.paths = paths
         self.devices = paths.devices
+        if not hasattr(paths, "grad_rows"):
+            self.value_and_grad = None  # not offered: the refinement stays on the stencil
 
     def __call__(self, x):
         return -self.paths(x)[:, 0]
+
+    def value_and_grad(self, x):
+        """(vals (M,), grads (M, d)) of -path_0.  Offered over unconstrained paths only: a ConstrainedPaths merit is
+        piecewise and has no ``grad_rows``."""
+        x = np.asarray(x, dtype=np.float64).reshape(-1, self.paths.dim)
+        v, g = self.paths.grad_rows(x, np.zeros(x.shape[0], dtype=np.int32))
+        return -v, -g
 
     def argmin_topk(self, x, k):
         idx, val, tops = self.paths.argmin_topk(x, k)
@@ -322,9 +344,16 @@ class PathBatchAcquisition:
         self.paths = paths
         self.devices = paths.devices
         self.n_paths = paths.n_paths
+        if not hasattr(paths, "grad_rows"):
+            self.value_and_grad = None  # not offered: the refinement stays on the stencil
 
     def __call__(self, x, path_idx):
         return -self.paths.eval_rows(x, path_idx)
+
+    def value_and_grad(self, x, path_idx):
+        """(vals (M,), grads (M, d)) of -path_{path_idx[i]}(x_i); unconstrained paths only."""
+        v, g = self.paths.grad_rows(x, path_idx)
+        return -v, -g
 
     def path(self, p):
         p, dim = int(p), self.paths.dim

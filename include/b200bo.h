@@ -200,6 +200,15 @@ int b200bo_gp_predict_cov(b200bo_gp* gp, const double* Xc, int64_t m, double* mu
  * acq_neg[i] = -base_acq(mu_i, sigma_i) * prod_j p_j(x_i).  Xc: (m,d) host, acq_neg: (m,) host. */
 int b200bo_acq_eval(const b200bo_acq* spec, const double* Xc, int64_t m, double* acq_neg);
 
+/* Value and analytic input gradient of the same closure: val[i] = the value b200bo_acq_eval returns for row i,
+ * grad[i*d + j] = d val[i] / d x_ij, for every acquisition kind and 0 .. B200BO_MAX_GPS - 1 constraint GPs.
+ * Xc: (m,d) host, val: (m,), grad: (m,d) host.  Always runs on the fp64 small-batch kernels (meant for tens to
+ * hundreds of rows; a GP in fp32 precision takes the same fp64 path), on the device of the spec's GPs.  val is
+ * bit-equal to b200bo_acq_eval on the small-batch path (B200BO_SMALL_PATH=1) and, like the gradient, depends on the
+ * row only.  A dimension with B200BO_XFORM_ROUND has gradient 0; at a training input the Matern nu=0.5 kernel's kink
+ * contributes 0; where the variance is clamped to 0, d sigma is taken as 0; a NaN value gives a NaN gradient row. */
+int b200bo_acq_value_grad(const b200bo_acq* spec, const double* Xc, int64_t m, double* val, double* grad);
+
 /* Replaces AcquisitionFunction._random_sample_minimize's evaluation + selection
  * (R/bayes_opt/acquisition.py:311-317): evaluates the closure on Xc and returns
  *   best_idx/best_val = np.argmin semantics (first NaN wins; ties -> lowest index),
@@ -297,6 +306,11 @@ int b200bo_paths_eval(b200bo_paths* paths, const double* Xc, int64_t m, double* 
  * bit-equal to column path_idx[i] of b200bo_paths_eval on that row.  path_idx: (m,) host, every entry in [0, q), else
  * B200BO_ERR_ARG.  Costs one path per row instead of q. */
 int b200bo_paths_eval_rows(b200bo_paths* paths, const double* Xc, const int* path_idx, int64_t m, double* out);
+/* Row mode with the analytic input gradient: val[i] = path path_idx[i] at row i (bit-equal to
+ * b200bo_paths_eval_rows), grad[i*d + j] = d val[i] / d x_ij (0 for a B200BO_XFORM_ROUND dimension).  val: (m,),
+ * grad: (m,d) host.  path_idx as above. */
+int b200bo_paths_grad_rows(b200bo_paths* paths, const double* Xc, const int* path_idx, int64_t m, double* val,
+                           double* grad);
 /* Per path p, ranks -path_p on the rows of Xc with the semantics of b200bo_acq_argmin_topk: best_val[p], best_idx[p]
  * (np.argmin), topk_val[p*k + i], topk_idx[p*k + i] (np.argsort order).  Large batches are streamed in chunks. */
 int b200bo_paths_argmin_topk(b200bo_paths* paths, const double* Xc, int64_t m, int k, double* best_val,
