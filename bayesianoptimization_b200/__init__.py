@@ -10,7 +10,7 @@ Two layers:
     PosteriorPaths, ConstrainedPaths (posterior sample paths, resolved lazily)
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, ThompsonSampling,
-    ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, GPHedge, AcquisitionFunction,
+    ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, KrigingBeliever, GPHedge, AcquisitionFunction,
     ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
 """
 from . import _lib
@@ -26,7 +26,7 @@ _PLUGIN = {
     "ExpectedImprovement": "acquisition", "ProbabilityOfImprovement": "acquisition",
     "ConstantLiar": "acquisition", "GPHedge": "acquisition", "DeviceHooks": "acquisition",
     "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
-    "MaxValueEntropySearch": "acquisition", "suggest_batch": "acquisition",
+    "MaxValueEntropySearch": "acquisition", "suggest_batch": "acquisition", "KrigingBeliever": "acquisition",
     "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
 }
 

@@ -20,6 +20,8 @@ ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`
 (the paths of the target and the constraint GPs, ranked feasible-first); ``suggest_batch`` proposes q points at once
 from q paths (batch Thompson sampling).  ``MaxValueEntropySearch`` is the
 information-based policy: samples of the maximum from posterior paths, then a fused-kernel epilogue of mu and sigma.
+``KrigingBeliever`` gives UCB / EI / PoI / MES pending points and batches: the fitted GP is conditioned on the points in
+flight on the device, with its own mean as their targets.
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
 (gpr.B200GaussianProcessRegressor), ``fused.FusedAcquisition`` and the C ABI do not need it.
@@ -33,6 +35,7 @@ import numpy as np
 try:
     from bayes_opt import acquisition as _ref
     from bayes_opt.exception import ConstraintNotSupportedError as _ConstraintNotSupportedError
+    from bayes_opt.exception import TargetSpaceEmptyError as _TargetSpaceEmptyError
     from bayes_opt.util import ensure_rng as _ensure_rng
 except ImportError as e:  # pragma: no cover - depends on the environment
     raise ImportError(
@@ -362,15 +365,20 @@ def distinct_picks(picks, tops):
 
 def suggest_batch(optimizer, q):
     """q parameter dicts to probe next from a ``bayes_opt.BayesianOptimization`` whose acquisition function is a
-    (Constrained)ThompsonSampling: ``BayesianOptimization.suggest`` for a batch (R/bayes_opt/bayesian_optimization.py:
-    323-333).  With no registered point it returns ``optimizer.random_sample(q)``; otherwise
-    ``ThompsonSampling.suggest_batch`` with the optimizer's GP, target space and RandomState, each row converted with
-    ``array_to_params``.  Nothing new enters ``save_state``: q is an argument, not state."""
+    (Constrained)ThompsonSampling or a KrigingBeliever: ``BayesianOptimization.suggest`` for a batch
+    (R/bayes_opt/bayesian_optimization.py:323-333).  With no registered point it returns ``optimizer.random_sample(q)``;
+    otherwise the acquisition's ``suggest_batch`` with the optimizer's GP, target space and RandomState, each row
+    converted with ``array_to_params``.  For Thompson sampling nothing new enters ``save_state`` (q is an argument, not
+    state); a KrigingBeliever records the q points as dummies, which ``save_state`` carries."""
     acq = optimizer._acquisition_function
-    if not isinstance(acq, ThompsonSampling):
-        raise TypeError(f"suggest_batch needs a ThompsonSampling or ConstrainedThompsonSampling acquisition function, "
-                        f"got {type(acq).__name__}; for a batch of other acquisition functions use ConstantLiar")
-    q = _check_int("q", q, 1, B.MAX_PATHS)
+    if isinstance(acq, KrigingBeliever):
+        q = _check_int("q", q, 1)
+    elif isinstance(acq, ThompsonSampling):
+        q = _check_int("q", q, 1, B.MAX_PATHS)
+    else:
+        raise TypeError(f"suggest_batch needs a ThompsonSampling, ConstrainedThompsonSampling or KrigingBeliever "
+                        f"acquisition function, got {type(acq).__name__}; for a batch of other acquisition functions "
+                        f"use ConstantLiar")
     space = optimizer._space
     if len(space) == 0:
         return optimizer.random_sample(q)
@@ -384,7 +392,8 @@ MES_MAX_CANDIDATES = 2**16
 
 def mes_max_values(gp, paths, space, random_state, n_candidates, candidate_source="host_rng"):
     """Samples y*_k of the maximum of the target: per path k of ``paths`` (a PosteriorPaths of ``gp``),
-    y*_k = max(max of path k over n_candidates random points and X_train_, the largest registered target).
+    y*_k = max(max of path k over n_candidates random points and X_train_, the largest registered target) - on a GP
+    conditioned on pending points (``condition_on_pending``), over its registered rows only.
     The floor keeps every sample consistent with the data: the maximum is at least what has been observed.
     The candidates are ``space.random_sample(n_candidates, random_state)``, or in device_philox mode on a continuous
     space one 64-bit seed drawn as DeviceHooks._random_sample_minimize draws it (rows generated in the kernel)."""
@@ -392,8 +401,9 @@ def mes_max_values(gp, paths, space, random_state, n_candidates, candidate_sourc
         _, neg_max, *_ = paths.argmin_topk_philox(_philox_seed(random_state), space.bounds, n_candidates, 0)
     else:
         _, neg_max, _ = paths.argmin_topk(space.random_sample(n_candidates, random_state=random_state), 0)
-    best = np.maximum(-np.asarray(neg_max, dtype=np.float64), paths(gp.X_train_).max(axis=0))
-    return np.maximum(best, float(np.max(gp._y_raw)))
+    n_reg = gp.__dict__.get("_b200_conditioned")  # a GP conditioned on pending points: its registered rows only
+    best = np.maximum(-np.asarray(neg_max, dtype=np.float64), paths(gp.X_train_[:n_reg]).max(axis=0))
+    return np.maximum(best, float(np.max(gp._y_raw[:n_reg])))
 
 
 class MaxValueEntropySearch(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
@@ -506,10 +516,127 @@ class GPHedge(_ref.GPHedge):
         super().__init__([accelerate(a) for a in base_acquisitions], *args, **kwargs)
 
 
+class KrigingBeliever(_ref.ConstantLiar):
+    """Batches and asynchronous suggestions for UCB, EI, PoI and MES: the fixed-hyper-parameter counterpart of
+    ``ConstantLiar`` (Kriging believer: Ginsbourger, Le Riche & Carraro, "Kriging is well-suited to parallelize
+    optimization", 2010; DESIGN.md 4.11).
+
+    A pending point - suggested, not yet registered - is a dummy, with ConstantLiar's bookkeeping (inherited:
+    ``dummies``, their expiry once a registered point is within atol / rtol, and get/set_acquisition_params, so
+    ``save_state`` carries them).  Where ConstantLiar registers the dummies with a made-up target and refits the GP on
+    that space, this class fits the hyper-parameters on the registered data only and then conditions the fitted GP on
+    the dummies with the GP's own posterior mean as their targets (``condition_on_pending``: one O(N^2) row update per
+    point on the device).  The mean is unchanged; the standard deviation shrinks near the dummies, so the base
+    acquisition turns away from them.  ``strategy`` is accepted for ConstantLiar's parameter layout and not used.
+
+    ``suggest()``: the base acquisition's own ``suggest`` (its empty-space error, one ``i += 1``, its y_max, its
+    kappa / xi decay) with the GP conditioned on the unexpired dummies between the fit and the closure; the pick
+    becomes a dummy.  ``suggest_batch(..., q)``: q points from one call by greedy rounds on one candidate set.
+    Constraints raise ConstraintNotSupportedError, as ConstantLiar does."""
+
+    def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
+        if _device_kind(base_acquisition) is None and not isinstance(base_acquisition, MaxValueEntropySearch):
+            raise TypeError(f"KrigingBeliever needs an UpperConfidenceBound, ExpectedImprovement, "
+                            f"ProbabilityOfImprovement or MaxValueEntropySearch base acquisition, got "
+                            f"{type(base_acquisition).__name__}")
+        super().__init__(accelerate(base_acquisition), strategy, random_state, atol, rtol)
+
+    def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        return self._believe(gp, target_space, None, n_random, n_smart, fit_gp, random_state)
+
+    def suggest_batch(self, gp, target_space, q, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        """q points to probe next, as a (q, dim) array.  In this order:
+          1. the base acquisition's ``suggest`` accounting, once for the batch (one ``i += 1``, one kappa / xi decay;
+             y_max is the registered data's for every round), the hyper-parameter fit on the registered data, then
+             the conditioning on the unexpired dummies, on a fork of the GP with room for the batch;
+          2. the base closure on that GP - MES draws its y* samples here, once per batch;
+          3. ONE candidate set shared by every round: ``space.random_sample(max(n_random, n_smart), rs)``, or one
+             Philox seed in device_philox mode;
+          4. per round j = 0..q-1: the fused selection over that set on round j's GP, the refinement of its top
+             n_smart (the L-BFGS-B runs in lockstep; mixed-integer spaces: the reference's DE branch), the reference's
+             random-vs-refined rule, the duplicate rule of ``distinct_picks`` against the earlier picks, then the GP
+             is conditioned in place on the pick;
+          5. the q picks become dummies.
+        q = 1 without dummies returns the base acquisition's ``suggest`` point and leaves the RandomState as it does.
+        q is an integer >= 1."""
+        q = _check_int("q", q, 1)
+        return self._believe(gp, target_space, q, n_random, n_smart, fit_gp, random_state)
+
+    def _believe(self, gp, target_space, q, n_random, n_smart, fit_gp, random_state):
+        if len(target_space) == 0:
+            raise _TargetSpaceEmptyError("Cannot suggest a point without previous samples: register a point first "
+                                         "(target_space.random_sample() / target_space.probe()).")
+        if target_space.constraint is not None:
+            raise _ConstraintNotSupportedError(f"{type(self).__name__} does not support constrained optimization: "
+                                               "the target space has a constraint")
+        self._remove_expired_dummies(target_space)
+        base = self.base_acquisition
+        pending = np.asarray(self.dummies, dtype=np.float64).reshape(len(self.dummies), target_space.dim)
+        round_gp = []
+
+        def get_acq(gp, constraint=None):  # between the base's fit and its closure
+            gp = _as_b200_gp(gp)
+            if len(pending) or (q or 1) > 1:
+                gp = gp.condition_on_pending(pending, extra_rows=q or 0)
+            round_gp.append(gp)
+            return type(base)._get_acq(base, gp=gp, constraint=constraint)
+
+        def acq_min(acq, space, random_state, n_random=10_000, n_smart=10):
+            return self._rounds(acq, round_gp[0], space, random_state, n_random, n_smart, q)
+
+        base._get_acq = get_acq
+        if q is not None:
+            base._acq_min = acq_min
+        try:
+            x = base.suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
+                             random_state=_ensure_rng(random_state))
+        finally:
+            base.__dict__.pop("_get_acq", None)
+            base.__dict__.pop("_acq_min", None)
+        if q is None:
+            self.dummies.append(x)
+        else:
+            self.dummies.extend(np.array(r) for r in x)
+        return x
+
+    def _rounds(self, acq, gp, space, random_state, n_random, n_smart, q):
+        if n_random == 0 and n_smart == 0:
+            raise ValueError("Either n_random or n_smart needs to be greater than 0.")
+        base = self.base_acquisition
+        n = max(n_random, n_smart)
+        philox = base.b200_candidate_source == "device_philox" and all(space.continuous_dimensions)
+        philox = philox and n_smart <= B.MAX_TOPK
+        if philox:
+            seed = _philox_seed(random_state)
+        else:
+            x_tries = space.random_sample(n, random_state=random_state)  # the reference's RNG stream
+        picks = []
+        for j in range(q):
+            # the random stage of DeviceHooks._random_sample_minimize on the shared set
+            if philox:
+                _, min_r, x_r, _, tops = acq.argmin_topk_philox(seed, space.bounds, n, n_smart)
+            elif n_smart <= B.MAX_TOPK:
+                idx, min_r, top = acq.argmin_topk(x_tries, n_smart)
+                x_r, tops = x_tries[idx], x_tries[top]
+            else:  # more seeds than the device selection holds: numpy selection on the device values
+                ys = acq(x_tries)
+                x_r, min_r, tops = x_tries[ys.argmin()], ys.min(), x_tries[np.argsort(ys)[:n_smart]]
+            x = x_r
+            if n_smart:
+                x_s, min_s = base._smart_minimize(acq, space, x_seeds=tops, random_state=random_state)
+                if min_r > min_s:  # the reference's choice (R/bayes_opt/acquisition.py:267-272)
+                    x = x_s
+            x = distinct_picks(picks + [x], [[]] * len(picks) + [tops])[-1]
+            picks.append(np.asarray(x, dtype=np.float64))
+            if j < q - 1:
+                gp.condition_on_pending(picks[-1][None])  # in place: the fork has room for the batch
+        return np.asarray(picks, dtype=np.float64)
+
+
 # isinstance(x, b200.AcquisitionFunction) holds for every acquisition of this module, as
 # isinstance(x, bayes_opt.acquisition.AcquisitionFunction) does in the reference (abc virtual subclasses:
 # the concrete classes keep the reference's MRO).
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, ConstantLiar, GPHedge,
-             ThompsonSampling, ConstrainedThompsonSampling, MaxValueEntropySearch):
+             ThompsonSampling, ConstrainedThompsonSampling, MaxValueEntropySearch, KrigingBeliever):
     AcquisitionFunction.register(_cls)
 del _cls

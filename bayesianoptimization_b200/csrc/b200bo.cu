@@ -131,6 +131,7 @@ struct b200bo_gp {
     std::vector<int> xform;      // host copy (d) or empty
     std::vector<double> ystar;   // MES samples of the maximum (b200bo_gp_set_max_values), or empty
     DevBuf X, Xs, y, K, L, W, WT, T, alphav, v1, v2, ls, xf, info, part;
+    DevBuf tscratch;  // b200bo_gp_condition: t = W^T l of the row update (np), so that alpha_ survives it
     // predict-side scratch (used when this handle is gps[0] of a call)
     DevBuf pscratch, xc, out_acq, out_mu, out_sd, sel, clamp;
     // small-batch path scratch (per GP) + work-unit tables (rebuilt when np changes)
@@ -293,7 +294,7 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
                       &gp->s_vsum, &gp->s_usum, &gp->s_partial_u, &gp->s_gpart, &gp->s_unit_u, &gp->s_rb_u, &gp->out_grad,
                       &gp->tc_linv, &gp->pad_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
                       &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside, &gp->prune_key, &gp->prune_idx,
-                      &gp->prune_tmp, &gp->prune_ctl};
+                      &gp->prune_tmp, &gp->prune_ctl, &gp->tscratch};
     for (DevBuf* b : bufs) b->release();
     if (gp->stream) cudaStreamDestroy(gp->stream);
     if (gp->fgraph_exec) cudaGraphExecDestroy(gp->fgraph_exec);
@@ -775,16 +776,13 @@ extern "C" int b200bo_gp_fit(b200bo_gp* gp, const double* X, const double* y, in
     return B200BO_OK;
 }
 
-// Append one training point at the hyper-parameters of the last fit, O(N^2) (SURVEY.md 8f rank 3).
-// Falls outside the padded capacity (n == np) -> B200BO_ERR_STATE: the caller refits from scratch.
-extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new, int64_t* info) {
-    if (!gp || !x_new) return set_err(B200BO_ERR_ARG, "NULL argument");
-    if (!gp->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
-    if (gp->replica) return set_err(B200BO_ERR_STATE, "handle is a predict-only replica: append to the source and replicate again");
-    if (gp->n >= gp->np) return set_err(B200BO_ERR_STATE, "no padding slack left (n == np): refit");
-    CU(cudaSetDevice(gp->device));
+// Row n of the O(N^2) factor update at the hyper-parameters of the last fit, shared by b200bo_gp_append and
+// b200bo_gp_condition: row n of X / Xs, row and column n of K, row n of L (pivot checked) and of L^-1 (W and WT).
+// tvec: n-entry device scratch.  believer (nullable, device): receives k(x, X) . alpha_ in normalised units, computed
+// from the new K row right after it is built - before anything writes tvec, which may be alpha_ itself.
+// *finfo = 0, or the failing pivot (1-based) and rows n of K / L are garbage.  gp->n is the caller's to advance.
+static int append_factor_row(b200bo_gp* gp, const double* x_new, double* tvec, double* believer, int* finfo) {
     const int n = (int)gp->n, np = gp->np, d = gp->d;
-    if (info) *info = 0;
     int rc;
     if ((rc = gp->xc.reserve(sizeof(double) * B200BO_MAX_DIM))) return rc;
     CU(cudaMemcpy(gp->xc.p, x_new, sizeof(double) * d, cudaMemcpyHostToDevice));
@@ -792,10 +790,13 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     const int* xf = gp->xform.empty() ? nullptr : gp->xf.as<int>();
     double* kvec = gp->v1.as<double>();
     double* lvec = gp->v2.as<double>();
-    double* tvec = gp->alphav.as<double>();  // alpha_ is recomputed below; reuse as scratch
     if (n > 0) {
         append_krow_kernel<<<(n + 127) / 128, 128>>>(gp->xc.as<double>(), gp->ls.as<double>(), xf, gp->Xs.as<double>(),
                                                      gp->X.as<double>(), kvec, n, d, gp->family, gp->nu, gp->constv);
+        if (believer) {  // mu_norm(x) = k^T alpha_: one warp, fixed-order reduction
+            gemv_rows_kernel<<<1, 32>>>(kvec, np, gp->alphav.as<double>(), believer, 1, n, 0);
+            LAUNCHED();
+        }
         const int wpb = 8;
         dim3 blk(32 * wpb), grd((n + wpb - 1) / wpb);
         gemv_rows_kernel<<<grd, blk>>>(gp->W.as<double>(), np, kvec, lvec, n, n, 1);   // l = W k
@@ -804,16 +805,34 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
         gemv_rows_kernel<<<grd, blk>>>(gp->WT.as<double>(), np, lvec, tvec, n, n, 2);  // t = W^T l
         for (int i = 0; i < 4; ++i) LAUNCHED();
     }
+    *finfo = 0;
+    CU(cudaMemcpy(finfo, gp->info.p, sizeof(int), cudaMemcpyDeviceToHost));
+    if (*finfo != 0) return B200BO_OK;
+    append_winv_kernel<<<(n + 1 + 127) / 128, 128>>>(gp->W.as<double>(), gp->WT.as<double>(), tvec,
+                                                     gp->part.as<double>(), n, np);
+    LAUNCHED();
+    return B200BO_OK;
+}
+
+// Append one training point at the hyper-parameters of the last fit, O(N^2) (SURVEY.md 8f rank 3).
+// Falls outside the padded capacity (n == np) -> B200BO_ERR_STATE: the caller refits from scratch.
+extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new, int64_t* info) {
+    if (!gp || !x_new) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!gp->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
+    if (gp->replica) return set_err(B200BO_ERR_STATE, "handle is a predict-only replica: append to the source and replicate again");
+    if (gp->n >= gp->np) return set_err(B200BO_ERR_STATE, "no padding slack left (n == np): refit");
+    CU(cudaSetDevice(gp->device));
+    const int n = (int)gp->n;
+    if (info) *info = 0;
+    int rc;
     int finfo = 0;
-    CU(cudaMemcpy(&finfo, gp->info.p, sizeof(int), cudaMemcpyDeviceToHost));
+    // alpha_ is recomputed below; reuse it as scratch
+    if ((rc = append_factor_row(gp, x_new, gp->alphav.as<double>(), nullptr, &finfo))) return rc;
     if (finfo != 0) {
         gp->fitted = false;  // row n of K/L is garbage now
         if (info) *info = finfo;
         return set_err(B200BO_ERR_NOT_PD, "%d-th leading minor of the array is not positive definite", finfo);
     }
-    append_winv_kernel<<<(n + 1 + 127) / 128, 128>>>(gp->W.as<double>(), gp->WT.as<double>(), tvec,
-                                                     gp->part.as<double>(), n, np);
-    LAUNCHED();
     // targets: new normalisation statistics, alpha_ = K^-1 y
     gp->y_raw.push_back(y_new);
     const int64_t nn = n + 1;
@@ -840,6 +859,121 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     gp->pad_valid = false;
     if ((rc = solve_alpha(gp))) return rc;
     CU(cudaDeviceSynchronize());
+    return B200BO_OK;
+}
+
+// Kriging believer (DESIGN.md 4.11): row n gets the target mu_norm(x) = k(x, X)^T alpha_, so K' [alpha_; 0] =
+// [y; mu_norm(x)] and alpha_ extends by a zero - no solve, the mean is unchanged everywhere, only K, L, L^-1 grow.
+extern "C" int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, double* mu_out) {
+    if (!gp || (p > 0 && !Xp)) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (p < 0) return set_err(B200BO_ERR_ARG, "p=%lld must be >= 0", (long long)p);
+    if (!gp->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
+    if (gp->replica)
+        return set_err(B200BO_ERR_STATE, "handle is a predict-only replica: condition the source or a fork of it");
+    if (p > gp->np - gp->n)
+        return set_err(B200BO_ERR_STATE, "no padding slack for %lld rows (n=%lld, np=%d): fork with extra_rows",
+                       (long long)p, gp->n, gp->np);
+    const int d = gp->d;
+    for (int64_t i = 0; i < p * d; ++i)
+        if (!std::isfinite(Xp[i])) return set_err(B200BO_ERR_ARG, "Input X contains NaN or infinity.");
+    CU(cudaSetDevice(gp->device));
+    NvtxRange nvtx_range("b200bo:condition");
+    int rc;
+    if ((rc = gp->tscratch.reserve(sizeof(double) * gp->np))) return rc;
+    for (int64_t r = 0; r < p; ++r) {
+        const int n = (int)gp->n;
+        double* yn = gp->y.as<double>() + n;  // the believer target lands in y's padding slot n
+        int finfo = 0;
+        if ((rc = append_factor_row(gp, Xp + r * d, gp->tscratch.as<double>(), yn, &finfo))) return rc;
+        if (finfo != 0) {
+            gp->fitted = false;  // row n of K/L is garbage now
+            return set_err(B200BO_ERR_NOT_PD, "%d-th leading minor of the array is not positive definite", finfo);
+        }
+        double mu_norm = 0.0;
+        CU(cudaMemcpy(&mu_norm, yn, sizeof(double), cudaMemcpyDeviceToHost));
+        CU(cudaMemset(gp->alphav.as<double>() + n, 0, sizeof(double)));  // alpha_ = [alpha_; 0]
+        const double mu = gp->y_std * mu_norm + gp->y_mean;  // data units, as the predict kernels form the mean
+        gp->y_norm.push_back(mu_norm);
+        gp->y_raw.push_back(mu);
+        if (mu_out) mu_out[r] = mu;
+        gp->n = n + 1;
+        gp->tc_valid = false;
+        gp->pad_valid = false;
+    }
+    CU(cudaDeviceSynchronize());
+    return B200BO_OK;
+}
+
+static int fork_into(const b200bo_gp* src, int64_t extra_rows, b200bo_gp* dst) {
+    dst->n = src->n;
+    dst->d = src->d;
+    dst->np = round_up(src->n + extra_rows, kPad);
+    dst->family = src->family;
+    dst->nu = src->nu;
+    dst->constv = src->constv;
+    dst->jitter = src->jitter;
+    dst->noise = src->noise;
+    dst->y_mean = src->y_mean;
+    dst->y_std = src->y_std;
+    dst->y_norm = src->y_norm;
+    dst->y_raw = src->y_raw;
+    dst->normalize = src->normalize;
+    dst->xform = src->xform;
+    dst->ystar = src->ystar;
+    dst->precision = src->precision;
+    const size_t n = src->n, d = src->d, np0 = src->np, np = dst->np;
+    int rc;
+    DevBuf* vecs[] = {&dst->X, &dst->Xs, &dst->y, &dst->alphav, &dst->v1, &dst->v2};
+    const size_t vec_len[] = {np * d, np * d, np, np, np, np};
+    for (int i = 0; i < 6; ++i) {
+        if ((rc = vecs[i]->reserve(sizeof(double) * vec_len[i]))) return rc;
+        CU(cudaMemset(vecs[i]->p, 0, sizeof(double) * vec_len[i]));
+    }
+    if ((rc = dst->ls.reserve(sizeof(double) * B200BO_MAX_DIM))) return rc;
+    if ((rc = dst->xf.reserve(sizeof(int) * B200BO_MAX_DIM))) return rc;
+    if ((rc = dst->info.reserve(sizeof(int)))) return rc;
+    if ((rc = dst->part.reserve(sizeof(double) * 64))) return rc;
+    CU(cudaMemcpy(dst->X.p, src->X.p, sizeof(double) * n * d, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(dst->Xs.p, src->Xs.p, sizeof(double) * n * d, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(dst->y.p, src->y.p, sizeof(double) * n, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(dst->alphav.p, src->alphav.p, sizeof(double) * n, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(dst->ls.p, src->ls.p, sizeof(double) * B200BO_MAX_DIM, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(dst->xf.p, src->xf.p, sizeof(int) * B200BO_MAX_DIM, cudaMemcpyDeviceToDevice));
+    struct Mat {
+        DevBuf* to;
+        const DevBuf* from;
+    } mats[] = {{&dst->K, &src->K}, {&dst->L, &src->L}, {&dst->W, &src->W}, {&dst->WT, &src->WT}};
+    const dim3 blk(32, 8), grd((unsigned)(np / 32), (unsigned)(np / 32));
+    for (const Mat& m : mats) {
+        if ((rc = m.to->reserve(sizeof(double) * np * np))) return rc;
+        repitch_identity_kernel<<<grd, blk>>>(m.from->as<double>(), (int)np0, m.to->as<double>(), (int)np);
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    CU(cudaDeviceSynchronize());
+    dst->fitted = true;
+    return B200BO_OK;
+}
+
+// A full, appendable copy of a fitted handle with capacity for extra_rows more rows (DESIGN.md 4.11).
+extern "C" int b200bo_gp_fork(const b200bo_gp* src, int64_t extra_rows, b200bo_gp** out) {
+    if (!src || !out) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (extra_rows < 0) return set_err(B200BO_ERR_ARG, "extra_rows=%lld must be >= 0", (long long)extra_rows);
+    if (!src->fitted) return set_err(B200BO_ERR_STATE, "source GP handle is not fitted");
+    if (src->replica)
+        return set_err(B200BO_ERR_STATE, "a predict-only replica holds no K / L: fork the source handle");
+    if (src->n + extra_rows > 38000)
+        return set_err(B200BO_ERR_ARG, "n + extra_rows = %lld too large (<= 38000)", (long long)(src->n + extra_rows));
+    b200bo_gp* dst = nullptr;
+    int rc;
+    if ((rc = b200bo_gp_create(&dst, src->device))) return rc;
+    NvtxRange nvtx_range("b200bo:fork");
+    if ((rc = fork_into(src, extra_rows, dst))) {
+        cudaGetLastError();  // an out-of-memory cudaMalloc leaves its error behind
+        b200bo_gp_destroy(dst);
+        return rc;
+    }
+    *out = dst;
     return B200BO_OK;
 }
 

@@ -794,6 +794,19 @@ __global__ void append_winv_kernel(double* __restrict__ W, double* __restrict__ 
     }
 }
 
+// Re-pitch of an np_src x np_src matrix into an np_dst x np_dst one (np_dst >= np_src, both multiples of 32), in one
+// pass: dst[i][j] = src[i][j] inside the source block, the identity outside it - the padding invariant of K, L, L^-1
+// and its transpose.  32x8 threads per 32x32 tile, 4 rows each; every store is a coalesced 256-byte row segment.
+__global__ void __launch_bounds__(256)
+repitch_identity_kernel(const double* __restrict__ src, int np_src, double* __restrict__ dst, int np_dst) {
+    const int j = blockIdx.x * 32 + threadIdx.x;
+    for (int r = threadIdx.y; r < 32; r += 8) {
+        const int i = blockIdx.y * 32 + r;
+        dst[(size_t)i * np_dst + j] =
+            (i < np_src && j < np_src) ? src[(size_t)i * np_src + j] : (i == j ? 1.0 : 0.0);
+    }
+}
+
 constexpr int kMaxTheta = B200BO_MAX_DIM + 1;
 
 // gradient factor such that dk/dlog(l_t) = gcommon * D_t  (D_t = scaled squared difference)

@@ -286,18 +286,34 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         return state
 
     def _ensure_device_fit(self):
-        """After unpickling / deepcopy the device factor is gone: rebuild it at kernel_.theta."""
+        """After unpickling / deepcopy the device factor is gone: rebuild it at kernel_.theta (a GP conditioned on
+        pending points: the fit on the registered rows, then the conditioning on the pending ones)."""
         if not self.__dict__.get("_b200_device_fitted", False):
             if not hasattr(self, "X_train_"):
                 raise B.B200Error("GP is not fitted")
-            self._device_fit(parse_kernel(self.kernel_))
+            n_reg = self.__dict__.get("_b200_conditioned")
+            if n_reg is None:
+                self._device_fit(parse_kernel(self.kernel_))
+                return
+            self._device_fit(parse_kernel(self.kernel_), self.X_train_[:n_reg], self._y_raw[:n_reg])
+            pending = B.c_f64(self.X_train_[n_reg:])
+            if -(-n_reg // 128) * 128 < self.X_train_.shape[0]:  # no slack for the pending rows: fork
+                self.__dict__["_b200_handle"] = self._fork_handle(pending.shape[0])
+            B.check(B.lib().b200bo_gp_condition(self._handle().ptr, B.as_dp(pending), pending.shape[0], None))
 
-    def _device_fit(self, ek: EngineKernel):
+    def _fork_handle(self, extra_rows):
+        h = _Handle.__new__(_Handle)
+        h.ptr = C.c_void_p()
+        B.check(B.lib().b200bo_gp_fork(self._handle().ptr, int(extra_rows), C.byref(h.ptr)))
+        return h
+
+    def _device_fit(self, ek: EngineKernel, X_train=None, y_raw=None):
         h = self._handle()
-        y = B.c_f64(self._y_raw)
-        mode, arg = resolve_transform(self.kernel_, self.X_train_.shape[1])
+        X_train = self.X_train_ if X_train is None else X_train
+        y = B.c_f64(self._y_raw if y_raw is None else y_raw)
+        mode, arg = resolve_transform(self.kernel_, X_train.shape[1])
         self.__dict__["_b200_xform"] = (mode, arg)
-        X = apply_transform(mode, arg, B.c_f64(self.X_train_))
+        X = apply_transform(mode, arg, B.c_f64(X_train))
         d = X.shape[1]
         codes = arg if mode == "device" else None
         L = B.lib()
@@ -401,6 +417,7 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         if np.iterable(self.alpha):
             raise NotImplementedError("per-sample alpha is not supported by the device engine")
         self.n_features_in_ = X.shape[1]
+        self.__dict__.pop("_b200_conditioned", None)
         ek = parse_kernel(self.kernel_)  # raises NotImplementedError for unsupported kernels
         if ek.length_scale.size not in (1, X.shape[1]):
             raise ValueError("Anisotropic kernel must have the same number of dimensions as data "
@@ -691,6 +708,60 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
                 warnings.warn("Predicted variances smaller than 0. Setting those variances to 0.")
             return mu, sd
         return mu
+
+    # ---- Kriging believer --------------------------------------------------------------------
+    def condition_on_pending(self, X, extra_rows=0):
+        """The GP conditioned on pending points ``X`` (n_pending, d) whose values are not known yet, each with the
+        Kriging-believer target: the posterior mean mu(x) (Ginsbourger, Le Riche & Carraro 2010; DESIGN.md 4.11).
+        The hyper-parameters and the y normalisation stay those of the fit, so the posterior mean is unchanged
+        everywhere and the standard deviation shrinks near the pending points - the whole effect of the fantasy.
+        One O(N^2) row update per point (``b200bo_gp_condition``); nothing is refitted.
+
+        Returns a fitted regressor: ``X_train_`` is the augmented set, ``y_train_`` / ``_y_raw`` end with the believer
+        values, ``kernel_`` is this GP's.  On a GP that is not itself conditioned, the result is a new object on a
+        fork of the device state (``b200bo_gp_fork``) and this GP is untouched; on a conditioned GP the call
+        conditions in place (and returns self) while the device capacity holds the rows, and forks otherwise.
+        ``extra_rows`` reserves capacity in a fork for that many later in-place calls.  Multi-device GPs and
+        host-side (categorical) input transforms raise NotImplementedError; a non-positive pivot raises
+        np.linalg.LinAlgError, as ``fit`` does."""
+        X = np.array(X, dtype=np.float64)
+        if X.ndim == 1:
+            X = X.reshape(1, -1)
+        if X.ndim != 2 or not hasattr(self, "X_train_") or X.shape[1] != self.X_train_.shape[1]:
+            raise ValueError("X must be (n_pending, d) with the d of a fitted GP")
+        if not np.all(np.isfinite(X)):
+            raise ValueError("Input contains NaN or infinity.")
+        if isinstance(extra_rows, bool) or not isinstance(extra_rows, (int, np.integer)) or extra_rows < 0:
+            raise ValueError(f"extra_rows must be an integer >= 0, got {extra_rows!r}")
+        if len(self.device_list()) > 1:
+            raise NotImplementedError("conditioning on pending points runs on one device: the GP is multi-device")
+        self._ensure_device_fit()
+        if self.__dict__.get("_b200_xform", ("device", None))[0] == "host":
+            raise NotImplementedError("conditioning on pending points with a host-side (categorical) kernel transform")
+        n, p = self.X_train_.shape[0], X.shape[0]
+        n_reg = self.__dict__.get("_b200_conditioned")
+        mu = np.empty(p)
+        Xc = B.c_f64(X)
+        L = B.lib()
+        out = self
+        # in place on a conditioned GP; B200BO_ERR_STATE (checked before any work) means no slack left: fork
+        rc = L.b200bo_gp_condition(self._handle().ptr, B.as_dp(Xc), p, B.as_dp(mu)) if n_reg is not None else B.ERR_STATE
+        if rc == B.ERR_STATE:
+            out = type(self).__new__(type(self))
+            skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha")
+            out.__dict__.update({k: v for k, v in self.__dict__.items() if k not in skip})
+            out.__dict__["_b200_handle"] = self._fork_handle(p + int(extra_rows))
+            out.__dict__["_b200_conditioned"] = n if n_reg is None else n_reg
+            rc = L.b200bo_gp_condition(out._handle().ptr, B.as_dp(Xc), p, B.as_dp(mu))
+        if rc != B.OK:
+            out.__dict__["_b200_device_fitted"] = False  # rebuilt from X_train_ on the next use
+        B.check(rc)
+        out.X_train_ = np.vstack([self.X_train_, Xc])
+        out.y_train_ = np.concatenate([self.y_train_, (mu - self._y_train_mean) / self._y_train_std])
+        out._y_raw = np.concatenate([self._y_raw, mu])
+        out.__dict__.pop("_b200_L", None)
+        out.__dict__.pop("_b200_alpha", None)
+        return out
 
     def _device_candidates(self, X):
         """Candidates as the device sees them (host-side transform applied when the kernel carries

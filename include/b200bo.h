@@ -163,6 +163,29 @@ int b200bo_gp_fit(b200bo_gp* gp, const double* X, const double* y, int64_t n, in
  * B200BO_ERR_STATE when the padded capacity is exhausted (caller refits), B200BO_ERR_NOT_PD as fit. */
 int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new, int64_t* info);
 
+/* ---- Kriging believer: conditioning on pending points (DESIGN.md 4.11) ----------------------
+ * (Ginsbourger, Le Riche & Carraro, "Kriging is well-suited to parallelize optimization", 2010.)  No counterpart in
+ * the reference, whose ConstantLiar refits the GP on dummy targets (R/bayes_opt/acquisition.py:1058-1148).
+ *
+ * b200bo_gp_fork: a new, full and appendable handle on src's device (not a predict-only replica) holding src's fitted
+ * state - X / Xs, K, L, L^-1 and its transpose, alpha_, y, the y statistics, the transform, the hyper-parameters, the
+ * precision and the MES samples - with capacity np' = ceil((n + extra_rows)/128)*128 rows.  The N^2 matrices are
+ * re-pitched from np to np' with identity padding.  Extra device memory: about 4 * 8 * np'^2 bytes, plus the stage
+ * images of L^-1 the predict kernels build on first use.  np' == np: predictions, acquisitions and selections are
+ * bit-equal to src's; np' > np: equal to round-off.  The fork's training set is for conditioning / appending:
+ * b200bo_gp_lml on it needs b200bo_gp_set_data first.  Out of memory: B200BO_ERR_CUDA; src not fitted or a replica:
+ * B200BO_ERR_STATE.  n + extra_rows <= 38000. */
+int b200bo_gp_fork(const b200bo_gp* src, int64_t extra_rows, b200bo_gp** out);
+/* Conditions gp in place on the p rows of Xp ((p,d) host), one O(N^2) row update each, at the hyper-parameters and y
+ * statistics of the last fit.  Row r's target is the believer value mu(Xp[r]) of the GP conditioned on rows 0..r-1,
+ * which equals the mean of the GP before the call (alpha_ extends by zeros: K'[alpha_; 0] = [y; k^T alpha_]), so the
+ * posterior mean does not change anywhere and only the variance shrinks near the rows.  mu_out (nullable, (p,) host)
+ * receives the believer values in data units; they also become the rows' targets (b200bo_gp_append on the result
+ * treats them as data).  Errors: not fitted or a replica, or p > np - n (no slack: fork first) -> B200BO_ERR_STATE;
+ * non-finite Xp -> B200BO_ERR_ARG; a non-positive pivot -> B200BO_ERR_NOT_PD with the 1-based index of the failing
+ * row in the message (LAPACK dpotrf convention), and the handle is left unfitted. */
+int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, double* mu_out);
+
 /* Replaces GaussianProcessRegressor.log_marginal_likelihood(theta, eval_gradient)
  * (SK/gaussian_process/_gpr.py:541-656) on the training set of the last b200bo_gp_set_data /
  * b200bo_gp_fit call.  grad (nullable) receives d LML / d log(theta): [log const_value if
