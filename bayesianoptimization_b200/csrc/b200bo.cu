@@ -152,10 +152,17 @@ struct b200bo_gp {
     // selection-only pruning: bound keys / local indices (two buffers each for the radix sort), its temp storage and
     // the control words of predict_acq16_kernel's prune mode
     DevBuf prune_key, prune_idx, prune_tmp, prune_ctl;
+    // its refine stages: K* alpha_ per candidate from the bound pass, the survivor list, the per-row-block partials
+    // and arrival counters of predict_units_kernel
+    DevBuf prune_mu, prune_surv, prune_part, prune_arrive;
     // candidates of the last call (chunked: all chunks) and those of them evaluated outside the prune mode; the
     // prune mode counts its own in prune_ctl[2] (prune_counted)
     long long stat_total = 0, stat_direct = 0;
     bool prune_counted = false;
+    // stage boundaries of the last pruned launch on its stream: after the bound pass, the sort, the lead, refine and
+    // final stages (b200bo_last_prune_stage_ms; the stages start at ev0 and the tile kernel ends at ev1)
+    cudaEvent_t ev_stage[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    bool stage_timed = false, stage_refined = false;
     DevBuf pbounds, prow;   // throughput mode: Philox bounds (lo, span) / regenerated winner rows
     bool replica = false;   // predict-only copy made by b200bo_gp_replicate
     // look-ahead Cholesky: bulk stream, chain/bulk events, copy of the next diagonal step's panel block
@@ -226,6 +233,7 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaDeviceGetAttribute(&gp->sm_count, cudaDevAttrMultiProcessorCount, gp->device));
     CU(cudaEventCreate(&gp->ev0));
     CU(cudaEventCreate(&gp->ev1));
+    for (cudaEvent_t& e : gp->ev_stage) CU(cudaEventCreate(&e));
     CU(cudaFuncSetAttribute(predict_acq_kernel<PREDICT_IMPL_DFMA, false>,
                             cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_acq_kernel<PREDICT_IMPL_DFMA, true>,
@@ -254,6 +262,10 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
+    CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_units_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_units_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
@@ -294,7 +306,8 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
                       &gp->s_vsum, &gp->s_usum, &gp->s_partial_u, &gp->s_gpart, &gp->s_unit_u, &gp->s_rb_u, &gp->out_grad,
                       &gp->tc_linv, &gp->pad_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
                       &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside, &gp->prune_key, &gp->prune_idx,
-                      &gp->prune_tmp, &gp->prune_ctl, &gp->tscratch};
+                      &gp->prune_tmp, &gp->prune_ctl, &gp->prune_mu, &gp->prune_surv, &gp->prune_part,
+                      &gp->prune_arrive, &gp->tscratch};
     for (DevBuf* b : bufs) b->release();
     if (gp->stream) cudaStreamDestroy(gp->stream);
     if (gp->fgraph_exec) cudaGraphExecDestroy(gp->fgraph_exec);
@@ -305,6 +318,8 @@ extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
     gp->upload.release();
     if (gp->ev0) cudaEventDestroy(gp->ev0);
     if (gp->ev1) cudaEventDestroy(gp->ev1);
+    for (cudaEvent_t e : gp->ev_stage)
+        if (e) cudaEventDestroy(e);
     if (g_last_timed == gp) g_last_timed = nullptr;
     delete gp;
 }
@@ -1293,6 +1308,69 @@ static bool prune_enabled() {
     return !(e && e[0] == '0');
 }
 
+// Leading row blocks of the refine stages of pruning (DESIGN.md 4.9), or 0 when the launch keeps to the tile kernel:
+// B200BO_PRUNE_REFINE=0 (read per call, for A/B measurements), fewer than 8 row blocks of L^-1 (the refined bound
+// would cost a sizeable part of the exact value) or too few tiles for a lead stage.  B200BO_PRUNE_REFINE_BLOCKS (default
+// 4) is clamped to an eighth of the row blocks.
+static int prune_refine_blocks(int np, long long ntiles) {
+    const char* e = getenv("B200BO_PRUNE_REFINE");
+    const int nb = np / PBM;
+    if ((e && e[0] == '0') || nb < 8 || ntiles < 4 * kLeadTiles) return 0;
+    const char* eb = getenv("B200BO_PRUNE_REFINE_BLOCKS");
+    int b = eb && *eb ? atoi(eb) : 4;
+    b = b < 1 ? 1 : b;
+    return b < nb / 8 ? b : nb / 8;
+}
+
+// control words of a launch with refine stages: the tile kernel starts behind the lead tiles, and the lead stage sees
+// the k-th key carried into the launch
+__global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
+    ctl[kCtlTile] = ctl[kCtlRefTile] = kLeadTiles;
+    ctl[kCtlSurv] = ctl[kCtlUnit] = ctl[kCtlUnitFinal] = 0ull;
+    ctl[kCtlKthLead] = ctl[kCtlKth];
+}
+
+// The lead, refine and final stages of a pruned launch (predict16.cuh), between prune_prepare and the tile kernel.
+static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg, int blocks, bool resume,
+                               cudaStream_t stream) {
+    const int nb = P.gp[0].np / PBM, grid = g0->sm_count;
+    int rc;
+    if ((rc = g0->prune_surv.reserve(sizeof(int) * (size_t)kRefineMaxTiles * PBN))) return rc;
+    if ((rc = g0->prune_part.reserve(sizeof(double) * (size_t)kUnitSlots * nb * 32 * PBN))) return rc;
+    if ((rc = g0->prune_arrive.reserve(sizeof(unsigned) * kUnitSlots))) return rc;
+    unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
+    if (!resume) CU(cudaMemsetAsync(ctl + kCtlRefined, 0, sizeof(unsigned long long), stream));
+    CU(cudaMemsetAsync(g0->prune_arrive.p, 0, sizeof(unsigned) * kUnitSlots, stream));
+    prune_ctl_refine_kernel<<<1, 1, 0, stream>>>(ctl);
+    LAUNCHED();
+    RefineParams R;
+    R.mu_n = g0->prune_mu.as<double>();
+    R.surv = g0->prune_surv.as<int>();
+    R.part = g0->prune_part.as<double>();
+    R.arrive = g0->prune_arrive.as<unsigned>();
+    R.blocks = blocks;
+    R.groups_max = nb / 2 < 32 ? nb / 2 : 32;
+    R.final_stage = 0;
+    auto units = dreg ? predict_units_kernel<true> : predict_units_kernel<false>;
+    units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
+    LAUNCHED();
+    CU(cudaEventRecord(g0->ev_stage[2], stream));
+    PredictParams Q = P;  // the lead stage has begun the per-CTA lists
+    Q.sel_resume = 1;
+    if (dreg)
+        predict_refine_kernel<true><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+    else
+        predict_refine_kernel<false><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+    LAUNCHED();
+    CU(cudaEventRecord(g0->ev_stage[3], stream));
+    R.final_stage = 1;
+    units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(g0->ev_stage[4], stream));
+    return B200BO_OK;
+}
+
 // Bound pass + radix sort of (bound key, local index): fills P.perm / P.perm_key / P.prune_ctl for predict_acq16_kernel.
 // The k-th key word and the evaluated count carry over from launch to launch of a chunked batch (resume).
 static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool dreg, bool resume, cudaStream_t stream) {
@@ -1300,17 +1378,20 @@ static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool dreg, bool resume
     int rc;
     if ((rc = g0->prune_key.reserve(sizeof(unsigned long long) * 2 * (size_t)m))) return rc;
     if ((rc = g0->prune_idx.reserve(sizeof(int) * 2 * (size_t)m))) return rc;
-    if ((rc = g0->prune_ctl.reserve(sizeof(unsigned long long) * 3))) return rc;
+    if ((rc = g0->prune_ctl.reserve(sizeof(unsigned long long) * kCtlWords))) return rc;
+    if ((rc = g0->prune_mu.reserve(sizeof(double) * (size_t)m))) return rc;
+    double* mu = g0->prune_mu.as<double>();
     unsigned long long* keys = g0->prune_key.as<unsigned long long>();
     int* idx = g0->prune_idx.as<int>();
     unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
     const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
     if (dreg)
-        predict_bound_kernel<true><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr);
+        predict_bound_kernel<true><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr, mu);
     else
-        predict_bound_kernel<false><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr);
+        predict_bound_kernel<false><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr, mu);
     LAUNCHED();
     CU(cudaGetLastError());
+    CU(cudaEventRecord(g0->ev_stage[0], stream));
     cub::DoubleBuffer<unsigned long long> kb(keys, keys + m);
     cub::DoubleBuffer<int> ib(idx, idx + m);
     size_t tmp = 0;
@@ -1318,11 +1399,12 @@ static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool dreg, bool resume
     if ((rc = g0->prune_tmp.reserve(tmp))) return rc;
     CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, kb, ib, (int)m, 0, 64, stream));
     LAUNCHED();
-    CU(cudaMemsetAsync(ctl, 0, sizeof(unsigned long long), stream));
+    CU(cudaMemsetAsync(ctl + kCtlTile, 0, sizeof(unsigned long long), stream));
     if (!resume) {
-        CU(cudaMemsetAsync(ctl + 1, 0xFF, sizeof(unsigned long long), stream));
-        CU(cudaMemsetAsync(ctl + 2, 0, sizeof(unsigned long long), stream));
+        CU(cudaMemsetAsync(ctl + kCtlKth, 0xFF, sizeof(unsigned long long), stream));
+        CU(cudaMemsetAsync(ctl + kCtlEval, 0, sizeof(unsigned long long), stream));
     }
+    CU(cudaEventRecord(g0->ev_stage[1], stream));
     P.perm = ib.Current();
     P.perm_key = kb.Current();
     P.prune_ctl = ctl;
@@ -1595,6 +1677,14 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
                     (kind == B200BO_ACQ_EI || kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_POI) &&
                     m <= std::numeric_limits<int>::max() && prune_enabled();
             if (prune && (rc = prune_prepare(g0, P, dreg, sm.resume, stream))) return rc;
+            const int refine = prune && predict_mma() == 1684 ? prune_refine_blocks(P.gp[0].np, ntiles) : 0;
+            g0->stage_refined = refine > 0;
+            if (refine) {
+                // every SM keeps a list, begun by the lead stage and continued by the final stage and the tile kernel
+                grid = g0->sm_count;
+                if ((rc = prune_refine_stages(g0, P, dreg, refine, sm.resume, stream))) return rc;
+                P.sel_resume = 1;
+            }
             if (predict_mma() == 884) {
                 rc = launch_predict16<884, PIPE_CPASYNC>(dreg, grid, stream, P);
             } else if (pipe == PIPE_BULK_MC) {
@@ -1630,6 +1720,7 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
         g0->prune_counted = false;
     }
     g0->stat_total += m;
+    g0->stage_timed = prune;
     if (prune)
         g0->prune_counted = true;
     else
@@ -1679,9 +1770,9 @@ extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* 
     const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
     auto keys = reinterpret_cast<unsigned long long*>(d_key);
     if (P.d <= kPredictMaxDimRegs)
-        predict_bound_kernel<true><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax);
+        predict_bound_kernel<true><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax, nullptr);
     else
-        predict_bound_kernel<false><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax);
+        predict_bound_kernel<false><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax, nullptr);
     LAUNCHED();
     CU(cudaGetLastError());
     return B200BO_OK;
@@ -1716,10 +1807,33 @@ extern "C" int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total) {
     CU(cudaSetDevice(g0->device));
     CU(cudaEventSynchronize(g0->ev1));
     unsigned long long pruned_eval = 0;
-    if (g0->prune_counted) CU(cudaMemcpy(&pruned_eval, g0->prune_ctl.as<unsigned long long>() + 2, sizeof(pruned_eval),
+    if (g0->prune_counted) CU(cudaMemcpy(&pruned_eval, g0->prune_ctl.as<unsigned long long>() + kCtlEval, sizeof(pruned_eval),
                                          cudaMemcpyDeviceToHost));
     *evaluated = g0->stat_direct + (int64_t)pruned_eval;
     *total = g0->stat_total;
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_last_prune_stage_ms(float* ms, int64_t* refined) {
+    if (!ms || !refined) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!g_last_timed) return set_err(B200BO_ERR_STATE, "no timed kernel on this thread");
+    b200bo_gp* g0 = g_last_timed;
+    if (!g0->stage_timed) return set_err(B200BO_ERR_STATE, "the last launch on this thread was not pruned");
+    CU(cudaSetDevice(g0->device));
+    CU(cudaEventSynchronize(g0->ev1));
+    for (int i = 0; i < 6; ++i) ms[i] = 0.f;
+    *refined = 0;
+    CU(cudaEventElapsedTime(&ms[0], g0->ev0, g0->ev_stage[0]));
+    CU(cudaEventElapsedTime(&ms[1], g0->ev_stage[0], g0->ev_stage[1]));
+    cudaEvent_t last = g0->ev_stage[1];
+    if (g0->stage_refined) {
+        for (int i = 2; i < 5; ++i) CU(cudaEventElapsedTime(&ms[i], g0->ev_stage[i - 1], g0->ev_stage[i]));
+        last = g0->ev_stage[4];
+        unsigned long long n = 0;
+        CU(cudaMemcpy(&n, g0->prune_ctl.as<unsigned long long>() + kCtlRefined, sizeof(n), cudaMemcpyDeviceToHost));
+        *refined = (int64_t)n;
+    }
+    CU(cudaEventElapsedTime(&ms[5], last, g0->ev1));
     return B200BO_OK;
 }
 

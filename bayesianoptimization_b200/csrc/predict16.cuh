@@ -54,14 +54,16 @@ __device__ __forceinline__ void st_global_hint(double* p, double v, unsigned lon
 // of a stage are then contiguous in global memory exactly as in shared memory, one copy per stage).
 // KSTR = 0: the bound pass of pruning (predict_bound_kernel): no K* is stored; each thread keeps the largest |K*_i| of
 // its rows in kmax_s[part][c] instead.
-// Column c is candidate c0 + c, or perm[c0 + c] when P.perm is set (tiles in bound order).
+// Column c is candidate c0 + c of the first mlim, or perm[c0 + c] when perm is set (tiles in bound order); rows: the
+// leading training rows to build (a multiple of PA_CHUNK; G.np for all of them - mu_s is K* alpha_ only then).
 template <bool DREG, int COV, int KSTR>
 __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
                                                        double* __restrict__ Ks, double* smem,
                                                        double (*mu_s)[PBN], unsigned long long pol_first,
-                                                       double (*kmax_s)[PBN]) {
+                                                       double (*kmax_s)[PBN], const int* perm, long long mlim,
+                                                       int rows) {
     const int tid = threadIdx.x;
-    const int d = P.d, np = G.np;
+    const int d = P.d;
     double* xc_s = smem;                              // [d][PBN]
     double* xs_s = smem + (size_t)d * PBN;            // [2][PA_CHUNK][d]
     double* al_s = xs_s + (size_t)2 * PA_CHUNK * d;   // [2][PA_CHUNK]
@@ -69,8 +71,8 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
         const int c = idx / d, j = idx - c * d;
         const long long gi = c0 + c;
         double v = 0.0;
-        if (gi < P.m) {
-            v = candidate_coord(P, P.perm ? (long long)P.perm[gi] : gi, j);
+        if (gi < mlim) {
+            v = candidate_coord(P, perm ? (long long)perm[gi] : gi, j);
             if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
             v = v / G.ls[j];
         }
@@ -84,7 +86,7 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
         if (tid < PA_CHUNK / 2)
             cp_async16_cg(al_s + buf * PA_CHUNK + 2 * tid, G.alphav + (size_t)ch * PA_CHUNK + 2 * tid);
     };
-    const int nch = np / PA_CHUNK;
+    const int nch = rows / PA_CHUNK;
     load_chunk(0, 0);
     cp_async_commit();
     __syncthreads();  // xc_s visible
@@ -166,12 +168,13 @@ __device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, c
 template <bool DREG, int KSTR>
 __device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const GpDev& G, long long c0,
                                                   double* __restrict__ Ks, double* smem, double (*mu_s)[PBN],
-                                                  unsigned long long pol_first, double (*kmax_s)[PBN] = nullptr) {
+                                                  unsigned long long pol_first, double (*kmax_s)[PBN],
+                                                  const int* perm, long long mlim, int rows) {
     switch (cov_code(G.family, G.nu)) {
-        case 0: predict16_phase_a_impl<DREG, 0, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
-        case 1: predict16_phase_a_impl<DREG, 1, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
-        case 2: predict16_phase_a_impl<DREG, 2, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
-        default: predict16_phase_a_impl<DREG, 3, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s); break;
+        case 0: predict16_phase_a_impl<DREG, 0, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        case 1: predict16_phase_a_impl<DREG, 1, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        case 2: predict16_phase_a_impl<DREG, 2, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        default: predict16_phase_a_impl<DREG, 3, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
     }
 }
 
@@ -186,10 +189,15 @@ __device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const 
 // np.argmin reports first).  mu is bit-equal to the epilogue's: the same phase A, the same order of sums.
 constexpr double kPruneVarEps = 1e-8, kPruneRelMargin = 1e-9, kPruneAbsMargin = 1e-300;
 
+// var_ub: an upper bound of sigma^2 in normalised units, margin included:
+//   max(0, min(prior, prior - r + eps * prior)) with r <= k*^T K^-1 k* (prune_var_ub)
+__device__ __forceinline__ double prune_var_ub(const GpDev& G, double r) {
+    return fmax(0.0, fmin(G.prior, G.prior - r + kPruneVarEps * G.prior));
+}
+
 __device__ __forceinline__ unsigned long long prune_bound_key(const PredictParams& P, const GpDev& G, double mu_n,
-                                                              double kmax) {
+                                                              double var_ub) {
     const double mean = G.y_std * mu_n + G.y_mean;
-    const double var_ub = fmax(0.0, fmin(G.prior, G.prior - kmax * kmax / G.kdiag + kPruneVarEps * G.prior));
     const double sd = sqrt(var_ub * (G.y_std * G.y_std));
     const double a = mean - P.y_max - P.xi;
     double base, scale;
@@ -211,36 +219,52 @@ __device__ __forceinline__ unsigned long long prune_bound_key(const PredictParam
     return key_nan_last(v_lb);
 }
 
-// One CTA per tile of PBN candidates: phase A without the K* stores, then (key, local index) per candidate; idx and
-// kmax_out (max_i |K*_i|, for b200bo_acq_prune_bound_dev) may be nullptr.
+// One CTA per tile of PBN candidates: phase A without the K* stores, then (key, local index) per candidate; idx,
+// kmax_out (max_i |K*_i|, for b200bo_acq_prune_bound_dev) and mu_out (K* alpha_, which the refine stages reuse: it is
+// the epilogue's value bit for bit) may be nullptr.
 template <bool DREG>
 __global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictParams P, unsigned long long* keys,
-                                                               int* idx, double* kmax_out) {
+                                                               int* idx, double* kmax_out, double* mu_out) {
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
     __shared__ double kmax_s[P16_SPLIT][PBN];
     const long long c0 = (long long)blockIdx.x * PBN;
     const GpDev& G = P.gp[0];
-    predict16_phase_a<DREG, 0>(P, G, c0, nullptr, smem, mu_s, 0ull, kmax_s);
+    predict16_phase_a<DREG, 0>(P, G, c0, nullptr, smem, mu_s, 0ull, kmax_s, nullptr, P.m, G.np);
     const int c = threadIdx.x;
     if (c < PBN && c0 + c < P.m) {
         const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
         const double kmax = fmax(fmax(kmax_s[0][c], kmax_s[1][c]), fmax(kmax_s[2][c], kmax_s[3][c]));
-        keys[c0 + c] = prune_bound_key(P, G, mu_n, kmax);
+        keys[c0 + c] = prune_bound_key(P, G, mu_n, prune_var_ub(G, kmax * kmax / G.kdiag));
         if (idx) idx[c0 + c] = (int)(c0 + c);
+        if (mu_out) mu_out[c0 + c] = mu_n;
         if (kmax_out) kmax_out[c0 + c] = kmax;
     }
 }
+
+// words of PredictParams::prune_ctl
+enum {
+    kCtlTile = 0,     // next tile of predict_acq16_kernel's prune mode, in bound order
+    kCtlKth = 1,      // least k-th key a full CTA list has published
+    kCtlEval = 2,     // candidates that went through the full phase B
+    kCtlRefTile = 3,  // next tile of the refine stage, in bound order
+    kCtlSurv = 4,     // candidates the refine stage let through
+    kCtlRefined = 5,  // candidates the refine stage looked at
+    kCtlUnit = 6,     // next unit of predict_units_kernel in the lead stage
+    kCtlKthLead = 7,  // the k-th key as it was before the lead stage
+    kCtlUnitFinal = 8,  // the same for the final stage
+    kCtlWords = 9
+};
 
 // Prune mode of predict_acq16_kernel: thread 0 claims the next tile in bound order and stops the CTA (returns ntiles)
 // once the tile's best bound key is above the least k-th key any CTA has published: every later tile's keys are
 // larger still, and a CTA's k-th key bounds the global k-th key from above.  Counts the candidates it lets through.
 __device__ __forceinline__ long long prune_claim(const PredictParams& P, long long ntiles, long long& tile_s) {
     if (threadIdx.x == 0) {
-        long long t = (long long)atomicAdd(P.prune_ctl, 1ull);
-        if (t < ntiles && P.perm_key[t * PBN] > *reinterpret_cast<volatile unsigned long long*>(P.prune_ctl + 1))
+        long long t = (long long)atomicAdd(P.prune_ctl + kCtlTile, 1ull);
+        if (t < ntiles && P.perm_key[t * PBN] > *reinterpret_cast<volatile unsigned long long*>(P.prune_ctl + kCtlKth))
             t = ntiles;
-        if (t < ntiles) atomicAdd(P.prune_ctl + 2, (unsigned long long)min((long long)PBN, P.m - t * PBN));
+        if (t < ntiles) atomicAdd(P.prune_ctl + kCtlEval, (unsigned long long)min((long long)PBN, P.m - t * PBN));
         tile_s = t;
     }
     __syncthreads();
@@ -268,9 +292,14 @@ __device__ __forceinline__ void predict16_load_stage(double* as, double* bs, con
 // conflict-free (PSTR_DMMA).  m16n8k4 tile mi takes a[2mi] (rows g) and a[2mi+1] (rows g+8) as its a0/a1, so its
 // c0..c3 are acc[2mi][j][0..1] and acc[2mi+1][j][0..1]: acc[i][j][e] is V row wm*32 + i*8 + g, candidate
 // wn*32 + j*8 + 2*t4 + e for both shapes and the epilogue is shared.
-template <int MMA>
+// Row blocks [ib0, ib1) of L^-1.  PART = false: red = the sums over those blocks (the whole product: 0, np / PBM).
+// PART = true (predict_units_kernel): nothing is summed across row blocks; every thread stores its s(ib) (the sum of
+// squares of its 4 rows, per column) to part[ib][wm][g][column], and the tile's finisher adds them in this function's
+// order (unit_finish_colsq).
+template <int MMA, bool PART>
 __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* __restrict__ Ks, double* smem,
-                                                  unsigned long long pol_last, unsigned long long pol_first) {
+                                                  unsigned long long pol_last, unsigned long long pol_first, int ib0,
+                                                  int ib1, double* __restrict__ part) {
     static_assert(MMA == 884 || MMA == 1684, "phase B shape");
     constexpr int STR = PSTR_DMMA, BK = PBK_DMMA;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -285,8 +314,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
     double csq[4][2];
 #pragma unroll
     for (int j = 0; j < 4; ++j) csq[j][0] = csq[j][1] = 0.0;
-    const int nb = np / PBM;
-    for (int ib = 0; ib < nb; ++ib) {
+    for (int ib = ib0; ib < ib1; ++ib) {
         double acc[4][4][2];
 #pragma unroll
         for (int i = 0; i < 4; ++i)
@@ -350,10 +378,16 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
                 s0 = fma(acc[i][j][0], acc[i][j][0], s0);
                 s1 = fma(acc[i][j][1], acc[i][j][1], s1);
             }
-            csq[j][0] += s0;
-            csq[j][1] += s1;
+            if constexpr (PART) {
+                double* q = part + ((size_t)(ib * 4 + wm) * 8 + g) * PBN + wn * 32 + j * 8 + t4 * 2;
+                *reinterpret_cast<double2*>(q) = make_double2(s0, s1);
+            } else {
+                csq[j][0] += s0;
+                csq[j][1] += s1;
+            }
         }
     }
+    if constexpr (PART) return;
 #pragma unroll
     for (int j = 0; j < 4; ++j)
 #pragma unroll
@@ -627,10 +661,11 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
             if constexpr (PIPE == PIPE_CPASYNC) {
-                predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first);
-                predict16_phase_b<MMA>(G, Ks, smem, pol_last, pol_first);
+                predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, G.np);
+                predict16_phase_b<MMA, false>(G, Ks, smem, pol_last, pol_first, 0, G.np / PBM, nullptr);
             } else {  // policies made where they are used: nothing extra stays live across phase B
-                predict16_phase_a<DREG, PSTR_DMMA>(P, G, c0, Ks, smem, mu_s, l2_policy_evict_first());
+                predict16_phase_a<DREG, PSTR_DMMA>(P, G, c0, Ks, smem, mu_s, l2_policy_evict_first(), nullptr, P.perm,
+                                                   P.m, G.np);
                 predict16_phase_b_bulk<PIPE == PIPE_BULK_MC>(P, G, smem, full_bar, empty_bar, done_cnt, it);
             }
             const double* red = smem;
@@ -644,13 +679,192 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
                 if (P.sel_cta && g == P.n_gps - 1) {
                     runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, c0 + c < P.m);
                     if (P.perm && tid == 0 && sel_s.list.idx[P.sel_k - 1] != SEL_NOIDX)
-                        atomicMin(P.prune_ctl + 1, sel_s.list.key[P.sel_k - 1]);
+                        atomicMin(P.prune_ctl + kCtlKth, sel_s.list.key[P.sel_k - 1]);
                 }
             }
             __syncthreads();
         }
     }
     if (P.sel_cta && tid < PBN) runsel_store(sel_s, P.sel_cta + blockIdx.x, tid);
+}
+
+// ---- selection-only pruning: the refine stages (DESIGN.md 4.9) ------------------------------------------------------
+// The tile kernel above pays one tile latency (phase B of a whole tile on one SM) for the first wave, which sets the
+// k-th key, and another for whatever the single-point bound leaves.  The refine stages replace both:
+//   lead    the first kLeadTiles tiles in bound order, evaluated exactly by predict_units_kernel, which splits the row
+//           blocks of every tile across CTAs, so the k-th key exists after a fraction of a tile latency;
+//   refine  predict_refine_kernel: for the following tiles in bound order (same stop rule as prune_claim) the product
+//           with the leading b row blocks of L^-1 only.  r_b = sum of V_i^2 over those rows is k*^T K^-1 k* of the GP
+//           conditioned on the first b * PBM training points alone, and the remaining terms are squares, so
+//           r_b <= k*^T K^-1 k* and prune_var_ub(r_b) bounds the variance as the single-point r does.  Candidates whose
+//           refined key and single-point key are both <= the k-th key are appended to the survivor list;
+//   final   the survivors through predict_units_kernel.
+// When more than kRefineMaxTiles tiles of survivors come up (little prunes: the refine stage stops claiming tiles as
+// soon as it sees that), the final stage does nothing and the tile kernel goes on in bound order behind the lead
+// tiles as it would have without these stages; otherwise the final stage closes the tile kernel's counter.
+// Exact values are bit-equal to the tile kernel's: K* entries carry no order, mu is the bound pass's (stored), and the
+// sum of squares is added up by unit_finish_colsq in the order of predict16_phase_b.  No CTA waits for another: the
+// stages are kernel boundaries, and within predict_units_kernel the last unit to arrive at a tile's counter finishes it.
+constexpr int kLeadTiles = 8, kRefineMaxTiles = 128, kUnitSlots = kLeadTiles + kRefineMaxTiles;
+constexpr long long kCtlClosed = 1ll << 40;  // value of kCtlTile no batch reaches
+
+struct RefineParams {
+    const double* mu_n;      // [m] K* alpha_ per candidate (local index), from the bound pass
+    int* surv;               // [kRefineMaxTiles * PBN] local indices the refine stage let through
+    double* part;            // [kUnitSlots][np / PBM][4][8][PBN] per-row-block partial sums of squares
+    unsigned* arrive;        // [kUnitSlots] units that have delivered their part of a tile
+    int blocks;              // leading row blocks of the refined bound
+    int groups_max;          // most units a tile is split into
+    int final_stage;         // predict_units_kernel: 0 lead, 1 final
+};
+
+// first row block of group j of G over nb row blocks, cut so that the groups' k-tile counts (row block ib: ib + 1) are
+// about equal; j = G gives nb.  Groups may be empty.
+__host__ __device__ inline int unit_cut(int nb, int G, int j) {
+    const long long total = (long long)nb * (nb + 1) / 2;
+    int ib = 0;
+    while (ib < nb && (long long)ib * (ib + 1) / 2 * G < total * j) ++ib;
+    return j >= G ? nb : ib;
+}
+
+// sum over the row blocks [0, nb) of a tile's partials, in the order of predict16_phase_b: per (row slab wm, lane
+// group g) over ib, then the xor-shuffle tree over g (4, 8, 16: ((0+1)+(2+3))+((4+5)+(6+7))), written to red[wm][c];
+// the caller adds the slabs.  512 threads: thread = (wm, column).
+__device__ __forceinline__ void unit_finish_colsq(const double* __restrict__ part, int nb, double* red) {
+    const int c = threadIdx.x & (PBN - 1), wm = threadIdx.x >> 7;
+    double v[8];
+#pragma unroll
+    for (int g = 0; g < 8; ++g) v[g] = 0.0;
+    for (int ib = 0; ib < nb; ++ib) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g) v[g] += __ldcg(part + ((size_t)(ib * 4 + wm) * 8 + g) * PBN + c);
+    }
+    red[wm * PBN + c] = ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
+}
+
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const PredictParams P, const RefineParams R) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    __shared__ long long tile_s;
+    const int tid = threadIdx.x;
+    const GpDev& G = P.gp[0];
+    double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
+    const long long ntiles = (P.m + PBN - 1) / PBN;
+    const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last), pol_first = l2_policy_evict_first();
+    // nothing moves the k-th key while this kernel runs
+    const unsigned long long kth = P.prune_ctl[kCtlKth];
+    for (;;) {
+        if (tid == 0) {
+            long long t = ntiles;
+            if (*reinterpret_cast<volatile unsigned long long*>(P.prune_ctl + kCtlSurv) <=
+                (unsigned long long)kRefineMaxTiles * PBN) {
+                t = (long long)atomicAdd(P.prune_ctl + kCtlRefTile, 1ull);
+                if (t < ntiles && P.perm_key[t * PBN] > kth) t = ntiles;
+            }
+            if (t < ntiles) atomicAdd(P.prune_ctl + kCtlRefined, (unsigned long long)min((long long)PBN, P.m - t * PBN));
+            tile_s = t;
+        }
+        __syncthreads();
+        const long long tile = tile_s;
+        if (tile >= ntiles) break;
+        const long long c0 = tile * PBN;
+        predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, R.blocks * PBM);
+        predict16_phase_b<1684, false>(G, Ks, smem, pol_last, pol_first, 0, R.blocks, nullptr);
+        const double* red = smem;
+        if (tid < PBN && c0 + tid < P.m) {
+            const int c = tid, li = P.perm[c0 + c];
+            const double r = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
+            const unsigned long long key = prune_bound_key(P, G, R.mu_n[li], prune_var_ub(G, r));
+            if (key <= kth && P.perm_key[c0 + c] <= kth) {
+                const unsigned long long pos = atomicAdd(P.prune_ctl + kCtlSurv, 1ull);
+                if (pos < (unsigned long long)kRefineMaxTiles * PBN) R.surv[pos] = li;
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// Exact evaluation in units of (tile, group of consecutive row blocks).  Lead stage: the tiles are the first
+// kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this launch (a
+// continued batch; read from kCtlKthLead, which does not move, so that all units of a tile decide alike).  Final
+// stage: the tiles are the survivor list.  A unit builds K* for the rows its row blocks need in its CTA's scratch,
+// runs phase B over its row blocks, and the last unit to arrive finishes the tile as the tile kernel's epilogue does.
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictParams P, const RefineParams R) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    __shared__ SelShared sel_s;
+    __shared__ long long unit_s;
+    __shared__ int last_s;
+    const int tid = threadIdx.x;
+    const GpDev& G = P.gp[0];
+    const int nb = G.np / PBM;
+    double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
+    const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last), pol_first = l2_policy_evict_first();
+    if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
+    __syncthreads();
+    // candidates of this stage, their tiles and the units per tile: the same in every CTA
+    const int* list = P.perm;
+    long long n = min(P.m, (long long)kLeadTiles * PBN);
+    int groups = R.groups_max, slot0 = 0;
+    unsigned long long* claim = P.prune_ctl + kCtlUnit;
+    if (R.final_stage) {
+        n = (long long)P.prune_ctl[kCtlSurv];
+        if (n > (long long)kRefineMaxTiles * PBN) n = 0;  // too many: the tile kernel takes over in bound order
+        else if (blockIdx.x == 0 && tid == 0) atomicExch(P.prune_ctl + kCtlTile, (unsigned long long)kCtlClosed);
+        list = R.surv;
+        slot0 = kLeadTiles;
+        claim = P.prune_ctl + kCtlUnitFinal;
+    }
+    const long long ntiles = (n + PBN - 1) / PBN;
+    if (R.final_stage && ntiles > 0)
+        groups = (int)max(1ll, min((long long)R.groups_max, 2ll * gridDim.x / ntiles));
+    for (;;) {
+        if (tid == 0) unit_s = (long long)atomicAdd(claim, 1ull);
+        __syncthreads();
+        const long long unit = unit_s;
+        const long long tile = unit / groups;
+        if (tile >= ntiles) break;
+        const long long c0 = tile * PBN;
+        if (!R.final_stage && P.perm_key[c0] > P.prune_ctl[kCtlKthLead]) {
+            __syncthreads();
+            continue;
+        }
+        const int grp = (int)(unit - tile * groups);
+        const int ib0 = unit_cut(nb, groups, grp), ib1 = unit_cut(nb, groups, grp + 1);
+        double* part = R.part + (size_t)(slot0 + tile) * nb * 32 * PBN;
+        if (ib1 > ib0) {
+            predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
+            predict16_phase_b<1684, true>(G, Ks, smem, pol_last, pol_first, ib0, ib1, part);
+        }
+        __threadfence();  // this unit's partials before its arrival
+        __syncthreads();
+        if (tid == 0) last_s = atomicAdd(R.arrive + slot0 + tile, 1u) == (unsigned)groups - 1;
+        __syncthreads();
+        if (last_s) {
+            __threadfence();
+            double* red = smem;
+            unit_finish_colsq(part, nb, red);
+            __syncthreads();
+            if (tid < PBN) {
+                const int c = tid;
+                const bool valid = c0 + c < n;
+                const long long gi = valid ? (long long)list[c0 + c] : P.m;
+                const double colsq = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
+                double val = 0.0, base, prod;
+                candidate_epilogue(P, G, 0, valid ? R.mu_n[gi] : 0.0, colsq, gi, base, prod, &val);
+                runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, valid);
+                if (tid == 0) {
+                    if (sel_s.list.idx[P.sel_k - 1] != SEL_NOIDX)
+                        atomicMin(P.prune_ctl + kCtlKth, sel_s.list.key[P.sel_k - 1]);
+                    atomicAdd(P.prune_ctl + kCtlEval, (unsigned long long)min((long long)PBN, n - c0));
+                }
+            }
+        }
+        __syncthreads();
+    }
+    if (tid < PBN) runsel_store(sel_s, P.sel_cta + blockIdx.x, tid);
 }
 
 }  // namespace b200bo

@@ -385,6 +385,15 @@ int b200bo_last_kernel_ms(float* ms);
  * acquisition bound cannot reach the top-k (DESIGN.md 4.9).  Synchronises on the stop event. */
 int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total);
 
+/* Where the kernel time of the most recent pruned launch on this thread went (a streamed or split batch: its last
+ * launch), from CUDA events recorded between the stages on the call's stream: ms[0] bound pass, ms[1] sort,
+ * ms[2] lead (the first tiles in bound order, split across SMs), ms[3] refine (leading-row-block bound), ms[4] final
+ * (exact evaluation of the refine survivors, split across SMs), ms[5] the whole-tile kernel in bound order.  ms[2..4]
+ * are 0 when the refine stages did not run (B200BO_PRUNE_REFINE=0, DESIGN.md 4.9).  *refined = candidates that went
+ * through the refine stage (all launches of the call).  B200BO_ERR_STATE when the launch was not pruned.  Synchronises
+ * on the stop event; nothing is read back unless this is called. */
+int b200bo_last_prune_stage_ms(float ms[6], int64_t* refined);
+
 /* The bound pass of selection-only pruning alone (EI, UCB or PoI on one GP; 1 <= m <= INT_MAX device rows d_Xc):
  * d_key[i] = the order key (key_nan_last of select.cuh) of a lower bound on candidate i's closure value -acq, 0 for a
  * candidate that is never pruned; d_kmax[i] (nullable) = max_j |k(x_i, X_j)| in normalised units.  Enqueued on
