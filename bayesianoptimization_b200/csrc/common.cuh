@@ -45,10 +45,28 @@ __device__ __forceinline__ double sqrt_pos(double x) {
     return s;
 }
 
+// x / 3.0 correctly rounded, without the division: q = RN(x RN(1/3)) is within 1 ulp of x/3, so one Markstein
+// correction RN(q + RN(x - 3q) RN(1/3)) gives RN(x/3) (the residual x - 3q is exact in the FMA).  Valid for normal x
+// far from overflow; the callers pass k^2 with k from sqrt_pos, i.e. x in [1e-30, 5e38].  The IEEE division it replaces
+// carried a conditional call to its slow path per pair, which cut phase A's unrolled row block into branch regions
+// the scheduler could not interleave.  Bit-identical to x / 3.0 (tests/test_covariance_primitives_cpu.py).
+__device__ __forceinline__ double div3_rn(double x) {
+    constexpr double third = 0.33333333333333331483;  // RN(1/3)
+    const double q = __dmul_rn(x, third);
+    const double r = fma(-q, 3.0, x);
+    return fma(r, third, q);
+}
+
 // exp(-k) for k >= 0 (k > 700 is clamped: the result, < 1e-304, is irrelevant at fp64 scale).
+// n = rint(-k log2e) comes from the 1.5 2^52 shift: the rounded product plus 1.5 2^52 lies in [2^52, 2^53), where the
+// add rounds it to an integer half to even exactly as rint does, and the low word of the sum is n.  2^n is applied by
+// an integer add to the exponent field of p (p in [sqrt(1/2), sqrt(2)], n in [-1010, 0]: the product is normal and the
+// multiply it replaces was exact).  Same bits as rint / (long long) / p * 2^n, without FRND, F2I and the multiply.
 __device__ __forceinline__ double exp_neg(double k) {
+    constexpr double shift = 6755399441055744.0;  // 1.5 * 2^52
     k = fmin(k, kExpR[3]);
-    const double n = rint(-k * kExpR[0]);
+    const double t = __dadd_rn(__dmul_rn(-k, kExpR[0]), shift);
+    const double n = __dsub_rn(t, shift);
     double r = fma(n, kExpR[1], -k);
     r = fma(n, kExpR[2], r);
     // degree-13 Taylor polynomial (|r| <= ln2/2: truncation 4e-18) in Estrin form: dependent
@@ -63,8 +81,8 @@ __device__ __forceinline__ double exp_neg(double k) {
     const double r8 = r4 * r4;
     const double d0 = fma(c1, r4, c0), d1 = fma(b6, r4, c2);
     const double p = fma(d1, r8, d0);
-    const long long e = ((long long)n + 1023ll) << 52;  // 2^n, n in [-1010, 0]
-    return p * __longlong_as_double(e);
+    const int e = (int)((unsigned)__double2loint(t) << 20);  // n in the exponent field of the high word
+    return __hiloint2double(__double2hiint(p) + e, __double2loint(p));
 }
 
 // ---- covariance functions -------------------------------------------------------------
@@ -77,7 +95,7 @@ __device__ __forceinline__ double cov_eval(double r2) {
     const double dist = sqrt_pos(r2);
     if (COV == 2) {
         const double k = dist * 2.23606797749978969641;  // math.sqrt(5)
-        return (1.0 + k + k * k / 3.0) * exp_neg(k);
+        return (1.0 + k + div3_rn(k * k)) * exp_neg(k);
     }
     if (COV == 1) {
         const double k = dist * 1.73205080756887729353;  // math.sqrt(3)

@@ -819,7 +819,7 @@ __device__ __forceinline__ void cov_and_gradfactor(double r2, double& kval, doub
     } else if (COV == 2) {
         const double tmp = sqrt_pos(5.0 * r2);
         const double e = exp_neg(tmp);
-        kval = (1.0 + tmp + tmp * tmp / 3.0) * e;
+        kval = (1.0 + tmp + div3_rn(tmp * tmp)) * e;
         gcommon = 5.0 / 3.0 * (tmp + 1.0) * e;
     } else if (COV == 1) {
         const double tmp = sqrt_pos(3.0 * r2);
