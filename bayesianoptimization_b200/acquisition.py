@@ -21,7 +21,8 @@ ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`
 from q paths (batch Thompson sampling).  ``MaxValueEntropySearch`` is the
 information-based policy: samples of the maximum from posterior paths, then a fused-kernel epilogue of mu and sigma.
 ``KrigingBeliever`` gives UCB / EI / PoI / MES pending points and batches: the fitted GP is conditioned on the points in
-flight on the device, with its own mean as their targets.
+flight on the device, with its own mean as their targets.  ``LogExpectedImprovement`` and
+``LogProbabilityOfImprovement`` are EI and PoI in log space, finite and well scaled where EI and PoI underflow.
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
 (gpr.B200GaussianProcessRegressor), ``fused.FusedAcquisition`` and the C ABI do not need it.
@@ -29,8 +30,12 @@ flight on the device, with its own mean as their targets.
 from __future__ import annotations
 
 import abc
+import warnings
 
 import numpy as np
+from scipy.special import erfcx as _erfcx
+from scipy.special import log_ndtr as _log_ndtr
+from scipy.special import ndtr as _ndtr
 
 try:
     from bayes_opt import acquisition as _ref
@@ -165,6 +170,126 @@ class ProbabilityOfImprovement(DeviceHooks, _ref.ProbabilityOfImprovement):
 
 class ExpectedImprovement(DeviceHooks, _ref.ExpectedImprovement):
     """bayes_opt.acquisition.ExpectedImprovement with the device hooks."""
+
+
+# ---- log-space acquisitions (DESIGN.md 4.12) ------------------------------------------------------------------
+# numpy forms of the device epilogue (csrc/common.cuh log_h, csrc/predict_kernels.cuh log_acq_term / log_cfactor),
+# for user subclasses that override base_acq and for calls outside the fused kernel.
+_LOG_H_TAIL = -(2.0**26)  # -1/sqrt(eps)
+_HALF_LOG_2PI = 0.91893853320467274178
+_HALF_LOG_PI_2 = 0.22579135264472743236
+
+
+def log1mexp(x):
+    """log(1 - exp(x)) for x <= 0: log(-expm1(x)) above -ln 2, log1p(-exp(x)) below."""
+    x = np.asarray(x, dtype=np.float64)
+    with np.errstate(all="ignore"):
+        return np.where(x > -np.log(2.0), np.log(-np.expm1(x)), np.log1p(-np.exp(x)))
+
+
+def log_h(z):
+    """log(phi(z) + z Phi(z)), the log of EI in units of sigma, in the three branches of Ament et al. (2023):
+    direct above z = -1, through erfcx and log1mexp down to -1/sqrt(eps), the asymptote -z^2/2 - log(2 pi)/2 - 2 log|z|
+    below."""
+    z = np.asarray(z, dtype=np.float64)
+    out = np.full(z.shape, np.nan)
+    with np.errstate(all="ignore"):
+        hi = z > -1.0
+        mid = ~hi & (z > _LOG_H_TAIL)
+        lo = ~hi & ~mid & ~np.isnan(z)
+        t = z[hi]
+        out[hi] = np.log(np.exp(-(t * t) / 2.0) / 2.50662827463100050242 + t * _ndtr(t))
+        t = z[mid]
+        out[mid] = (-0.5 * (t * t) - _HALF_LOG_2PI) + log1mexp(np.log(_erfcx(-t * np.sqrt(0.5)) * -t) + _HALF_LOG_PI_2)
+        t = z[lo]
+        out[lo] = (-0.5 * (t * t) - _HALF_LOG_2PI) - 2.0 * np.log(-t)
+    return out
+
+
+def log_expected_improvement(a, std):
+    """log EI at a = mean - y_max - xi: log_h(a / std) + log std; std = 0 (or an infinite a / std) gives the log of the
+    EI limit max(a, 0): log a, -inf for a < 0, NaN for a = 0."""
+    a, std = np.broadcast_arrays(np.asarray(a, dtype=np.float64), np.asarray(std, dtype=np.float64))
+    with np.errstate(all="ignore"):
+        z = a / std
+        lim = np.where(a > 0.0, np.log(np.where(a > 0.0, a, 1.0)), np.where(a < 0.0, -np.inf, np.nan))
+        return np.where((std == 0.0) | np.isinf(z), lim, log_h(z) + np.log(std))
+
+
+def log_constraint_factor(mean, std, lb, ub):
+    """log P(lb <= c <= ub) for c ~ N(mean, std^2): one-sided bounds through log_ndtr, a pair of bounds in one tail
+    reflected to the lower tail and combined through log1mexp, a straddling pair directly.  NaN where std <= 0 and a
+    bound is finite (scipy's frozen norm), 0 when both bounds are infinite."""
+    mean, std = np.broadcast_arrays(np.asarray(mean, dtype=np.float64), np.asarray(std, dtype=np.float64))
+    lb, ub = float(lb), float(ub)
+    if lb == -np.inf and ub == np.inf:
+        return np.zeros(mean.shape)
+    with np.errstate(all="ignore"):
+        u, l = (ub - mean) / std, (lb - mean) / std
+        if lb == -np.inf:
+            out = _log_ndtr(u)
+        elif ub == np.inf:
+            out = _log_ndtr(-l)
+        else:
+            refl = l >= 0.0
+            a, b = np.where(refl, -u, l), np.where(refl, -l, u)
+            lpb = _log_ndtr(b)
+            out = np.where((l < 0.0) & (u > 0.0), np.log(_ndtr(u) - _ndtr(l)), lpb + log1mexp(_log_ndtr(a) - lpb))
+        return np.where((std > 0.0) & ~np.isnan(mean), out, np.nan)
+
+
+class _LogSpace:
+    """Mixin of the log-space acquisitions: the closure is -(base_acq(mean, std) + sum_j log p_j(x)), the constraint
+    factors added in log space in constraint order (DeviceHooks runs the stock formulas in the fused kernel; this
+    host closure serves a subclass that overrides base_acq)."""
+
+    def _get_acq(self, gp, constraint=None):
+        dim = gp.X_train_.shape[1]
+
+        def acq(x):
+            x = np.asarray(x, dtype=np.float64).reshape(-1, dim)
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                mean, std = gp.predict(x, return_std=True)
+                v = np.asarray(self.base_acq(mean, std), dtype=np.float64)
+                if constraint is not None:
+                    for j, m in enumerate(constraint.model):
+                        cm, cs = m.predict(x, return_std=True)
+                        v = v + log_constraint_factor(cm, cs, constraint.lb[j], constraint.ub[j])
+            return -1 * v
+
+        return acq
+
+
+class LogExpectedImprovement(DeviceHooks, _LogSpace, _ref.ExpectedImprovement):
+    """Log expected improvement (Ament et al., "Unexpected Improvements to Expected Improvement for Bayesian
+    Optimization", NeurIPS 2023): log EI(x), evaluated so that it stays finite, smooth and well scaled where EI itself
+    underflows to 0 - late in a run, when most candidates lie many sigma below the incumbent and EI's gradient is
+    below any optimiser's tolerance.  Same maximiser as EI wherever EI is representable.
+
+    Parameters, y_max, the xi decay, NoValidPointRegisteredError under constraints and get/set of the acquisition
+    parameters are bayes_opt.acquisition.ExpectedImprovement's.  Constraints enter as sum_j log p_j."""
+
+    def base_acq(self, mean, std):
+        if self.y_max is None:
+            return super().base_acq(mean, std)  # the reference's "y_max is not set" ValueError
+        return log_expected_improvement(np.asarray(mean, dtype=np.float64) - self.y_max - self.xi, std)
+
+
+class LogProbabilityOfImprovement(DeviceHooks, _LogSpace, _ref.ProbabilityOfImprovement):
+    """Log probability of improvement: log PoI(x) = log Phi((mean - y_max - xi) / std) through a tail-safe log_ndtr,
+    finite where PoI underflows to 0.  Everything else is bayes_opt.acquisition.ProbabilityOfImprovement's;
+    constraints enter as sum_j log p_j."""
+
+    def base_acq(self, mean, std):
+        if self.y_max is None:
+            return super().base_acq(mean, std)  # the reference's "y_max is not set" ValueError
+        with np.errstate(all="ignore"):
+            return _log_ndtr((np.asarray(mean, dtype=np.float64) - self.y_max - self.xi) / std)
+
+
+# before the EI / PoI entries: the log classes are subclasses of them
+_STOCK = {LogExpectedImprovement: B.ACQ_LOGEI, LogProbabilityOfImprovement: B.ACQ_LOGPOI, **_STOCK}
 
 
 class _SuggestStream:
@@ -537,8 +662,8 @@ class KrigingBeliever(_ref.ConstantLiar):
     def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
         if _device_kind(base_acquisition) is None and not isinstance(base_acquisition, MaxValueEntropySearch):
             raise TypeError(f"KrigingBeliever needs an UpperConfidenceBound, ExpectedImprovement, "
-                            f"ProbabilityOfImprovement or MaxValueEntropySearch base acquisition, got "
-                            f"{type(base_acquisition).__name__}")
+                            f"ProbabilityOfImprovement, LogExpectedImprovement, LogProbabilityOfImprovement or "
+                            f"MaxValueEntropySearch base acquisition, got {type(base_acquisition).__name__}")
         super().__init__(accelerate(base_acquisition), strategy, random_state, atol, rtol)
 
     def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
@@ -636,7 +761,8 @@ class KrigingBeliever(_ref.ConstantLiar):
 # isinstance(x, b200.AcquisitionFunction) holds for every acquisition of this module, as
 # isinstance(x, bayes_opt.acquisition.AcquisitionFunction) does in the reference (abc virtual subclasses:
 # the concrete classes keep the reference's MRO).
-for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, ConstantLiar, GPHedge,
-             ThompsonSampling, ConstrainedThompsonSampling, MaxValueEntropySearch, KrigingBeliever):
+for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, LogExpectedImprovement,
+             LogProbabilityOfImprovement, ConstantLiar, GPHedge, ThompsonSampling, ConstrainedThompsonSampling,
+             MaxValueEntropySearch, KrigingBeliever):
     AcquisitionFunction.register(_cls)
 del _cls

@@ -1443,7 +1443,7 @@ static int check_spec(const b200bo_acq* spec) {
     if (!spec) return set_err(B200BO_ERR_ARG, "spec is NULL");
     if (spec->n_gps < 1 || spec->n_gps > B200BO_MAX_GPS)
         return set_err(B200BO_ERR_ARG, "n_gps=%d out of range [1,%d]", spec->n_gps, B200BO_MAX_GPS);
-    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_MES)
+    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_LOGPOI || spec->kind == 5)
         return set_err(B200BO_ERR_ARG, "unknown acquisition kind %d", spec->kind);
     if (spec->path != B200BO_PATH_AUTO && spec->path != B200BO_PATH_STABLE)
         return set_err(B200BO_ERR_ARG, "unknown path policy %d", spec->path);
@@ -1674,7 +1674,8 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             }
             const int kind = spec->kind;
             prune = fused_sel && !P.acq_out && !P.mu_out && !P.sd_out && P.n_gps == 1 && pipe != PIPE_BULK_MC &&
-                    (kind == B200BO_ACQ_EI || kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_POI) &&
+                    (kind == B200BO_ACQ_EI || kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_POI ||
+                     kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI) &&
                     m <= std::numeric_limits<int>::max() && prune_enabled();
             if (prune && (rc = prune_prepare(g0, P, dreg, sm.resume, stream))) return rc;
             const int refine = prune && predict_mma() == 1684 ? prune_refine_blocks(P.gp[0].np, ntiles) : 0;
@@ -1754,8 +1755,9 @@ extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* 
     int rc;
     if ((rc = check_spec(spec))) return rc;
     if (spec->n_gps != 1 ||
-        (spec->kind != B200BO_ACQ_EI && spec->kind != B200BO_ACQ_UCB && spec->kind != B200BO_ACQ_POI))
-        return set_err(B200BO_ERR_ARG, "the pruning bound covers EI, UCB and PoI on one GP");
+        (spec->kind != B200BO_ACQ_EI && spec->kind != B200BO_ACQ_UCB && spec->kind != B200BO_ACQ_POI &&
+         spec->kind != B200BO_ACQ_LOGEI && spec->kind != B200BO_ACQ_LOGPOI))
+        return set_err(B200BO_ERR_ARG, "the pruning bound covers EI, UCB, PoI, LogEI and LogPoI on one GP");
     if (m <= 0 || m > std::numeric_limits<int>::max() || !d_Xc || !d_key)
         return set_err(B200BO_ERR_ARG, "bad candidates or key buffer");
     b200bo_gp* g0 = spec->gps[0];

@@ -173,6 +173,45 @@ __device__ __forceinline__ double inv_mills(double g) {
     return norm_pdf(g) / ndtr(g);
 }
 
+// log(1 - e^x) for x <= 0 in its two stable branches (Maechler, "Accurately Computing log(1 - exp(-|a|))", 2012):
+// log(-expm1(x)) above -ln 2, log1p(-exp(x)) below.
+__device__ __forceinline__ double log1mexp(double x) {
+    return x > -0.69314718055994530942 ? log(-expm1(x)) : log1p(-exp(x));
+}
+
+// log h(z), h(z) = phi(z) + z Phi(z), the expected improvement in units of sigma, in the three branches of Ament et
+// al. (NeurIPS 2023, eq. 9).  Below z = -1, h = phi(z) w(z) with w = 1 - sqrt(pi/2) |z| erfcx(-z/sqrt2) (Phi = phi
+// sqrt(pi/2) erfcx(-z/sqrt2)), so log h = log phi + log1mexp(log(erfcx |z|) + log(pi/2)/2).  Below -1/sqrt(eps) = -2^26
+// the log1mexp argument is within rounding of 0 and the asymptote w = 1/z^2 takes over.
+constexpr double kLogHTail = -67108864.0;
+__device__ __forceinline__ double log_h_tail_arg(double z) {
+    return log(erfcx(-z * 0.70710678118654752440) * -z) + 0.22579135264472743236;
+}
+__device__ __forceinline__ double log_h(double z) {
+    if (z > -1.0) return log(norm_pdf(z) + z * ndtr(z));
+    const double log_phi = -0.5 * (z * z) - 0.91893853320467274178;
+    if (z > kLogHTail) return log_phi + log1mexp(log_h_tail_arg(z));
+    return log_phi - 2.0 * log(-z);
+}
+// d log h / dz = Phi/h = r and phi/h = q (LogEI: d = r d mean / sigma + q d sigma / sigma), finite for every finite z
+// (q = z^2 overflows beyond |z| ~ 1.3e154, where its exact value does).  Below z = -1 from the same w as log_h:
+// q = 1/w, r = sqrt(pi/2) erfcx(-z/sqrt2) / w; below -2^26 r = |z| and q = z^2 (relative error 1/z^2 < eps).
+__device__ __forceinline__ void log_h_ratios(double z, double& r, double& q) {
+    if (z > -1.0) {
+        const double pz = norm_pdf(z), cz = ndtr(z), h = pz + z * cz;
+        r = cz / h;
+        q = pz / h;
+    } else if (z > kLogHTail) {
+        const double e = erfcx(-z * 0.70710678118654752440);
+        const double w = -expm1(log(e * -z) + 0.22579135264472743236);
+        r = 1.25331413731550025121 * e / w;
+        q = 1.0 / w;
+    } else {
+        r = -z;
+        q = z * z;
+    }
+}
+
 // frozen norm(loc, scale).cdf(b) as scipy evaluates it: NaN unless scale > 0
 // (rv_continuous.cdf argcheck), else ndtr((b - loc)/scale).
 __device__ __forceinline__ double norm_cdf_loc_scale(double b, double loc, double scale) {

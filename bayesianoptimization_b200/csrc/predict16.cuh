@@ -179,15 +179,20 @@ __device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const 
 }
 
 // ---- selection-only pruning: the bound pass ------------------------------------------------------------------
-// For the selection of the k smallest closure values -acq (EI, UCB, PoI on one GP; DESIGN.md 4.9), a key per candidate
+// For the selection of the k smallest closure values -acq (EI, UCB, PoI, LogEI, LogPoI on one GP; DESIGN.md 4.9,
+// 4.12), a key per candidate
 // that no candidate's exact key can be below: key_nan_last(v_lb) with v_lb <= -acq(mu, sigma).
 //   sigma^2 = prior - k*^T K^-1 k* <= prior - max_i k*_i^2 / K_ii (Cauchy-Schwarz in the K^-1 inner product) = var_ub;
 //   eps * prior absorbs the rounding of the explicit-inverse sum of squares the exact value is computed from;
 //   EI and UCB (as max(mu, mu + kappa sigma)) do not decrease with sigma, nor does PoI while a = mu - y_max - xi < 0
 //   (PoI <= 1 otherwise); v_lb is lowered by a relative and an absolute margin against the rounding of ndtr / pdf.
+//   LogEI and LogPoI are the logs of EI and PoI, so the same monotonicity holds (LogPoI <= 0 for a >= 0).  Their
+//   rounding error is absolute: up to a few ulps of |log h| + |log sigma| (the two can cancel), and in the tail of
+//   log h it grows with z^2 ~ 2 |value|.  The margin is 1e-9 |value| + 1e-9 (kPruneLogAbsMargin): the floor covers
+//   |log sigma| <= 745 with 1e4 headroom, the relative part the tail with about 1e6.
 // Key 0 (never pruned): mu or v_lb non-finite, or a within a few ulps of 0 (sigma = 0 with a = 0 gives the NaN that
 // np.argmin reports first).  mu is bit-equal to the epilogue's: the same phase A, the same order of sums.
-constexpr double kPruneVarEps = 1e-8, kPruneRelMargin = 1e-9, kPruneAbsMargin = 1e-300;
+constexpr double kPruneVarEps = 1e-8, kPruneRelMargin = 1e-9, kPruneAbsMargin = 1e-300, kPruneLogAbsMargin = 1e-9;
 
 // var_ub: an upper bound of sigma^2 in normalised units, margin included:
 //   max(0, min(prior, prior - r + eps * prior)) with r <= k*^T K^-1 k* (prune_var_ub)
@@ -208,6 +213,9 @@ __device__ __forceinline__ unsigned long long prune_bound_key(const PredictParam
         const double z = a / sd;
         base = a * ndtr(z) + sd * norm_pdf(z);
         scale = fabs(base);
+    } else if (log_kind(P.acq_kind)) {
+        base = (P.acq_kind == B200BO_ACQ_LOGPOI && a >= 0.0) ? 0.0 : log_acq_term(P.acq_kind, a, sd);
+        scale = fabs(base) + kPruneLogAbsMargin / kPruneRelMargin;
     } else {
         base = a < 0.0 ? ndtr(a / sd) : 1.0;
         scale = fabs(base);

@@ -127,11 +127,44 @@ __device__ __noinline__ double mes_term(double g) {
     return a - log_ndtr(g);
 }
 
+__device__ __forceinline__ bool log_kind(int kind) {
+    return kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI;
+}
+
+// LogEI / LogPoI at a = mean - y_max - xi (include/b200bo.h), out of line like mes_term.  sigma = 0, or a sigma so
+// small that z = a / sigma is infinite: the log of the EI limit max(a, 0) (log a, -inf, NaN at a = 0); log_ndtr has
+// the PoI limits already (0 at z = +inf, -inf at -inf, NaN at NaN).
+__device__ __noinline__ double log_acq_term(int kind, double a, double sd) {
+    const double z = a / sd;
+    if (kind == B200BO_ACQ_LOGPOI) return log_ndtr(z);
+    if (sd == 0.0 || isinf(z)) return a > 0.0 ? log(a) : (a < 0.0 ? -CUDART_INF : CUDART_NAN);
+    return log_h(z) + log(sd);
+}
+
+// log p of one constraint factor, p = Phi(u) - Phi(l), u = (ub - mean)/sd, l = (lb - mean)/sd: one-sided bounds
+// through log_ndtr(u) / log_ndtr(-l); a pair in one tail reflected so that both arguments a <= b are <= 0, then
+// log Phi(b) + log1mexp(log Phi(a) - log Phi(b)); a straddling pair directly.  A finite bound with sd <= 0 (or a NaN
+// mean) is the frozen-norm NaN of norm_cdf_loc_scale.
+__device__ __noinline__ double log_cfactor(double lb, double ub, double mean, double sd) {
+    const bool has_l = lb != -CUDART_INF, has_u = ub != CUDART_INF;
+    if (!has_l && !has_u) return 0.0;
+    if (!(sd > 0.0) || isnan(mean)) return CUDART_NAN;
+    const double u = (ub - mean) / sd, l = (lb - mean) / sd;
+    if (!has_l) return log_ndtr(u);
+    if (!has_u) return log_ndtr(-l);
+    if (l < 0.0 && u > 0.0) return log(ndtr(u) - ndtr(l));
+    const double a = l >= 0.0 ? -u : l, b = l >= 0.0 ? -l : u;
+    const double lpb = log_ndtr(b);
+    return lpb + log1mexp(log_ndtr(a) - lpb);
+}
+
 // ---- per-candidate epilogue shared by the tiled and the small-batch kernels ---------------------
 // mu_n: K* alpha_ (normalised units); colsq: sum_i V_i^2.  g = 0: target GP -> base acquisition;
 // g >= 1: constraint GP -> probability factor.  The last GP writes -base * prod.
 // MES: base = (1/K) sum_k, in k order, mes_term((y*_k - mean) / sd); base = 0 when sd == 0 (a clamped variance:
 // the predictive distribution is a point mass, an observation there teaches nothing).
+// LogEI / LogPoI: base_neg = -log_acq_term, then base_neg -= log p_g per constraint GP, which is -(alpha + sum log p)
+// summed in g order bit for bit (negation is exact); prod stays 1 and is not used.
 __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const GpDev& G, int g,
                                                    double mu_n, double colsq, long long gi,
                                                    double& base_neg, double& prod, double* final_val = nullptr) {
@@ -159,6 +192,8 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
                 for (int k = 0; k < P.n_ystar; ++k) s += mes_term((P.ystar[k] - mean) / sd);
                 base = s / (double)P.n_ystar;
             }
+        } else if (log_kind(P.acq_kind)) {
+            base = log_acq_term(P.acq_kind, mean - P.y_max - P.xi, sd);
         }
         base_neg = -1.0 * base;
         prod = 1.0;
@@ -166,6 +201,8 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
             if (P.mu_out) P.mu_out[gi] = mean;
             if (P.sd_out) P.sd_out[gi] = sd;
         }
+    } else if (log_kind(P.acq_kind)) {
+        base_neg = base_neg - log_cfactor(G.lb, G.ub, mean, sd);
     } else {
         const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
         const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
@@ -173,7 +210,7 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
         prod = (g == 1) ? (p_hi - p_lo) : prod * (p_hi - p_lo);
     }
     if (g == P.n_gps - 1) {
-        const double val = (P.n_gps > 1) ? base_neg * prod : base_neg;
+        const double val = (P.n_gps > 1 && !log_kind(P.acq_kind)) ? base_neg * prod : base_neg;
         if (final_val) *final_val = val;
         if (P.acq_out && gi < P.m) P.acq_out[gi] = val;
     }
@@ -1095,6 +1132,63 @@ __device__ __noinline__ double mes_term_deriv(double g) {
     return -0.5 * r - 0.5 * g * r * (g + r);
 }
 
+// LogEI / LogPoI: the value of log_acq_term and its coefficients of d mean and d sd, out of line like mes_term_deriv.
+//   LogEI: cm = r / sd, cs = q / sd (log_h_ratios);   LogPoI: cm = lambda / sd, cs = -z lambda / sd (inv_mills).
+// sd = 0 or an infinite z: LogEI = log a for a > 0 has cm = 1/a; everything else is a constant (cm = cs = 0).
+__device__ __noinline__ double log_acq_term_grad(int kind, double a, double sd, double& cm, double& cs) {
+    const double z = a / sd;
+    cm = cs = 0.0;
+    if (kind == B200BO_ACQ_LOGPOI) {
+        if (sd > 0.0 && !isinf(z)) {
+            const double lam = inv_mills(z);
+            cm = lam / sd;
+            cs = lam == 0.0 ? 0.0 : -z * lam / sd;
+        }
+        return log_ndtr(z);
+    }
+    if (sd == 0.0 || isinf(z)) {
+        if (a > 0.0) cm = 1.0 / a;
+        return a > 0.0 ? log(a) : (a < 0.0 ? -CUDART_INF : CUDART_NAN);
+    }
+    double r, q;
+    log_h_ratios(z, r, q);
+    cm = r / sd;
+    cs = q / sd;
+    return log_h(z) + log(sd);
+}
+
+// d log p = cm d mean + cs d sd for one constraint factor (log_cfactor), with F_l, F_u the partials of log p in l and u
+// (d u = -(d mean + u d sd) / sd, the same for l), each ratio phi / p in the same tail-safe form as the value:
+//   one-sided: F_u = lambda(u), F_l = -lambda(-l);   straddling: F_u = phi(u)/p, F_l = -phi(l)/p;
+//   one tail, a <= b <= 0, d = log Phi(a) - log Phi(b): phi(b)/p = lambda(b)/(-expm1(d)),
+//   phi(a)/p = lambda(a) e^d/(-expm1(d)), with the signs of the reflection.  sd <= 0 or a NaN mean: the value is NaN.
+__device__ __noinline__ void log_cfactor_grad(double lb, double ub, double mean, double sd, double& cm, double& cs) {
+    cm = cs = 0.0;
+    const bool has_l = lb != -CUDART_INF, has_u = ub != CUDART_INF;
+    if ((!has_l && !has_u) || !(sd > 0.0)) return;
+    const double u = (ub - mean) / sd, l = (lb - mean) / sd;
+    double fl = 0.0, fu = 0.0;
+    if (!has_l) {
+        fu = inv_mills(u);
+    } else if (!has_u) {
+        fl = -inv_mills(-l);
+    } else if (l < 0.0 && u > 0.0) {
+        const double p = ndtr(u) - ndtr(l);
+        fu = norm_pdf(u) / p;
+        fl = -norm_pdf(l) / p;
+    } else {
+        const bool refl = l >= 0.0;
+        const double a = refl ? -u : l, b = refl ? -l : u;
+        const double d = log_ndtr(a) - log_ndtr(b), om = -expm1(d);
+        const double gb = inv_mills(b) / om;
+        const double la = inv_mills(a), ga = la == 0.0 ? 0.0 : -la * exp(d) / om;
+        fl = refl ? -gb : ga;
+        fu = refl ? -ga : gb;
+    }
+    cm = -(fl + fu) / sd;
+    cs = -((fl == 0.0 ? 0.0 : l * fl) + (fu == 0.0 ? 0.0 : u * fu)) / sd;
+}
+
 // Chain rule of one GP's factor in data units, as the coefficients of d mean and d sd:
 //   d term = cm d mean + cs d sd,   term = the base acquisition (g = 0) or the probability factor p (g >= 1).
 // Returns the term itself in `term`.  sd == 0 (a clamped or vanished variance): the caller sets d sd := 0, and the
@@ -1136,7 +1230,12 @@ __device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, 
                 cm = -sm / ((double)P.n_ystar * sd);
                 cs = -ss / ((double)P.n_ystar * sd);
             }
+        } else if (log_kind(P.acq_kind)) {
+            term = log_acq_term_grad(P.acq_kind, mean - P.y_max - P.xi, sd, cm, cs);
         }
+    } else if (log_kind(P.acq_kind)) {
+        term = log_cfactor(G.lb, G.ub, mean, sd);
+        log_cfactor_grad(G.lb, G.ub, mean, sd, cm, cs);
     } else {
         const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
         const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
@@ -1161,6 +1260,7 @@ __device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, 
 //   grad_j = sum_g ( wa_g sum_b gpart_g[b][0][j] + wu_g sum_b gpart_g[b][1][j] ) / ls_gj      (blocks b in index order)
 //   wa_g = -w_g cm_g s_y,   wu_g = w_g cs_g s_y / sqrt(var_g)   (0 where var_g <= 0: d sd := 0)
 //   w_0 = -prod_i p_i,   w_g = -base prod_{i != g} p_i           (product rule over the GPs, g order)
+//   LogEI / LogPoI: w_g = -1 (the value is -(alpha + sum_g log p_g), a plain sum)
 // A rounded dimension has gradient 0; a NaN value gives a NaN row.
 __global__ void __launch_bounds__(256)
 small_finish_grad_kernel(const SmallParams S) {
@@ -1194,13 +1294,14 @@ small_finish_grad_kernel(const SmallParams S) {
                 wu_s[g][c] = var > 0.0 ? cs * G.y_std / sqrt(var) : 0.0;
             }
         }
+        const bool logk = log_kind(S.P.acq_kind);  // the value is -sum_g term_g: w_g = -1, no product rule
 #pragma unroll
         for (int g = 0; g < B200BO_MAX_GPS; ++g) {
             if (g < ng) {
                 double w = -1.0;
 #pragma unroll
                 for (int i = 0; i < B200BO_MAX_GPS; ++i)
-                    if (i < ng && i != g) w *= term[i];
+                    if (i < ng && i != g && !logk) w *= term[i];
                 wa_s[g][c] = wa_s[g][c] == 0.0 ? 0.0 : w * wa_s[g][c];
                 wu_s[g][c] = wu_s[g][c] == 0.0 ? 0.0 : w * wu_s[g][c];
             }

@@ -37,10 +37,13 @@ def _as_b200_gp(gp):
     return gp
 
 
+_NEEDS_Y_MAX = (B.ACQ_EI, B.ACQ_POI, B.ACQ_LOGEI, B.ACQ_LOGPOI)
+
+
 class FusedAcquisition:
     """Callable closure over fitted device GPs.
 
-    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES
+    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES / ACQ_LOGEI / ACQ_LOGPOI
     gp        fitted B200GaussianProcessRegressor (target)
     constraint  object with .model (list of device GPs), .lb, .ub  (bayes_opt ConstraintModel) or None
     params    either fixed ``kappa``/``xi``/``y_max`` values or ``owner``: an acquisition object whose
@@ -89,7 +92,7 @@ class FusedAcquisition:
             return self._fixed
         o = self._owner
         y_max = getattr(o, "y_max", None)
-        if self.kind in (B.ACQ_EI, B.ACQ_POI) and y_max is None:
+        if self.kind in _NEEDS_Y_MAX and y_max is None:
             o.base_acq(np.zeros(1), np.ones(1))  # raises the reference's own "y_max is not set" ValueError
         return float(getattr(o, "kappa", 0.0)), float(getattr(o, "xi", 0.0)), y_max
 
@@ -98,7 +101,7 @@ class FusedAcquisition:
         handles = [g._device_handles() for g in self._gps]  # [gp][device]
         sig = tuple(h.ptr.value for hs in handles for h in hs)
         kappa, xi, y_max = self._params()
-        if self.kind in (B.ACQ_EI, B.ACQ_POI) and y_max is None:
+        if self.kind in _NEEDS_Y_MAX and y_max is None:
             raise ValueError("y_max is not set. If you are calling this method outside of suggest(), "
                              "you must set y_max manually.")
         if self._specs is None or sig != self._sig:

@@ -62,6 +62,20 @@ extern "C" {
  * evaluated through erfcx below g = 0 and through ndtr / log1p at and above it: finite for every finite g.
  * Without a feasible registered point the constrained form still ranks candidates (EI / PoI raise there). */
 #define B200BO_ACQ_MES 4
+/* Log expected improvement and log probability of improvement (Ament et al., "Unexpected Improvements to Expected
+ * Improvement for Bayesian Optimization", NeurIPS 2023).  No counterpart in the reference.  With mu, sigma,
+ * a = mu - y_max - xi and z = a / sigma exactly as for EI / PoI, and h(z) = phi(z) + z Phi(z):
+ *   LOGEI:  alpha = log h(z) + log sigma       (= log EI)
+ *   LOGPOI: alpha = log Phi(z)                 (= log PoI)
+ *   acq_neg = -(alpha + sum_j log p_j)          (the constraint factors in log space, summed in j order)
+ * log h takes three branches: log(phi + z Phi) above z = -1; below it log phi(z) + log(1 - sqrt(pi/2) |z| erfcx(-z/sqrt2))
+ * through log1mexp; below z = -2^26 the asymptote -z^2/2 - log(2 pi)/2 - 2 log|z|.  log Phi and log p_j go through
+ * erfcx in the lower tail (a pair of bounds in one tail is reflected so that both arguments are <= 0), so both are
+ * finite where EI, PoI or p_j underflow to 0.  sigma = 0: alpha = log of the EI / PoI limit (-inf for a < 0, NaN for
+ * a = 0); a constraint GP with sigma = 0 makes the value NaN, as for EI / PoI. */
+#define B200BO_ACQ_LOGEI 6
+#define B200BO_ACQ_LOGPOI 7
+/* Code 5 is not assigned: it is rejected as an unknown kind (B200BO_ERR_ARG), as before these kinds existed. */
 
 #define B200BO_MAX_GPS 8   /* 1 target GP + up to 7 constraint GPs per call */
 #define B200BO_MAX_DIM 64  /* max input dimension d */
