@@ -65,9 +65,14 @@ struct NvtxRange {
 // ---------------------------------------------------------------------------------------
 // handle
 // ---------------------------------------------------------------------------------------
+// A device allocation that grows on demand and is freed with its owner (on the device current at that point).
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     int reserve(size_t bytes) {
         if (bytes <= cap) return B200BO_OK;
         if (p) cudaFree(p);
@@ -298,17 +303,7 @@ extern "C" int b200bo_gp_create(b200bo_gp** out, int device) {
 
 extern "C" void b200bo_gp_destroy(b200bo_gp* gp) {
     if (!gp) return;
-    cudaSetDevice(gp->device);
-    DevBuf* bufs[] = {&gp->X, &gp->Xs, &gp->y, &gp->K, &gp->L, &gp->W, &gp->WT, &gp->T,
-                      &gp->alphav, &gp->v1, &gp->v2, &gp->ls, &gp->xf, &gp->info, &gp->part,
-                      &gp->pscratch, &gp->xc, &gp->out_acq, &gp->out_mu, &gp->out_sd, &gp->sel,
-                      &gp->clamp, &gp->s_ksm, &gp->s_partial, &gp->s_mupart, &gp->s_unit, &gp->s_rb, &gp->s_colsq,
-                      &gp->s_vsum, &gp->s_usum, &gp->s_partial_u, &gp->s_gpart, &gp->s_unit_u, &gp->s_rb_u, &gp->out_grad,
-                      &gp->tc_linv, &gp->pad_linv, &gp->cov_xc, &gp->cov_kst, &gp->cov_v, &gp->cov_c, &gp->cov_out, &gp->cov_mu,
-                      &gp->sel_cta, &gp->pbounds, &gp->prow, &gp->pside, &gp->prune_key, &gp->prune_idx,
-                      &gp->prune_tmp, &gp->prune_ctl, &gp->prune_mu, &gp->prune_surv, &gp->prune_part,
-                      &gp->prune_arrive, &gp->tscratch};
-    for (DevBuf* b : bufs) b->release();
+    cudaSetDevice(gp->device);  // the buffers are freed by delete, on this device
     if (gp->stream) cudaStreamDestroy(gp->stream);
     if (gp->fgraph_exec) cudaGraphExecDestroy(gp->fgraph_exec);
     if (gp->cap_stream) cudaStreamDestroy(gp->cap_stream);
@@ -376,6 +371,30 @@ extern "C" int b200bo_gp_set_max_values(b200bo_gp* gp, const double* ystar, int 
 // ---------------------------------------------------------------------------------------
 // data upload + y normalisation (SK/gaussian_process/_gpr.py:275-285)
 // ---------------------------------------------------------------------------------------
+// y_norm, y_mean and y_std of gp->y_raw under gp->normalize.  y statistics in the order numpy uses for small arrays
+// is irrelevant at 1e-16; use a compensated sum so the result is the correctly rounded mean / population std.
+static void normalize_targets(b200bo_gp* gp) {
+    const std::vector<double>& y = gp->y_raw;
+    const size_t n = y.size();
+    double mean = 0.0, sd = 1.0;
+    gp->y_norm = y;
+    if (gp->normalize) {
+        long double s = 0.0L;
+        for (size_t i = 0; i < n; ++i) s += y[i];
+        mean = (double)(s / (long double)n);
+        long double q = 0.0L;
+        for (size_t i = 0; i < n; ++i) {
+            const long double t = (long double)y[i] - (long double)mean;
+            q += t * t;
+        }
+        sd = (double)sqrtl(q / (long double)n);
+        if (sd == 0.0) sd = 1.0;
+        for (size_t i = 0; i < n; ++i) gp->y_norm[i] = (y[i] - mean) / sd;
+    }
+    gp->y_mean = mean;
+    gp->y_std = sd;
+}
+
 extern "C" int b200bo_gp_set_data(b200bo_gp* gp, const double* X, const double* y, int64_t n, int d,
                                   int normalize_y) {
     if (!gp || !X || !y) return set_err(B200BO_ERR_ARG, "NULL argument");
@@ -396,27 +415,9 @@ extern "C" int b200bo_gp_set_data(b200bo_gp* gp, const double* X, const double* 
     gp->d = d;
     gp->np = round_up(n, kPad);
     const size_t np = gp->np;
-    // y statistics in the order numpy uses for small arrays is irrelevant at 1e-16; use
-    // a compensated sum so the result is the correctly rounded mean / population std.
-    double mean = 0.0, sd = 1.0;
-    gp->y_norm.assign(y, y + n);
     gp->y_raw.assign(y, y + n);
     gp->normalize = normalize_y != 0;
-    if (normalize_y) {
-        long double s = 0.0L;
-        for (int64_t i = 0; i < n; ++i) s += y[i];
-        mean = (double)(s / (long double)n);
-        long double q = 0.0L;
-        for (int64_t i = 0; i < n; ++i) {
-            const long double t = (long double)y[i] - (long double)mean;
-            q += t * t;
-        }
-        sd = (double)sqrtl(q / (long double)n);
-        if (sd == 0.0) sd = 1.0;
-        for (int64_t i = 0; i < n; ++i) gp->y_norm[i] = (y[i] - mean) / sd;
-    }
-    gp->y_mean = mean;
-    gp->y_std = sd;
+    normalize_targets(gp);
     int rc;
     if ((rc = gp->X.reserve(sizeof(double) * np * d))) return rc;
     if ((rc = gp->Xs.reserve(sizeof(double) * np * d))) return rc;
@@ -851,23 +852,7 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     // targets: new normalisation statistics, alpha_ = K^-1 y
     gp->y_raw.push_back(y_new);
     const int64_t nn = n + 1;
-    gp->y_norm = gp->y_raw;
-    double mean = 0.0, sd = 1.0;
-    if (gp->normalize) {
-        long double s = 0.0L;
-        for (int64_t i = 0; i < nn; ++i) s += gp->y_raw[i];
-        mean = (double)(s / (long double)nn);
-        long double q = 0.0L;
-        for (int64_t i = 0; i < nn; ++i) {
-            const long double t = (long double)gp->y_raw[i] - (long double)mean;
-            q += t * t;
-        }
-        sd = (double)sqrtl(q / (long double)nn);
-        if (sd == 0.0) sd = 1.0;
-        for (int64_t i = 0; i < nn; ++i) gp->y_norm[i] = (gp->y_raw[i] - mean) / sd;
-    }
-    gp->y_mean = mean;
-    gp->y_std = sd;
+    normalize_targets(gp);
     CU(cudaMemcpy(gp->y.p, gp->y_norm.data(), sizeof(double) * nn, cudaMemcpyHostToDevice));
     gp->n = nn;
     gp->tc_valid = false;
@@ -919,10 +904,10 @@ extern "C" int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, d
     return B200BO_OK;
 }
 
-static int fork_into(const b200bo_gp* src, int64_t extra_rows, b200bo_gp* dst) {
+// the fitted model's shape, hyper-parameters and target statistics: what a fork and a replica both take from the source
+static void copy_model_state(const b200bo_gp* src, b200bo_gp* dst) {
     dst->n = src->n;
     dst->d = src->d;
-    dst->np = round_up(src->n + extra_rows, kPad);
     dst->family = src->family;
     dst->nu = src->nu;
     dst->constv = src->constv;
@@ -930,12 +915,17 @@ static int fork_into(const b200bo_gp* src, int64_t extra_rows, b200bo_gp* dst) {
     dst->noise = src->noise;
     dst->y_mean = src->y_mean;
     dst->y_std = src->y_std;
-    dst->y_norm = src->y_norm;
-    dst->y_raw = src->y_raw;
     dst->normalize = src->normalize;
     dst->xform = src->xform;
-    dst->ystar = src->ystar;
     dst->precision = src->precision;
+}
+
+static int fork_into(const b200bo_gp* src, int64_t extra_rows, b200bo_gp* dst) {
+    copy_model_state(src, dst);
+    dst->np = round_up(src->n + extra_rows, kPad);
+    dst->y_norm = src->y_norm;
+    dst->y_raw = src->y_raw;
+    dst->ystar = src->ystar;
     const size_t n = src->n, d = src->d, np0 = src->np, np = dst->np;
     int rc;
     DevBuf* vecs[] = {&dst->X, &dst->Xs, &dst->y, &dst->alphav, &dst->v1, &dst->v2};
@@ -1123,17 +1113,23 @@ extern "C" int b200bo_gp_get(b200bo_gp* gp, int what, double* out, int64_t len) 
 // ---------------------------------------------------------------------------------------
 // predict / acquisition
 // ---------------------------------------------------------------------------------------
-// gradient calls: the work units of u = L^-T v (row block i: k chunks of [64 i, np)) + their scratch for one GP
+// work units of the small path's triangular products: row block i covers k in [0, 64 (i + 1)) of L^-1 v, or
+// [64 i, np) of L^-T v (upper), in SKCH chunks; rbs[i] = (first unit of row block i, its number of units)
+static void small_units(int np, bool upper, std::vector<int2>& units, std::vector<int2>& rbs) {
+    for (int i = 0; i < np / SROWS; ++i) {
+        const int nk = upper ? np - i * SROWS : (i + 1) * SROWS;
+        const int nj = (nk + SKCH - 1) / SKCH;
+        rbs.push_back(make_int2((int)units.size(), nj));
+        for (int j = 0; j < nj; ++j) units.push_back(make_int2(i, j));
+    }
+}
+
+// gradient calls: the work units of u = L^-T v + their scratch for one GP
 static int ensure_small_grad(b200bo_gp* gp) {
     const int np = gp->np, d = gp->d;
     if (gp->s_grad_np == np && gp->s_grad_d == d) return B200BO_OK;
     std::vector<int2> units, rbs;
-    const int nrb = np / SROWS;
-    for (int i = 0; i < nrb; ++i) {
-        const int nj = (np - i * SROWS + SKCH - 1) / SKCH;
-        rbs.push_back(make_int2((int)units.size(), nj));
-        for (int j = 0; j < nj; ++j) units.push_back(make_int2(i, j));
-    }
+    small_units(np, true, units, rbs);
     int rc;
     if ((rc = gp->s_unit_u.reserve(sizeof(int2) * units.size()))) return rc;
     if ((rc = gp->s_rb_u.reserve(sizeof(int2) * rbs.size()))) return rc;
@@ -1158,13 +1154,7 @@ static int ensure_small(b200bo_gp* gp, bool grad = false) {
     const int np = gp->np;
     if (gp->s_np == np) return B200BO_OK;
     std::vector<int2> units, rbs;
-    const int nrb = np / SROWS;
-    for (int i = 0; i < nrb; ++i) {
-        const int K = (i + 1) * SROWS;
-        const int nj = (K + SKCH - 1) / SKCH;
-        rbs.push_back(make_int2((int)units.size(), nj));
-        for (int j = 0; j < nj; ++j) units.push_back(make_int2(i, j));
-    }
+    small_units(np, false, units, rbs);
     int rc;
     if ((rc = gp->s_unit.reserve(sizeof(int2) * units.size()))) return rc;
     if ((rc = gp->s_rb.reserve(sizeof(int2) * rbs.size()))) return rc;
@@ -1234,23 +1224,30 @@ static int predict_pipe() {
     return kDefaultPredictPipe;
 }
 
-template <int MMA, int PIPE>
-static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
-    auto fn = dreg ? predict_acq16_kernel<true, MMA, PIPE> : predict_acq16_kernel<false, MMA, PIPE>;
-    cudaLaunchConfig_t cfg = {};
+// launch configuration of predict_acq16_kernel, in 2-CTA clusters when pair (attr: the storage cfg points to)
+static void predict16_config(int grid, cudaStream_t stream, bool pair, cudaLaunchConfig_t& cfg,
+                             cudaLaunchAttribute& attr) {
+    cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(P16_NT);
     cfg.dynamicSmemBytes = kPredictSmemBytesDmma;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    if (PIPE == PIPE_BULK_MC) {
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
+    if (pair) {
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = 2;
+        attr.val.clusterDim.y = 1;
+        attr.val.clusterDim.z = 1;
+        cfg.attrs = &attr;
         cfg.numAttrs = 1;
     }
+}
+
+template <int MMA, int PIPE>
+static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
+    auto fn = dreg ? predict_acq16_kernel<true, MMA, PIPE> : predict_acq16_kernel<false, MMA, PIPE>;
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr;
+    predict16_config(grid, stream, PIPE == PIPE_BULK_MC, cfg, attr);
     CU(cudaLaunchKernelEx(&cfg, fn, P));
     return B200BO_OK;
 }
@@ -1258,17 +1255,9 @@ static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const Pred
 // grid of the clustered launch: two CTAs per cluster that can be resident at once, never more than one per SM
 static int predict_pair_grid(b200bo_gp* g0) {
     if (g0->pair_grid > 0) return B200BO_OK;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2);
-    cfg.blockDim = dim3(P16_NT);
-    cfg.dynamicSmemBytes = kPredictSmemBytesDmma;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr;
+    predict16_config(2, nullptr, true, cfg, attr);
     int clusters = 0;
     CU(cudaOccupancyMaxActiveClusters(&clusters, predict_acq16_kernel<true, 1684, PIPE_BULK_MC>, &cfg));
     int nodreg = 0;
@@ -1479,6 +1468,16 @@ struct SelMode {
     int finish = 1;
 };
 
+// Philox bounds of the throughput mode as the kernels read them: pb = (lo_j, hi_j - lo_j), 2 d entries
+static int pack_pbounds(const double* lo, const double* hi, int d, double* pb) {
+    for (int j = 0; j < d; ++j) {
+        if (!(lo[j] <= hi[j])) return set_err(B200BO_ERR_ARG, "Philox bounds: lo > hi in column %d", j);
+        pb[j] = lo[j];
+        pb[d + j] = hi[j] - lo[j];
+    }
+    return B200BO_OK;
+}
+
 // launch parameters of the predict kernels for spec over the candidates of src (everything but outputs and scratch);
 // np_max: the largest padded training size of the spec's GPs
 static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, int64_t index_base, cudaStream_t stream,
@@ -1523,17 +1522,74 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
     P.index_base = index_base;
     if (src.philox) {
         double pb[2 * B200BO_MAX_DIM];
-        for (int j = 0; j < P.d; ++j) {
-            if (!(src.lo[j] <= src.hi[j])) return set_err(B200BO_ERR_ARG, "Philox bounds: lo > hi in column %d", j);
-            pb[j] = src.lo[j];
-            pb[P.d + j] = src.hi[j] - src.lo[j];
-        }
+        if ((rc = pack_pbounds(src.lo, src.hi, P.d, pb))) return rc;
         if ((rc = g0->pbounds.reserve(sizeof(double) * 2 * B200BO_MAX_DIM))) return rc;
         CU(cudaMemcpyAsync(g0->pbounds.p, pb, sizeof(double) * 2 * P.d, cudaMemcpyHostToDevice, stream));
         P.pbounds = g0->pbounds.as<double>();
         P.seed = src.seed;
     }
     P.m = m;
+    return B200BO_OK;
+}
+
+// The small-batch kernels over the m candidates of S.P (predict_kernels.cuh).  Per launch group of up to SMAXP passes
+// and per GP: K*, v = L^-1 k* and its sums; grad adds u = L^-T v and the gradient partials into S.grad_out.  Then one
+// finish for every GP.
+static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool grad, cudaStream_t stream) {
+    b200bo_gp* g0 = spec->gps[0];
+    int rc;
+    for (int g = 0; g < spec->n_gps; ++g) {
+        b200bo_gp* gp = spec->gps[g];
+        if ((rc = ensure_small(gp, grad))) return rc;
+        SmallGp& Q = S.sg[g];
+        Q.W = gp->W.as<double>();
+        Q.ksm = gp->s_ksm.as<double>();
+        Q.partial = gp->s_partial.as<double>();
+        Q.mu_part = gp->s_mupart.as<double>();
+        Q.colsq_rb = gp->s_colsq.as<double>();
+        Q.unit_tab = gp->s_unit.as<int2>();
+        Q.rb_tab = gp->s_rb.as<int2>();
+        S.nunits[g] = gp->s_nunits;
+        if (grad) {
+            Q.vsum = gp->s_vsum.as<double>();
+            Q.usum = gp->s_usum.as<double>();
+            Q.partial_u = gp->s_partial_u.as<double>();
+            Q.gpart = gp->s_gpart.as<double>();
+            Q.unit_tab_u = gp->s_unit_u.as<int2>();
+            Q.rb_tab_u = gp->s_rb_u.as<int2>();
+            S.nunits_u[g] = gp->s_nunits_u;
+        }
+    }
+    S.m_end = m;
+    CU(cudaEventRecord(g0->ev0, stream));
+    for (long long c0 = 0; c0 < m; c0 += (long long)SMAXP * SMC) {
+        S.c0 = c0;
+        const long long left = m - c0;
+        const int npass = (int)((left + SMC - 1) / SMC < SMAXP ? (left + SMC - 1) / SMC : SMAXP);
+        const int ngrp = (npass + STPG - 1) / STPG;
+        for (int g = 0; g < spec->n_gps; ++g) {
+            const b200bo_gp* gp = spec->gps[g];
+            small_kstar_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+            small_trsv_kernel<false><<<dim3(gp->s_nunits, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
+            if (grad) {
+                small_reduce_kernel<1><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
+                small_trsv_kernel<true><<<dim3(gp->s_nunits_u, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
+                small_reduce_kernel<2><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
+                small_grad_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+            } else {
+                small_reduce_kernel<0><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
+            }
+            for (int i = 0; i < (grad ? 6 : 3); ++i) LAUNCHED();
+        }
+        if (grad)
+            small_finish_grad_kernel<<<npass, 256, 0, stream>>>(S);
+        else
+            small_finish_kernel<<<npass, 256, 0, stream>>>(S);
+        LAUNCHED();
+    }
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(g0->ev1, stream));
+    g_last_timed = g0;
     return B200BO_OK;
 }
 
@@ -1598,38 +1654,7 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
         SmallParams S;
         memset(&S, 0, sizeof(S));
         S.P = P;
-        for (int g = 0; g < spec->n_gps; ++g) {
-            b200bo_gp* gp = spec->gps[g];
-            if ((rc = ensure_small(gp))) return rc;
-            S.sg[g].W = gp->W.as<double>();
-            S.sg[g].ksm = gp->s_ksm.as<double>();
-            S.sg[g].partial = gp->s_partial.as<double>();
-            S.sg[g].mu_part = gp->s_mupart.as<double>();
-            S.sg[g].colsq_rb = gp->s_colsq.as<double>();
-            S.sg[g].unit_tab = gp->s_unit.as<int2>();
-            S.sg[g].rb_tab = gp->s_rb.as<int2>();
-            S.nunits[g] = gp->s_nunits;
-        }
-        S.m_end = m;
-        CU(cudaEventRecord(g0->ev0, stream));
-        for (long long c0 = 0; c0 < m; c0 += (long long)SMAXP * SMC) {
-            S.c0 = c0;
-            const long long left = m - c0;
-            const int npass = (int)((left + SMC - 1) / SMC < SMAXP ? (left + SMC - 1) / SMC : SMAXP);
-            for (int g = 0; g < spec->n_gps; ++g) {
-                small_kstar_kernel<<<dim3(spec->gps[g]->np / 128, npass), 256, 0, stream>>>(S, g);
-                small_trsv_kernel<false><<<dim3(spec->gps[g]->s_nunits, (npass + STPG - 1) / STPG), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
-                small_reduce_kernel<0><<<dim3(spec->gps[g]->np / SROWS, npass), 256, 0, stream>>>(S, g);
-                LAUNCHED();
-                LAUNCHED();
-                LAUNCHED();
-            }
-            small_finish_kernel<<<npass, 256, 0, stream>>>(S);
-            LAUNCHED();
-        }
-        CU(cudaGetLastError());
-        CU(cudaEventRecord(g0->ev1, stream));
-        g_last_timed = g0;
+        if ((rc = small_launch(spec, S, m, false, stream))) return rc;
     } else if (grid > 0) {
         if (k > 0) {  // selection fused into the epilogue: no acq[M] needed
             if ((rc = g0->sel_cta.reserve(sizeof(SelList) * (size_t)g0->sm_count))) return rc;
@@ -2017,9 +2042,8 @@ extern "C" int b200bo_acq_eval(const b200bo_acq* spec, const double* Xc, int64_t
     return run_host(spec, Xc, m, acq_neg, nullptr, nullptr, 0, nullptr, nullptr);
 }
 
-// Value and input gradient of the closure on the small-batch kernels (predict_kernels.cuh: small_grad_kernel,
-// small_finish_grad_kernel).  Per launch group of up to SMAXP passes and per GP: K*, v = L^-1 k* (its sums exactly
-// those of the value path), u = L^-T v, the gradient partials; then one finish for every GP.
+// Value and input gradient of the closure on the small-batch kernels (small_launch with grad: v = L^-1 k* and its sums
+// exactly those of the value path).
 extern "C" int b200bo_acq_value_grad(const b200bo_acq* spec, const double* Xc, int64_t m, double* val, double* grad) {
     int rc;
     if ((rc = check_spec(spec))) return rc;
@@ -2045,50 +2069,8 @@ extern "C" int b200bo_acq_value_grad(const b200bo_acq* spec, const double* Xc, i
     if ((rc = g0->clamp.reserve(2 * sizeof(unsigned long long)))) return rc;
     S.P.clamp_count = g0->clamp.as<unsigned long long>();
     CU(cudaMemsetAsync(g0->clamp.p, 0, 2 * sizeof(unsigned long long), stream));
-    for (int g = 0; g < spec->n_gps; ++g) {
-        b200bo_gp* gp = spec->gps[g];
-        if ((rc = ensure_small(gp, true))) return rc;
-        SmallGp& Q = S.sg[g];
-        Q.W = gp->W.as<double>();
-        Q.ksm = gp->s_ksm.as<double>();
-        Q.partial = gp->s_partial.as<double>();
-        Q.mu_part = gp->s_mupart.as<double>();
-        Q.colsq_rb = gp->s_colsq.as<double>();
-        Q.unit_tab = gp->s_unit.as<int2>();
-        Q.rb_tab = gp->s_rb.as<int2>();
-        Q.vsum = gp->s_vsum.as<double>();
-        Q.usum = gp->s_usum.as<double>();
-        Q.partial_u = gp->s_partial_u.as<double>();
-        Q.gpart = gp->s_gpart.as<double>();
-        Q.unit_tab_u = gp->s_unit_u.as<int2>();
-        Q.rb_tab_u = gp->s_rb_u.as<int2>();
-        S.nunits[g] = gp->s_nunits;
-        S.nunits_u[g] = gp->s_nunits_u;
-    }
-    S.m_end = m;
     S.grad_out = g0->out_grad.as<double>();
-    CU(cudaEventRecord(g0->ev0, stream));
-    for (long long c0 = 0; c0 < m; c0 += (long long)SMAXP * SMC) {
-        S.c0 = c0;
-        const long long left = m - c0;
-        const int npass = (int)((left + SMC - 1) / SMC < SMAXP ? (left + SMC - 1) / SMC : SMAXP);
-        const int ngrp = (npass + STPG - 1) / STPG;
-        for (int g = 0; g < spec->n_gps; ++g) {
-            const b200bo_gp* gp = spec->gps[g];
-            small_kstar_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
-            small_trsv_kernel<false><<<dim3(gp->s_nunits, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
-            small_reduce_kernel<1><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
-            small_trsv_kernel<true><<<dim3(gp->s_nunits_u, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
-            small_reduce_kernel<2><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
-            small_grad_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
-            for (int i = 0; i < 6; ++i) LAUNCHED();
-        }
-        small_finish_grad_kernel<<<npass, 256, 0, stream>>>(S);
-        LAUNCHED();
-    }
-    CU(cudaGetLastError());
-    CU(cudaEventRecord(g0->ev1, stream));
-    g_last_timed = g0;
+    if ((rc = small_launch(spec, S, m, true, stream))) return rc;
     g0->stat_total = g0->stat_direct = m;
     g0->prune_counted = false;
     CU(cudaDeviceSynchronize());
@@ -2097,14 +2079,29 @@ extern "C" int b200bo_acq_value_grad(const b200bo_acq* spec, const double* Xc, i
     return check_nonfinite(g0);
 }
 
-static void unpack_records(const SelRecord* sel, int k, double* best_val, int64_t* best_idx, double* topk_val,
+// q sets of (kk+1) records, kk = max(k, 1) (k = 0 still runs one round for the argmin record): set p's argmin into
+// best_*[p], its top k into topk_*[p k, p k + k); every output nullable
+static void unpack_records(const SelRecord* sel, int q, int k, double* best_val, int64_t* best_idx, double* topk_val,
                            int64_t* topk_idx) {
-    if (best_val) *best_val = sel[0].value;
-    if (best_idx) *best_idx = sel[0].index;
-    for (int i = 0; i < k; ++i) {
-        if (topk_val) topk_val[i] = sel[1 + i].value;
-        if (topk_idx) topk_idx[i] = sel[1 + i].index;
+    const int kk = k > 0 ? k : 1;
+    for (int p = 0; p < q; ++p) {
+        const SelRecord* s = sel + (size_t)p * (kk + 1);
+        if (best_val) best_val[p] = s[0].value;
+        if (best_idx) best_idx[p] = s[0].index;
+        for (int i = 0; i < k; ++i) {
+            if (topk_val) topk_val[(size_t)p * k + i] = s[1 + i].value;
+            if (topk_idx) topk_idx[(size_t)p * k + i] = s[1 + i].index;
+        }
     }
+}
+
+// the q sets of records of a finished selection at d_sel, read back and unpacked
+static int read_records(const void* d_sel, int q, int k, double* best_val, int64_t* best_idx, double* topk_val,
+                        int64_t* topk_idx) {
+    std::vector<SelRecord> rec((size_t)q * ((k > 0 ? k : 1) + 1));
+    CU(cudaMemcpy(rec.data(), d_sel, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
+    unpack_records(rec.data(), q, k, best_val, best_idx, topk_val, topk_idx);
+    return B200BO_OK;
 }
 
 extern "C" int b200bo_acq_argmin_topk(const b200bo_acq* spec, const double* Xc, int64_t m, int k,
@@ -2117,23 +2114,32 @@ extern "C" int b200bo_acq_argmin_topk(const b200bo_acq* spec, const double* Xc, 
     // k = 0 still needs the argmin record: run the selection with one round
     int rc = run_host(spec, Xc, m, acq_neg, nullptr, nullptr, k > 0 ? k : 1, sel, nullptr);
     if (rc) return rc;
-    unpack_records(sel, k, best_val, best_idx, topk_val, topk_idx);
+    unpack_records(sel, 1, k, best_val, best_idx, topk_val, topk_idx);
     return B200BO_OK;
 }
 
 // ---------------------------------------------------------------------------------------
 // throughput mode (device Philox candidates)
 // ---------------------------------------------------------------------------------------
-// coordinates of the records' rows, regenerated on the device of g0 into host memory (k+1 rows)
-static int philox_rows_of_records(b200bo_gp* g0, uint64_t seed, const SelRecord* d_rec, int nrec, int d,
-                                  double* rows_host, cudaStream_t stream) {
+// The Philox rows of q sets of (kk+1) merged records at d_rec (kk = max(k, 1)), regenerated on stream into prow from
+// the device bounds pbounds: best_x (q,d), topk_x (q,k,d) host, either nullable
+static int philox_winner_rows(DevBuf& prow, const DevBuf& pbounds, uint64_t seed, const SelRecord* d_rec, int q, int k,
+                              int d, double* best_x, double* topk_x, cudaStream_t stream) {
+    if (!best_x && !(topk_x && k > 0)) return B200BO_OK;
+    const int kk = k > 0 ? k : 1, nrec = q * (kk + 1);
     int rc;
-    if ((rc = g0->prow.reserve(sizeof(double) * (size_t)(B200BO_MAX_TOPK + 1) * B200BO_MAX_DIM))) return rc;
-    philox_rows_kernel<<<nrec, 64, 0, stream>>>(seed, g0->pbounds.as<double>(), d, d_rec, nrec, g0->prow.as<double>());
+    if ((rc = prow.reserve(sizeof(double) * (size_t)nrec * d))) return rc;
+    philox_rows_kernel<<<nrec, 64, 0, stream>>>(seed, pbounds.as<double>(), d, d_rec, nrec, prow.as<double>());
     LAUNCHED();
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(rows_host, g0->prow.p, sizeof(double) * (size_t)nrec * d, cudaMemcpyDeviceToHost, stream));
+    std::vector<double> rows((size_t)nrec * d);
+    CU(cudaMemcpyAsync(rows.data(), prow.p, sizeof(double) * rows.size(), cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));
+    for (int p = 0; p < q; ++p) {
+        const double* rp = rows.data() + (size_t)p * (kk + 1) * d;
+        if (best_x) memcpy(best_x + (size_t)p * d, rp, sizeof(double) * d);
+        if (topk_x && k > 0) memcpy(topk_x + (size_t)p * k * d, rp + d, sizeof(double) * (size_t)k * d);
+    }
     return B200BO_OK;
 }
 
@@ -2151,17 +2157,8 @@ extern "C" int b200bo_acq_argmin_topk_philox(const b200bo_acq* spec, uint64_t se
     if ((rc = g0->sel.reserve(sizeof(SelRecord) * (B200BO_MAX_TOPK + 1)))) return rc;
     const int kk = k > 0 ? k : 1;
     if ((rc = b200bo_acq_select_philox_dev(spec, seed, lo, hi, m, index_base, kk, g0->sel.p, nullptr))) return rc;
-    SelRecord sel[B200BO_MAX_TOPK + 1];
-    CU(cudaMemcpy(sel, g0->sel.p, sizeof(SelRecord) * (kk + 1), cudaMemcpyDeviceToHost));
-    unpack_records(sel, k, best_val, best_idx, topk_val, topk_idx);
-    if (best_x || (topk_x && k > 0)) {
-        std::vector<double> rows((size_t)(kk + 1) * g0->d);
-        if ((rc = philox_rows_of_records(g0, seed, g0->sel.as<SelRecord>(), kk + 1, g0->d, rows.data(), nullptr)))
-            return rc;
-        if (best_x) memcpy(best_x, rows.data(), sizeof(double) * g0->d);
-        if (topk_x && k > 0) memcpy(topk_x, rows.data() + g0->d, sizeof(double) * (size_t)k * g0->d);
-    }
-    return B200BO_OK;
+    if ((rc = read_records(g0->sel.p, 1, k, best_val, best_idx, topk_val, topk_idx))) return rc;
+    return philox_winner_rows(g0->prow, g0->pbounds, seed, g0->sel.as<SelRecord>(), 1, k, g0->d, best_x, topk_x, nullptr);
 }
 
 extern "C" int b200bo_philox_rows(int device, uint64_t seed, const double* lo, const double* hi, int d,
@@ -2171,7 +2168,7 @@ extern "C" int b200bo_philox_rows(int device, uint64_t seed, const double* lo, c
     if (n_idx == 0) return B200BO_OK;
     CU(cudaSetDevice(device));
     std::vector<SelRecord> rec((size_t)n_idx);
-    std::vector<double> pb(2 * d);
+    std::vector<double> pb(2 * d);  // pack_pbounds' layout, unchecked: rows of any bounds, lo > hi included
     for (int j = 0; j < d; ++j) {
         pb[j] = lo[j];
         pb[d + j] = hi[j] - lo[j];
@@ -2180,19 +2177,17 @@ extern "C" int b200bo_philox_rows(int device, uint64_t seed, const double* lo, c
         rec[i].value = 0.0;
         rec[i].index = idx[i];
     }
-    SelRecord* d_rec = nullptr;
-    double *d_pb = nullptr, *d_out = nullptr;
-    CU(cudaMalloc(&d_rec, sizeof(SelRecord) * n_idx));
-    CU(cudaMalloc(&d_pb, sizeof(double) * 2 * d));
-    CU(cudaMalloc(&d_out, sizeof(double) * n_idx * d));
-    CU(cudaMemcpy(d_rec, rec.data(), sizeof(SelRecord) * n_idx, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(d_pb, pb.data(), sizeof(double) * 2 * d, cudaMemcpyHostToDevice));
-    philox_rows_kernel<<<(unsigned)n_idx, 64>>>(seed, d_pb, d, d_rec, (int)n_idx, d_out);
+    DevBuf d_rec, d_pb, d_out;
+    int rc;
+    if ((rc = d_rec.reserve(sizeof(SelRecord) * n_idx))) return rc;
+    if ((rc = d_pb.reserve(sizeof(double) * 2 * d))) return rc;
+    if ((rc = d_out.reserve(sizeof(double) * n_idx * d))) return rc;
+    CU(cudaMemcpy(d_rec.p, rec.data(), sizeof(SelRecord) * n_idx, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_pb.p, pb.data(), sizeof(double) * 2 * d, cudaMemcpyHostToDevice));
+    philox_rows_kernel<<<(unsigned)n_idx, 64>>>(seed, d_pb.as<double>(), d, d_rec.as<SelRecord>(), (int)n_idx,
+                                                d_out.as<double>());
     LAUNCHED();
-    cudaError_t e = cudaMemcpy(out, d_out, sizeof(double) * n_idx * d, cudaMemcpyDeviceToHost);
-    cudaFree(d_rec);
-    cudaFree(d_pb);
-    cudaFree(d_out);
+    cudaError_t e = cudaMemcpy(out, d_out.p, sizeof(double) * n_idx * d, cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) return set_err(B200BO_ERR_CUDA, "philox_rows: %s", cudaGetErrorString(e));
     return B200BO_OK;
 }
@@ -2294,22 +2289,6 @@ static int paths_check_nonfinite(b200bo_paths* ps) {
     return B200BO_OK;
 }
 
-static void paths_unpack(const std::vector<SelRecord>& rec, int q, int k, double* best_val, int64_t* best_idx,
-                         double* topk_val, int64_t* topk_idx) {
-    const int kk = k > 0 ? k : 1;
-    for (int p = 0; p < q; ++p)
-        unpack_records(rec.data() + (size_t)p * (kk + 1), k, best_val ? best_val + p : nullptr,
-                       best_idx ? best_idx + p : nullptr, topk_val ? topk_val + (size_t)p * k : nullptr,
-                       topk_idx ? topk_idx + (size_t)p * k : nullptr);
-}
-
-struct ScopedBufs {
-    DevBuf b[4];
-    ~ScopedBufs() {
-        for (DevBuf& x : b) x.release();
-    }
-};
-
 // copies of the GP's evaluation state, the draws, and V = K^-1 (y_norm - Phi(Xs) W - eps) column by column
 static int paths_setup(b200bo_gp* gp, b200bo_paths* ps, const double* omega, const double* bv, const double* w,
                        const double* eps) {
@@ -2368,8 +2347,7 @@ static int paths_setup(b200bo_gp* gp, b200bo_paths* ps, const double* omega, con
     for (int i = 0; i < n; ++i)
         for (int p = 0; p < q; ++p)
             R[(size_t)p * np + i] = gp->y_norm[i] - prior[(size_t)i * q + p] - eps[(size_t)i * q + p];
-    ScopedBufs s;
-    DevBuf &r = s.b[0], &x = s.b[1], &t1 = s.b[2], &t2 = s.b[3];
+    DevBuf r, x, t1, t2;
     if ((rc = r.reserve(sizeof(double) * R.size()))) return rc;
     if ((rc = x.reserve(sizeof(double) * R.size()))) return rc;
     if ((rc = t1.reserve(sizeof(double) * np))) return rc;
@@ -2431,32 +2409,9 @@ extern "C" int b200bo_paths_create(b200bo_gp* gp, int q, int L, const double* om
 
 extern "C" void b200bo_paths_destroy(b200bo_paths* ps) {
     if (!ps) return;
-    cudaSetDevice(ps->device);
-    DevBuf* bufs[] = {&ps->Xs, &ps->V, &ps->omega, &ps->bias, &ps->W, &ps->ls, &ps->xf, &ps->xc,
-                      &ps->out, &ps->sel_cta, &ps->sel, &ps->pbounds, &ps->prow, &ps->bad,
-                      &ps->cvals, &ps->cmerit, &ps->craw, &ps->pidx, &ps->grad};
-    for (DevBuf* b : bufs) b->release();
+    cudaSetDevice(ps->device);  // the buffers are freed by delete, on this device
     ps->upload.release();
     delete ps;
-}
-
-extern "C" int b200bo_paths_eval(b200bo_paths* ps, const double* Xc, int64_t m, double* out) {
-    if (!ps || m < 0 || (m > 0 && (!Xc || !out))) return set_err(B200BO_ERR_ARG, "bad arguments");
-    if (m == 0) return B200BO_OK;
-    CU(cudaSetDevice(ps->device));
-    NvtxRange nvtx_range("b200bo:paths_eval");
-    int rc;
-    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * ps->d))) return rc;
-    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m * ps->q))) return rc;
-    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * ps->d, cudaMemcpyHostToDevice));
-    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
-    PathsParams P = paths_params(ps);
-    P.Xc = ps->xc.as<double>();
-    P.m = m;
-    P.out = ps->out.as<double>();
-    if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
-    CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m * ps->q, cudaMemcpyDeviceToHost));
-    return paths_check_nonfinite(ps);
 }
 
 // path_idx (m,) host: every entry in [0, q), then copied into dst->pidx
@@ -2470,24 +2425,44 @@ static int paths_upload_rows(b200bo_paths* dst, int q, const int* path_idx, int6
     return B200BO_OK;
 }
 
+// The evaluation kernel over m host rows into ps->out: (m, q) values, or with path_idx (row mode) row i on path
+// path_idx[i] only, (m,) values.  P: the parameters it ran with.
+static int paths_eval_launch(b200bo_paths* ps, const double* Xc, const int* path_idx, int64_t m, PathsParams& P) {
+    int rc;
+    if (path_idx && (rc = paths_upload_rows(ps, ps->q, path_idx, m))) return rc;
+    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * ps->d))) return rc;
+    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m * (path_idx ? 1 : ps->q)))) return rc;
+    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * ps->d, cudaMemcpyHostToDevice));
+    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
+    P = paths_params(ps);
+    P.Xc = ps->xc.as<double>();
+    P.m = m;
+    P.out = ps->out.as<double>();
+    if (path_idx) P.path_idx = ps->pidx.as<int>();
+    return paths_launch(ps, P, paths_grid(ps, m), nullptr);
+}
+
+extern "C" int b200bo_paths_eval(b200bo_paths* ps, const double* Xc, int64_t m, double* out) {
+    if (!ps || m < 0 || (m > 0 && (!Xc || !out))) return set_err(B200BO_ERR_ARG, "bad arguments");
+    if (m == 0) return B200BO_OK;
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_eval");
+    PathsParams P;
+    int rc;
+    if ((rc = paths_eval_launch(ps, Xc, nullptr, m, P))) return rc;
+    CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m * ps->q, cudaMemcpyDeviceToHost));
+    return paths_check_nonfinite(ps);
+}
+
 extern "C" int b200bo_paths_eval_rows(b200bo_paths* ps, const double* Xc, const int* path_idx, int64_t m,
                                       double* out) {
     if (!ps || m < 0 || (m > 0 && (!Xc || !path_idx || !out))) return set_err(B200BO_ERR_ARG, "bad arguments");
     if (m == 0) return B200BO_OK;
     CU(cudaSetDevice(ps->device));
     NvtxRange nvtx_range("b200bo:paths_eval_rows");
+    PathsParams P;
     int rc;
-    if ((rc = paths_upload_rows(ps, ps->q, path_idx, m))) return rc;
-    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * ps->d))) return rc;
-    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m))) return rc;
-    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * ps->d, cudaMemcpyHostToDevice));
-    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
-    PathsParams P = paths_params(ps);
-    P.Xc = ps->xc.as<double>();
-    P.m = m;
-    P.out = ps->out.as<double>();
-    P.path_idx = ps->pidx.as<int>();
-    if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
+    if ((rc = paths_eval_launch(ps, Xc, path_idx, m, P))) return rc;
     CU(cudaMemcpy(out, ps->out.p, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost));
     return paths_check_nonfinite(ps);
 }
@@ -2502,19 +2477,10 @@ extern "C" int b200bo_paths_grad_rows(b200bo_paths* ps, const double* Xc, const 
     CU(cudaSetDevice(ps->device));
     NvtxRange nvtx_range("b200bo:paths_grad_rows");
     const int d = ps->d;
+    PathsParams P;
     int rc;
-    if ((rc = paths_upload_rows(ps, ps->q, path_idx, m))) return rc;
-    if ((rc = ps->xc.reserve(sizeof(double) * (size_t)m * d))) return rc;
-    if ((rc = ps->out.reserve(sizeof(double) * (size_t)m))) return rc;
+    if ((rc = paths_eval_launch(ps, Xc, path_idx, m, P))) return rc;
     if ((rc = ps->grad.reserve(sizeof(double) * (size_t)m * d))) return rc;
-    CU(cudaMemcpy(ps->xc.p, Xc, sizeof(double) * (size_t)m * d, cudaMemcpyHostToDevice));
-    CU(cudaMemset(ps->bad.p, 0, 2 * sizeof(unsigned long long)));
-    PathsParams P = paths_params(ps);
-    P.Xc = ps->xc.as<double>();
-    P.m = m;
-    P.out = ps->out.as<double>();
-    P.path_idx = ps->pidx.as<int>();
-    if ((rc = paths_launch(ps, P, paths_grid(ps, m), nullptr))) return rc;
     double* dg = ps->grad.as<double>();
     switch (ps->cov) {
         case 0: paths_grad_kernel<0><<<(unsigned)m, PG_NT>>>(P, dg); break;
@@ -2564,45 +2530,17 @@ extern "C" int b200bo_paths_argmin_topk(b200bo_paths* ps, const double* Xc, int6
     if (rc) return rc;
     if ((rc = paths_merge(ps, grid, kk, U.exec))) return rc;
     CU(cudaStreamSynchronize(U.exec));
-    std::vector<SelRecord> rec((size_t)q * (kk + 1));
-    CU(cudaMemcpy(rec.data(), ps->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
     if ((rc = paths_check_nonfinite(ps))) return rc;
-    paths_unpack(rec, q, k, best_val, best_idx, topk_val, topk_idx);
-    return B200BO_OK;
+    return read_records(ps->sel.p, q, k, best_val, best_idx, topk_val, topk_idx);
 }
 
-// Philox bounds (lo_j, hi_j - lo_j) of the throughput mode into ps->pbounds
+// Philox bounds into ps->pbounds, on the device when this returns (the selection may run on a non-blocking stream)
 static int paths_set_pbounds(b200bo_paths* ps, const double* lo, const double* hi) {
-    const int d = ps->d;
     double pb[2 * B200BO_MAX_DIM];
-    for (int j = 0; j < d; ++j) {
-        if (!(lo[j] <= hi[j])) return set_err(B200BO_ERR_ARG, "Philox bounds: lo > hi in column %d", j);
-        pb[j] = lo[j];
-        pb[d + j] = hi[j] - lo[j];
-    }
     int rc;
+    if ((rc = pack_pbounds(lo, hi, ps->d, pb))) return rc;
     if ((rc = ps->pbounds.reserve(sizeof(double) * 2 * B200BO_MAX_DIM))) return rc;
-    CU(cudaMemcpy(ps->pbounds.p, pb, sizeof(double) * 2 * d, cudaMemcpyHostToDevice));
-    return B200BO_OK;
-}
-
-// the Philox rows of the q (k+1) merged records in ps->sel: best_x (q,d), topk_x (q,k,d) host, either nullable
-static int paths_winner_rows(b200bo_paths* ps, uint64_t seed, int k, double* best_x, double* topk_x) {
-    if (!best_x && !(topk_x && k > 0)) return B200BO_OK;
-    const int kk = k > 0 ? k : 1, d = ps->d, q = ps->q, nrec = q * (kk + 1);
-    int rc;
-    if ((rc = ps->prow.reserve(sizeof(double) * (size_t)nrec * d))) return rc;
-    philox_rows_kernel<<<nrec, 64>>>(seed, ps->pbounds.as<double>(), d, ps->sel.as<SelRecord>(), nrec,
-                                     ps->prow.as<double>());
-    LAUNCHED();
-    CU(cudaGetLastError());
-    std::vector<double> rows((size_t)nrec * d);
-    CU(cudaMemcpy(rows.data(), ps->prow.p, sizeof(double) * rows.size(), cudaMemcpyDeviceToHost));
-    for (int p = 0; p < q; ++p) {
-        const double* rp = rows.data() + (size_t)p * (kk + 1) * d;
-        if (best_x) memcpy(best_x + (size_t)p * d, rp, sizeof(double) * d);
-        if (topk_x && k > 0) memcpy(topk_x + (size_t)p * k * d, rp + d, sizeof(double) * (size_t)k * d);
-    }
+    CU(cudaMemcpy(ps->pbounds.p, pb, sizeof(double) * 2 * ps->d, cudaMemcpyHostToDevice));
     return B200BO_OK;
 }
 
@@ -2630,10 +2568,8 @@ extern "C" int b200bo_paths_argmin_topk_philox(b200bo_paths* ps, uint64_t seed, 
     P.sel_k = kk;
     if ((rc = paths_launch(ps, P, grid, nullptr))) return rc;
     if ((rc = paths_merge(ps, grid, kk, nullptr))) return rc;
-    std::vector<SelRecord> rec((size_t)q * (kk + 1));
-    CU(cudaMemcpy(rec.data(), ps->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
-    paths_unpack(rec, q, k, best_val, best_idx, topk_val, topk_idx);
-    return paths_winner_rows(ps, seed, k, best_x, topk_x);
+    if ((rc = read_records(ps->sel.p, q, k, best_val, best_idx, topk_val, topk_idx))) return rc;
+    return philox_winner_rows(ps->prow, ps->pbounds, seed, ps->sel.as<SelRecord>(), q, k, ps->d, best_x, topk_x, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2789,10 +2725,7 @@ extern "C" int b200bo_cpaths_argmin_topk(b200bo_paths* const* sets, int G, const
     NvtxRange nvtx_range("b200bo:cpaths_select");
     const int kk = k > 0 ? k : 1;
     if ((rc = cpaths_run(sets, C, Xc, 0, m, 0, kk, nullptr, nullptr))) return rc;
-    std::vector<SelRecord> rec((size_t)C.q * (kk + 1));
-    CU(cudaMemcpy(rec.data(), s0->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
-    paths_unpack(rec, C.q, k, best_val, best_idx, topk_val, topk_idx);
-    return B200BO_OK;
+    return read_records(s0->sel.p, C.q, k, best_val, best_idx, topk_val, topk_idx);
 }
 
 extern "C" int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G, const double* lb,
@@ -2812,10 +2745,9 @@ extern "C" int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G
     const int kk = k > 0 ? k : 1;
     if ((rc = paths_set_pbounds(s0, lo, hi))) return rc;
     if ((rc = cpaths_run(sets, C, nullptr, seed, m, index_base, kk, nullptr, nullptr))) return rc;
-    std::vector<SelRecord> rec((size_t)C.q * (kk + 1));
-    CU(cudaMemcpy(rec.data(), s0->sel.p, sizeof(SelRecord) * rec.size(), cudaMemcpyDeviceToHost));
-    paths_unpack(rec, C.q, k, best_val, best_idx, topk_val, topk_idx);
-    return paths_winner_rows(s0, seed, k, best_x, topk_x);
+    if ((rc = read_records(s0->sel.p, C.q, k, best_val, best_idx, topk_val, topk_idx))) return rc;
+    return philox_winner_rows(s0->prow, s0->pbounds, seed, s0->sel.as<SelRecord>(), C.q, k, s0->d, best_x, topk_x,
+                              nullptr);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -2828,19 +2760,8 @@ extern "C" int b200bo_gp_replicate(const b200bo_gp* src, int device, b200bo_gp**
     int rc;
     if ((rc = b200bo_gp_create(&dst, device))) return rc;
     NvtxRange nvtx_range("b200bo:replicate");
-    dst->n = src->n;
+    copy_model_state(src, dst);
     dst->np = src->np;
-    dst->d = src->d;
-    dst->family = src->family;
-    dst->nu = src->nu;
-    dst->constv = src->constv;
-    dst->jitter = src->jitter;
-    dst->noise = src->noise;
-    dst->y_mean = src->y_mean;
-    dst->y_std = src->y_std;
-    dst->normalize = src->normalize;
-    dst->xform = src->xform;
-    dst->precision = src->precision;
     dst->replica = true;
     const size_t np = src->np, d = src->d;
     struct Item {
@@ -2878,6 +2799,7 @@ extern "C" int b200bo_gp_replicate(const b200bo_gp* src, int device, b200bo_gp**
 struct NcclApi {
     void* handle = nullptr;
     ncclResult_t (*CommInitAll)(ncclComm_t*, int, const int*) = nullptr;
+    ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
     ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
     ncclResult_t (*GroupStart)() = nullptr;
     ncclResult_t (*GroupEnd)() = nullptr;
@@ -2892,11 +2814,13 @@ static int load_nccl() {
     if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
     if (!h) return set_err(B200BO_ERR_CUDA, "cannot load libnccl.so.2: %s", dlerror());
     g_nccl.CommInitAll = (decltype(g_nccl.CommInitAll))dlsym(h, "ncclCommInitAll");
+    g_nccl.CommDestroy = (decltype(g_nccl.CommDestroy))dlsym(h, "ncclCommDestroy");
     g_nccl.AllGather = (decltype(g_nccl.AllGather))dlsym(h, "ncclAllGather");
     g_nccl.GroupStart = (decltype(g_nccl.GroupStart))dlsym(h, "ncclGroupStart");
     g_nccl.GroupEnd = (decltype(g_nccl.GroupEnd))dlsym(h, "ncclGroupEnd");
     g_nccl.GetErrorString = (decltype(g_nccl.GetErrorString))dlsym(h, "ncclGetErrorString");
-    if (!g_nccl.CommInitAll || !g_nccl.AllGather || !g_nccl.GroupStart || !g_nccl.GroupEnd || !g_nccl.GetErrorString)
+    if (!g_nccl.CommInitAll || !g_nccl.CommDestroy || !g_nccl.AllGather || !g_nccl.GroupStart || !g_nccl.GroupEnd ||
+        !g_nccl.GetErrorString)
         return set_err(B200BO_ERR_CUDA, "libnccl.so.2 lacks a required symbol");
     g_nccl.handle = h;
     return B200BO_OK;
@@ -2913,13 +2837,42 @@ constexpr int kMaxDev = 16;
 struct MultiCtx {
     int n = 0;
     int dev[kMaxDev];
+    bool has_comm = false;
     ncclComm_t comm[kMaxDev];
-    cudaStream_t stream[kMaxDev];
-    SelRecord* sel[kMaxDev];     // (MAX_TOPK+1) local records on device g
-    SelRecord* gather[kMaxDev];  // n * (MAX_TOPK+1) records on device g
-    SelRecord* merged = nullptr; // (MAX_TOPK+1) on device 0
+    cudaStream_t stream[kMaxDev] = {};
+    SelRecord* sel[kMaxDev] = {};     // (MAX_TOPK+1) local records on device g
+    SelRecord* gather[kMaxDev] = {};  // n * (MAX_TOPK+1) records on device g
+    SelRecord* merged = nullptr;      // (MAX_TOPK+1) on device 0
 };
 static std::map<std::vector<int>, MultiCtx*> g_multi;
+
+// communicators, streams and exchange buffers of c->dev[0..n)
+static int multi_ctx_init(MultiCtx* c) {
+    NC(g_nccl.CommInitAll(c->comm, c->n, c->dev));
+    c->has_comm = true;
+    for (int g = 0; g < c->n; ++g) {
+        CU(cudaSetDevice(c->dev[g]));
+        CU(cudaStreamCreateWithFlags(&c->stream[g], cudaStreamNonBlocking));
+        CU(cudaMalloc(&c->sel[g], sizeof(SelRecord) * (B200BO_MAX_TOPK + 1)));
+        CU(cudaMalloc(&c->gather[g], sizeof(SelRecord) * (B200BO_MAX_TOPK + 1) * c->n));
+    }
+    CU(cudaSetDevice(c->dev[0]));
+    CU(cudaMalloc(&c->merged, sizeof(SelRecord) * (B200BO_MAX_TOPK + 1)));
+    return B200BO_OK;
+}
+
+// frees whatever multi_ctx_init built of c before it failed, then c
+static void multi_ctx_free(MultiCtx* c) {
+    for (int g = 0; g < c->n; ++g) {
+        cudaSetDevice(c->dev[g]);
+        if (c->has_comm) g_nccl.CommDestroy(c->comm[g]);
+        if (c->stream[g]) cudaStreamDestroy(c->stream[g]);
+        cudaFree(c->sel[g]);
+        cudaFree(c->gather[g]);
+        if (g == 0) cudaFree(c->merged);
+    }
+    delete c;
+}
 
 // communicators + exchange buffers for a device list (created on first use, kept for the process lifetime)
 static int multi_ctx(const b200bo_acq* specs, int n_dev, MultiCtx** out) {
@@ -2944,15 +2897,10 @@ static int multi_ctx(const b200bo_acq* specs, int n_dev, MultiCtx** out) {
     MultiCtx* c = new MultiCtx();
     c->n = n_dev;
     for (int g = 0; g < n_dev; ++g) c->dev[g] = devs[g];
-    NC(g_nccl.CommInitAll(c->comm, n_dev, c->dev));
-    for (int g = 0; g < n_dev; ++g) {
-        CU(cudaSetDevice(c->dev[g]));
-        CU(cudaStreamCreateWithFlags(&c->stream[g], cudaStreamNonBlocking));
-        CU(cudaMalloc(&c->sel[g], sizeof(SelRecord) * (B200BO_MAX_TOPK + 1)));
-        CU(cudaMalloc(&c->gather[g], sizeof(SelRecord) * (B200BO_MAX_TOPK + 1) * n_dev));
+    if ((rc = multi_ctx_init(c))) {
+        multi_ctx_free(c);
+        return rc;
     }
-    CU(cudaSetDevice(c->dev[0]));
-    CU(cudaMalloc(&c->merged, sizeof(SelRecord) * (B200BO_MAX_TOPK + 1)));
     g_multi[devs] = c;
     *out = c;
     return B200BO_OK;
@@ -3035,7 +2983,7 @@ extern "C" int b200bo_multi_gpu_acq_argmin_topk(const b200bo_acq* specs, int n_d
         CU(cudaSetDevice(specs[g].gps[0]->device));
         if (specs[g].gps[0]->clamp.p && (rc = check_nonfinite(specs[g].gps[0]))) return rc;
     }
-    unpack_records(sel, k, best_val, best_idx, topk_val, topk_idx);
+    unpack_records(sel, 1, k, best_val, best_idx, topk_val, topk_idx);
     return B200BO_OK;
 }
 
@@ -3070,16 +3018,11 @@ extern "C" int b200bo_multi_gpu_acq_argmin_topk_philox(const b200bo_acq* specs, 
     if (rc) return rc;
     SelRecord sel[B200BO_MAX_TOPK + 1];
     if ((rc = multi_exchange(c, kk, sel))) return rc;
-    unpack_records(sel, k, best_val, best_idx, topk_val, topk_idx);
-    if (best_x || (topk_x && k > 0)) {
-        b200bo_gp* g0 = specs[0].gps[0];
-        CU(cudaSetDevice(g0->device));
-        std::vector<double> rows((size_t)(kk + 1) * g0->d);
-        if ((rc = philox_rows_of_records(g0, seed, c->merged, kk + 1, g0->d, rows.data(), c->stream[0]))) return rc;
-        if (best_x) memcpy(best_x, rows.data(), sizeof(double) * g0->d);
-        if (topk_x && k > 0) memcpy(topk_x, rows.data() + g0->d, sizeof(double) * (size_t)k * g0->d);
-    }
-    return B200BO_OK;
+    unpack_records(sel, 1, k, best_val, best_idx, topk_val, topk_idx);
+    if (!best_x && !(topk_x && k > 0)) return B200BO_OK;
+    b200bo_gp* g0 = specs[0].gps[0];
+    CU(cudaSetDevice(g0->device));
+    return philox_winner_rows(g0->prow, g0->pbounds, seed, c->merged, 1, k, g0->d, best_x, topk_x, c->stream[0]);
 }
 
 extern "C" int b200bo_multi_gpu_acq_eval(const b200bo_acq* specs, int n_dev, const double* Xc, int64_t m,

@@ -112,6 +112,12 @@ class PosteriorPaths:
                                       B.as_dp(B.c_f64(b)), B.as_dp(B.c_f64(w)), B.as_dp(B.c_f64(eps)),
                                       C.byref(self._handle.ptr)))
 
+    # the selection entry points: _c_select and _c_select + "_philox", called with _args() in front
+    _c_select = "b200bo_paths_argmin_topk"
+
+    def _args(self):
+        return (self._handle.ptr,)
+
     def _candidates(self, X):
         X = B.c_f64(np.asarray(X, dtype=np.float64).reshape(-1, self.dim))
         mode, arg = self._xform
@@ -150,14 +156,14 @@ class PosteriorPaths:
         return vals, grads
 
     def argmin_topk(self, X, k):
-        """Per path p: np.argmin and the k smallest (np.argsort order) of -path_p over the rows of X.
-        Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
+        """Per path p: np.argmin and the k smallest (np.argsort order) of -path_p (ConstrainedPaths: -merit_p) over
+        the rows of X.  Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
         X = self._candidates(X)
         k = int(k)
         q = self.n_paths
         bv, bi = np.empty(q), np.empty(q, dtype=np.int64)
         tv, ti = np.empty(q * max(k, 1)), np.empty(q * max(k, 1), dtype=np.int64)
-        B.check(B.lib().b200bo_paths_argmin_topk(self._handle.ptr, B.as_dp(X), X.shape[0], k, B.as_dp(bv),
+        B.check(getattr(B.lib(), self._c_select)(*self._args(), B.as_dp(X), X.shape[0], k, B.as_dp(bv),
                                                  bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tv),
                                                  ti.ctypes.data_as(C.POINTER(C.c_int64))))
         tops = [t[t >= 0] for t in ti[:q * k].reshape(q, k)]
@@ -175,8 +181,8 @@ class PosteriorPaths:
         kk = max(k, 1)
         bv, bi, bx = np.empty(q), np.empty(q, dtype=np.int64), np.empty((q, d))
         tv, ti, tx = np.empty(q * kk), np.empty(q * kk, dtype=np.int64), np.empty((q * kk, d))
-        B.check(B.lib().b200bo_paths_argmin_topk_philox(
-            self._handle.ptr, int(seed) & 0xFFFFFFFFFFFFFFFF, B.as_dp(lo), B.as_dp(hi), int(m), int(index_base), k,
+        B.check(getattr(B.lib(), self._c_select + "_philox")(
+            *self._args(), int(seed) & 0xFFFFFFFFFFFFFFFF, B.as_dp(lo), B.as_dp(hi), int(m), int(index_base), k,
             B.as_dp(bv), bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(bx), B.as_dp(tv),
             ti.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tx)))
         ti, tx = ti[:q * k].reshape(q, k), tx[:q * k].reshape(q, k, d)
@@ -271,37 +277,10 @@ class ConstrainedPaths:
                                                 X.shape[0], B.as_dp(out)))
         return out
 
-    def argmin_topk(self, X, k):
-        """Per path p: np.argmin and the k smallest (np.argsort order) of -merit_p over the rows of X.
-        Returns (idx (q,), values (q,), [top-k indices of path p for p < q])."""
-        X = self._candidates(X)
-        k, q = int(k), self.n_paths
-        bv, bi = np.empty(q), np.empty(q, dtype=np.int64)
-        tv, ti = np.empty(q * max(k, 1)), np.empty(q * max(k, 1), dtype=np.int64)
-        B.check(B.lib().b200bo_cpaths_argmin_topk(*self._args(), B.as_dp(X), X.shape[0], k, B.as_dp(bv),
-                                                  bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tv),
-                                                  ti.ctypes.data_as(C.POINTER(C.c_int64))))
-        tops = [t[t >= 0] for t in ti[:q * k].reshape(q, k)]
-        return bi, bv, tops
-
-    def argmin_topk_philox(self, seed, bounds, m, k, index_base=0):
-        """Throughput mode as PosteriorPaths.argmin_topk_philox, ranking -merit_p.
-        Returns (idx (q,), values (q,), x_best (q, d), [top-k indices], [top-k rows])."""
-        if self._xform[0] == "host":
-            raise NotImplementedError("device candidate generation with a host-side kernel transform")
-        bounds = B.c_f64(np.asarray(bounds, dtype=np.float64).reshape(self.dim, 2))
-        lo, hi = B.c_f64(bounds[:, 0]), B.c_f64(bounds[:, 1])
-        k, q, d = int(k), self.n_paths, self.dim
-        kk = max(k, 1)
-        bv, bi, bx = np.empty(q), np.empty(q, dtype=np.int64), np.empty((q, d))
-        tv, ti, tx = np.empty(q * kk), np.empty(q * kk, dtype=np.int64), np.empty((q * kk, d))
-        B.check(B.lib().b200bo_cpaths_argmin_topk_philox(
-            *self._args(), int(seed) & 0xFFFFFFFFFFFFFFFF, B.as_dp(lo), B.as_dp(hi), int(m), int(index_base), k,
-            B.as_dp(bv), bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(bx), B.as_dp(tv),
-            ti.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tx)))
-        ti, tx = ti[:q * k].reshape(q, k), tx[:q * k].reshape(q, k, d)
-        keep = ti >= 0
-        return bi, bv, bx, [ti[p][keep[p]] for p in range(q)], [tx[p][keep[p]] for p in range(q)]
+    # PosteriorPaths' selection over the b200bo_cpaths_* entry points, ranking -merit_p
+    _c_select = "b200bo_cpaths_argmin_topk"
+    argmin_topk = PosteriorPaths.argmin_topk
+    argmin_topk_philox = PosteriorPaths.argmin_topk_philox
 
 
 class PathAcquisition:
