@@ -1,7 +1,7 @@
 """bayesianoptimization_b200 - a H100-native GP-surrogate + acquisition engine that drops in
 behind ``bayes_opt.BayesianOptimization.suggest()`` and the ``bayes_opt.acquisition`` classes.
 
-Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI/MES/LogEI/LogPoI (x constraint probability) ->
+Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI/MES/LogEI/LogPoI/NEI/LogNEI (x constraint probability) ->
 argmin/top-k, in hand-written sm_90a CUDA behind the C ABI declared in include/b200bo.h.
 No CPU fallback: importing the compute classes without the built library raises ImportError.
 
@@ -10,7 +10,7 @@ Two layers:
     PosteriorPaths, ConstrainedPaths (posterior sample paths, resolved lazily)
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, LogExpectedImprovement,
-    LogProbabilityOfImprovement, ThompsonSampling,
+    LogProbabilityOfImprovement, NoisyExpectedImprovement, LogNoisyExpectedImprovement, ThompsonSampling,
     ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, KrigingBeliever, GPHedge, AcquisitionFunction,
     ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
 """
@@ -29,6 +29,7 @@ _PLUGIN = {
     "ConstantLiar": "acquisition", "GPHedge": "acquisition", "DeviceHooks": "acquisition",
     "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
     "MaxValueEntropySearch": "acquisition", "suggest_batch": "acquisition", "KrigingBeliever": "acquisition",
+    "NoisyExpectedImprovement": "acquisition", "LogNoisyExpectedImprovement": "acquisition",
     "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
 }
 

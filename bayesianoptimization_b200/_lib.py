@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(HERE, "libb200bo.so")
 OK, ERR_CUDA, ERR_ARG, ERR_NOT_PD, ERR_UNSUPPORTED, ERR_STATE = 0, -1, -2, -3, -4, -5
 KERNEL_MATERN, KERNEL_RBF = 0, 1
 NU_05, NU_15, NU_25, NU_INF = 0, 1, 2, 3
-ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE, ACQ_MES, ACQ_LOGEI, ACQ_LOGPOI = 0, 1, 2, 3, 4, 6, 7
+ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE, ACQ_MES, ACQ_LOGEI, ACQ_LOGPOI, ACQ_NEI, ACQ_LOGNEI = 0, 1, 2, 3, 4, 6, 7, 8, 9
 MAX_GPS, MAX_DIM, MAX_TOPK, MAX_PATHS = 8, 64, 64, 16
 XFORM_IDENTITY, XFORM_ROUND = 0, 1
 GET_L, GET_ALPHA, GET_YSTATS, GET_K, GET_LINV = 0, 1, 2, 3, 4
@@ -34,6 +34,7 @@ EXPORTS = [
     "b200bo_paths_argmin_topk_philox", "b200bo_paths_bound", "b200bo_cpaths_eval", "b200bo_cpaths_argmin_topk",
     "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
     "b200bo_acq_value_grad", "b200bo_paths_grad_rows", "b200bo_gp_fork", "b200bo_gp_condition",
+    "b200bo_gp_set_fantasies",
 ]
 
 
@@ -86,6 +87,7 @@ def lib():
     L.b200bo_gp_set_private_stream.argtypes = [C.c_void_p, C.c_int]
     L.b200bo_gp_set_transform.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
     L.b200bo_gp_set_max_values.argtypes = [C.c_void_p, dp, C.c_int]
+    L.b200bo_gp_set_fantasies.argtypes = [C.c_void_p, C.c_void_p, dp, dp, C.c_int, C.POINTER(C.c_uint8), dp, dp]
     L.b200bo_gp_fit.argtypes = [C.c_void_p, dp, dp, C.c_int64, C.c_int, C.POINTER(KernelSpec),
                                 C.c_double, C.c_int, i64p]
     L.b200bo_gp_set_data.argtypes = [C.c_void_p, dp, dp, C.c_int64, C.c_int, C.c_int]

@@ -592,6 +592,87 @@ class MaxValueEntropySearch(_SuggestStream, DeviceHooks, _ref.AcquisitionFunctio
         self.n_max_candidates = _check_int("n_max_candidates", params["n_max_candidates"], 1)
 
 
+class _NoisyEI(_SuggestStream, DeviceHooks, _ref.ExpectedImprovement):
+    """Noisy expected improvement (Letham, Karrer, Ottoni & Bakshy, "Constrained Bayesian Optimization with Noisy
+    Experiments", Bayesian Analysis 2019; DESIGN.md 4.13): EI averaged over S joint samples of the noise-free function
+    values at the registered points, each conditioned on as if observed exactly.  Under observation noise the largest
+    registered target is the luckiest draw, not the best point, and EI against it scores little near the real optimum;
+    NEI measures each fantasy against its own incumbent best_s.
+
+    Every ``suggest()`` refuses before any draw (TargetSpaceEmptyError, NoValidPointRegisteredError without a feasible
+    registered point, as EI), then draws from the RandomState it receives, in this order:
+      1. Z = standard_normal((n, S)), 2. E = standard_normal((n, S))  (``noiseless_fantasies``);
+      3. the reference's random stage and L-BFGS-B refinement (refine="analytic": the device gradient of NEI).
+    The incumbent of each fantasy is its largest value over ``target_space.mask`` (the rows ``_target_max`` uses).
+    Parameters, y_max, the xi decay and saved state are ExpectedImprovement's, plus ``n_samples`` (S, 1..16) and
+    ``jitter`` (tau = min(alpha, jitter) on the noiseless GP's diagonal).  Constraints enter as for EI / LogEI.
+    Not inside KrigingBeliever, ConstantLiar or GPHedge; one device."""
+
+    _nei_kind = None
+
+    def __init__(self, xi=0.0, n_samples=16, jitter=1e-6, exploration_decay=None, exploration_decay_delay=None,
+                 random_state=None):
+        super().__init__(xi, exploration_decay=exploration_decay, exploration_decay_delay=exploration_decay_delay,
+                         random_state=random_state)
+        self.n_samples = _check_int("n_samples", n_samples, 1, B.MAX_PATHS)
+        self.jitter = _check_jitter(jitter)
+        self.fantasies = None  # the NoiselessFantasies of the latest closure
+
+    def base_acq(self, *args, **kwargs):
+        raise NotImplementedError(
+            f"{type(self).__name__} has no base_acq(mean, std): it averages over fantasies of the noise-free values "
+            "drawn per suggest(), and it runs in the fused device kernel")
+
+    def _get_acq(self, gp, constraint=None):
+        gp = _as_b200_gp(gp)
+        if constraint is not None:  # before any draw: a refusal consumes no random numbers
+            models = [_as_b200_gp(m) for m in constraint.model]
+            if len(models) + 1 > B.MAX_GPS:
+                raise NotImplementedError(f"at most {B.MAX_GPS - 1} constraint GPs are supported")
+        space = self._suggest_space
+        if space is None:
+            raise RuntimeError(f"{type(self).__name__} draws its fantasies against the target space of suggest(): "
+                               "build its closure through suggest()")
+        self.fantasies = None  # the previous closure's fantasies are not needed past this point
+        fant = gp.noiseless_fantasies(self.n_samples, self.jitter, incumbent=np.asarray(space.mask, dtype=bool),
+                                      random_state=self._suggest_rng())
+        self.fantasies = fant
+        return FusedAcquisition(self._nei_kind, gp, constraint, owner=self, fantasies=fant)
+
+    def get_acquisition_params(self):
+        return {**super().get_acquisition_params(), "n_samples": self.n_samples, "jitter": self.jitter}
+
+    def set_acquisition_params(self, params):
+        super().set_acquisition_params(params)
+        self.n_samples = _check_int("n_samples", params["n_samples"], 1, B.MAX_PATHS)
+        self.jitter = _check_jitter(params["jitter"])
+
+
+def _check_jitter(v):
+    if isinstance(v, bool) or not isinstance(v, (int, float, np.floating, np.integer)) or not 0.0 < float(v) < np.inf:
+        raise ValueError(f"jitter must be a positive float, got {v!r}")
+    return float(v)
+
+
+class NoisyExpectedImprovement(_NoisyEI):
+    __doc__ = _NoisyEI.__doc__
+    _nei_kind = B.ACQ_NEI
+
+
+class LogNoisyExpectedImprovement(_NoisyEI):
+    """Log noisy expected improvement: log NEI(x) = log of the mean over the fantasies of EI, formed from LogEI's
+    tail-safe terms (Ament et al. 2023), finite where NEI underflows.  Otherwise NoisyExpectedImprovement; constraints
+    enter as sum_j log p_j."""
+
+    _nei_kind = B.ACQ_LOGNEI
+
+
+def _refuse_nei(acq, where):
+    if isinstance(acq, _NoisyEI):
+        raise TypeError(f"{where} does not support {type(acq).__name__}: its fantasies are drawn per suggest() against "
+                        "the registered data")
+
+
 _HOOKED = {
     _ref.UpperConfidenceBound: UpperConfidenceBound,
     _ref.ProbabilityOfImprovement: ProbabilityOfImprovement,
@@ -608,9 +689,12 @@ def accelerate(acq, candidate_source=None, refine=None):
     if refine not in (None, "stencil", "analytic"):
         raise ValueError("refine must be 'stencil' or 'analytic'")
     if isinstance(acq, _ref.ConstantLiar):
+        _refuse_nei(acq.base_acquisition, type(acq).__name__)
         acq.base_acquisition = accelerate(acq.base_acquisition, candidate_source, refine)
         return acq
     if isinstance(acq, _ref.GPHedge):
+        for a in acq.base_acquisitions:
+            _refuse_nei(a, type(acq).__name__)
         acq.base_acquisitions = [accelerate(a, candidate_source, refine) for a in acq.base_acquisitions]
         return acq
     if candidate_source is not None:
@@ -631,6 +715,7 @@ class ConstantLiar(_ref.ConstantLiar):
     """bayes_opt.acquisition.ConstantLiar whose base acquisition runs on the device."""
 
     def __init__(self, base_acquisition, *args, **kwargs):
+        _refuse_nei(base_acquisition, "ConstantLiar")
         super().__init__(accelerate(base_acquisition), *args, **kwargs)
 
 
@@ -638,6 +723,8 @@ class GPHedge(_ref.GPHedge):
     """bayes_opt.acquisition.GPHedge over device base acquisitions."""
 
     def __init__(self, base_acquisitions, *args, **kwargs):
+        for a in base_acquisitions:
+            _refuse_nei(a, "GPHedge")
         super().__init__([accelerate(a) for a in base_acquisitions], *args, **kwargs)
 
 
@@ -660,6 +747,7 @@ class KrigingBeliever(_ref.ConstantLiar):
     Constraints raise ConstraintNotSupportedError, as ConstantLiar does."""
 
     def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
+        _refuse_nei(base_acquisition, "KrigingBeliever")
         if _device_kind(base_acquisition) is None and not isinstance(base_acquisition, MaxValueEntropySearch):
             raise TypeError(f"KrigingBeliever needs an UpperConfidenceBound, ExpectedImprovement, "
                             f"ProbabilityOfImprovement, LogExpectedImprovement, LogProbabilityOfImprovement or "
@@ -763,6 +851,6 @@ class KrigingBeliever(_ref.ConstantLiar):
 # the concrete classes keep the reference's MRO).
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, LogExpectedImprovement,
              LogProbabilityOfImprovement, ConstantLiar, GPHedge, ThompsonSampling, ConstrainedThompsonSampling,
-             MaxValueEntropySearch, KrigingBeliever):
+             MaxValueEntropySearch, KrigingBeliever, NoisyExpectedImprovement, LogNoisyExpectedImprovement):
     AcquisitionFunction.register(_cls)
 del _cls

@@ -135,6 +135,10 @@ struct b200bo_gp {
     bool normalize = false;
     std::vector<int> xform;      // host copy (d) or empty
     std::vector<double> ystar;   // MES samples of the maximum (b200bo_gp_set_max_values), or empty
+    // NEI fantasies (b200bo_gp_set_fantasies): A = K0^-1 F ([np][S]) then best_s on the device, and the host copy of
+    // best_s (empty: no fantasies)
+    DevBuf fant_a;
+    std::vector<double> fant_best;
     DevBuf X, Xs, y, K, L, W, WT, T, alphav, v1, v2, ls, xf, info, part;
     DevBuf tscratch;  // b200bo_gp_condition: t = W^T l of the row update (np), so that alpha_ survives it
     // predict-side scratch (used when this handle is gps[0] of a call)
@@ -265,6 +269,11 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    // the NEI / LogNEI instantiations
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -355,6 +364,7 @@ extern "C" int b200bo_gp_set_transform(b200bo_gp* gp, const int32_t* xform, int 
         }
     }
     gp->fitted = false;
+    gp->fant_best.clear();
     return B200BO_OK;
 }
 
@@ -408,6 +418,7 @@ extern "C" int b200bo_gp_set_data(b200bo_gp* gp, const double* X, const double* 
     CU(cudaSetDevice(gp->device));
     StreamScope scope(gp);
     gp->fitted = false;
+    gp->fant_best.clear();
     gp->replica = false;
     gp->tc_valid = false;
     gp->pad_valid = false;
@@ -792,6 +803,85 @@ extern "C" int b200bo_gp_fit(b200bo_gp* gp, const double* X, const double* y, in
     return B200BO_OK;
 }
 
+// NEI fantasies (include/b200bo.h, DESIGN.md 4.13): per sample s one product with L0 and the solves with K and K0 on
+// the device; the O(n) combinations on the host, in double, in the order of the definition.
+extern "C" int b200bo_gp_set_fantasies(b200bo_gp* nl, const b200bo_gp* ny, const double* z, const double* e, int S,
+                                       const uint8_t* incumbent, double* f_out, double* best_out) {
+    if (!nl || !ny || !z || !e || !incumbent) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (S < 1 || S > B200BO_MAX_PATHS) return set_err(B200BO_ERR_ARG, "S=%d out of range [1,%d]", S, B200BO_MAX_PATHS);
+    if (!nl->fitted || !ny->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
+    if (nl->replica || ny->replica) return set_err(B200BO_ERR_STATE, "handle is a predict-only replica");
+    if (nl->device != ny->device) return set_err(B200BO_ERR_ARG, "the two handles live on different devices");
+    if (nl->n != ny->n || nl->d != ny->d || nl->np != ny->np)
+        return set_err(B200BO_ERR_ARG, "the two handles hold different training sets (n, d or capacity)");
+    if (nl->y_mean != ny->y_mean || nl->y_std != ny->y_std)
+        return set_err(B200BO_ERR_ARG, "the two handles have different y statistics");
+    if (nl->noise != 0.0) return set_err(B200BO_ERR_ARG, "the noiseless handle has a WhiteKernel term");
+    const double tau = nl->jitter, s2 = ny->jitter;
+    if (!(s2 >= tau))
+        return set_err(B200BO_ERR_ARG, "noise variance %.17g of the fitted GP is below tau = %.17g", s2, tau);
+    const int n = (int)nl->n, np = nl->np;
+    bool any = false;
+    for (int i = 0; i < n; ++i) any = any || incumbent[i] != 0;
+    if (!any) return set_err(B200BO_ERR_ARG, "the incumbent mask is empty");
+    for (long long i = 0; i < (long long)n * S; ++i)
+        if (!std::isfinite(z[i]) || !std::isfinite(e[i])) return set_err(B200BO_ERR_ARG, "non-finite draw at %lld", i);
+    CU(cudaSetDevice(nl->device));
+    StreamScope scope(nl);
+    NvtxRange nvtx_range("b200bo:set_fantasies");
+    nl->fant_best.clear();
+    int rc;
+    DevBuf in, out, v1, v2;
+    for (DevBuf* b : {&in, &out, &v1, &v2})
+        if ((rc = b->reserve(sizeof(double) * np))) return rc;
+    b200bo_gp* noisy = const_cast<b200bo_gp*>(ny);
+    const double sq = std::sqrt(s2 - tau), ds = s2 - tau;
+    const std::vector<double>& y = nl->y_norm;
+    std::vector<double> col(np, 0.0), fp(n), kr(n), F((size_t)n * S), A((size_t)np * S, 0.0), a(n);
+    const int wpb = 8;
+    const dim3 blk(32 * wpb), grd((np + wpb - 1) / wpb);
+    for (int s = 0; s < S; ++s) {
+        for (int i = 0; i < n; ++i) col[i] = z[(size_t)i * S + s];
+        if ((rc = h2d(in.p, col.data(), sizeof(double) * np))) return rc;
+        gemv_rows_kernel<<<grd, blk, 0, g_st>>>(nl->L.as<double>(), np, in.as<double>(), out.as<double>(), np, np, 1);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        if ((rc = d2h(fp.data(), out.p, sizeof(double) * n))) return rc;  // F_prior = L0 z
+        if (ds > 0.0) {
+            for (int i = 0; i < n; ++i) col[i] = (y[i] - fp[i]) - sq * e[(size_t)i * S + s];  // R
+            if ((rc = h2d(in.p, col.data(), sizeof(double) * np))) return rc;
+            if ((rc = solve_spd(noisy, in.as<double>(), out.as<double>(), v1.as<double>(), v2.as<double>()))) return rc;
+            if ((rc = d2h(kr.data(), out.p, sizeof(double) * n))) return rc;  // K^-1 R
+            for (int i = 0; i < n; ++i) col[i] = (y[i] - sq * e[(size_t)i * S + s]) - ds * kr[i];
+        } else {
+            for (int i = 0; i < n; ++i) col[i] = y[i];  // sigma_n^2 = tau: F = y_n exactly
+        }
+        for (int i = 0; i < n; ++i) F[(size_t)i * S + s] = col[i];
+        if ((rc = h2d(in.p, col.data(), sizeof(double) * np))) return rc;
+        if ((rc = solve_spd(nl, in.as<double>(), out.as<double>(), v1.as<double>(), v2.as<double>()))) return rc;
+        if ((rc = d2h(a.data(), out.p, sizeof(double) * n))) return rc;  // a_s = K0^-1 f_s
+        for (int i = 0; i < n; ++i) A[(size_t)i * S + s] = a[i];
+    }
+    std::vector<double> best(S, -std::numeric_limits<double>::infinity());
+    for (int s = 0; s < S; ++s)
+        for (int i = 0; i < n; ++i)
+            if (incumbent[i]) best[s] = std::fmax(best[s], nl->y_std * F[(size_t)i * S + s] + nl->y_mean);
+    A.insert(A.end(), best.begin(), best.end());  // the kernels read best_s behind A
+    if ((rc = nl->fant_a.reserve(sizeof(double) * A.size()))) return rc;
+    if ((rc = h2d(nl->fant_a.p, A.data(), sizeof(double) * A.size()))) return rc;
+    if ((rc = sync_fit_stream())) return rc;
+    for (size_t i = 0; i < F.size(); ++i)  // A's first n * S entries are the rows of F
+        if (!std::isfinite(F[i]) || !std::isfinite(A[i]))
+            return set_err(B200BO_ERR_NOT_PD, "the fantasies are not finite: K0 = c k(X, X) + tau I is too "
+                                              "ill-conditioned (raise jitter)");
+    if (f_out)
+        for (size_t i = 0; i < F.size(); ++i) f_out[i] = nl->y_std * F[i] + nl->y_mean;
+    if (best_out)
+        for (int s = 0; s < S; ++s) best_out[s] = best[s];
+    nl->fant_best = best;
+    return B200BO_OK;
+}
+
 // Row n of the O(N^2) factor update at the hyper-parameters of the last fit, shared by b200bo_gp_append and
 // b200bo_gp_condition: row n of X / Xs, row and column n of K, row n of L (pivot checked) and of L^-1 (W and WT).
 // tvec: n-entry device scratch.  believer (nullable, device): receives k(x, X) . alpha_ in normalised units, computed
@@ -840,6 +930,7 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     CU(cudaSetDevice(gp->device));
     const int n = (int)gp->n;
     if (info) *info = 0;
+    gp->fant_best.clear();
     int rc;
     int finfo = 0;
     // alpha_ is recomputed below; reuse it as scratch
@@ -878,6 +969,7 @@ extern "C" int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, d
         if (!std::isfinite(Xp[i])) return set_err(B200BO_ERR_ARG, "Input X contains NaN or infinity.");
     CU(cudaSetDevice(gp->device));
     NvtxRange nvtx_range("b200bo:condition");
+    gp->fant_best.clear();
     int rc;
     if ((rc = gp->tscratch.reserve(sizeof(double) * gp->np))) return rc;
     for (int64_t r = 0; r < p; ++r) {
@@ -1245,6 +1337,10 @@ static void predict16_config(int grid, cudaStream_t stream, bool pair, cudaLaunc
 template <int MMA, int PIPE>
 static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
     auto fn = dreg ? predict_acq16_kernel<true, MMA, PIPE> : predict_acq16_kernel<false, MMA, PIPE>;
+    if constexpr (PIPE != PIPE_CPASYNC) {  // NEI / LogNEI: bulk-copy pipes only (DESIGN.md 4.13)
+        if (P.acq_kind == B200BO_ACQ_NEI || P.acq_kind == B200BO_ACQ_LOGNEI)
+            fn = dreg ? predict_acq16_kernel<true, MMA, PIPE, true> : predict_acq16_kernel<false, MMA, PIPE, true>;
+    }
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
     predict16_config(grid, stream, PIPE == PIPE_BULK_MC, cfg, attr);
@@ -1432,7 +1528,7 @@ static int check_spec(const b200bo_acq* spec) {
     if (!spec) return set_err(B200BO_ERR_ARG, "spec is NULL");
     if (spec->n_gps < 1 || spec->n_gps > B200BO_MAX_GPS)
         return set_err(B200BO_ERR_ARG, "n_gps=%d out of range [1,%d]", spec->n_gps, B200BO_MAX_GPS);
-    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_LOGPOI || spec->kind == 5)
+    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_LOGNEI || spec->kind == 5)
         return set_err(B200BO_ERR_ARG, "unknown acquisition kind %d", spec->kind);
     if (spec->path != B200BO_PATH_AUTO && spec->path != B200BO_PATH_STABLE)
         return set_err(B200BO_ERR_ARG, "unknown path policy %d", spec->path);
@@ -1448,6 +1544,8 @@ static int check_spec(const b200bo_acq* spec) {
     }
     if (spec->kind == B200BO_ACQ_MES && spec->gps[0]->ystar.empty())
         return set_err(B200BO_ERR_STATE, "MES: gps[0] holds no samples of the maximum (b200bo_gp_set_max_values)");
+    if ((spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI) && spec->gps[0]->fant_best.empty())
+        return set_err(B200BO_ERR_STATE, "NEI: gps[0] holds no fantasies (b200bo_gp_set_fantasies)");
     return B200BO_OK;
 }
 
@@ -1517,6 +1615,9 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
     if (spec->kind == B200BO_ACQ_MES) {
         P.n_ystar = (int)g0->ystar.size();
         for (int k = 0; k < P.n_ystar; ++k) P.ystar[k] = g0->ystar[k];
+    } else if (spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI) {  // A and best_s on the device
+        P.n_ystar = (int)g0->fant_best.size();
+        P.fant_a = g0->fant_a.as<double>();
     }
     P.Xc = src.philox ? nullptr : src.d_Xc;
     P.index_base = index_base;
@@ -1537,6 +1638,7 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
 // finish for every GP.
 static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool grad, cudaStream_t stream) {
     b200bo_gp* g0 = spec->gps[0];
+    const bool nei = spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI;
     int rc;
     for (int g = 0; g < spec->n_gps; ++g) {
         b200bo_gp* gp = spec->gps[g];
@@ -1550,6 +1652,11 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
         Q.unit_tab = gp->s_unit.as<int2>();
         Q.rb_tab = gp->s_rb.as<int2>();
         S.nunits[g] = gp->s_nunits;
+        if (grad && g == 0 && nei) {  // S mean lists + the u list per block (small_grad_kernel<true>)
+            const size_t lists = g0->fant_best.size() + 1;
+            if ((rc = gp->s_gpart.reserve(sizeof(double) * (size_t)SMAXP * (gp->np / 128) * lists * gp->d * SMC)))
+                return rc;
+        }
         if (grad) {
             Q.vsum = gp->s_vsum.as<double>();
             Q.usum = gp->s_usum.as<double>();
@@ -1575,16 +1682,22 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
                 small_reduce_kernel<1><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
                 small_trsv_kernel<true><<<dim3(gp->s_nunits_u, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
                 small_reduce_kernel<2><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
-                small_grad_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+                if (nei && g == 0)
+                    small_grad_kernel<true><<<dim3(gp->np / 128, npass, (unsigned)g0->fant_best.size()), 256, 0,
+                                              stream>>>(S, g);
+                else
+                    small_grad_kernel<false><<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
             } else {
                 small_reduce_kernel<0><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
             }
             for (int i = 0; i < (grad ? 6 : 3); ++i) LAUNCHED();
         }
         if (grad)
-            small_finish_grad_kernel<<<npass, 256, 0, stream>>>(S);
+            (nei ? small_finish_grad_kernel<true> : small_finish_grad_kernel<false>)<<<npass, 256, 0, stream>>>(S);
+        else if (nei)
+            small_finish_kernel<true><<<npass, 256, 0, stream>>>(S);
         else
-            small_finish_kernel<<<npass, 256, 0, stream>>>(S);
+            small_finish_kernel<false><<<npass, 256, 0, stream>>>(S);
         LAUNCHED();
     }
     CU(cudaGetLastError());
@@ -1629,6 +1742,12 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
     if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
     if (k > 0 && !d_sel) return set_err(B200BO_ERR_ARG, "d_sel is NULL");
     b200bo_gp* g0 = spec->gps[0];
+    // NEI / LogNEI: no single mean to report; always fp64 (the 16-warp kernel or the small-batch kernels)
+    const bool nei = spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI;
+    if (nei && (d_mu || d_sd))
+        return set_err(B200BO_ERR_ARG, "NEI averages over fantasies and has no single posterior mean: mu / sd outputs "
+                                       "are not available");
+    const int precision = nei ? B200BO_PRECISION_FP64 : g0->precision;
     CU(cudaSetDevice(g0->device));
     NvtxRange nvtx_range("b200bo:predict_acq");
     PredictParams P;
@@ -1664,14 +1783,20 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             fused_sel = true;
         }
         // phase B path of the 16-warp fp64 kernel; the bulk-copy paths read K* in the padded stage layout
-        const bool fp64_16 = predict_impl(g0->precision) == PREDICT_IMPL_DMMA && predict_warps() == 16;
+        const bool fp64_16 = predict_impl(precision) == PREDICT_IMPL_DMMA && predict_warps() == 16;
+        if (nei && !fp64_16)
+            return set_err(B200BO_ERR_UNSUPPORTED, "NEI runs on the 16-warp fp64 kernel only (B200BO_PREDICT_IMPL / "
+                                                   "B200BO_PREDICT_WARPS select a kernel without it)");
         const int pipe = fp64_16 && predict_mma() != 884 ? predict_pipe() : PIPE_CPASYNC;
+        if (nei && (pipe == PIPE_CPASYNC || predict_mma() == 884))
+            return set_err(B200BO_ERR_UNSUPPORTED, "NEI runs on the bulk-copy phase-B pipes only (B200BO_PREDICT_PIPE="
+                                                   "cpasync / B200BO_PREDICT_MMA=884 select a pipe without it)");
         P.scratch_stride = (long long)np_max * (pipe == PIPE_CPASYNC ? PBN : PSTR_DMMA);
         if ((rc = g0->pscratch.reserve(sizeof(double) * (size_t)P.scratch_stride * g0->sm_count))) return rc;
         P.scratch = g0->pscratch.as<double>();
         CU(cudaEventRecord(g0->ev0, stream));
         const bool dreg = P.d <= kPredictMaxDimRegs;
-        if (predict_impl(g0->precision) == PREDICT_IMPL_TF32) {
+        if (predict_impl(precision) == PREDICT_IMPL_TF32) {
             for (int g = 0; g < spec->n_gps; ++g) {
                 if ((rc = ensure_tc(spec->gps[g], stream))) return rc;
                 P.gp[g].linv_tc = spec->gps[g]->tc_linv.as<uint8_t>();
@@ -1725,7 +1850,7 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
                 rc = launch_predict16<1684, PIPE_CPASYNC>(dreg, grid, stream, P);
             }
             if (rc) return rc;
-        } else if (predict_impl(g0->precision) == PREDICT_IMPL_DMMA) {
+        } else if (predict_impl(precision) == PREDICT_IMPL_DMMA) {
             if (dreg)
                 predict_acq_kernel<PREDICT_IMPL_DMMA, true><<<grid, PNT, kPredictSmemBytesDmma, stream>>>(P);
             else

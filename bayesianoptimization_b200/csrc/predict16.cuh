@@ -629,7 +629,8 @@ __device__ __forceinline__ void predict16_phase_b_bulk(const PredictParams& P, c
 // PIPE: phase B data path; PIPE_BULK_MC is launched in clusters of 2 CTAs, and the two CTAs of a cluster run the
 // same number of tiles: when the pair's second tile lies past the batch (odd tile count), the second CTA runs it
 // with every column masked (c0 >= m: zero coordinates, no output, no selection entry).
-template <bool DREG, int MMA, int PIPE>
+// NEI: the instantiation that serves B200BO_ACQ_NEI / LOGNEI (candidate_epilogue<true>).
+template <bool DREG, int MMA, int PIPE, bool NEI = false>
 __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictParams P) {
     static_assert(PIPE == PIPE_CPASYNC || MMA == 1684, "the bulk-copy phase B runs on m16n8k4");
     extern __shared__ __align__(16) double smem[];
@@ -683,7 +684,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
                 const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
                 const long long gi = (P.perm && c0 + c < P.m) ? (long long)P.perm[c0 + c] : c0 + c;
                 double val = 0.0;
-                candidate_epilogue(P, G, g, mu_n, colsq, gi, base_s[c], prod_s[c], &val);
+                candidate_epilogue<NEI>(P, G, g, mu_n, colsq, gi, base_s[c], prod_s[c], &val, Ks + c,
+                                        PIPE == PIPE_CPASYNC ? PBN : PSTR_DMMA);
                 if (P.sel_cta && g == P.n_gps - 1) {
                     runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, c0 + c < P.m);
                     if (P.perm && tid == 0 && sel_s.list.idx[P.sel_k - 1] != SEL_NOIDX)

@@ -66,6 +66,8 @@ struct PredictParams {
     const int* perm;
     const unsigned long long* perm_key;
     unsigned long long* prune_ctl;  // [0] next tile to claim, [1] least k-th key of a full CTA list, [2] evaluated
+    // NEI / LogNEI (DESIGN.md 4.13): A = K0^-1 F of gps[0], [np][n_ystar] row-major, then best_0 .. best_{n_ystar-1}
+    const double* fant_a;
 };
 
 // coordinate j of candidate gi (local index) as the reference's x_tries[gi, j]
@@ -131,6 +133,8 @@ __device__ __forceinline__ bool log_kind(int kind) {
     return kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI;
 }
 
+__device__ __forceinline__ bool nei_kind(int kind) { return kind == B200BO_ACQ_NEI || kind == B200BO_ACQ_LOGNEI; }
+
 // LogEI / LogPoI at a = mean - y_max - xi (include/b200bo.h), out of line like mes_term.  sigma = 0, or a sigma so
 // small that z = a / sigma is infinite: the log of the EI limit max(a, 0) (log a, -inf, NaN at a = 0); log_ndtr has
 // the PoI limits already (0 at z = +inf, -inf at -inf, NaN at NaN).
@@ -158,6 +162,57 @@ __device__ __noinline__ double log_cfactor(double lb, double ub, double mean, do
     return lpb + log1mexp(log_ndtr(a) - lpb);
 }
 
+// One fantasy's EI at a = mu_s - best_s - xi: EI's formula of candidate_epilogue, with its sigma = 0 limits.
+__device__ __noinline__ double nei_ei_term(double a, double sd) {
+    const double z = a / sd;
+    return a * ndtr(z) + sd * norm_pdf(z);
+}
+
+// NEI / LogNEI (DESIGN.md 4.13) of one candidate, out of line like mes_term and with scalar arguments only, so that
+// the kernels that inline candidate_epilogue keep their register allocation.  The S fantasy means k*^T a_s
+// (normalised units) come from the candidate's column of the K* tile the kernel already holds (kcol[i * kstr] =
+// const_value k(xs, Xs_i)) and A = K0^-1 F ([np][S] row-major), each summed over the training rows in index order;
+// best = best_0 .. best_{S-1} (data units).  NEI: the mean of the S EI terms in s order; LogNEI: the log of that mean
+// from the LogEI terms, shifted by their maximum.
+__device__ __noinline__ double nei_term(int kind, const double* __restrict__ kcol, int kstr, int n,
+                                        const double* __restrict__ A, const double* __restrict__ best, int S,
+                                        double y_std, double y_mean, double xi, double sd) {
+    double t[B200BO_MAX_PATHS];
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s) t[s] = 0.0;
+    for (int i = 0; i < n; ++i) {
+        const double k = kcol[(size_t)i * kstr];
+        const double* a = A + (size_t)i * S;
+#pragma unroll
+        for (int s = 0; s < B200BO_MAX_PATHS; ++s)
+            if (s < S) t[s] = fma(a[s], k, t[s]);
+    }
+    if (kind == B200BO_ACQ_NEI) {
+        double sum = 0.0;
+#pragma unroll
+        for (int s = 0; s < B200BO_MAX_PATHS; ++s)
+            if (s < S) sum += nei_ei_term(y_std * t[s] + y_mean - best[s] - xi, sd);
+        return sum / (double)S;
+    }
+    double mx = -CUDART_INF;
+    bool nan = false;
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s) {
+        if (s < S) {
+            t[s] = log_acq_term(B200BO_ACQ_LOGEI, y_std * t[s] + y_mean - best[s] - xi, sd);
+            nan = nan || isnan(t[s]);
+            mx = fmax(mx, t[s]);
+        }
+    }
+    if (nan) return CUDART_NAN;
+    if (mx == -CUDART_INF) return -CUDART_INF;
+    double e = 0.0;
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s)
+        if (s < S) e += exp(t[s] - mx);
+    return mx + log(e) - log((double)S);
+}
+
 // ---- per-candidate epilogue shared by the tiled and the small-batch kernels ---------------------
 // mu_n: K* alpha_ (normalised units); colsq: sum_i V_i^2.  g = 0: target GP -> base acquisition;
 // g >= 1: constraint GP -> probability factor.  The last GP writes -base * prod.
@@ -165,9 +220,15 @@ __device__ __noinline__ double log_cfactor(double lb, double ub, double mean, do
 // the predictive distribution is a point mass, an observation there teaches nothing).
 // LogEI / LogPoI: base_neg = -log_acq_term, then base_neg -= log p_g per constraint GP, which is -(alpha + sum log p)
 // summed in g order bit for bit (negation is exact); prod stays 1 and is not used.
+// NEI (template flag, set in the kernel instantiations that serve NEI / LogNEI only, so that every other
+// instantiation compiles as without these kinds): base = nei_term over the candidate's K* column kcol (stride kstr);
+// constraints as for EI / LogEI.
+template <bool NEI = false>
 __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const GpDev& G, int g,
                                                    double mu_n, double colsq, long long gi,
-                                                   double& base_neg, double& prod, double* final_val = nullptr) {
+                                                   double& base_neg, double& prod, double* final_val = nullptr,
+                                                   const double* kcol = nullptr, int kstr = 0) {
+    const bool logk = log_kind(P.acq_kind) || (NEI && P.acq_kind == B200BO_ACQ_LOGNEI);
     const double mean = G.y_std * mu_n + G.y_mean;
     double var = G.prior - colsq;
     if (var < 0.0) {
@@ -192,6 +253,9 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
                 for (int k = 0; k < P.n_ystar; ++k) s += mes_term((P.ystar[k] - mean) / sd);
                 base = s / (double)P.n_ystar;
             }
+        } else if (NEI && nei_kind(P.acq_kind)) {
+            base = nei_term(P.acq_kind, kcol, kstr, G.n, P.fant_a, P.fant_a + (size_t)G.np * P.n_ystar, P.n_ystar,
+                            G.y_std, G.y_mean, P.xi, sd);
         } else if (log_kind(P.acq_kind)) {
             base = log_acq_term(P.acq_kind, mean - P.y_max - P.xi, sd);
         }
@@ -201,7 +265,7 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
             if (P.mu_out) P.mu_out[gi] = mean;
             if (P.sd_out) P.sd_out[gi] = sd;
         }
-    } else if (log_kind(P.acq_kind)) {
+    } else if (logk) {
         base_neg = base_neg - log_cfactor(G.lb, G.ub, mean, sd);
     } else {
         const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
@@ -210,7 +274,7 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
         prod = (g == 1) ? (p_hi - p_lo) : prod * (p_hi - p_lo);
     }
     if (g == P.n_gps - 1) {
-        const double val = (P.n_gps > 1 && !log_kind(P.acq_kind)) ? base_neg * prod : base_neg;
+        const double val = (P.n_gps > 1 && !logk) ? base_neg * prod : base_neg;
         if (final_val) *final_val = val;
         if (P.acq_out && gi < P.m) P.acq_out[gi] = val;
     }
@@ -1025,7 +1089,8 @@ __device__ __forceinline__ void small_finish_sums(const SmallParams& S, int pass
     }
 }
 
-// Per pass (blockIdx.x): the sums above, then the per-candidate epilogue of every GP.
+// Per pass (blockIdx.x): the sums above, then the per-candidate epilogue of every GP (NEI: the NEI / LogNEI kinds).
+template <bool NEI>
 __global__ void __launch_bounds__(256)
 small_finish_kernel(const SmallParams S) {
     __shared__ double red[8][SMC];
@@ -1037,8 +1102,10 @@ small_finish_kernel(const SmallParams S) {
     small_finish_sums(S, pass, red, colsq_s, mu_s);
     if (sl == 0 && c < mc) {
         double base_neg = 0.0, prod = 1.0;
+        const double* kcol = S.sg[0].ksm + (size_t)pass * S.P.gp[0].np * SMC + c;  // gps[0]'s K* column (NEI)
         for (int g = 0; g < S.P.n_gps; ++g)
-            candidate_epilogue(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod);
+            candidate_epilogue<NEI>(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, nullptr,
+                                    kcol, SMC);
     }
 }
 
@@ -1050,7 +1117,10 @@ small_finish_kernel(const SmallParams S) {
 //   gpart[0][j][c] = sum_n alpha_n c h(r_n) (xs_j - Xs_nj),   gpart[1][j][c] = the same with u_n,
 // by direct differences, rows in index order.  Sub-chunks of 32 rows: first thread = (candidate, 4 rows) forms the two
 // coefficients of each row, then thread = (candidate, dimensions j = jg, jg + 8, ..) adds the 32 rows in order.
+// NEI (gps[0] of an NEI / LogNEI call): blockIdx.z = fantasy s, the first list takes a_s = column s of A instead of
+// alpha_, and gpart holds S + 1 lists per block: [b][s][j][c] for s < S, then the u list (written by s = 0).
 constexpr int SGR = 32;  // rows per sub-chunk
+template <bool NEI>
 __global__ void __launch_bounds__(256)
 small_grad_kernel(const SmallParams S, int g) {
     const GpDev& G = S.P.gp[g];
@@ -1090,7 +1160,10 @@ small_grad_kernel(const SmallParams S, int g) {
                     r2 = fma(df, df, r2);
                 }
                 const double ch = G.constv * cov_dh_from_r2(r2, G.family, G.nu);
-                ca = G.alphav[n] * ch;
+                if constexpr (NEI)
+                    ca = S.P.fant_a[(size_t)n * S.P.n_ystar + blockIdx.z] * ch;
+                else
+                    ca = G.alphav[n] * ch;
                 cu = usum[(size_t)n * SMC + c] * ch;
             }
             coef[0][rl][c] = ca;
@@ -1112,13 +1185,26 @@ small_grad_kernel(const SmallParams S, int g) {
         }
         __syncthreads();
     }
-    double* out = Q.gpart + ((size_t)pass * (G.np / 128) + blockIdx.x) * 2 * d * SMC;
+    if constexpr (NEI) {
+        const int nl = S.P.n_ystar + 1;  // lists per block
+        double* out = Q.gpart + ((size_t)pass * (G.np / 128) + blockIdx.x) * nl * d * SMC;
 #pragma unroll
-    for (int t = 0; t < JT; ++t) {
-        const int j = rg + 8 * t;
-        if (j < d) {
-            out[(size_t)j * SMC + c] = sa[t];
-            out[(size_t)(d + j) * SMC + c] = su[t];
+        for (int t = 0; t < JT; ++t) {
+            const int j = rg + 8 * t;
+            if (j < d) {
+                out[((size_t)blockIdx.z * d + j) * SMC + c] = sa[t];
+                if (blockIdx.z == 0) out[((size_t)(nl - 1) * d + j) * SMC + c] = su[t];
+            }
+        }
+    } else {
+        double* out = Q.gpart + ((size_t)pass * (G.np / 128) + blockIdx.x) * 2 * d * SMC;
+#pragma unroll
+        for (int t = 0; t < JT; ++t) {
+            const int j = rg + 8 * t;
+            if (j < d) {
+                out[(size_t)j * SMC + c] = sa[t];
+                out[(size_t)(d + j) * SMC + c] = su[t];
+            }
         }
     }
 }
@@ -1157,6 +1243,54 @@ __device__ __noinline__ double log_acq_term_grad(int kind, double a, double sd, 
     return log_h(z) + log(sd);
 }
 
+// NEI / LogNEI value of one candidate (as nei_term) and its coefficients: d value = sum_s cms[s * SMC] d mu_s + cs d sd.
+//   NEI:    cms_s = Phi(z_s) / S,  cs = sum_s phi(z_s) / S                   (EI's cm / cs per fantasy, averaged)
+//   LogNEI: cms_s = p_s cm_s,       cs = sum_s p_s cs_s,  p_s = exp(l_s - M) / sum exp(l - M)   (LogEI's, softmax-weighted)
+// cms: S coefficients with stride SMC (shared memory of small_finish_grad_kernel).  Out of line like nei_term.
+__device__ __noinline__ double nei_term_grad(int kind, const double* __restrict__ kcol, int kstr, int n,
+                                             const double* __restrict__ A, const double* __restrict__ best, int S,
+                                             double y_std, double y_mean, double xi, double sd, double* cms,
+                                             double& cs) {
+    double t[B200BO_MAX_PATHS];
+    for (int s = 0; s < S; ++s) t[s] = 0.0;
+    for (int i = 0; i < n; ++i) {
+        const double k = kcol[(size_t)i * kstr];
+        for (int s = 0; s < S; ++s) t[s] = fma(A[(size_t)i * S + s], k, t[s]);
+    }
+    cs = 0.0;
+    if (kind == B200BO_ACQ_NEI) {
+        double sum = 0.0;
+        for (int s = 0; s < S; ++s) {
+            const double a = y_std * t[s] + y_mean - best[s] - xi;
+            const double z = a / sd;
+            sum += nei_ei_term(a, sd);
+            cms[s * SMC] = ndtr(z) / (double)S;
+            cs += norm_pdf(z);
+        }
+        cs = cs / (double)S;
+        return sum / (double)S;
+    }
+    double cm_s[B200BO_MAX_PATHS], cs_s[B200BO_MAX_PATHS];
+    double mx = -CUDART_INF;
+    bool nan = false;
+    for (int s = 0; s < S; ++s) {
+        t[s] = log_acq_term_grad(B200BO_ACQ_LOGEI, y_std * t[s] + y_mean - best[s] - xi, sd, cm_s[s], cs_s[s]);
+        nan = nan || isnan(t[s]);
+        mx = fmax(mx, t[s]);
+    }
+    for (int s = 0; s < S; ++s) cms[s * SMC] = 0.0;
+    if (nan) return CUDART_NAN;
+    if (mx == -CUDART_INF) return -CUDART_INF;
+    double e = 0.0;
+    for (int s = 0; s < S; ++s) e += exp(t[s] - mx);
+    for (int s = 0; s < S; ++s) {
+        const double p = exp(t[s] - mx) / e;
+        cms[s * SMC] = p * cm_s[s];
+        cs += p * cs_s[s];
+    }
+    return mx + log(e) - log((double)S);
+}
+
 // d log p = cm d mean + cs d sd for one constraint factor (log_cfactor), with F_l, F_u the partials of log p in l and u
 // (d u = -(d mean + u d sd) / sd, the same for l), each ratio phi / p in the same tail-safe form as the value:
 //   one-sided: F_u = lambda(u), F_l = -lambda(-l);   straddling: F_u = phi(u)/p, F_l = -phi(l)/p;
@@ -1193,8 +1327,11 @@ __device__ __noinline__ void log_cfactor_grad(double lb, double ub, double mean,
 //   d term = cm d mean + cs d sd,   term = the base acquisition (g = 0) or the probability factor p (g >= 1).
 // Returns the term itself in `term`.  sd == 0 (a clamped or vanished variance): the caller sets d sd := 0, and the
 // coefficients that divide by sd (PoI, MES) are 0 - the value there is a step or constant in x.
+// NEI: as candidate_epilogue's flag - LogNEI's constraint GPs enter as log p_j, like LogEI's.
+template <bool NEI = false>
 __device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, const GpDev& G, int g, double mean,
                                                         double sd, double& term, double& cm, double& cs) {
+    const bool logk = log_kind(P.acq_kind) || (NEI && P.acq_kind == B200BO_ACQ_LOGNEI);
     cm = cs = 0.0;
     if (g == 0) {
         term = 0.0;
@@ -1233,7 +1370,7 @@ __device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, 
         } else if (log_kind(P.acq_kind)) {
             term = log_acq_term_grad(P.acq_kind, mean - P.y_max - P.xi, sd, cm, cs);
         }
-    } else if (log_kind(P.acq_kind)) {
+    } else if (logk) {
         term = log_cfactor(G.lb, G.ub, mean, sd);
         log_cfactor_grad(G.lb, G.ub, mean, sd, cm, cs);
     } else {
@@ -1262,6 +1399,9 @@ __device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, 
 //   w_0 = -prod_i p_i,   w_g = -base prod_{i != g} p_i           (product rule over the GPs, g order)
 //   LogEI / LogPoI: w_g = -1 (the value is -(alpha + sum_g log p_g), a plain sum)
 // A rounded dimension has gradient 0; a NaN value gives a NaN row.
+// NEI: gps[0] is the noiseless handle of an NEI / LogNEI call: its mean coefficient is one per fantasy (nei_term_grad,
+// held in wn_s) against the S lists of gpart, its sd coefficient multiplies the u list as usual.
+template <bool NEI>
 __global__ void __launch_bounds__(256)
 small_finish_grad_kernel(const SmallParams S) {
     __shared__ double red[8][SMC];
@@ -1269,14 +1409,17 @@ small_finish_grad_kernel(const SmallParams S) {
     __shared__ double mu_s[B200BO_MAX_GPS][SMC];
     __shared__ double wa_s[B200BO_MAX_GPS][SMC], wu_s[B200BO_MAX_GPS][SMC];
     __shared__ double val_s[SMC];
+    __shared__ double wn_s[NEI ? B200BO_MAX_PATHS : 1][SMC];
     const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
     const int pass = blockIdx.x, mc = small_pass_mc(S, pass), d = S.P.d, ng = S.P.n_gps;
     const long long pc0 = small_pass_c0(S, pass);
     small_finish_sums(S, pass, red, colsq_s, mu_s);
     if (sl == 0 && c < mc) {
         double base_neg = 0.0, prod = 1.0, val = 0.0;
+        const double* kcol = S.sg[0].ksm + (size_t)pass * S.P.gp[0].np * SMC + c;
         for (int g = 0; g < ng; ++g)
-            candidate_epilogue(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, &val);
+            candidate_epilogue<NEI>(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, &val, kcol,
+                                    SMC);
         val_s[c] = val;
         // term_g, then w_g from the terms of the other GPs; wa_s / wu_s hold cm / cs until the second loop
         double term[B200BO_MAX_GPS];
@@ -1289,12 +1432,21 @@ small_finish_grad_kernel(const SmallParams S) {
                 const double var = fmax(G.prior - colsq_s[g][c], 0.0);
                 const double sd = sqrt(var * (G.y_std * G.y_std));
                 double cm, cs;
-                candidate_epilogue_grad(S.P, G, g, mean, sd, term[g], cm, cs);
+                if (NEI && g == 0) {
+                    const GpDev& G0 = S.P.gp[0];
+                    term[0] = nei_term_grad(S.P.acq_kind, kcol, SMC, G0.n, S.P.fant_a,
+                                            S.P.fant_a + (size_t)G0.np * S.P.n_ystar, S.P.n_ystar, G0.y_std,
+                                            G0.y_mean, S.P.xi, sd, &wn_s[0][c], cs);
+                    cm = 1.0;  // the per-fantasy coefficients are in wn_s
+                } else {
+                    candidate_epilogue_grad<NEI>(S.P, G, g, mean, sd, term[g], cm, cs);
+                }
                 wa_s[g][c] = -cm * G.y_std;
                 wu_s[g][c] = var > 0.0 ? cs * G.y_std / sqrt(var) : 0.0;
             }
         }
-        const bool logk = log_kind(S.P.acq_kind);  // the value is -sum_g term_g: w_g = -1, no product rule
+        // the value is -sum_g term_g: w_g = -1, no product rule
+        const bool logk = log_kind(S.P.acq_kind) || (NEI && S.P.acq_kind == B200BO_ACQ_LOGNEI);
 #pragma unroll
         for (int g = 0; g < B200BO_MAX_GPS; ++g) {
             if (g < ng) {
@@ -1304,6 +1456,8 @@ small_finish_grad_kernel(const SmallParams S) {
                     if (i < ng && i != g && !logk) w *= term[i];
                 wa_s[g][c] = wa_s[g][c] == 0.0 ? 0.0 : w * wa_s[g][c];
                 wu_s[g][c] = wu_s[g][c] == 0.0 ? 0.0 : w * wu_s[g][c];
+                if (NEI && g == 0)
+                    for (int s = 0; s < S.P.n_ystar; ++s) wn_s[s][c] = wn_s[s][c] == 0.0 ? 0.0 : w * wn_s[s][c];
             }
         }
     }
@@ -1316,6 +1470,21 @@ small_finish_grad_kernel(const SmallParams S) {
             const GpDev& G = S.P.gp[g];
             if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) continue;
             const int nb = G.np / 128;
+            if (NEI && g == 0) {  // sum_s wn_s (-y_std) sum_b list s, then the u list
+                const int nl = S.P.n_ystar + 1;
+                const double* gp = S.sg[0].gpart + (size_t)pass * nb * nl * d * SMC;
+                double an = 0.0, u = 0.0;
+                for (int s = 0; s < nl - 1; ++s) {
+                    double a = 0.0;
+                    for (int b = 0; b < nb; ++b) a += gp[(((size_t)b * nl + s) * d + j) * SMC + cc];
+                    const double wn = wn_s[s][cc];
+                    an += wn == 0.0 ? 0.0 : -G.y_std * wn * a;
+                }
+                for (int b = 0; b < nb; ++b) u += gp[(((size_t)b * nl + nl - 1) * d + j) * SMC + cc];
+                const double wu = wu_s[0][cc];
+                gr += (an + (wu == 0.0 ? 0.0 : wu * u)) / G.ls[j];
+                continue;
+            }
             const double* gp = S.sg[g].gpart + (size_t)pass * nb * 2 * d * SMC;
             double a = 0.0, u = 0.0;
             for (int b = 0; b < nb; ++b) {

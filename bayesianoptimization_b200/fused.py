@@ -43,7 +43,7 @@ _NEEDS_Y_MAX = (B.ACQ_EI, B.ACQ_POI, B.ACQ_LOGEI, B.ACQ_LOGPOI)
 class FusedAcquisition:
     """Callable closure over fitted device GPs.
 
-    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES / ACQ_LOGEI / ACQ_LOGPOI
+    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES / ACQ_LOGEI / ACQ_LOGPOI / ACQ_NEI / ACQ_LOGNEI
     gp        fitted B200GaussianProcessRegressor (target)
     constraint  object with .model (list of device GPs), .lb, .ub  (bayes_opt ConstraintModel) or None
     params    either fixed ``kappa``/``xi``/``y_max`` values or ``owner``: an acquisition object whose
@@ -52,12 +52,24 @@ class FusedAcquisition:
     max_values  ACQ_MES only: the K (1..16) samples y* of the maximum, data units (include/b200bo.h).  They are
               set on every device handle of the target GP each time the specs are built, so several MES closures
               over one GP, called alternately, each see their own samples.
+    fantasies   ACQ_NEI / ACQ_LOGNEI only: ``gp.noiseless_fantasies(...)``.  The spec's gps[0] is its noiseless handle;
+              candidate transforms and the device come from ``gp``.  One device; always fp64 (DESIGN.md 4.13).
     """
 
-    def __init__(self, kind, gp, constraint=None, kappa=0.0, xi=0.0, y_max=None, owner=None, max_values=None):
+    def __init__(self, kind, gp, constraint=None, kappa=0.0, xi=0.0, y_max=None, owner=None, max_values=None,
+                 fantasies=None):
         gp = _as_b200_gp(gp)
         self.kind = int(kind)
         self._ystar = None
+        self._fant = None
+        if self.kind in (B.ACQ_NEI, B.ACQ_LOGNEI):
+            if fantasies is None:
+                raise ValueError("NEI needs fantasies (B200GaussianProcessRegressor.noiseless_fantasies)")
+            if len(gp.device_list()) > 1:
+                raise NotImplementedError("noisy expected improvement runs on one device: the GP is multi-device")
+            self._fant = fantasies
+        elif fantasies is not None:
+            raise ValueError("fantasies belong to ACQ_NEI / ACQ_LOGNEI only")
         if self.kind == B.ACQ_MES:
             ys = B.c_f64(np.asarray(max_values if max_values is not None else [], dtype=np.float64).reshape(-1))
             if not 1 <= ys.size <= B.MAX_PATHS or not np.all(np.isfinite(ys)):
@@ -99,6 +111,8 @@ class FusedAcquisition:
     def _build_specs(self):
         # an LML evaluation in between re-uses the factor buffers: refit lazily, then (re)bind handles
         handles = [g._device_handles() for g in self._gps]  # [gp][device]
+        if self._fant is not None:
+            handles[0] = [self._fant.handle]  # the noiseless handle holding the fantasies
         sig = tuple(h.ptr.value for hs in handles for h in hs)
         kappa, xi, y_max = self._params()
         if self.kind in _NEEDS_Y_MAX and y_max is None:

@@ -282,6 +282,7 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         state.pop("_b200_handle", None)
         state.pop("_b200_restart_handles", None)
         state.pop("_b200_replicas", None)
+        state.pop("_b200_noiseless", None)
         state["_b200_device_fitted"] = False
         return state
 
@@ -748,7 +749,8 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         rc = L.b200bo_gp_condition(self._handle().ptr, B.as_dp(Xc), p, B.as_dp(mu)) if n_reg is not None else B.ERR_STATE
         if rc == B.ERR_STATE:
             out = type(self).__new__(type(self))
-            skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha")
+            skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha",
+                    "_b200_noiseless")
             out.__dict__.update({k: v for k, v in self.__dict__.items() if k not in skip})
             out.__dict__["_b200_handle"] = self._fork_handle(p + int(extra_rows))
             out.__dict__["_b200_conditioned"] = n if n_reg is None else n_reg
@@ -781,3 +783,87 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         from .paths import PosteriorPaths
 
         return PosteriorPaths(self, n_paths, n_features, random_state)
+
+    def noiseless_fantasies(self, n_samples, jitter=1e-6, incumbent=None, random_state=None):
+        """S = ``n_samples`` (1..16) joint samples of the noise-free function values at the training inputs, for noisy
+        expected improvement (DESIGN.md 4.13, ``b200bo_gp_set_fantasies``).
+
+        The noiseless GP has this GP's inputs, hyper-parameters and y statistics, no WhiteKernel term and
+        alpha = tau = min(alpha, jitter).  When the fitted noise variance sigma_n^2 = alpha + noise_level equals tau
+        (no WhiteKernel, alpha <= jitter) it is this GP itself and nothing is factorised again; otherwise it is a second
+        regressor on a device handle of its own, always in fp64.  From ``random_state`` (``check_random_state``) it
+        draws Z = standard_normal((n, S)), then E = standard_normal((n, S)).  ``incumbent`` is the (n,) mask of the
+        rows whose fantasy values may be the incumbent best_s (all rows when None).  Returns a ``NoiselessFantasies``.
+        One device, no pending-point conditioning; a non-PD K0 raises np.linalg.LinAlgError naming ``jitter``."""
+        S = int(n_samples)
+        if isinstance(n_samples, bool) or S != n_samples or not 1 <= S <= B.MAX_PATHS:
+            raise ValueError(f"n_samples must be an integer in [1, {B.MAX_PATHS}], got {n_samples!r}")
+        jitter = float(jitter)
+        if not jitter > 0.0 or not np.isfinite(jitter):
+            raise ValueError(f"jitter must be a positive float, got {jitter!r}")
+        if not hasattr(self, "X_train_"):
+            raise B.B200Error("GP is not fitted")
+        if len(self.device_list()) > 1:
+            raise NotImplementedError("noisy expected improvement runs on one device: the GP is multi-device")
+        if self.__dict__.get("_b200_conditioned") is not None:
+            raise NotImplementedError("noisy expected improvement on a GP conditioned on pending points")
+        n = self.X_train_.shape[0]
+        mask = np.ones(n, dtype=np.uint8) if incumbent is None else np.asarray(incumbent, dtype=bool).astype(np.uint8)
+        if mask.shape != (n,):
+            raise ValueError(f"incumbent must be a mask of the {n} training rows")
+        if not mask.any():
+            raise ValueError("the incumbent mask selects no training row")
+        self._ensure_device_fit()
+        ek = parse_kernel(self.kernel_)
+        alpha = float(self.alpha)
+        tau = min(alpha, jitter)
+        rs = check_random_state(random_state)
+        Z = B.c_f64(rs.standard_normal((n, S)))
+        E = B.c_f64(rs.standard_normal((n, S)))
+        if ek.noise == 0.0 and tau == alpha:
+            nl = self
+        else:
+            # one noiseless regressor per GP, refitted in place: b200bo_gp_fit on the same handle reuses its device
+            # buffers, so at most two N^2 handles (this GP's and the noiseless one) are ever live for NEI
+            nl = self.__dict__.get("_b200_noiseless")
+            handle = nl._handle() if nl is not None and nl.device == self.device else _Handle(self.device)
+            nl = type(self).__new__(type(self))
+            skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha",
+                    "_b200_noiseless")
+            nl.__dict__.update({k: v for k, v in self.__dict__.items() if k not in skip})
+            nl.__dict__["_b200_handle"] = handle
+            self.__dict__["_b200_noiseless"] = nl
+            nl.alpha = tau
+            nl.precision = "fp64"
+            # kernel_ stays this GP's (its input transform is found there); the fit drops the WhiteKernel term
+            ek0 = parse_kernel(self.kernel_)
+            ek0.noise = 0.0
+            try:
+                nl._device_fit(ek0)
+            except np.linalg.LinAlgError as e:
+                raise np.linalg.LinAlgError(f"{e} (noiseless GP with tau = {tau!r}: raise jitter)") from None
+        F = np.empty((n, S))
+        best = np.empty(S)
+        B.check(B.lib().b200bo_gp_set_fantasies(nl._handle().ptr, self._handle().ptr, B.as_dp(Z), B.as_dp(E), S,
+                                                mask.ctypes.data_as(C.POINTER(C.c_uint8)), B.as_dp(F), B.as_dp(best)))
+        return NoiselessFantasies(nl, F, best, tau)
+
+
+class NoiselessFantasies:
+    """S joint samples of the noise-free function values at the training inputs (``noiseless_fantasies``).
+
+    gp    the noiseless regressor holding A = K0^-1 F on its device handle (the fitted GP itself when tau = sigma_n^2)
+    F     (n, S) fantasy values, data units
+    best  (S,) best_s, the largest fantasy value over the incumbent rows
+    tau   the noiseless GP's diagonal term"""
+
+    def __init__(self, gp, F, best, tau):
+        self.gp, self.F, self.best, self.tau = gp, F, best, tau
+
+    @property
+    def n_samples(self):
+        return self.best.size
+
+    @property
+    def handle(self):
+        return self.gp._handle()

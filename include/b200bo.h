@@ -76,6 +76,23 @@ extern "C" {
 #define B200BO_ACQ_LOGEI 6
 #define B200BO_ACQ_LOGPOI 7
 /* Code 5 is not assigned: it is rejected as an unknown kind (B200BO_ERR_ARG), as before these kinds existed. */
+/* Noisy expected improvement and its log (Letham, Karrer, Ottoni & Bakshy, "Constrained Bayesian Optimization with
+ * Noisy Experiments", Bayesian Analysis 2019; Ament et al. 2023 for the log form).  No counterpart in the reference.
+ * gps[0] is the NOISELESS handle holding S fantasies (b200bo_gp_set_fantasies): A = K0^-1 F and best_0 .. best_{S-1}.
+ * With k* = const_value k(xs, Xs), mu_s = y_std k*^T a_s + y_mean, sigma0 the noiseless GP's posterior sd (data
+ * units, the negative-variance clamp counted as usual) and a_s = mu_s - best_s - xi:
+ *   NEI:    alpha = (1/S) sum_{s=0..S-1}, in s order, EI(a_s, sigma0)                 (EI's formula and sigma = 0 rules)
+ *   LOGNEI: alpha = M + log sum_s exp(l_s - M) - log S,  l_s = LogEI(a_s, sigma0),  M = max_s l_s
+ *           (-inf when every l_s is -inf; NaN when any l_s is NaN)
+ *   acq_neg = -alpha * prod_j p_j  (NEI)   or   -(alpha + sum_j log p_j)  (LOGNEI), the constraint GPs as for EI / LogEI.
+ * Served by the 16-warp fp64 kernel on its bulk-copy phase-B pipes (the default and the multicast one; host / device /
+ * Philox candidates), the small-batch kernels and b200bo_acq_value_grad, in fp64 whatever the handle's precision.  The
+ * 8-warp, DFMA and fp32 kernels and the cp.async / m8n8k4 phase B selected by the A/B switches return
+ * B200BO_ERR_UNSUPPORTED.  Never pruned.  mu / sd outputs (d_mu, d_sd) are refused with B200BO_ERR_ARG (there is no
+ * single mean).  Gradient: d NEI = (1/S) sum_s [Phi(z_s) d mu_s + phi(z_s) d sigma0]; d LogNEI = sum_s p_s d l_s with
+ * p_s = exp(l_s - M) / sum exp(l - M) (LogEI's per-fantasy derivative, softmax-weighted). */
+#define B200BO_ACQ_NEI 8
+#define B200BO_ACQ_LOGNEI 9
 
 #define B200BO_MAX_GPS 8   /* 1 target GP + up to 7 constraint GPs per call */
 #define B200BO_MAX_DIM 64  /* max input dimension d */
@@ -161,6 +178,25 @@ int b200bo_gp_set_transform(b200bo_gp* gp, const int32_t* xform, int d);
  * them.  Non-finite values or K out of range: B200BO_ERR_ARG.  An MES call whose gps[0] holds none returns
  * B200BO_ERR_STATE.  Fits keep them; a replica (b200bo_gp_replicate) is a handle of its own and needs its own call. */
 int b200bo_gp_set_max_values(b200bo_gp* gp, const double* ystar, int K);
+
+/* Fantasies for B200BO_ACQ_NEI / B200BO_ACQ_LOGNEI (DESIGN.md 4.13).  `noisy` is the fitted GP, K = const_value
+ * k(Xs, Xs) + sigma_n^2 I with sigma_n^2 = alpha + noise_level; `noiseless` is b200bo_gp_fit on the same data with the
+ * WhiteKernel term dropped and alpha = tau, K0 = const_value k(Xs, Xs) + tau I.  noisy may equal noiseless
+ * (sigma_n^2 = tau).  z, e: (n, S) host draws, row-major; incumbent: (n,) host mask of the registered rows that may be
+ * the incumbent.  In the normalised units of the fit (y_n the normalised targets, L0 = chol(K0)):
+ *   F_prior = L0 Z,   R = y_n 1^T - F_prior - sqrt(sigma_n^2 - tau) E,
+ *   F = y_n 1^T - sqrt(sigma_n^2 - tau) E - (sigma_n^2 - tau) K^-1 R,   A = K0^-1 F,
+ *   best_s = max over incumbent rows i of (y_std F_is + y_mean).
+ * Column s of F is a joint sample of the latent values at X (Matheron's rule, exact for the kernel const_value k + tau
+ * delta observed with noise sigma_n^2 - tau).  The N^2 work (one product with L0, one solve with K and one with K0 per
+ * sample: O(N^2 S)) runs on the device with the solve and matvec kernels of the fit.  A (np x S, zero padded) and
+ * best_s behind it are stored on `noiseless` in device memory (the kernels evaluate NEI out of line from pointers).  f_out (nullable, (n, S) host) receives F in data
+ * units (y_std F + y_mean), best_out (nullable, (S,) host) best_s.  1 <= S <= B200BO_MAX_PATHS.  B200BO_ERR_ARG: handles
+ * on different devices, a different n, d or y statistics, noiseless with a WhiteKernel term, sigma_n^2 < tau, an empty
+ * incumbent mask, non-finite draws; B200BO_ERR_STATE: a handle not fitted or a replica.  A later fit, append, condition
+ * or set_transform on `noiseless` drops the fantasies; an NEI call on it then returns B200BO_ERR_STATE. */
+int b200bo_gp_set_fantasies(b200bo_gp* noiseless, const b200bo_gp* noisy, const double* z, const double* e, int S,
+                            const uint8_t* incumbent, double* f_out, double* best_out);
 
 /* Replaces the tail of GaussianProcessRegressor.fit (SK/gaussian_process/_gpr.py:275-285,
  * :349-367): y normalisation, K = k(X,X), K_ii += alpha, L = chol(K), alpha_ = K^-1 y, plus
