@@ -1338,7 +1338,7 @@ template <int MMA, int PIPE>
 static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
     auto fn = dreg ? predict_acq16_kernel<true, MMA, PIPE> : predict_acq16_kernel<false, MMA, PIPE>;
     if constexpr (PIPE != PIPE_CPASYNC) {  // NEI / LogNEI: bulk-copy pipes only (DESIGN.md 4.13)
-        if (P.acq_kind == B200BO_ACQ_NEI || P.acq_kind == B200BO_ACQ_LOGNEI)
+        if (acq_is_nei(P.acq_kind))
             fn = dreg ? predict_acq16_kernel<true, MMA, PIPE, true> : predict_acq16_kernel<false, MMA, PIPE, true>;
     }
     cudaLaunchConfig_t cfg;
@@ -1528,7 +1528,7 @@ static int check_spec(const b200bo_acq* spec) {
     if (!spec) return set_err(B200BO_ERR_ARG, "spec is NULL");
     if (spec->n_gps < 1 || spec->n_gps > B200BO_MAX_GPS)
         return set_err(B200BO_ERR_ARG, "n_gps=%d out of range [1,%d]", spec->n_gps, B200BO_MAX_GPS);
-    if (spec->kind < B200BO_ACQ_UCB || spec->kind > B200BO_ACQ_LOGNEI || spec->kind == 5)
+    if (!acq_kind_valid(spec->kind))
         return set_err(B200BO_ERR_ARG, "unknown acquisition kind %d", spec->kind);
     if (spec->path != B200BO_PATH_AUTO && spec->path != B200BO_PATH_STABLE)
         return set_err(B200BO_ERR_ARG, "unknown path policy %d", spec->path);
@@ -1544,7 +1544,7 @@ static int check_spec(const b200bo_acq* spec) {
     }
     if (spec->kind == B200BO_ACQ_MES && spec->gps[0]->ystar.empty())
         return set_err(B200BO_ERR_STATE, "MES: gps[0] holds no samples of the maximum (b200bo_gp_set_max_values)");
-    if ((spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI) && spec->gps[0]->fant_best.empty())
+    if (acq_is_nei(spec->kind) && spec->gps[0]->fant_best.empty())
         return set_err(B200BO_ERR_STATE, "NEI: gps[0] holds no fantasies (b200bo_gp_set_fantasies)");
     return B200BO_OK;
 }
@@ -1615,7 +1615,7 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
     if (spec->kind == B200BO_ACQ_MES) {
         P.n_ystar = (int)g0->ystar.size();
         for (int k = 0; k < P.n_ystar; ++k) P.ystar[k] = g0->ystar[k];
-    } else if (spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI) {  // A and best_s on the device
+    } else if (acq_is_nei(spec->kind)) {  // A and best_s on the device
         P.n_ystar = (int)g0->fant_best.size();
         P.fant_a = g0->fant_a.as<double>();
     }
@@ -1638,7 +1638,7 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
 // finish for every GP.
 static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool grad, cudaStream_t stream) {
     b200bo_gp* g0 = spec->gps[0];
-    const bool nei = spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI;
+    const bool nei = acq_is_nei(spec->kind);
     int rc;
     for (int g = 0; g < spec->n_gps; ++g) {
         b200bo_gp* gp = spec->gps[g];
@@ -1743,7 +1743,7 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
     if (k > 0 && !d_sel) return set_err(B200BO_ERR_ARG, "d_sel is NULL");
     b200bo_gp* g0 = spec->gps[0];
     // NEI / LogNEI: no single mean to report; always fp64 (the 16-warp kernel or the small-batch kernels)
-    const bool nei = spec->kind == B200BO_ACQ_NEI || spec->kind == B200BO_ACQ_LOGNEI;
+    const bool nei = acq_is_nei(spec->kind);
     if (nei && (d_mu || d_sd))
         return set_err(B200BO_ERR_ARG, "NEI averages over fantasies and has no single posterior mean: mu / sd outputs "
                                        "are not available");
@@ -1822,11 +1822,8 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
                 }
                 CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off staging from the kernel time
             }
-            const int kind = spec->kind;
             prune = fused_sel && !P.acq_out && !P.mu_out && !P.sd_out && P.n_gps == 1 && pipe != PIPE_BULK_MC &&
-                    (kind == B200BO_ACQ_EI || kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_POI ||
-                     kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI) &&
-                    m <= std::numeric_limits<int>::max() && prune_enabled();
+                    acq_prunable(spec->kind) && m <= std::numeric_limits<int>::max() && prune_enabled();
             if (prune && (rc = prune_prepare(g0, P, dreg, sm.resume, stream))) return rc;
             const int refine = prune && predict_mma() == 1684 ? prune_refine_blocks(P.gp[0].np, ntiles) : 0;
             g0->stage_refined = refine > 0;
@@ -1904,9 +1901,7 @@ extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* 
                                           double* d_kmax, void* stream_) {
     int rc;
     if ((rc = check_spec(spec))) return rc;
-    if (spec->n_gps != 1 ||
-        (spec->kind != B200BO_ACQ_EI && spec->kind != B200BO_ACQ_UCB && spec->kind != B200BO_ACQ_POI &&
-         spec->kind != B200BO_ACQ_LOGEI && spec->kind != B200BO_ACQ_LOGPOI))
+    if (spec->n_gps != 1 || !acq_prunable(spec->kind))
         return set_err(B200BO_ERR_ARG, "the pruning bound covers EI, UCB, PoI, LogEI and LogPoI on one GP");
     if (m <= 0 || m > std::numeric_limits<int>::max() || !d_Xc || !d_key)
         return set_err(B200BO_ERR_ARG, "bad candidates or key buffer");

@@ -10,6 +10,26 @@ namespace b200bo {
 
 constexpr int kPad = 128;  // training-set size is padded to a multiple of this
 
+// ---- acquisition kinds (B200BO_ACQ_*, include/b200bo.h) -------------------------------------
+__host__ __device__ constexpr bool acq_is_nei(int kind) {
+    return kind == B200BO_ACQ_NEI || kind == B200BO_ACQ_LOGNEI;
+}
+__host__ __device__ constexpr bool acq_kind_valid(int kind) {
+    return kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_EI || kind == B200BO_ACQ_POI || kind == B200BO_ACQ_NONE ||
+           kind == B200BO_ACQ_MES || kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI || acq_is_nei(kind);
+}
+// The log-space kinds: the value is -(alpha + sum_j log p_j), the constraint factors summed as logs.  NEI = false in
+// the kernels built without NEI / LogNEI (DESIGN.md 4.13), which then test for LogEI and LogPoI only.
+template <bool NEI = true>
+__host__ __device__ constexpr bool acq_constraints_in_log(int kind) {
+    return kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI || (NEI && kind == B200BO_ACQ_LOGNEI);
+}
+// The kinds of one GP that selection pruning bounds (prune_bound_key, predict16.cuh; DESIGN.md 4.9)
+__host__ __device__ constexpr bool acq_prunable(int kind) {
+    return kind == B200BO_ACQ_EI || kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_POI ||
+           acq_constraints_in_log<false>(kind);
+}
+
 // ---- branch-free fp64 primitives for the covariance functions -----------------------------
 // The kernel-matrix builders evaluate sqrt and exp for every (training point, candidate) pair
 // with only a few resident warps, so data-dependent slow-path branches (libm special cases) and

@@ -210,10 +210,9 @@ __device__ __forceinline__ unsigned long long prune_bound_key(const PredictParam
         base = fmax(mean, mean + P.kappa * sd);
         scale = fabs(mean) + fabs(P.kappa * sd);
     } else if (P.acq_kind == B200BO_ACQ_EI) {
-        const double z = a / sd;
-        base = a * ndtr(z) + sd * norm_pdf(z);
+        base = ei_term(a, sd);
         scale = fabs(base);
-    } else if (log_kind(P.acq_kind)) {
+    } else if (acq_constraints_in_log<false>(P.acq_kind)) {
         base = (P.acq_kind == B200BO_ACQ_LOGPOI && a >= 0.0) ? 0.0 : log_acq_term(P.acq_kind, a, sd);
         scale = fabs(base) + kPruneLogAbsMargin / kPruneRelMargin;
     } else {

@@ -117,31 +117,78 @@ __device__ __forceinline__ void dmma1684(double& c0, double& c1, double& c2, dou
                  : "d"(a0), "d"(a1), "d"(b));
 }
 
+// The out-of-line terms below and candidate_epilogue take a GRAD flag.  GRAD = false is the value alone: the
+// out-pointers are unused and dropped, so the value keeps its scalar-and-pointer signature and the predict kernels
+// compile as without them.  GRAD = true (small_finish_grad_kernel) also writes, from the same evaluation, the term's
+// coefficients of d mean and d sd (data units): d term = cm d mean + cs d sd.  Callers pass the out-pointers through
+// grad_out, so that no local's address reaches a value-form call: an escaping address alone changes the code the
+// value kernels compile to.
+template <bool GRAD>
+__device__ __forceinline__ double* grad_out(double& x) {
+    return GRAD ? &x : nullptr;
+}
+
 // One sample's term of max-value entropy search (Wang & Jegelka, ICML 2017, eq. 6) at g = (y*_k - mu) / sigma:
-//   g psi(g) / (2 Psi(g)) - log Psi(g)
+//   t(g) = g psi(g) / (2 Psi(g)) - log Psi(g)
 // Out of line (DESIGN.md 4.8): inlined into the 16-warp kernel, which runs at its 128-register cap, the term's
 // libdevice code made ptxas place spill code in the clustered kernel's phase-B k-loop; as a call, the spill code the
 // MES branch adds in every predict kernel lies outside the phase-B k-loops.  For finite g the product is finite (psi
 // underflows to 0 above g ~ 38.6); the guard keeps g = +inf (sigma underflowing against y* - mu) at its limit 0.
-__device__ __noinline__ double mes_term(double g) {
+// GRAD: dt = t'(g).  With lambda = psi / Psi (inv_mills), lambda' = -lambda (g + lambda), so
+// t' = -lambda/2 - g lambda (g + lambda)/2; lambda = 0 is the limit 0.
+template <bool GRAD = false>
+__device__ __noinline__ double mes_term(double g, double* dt = nullptr) {
     const double r = inv_mills(g);
     const double a = (r == 0.0) ? 0.0 : 0.5 * g * r;
+    if constexpr (GRAD) *dt = (r == 0.0) ? 0.0 : -0.5 * r - 0.5 * g * r * (g + r);
     return a - log_ndtr(g);
 }
 
-__device__ __forceinline__ bool log_kind(int kind) {
-    return kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI;
+// EI at a = mean - y_max - xi; GRAD: cm = Phi(z), cs = phi(z).  The compiler contracts the sum into one FMA, and
+// which product it fuses depends on the surrounding code (see the gradient form of candidate_epilogue).
+template <bool GRAD = false>
+__device__ __forceinline__ double ei_term(double a, double sd, double* cm = nullptr, double* cs = nullptr) {
+    const double z = a / sd;
+    if constexpr (GRAD) {
+        *cm = ndtr(z);
+        *cs = norm_pdf(z);
+    }
+    return a * ndtr(z) + sd * norm_pdf(z);
 }
 
-__device__ __forceinline__ bool nei_kind(int kind) { return kind == B200BO_ACQ_NEI || kind == B200BO_ACQ_LOGNEI; }
+// One fantasy's EI in nei_term, out of line like mes_term.
+template <bool GRAD = false>
+__device__ __noinline__ double nei_ei_term(double a, double sd, double* cm = nullptr, double* cs = nullptr) {
+    return ei_term<GRAD>(a, sd, cm, cs);
+}
 
 // LogEI / LogPoI at a = mean - y_max - xi (include/b200bo.h), out of line like mes_term.  sigma = 0, or a sigma so
 // small that z = a / sigma is infinite: the log of the EI limit max(a, 0) (log a, -inf, NaN at a = 0); log_ndtr has
 // the PoI limits already (0 at z = +inf, -inf at -inf, NaN at NaN).
-__device__ __noinline__ double log_acq_term(int kind, double a, double sd) {
+// GRAD: LogEI cm = r / sd, cs = q / sd (log_h_ratios); LogPoI cm = lambda / sd, cs = -z lambda / sd (inv_mills).
+// sd = 0 or an infinite z: LogEI = log a for a > 0 has cm = 1/a; everything else is a constant (cm = cs = 0).
+template <bool GRAD = false>
+__device__ __noinline__ double log_acq_term(int kind, double a, double sd, double* cm = nullptr, double* cs = nullptr) {
     const double z = a / sd;
-    if (kind == B200BO_ACQ_LOGPOI) return log_ndtr(z);
-    if (sd == 0.0 || isinf(z)) return a > 0.0 ? log(a) : (a < 0.0 ? -CUDART_INF : CUDART_NAN);
+    if constexpr (GRAD) *cm = *cs = 0.0;
+    if (kind == B200BO_ACQ_LOGPOI) {
+        if (GRAD && sd > 0.0 && !isinf(z)) {
+            const double lam = inv_mills(z);
+            *cm = lam / sd;
+            *cs = lam == 0.0 ? 0.0 : -z * lam / sd;
+        }
+        return log_ndtr(z);
+    }
+    if (sd == 0.0 || isinf(z)) {
+        if (GRAD && a > 0.0) *cm = 1.0 / a;
+        return a > 0.0 ? log(a) : (a < 0.0 ? -CUDART_INF : CUDART_NAN);
+    }
+    if constexpr (GRAD) {
+        double r, q;
+        log_h_ratios(z, r, q);
+        *cm = r / sd;
+        *cs = q / sd;
+    }
     return log_h(z) + log(sd);
 }
 
@@ -149,23 +196,45 @@ __device__ __noinline__ double log_acq_term(int kind, double a, double sd) {
 // through log_ndtr(u) / log_ndtr(-l); a pair in one tail reflected so that both arguments a <= b are <= 0, then
 // log Phi(b) + log1mexp(log Phi(a) - log Phi(b)); a straddling pair directly.  A finite bound with sd <= 0 (or a NaN
 // mean) is the frozen-norm NaN of norm_cdf_loc_scale.
-__device__ __noinline__ double log_cfactor(double lb, double ub, double mean, double sd) {
+// GRAD: cm = -(F_l + F_u) / sd, cs = -(l F_l + u F_u) / sd, with F_l, F_u the partials of log p in l and u, each ratio
+// phi / p in the same tail-safe form as the value:
+//   one-sided: F_u = lambda(u), F_l = -lambda(-l);   straddling: F_u = phi(u)/p, F_l = -phi(l)/p;
+//   one tail, d = log Phi(a) - log Phi(b): phi(b)/p = lambda(b)/(-expm1(d)), phi(a)/p = lambda(a) e^d/(-expm1(d)),
+//   with the signs of the reflection.  Where the value is NaN the coefficients are 0.
+template <bool GRAD = false>
+__device__ __noinline__ double log_cfactor(double lb, double ub, double mean, double sd, double* cm = nullptr,
+                                           double* cs = nullptr) {
+    if constexpr (GRAD) *cm = *cs = 0.0;
     const bool has_l = lb != -CUDART_INF, has_u = ub != CUDART_INF;
     if (!has_l && !has_u) return 0.0;
     if (!(sd > 0.0) || isnan(mean)) return CUDART_NAN;
     const double u = (ub - mean) / sd, l = (lb - mean) / sd;
-    if (!has_l) return log_ndtr(u);
-    if (!has_u) return log_ndtr(-l);
-    if (l < 0.0 && u > 0.0) return log(ndtr(u) - ndtr(l));
-    const double a = l >= 0.0 ? -u : l, b = l >= 0.0 ? -l : u;
-    const double lpb = log_ndtr(b);
-    return lpb + log1mexp(log_ndtr(a) - lpb);
-}
-
-// One fantasy's EI at a = mu_s - best_s - xi: EI's formula of candidate_epilogue, with its sigma = 0 limits.
-__device__ __noinline__ double nei_ei_term(double a, double sd) {
-    const double z = a / sd;
-    return a * ndtr(z) + sd * norm_pdf(z);
+    auto coef = [&](double fl, double fu) {
+        *cm = -(fl + fu) / sd;
+        *cs = -((fl == 0.0 ? 0.0 : l * fl) + (fu == 0.0 ? 0.0 : u * fu)) / sd;
+    };
+    if (!has_l) {
+        if constexpr (GRAD) coef(0.0, inv_mills(u));
+        return log_ndtr(u);
+    }
+    if (!has_u) {
+        if constexpr (GRAD) coef(-inv_mills(-l), 0.0);
+        return log_ndtr(-l);
+    }
+    if (l < 0.0 && u > 0.0) {
+        const double p = ndtr(u) - ndtr(l);
+        if constexpr (GRAD) coef(-norm_pdf(l) / p, norm_pdf(u) / p);
+        return log(p);
+    }
+    const bool refl = l >= 0.0;
+    const double a = refl ? -u : l, b = refl ? -l : u;
+    const double lpb = log_ndtr(b), d = log_ndtr(a) - lpb;
+    if constexpr (GRAD) {
+        const double om = -expm1(d), gb = inv_mills(b) / om;
+        const double la = inv_mills(a), ga = la == 0.0 ? 0.0 : -la * exp(d) / om;
+        coef(refl ? -gb : ga, refl ? -ga : gb);
+    }
+    return lpb + log1mexp(d);
 }
 
 // NEI / LogNEI (DESIGN.md 4.13) of one candidate, out of line like mes_term and with scalar arguments only, so that
@@ -174,10 +243,15 @@ __device__ __noinline__ double nei_ei_term(double a, double sd) {
 // const_value k(xs, Xs_i)) and A = K0^-1 F ([np][S] row-major), each summed over the training rows in index order;
 // best = best_0 .. best_{S-1} (data units).  NEI: the mean of the S EI terms in s order; LogNEI: the log of that mean
 // from the LogEI terms, shifted by their maximum.
+// GRAD: cms[s * kstr] (kcol's layout) = the coefficient of d mu_s, cs that of d sd:
+//   NEI:    cms_s = Phi(z_s) / S,  cs = sum_s phi(z_s) / S                       (EI's cm / cs per fantasy, averaged)
+//   LogNEI: cms_s = p_s cm_s,  cs = sum_s p_s cs_s,  p_s = exp(l_s - M) / sum exp(l - M)   (LogEI's, softmax-weighted)
+template <bool GRAD = false>
 __device__ __noinline__ double nei_term(int kind, const double* __restrict__ kcol, int kstr, int n,
                                         const double* __restrict__ A, const double* __restrict__ best, int S,
-                                        double y_std, double y_mean, double xi, double sd) {
-    double t[B200BO_MAX_PATHS];
+                                        double y_std, double y_mean, double xi, double sd, double* cms = nullptr,
+                                        double* cs = nullptr) {
+    double t[B200BO_MAX_PATHS], cm_s[B200BO_MAX_PATHS], cs_s[B200BO_MAX_PATHS];
 #pragma unroll
     for (int s = 0; s < B200BO_MAX_PATHS; ++s) t[s] = 0.0;
     for (int i = 0; i < n; ++i) {
@@ -187,11 +261,21 @@ __device__ __noinline__ double nei_term(int kind, const double* __restrict__ kco
         for (int s = 0; s < B200BO_MAX_PATHS; ++s)
             if (s < S) t[s] = fma(a[s], k, t[s]);
     }
+    double c = 0.0;
     if (kind == B200BO_ACQ_NEI) {
         double sum = 0.0;
 #pragma unroll
-        for (int s = 0; s < B200BO_MAX_PATHS; ++s)
-            if (s < S) sum += nei_ei_term(y_std * t[s] + y_mean - best[s] - xi, sd);
+        for (int s = 0; s < B200BO_MAX_PATHS; ++s) {
+            if (s < S) {
+                sum += nei_ei_term<GRAD>(y_std * t[s] + y_mean - best[s] - xi, sd, grad_out<GRAD>(cm_s[s]),
+                                         grad_out<GRAD>(cs_s[s]));
+                if constexpr (GRAD) {
+                    cms[s * kstr] = cm_s[s] / (double)S;
+                    c += cs_s[s];
+                }
+            }
+        }
+        if constexpr (GRAD) *cs = c / (double)S;
         return sum / (double)S;
     }
     double mx = -CUDART_INF;
@@ -199,17 +283,31 @@ __device__ __noinline__ double nei_term(int kind, const double* __restrict__ kco
 #pragma unroll
     for (int s = 0; s < B200BO_MAX_PATHS; ++s) {
         if (s < S) {
-            t[s] = log_acq_term(B200BO_ACQ_LOGEI, y_std * t[s] + y_mean - best[s] - xi, sd);
+            t[s] = log_acq_term<GRAD>(B200BO_ACQ_LOGEI, y_std * t[s] + y_mean - best[s] - xi, sd,
+                                      grad_out<GRAD>(cm_s[s]), grad_out<GRAD>(cs_s[s]));
             nan = nan || isnan(t[s]);
             mx = fmax(mx, t[s]);
+            if constexpr (GRAD) cms[s * kstr] = 0.0;
         }
     }
+    if constexpr (GRAD) *cs = 0.0;
     if (nan) return CUDART_NAN;
     if (mx == -CUDART_INF) return -CUDART_INF;
     double e = 0.0;
 #pragma unroll
     for (int s = 0; s < B200BO_MAX_PATHS; ++s)
         if (s < S) e += exp(t[s] - mx);
+    if constexpr (GRAD) {
+#pragma unroll
+        for (int s = 0; s < B200BO_MAX_PATHS; ++s) {
+            if (s < S) {
+                const double p = exp(t[s] - mx) / e;
+                cms[s * kstr] = p * cm_s[s];
+                c += p * cs_s[s];
+            }
+        }
+        *cs = c;
+    }
     return mx + log(e) - log((double)S);
 }
 
@@ -223,12 +321,21 @@ __device__ __noinline__ double nei_term(int kind, const double* __restrict__ kco
 // NEI (template flag, set in the kernel instantiations that serve NEI / LogNEI only, so that every other
 // instantiation compiles as without these kinds): base = nei_term over the candidate's K* column kcol (stride kstr);
 // constraints as for EI / LogEI.
-template <bool NEI = false>
+// GRAD: *gr = this GP's term (the base acquisition for g = 0, the factor p or log p for g >= 1) and its coefficients.
+// sd == 0 (a clamped or vanished variance): the caller sets d sd := 0, and the coefficients that divide by sd (PoI,
+// MES, the factors) are 0 - the value there is a step or constant in x.
+struct EpilogueGrad {
+    double term, cm, cs;
+    double* cms;  // NEI: the coefficients of d mu_s, cms[s * kstr] (nei_term); cm is 0
+};
+
+template <bool NEI = false, bool GRAD = false>
 __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const GpDev& G, int g,
                                                    double mu_n, double colsq, long long gi,
                                                    double& base_neg, double& prod, double* final_val = nullptr,
-                                                   const double* kcol = nullptr, int kstr = 0) {
-    const bool logk = log_kind(P.acq_kind) || (NEI && P.acq_kind == B200BO_ACQ_LOGNEI);
+                                                   const double* kcol = nullptr, int kstr = 0,
+                                                   EpilogueGrad* gr = nullptr) {
+    const bool logk = acq_constraints_in_log<NEI>(P.acq_kind);
     const double mean = G.y_std * mu_n + G.y_mean;
     double var = G.prior - colsq;
     if (var < 0.0) {
@@ -236,42 +343,90 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
         if (P.clamp_count && gi < P.m) atomicAdd(P.clamp_count, 1ull);
     }
     const double sd = sqrt(var * (G.y_std * G.y_std));
+    double term = 0.0, cm = 0.0, cs = 0.0;
     if (g == 0) {
-        double base = 0.0;
         if (P.acq_kind == B200BO_ACQ_UCB) {
-            base = mean + P.kappa * sd;
+            term = mean + P.kappa * sd;
+            cm = 1.0;
+            cs = P.kappa;
         } else if (P.acq_kind == B200BO_ACQ_EI) {
             const double a = mean - P.y_max - P.xi;
-            const double z = a / sd;
-            base = a * ndtr(z) + sd * norm_pdf(z);
+            if constexpr (GRAD) {
+                // the FMA every value kernel contracts ei_term's sum to, written out: left to the compiler, this form
+                // fuses the other product and the value loses its bits
+                const double z = a / sd;
+                cm = ndtr(z);
+                cs = norm_pdf(z);
+                term = fma(sd, cs, a * cm);
+            } else {
+                term = ei_term(a, sd);
+            }
         } else if (P.acq_kind == B200BO_ACQ_POI) {
             const double z = (mean - P.y_max - P.xi) / sd;
-            base = ndtr(z);
+            term = ndtr(z);
+            if (GRAD && sd > 0.0) {
+                const double pz = norm_pdf(z);
+                cm = pz / sd;
+                cs = pz == 0.0 ? 0.0 : -z * pz / sd;
+            }
         } else if (P.acq_kind == B200BO_ACQ_MES) {
             if (sd > 0.0) {
-                double s = 0.0;
-                for (int k = 0; k < P.n_ystar; ++k) s += mes_term((P.ystar[k] - mean) / sd);
-                base = s / (double)P.n_ystar;
+                double s = 0.0, sm = 0.0, ss = 0.0;
+                for (int k = 0; k < P.n_ystar; ++k) {
+                    const double gk = (P.ystar[k] - mean) / sd;
+                    double td;
+                    s += mes_term<GRAD>(gk, grad_out<GRAD>(td));
+                    if constexpr (GRAD) {
+                        sm += td;
+                        ss += td == 0.0 ? 0.0 : td * gk;
+                    }
+                }
+                term = s / (double)P.n_ystar;
+                cm = -sm / ((double)P.n_ystar * sd);
+                cs = -ss / ((double)P.n_ystar * sd);
             }
-        } else if (NEI && nei_kind(P.acq_kind)) {
-            base = nei_term(P.acq_kind, kcol, kstr, G.n, P.fant_a, P.fant_a + (size_t)G.np * P.n_ystar, P.n_ystar,
-                            G.y_std, G.y_mean, P.xi, sd);
-        } else if (log_kind(P.acq_kind)) {
-            base = log_acq_term(P.acq_kind, mean - P.y_max - P.xi, sd);
+        } else if (NEI && acq_is_nei(P.acq_kind)) {
+            term = nei_term<GRAD>(P.acq_kind, kcol, kstr, G.n, P.fant_a, P.fant_a + (size_t)G.np * P.n_ystar,
+                                  P.n_ystar, G.y_std, G.y_mean, P.xi, sd, GRAD ? gr->cms : nullptr,
+                                  grad_out<GRAD>(cs));
+        } else if (acq_constraints_in_log<false>(P.acq_kind)) {  // LogEI / LogPoI
+            term = log_acq_term<GRAD>(P.acq_kind, mean - P.y_max - P.xi, sd, grad_out<GRAD>(cm), grad_out<GRAD>(cs));
         }
-        base_neg = -1.0 * base;
+        base_neg = -1.0 * term;
         prod = 1.0;
         if (gi < P.m) {
             if (P.mu_out) P.mu_out[gi] = mean;
             if (P.sd_out) P.sd_out[gi] = sd;
         }
     } else if (logk) {
-        base_neg = base_neg - log_cfactor(G.lb, G.ub, mean, sd);
+        // base_neg is read before the call, the order the value kernels have always been compiled from
+        base_neg = base_neg -
+                   (term = log_cfactor<GRAD>(G.lb, G.ub, mean, sd, grad_out<GRAD>(cm), grad_out<GRAD>(cs)));
     } else {
         const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
         const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
         // constraint.py:208 (J=1: result = p_hi - p_lo) / :219 (result *= ...)
         prod = (g == 1) ? (p_hi - p_lo) : prod * (p_hi - p_lo);
+        if constexpr (GRAD) {
+            term = p_hi - p_lo;
+            if (sd > 0.0) {
+                if (G.lb != -CUDART_INF) {
+                    const double z = (G.lb - mean) / sd, pz = norm_pdf(z);
+                    cm += pz / sd;
+                    cs += pz == 0.0 ? 0.0 : z * pz / sd;
+                }
+                if (G.ub != CUDART_INF) {
+                    const double z = (G.ub - mean) / sd, pz = norm_pdf(z);
+                    cm -= pz / sd;
+                    cs -= pz == 0.0 ? 0.0 : z * pz / sd;
+                }
+            }
+        }
+    }
+    if constexpr (GRAD) {
+        gr->term = term;
+        gr->cm = cm;
+        gr->cs = cs;
     }
     if (g == P.n_gps - 1) {
         const double val = (P.n_gps > 1 && !logk) ? base_neg * prod : base_neg;
@@ -1209,197 +1364,15 @@ small_grad_kernel(const SmallParams S, int g) {
     }
 }
 
-// t'(g) of one MES sample's term t(g) = g lambda / 2 - log Psi(g), lambda = psi / Psi (inv_mills):
-// lambda' = -lambda (g + lambda), so t' = -lambda/2 - g lambda (g + lambda)/2.  Out of line like mes_term;
-// lambda = 0 (g above ~38.6) is the limit 0.
-__device__ __noinline__ double mes_term_deriv(double g) {
-    const double r = inv_mills(g);
-    if (r == 0.0) return 0.0;
-    return -0.5 * r - 0.5 * g * r * (g + r);
-}
-
-// LogEI / LogPoI: the value of log_acq_term and its coefficients of d mean and d sd, out of line like mes_term_deriv.
-//   LogEI: cm = r / sd, cs = q / sd (log_h_ratios);   LogPoI: cm = lambda / sd, cs = -z lambda / sd (inv_mills).
-// sd = 0 or an infinite z: LogEI = log a for a > 0 has cm = 1/a; everything else is a constant (cm = cs = 0).
-__device__ __noinline__ double log_acq_term_grad(int kind, double a, double sd, double& cm, double& cs) {
-    const double z = a / sd;
-    cm = cs = 0.0;
-    if (kind == B200BO_ACQ_LOGPOI) {
-        if (sd > 0.0 && !isinf(z)) {
-            const double lam = inv_mills(z);
-            cm = lam / sd;
-            cs = lam == 0.0 ? 0.0 : -z * lam / sd;
-        }
-        return log_ndtr(z);
-    }
-    if (sd == 0.0 || isinf(z)) {
-        if (a > 0.0) cm = 1.0 / a;
-        return a > 0.0 ? log(a) : (a < 0.0 ? -CUDART_INF : CUDART_NAN);
-    }
-    double r, q;
-    log_h_ratios(z, r, q);
-    cm = r / sd;
-    cs = q / sd;
-    return log_h(z) + log(sd);
-}
-
-// NEI / LogNEI value of one candidate (as nei_term) and its coefficients: d value = sum_s cms[s * SMC] d mu_s + cs d sd.
-//   NEI:    cms_s = Phi(z_s) / S,  cs = sum_s phi(z_s) / S                   (EI's cm / cs per fantasy, averaged)
-//   LogNEI: cms_s = p_s cm_s,       cs = sum_s p_s cs_s,  p_s = exp(l_s - M) / sum exp(l - M)   (LogEI's, softmax-weighted)
-// cms: S coefficients with stride SMC (shared memory of small_finish_grad_kernel).  Out of line like nei_term.
-__device__ __noinline__ double nei_term_grad(int kind, const double* __restrict__ kcol, int kstr, int n,
-                                             const double* __restrict__ A, const double* __restrict__ best, int S,
-                                             double y_std, double y_mean, double xi, double sd, double* cms,
-                                             double& cs) {
-    double t[B200BO_MAX_PATHS];
-    for (int s = 0; s < S; ++s) t[s] = 0.0;
-    for (int i = 0; i < n; ++i) {
-        const double k = kcol[(size_t)i * kstr];
-        for (int s = 0; s < S; ++s) t[s] = fma(A[(size_t)i * S + s], k, t[s]);
-    }
-    cs = 0.0;
-    if (kind == B200BO_ACQ_NEI) {
-        double sum = 0.0;
-        for (int s = 0; s < S; ++s) {
-            const double a = y_std * t[s] + y_mean - best[s] - xi;
-            const double z = a / sd;
-            sum += nei_ei_term(a, sd);
-            cms[s * SMC] = ndtr(z) / (double)S;
-            cs += norm_pdf(z);
-        }
-        cs = cs / (double)S;
-        return sum / (double)S;
-    }
-    double cm_s[B200BO_MAX_PATHS], cs_s[B200BO_MAX_PATHS];
-    double mx = -CUDART_INF;
-    bool nan = false;
-    for (int s = 0; s < S; ++s) {
-        t[s] = log_acq_term_grad(B200BO_ACQ_LOGEI, y_std * t[s] + y_mean - best[s] - xi, sd, cm_s[s], cs_s[s]);
-        nan = nan || isnan(t[s]);
-        mx = fmax(mx, t[s]);
-    }
-    for (int s = 0; s < S; ++s) cms[s * SMC] = 0.0;
-    if (nan) return CUDART_NAN;
-    if (mx == -CUDART_INF) return -CUDART_INF;
-    double e = 0.0;
-    for (int s = 0; s < S; ++s) e += exp(t[s] - mx);
-    for (int s = 0; s < S; ++s) {
-        const double p = exp(t[s] - mx) / e;
-        cms[s * SMC] = p * cm_s[s];
-        cs += p * cs_s[s];
-    }
-    return mx + log(e) - log((double)S);
-}
-
-// d log p = cm d mean + cs d sd for one constraint factor (log_cfactor), with F_l, F_u the partials of log p in l and u
-// (d u = -(d mean + u d sd) / sd, the same for l), each ratio phi / p in the same tail-safe form as the value:
-//   one-sided: F_u = lambda(u), F_l = -lambda(-l);   straddling: F_u = phi(u)/p, F_l = -phi(l)/p;
-//   one tail, a <= b <= 0, d = log Phi(a) - log Phi(b): phi(b)/p = lambda(b)/(-expm1(d)),
-//   phi(a)/p = lambda(a) e^d/(-expm1(d)), with the signs of the reflection.  sd <= 0 or a NaN mean: the value is NaN.
-__device__ __noinline__ void log_cfactor_grad(double lb, double ub, double mean, double sd, double& cm, double& cs) {
-    cm = cs = 0.0;
-    const bool has_l = lb != -CUDART_INF, has_u = ub != CUDART_INF;
-    if ((!has_l && !has_u) || !(sd > 0.0)) return;
-    const double u = (ub - mean) / sd, l = (lb - mean) / sd;
-    double fl = 0.0, fu = 0.0;
-    if (!has_l) {
-        fu = inv_mills(u);
-    } else if (!has_u) {
-        fl = -inv_mills(-l);
-    } else if (l < 0.0 && u > 0.0) {
-        const double p = ndtr(u) - ndtr(l);
-        fu = norm_pdf(u) / p;
-        fl = -norm_pdf(l) / p;
-    } else {
-        const bool refl = l >= 0.0;
-        const double a = refl ? -u : l, b = refl ? -l : u;
-        const double d = log_ndtr(a) - log_ndtr(b), om = -expm1(d);
-        const double gb = inv_mills(b) / om;
-        const double la = inv_mills(a), ga = la == 0.0 ? 0.0 : -la * exp(d) / om;
-        fl = refl ? -gb : ga;
-        fu = refl ? -ga : gb;
-    }
-    cm = -(fl + fu) / sd;
-    cs = -((fl == 0.0 ? 0.0 : l * fl) + (fu == 0.0 ? 0.0 : u * fu)) / sd;
-}
-
-// Chain rule of one GP's factor in data units, as the coefficients of d mean and d sd:
-//   d term = cm d mean + cs d sd,   term = the base acquisition (g = 0) or the probability factor p (g >= 1).
-// Returns the term itself in `term`.  sd == 0 (a clamped or vanished variance): the caller sets d sd := 0, and the
-// coefficients that divide by sd (PoI, MES) are 0 - the value there is a step or constant in x.
-// NEI: as candidate_epilogue's flag - LogNEI's constraint GPs enter as log p_j, like LogEI's.
-template <bool NEI = false>
-__device__ __forceinline__ void candidate_epilogue_grad(const PredictParams& P, const GpDev& G, int g, double mean,
-                                                        double sd, double& term, double& cm, double& cs) {
-    const bool logk = log_kind(P.acq_kind) || (NEI && P.acq_kind == B200BO_ACQ_LOGNEI);
-    cm = cs = 0.0;
-    if (g == 0) {
-        term = 0.0;
-        if (P.acq_kind == B200BO_ACQ_UCB) {
-            term = mean + P.kappa * sd;
-            cm = 1.0;
-            cs = P.kappa;
-        } else if (P.acq_kind == B200BO_ACQ_EI) {
-            const double a = mean - P.y_max - P.xi;
-            const double z = a / sd;
-            term = a * ndtr(z) + sd * norm_pdf(z);
-            cm = ndtr(z);
-            cs = norm_pdf(z);
-        } else if (P.acq_kind == B200BO_ACQ_POI) {
-            const double z = (mean - P.y_max - P.xi) / sd;
-            term = ndtr(z);
-            if (sd > 0.0) {
-                const double pz = norm_pdf(z);
-                cm = pz / sd;
-                cs = pz == 0.0 ? 0.0 : -z * pz / sd;
-            }
-        } else if (P.acq_kind == B200BO_ACQ_MES) {
-            if (sd > 0.0) {
-                double s = 0.0, sm = 0.0, ss = 0.0;
-                for (int k = 0; k < P.n_ystar; ++k) {
-                    const double gk = (P.ystar[k] - mean) / sd;
-                    s += mes_term(gk);
-                    const double td = mes_term_deriv(gk);
-                    sm += td;
-                    ss += td == 0.0 ? 0.0 : td * gk;
-                }
-                term = s / (double)P.n_ystar;
-                cm = -sm / ((double)P.n_ystar * sd);
-                cs = -ss / ((double)P.n_ystar * sd);
-            }
-        } else if (log_kind(P.acq_kind)) {
-            term = log_acq_term_grad(P.acq_kind, mean - P.y_max - P.xi, sd, cm, cs);
-        }
-    } else if (logk) {
-        term = log_cfactor(G.lb, G.ub, mean, sd);
-        log_cfactor_grad(G.lb, G.ub, mean, sd, cm, cs);
-    } else {
-        const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
-        const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
-        term = p_hi - p_lo;
-        if (sd > 0.0) {
-            if (G.lb != -CUDART_INF) {
-                const double z = (G.lb - mean) / sd, pz = norm_pdf(z);
-                cm += pz / sd;
-                cs += pz == 0.0 ? 0.0 : z * pz / sd;
-            }
-            if (G.ub != CUDART_INF) {
-                const double z = (G.ub - mean) / sd, pz = norm_pdf(z);
-                cm -= pz / sd;
-                cs -= pz == 0.0 ? 0.0 : z * pz / sd;
-            }
-        }
-    }
-}
-
-// Gradient finish, per pass (blockIdx.x): the value exactly as small_finish_kernel forms it (same sums, same
-// epilogue), then per candidate and GP the weights of the two partial-sum lists,
+// Gradient finish, per pass (blockIdx.x): per candidate and GP one candidate_epilogue<NEI, true>, which forms the value
+// exactly as small_finish_kernel does (same sums, same epilogue) and gives the GP's term and its coefficients; from
+// them the weights of the two partial-sum lists,
 //   grad_j = sum_g ( wa_g sum_b gpart_g[b][0][j] + wu_g sum_b gpart_g[b][1][j] ) / ls_gj      (blocks b in index order)
 //   wa_g = -w_g cm_g s_y,   wu_g = w_g cs_g s_y / sqrt(var_g)   (0 where var_g <= 0: d sd := 0)
 //   w_0 = -prod_i p_i,   w_g = -base prod_{i != g} p_i           (product rule over the GPs, g order)
 //   LogEI / LogPoI: w_g = -1 (the value is -(alpha + sum_g log p_g), a plain sum)
 // A rounded dimension has gradient 0; a NaN value gives a NaN row.
-// NEI: gps[0] is the noiseless handle of an NEI / LogNEI call: its mean coefficient is one per fantasy (nei_term_grad,
+// NEI: gps[0] is the noiseless handle of an NEI / LogNEI call: its mean coefficient is one per fantasy (nei_term,
 // held in wn_s) against the S lists of gpart, its sd coefficient multiplies the u list as usual.
 template <bool NEI>
 __global__ void __launch_bounds__(256)
@@ -1417,10 +1390,6 @@ small_finish_grad_kernel(const SmallParams S) {
     if (sl == 0 && c < mc) {
         double base_neg = 0.0, prod = 1.0, val = 0.0;
         const double* kcol = S.sg[0].ksm + (size_t)pass * S.P.gp[0].np * SMC + c;
-        for (int g = 0; g < ng; ++g)
-            candidate_epilogue<NEI>(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, &val, kcol,
-                                    SMC);
-        val_s[c] = val;
         // term_g, then w_g from the terms of the other GPs; wa_s / wu_s hold cm / cs until the second loop
         double term[B200BO_MAX_GPS];
 #pragma unroll
@@ -1428,25 +1397,19 @@ small_finish_grad_kernel(const SmallParams S) {
             term[g] = 1.0;
             if (g < ng) {
                 const GpDev& G = S.P.gp[g];
-                const double mean = G.y_std * mu_s[g][c] + G.y_mean;
+                EpilogueGrad e;
+                e.cms = &wn_s[0][c];
+                candidate_epilogue<NEI, true>(S.P, G, g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, &val,
+                                              kcol, SMC, &e);
                 const double var = fmax(G.prior - colsq_s[g][c], 0.0);
-                const double sd = sqrt(var * (G.y_std * G.y_std));
-                double cm, cs;
-                if (NEI && g == 0) {
-                    const GpDev& G0 = S.P.gp[0];
-                    term[0] = nei_term_grad(S.P.acq_kind, kcol, SMC, G0.n, S.P.fant_a,
-                                            S.P.fant_a + (size_t)G0.np * S.P.n_ystar, S.P.n_ystar, G0.y_std,
-                                            G0.y_mean, S.P.xi, sd, &wn_s[0][c], cs);
-                    cm = 1.0;  // the per-fantasy coefficients are in wn_s
-                } else {
-                    candidate_epilogue_grad<NEI>(S.P, G, g, mean, sd, term[g], cm, cs);
-                }
-                wa_s[g][c] = -cm * G.y_std;
-                wu_s[g][c] = var > 0.0 ? cs * G.y_std / sqrt(var) : 0.0;
+                term[g] = e.term;
+                wa_s[g][c] = -e.cm * G.y_std;
+                wu_s[g][c] = var > 0.0 ? e.cs * G.y_std / sqrt(var) : 0.0;
             }
         }
+        val_s[c] = val;
         // the value is -sum_g term_g: w_g = -1, no product rule
-        const bool logk = log_kind(S.P.acq_kind) || (NEI && S.P.acq_kind == B200BO_ACQ_LOGNEI);
+        const bool logk = acq_constraints_in_log<NEI>(S.P.acq_kind);
 #pragma unroll
         for (int g = 0; g < B200BO_MAX_GPS; ++g) {
             if (g < ng) {
