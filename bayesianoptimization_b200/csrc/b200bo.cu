@@ -156,14 +156,17 @@ struct b200bo_gp {
     // bulk-copy phase B of the fp64 kernel: L^-1 as padded stage images (built on first use after a fit)
     DevBuf pad_linv;
     bool pad_valid = false;
+    // Gram bound pass of pruning: the training-side operand, A1 and Ymax (built on first use after a fit)
+    DevBuf gram;
+    bool gram_valid = false;
     DevBuf cov_xc, cov_kst, cov_v, cov_c, cov_out, cov_mu;  // predict(return_cov=True) scratch
     DevBuf sel_cta;         // per-CTA running selection lists of the fused kernels
     // selection-only pruning: bound keys / local indices (two buffers each for the radix sort), its temp storage and
     // the control words of predict_acq16_kernel's prune mode
     DevBuf prune_key, prune_idx, prune_tmp, prune_ctl;
-    // its refine stages: K* alpha_ per candidate from the bound pass, the survivor list, the per-row-block partials
-    // and arrival counters of predict_units_kernel
-    DevBuf prune_mu, prune_surv, prune_part, prune_arrive;
+    // its refine stages: the interval of K* alpha_ per candidate from the bound pass, the survivor list, the
+    // per-row-block partials, K* alpha_ of the tiles and the arrival counters of predict_units_kernel
+    DevBuf prune_mu, prune_surv, prune_part, prune_mu_unit, prune_arrive;
     // candidates of the last call (chunked: all chunks) and those of them evaluated outside the prune mode; the
     // prune mode counts its own in prune_ctl[2] (prune_counted)
     long long stat_total = 0, stat_direct = 0;
@@ -276,6 +279,9 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_units_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -422,6 +428,7 @@ extern "C" int b200bo_gp_set_data(b200bo_gp* gp, const double* X, const double* 
     gp->replica = false;
     gp->tc_valid = false;
     gp->pad_valid = false;
+    gp->gram_valid = false;
     gp->n = n;
     gp->d = d;
     gp->np = round_up(n, kPad);
@@ -948,6 +955,7 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     gp->n = nn;
     gp->tc_valid = false;
     gp->pad_valid = false;
+    gp->gram_valid = false;
     if ((rc = solve_alpha(gp))) return rc;
     CU(cudaDeviceSynchronize());
     return B200BO_OK;
@@ -991,6 +999,7 @@ extern "C" int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, d
         gp->n = n + 1;
         gp->tc_valid = false;
         gp->pad_valid = false;
+        gp->gram_valid = false;
     }
     CU(cudaDeviceSynchronize());
     return B200BO_OK;
@@ -1086,6 +1095,7 @@ extern "C" int b200bo_gp_lml(b200bo_gp* gp, const b200bo_kernel* kern, double al
     gp->fitted = false;  // buffers are being overwritten
     gp->tc_valid = false;
     gp->pad_valid = false;
+    gp->gram_valid = false;
     const int n = (int)gp->n, np = gp->np, d = gp->d;
     const int aniso = kern->n_length_scale > 1;
     const int want_noise = (has_const & 2) ? 1 : 0;
@@ -1422,6 +1432,7 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     int rc;
     if ((rc = g0->prune_surv.reserve(sizeof(int) * (size_t)kRefineMaxTiles * PBN))) return rc;
     if ((rc = g0->prune_part.reserve(sizeof(double) * (size_t)kUnitSlots * nb * 32 * PBN))) return rc;
+    if ((rc = g0->prune_mu_unit.reserve(sizeof(double) * (size_t)kUnitSlots * PBN))) return rc;
     if ((rc = g0->prune_arrive.reserve(sizeof(unsigned) * kUnitSlots))) return rc;
     unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
     if (!resume) CU(cudaMemsetAsync(ctl + kCtlRefined, 0, sizeof(unsigned long long), stream));
@@ -1429,7 +1440,8 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     prune_ctl_refine_kernel<<<1, 1, 0, stream>>>(ctl);
     LAUNCHED();
     RefineParams R;
-    R.mu_n = g0->prune_mu.as<double>();
+    R.mu = g0->prune_mu.as<double2>();
+    R.mu_unit = g0->prune_mu_unit.as<double>();
     R.surv = g0->prune_surv.as<int>();
     R.part = g0->prune_part.as<double>();
     R.arrive = g0->prune_arrive.as<unsigned>();
@@ -1456,26 +1468,69 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     return B200BO_OK;
 }
 
+// Gram bound pass operand of pruning (once per fit)
+static int ensure_gram(b200bo_gp* gp, cudaStream_t stream) {
+    if (gp->gram_valid) return B200BO_OK;
+    const int np = gp->np, d = gp->d;
+    int rc;
+    if ((rc = gp->gram.reserve(sizeof(double) * ((size_t)np * gram_stride(d) + 2)))) return rc;
+    double* img = gp->gram.as<double>();
+    gram_operand_kernel<<<(np + 255) / 256, 256, 0, stream>>>(gp->Xs.as<double>(), (int)gp->n, np, d, img);
+    LAUNCHED();
+    gram_stats_kernel<<<1, 1024, 0, stream>>>(gp->alphav.as<double>(), (int)gp->n, d, img,
+                                              img + (size_t)np * gram_stride(d));
+    LAUNCHED();
+    CU(cudaGetLastError());
+    gp->gram_valid = true;
+    return B200BO_OK;
+}
+
+// The bound pass of a pruned launch: the Gram pass (distances on the fp64 tensor pipe) for every covariance whose
+// dk/d(r^2) is bounded, the direct pass for Matern-0.5 (DESIGN.md 4.9).  mu: [m] interval (mu_lo, mu_hi); idx, kmax
+// may be nullptr.
+static int launch_bound_pass(b200bo_gp* g0, PredictParams& P, bool gram, unsigned long long* keys, int* idx,
+                             double* kmax, double2* mu, cudaStream_t stream) {
+    const unsigned ntiles = (unsigned)((P.m + PBN - 1) / PBN);
+    if (gram) {
+        int rc;
+        if ((rc = ensure_gram(g0, stream))) return rc;
+        P.gp[0].gram = g0->gram.as<double>();
+        const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * gram_stride(P.d) + 2 * PA_CHUNK);
+        switch (cov_code(P.gp[0].family, P.gp[0].nu)) {
+            case 1: predict_bound_gram_kernel<1><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+            case 2: predict_bound_gram_kernel<2><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+            default: predict_bound_gram_kernel<3><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        }
+    } else {
+        const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
+        if (P.d <= kPredictMaxDimRegs)
+            predict_bound_kernel<true><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu);
+        else
+            predict_bound_kernel<false><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu);
+    }
+    LAUNCHED();
+    CU(cudaGetLastError());
+    return B200BO_OK;
+}
+
 // Bound pass + radix sort of (bound key, local index): fills P.perm / P.perm_key / P.prune_ctl for predict_acq16_kernel.
 // The k-th key word and the evaluated count carry over from launch to launch of a chunked batch (resume).
-static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool dreg, bool resume, cudaStream_t stream) {
-    const long long m = P.m, ntiles = (m + PBN - 1) / PBN;
+static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool resume, cudaStream_t stream) {
+    const long long m = P.m;
     int rc;
     if ((rc = g0->prune_key.reserve(sizeof(unsigned long long) * 2 * (size_t)m))) return rc;
     if ((rc = g0->prune_idx.reserve(sizeof(int) * 2 * (size_t)m))) return rc;
     if ((rc = g0->prune_ctl.reserve(sizeof(unsigned long long) * kCtlWords))) return rc;
-    if ((rc = g0->prune_mu.reserve(sizeof(double) * (size_t)m))) return rc;
-    double* mu = g0->prune_mu.as<double>();
+    if ((rc = g0->prune_mu.reserve(sizeof(double2) * (size_t)m))) return rc;
     unsigned long long* keys = g0->prune_key.as<unsigned long long>();
     int* idx = g0->prune_idx.as<int>();
     unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
-    const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
-    if (dreg)
-        predict_bound_kernel<true><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr, mu);
-    else
-        predict_bound_kernel<false><<<(unsigned)ntiles, P16_NT, smem, stream>>>(P, keys, idx, nullptr, mu);
-    LAUNCHED();
-    CU(cudaGetLastError());
+    const bool gram = cov_code(P.gp[0].family, P.gp[0].nu) != 0;
+    if (gram && !g0->gram_valid) {
+        if ((rc = ensure_gram(g0, stream))) return rc;
+        CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off operand build from the kernel time
+    }
+    if ((rc = launch_bound_pass(g0, P, gram, keys, idx, nullptr, g0->prune_mu.as<double2>(), stream))) return rc;
     CU(cudaEventRecord(g0->ev_stage[0], stream));
     cub::DoubleBuffer<unsigned long long> kb(keys, keys + m);
     cub::DoubleBuffer<int> ib(idx, idx + m);
@@ -1824,7 +1879,7 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             }
             prune = fused_sel && !P.acq_out && !P.mu_out && !P.sd_out && P.n_gps == 1 && pipe != PIPE_BULK_MC &&
                     acq_prunable(spec->kind) && m <= std::numeric_limits<int>::max() && prune_enabled();
-            if (prune && (rc = prune_prepare(g0, P, dreg, sm.resume, stream))) return rc;
+            if (prune && (rc = prune_prepare(g0, P, sm.resume, stream))) return rc;
             const int refine = prune && predict_mma() == 1684 ? prune_refine_blocks(P.gp[0].np, ntiles) : 0;
             g0->stage_refined = refine > 0;
             if (refine) {
@@ -1897,8 +1952,9 @@ extern "C" int b200bo_acq_eval_dev(const b200bo_acq* spec, const double* d_Xc, i
     return eval_core(spec, src, m, d_acq_neg, d_mu, d_sd, k, d_sel, index_base, (cudaStream_t)stream_);
 }
 
-extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
-                                          double* d_kmax, void* stream_) {
+// the bound pass alone, direct (gram = false) or Gram; d_mu (Gram only): [m][2] (mu_lo, mu_hi)
+static int prune_bound_entry(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key, double* d_kmax,
+                             double* d_mu, bool gram, void* stream_) {
     int rc;
     if ((rc = check_spec(spec))) return rc;
     if (spec->n_gps != 1 || !acq_prunable(spec->kind))
@@ -1906,6 +1962,8 @@ extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* 
     if (m <= 0 || m > std::numeric_limits<int>::max() || !d_Xc || !d_key)
         return set_err(B200BO_ERR_ARG, "bad candidates or key buffer");
     b200bo_gp* g0 = spec->gps[0];
+    if (gram && cov_code(g0->family, g0->nu) == 0)
+        return set_err(B200BO_ERR_UNSUPPORTED, "Matern-0.5 has no Gram bound (dk/d(r^2) is unbounded at r = 0)");
     CU(cudaSetDevice(g0->device));
     const cudaStream_t stream = (cudaStream_t)stream_;
     CandSrc src;
@@ -1913,16 +1971,18 @@ extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* 
     PredictParams P;
     int np_max = 0;
     if ((rc = fill_params(spec, src, m, 0, stream, P, np_max))) return rc;
-    const unsigned ntiles = (unsigned)((m + PBN - 1) / PBN);
-    const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
-    auto keys = reinterpret_cast<unsigned long long*>(d_key);
-    if (P.d <= kPredictMaxDimRegs)
-        predict_bound_kernel<true><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax, nullptr);
-    else
-        predict_bound_kernel<false><<<ntiles, P16_NT, smem, stream>>>(P, keys, nullptr, d_kmax, nullptr);
-    LAUNCHED();
-    CU(cudaGetLastError());
-    return B200BO_OK;
+    return launch_bound_pass(g0, P, gram, reinterpret_cast<unsigned long long*>(d_key), nullptr, d_kmax,
+                             reinterpret_cast<double2*>(d_mu), stream);
+}
+
+extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
+                                          double* d_kmax, void* stream_) {
+    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax, nullptr, false, stream_);
+}
+
+extern "C" int b200bo_acq_prune_bound_gram_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
+                                               double* d_mu, double* d_kmax_lb, void* stream_) {
+    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax_lb, d_mu, true, stream_);
 }
 
 extern "C" int b200bo_acq_select_philox_dev(const b200bo_acq* spec, uint64_t seed, const double* lo,

@@ -190,8 +190,12 @@ __device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const 
 //   rounding error is absolute: up to a few ulps of |log h| + |log sigma| (the two can cancel), and in the tail of
 //   log h it grows with z^2 ~ 2 |value|.  The margin is 1e-9 |value| + 1e-9 (kPruneLogAbsMargin): the floor covers
 //   |log sigma| <= 745 with 1e4 headroom, the relative part the tail with about 1e6.
-// Key 0 (never pruned): mu or v_lb non-finite, or a within a few ulps of 0 (sigma = 0 with a = 0 gives the NaN that
-// np.argmin reports first).  mu is bit-equal to the epilogue's: the same phase A, the same order of sums.
+// mu is known as an interval [mu_lo, mu_hi] that holds the epilogue's mu (normalised units): a point (mu_lo = mu_hi,
+// bit-equal to the epilogue's: the same phase A, the same order of sums) from the direct bound pass, a margin around the
+// Gram form's mu from the Gram bound pass (predict_bound_gram_kernel).  Every kind above increases with mu, so v_lb is
+// evaluated at mu_hi.
+// Key 0 (never pruned): mu_lo, mu_hi or v_lb non-finite, or the interval of a widened by a few ulps contains 0 (sigma
+// = 0 with a = 0 gives the NaN that np.argmin reports first).
 constexpr double kPruneVarEps = 1e-8, kPruneRelMargin = 1e-9, kPruneAbsMargin = 1e-300, kPruneLogAbsMargin = 1e-9;
 
 // var_ub: an upper bound of sigma^2 in normalised units, margin included:
@@ -200,11 +204,11 @@ __device__ __forceinline__ double prune_var_ub(const GpDev& G, double r) {
     return fmax(0.0, fmin(G.prior, G.prior - r + kPruneVarEps * G.prior));
 }
 
-__device__ __forceinline__ unsigned long long prune_bound_key(const PredictParams& P, const GpDev& G, double mu_n,
-                                                              double var_ub) {
-    const double mean = G.y_std * mu_n + G.y_mean;
+__device__ __forceinline__ unsigned long long prune_bound_key(const PredictParams& P, const GpDev& G, double mu_lo,
+                                                              double mu_hi, double var_ub) {
+    const double mean = G.y_std * mu_hi + G.y_mean, mean_lo = G.y_std * mu_lo + G.y_mean;
     const double sd = sqrt(var_ub * (G.y_std * G.y_std));
-    const double a = mean - P.y_max - P.xi;
+    const double a = mean - P.y_max - P.xi, a_lo = mean_lo - P.y_max - P.xi;
     double base, scale;
     if (P.acq_kind == B200BO_ACQ_UCB) {
         base = fmax(mean, mean + P.kappa * sd);
@@ -220,18 +224,18 @@ __device__ __forceinline__ unsigned long long prune_bound_key(const PredictParam
         scale = fabs(base);
     }
     const double v_lb = -base - (kPruneRelMargin * scale + kPruneAbsMargin);
-    const bool a_near_0 = P.acq_kind != B200BO_ACQ_UCB &&
-                          fabs(a) <= 8.0 * 2.220446049250313e-16 * (fabs(mean) + fabs(P.y_max) + fabs(P.xi));
-    if (!isfinite(mean) || !isfinite(v_lb) || a_near_0) return 0ull;
+    const double tol = 8.0 * 2.220446049250313e-16 * (fmax(fabs(mean), fabs(mean_lo)) + fabs(P.y_max) + fabs(P.xi));
+    const bool a_near_0 = P.acq_kind != B200BO_ACQ_UCB && a_lo <= tol && a >= -tol;
+    if (!isfinite(mean) || !isfinite(mean_lo) || !isfinite(v_lb) || a_near_0) return 0ull;
     return key_nan_last(v_lb);
 }
 
 // One CTA per tile of PBN candidates: phase A without the K* stores, then (key, local index) per candidate; idx,
-// kmax_out (max_i |K*_i|, for b200bo_acq_prune_bound_dev) and mu_out (K* alpha_, which the refine stages reuse: it is
-// the epilogue's value bit for bit) may be nullptr.
+// kmax_out (max_i |K*_i|, for b200bo_acq_prune_bound_dev) and mu_out ((mu, mu) with mu = K* alpha_, the epilogue's
+// value bit for bit; the refine stages key with it) may be nullptr.
 template <bool DREG>
 __global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictParams P, unsigned long long* keys,
-                                                               int* idx, double* kmax_out, double* mu_out) {
+                                                               int* idx, double* kmax_out, double2* mu_out) {
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
     __shared__ double kmax_s[P16_SPLIT][PBN];
@@ -242,10 +246,213 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictPara
     if (c < PBN && c0 + c < P.m) {
         const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
         const double kmax = fmax(fmax(kmax_s[0][c], kmax_s[1][c]), fmax(kmax_s[2][c], kmax_s[3][c]));
-        keys[c0 + c] = prune_bound_key(P, G, mu_n, prune_var_ub(G, kmax * kmax / G.kdiag));
+        keys[c0 + c] = prune_bound_key(P, G, mu_n, mu_n, prune_var_ub(G, kmax * kmax / G.kdiag));
         if (idx) idx[c0 + c] = (int)(c0 + c);
-        if (mu_out) mu_out[c0 + c] = mu_n;
+        if (mu_out) mu_out[c0 + c] = make_double2(mu_n, mu_n);
         if (kmax_out) kmax_out[c0 + c] = kmax;
+    }
+}
+
+// ---- selection-only pruning: the Gram bound pass (DESIGN.md 4.9) ----------------------------------------------------
+// The direct pass spends about 40 % (d = 16) to 55 % (d = 32) of its fp64 instructions per (candidate, training row)
+// pair on the distance.  Here the distance comes from the fp64 tensor pipe in the Gram form
+//   r~^2 = [x, |x|^2, 1] . [-2y, 1, |y|^2]     (x = candidate / ls, y = Xs_i; K = d + 2 terms)
+// as one m16n8k4 f64 GEMM per tile, and the covariance, the mu sum and the |k| max are all that is left on the CUDA
+// cores.  The Gram form cancels (DESIGN.md 7), so mu and max |k| come out as intervals around the exact path's values:
+//   r^2      Every DMMA product-add is assumed IEEE-rounded, in any order (tests/test_gpu_prune_gram.py checks the
+//            device's r~^2 against this bound).  With S = |x|^2 + Ymax from the rounded norms, u = 2^-53 and
+//            g_n = n u / (1 - n u):  Gram sum <= g_K sum|a_k b_k| <= 2 g_K S (1 + g_d),  rounded norms <= g_d S,
+//            and phase A's direct sum of squared differences (the value compared against) <= (g_d + 2u) 2 S, so
+//            |r~^2 - r^2_direct| <= 5 g_{d+2} S (1 + O(g)) <= kGramCg g_{d+2} S = dr2.
+//   k        |dk/d(r^2)| <= Lip (Matern-2.5: 5/6, Matern-1.5: 3/2, RBF: 1/2 - plus e^{dr2/2} for r~^2 < 0, inside the
+//            slack below; Matern-0.5 is unbounded at r = 0 and keeps the direct pass).  cov_eval is within
+//            4 (1 + k) ulp of the formula (common.cuh), under 8 u for RBF, 12 u for Matern-1.5, 15 u for Matern-2.5
+//            in absolute terms, so both evaluations and the product with constv stay under kGramCcov u:
+//            dk = constv (Lip dr2 + kGramCcov u) bounds |k~_i - k_i| for every row i.
+//   mu       |mu~ - mu| <= A1 dk + (rounding of both sums, any order of np terms: 2 g_np A1 constv, and the final
+//            product with constv) <= A1 (dk + 3 g_np constv) (1 + 2^-20) = dmu, the last factor for the rounding of A1.
+//   max |k|  max_i |k_i| >= constv max_i k~_i - dk = kmax_lb.
+// mu_lo / mu_hi and kmax_lb are rounded outward (directed rounding).  With these, prune_bound_key and prune_var_ub
+// give a key no larger than the direct pass's, so the same candidates can be pruned, less a few near the k-th key.
+constexpr double kGramCg = 6.0, kGramCcov = 64.0;
+
+// row stride (doubles) of the Gram operands: K = d + 2 rounded up to the k-step 4, then to an odd multiple of 4, so
+// that the 8 rows x 4 k-columns of a fragment load fall on distinct banks within each half-warp
+__host__ __device__ inline int gram_stride(int d) {
+    const int k = (d + 2 + 3) / 4 * 4;
+    return (k / 4) & 1 ? k : k + 4;
+}
+
+// training-side operand, once per fit: row i < n = [-2 Xs_i | 1 | |Xs_i|^2 | 0 ...], zero rows for i >= n
+__global__ void __launch_bounds__(256) gram_operand_kernel(const double* __restrict__ Xs, int n, int np, int d,
+                                                           double* __restrict__ img) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= np) return;
+    const int str = gram_stride(d);
+    double* row = img + (size_t)i * str;
+    double y2 = 0.0;
+    for (int j = 0; j < d; ++j) {
+        const double v = Xs[(size_t)i * d + j];
+        y2 = fma(v, v, y2);
+        row[j] = i < n ? -2.0 * v : 0.0;
+    }
+    for (int j = d; j < str; ++j) row[j] = 0.0;
+    if (i < n) {
+        row[d] = 1.0;
+        row[d + 1] = y2;
+    }
+}
+
+// A1 = sum_i |alpha_i| and Ymax = max_i |Xs_i|^2 (i < n) behind the operand image; one CTA, fixed order
+__global__ void __launch_bounds__(1024) gram_stats_kernel(const double* __restrict__ alphav, int n, int d,
+                                                          double* __restrict__ img, double* __restrict__ stats) {
+    __shared__ double sa[1024], sy[1024];
+    const int t = threadIdx.x, str = gram_stride(d);
+    double a = 0.0, y = 0.0;
+    for (int i = t; i < n; i += 1024) {
+        a += fabs(alphav[i]);
+        y = fmax(y, img[(size_t)i * str + d + 1]);
+    }
+    sa[t] = a;
+    sy[t] = y;
+    __syncthreads();
+    for (int s = 512; s > 0; s >>= 1) {
+        if (t < s) {
+            sa[t] += sa[t + s];
+            sy[t] = fmax(sy[t], sy[t + s]);
+        }
+        __syncthreads();
+    }
+    if (t == 0) {
+        stats[0] = sa[0];
+        stats[1] = sy[0];
+    }
+}
+
+// One CTA per tile of PBN candidates.  Warp w owns candidates (w & 3) * 32 .. +32 and rows (w >> 2) * 16 .. +16 of
+// every PA_CHUNK-row chunk: 2 x 2 m16n8k4 tiles (m: candidates, n: training rows) over ceil(K / 4) k-steps.  Thread
+// (g, t4) accumulates candidates i * 8 + g (i < 4) of its warp over rows 2 t4, 2 t4 + 1 (+ 8) of its slab; the partials
+// are added over the quad, then over the four row slabs in a fixed order.  Outputs as predict_bound_kernel's;
+// mu_out gets (mu_lo, mu_hi) and kmax_out kmax_lb.
+template <int COV>
+__global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const PredictParams P, unsigned long long* keys,
+                                                                    int* idx, double* kmax_out, double2* mu_out) {
+    static_assert(COV != 0, "Matern-0.5 has no Lipschitz bound in r^2");
+    constexpr double lip = COV == 1 ? 1.5 : COV == 2 ? 5.0 / 6.0 : 0.5;
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[4][PBN];
+    __shared__ double kmax_s[4][PBN];
+    const GpDev& G = P.gp[0];
+    const int tid = threadIdx.x, d = P.d, str = gram_stride(d), nks = (d + 2 + 3) / 4;
+    const long long c0 = (long long)blockIdx.x * PBN;
+    double* xa_s = smem;                          // [PBN][str]: [x | |x|^2 | 1 | 0 ...]
+    double* xb_s = smem + (size_t)PBN * str;      // [2][PA_CHUNK][str]
+    double* al_s = xb_s + (size_t)2 * PA_CHUNK * str;  // [2][PA_CHUNK]
+    for (int q = tid; q < PBN * str; q += P16_NT) {
+        const int c = q / str, j = q - c * str;
+        const long long gi = c0 + c;
+        double v = j == d + 1 ? 1.0 : 0.0;
+        if (j < d && gi < P.m) {  // the coordinates phase A builds
+            v = candidate_coord(P, gi, j);
+            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
+            v = v / G.ls[j];
+        }
+        xa_s[q] = v;
+    }
+    auto load_chunk = [&](int buf, int ch) {
+        const double* src = G.gram + (size_t)ch * PA_CHUNK * str;
+        double* dst = xb_s + (size_t)buf * PA_CHUNK * str;
+        for (int q = tid; q < PA_CHUNK * str / 2; q += P16_NT) cp_async16_cg(dst + 2 * q, src + 2 * q);
+        if (tid < PA_CHUNK / 2)
+            cp_async16_cg(al_s + buf * PA_CHUNK + 2 * tid, G.alphav + (size_t)ch * PA_CHUNK + 2 * tid);
+    };
+    const int nch = G.np / PA_CHUNK;
+    load_chunk(0, 0);
+    cp_async_commit();
+    __syncthreads();  // coordinates visible
+    if (tid < PBN) {
+        double x2 = 0.0;
+        for (int j = 0; j < d; ++j) x2 = fma(xa_s[tid * str + j], xa_s[tid * str + j], x2);
+        xa_s[tid * str + d] = x2;
+    }
+    const int lane = tid & 31, warp = tid >> 5, g = lane >> 2, t4 = lane & 3;
+    const int cg = warp & 3, rg = warp >> 2;
+    const double* xa = xa_s + (size_t)(cg * 32 + g) * str + t4;
+    double macc[4], kmx[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) macc[i] = kmx[i] = 0.0;
+    for (int ch = 0; ch < nch; ++ch) {
+        if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();  // chunk ch (and, at ch = 0, the norms |x|^2) visible
+        const double* xb = xb_s + (size_t)(ch & 1) * PA_CHUNK * str + (size_t)(rg * 16 + g) * str + t4;
+        const double* al = al_s + (ch & 1) * PA_CHUNK + rg * 16 + 2 * t4;
+        double acc[2][2][4];
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) acc[mi][ni][e] = 0.0;
+        for (int ks = 0; ks < nks; ++ks) {
+            double a[4], b[2];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) a[i] = xa[(size_t)i * 8 * str + 4 * ks];
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni) b[ni] = xb[(size_t)ni * 8 * str + 4 * ks];
+#pragma unroll
+            for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                for (int ni = 0; ni < 2; ++ni)
+                    dmma1684(acc[mi][ni][0], acc[mi][ni][1], acc[mi][ni][2], acc[mi][ni][3], a[2 * mi],
+                             a[2 * mi + 1], b[ni]);
+        }
+        // acc[mi][ni][e]: candidate (2 mi + (e >> 1)) * 8 + g, row ni * 8 + 2 t4 + (e & 1) of the slab
+        const int row0 = ch * PA_CHUNK + rg * 16 + 2 * t4;
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
+                    double k = cov_eval<COV>(acc[mi][ni][e]);
+                    if (row0 + r >= G.n) k = 0.0;
+                    macc[i] = fma(al[r], k, macc[i]);
+                    kmx[i] = fmax(kmx[i], k);
+                }
+        __syncthreads();  // chunk buffer free for the prefetch of chunk ch+2
+    }
+    cp_async_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        macc[i] += __shfl_xor_sync(0xffffffffu, macc[i], 1);
+        macc[i] += __shfl_xor_sync(0xffffffffu, macc[i], 2);
+        kmx[i] = fmax(kmx[i], __shfl_xor_sync(0xffffffffu, kmx[i], 1));
+        kmx[i] = fmax(kmx[i], __shfl_xor_sync(0xffffffffu, kmx[i], 2));
+        if (t4 == 0) {
+            mu_s[rg][cg * 32 + i * 8 + g] = macc[i];
+            kmax_s[rg][cg * 32 + i * 8 + g] = kmx[i];
+        }
+    }
+    __syncthreads();
+    const int c = tid;
+    if (c < PBN && c0 + c < P.m) {
+        const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax
+        const double u = 0x1p-53;
+        const double gk = (d + 2) * u / (1.0 - (d + 2) * u), gn = G.np * u / (1.0 - G.np * u);
+        const double dr2 = __dmul_ru(kGramCg * gk, __dadd_ru(xa_s[c * str + d], stats[1]));
+        const double dk = __dmul_ru(G.constv, __fma_ru(lip, dr2, kGramCcov * u));
+        const double dmu = __dmul_ru(__dmul_ru(stats[0], 1.0 + 0x1p-20), __fma_ru(3.0 * gn, G.constv, dk));
+        const double mu = G.constv * (((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c]);
+        const double kt = fmax(fmax(kmax_s[0][c], kmax_s[1][c]), fmax(kmax_s[2][c], kmax_s[3][c]));
+        const double mu_lo = __dsub_rd(mu, dmu), mu_hi = __dadd_ru(mu, dmu);
+        const double kmax_lb = fmax(0.0, __dsub_rd(__dmul_rd(G.constv, kt), dk));
+        keys[c0 + c] = prune_bound_key(P, G, mu_lo, mu_hi, prune_var_ub(G, kmax_lb * kmax_lb / G.kdiag));
+        if (idx) idx[c0 + c] = (int)(c0 + c);
+        if (mu_out) mu_out[c0 + c] = make_double2(mu_lo, mu_hi);
+        if (kmax_out) kmax_out[c0 + c] = kmax_lb;
     }
 }
 
@@ -711,14 +918,16 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
 // When more than kRefineMaxTiles tiles of survivors come up (little prunes: the refine stage stops claiming tiles as
 // soon as it sees that), the final stage does nothing and the tile kernel goes on in bound order behind the lead
 // tiles as it would have without these stages; otherwise the final stage closes the tile kernel's counter.
-// Exact values are bit-equal to the tile kernel's: K* entries carry no order, mu is the bound pass's (stored), and the
-// sum of squares is added up by unit_finish_colsq in the order of predict16_phase_b.  No CTA waits for another: the
+// Exact values are bit-equal to the tile kernel's: K* entries carry no order, mu comes from the unit that runs phase A
+// over all np rows (the last group of a tile; the same function and order of sums as the tile kernel), and the sum of
+// squares is added up by unit_finish_colsq in the order of predict16_phase_b.  No CTA waits for another: the
 // stages are kernel boundaries, and within predict_units_kernel the last unit to arrive at a tile's counter finishes it.
 constexpr int kLeadTiles = 8, kRefineMaxTiles = 128, kUnitSlots = kLeadTiles + kRefineMaxTiles;
 constexpr long long kCtlClosed = 1ll << 40;  // value of kCtlTile no batch reaches
 
 struct RefineParams {
-    const double* mu_n;      // [m] K* alpha_ per candidate (local index), from the bound pass
+    const double2* mu;       // [m] interval (mu_lo, mu_hi) of K* alpha_ per candidate (local index), from the bound pass
+    double* mu_unit;         // [kUnitSlots][PBN] K* alpha_ of a tile's candidates, from its last group's phase A
     int* surv;               // [kRefineMaxTiles * PBN] local indices the refine stage let through
     double* part;            // [kUnitSlots][np / PBM][4][8][PBN] per-row-block partial sums of squares
     unsigned* arrive;        // [kUnitSlots] units that have delivered their part of a tile
@@ -784,7 +993,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
         if (tid < PBN && c0 + tid < P.m) {
             const int c = tid, li = P.perm[c0 + c];
             const double r = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
-            const unsigned long long key = prune_bound_key(P, G, R.mu_n[li], prune_var_ub(G, r));
+            const double2 mu = R.mu[li];
+            const unsigned long long key = prune_bound_key(P, G, mu.x, mu.y, prune_var_ub(G, r));
             if (key <= kth && P.perm_key[c0 + c] <= kth) {
                 const unsigned long long pos = atomicAdd(P.prune_ctl + kCtlSurv, 1ull);
                 if (pos < (unsigned long long)kRefineMaxTiles * PBN) R.surv[pos] = li;
@@ -846,8 +1056,11 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
         if (ib1 > ib0) {
             predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
             predict16_phase_b<1684, true>(G, Ks, smem, pol_last, pol_first, ib0, ib1, part);
+            if (ib1 == nb && tid < PBN)  // phase A ran over all np rows: mu_s holds the tile kernel's K* alpha_ sums
+                R.mu_unit[(size_t)(slot0 + tile) * PBN + tid] =
+                    ((mu_s[0][tid] + mu_s[1][tid]) + mu_s[2][tid]) + mu_s[3][tid];
         }
-        __threadfence();  // this unit's partials before its arrival
+        __threadfence();  // this unit's partials and mu before its arrival
         __syncthreads();
         if (tid == 0) last_s = atomicAdd(R.arrive + slot0 + tile, 1u) == (unsigned)groups - 1;
         __syncthreads();
@@ -862,7 +1075,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
                 const long long gi = valid ? (long long)list[c0 + c] : P.m;
                 const double colsq = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
                 double val = 0.0, base, prod;
-                candidate_epilogue(P, G, 0, valid ? R.mu_n[gi] : 0.0, colsq, gi, base, prod, &val);
+                const double mu_n = valid ? __ldcg(R.mu_unit + (size_t)(slot0 + tile) * PBN + c) : 0.0;
+                candidate_epilogue(P, G, 0, mu_n, colsq, gi, base, prod, &val);
                 runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, valid);
                 if (tid == 0) {
                     if (sel_s.list.idx[P.sel_k - 1] != SEL_NOIDX)

@@ -35,6 +35,8 @@ struct GpDev {
     const int* xform;      // [d] or nullptr
     const uint8_t* linv_tc;  // fp32 mode: L^-1 as tf32 (hi,lo) wgmma operand images, or nullptr
     const double* linv_pad;  // bulk-copy phase B of predict_acq16_kernel: L^-1 as padded stage images, or nullptr
+    // Gram bound pass of pruning: [np][gram_stride(d)] training operand, then A1 and Ymax (predict16.cuh), or nullptr
+    const double* gram;
     int n, np, family, nu;
     double constv, y_mean, y_std, lb, ub;
     double prior;  // prior variance kernel_.diag(x*) = constv + WhiteKernel noise_level

@@ -444,12 +444,19 @@ int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total);
  * on the stop event; nothing is read back unless this is called. */
 int b200bo_last_prune_stage_ms(float ms[6], int64_t* refined);
 
-/* The bound pass of selection-only pruning alone (EI, UCB or PoI on one GP; 1 <= m <= INT_MAX device rows d_Xc):
+/* The direct bound pass of selection-only pruning alone (the one the selection runs for Matern-0.5; EI, UCB, PoI,
+ * LogEI or LogPoI on one GP; 1 <= m <= INT_MAX device rows d_Xc):
  * d_key[i] = the order key (key_nan_last of select.cuh) of a lower bound on candidate i's closure value -acq, 0 for a
  * candidate that is never pruned; d_kmax[i] (nullable) = max_j |k(x_i, X_j)| in normalised units.  Enqueued on
  * `stream`, not synchronised.  For checking the bound against exact values. */
 int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key, double* d_kmax,
                                void* stream);
+/* The Gram bound pass of pruning (distances on the fp64 tensor pipe, DESIGN.md 4.9), as the selection uses it for
+ * every covariance but Matern-0.5: per candidate a key no larger than the key of its exact value, the interval
+ * d_mu[2i], d_mu[2i+1] (nullable, normalised units) that holds its exact K* alpha_, and d_kmax_lb (nullable) <= its
+ * max_i |K*_i|.  B200BO_ERR_UNSUPPORTED for Matern-0.5. */
+int b200bo_acq_prune_bound_gram_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
+                                    double* d_mu, double* d_kmax_lb, void* stream);
 
 #ifdef __cplusplus
 }
