@@ -27,7 +27,8 @@ EXPORTS = [
     "b200bo_gp_set_data", "b200bo_gp_append", "b200bo_gp_lml", "b200bo_gp_get", "b200bo_gp_n", "b200bo_gp_dim",
     "b200bo_gp_predict", "b200bo_gp_predict_cov", "b200bo_acq_eval", "b200bo_acq_argmin_topk", "b200bo_acq_eval_dev",
     "b200bo_last_kernel_ms", "b200bo_last_prune_stats", "b200bo_last_prune_stage_ms", "b200bo_acq_prune_bound_dev",
-    "b200bo_acq_prune_bound_gram_dev",
+    "b200bo_acq_prune_bound_gram_dev", "b200bo_acq_prune_bound_gram32_dev", "b200bo_acq_prune_bound_pass",
+    "b200bo_cov_f32_dev",
     "b200bo_acq_argmin_topk_philox", "b200bo_acq_select_philox_dev", "b200bo_philox_rows",
     "b200bo_gp_replicate", "b200bo_multi_gpu_acq_argmin_topk", "b200bo_multi_gpu_acq_argmin_topk_philox",
     "b200bo_multi_gpu_acq_eval",
@@ -114,6 +115,10 @@ def lib():
                                              C.c_void_p]
     L.b200bo_acq_prune_bound_gram_dev.argtypes = [C.POINTER(AcqSpec), C.c_void_p, C.c_int64, C.c_void_p,
                                                   C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b200bo_acq_prune_bound_gram32_dev.argtypes = [C.POINTER(AcqSpec), C.c_void_p, C.c_int64, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b200bo_acq_prune_bound_pass.argtypes = [C.POINTER(AcqSpec), C.POINTER(C.c_int), C.c_void_p]
+    L.b200bo_cov_f32_dev.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
     philox_outs = [dp, i64p, dp, dp, i64p, dp]
     L.b200bo_acq_argmin_topk_philox.argtypes = [C.POINTER(AcqSpec), C.c_uint64, dp, dp, C.c_int64, C.c_int64,
                                                 C.c_int, *philox_outs]

@@ -156,9 +156,11 @@ struct b200bo_gp {
     // bulk-copy phase B of the fp64 kernel: L^-1 as padded stage images (built on first use after a fit)
     DevBuf pad_linv;
     bool pad_valid = false;
-    // Gram bound pass of pruning: the training-side operand, A1 and Ymax (built on first use after a fit)
+    // Gram bound pass of pruning: the training-side operand, A1 and Ymax, alpha_ in fp32 (built on first use after a
+    // fit), and the host copy of A1 the choice between the fp64 and the fp32 pass reads
     DevBuf gram;
     bool gram_valid = false;
+    double gram_a1 = 0.0;
     DevBuf cov_xc, cov_kst, cov_v, cov_c, cov_out, cov_mu;  // predict(return_cov=True) scratch
     DevBuf sel_cta;         // per-CTA running selection lists of the fused kernels
     // selection-only pruning: bound keys / local indices (two buffers each for the radix sort), its temp storage and
@@ -279,9 +281,12 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_units_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -1468,39 +1473,72 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     return B200BO_OK;
 }
 
-// Gram bound pass operand of pruning (once per fit)
+// Gram bound pass operand of pruning (once per fit): [np][stride] doubles, A1, Ymax, then np floats (alpha_).  A1 is
+// read back (one synchronisation per fit) for the choice of pass.
 static int ensure_gram(b200bo_gp* gp, cudaStream_t stream) {
     if (gp->gram_valid) return B200BO_OK;
     const int np = gp->np, d = gp->d;
     int rc;
-    if ((rc = gp->gram.reserve(sizeof(double) * ((size_t)np * gram_stride(d) + 2)))) return rc;
+    if ((rc = gp->gram.reserve(sizeof(double) * ((size_t)np * gram_stride(d) + 2) + sizeof(float) * np))) return rc;
     double* img = gp->gram.as<double>();
-    gram_operand_kernel<<<(np + 255) / 256, 256, 0, stream>>>(gp->Xs.as<double>(), (int)gp->n, np, d, img);
+    gram_operand_kernel<<<(np + 255) / 256, 256, 0, stream>>>(gp->Xs.as<double>(), gp->alphav.as<double>(),
+                                                              (int)gp->n, np, d, img);
     LAUNCHED();
     gram_stats_kernel<<<1, 1024, 0, stream>>>(gp->alphav.as<double>(), (int)gp->n, d, img,
                                               img + (size_t)np * gram_stride(d));
     LAUNCHED();
     CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&gp->gram_a1, img + (size_t)np * gram_stride(d), sizeof(double), cudaMemcpyDeviceToHost,
+                       stream));
+    CU(cudaStreamSynchronize(stream));
     gp->gram_valid = true;
     return B200BO_OK;
 }
 
-// The bound pass of a pruned launch: the Gram pass (distances on the fp64 tensor pipe) for every covariance whose
-// dk/d(r^2) is bounded, the direct pass for Matern-0.5 (DESIGN.md 4.9).  mu: [m] interval (mu_lo, mu_hi); idx, kmax
-// may be nullptr.
-static int launch_bound_pass(b200bo_gp* g0, PredictParams& P, bool gram, unsigned long long* keys, int* idx,
+// The bound passes of pruning (DESIGN.md 4.9)
+enum { kBoundDirect = 0, kBoundGram64 = 1, kBoundGram32 = 2 };
+
+// The fp32 Gram pass widens mu by about A1 constv 2^-24 times a few tens (the covariance's rounding, summed with the
+// weights |alpha_i|); the fp64 Gram pass by about A1 constv 2^-53 (DESIGN.md 4.9).  Above A1 constv 2^-24 = 1e-3
+// (normalised units) the fp32 interval starts to let candidates through that the fp64 one prunes, so such GPs (large
+// alpha_ on an ill-conditioned K) keep the fp64 pass.  B200BO_PRUNE_BOUND=f64 / f32 (read per call) forces one of the
+// Gram passes for A/B measurements; Matern-0.5 always runs the direct pass.  Needs ensure_gram.
+constexpr double kPruneF32MaxMargin = 1e-3;
+static int bound_pass_choice(const b200bo_gp* g0, const GpDev& G) {
+    if (cov_code(G.family, G.nu) == 0) return kBoundDirect;
+    const char* e = getenv("B200BO_PRUNE_BOUND");
+    if (e && !strcmp(e, "f64")) return kBoundGram64;
+    if (e && !strcmp(e, "f32")) return kBoundGram32;
+    return g0->gram_a1 * G.constv * 0x1p-24 <= kPruneF32MaxMargin ? kBoundGram32 : kBoundGram64;
+}
+
+template <bool F32>
+static void launch_bound_gram(const PredictParams& P, unsigned ntiles, size_t smem, unsigned long long* keys,
+                              int* idx, double* kmax, double2* mu, cudaStream_t stream) {
+    switch (cov_code(P.gp[0].family, P.gp[0].nu)) {
+        case 1: predict_bound_gram_kernel<1, F32><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        case 2: predict_bound_gram_kernel<2, F32><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        default: predict_bound_gram_kernel<3, F32><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+    }
+}
+
+// The bound pass of a pruned launch (kBound*; -1: bound_pass_choice): a Gram pass (distances on the fp64 tensor pipe)
+// for every covariance whose dk/d(r^2) is bounded, the direct pass for Matern-0.5 (DESIGN.md 4.9).  mu: [m] interval
+// (mu_lo, mu_hi); idx, kmax may be nullptr.
+static int launch_bound_pass(b200bo_gp* g0, PredictParams& P, int pass, unsigned long long* keys, int* idx,
                              double* kmax, double2* mu, cudaStream_t stream) {
     const unsigned ntiles = (unsigned)((P.m + PBN - 1) / PBN);
-    if (gram) {
+    if (cov_code(P.gp[0].family, P.gp[0].nu) == 0) pass = kBoundDirect;
+    if (pass != kBoundDirect) {
         int rc;
         if ((rc = ensure_gram(g0, stream))) return rc;
+        if (pass < 0) pass = bound_pass_choice(g0, P.gp[0]);
         P.gp[0].gram = g0->gram.as<double>();
         const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * gram_stride(P.d) + 2 * PA_CHUNK);
-        switch (cov_code(P.gp[0].family, P.gp[0].nu)) {
-            case 1: predict_bound_gram_kernel<1><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
-            case 2: predict_bound_gram_kernel<2><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
-            default: predict_bound_gram_kernel<3><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
-        }
+        if (pass == kBoundGram32)
+            launch_bound_gram<true>(P, ntiles, smem, keys, idx, kmax, mu, stream);
+        else
+            launch_bound_gram<false>(P, ntiles, smem, keys, idx, kmax, mu, stream);
     } else {
         const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
         if (P.d <= kPredictMaxDimRegs)
@@ -1530,7 +1568,7 @@ static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool resume, cudaStrea
         if ((rc = ensure_gram(g0, stream))) return rc;
         CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off operand build from the kernel time
     }
-    if ((rc = launch_bound_pass(g0, P, gram, keys, idx, nullptr, g0->prune_mu.as<double2>(), stream))) return rc;
+    if ((rc = launch_bound_pass(g0, P, -1, keys, idx, nullptr, g0->prune_mu.as<double2>(), stream))) return rc;
     CU(cudaEventRecord(g0->ev_stage[0], stream));
     cub::DoubleBuffer<unsigned long long> kb(keys, keys + m);
     cub::DoubleBuffer<int> ib(idx, idx + m);
@@ -1952,9 +1990,10 @@ extern "C" int b200bo_acq_eval_dev(const b200bo_acq* spec, const double* d_Xc, i
     return eval_core(spec, src, m, d_acq_neg, d_mu, d_sd, k, d_sel, index_base, (cudaStream_t)stream_);
 }
 
-// the bound pass alone, direct (gram = false) or Gram; d_mu (Gram only): [m][2] (mu_lo, mu_hi)
+// the bound pass alone (kBound*); d_mu (Gram only): [m][2] (mu_lo, mu_hi)
 static int prune_bound_entry(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key, double* d_kmax,
-                             double* d_mu, bool gram, void* stream_) {
+                             double* d_mu, int pass, void* stream_) {
+    const bool gram = pass != kBoundDirect;
     int rc;
     if ((rc = check_spec(spec))) return rc;
     if (spec->n_gps != 1 || !acq_prunable(spec->kind))
@@ -1971,18 +2010,63 @@ static int prune_bound_entry(const b200bo_acq* spec, const double* d_Xc, int64_t
     PredictParams P;
     int np_max = 0;
     if ((rc = fill_params(spec, src, m, 0, stream, P, np_max))) return rc;
-    return launch_bound_pass(g0, P, gram, reinterpret_cast<unsigned long long*>(d_key), nullptr, d_kmax,
+    return launch_bound_pass(g0, P, pass, reinterpret_cast<unsigned long long*>(d_key), nullptr, d_kmax,
                              reinterpret_cast<double2*>(d_mu), stream);
 }
 
 extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
                                           double* d_kmax, void* stream_) {
-    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax, nullptr, false, stream_);
+    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax, nullptr, kBoundDirect, stream_);
 }
 
 extern "C" int b200bo_acq_prune_bound_gram_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
                                                double* d_mu, double* d_kmax_lb, void* stream_) {
-    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax_lb, d_mu, true, stream_);
+    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax_lb, d_mu, kBoundGram64, stream_);
+}
+
+extern "C" int b200bo_acq_prune_bound_gram32_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m,
+                                                 uint64_t* d_key, double* d_mu, double* d_kmax_lb, void* stream_) {
+    return prune_bound_entry(spec, d_Xc, m, d_key, d_kmax_lb, d_mu, kBoundGram32, stream_);
+}
+
+extern "C" int b200bo_acq_prune_bound_pass(const b200bo_acq* spec, int* pass, void* stream_) {
+    int rc;
+    if ((rc = check_spec(spec))) return rc;
+    if (spec->n_gps != 1 || !pass) return set_err(B200BO_ERR_ARG, "one GP and a result pointer");
+    b200bo_gp* g0 = spec->gps[0];
+    CU(cudaSetDevice(g0->device));
+    if (cov_code(g0->family, g0->nu) != 0 && (rc = ensure_gram(g0, (cudaStream_t)stream_))) return rc;
+    GpDev G;
+    G.family = g0->family;
+    G.nu = g0->nu;
+    G.constv = g0->constv;
+    *pass = bound_pass_choice(g0, G);
+    return B200BO_OK;
+}
+
+// the fp32 covariance of the fp32 Gram pass on n fp32 arguments (tests)
+template <int COV>
+__global__ void cov_f32_kernel(const float* __restrict__ s, int64_t n, float* __restrict__ k, float* __restrict__ z) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float zi;
+        k[i] = cov_f32<COV>((double)s[i], zi);
+        if (z) z[i] = zi;
+    }
+}
+
+extern "C" int b200bo_cov_f32_dev(int family, int nu, const float* d_s, int64_t n, float* d_k, float* d_z,
+                                  void* stream_) {
+    const int cov = cov_code(family, nu);
+    if (cov == 0) return set_err(B200BO_ERR_UNSUPPORTED, "Matern-0.5 has no fp32 Gram pass");
+    if (n <= 0 || !d_s || !d_k) return set_err(B200BO_ERR_ARG, "bad arguments");
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 132 * 16);
+    if (cov == 1) cov_f32_kernel<1><<<grid, 256, 0, stream>>>(d_s, n, d_k, d_z);
+    else if (cov == 2) cov_f32_kernel<2><<<grid, 256, 0, stream>>>(d_s, n, d_k, d_z);
+    else cov_f32_kernel<3><<<grid, 256, 0, stream>>>(d_s, n, d_k, d_z);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    return B200BO_OK;
 }
 
 extern "C" int b200bo_acq_select_philox_dev(const b200bo_acq* spec, uint64_t seed, const double* lo,

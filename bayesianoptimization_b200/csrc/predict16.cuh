@@ -283,12 +283,57 @@ __host__ __device__ inline int gram_stride(int d) {
     return (k / 4) & 1 ? k : k + 4;
 }
 
-// training-side operand, once per fit: row i < n = [-2 Xs_i | 1 | |Xs_i|^2 | 0 ...], zero rows for i >= n
-__global__ void __launch_bounds__(256) gram_operand_kernel(const double* __restrict__ Xs, int n, int np, int d,
-                                                           double* __restrict__ img) {
+// ---- the fp32 covariance of the Gram bound pass (predict_bound_gram_kernel<COV, true>) ------------------------------
+// r~^2 is rounded to fp32 and clamped to [2^-100, kF32R2Max]: above the clamp the exp argument would leave the normal
+// range (2^-126), and the covariance there is below 1.2e-33 (Matern-2.5 at 1400, Matern-1.5 at 2300, RBF at 166),
+// inside the absolute part of the margin; below it rsqrtf stays finite.  sqrt and exp are one rsqrtf and one exp2f
+// (each within 2 ulp, CUDA C++ Programming Guide, single-precision mathematical functions), the rest is FMA-pipe work:
+//   Matern-2.5: z = sqrt5 r,  k = (1 + z + z^2/3) 2^(-sqrt5 log2e r);   Matern-1.5: z = sqrt3 r, k = (1 + z) 2^(...);
+//   RBF: z = s / 2, k = 2^(-log2e s / 2).
+// Error against the formula at the exact r~^2 (u = 2^-24; first order, every constant and product rounded):
+//   r = s rsqrtf(s) is within 5 u, z and the exp argument within 7 u, plus 1/2 u from the rounding of r~^2 to s;
+//   the exp argument's error x is a relative error z x of 2^(...), so it grows with z; the Matern polynomial (positive
+//   terms) is within 2 x 7.5 u + 3 u, exp2f within 4 u, the last product u.  Per row, with z~ from the pass,
+//     |k~ - k| <= u k~ (R + Q z~) + (clamps: < 1e-30),
+//   R = 23, 14.5, 5 and Q = 7.5, 7.5, 3 (Matern-2.5, Matern-1.5, RBF) - the constants below leave headroom and add the
+//   fp32 mu partial of the kernel (alpha_ rounded to fp32, four fused products: 6 u relative to sum |alpha_ k~|).
+//   tests/test_prune_f32_cpu.py restates this with rsqrtf and exp2f perturbed to their documented error and
+//   tests/test_gpu_prune_f32.py checks the device function exhaustively over its fp32 arguments.
+template <int COV>
+struct CovF32 {
+    static constexpr float r2max = COV == 1 ? 2300.f : COV == 2 ? 1400.f : 166.f;
+    static constexpr float rel = COV == 1 ? 24.f : COV == 2 ? 32.f : 12.f;  // R, the mu partial included
+    static constexpr float qz = COV == 3 ? 4.f : 8.f;                       // Q
+};
+constexpr double kF32Abs = 1e-30;  // the clamps, per unit covariance
+
+// k~ of one pair from r~^2 (fp64); z: the exp argument's magnitude (natural units)
+template <int COV>
+__device__ __forceinline__ float cov_f32(double r2, float& z) {
+    const float s = fminf(fmaxf(__double2float_rn(r2), 0x1p-100f), CovF32<COV>::r2max);
+    if (COV == 3) {
+        z = 0.5f * s;
+        return exp2f(s * -0.72134751081466674805f);  // -log2e / 2
+    }
+    const float r = s * rsqrtf(s);
+    if (COV == 2) {
+        z = r * 2.23606801033020019531f;                  // sqrt5
+        const float e = exp2f(r * -3.22596406936645507812f);  // -sqrt5 log2e
+        return fmaf(fmaf(z, 0.33333334326744079590f, 1.f), z, 1.f) * e;
+    }
+    z = r * 1.73205077648162841797f;                  // sqrt3
+    const float e = exp2f(r * -2.49882102012634277344f);  // -sqrt3 log2e
+    return (1.f + z) * e;
+}
+
+// training-side operand, once per fit: row i < n = [-2 Xs_i | 1 | |Xs_i|^2 | 0 ...], zero rows for i >= n; alpha_ in
+// fp32 (0 for i >= n) behind A1 and Ymax, for the fp32 pass
+__global__ void __launch_bounds__(256) gram_operand_kernel(const double* __restrict__ Xs, const double* __restrict__ alphav,
+                                                           int n, int np, int d, double* __restrict__ img) {
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= np) return;
     const int str = gram_stride(d);
+    reinterpret_cast<float*>(img + (size_t)np * str + 2)[i] = i < n ? (float)alphav[i] : 0.f;
     double* row = img + (size_t)i * str;
     double y2 = 0.0;
     for (int j = 0; j < d; ++j) {
@@ -334,7 +379,13 @@ __global__ void __launch_bounds__(1024) gram_stats_kernel(const double* __restri
 // (g, t4) accumulates candidates i * 8 + g (i < 4) of its warp over rows 2 t4, 2 t4 + 1 (+ 8) of its slab; the partials
 // are added over the quad, then over the four row slabs in a fixed order.  Outputs as predict_bound_kernel's;
 // mu_out gets (mu_lo, mu_hi) and kmax_out kmax_lb.
-template <int COV>
+// F32: the covariance in fp32 (cov_f32).  Per thread and chunk the four alpha_ k~ products of a candidate are summed in
+// fp32 and then added to the fp64 partial; W = sum_i |alpha_i| k~_i (R + Q z~_i) (fp32) carries the relative part of
+// the margin, and the |k| maximum is taken over k~_i (1 - u (R + Q z~_i)), a lower bound of the row's exact k:
+//   dmu = constv (A1 (Lip dr2 + 64 u53 + kF32Abs + 3 g_np) + u W (1 + (np + 16) 2^-23)) (1 + 2^-20)
+//   kmax_lb = constv (max_i k~_i (1 - u (R + Q z~_i))) (1 - 2^-22) - constv (Lip dr2 + 64 u53 + kF32Abs)
+// (every fp32 sum of positive terms is within (np + 16) 2^-23 of its value; 2^-22 covers the rounding of the product).
+template <int COV, bool F32>
 __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const PredictParams P, unsigned long long* keys,
                                                                     int* idx, double* kmax_out, double2* mu_out) {
     static_assert(COV != 0, "Matern-0.5 has no Lipschitz bound in r^2");
@@ -342,12 +393,13 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[4][PBN];
     __shared__ double kmax_s[4][PBN];
+    __shared__ double w_s[F32 ? 4 : 1][PBN];
     const GpDev& G = P.gp[0];
     const int tid = threadIdx.x, d = P.d, str = gram_stride(d), nks = (d + 2 + 3) / 4;
     const long long c0 = (long long)blockIdx.x * PBN;
     double* xa_s = smem;                          // [PBN][str]: [x | |x|^2 | 1 | 0 ...]
     double* xb_s = smem + (size_t)PBN * str;      // [2][PA_CHUNK][str]
-    double* al_s = xb_s + (size_t)2 * PA_CHUNK * str;  // [2][PA_CHUNK]
+    double* al_s = xb_s + (size_t)2 * PA_CHUNK * str;  // [2][PA_CHUNK] (fp64), or [2][PA_CHUNK] floats (F32)
     for (int q = tid; q < PBN * str; q += P16_NT) {
         const int c = q / str, j = q - c * str;
         const long long gi = c0 + c;
@@ -359,12 +411,18 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
         }
         xa_s[q] = v;
     }
+    const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax, then alpha_ in fp32
     auto load_chunk = [&](int buf, int ch) {
         const double* src = G.gram + (size_t)ch * PA_CHUNK * str;
         double* dst = xb_s + (size_t)buf * PA_CHUNK * str;
         for (int q = tid; q < PA_CHUNK * str / 2; q += P16_NT) cp_async16_cg(dst + 2 * q, src + 2 * q);
-        if (tid < PA_CHUNK / 2)
+        if (F32) {
+            if (tid < PA_CHUNK / 4)
+                cp_async16_cg(reinterpret_cast<float*>(al_s) + buf * PA_CHUNK + 4 * tid,
+                              reinterpret_cast<const float*>(stats + 2) + (size_t)ch * PA_CHUNK + 4 * tid);
+        } else if (tid < PA_CHUNK / 2) {
             cp_async16_cg(al_s + buf * PA_CHUNK + 2 * tid, G.alphav + (size_t)ch * PA_CHUNK + 2 * tid);
+        }
     };
     const int nch = G.np / PA_CHUNK;
     load_chunk(0, 0);
@@ -379,8 +437,12 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
     const int cg = warp & 3, rg = warp >> 2;
     const double* xa = xa_s + (size_t)(cg * 32 + g) * str + t4;
     double macc[4], kmx[4];
+    float kmxf[4], wsum[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) macc[i] = kmx[i] = 0.0;
+    for (int i = 0; i < 4; ++i) {
+        macc[i] = kmx[i] = 0.0;
+        kmxf[i] = wsum[i] = 0.f;
+    }
     for (int ch = 0; ch < nch; ++ch) {
         if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
         cp_async_commit();
@@ -388,6 +450,7 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
         __syncthreads();  // chunk ch (and, at ch = 0, the norms |x|^2) visible
         const double* xb = xb_s + (size_t)(ch & 1) * PA_CHUNK * str + (size_t)(rg * 16 + g) * str + t4;
         const double* al = al_s + (ch & 1) * PA_CHUNK + rg * 16 + 2 * t4;
+        const float* alf = reinterpret_cast<const float*>(al_s) + (ch & 1) * PA_CHUNK + rg * 16 + 2 * t4;
         double acc[2][2][4];
 #pragma unroll
         for (int mi = 0; mi < 2; ++mi)
@@ -410,23 +473,50 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
         }
         // acc[mi][ni][e]: candidate (2 mi + (e >> 1)) * 8 + g, row ni * 8 + 2 t4 + (e & 1) of the slab
         const int row0 = ch * PA_CHUNK + rg * 16 + 2 * t4;
+        if constexpr (F32) {
+            float mp[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-        for (int mi = 0; mi < 2; ++mi)
+            for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-            for (int ni = 0; ni < 2; ++ni)
+                for (int ni = 0; ni < 2; ++ni)
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
-                    double k = cov_eval<COV>(acc[mi][ni][e]);
-                    if (row0 + r >= G.n) k = 0.0;
-                    macc[i] = fma(al[r], k, macc[i]);
-                    kmx[i] = fmax(kmx[i], k);
-                }
+                    for (int e = 0; e < 4; ++e) {
+                        const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
+                        float z;
+                        float k = cov_f32<COV>(acc[mi][ni][e], z);
+                        if (row0 + r >= G.n) k = 0.f;
+                        const float a = alf[r];
+                        const float w = fmaf(z, CovF32<COV>::qz, CovF32<COV>::rel);
+                        mp[i] = fmaf(a, k, mp[i]);
+                        wsum[i] = fmaf(fabsf(a) * k, w, wsum[i]);
+                        kmxf[i] = fmaxf(kmxf[i], fmaf(k * -0x1p-24f, w, k));
+                    }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) macc[i] += (double)mp[i];
+        } else {
+#pragma unroll
+            for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
+                        double k = cov_eval<COV>(acc[mi][ni][e]);
+                        if (row0 + r >= G.n) k = 0.0;
+                        macc[i] = fma(al[r], k, macc[i]);
+                        kmx[i] = fmax(kmx[i], k);
+                    }
+        }
         __syncthreads();  // chunk buffer free for the prefetch of chunk ch+2
     }
     cp_async_wait<0>();
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
+        if (F32) {
+            wsum[i] += __shfl_xor_sync(0xffffffffu, wsum[i], 1);
+            wsum[i] += __shfl_xor_sync(0xffffffffu, wsum[i], 2);
+            kmx[i] = (double)kmxf[i];
+        }
         macc[i] += __shfl_xor_sync(0xffffffffu, macc[i], 1);
         macc[i] += __shfl_xor_sync(0xffffffffu, macc[i], 2);
         kmx[i] = fmax(kmx[i], __shfl_xor_sync(0xffffffffu, kmx[i], 1));
@@ -434,21 +524,31 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
         if (t4 == 0) {
             mu_s[rg][cg * 32 + i * 8 + g] = macc[i];
             kmax_s[rg][cg * 32 + i * 8 + g] = kmx[i];
+            if (F32) w_s[rg][cg * 32 + i * 8 + g] = wsum[i];
         }
     }
     __syncthreads();
     const int c = tid;
     if (c < PBN && c0 + c < P.m) {
-        const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax
         const double u = 0x1p-53;
         const double gk = (d + 2) * u / (1.0 - (d + 2) * u), gn = G.np * u / (1.0 - G.np * u);
         const double dr2 = __dmul_ru(kGramCg * gk, __dadd_ru(xa_s[c * str + d], stats[1]));
-        const double dk = __dmul_ru(G.constv, __fma_ru(lip, dr2, kGramCcov * u));
-        const double dmu = __dmul_ru(__dmul_ru(stats[0], 1.0 + 0x1p-20), __fma_ru(3.0 * gn, G.constv, dk));
         const double mu = G.constv * (((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c]);
         const double kt = fmax(fmax(kmax_s[0][c], kmax_s[1][c]), fmax(kmax_s[2][c], kmax_s[3][c]));
+        double dmu, kmax_lb;
+        if constexpr (F32) {
+            const double dk1 = __fma_ru(lip, dr2, kGramCcov * u + kF32Abs);  // per unit covariance and row
+            const double w = __dadd_ru(__dadd_ru(w_s[0][c], w_s[1][c]), __dadd_ru(w_s[2][c], w_s[3][c]));
+            const double wr = __dmul_ru(__dmul_ru(w, 0x1p-24), 1.0 + (G.np + 16) * 0x1p-23);
+            dmu = __dmul_ru(__dmul_ru(G.constv, 1.0 + 0x1p-20),
+                            __fma_ru(stats[0], __dadd_ru(dk1, 3.0 * gn), wr));
+            kmax_lb = fmax(0.0, __dsub_rd(__dmul_rd(__dmul_rd(G.constv, kt), 1.0 - 0x1p-22), __dmul_ru(G.constv, dk1)));
+        } else {
+            const double dk = __dmul_ru(G.constv, __fma_ru(lip, dr2, kGramCcov * u));
+            dmu = __dmul_ru(__dmul_ru(stats[0], 1.0 + 0x1p-20), __fma_ru(3.0 * gn, G.constv, dk));
+            kmax_lb = fmax(0.0, __dsub_rd(__dmul_rd(G.constv, kt), dk));
+        }
         const double mu_lo = __dsub_rd(mu, dmu), mu_hi = __dadd_ru(mu, dmu);
-        const double kmax_lb = fmax(0.0, __dsub_rd(__dmul_rd(G.constv, kt), dk));
         keys[c0 + c] = prune_bound_key(P, G, mu_lo, mu_hi, prune_var_ub(G, kmax_lb * kmax_lb / G.kdiag));
         if (idx) idx[c0 + c] = (int)(c0 + c);
         if (mu_out) mu_out[c0 + c] = make_double2(mu_lo, mu_hi);

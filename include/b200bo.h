@@ -457,6 +457,16 @@ int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64
  * max_i |K*_i|.  B200BO_ERR_UNSUPPORTED for Matern-0.5. */
 int b200bo_acq_prune_bound_gram_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
                                     double* d_mu, double* d_kmax_lb, void* stream);
+/* The same with the covariance in fp32 (DESIGN.md 4.9): the same outputs and guarantees, with a wider mu interval.
+ * The selection runs it when A1 constv 2^-24 <= 1e-3 (A1 = sum |alpha_|), see b200bo_acq_prune_bound_pass. */
+int b200bo_acq_prune_bound_gram32_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,
+                                      double* d_mu, double* d_kmax_lb, void* stream);
+/* *pass = the bound pass a pruned selection of this spec's GP runs: 0 direct (Matern-0.5), 1 fp64 Gram, 2 fp32 Gram
+ * (B200BO_PRUNE_BOUND=auto|f64|f32, read per call).  Builds the Gram operand if needed and synchronises `stream`. */
+int b200bo_acq_prune_bound_pass(const b200bo_acq* spec, int* pass, void* stream);
+/* The fp32 covariance of the fp32 Gram pass on n fp32 arguments r^2 (device): d_k[i], and d_z[i] (nullable) the
+ * magnitude of its exp argument.  For tests of the margin. */
+int b200bo_cov_f32_dev(int family, int nu, const float* d_r2, int64_t n, float* d_k, float* d_z, void* stream);
 
 #ifdef __cplusplus
 }
