@@ -30,6 +30,18 @@ __host__ __device__ constexpr bool acq_prunable(int kind) {
            acq_constraints_in_log<false>(kind);
 }
 
+// ---- input transform (B200BO_XFORM_*, include/b200bo.h) -----------------------------------
+// The reference's per-dimension np.round (half to even: rint), then sklearn's division by the length scale before
+// differencing: cdist(X / length_scale, Y / length_scale) (SK/gaussian_process/kernels.py:1716-1720).  Training rows and
+// candidates go through the same rule, or every K* entry is wrong.  xform: [d] transform codes, or nullptr (identity).
+// Each use tests xform for null itself: behind a bool-valued helper the two tests compile to a materialised flag and an
+// extra branch in every kernel that stages coordinates.
+__host__ __device__ constexpr bool xform_rounds(int code) { return code == B200BO_XFORM_ROUND; }
+__device__ __forceinline__ double scale_input(double v, const int* xform, const double* ls, int j) {
+    if (xform && xform_rounds(xform[j])) v = rint(v);
+    return v / ls[j];
+}
+
 // ---- branch-free fp64 primitives for the covariance functions -----------------------------
 // The kernel-matrix builders evaluate sqrt and exp for every (training point, candidate) pair
 // with only a few resident warps, so data-dependent slow-path branches (libm special cases) and

@@ -19,11 +19,7 @@ __global__ void scale_x_kernel(const double* __restrict__ X, const double* __res
     if (idx >= (long long)np * d) return;
     const int i = (int)(idx / d), j = (int)(idx % d);
     double v = 0.0;
-    if (i < n) {
-        v = X[idx];
-        if (xform && xform[j] == B200BO_XFORM_ROUND) v = rint(v);  // np.round: half-to-even
-        v = v / ls[j];
-    }
+    if (i < n) v = scale_input(X[idx], xform, ls, j);
     Xs[idx] = v;
 }
 
@@ -661,11 +657,7 @@ __global__ void scale_xc_kernel(const double* __restrict__ Xc, const double* __r
     if (idx >= (long long)mp * d) return;
     const int i = (int)(idx / d), j = (int)(idx % d);
     double v = 0.0;
-    if (i < m) {
-        v = Xc[idx];
-        if (xform && xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-        v = v / ls[j];
-    }
+    if (i < m) v = scale_input(Xc[idx], xform, ls, j);
     Xcs[idx] = v;
 }
 // Kst[k][c] = const * cov(Xs[k], Xcs[c])  (np x mp, zero for padded rows/columns)
@@ -732,8 +724,7 @@ __global__ void append_krow_kernel(const double* __restrict__ x_new, const doubl
     if (threadIdx.x < d) {
         double v = x_new[threadIdx.x];
         if (blockIdx.x == 0) X[(size_t)n * d + threadIdx.x] = v;
-        if (xform && xform[threadIdx.x] == B200BO_XFORM_ROUND) v = rint(v);
-        v = v / ls[threadIdx.x];
+        v = scale_input(v, xform, ls, threadIdx.x);
         xs[threadIdx.x] = v;
         if (blockIdx.x == 0) Xs[(size_t)n * d + threadIdx.x] = v;
     }

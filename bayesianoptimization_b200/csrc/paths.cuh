@@ -87,11 +87,7 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
             const int cc = idx / d, j = idx - cc * d;
             const long long gi = c0 + cc;
             double v = 0.0;
-            if (gi < P.m) {
-                v = candidate_coord(P, gi, j);
-                if (P.xform && P.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-                v = v / P.ls[j];
-            }
+            if (gi < P.m) v = scale_input(candidate_coord(P, gi, j), P.xform, P.ls, j);
             xc_s[j * PBN + cc] = v;
         }
         int pc = 0;  // ROWS: the column of V / W this thread's candidate reads
@@ -211,11 +207,7 @@ __global__ void __launch_bounds__(PG_NT) paths_grad_kernel(const PathsParams P, 
     const int tid = threadIdx.x, d = P.d, q = P.q;
     const long long gi = blockIdx.x;
     const int p = P.path_idx[gi];
-    if (tid < d) {
-        double v = P.Xc[gi * d + tid];
-        if (P.xform && P.xform[tid] == B200BO_XFORM_ROUND) v = rint(v);
-        xs_s[tid] = v / P.ls[tid];
-    }
+    if (tid < d) xs_s[tid] = scale_input(P.Xc[gi * d + tid], P.xform, P.ls, tid);
     __syncthreads();
     const int nsl = PG_NT / d, per = PG_NT / nsl;  // slices per dimension, items of a chunk per slice (the last
     const int j = tid % d, sl = tid / d;           // slice also takes the remainder)
@@ -262,8 +254,7 @@ __global__ void __launch_bounds__(PG_NT) paths_grad_kernel(const PathsParams P, 
     if (tid < d) {
         double t = 0.0;
         for (int s2 = 0; s2 < nsl; ++s2) t += red[s2 * d + tid];
-        const bool rounded = P.xform && P.xform[tid] == B200BO_XFORM_ROUND;
-        grad[gi * d + tid] = rounded ? 0.0 : P.y_std * t / P.ls[tid];
+        grad[gi * d + tid] = P.xform && xform_rounds(P.xform[tid]) ? 0.0 : P.y_std * t / P.ls[tid];
     }
 }
 

@@ -6,8 +6,8 @@
 //     the kernel fits in 128 registers/thread, and every SM sub-partition holds FOUR resident warps whose
 //     LDS -> DMMA dependencies interleave (the 8-warp kernel has two: ncu showed ~6 % issue gaps inside the
 //     DMMA loop, stalled_wait 4.8 / math_pipe_throttle 3.2 per issue);
-//   * phase A (K* build, DFMA + sqrt/exp latency chains) runs with 16 warps, four row-quarters per candidate
-//     column, so its latency-bound part shrinks;
+//   * phase A (phase_a<P16_NT>: K* build, DFMA + sqrt/exp latency chains) runs with 16 warps, four row-quarters per
+//     candidate column, so its latency-bound part shrinks;
 //   * phase B runs on the sm_90 shape mma.sync m16n8k4 f64 (MMA = 1684, the default: twice the fp64 tensor rate of
 //     the sm_80 shape m8n8k4 per SM and clock on H100); m8n8k4 (MMA = 884) stays selectable with
 //     B200BO_PREDICT_MMA=884 for A/B measurements (DESIGN.md 4.1, 6, 6.1);
@@ -44,138 +44,6 @@ __device__ __forceinline__ unsigned long long l2_policy_evict_first() {
 __device__ __forceinline__ void cp_async16_cg_hint(void* smem_dst, const void* gmem_src, unsigned long long pol) {
     unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem_src), "l"(pol));
-}
-__device__ __forceinline__ void st_global_hint(double* p, double v, unsigned long long pol) {
-    asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;\n" ::"l"(p), "d"(v), "l"(pol) : "memory");
-}
-
-// ---- phase A: K*^T tile (np x 128) into the CTA's scratch + K* alpha_ -----------------------------
-// KSTR: row stride of the K* scratch in doubles: PBN (cp.async phase B) or PSTR_DMMA (bulk-copy phase B: the rows
-// of a stage are then contiguous in global memory exactly as in shared memory, one copy per stage).
-// KSTR = 0: the bound pass of pruning (predict_bound_kernel): no K* is stored; each thread keeps the largest |K*_i| of
-// its rows in kmax_s[part][c] instead.
-// Column c is candidate c0 + c of the first mlim, or perm[c0 + c] when perm is set (tiles in bound order); rows: the
-// leading training rows to build (a multiple of PA_CHUNK; G.np for all of them - mu_s is K* alpha_ only then).
-template <bool DREG, int COV, int KSTR>
-__device__ __forceinline__ void predict16_phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
-                                                       double* __restrict__ Ks, double* smem,
-                                                       double (*mu_s)[PBN], unsigned long long pol_first,
-                                                       double (*kmax_s)[PBN], const int* perm, long long mlim,
-                                                       int rows) {
-    const int tid = threadIdx.x;
-    const int d = P.d;
-    double* xc_s = smem;                              // [d][PBN]
-    double* xs_s = smem + (size_t)d * PBN;            // [2][PA_CHUNK][d]
-    double* al_s = xs_s + (size_t)2 * PA_CHUNK * d;   // [2][PA_CHUNK]
-    for (int idx = tid; idx < PBN * d; idx += P16_NT) {
-        const int c = idx / d, j = idx - c * d;
-        const long long gi = c0 + c;
-        double v = 0.0;
-        if (gi < mlim) {
-            v = candidate_coord(P, perm ? (long long)perm[gi] : gi, j);
-            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-            v = v / G.ls[j];
-        }
-        xc_s[j * PBN + c] = v;
-    }
-    const int chunk_pieces = PA_CHUNK * d / 2;
-    auto load_chunk = [&](int buf, int ch) {
-        const double* src = G.Xs + (size_t)ch * PA_CHUNK * d;
-        double* dst = xs_s + (size_t)buf * PA_CHUNK * d;
-        for (int q = tid; q < chunk_pieces; q += P16_NT) cp_async16_cg(dst + 2 * q, src + 2 * q);
-        if (tid < PA_CHUNK / 2)
-            cp_async16_cg(al_s + buf * PA_CHUNK + 2 * tid, G.alphav + (size_t)ch * PA_CHUNK + 2 * tid);
-    };
-    const int nch = rows / PA_CHUNK;
-    load_chunk(0, 0);
-    cp_async_commit();
-    __syncthreads();  // xc_s visible
-    const int c = tid & (PBN - 1), part = tid >> 7;  // part in [0, P16_SPLIT)
-    double xc[kPredictMaxDimRegs];
-    if (DREG) {
-#pragma unroll
-        for (int j = 0; j < kPredictMaxDimRegs; ++j) xc[j] = (j < d) ? xc_s[j * PBN + c] : 0.0;
-    }
-    double mu_acc = 0.0, kmax = 0.0;
-    constexpr int R = 8;
-    constexpr int ROWS = PA_CHUNK / P16_SPLIT;  // 16 rows of every chunk per thread
-    for (int ch = 0; ch < nch; ++ch) {
-        if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
-        cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        const double* xs = xs_s + (size_t)(ch & 1) * PA_CHUNK * d;
-        const double* al = al_s + (ch & 1) * PA_CHUNK;
-        for (int r0 = part * ROWS; r0 < (part + 1) * ROWS; r0 += R) {
-            double r2[R];
-#pragma unroll
-            for (int q = 0; q < R; ++q) r2[q] = 0.0;
-            if (DREG && (d & 1) == 0) {
-#pragma unroll
-                for (int j = 0; j < kPredictMaxDimRegs; j += 2) {
-                    if (j < d) {
-#pragma unroll
-                        for (int q = 0; q < R; ++q) {
-                            const double2 xv = *reinterpret_cast<const double2*>(xs + (r0 + q) * d + j);
-                            const double d0 = xc[j] - xv.x, d1 = xc[j + 1] - xv.y;
-                            r2[q] = fma(d0, d0, r2[q]);
-                            r2[q] = fma(d1, d1, r2[q]);
-                        }
-                    }
-                }
-            } else if (DREG) {
-#pragma unroll
-                for (int j = 0; j < kPredictMaxDimRegs; ++j) {
-                    if (j < d) {
-#pragma unroll
-                        for (int q = 0; q < R; ++q) {
-                            const double df = xc[j] - xs[(r0 + q) * d + j];
-                            r2[q] = fma(df, df, r2[q]);
-                        }
-                    }
-                }
-            } else {
-                for (int j = 0; j < d; ++j) {
-                    const double xv = xc_s[j * PBN + c];
-#pragma unroll
-                    for (int q = 0; q < R; ++q) {
-                        const double df = xv - xs[(r0 + q) * d + j];
-                        r2[q] = fma(df, df, r2[q]);
-                    }
-                }
-            }
-#pragma unroll
-            for (int q = 0; q < R; ++q) {
-                const int n = ch * PA_CHUNK + r0 + q;
-                double kv = G.constv * cov_eval<COV>(r2[q]);
-                if (n >= G.n) kv = 0.0;
-                if constexpr (KSTR == 0)
-                    kmax = fmax(kmax, fabs(kv));
-                else
-                    st_global_hint(Ks + (size_t)n * KSTR + c, kv, pol_first);
-                mu_acc = fma(al[r0 + q], kv, mu_acc);
-            }
-        }
-        __syncthreads();  // chunk buffer free for the prefetch of chunk ch+2
-    }
-    cp_async_wait<0>();
-    mu_s[part][c] = mu_acc;
-    if constexpr (KSTR == 0) kmax_s[part][c] = kmax;
-    __threadfence_block();
-    __syncthreads();
-}
-
-template <bool DREG, int KSTR>
-__device__ __forceinline__ void predict16_phase_a(const PredictParams& P, const GpDev& G, long long c0,
-                                                  double* __restrict__ Ks, double* smem, double (*mu_s)[PBN],
-                                                  unsigned long long pol_first, double (*kmax_s)[PBN],
-                                                  const int* perm, long long mlim, int rows) {
-    switch (cov_code(G.family, G.nu)) {
-        case 0: predict16_phase_a_impl<DREG, 0, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-        case 1: predict16_phase_a_impl<DREG, 1, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-        case 2: predict16_phase_a_impl<DREG, 2, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-        default: predict16_phase_a_impl<DREG, 3, KSTR>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-    }
 }
 
 // ---- selection-only pruning: the bound pass ------------------------------------------------------------------
@@ -241,7 +109,7 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictPara
     __shared__ double kmax_s[P16_SPLIT][PBN];
     const long long c0 = (long long)blockIdx.x * PBN;
     const GpDev& G = P.gp[0];
-    predict16_phase_a<DREG, 0>(P, G, c0, nullptr, smem, mu_s, 0ull, kmax_s, nullptr, P.m, G.np);
+    phase_a<P16_NT, DREG, KS_KMAX>(P, G, c0, nullptr, smem, mu_s, 0ull, kmax_s, nullptr, P.m, G.np);
     const int c = threadIdx.x;
     if (c < PBN && c0 + c < P.m) {
         const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
@@ -404,11 +272,7 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
         const int c = q / str, j = q - c * str;
         const long long gi = c0 + c;
         double v = j == d + 1 ? 1.0 : 0.0;
-        if (j < d && gi < P.m) {  // the coordinates phase A builds
-            v = candidate_coord(P, gi, j);
-            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-            v = v / G.ls[j];
-        }
+        if (j < d && gi < P.m) v = scale_input(candidate_coord(P, gi, j), G.xform, G.ls, j);  // as phase A builds them
         xa_s[q] = v;
     }
     const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax, then alpha_ in fp32
@@ -976,11 +840,11 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
             if constexpr (PIPE == PIPE_CPASYNC) {
-                predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, G.np);
+                phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, G.np);
                 predict16_phase_b<MMA, false>(G, Ks, smem, pol_last, pol_first, 0, G.np / PBM, nullptr);
             } else {  // policies made where they are used: nothing extra stays live across phase B
-                predict16_phase_a<DREG, PSTR_DMMA>(P, G, c0, Ks, smem, mu_s, l2_policy_evict_first(), nullptr, P.perm,
-                                                   P.m, G.np);
+                phase_a<P16_NT, DREG, KS_F64_EF, PSTR_DMMA>(P, G, c0, Ks, smem, mu_s, l2_policy_evict_first(), nullptr,
+                                                            P.perm, P.m, G.np);
                 predict16_phase_b_bulk<PIPE == PIPE_BULK_MC>(P, G, smem, full_bar, empty_bar, done_cnt, it);
             }
             const double* red = smem;
@@ -1087,7 +951,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
         const long long tile = tile_s;
         if (tile >= ntiles) break;
         const long long c0 = tile * PBN;
-        predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, R.blocks * PBM);
+        phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, R.blocks * PBM);
         predict16_phase_b<1684, false>(G, Ks, smem, pol_last, pol_first, 0, R.blocks, nullptr);
         const double* red = smem;
         if (tid < PBN && c0 + tid < P.m) {
@@ -1154,7 +1018,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
         const int ib0 = unit_cut(nb, groups, grp), ib1 = unit_cut(nb, groups, grp + 1);
         double* part = R.part + (size_t)(slot0 + tile) * nb * 32 * PBN;
         if (ib1 > ib0) {
-            predict16_phase_a<DREG, PBN>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
+            phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
             predict16_phase_b<1684, true>(G, Ks, smem, pol_last, pol_first, ib0, ib1, part);
             if (ib1 == nb && tid < PBN)  // phase A ran over all np rows: mu_s holds the tile kernel's K* alpha_ sums
                 R.mu_unit[(size_t)(slot0 + tile) * PBN + tid] =

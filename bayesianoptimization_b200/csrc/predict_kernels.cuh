@@ -14,7 +14,8 @@
 //
 // Decomposition: a persistent grid (one CTA per SM); each CTA owns tiles of BN = 128
 // candidates.  Per tile and per GP:
-//   phase A  build K*^T (np x 128) once into a CTA-private HBM/L2 scratch + accumulate K* alpha_
+//   phase A  build K*^T (np x 128) once into a CTA-private HBM/L2 scratch + accumulate K* alpha_ (phase_a, which
+//            every fused predict kernel here and in predict16.cuh runs)
 //   phase B  for each 128-row block of Linv: acc(128x128) = sum_{k<=rows} LinvT[k][rows]^T K*[k][:],
 //            8x8 register tiles, 3-stage cp.async pipeline; then colsq += sum_rows acc^2
 //   phase C  mu, sd, acquisition / constraint probability per candidate
@@ -437,55 +438,72 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
     }
 }
 
-// ---- phase A: K*^T tile (np x 128) into the CTA's scratch + K* alpha_ ---------------------------
-// Thread = one candidate column (two threads per column split the rows).  Training rows stream
-// through shared memory in chunks of 64 (double-buffered cp.async), so every row read is a
-// warp-wide broadcast LDS; DREG keeps the candidate's coordinates in registers (d <= 16).
-// COV is a template parameter so that the covariance is branch-free straight-line code.
+// ---- phase A: the tile's K*^T (np x PBN) + K* alpha_ -----------------------------------------------
+// Every fused predict kernel builds its tile's covariances with this one function, so the tile kernels, the bound pass
+// and the refine / units stages get the same K* entries and the same mu = K* alpha_, bit for bit (DESIGN.md 4.9).
+// Thread = one candidate column; the NT / PBN threads of a column split the rows of every chunk into parts.  Training
+// rows stream through shared memory in chunks of 64 (double-buffered cp.async), so every row read is a warp-wide
+// broadcast LDS; DREG keeps the candidate's coordinates in registers (d <= 16).  COV is a template parameter so that
+// the covariance is branch-free straight-line code.
 constexpr int PA_CHUNK = 64;  // training rows per staged chunk
 
-// TC = false: K* written as fp64 [np][128] (operand of the fp64 GEMM variants).
-// TC = true : K* written as tf32 (hi, lo) pairs in the wgmma operand-image layout of tc_common.cuh
-//             ([np/32][hi|lo][16 KiB], candidate = operand row, training index = K).
-template <bool DREG, int COV, bool TC>
-__device__ __forceinline__ void predict_phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
-                                                     double* __restrict__ Ks, double* smem,
-                                                     double (*mu_s)[PBN]) {
+// Where phase A puts K* (KS):
+//   KS_F64     fp64 [np][KSTR], plain stores (the 8-warp kernel)
+//   KS_F64_EF  fp64 [np][KSTR], stores under the L2 policy pol_first (evict_first: the CTA-private scratch is written
+//              once and swept cyclically, LRU-hostile).  KSTR = PBN for the cp.async phase B, PSTR_DMMA for the
+//              bulk-copy phase B: the rows of a stage are then contiguous in global memory exactly as in shared memory.
+//   KS_TF32    tf32 (hi, lo) pairs in the wgmma operand-image layout of tc_common.cuh ([np/32][hi|lo][16 KiB],
+//              candidate = operand row, training index = K), fenced for the bulk copies that read them (fp32 mode)
+//   KS_KMAX    nowhere: each thread keeps the largest |K*_i| of its rows in kmax_s[part][c] (the bound pass of pruning)
+// mu_s[part][c] is the part's share of K* alpha_; each caller adds the NT / PBN parts in its fixed order.
+// Column c is candidate c0 + c of the first mlim, or perm[c0 + c] when perm is set (tiles in bound order); rows: the
+// leading training rows to build (a multiple of PA_CHUNK; G.np for all of them - mu_s is K* alpha_ only then).
+enum { KS_F64, KS_F64_EF, KS_TF32, KS_KMAX };
+
+__device__ __forceinline__ void st_global_hint(double* p, double v, unsigned long long pol) {
+    asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;\n" ::"l"(p), "d"(v), "l"(pol) : "memory");
+}
+
+template <int NT, bool DREG, int KS, int KSTR, int COV>
+__device__ __forceinline__ void phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
+                                             double* __restrict__ Ks, double* smem, double (*mu_s)[PBN],
+                                             unsigned long long pol_first, double (*kmax_s)[PBN], const int* perm,
+                                             long long mlim, int rows) {
+    constexpr int ROWS = PA_CHUNK / (NT / PBN);  // rows of every chunk per thread
     const int tid = threadIdx.x;
     const int d = P.d, np = G.np;
-    double* xc_s = smem;                       // [d][PBN]
-    double* xs_s = smem + (size_t)d * PBN;     // [2][PA_CHUNK][d]
+    double* xc_s = smem;                             // [d][PBN]
+    double* xs_s = smem + (size_t)d * PBN;           // [2][PA_CHUNK][d]
     double* al_s = xs_s + (size_t)2 * PA_CHUNK * d;  // [2][PA_CHUNK] alpha_ of the staged rows
-    for (int idx = tid; idx < PBN * d; idx += PNT) {
+    for (int idx = tid; idx < PBN * d; idx += NT) {
         const int c = idx / d, j = idx - c * d;
         const long long gi = c0 + c;
         double v = 0.0;
-        if (gi < P.m) {
-            v = candidate_coord(P, gi, j);
-            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-            v = v / G.ls[j];
-        }
+        if (gi < mlim) v = scale_input(candidate_coord(P, perm ? (long long)perm[gi] : gi, j), G.xform, G.ls, j);
         xc_s[j * PBN + c] = v;
     }
     const int chunk_pieces = PA_CHUNK * d / 2;  // 16-byte pieces per chunk (PA_CHUNK*d is even)
     auto load_chunk = [&](int buf, int ch) {
         const double* src = G.Xs + (size_t)ch * PA_CHUNK * d;
         double* dst = xs_s + (size_t)buf * PA_CHUNK * d;
-        for (int q = tid; q < chunk_pieces; q += PNT) cp_async16_cg(dst + 2 * q, src + 2 * q);
+        for (int q = tid; q < chunk_pieces; q += NT) cp_async16_cg(dst + 2 * q, src + 2 * q);
         if (tid < PA_CHUNK / 2)
             cp_async16_cg(al_s + buf * PA_CHUNK + 2 * tid, G.alphav + (size_t)ch * PA_CHUNK + 2 * tid);
     };
-    const int nch = np / PA_CHUNK;
+    // The 256-thread kernels always build all np rows; they take np from G here rather than rows from the call site,
+    // because where that load sits steers their instruction schedule (read at the call, fp32 mode ran 0.2 % slower on an
+    // H100 80GB HBM3 at 700 W).
+    const int nch = (NT == PNT ? np : rows) / PA_CHUNK;
     load_chunk(0, 0);
     cp_async_commit();
     __syncthreads();  // xc_s visible
-    const int c = tid & (PBN - 1), half = tid >> 7;
+    const int c = tid & (PBN - 1), part = tid >> 7;  // part in [0, NT / PBN)
     double xc[kPredictMaxDimRegs];
     if (DREG) {
 #pragma unroll
         for (int j = 0; j < kPredictMaxDimRegs; ++j) xc[j] = (j < d) ? xc_s[j * PBN + c] : 0.0;
     }
-    double mu_acc = 0.0;
+    double mu_acc = 0.0, kmax = 0.0;
     constexpr int R = 8;
     for (int ch = 0; ch < nch; ++ch) {
         if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
@@ -494,7 +512,7 @@ __device__ __forceinline__ void predict_phase_a_impl(const PredictParams& P, con
         __syncthreads();
         const double* xs = xs_s + (size_t)(ch & 1) * PA_CHUNK * d;
         const double* al = al_s + (ch & 1) * PA_CHUNK;
-        for (int r0 = half * (PA_CHUNK / 2); r0 < (half + 1) * (PA_CHUNK / 2); r0 += R) {
+        for (int r0 = part * ROWS; r0 < (part + 1) * ROWS; r0 += R) {
             double r2[R];
 #pragma unroll
             for (int q = 0; q < R; ++q) r2[q] = 0.0;
@@ -538,15 +556,19 @@ __device__ __forceinline__ void predict_phase_a_impl(const PredictParams& P, con
                 const int n = ch * PA_CHUNK + r0 + q;
                 double kv = G.constv * cov_eval<COV>(r2[q]);
                 if (n >= G.n) kv = 0.0;
-                if (TC) {
+                if constexpr (KS == KS_F64) {
+                    Ks[(size_t)n * KSTR + c] = kv;
+                } else if constexpr (KS == KS_F64_EF) {
+                    st_global_hint(Ks + (size_t)n * KSTR + c, kv, pol_first);
+                } else if constexpr (KS == KS_TF32) {
                     hi[q] = tc::to_tf32((float)kv);
                     lo[q] = tc::to_tf32((float)(kv - (double)hi[q]));
                 } else {
-                    Ks[(size_t)n * PBN + c] = kv;
+                    kmax = fmax(kmax, fabs(kv));
                 }
                 mu_acc = fma(al[r0 + q], kv, mu_acc);
             }
-            if (TC) {
+            if constexpr (KS == KS_TF32) {
                 const int n0 = ch * PA_CHUNK + r0;  // multiple of 8: two groups of 4 consecutive k
                 uint8_t* img = reinterpret_cast<uint8_t*>(Ks) + (size_t)(n0 >> 5) * (2 * tc::kTcImgBytes);
 #pragma unroll
@@ -562,8 +584,9 @@ __device__ __forceinline__ void predict_phase_a_impl(const PredictParams& P, con
         __syncthreads();  // chunk buffer free for the prefetch of chunk ch+2
     }
     cp_async_wait<0>();
-    mu_s[half][c] = mu_acc;
-    if (TC) {
+    mu_s[part][c] = mu_acc;
+    if constexpr (KS == KS_KMAX) kmax_s[part][c] = kmax;
+    if constexpr (KS == KS_TF32) {
         tc::fence_proxy_async_global();  // scratch images will be read by bulk async copies
         tc::fence_proxy_async_smem();    // and the stage buffers overwritten by them
     }
@@ -571,15 +594,15 @@ __device__ __forceinline__ void predict_phase_a_impl(const PredictParams& P, con
     __syncthreads();
 }
 
-template <bool DREG, bool TC = false>
-__device__ __forceinline__ void predict_phase_a(const PredictParams& P, const GpDev& G, long long c0,
-                                                double* __restrict__ Ks, double* smem,
-                                                double (*mu_s)[PBN]) {
+template <int NT, bool DREG, int KS, int KSTR = PBN>
+__device__ __forceinline__ void phase_a(const PredictParams& P, const GpDev& G, long long c0, double* __restrict__ Ks,
+                                        double* smem, double (*mu_s)[PBN], unsigned long long pol_first,
+                                        double (*kmax_s)[PBN], const int* perm, long long mlim, int rows) {
     switch (cov_code(G.family, G.nu)) {
-        case 0: predict_phase_a_impl<DREG, 0, TC>(P, G, c0, Ks, smem, mu_s); break;
-        case 1: predict_phase_a_impl<DREG, 1, TC>(P, G, c0, Ks, smem, mu_s); break;
-        case 2: predict_phase_a_impl<DREG, 2, TC>(P, G, c0, Ks, smem, mu_s); break;
-        default: predict_phase_a_impl<DREG, 3, TC>(P, G, c0, Ks, smem, mu_s); break;
+        case 0: phase_a_impl<NT, DREG, KS, KSTR, 0>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        case 1: phase_a_impl<NT, DREG, KS, KSTR, 1>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        case 2: phase_a_impl<NT, DREG, KS, KSTR, 2>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        default: phase_a_impl<NT, DREG, KS, KSTR, 3>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
     }
 }
 
@@ -797,7 +820,7 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_kernel(const PredictParams
         const long long c0 = tile * PBN;
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
-            predict_phase_a<DREG>(P, G, c0, Ks, smem, mu_s);
+            phase_a<PNT, DREG, KS_F64>(P, G, c0, Ks, smem, mu_s, 0ull, nullptr, nullptr, P.m, G.np);
             if (IMPL == PREDICT_IMPL_DMMA)
                 predict_phase_b_dmma(G, Ks, smem);
             else
@@ -874,7 +897,7 @@ __global__ void __launch_bounds__(PNT, 1) predict_acq_tc_kernel(const PredictPar
         const long long c0 = tile * PBN;
         for (int g = 0; g < P.n_gps; ++g) {
             const GpDev& G = P.gp[g];
-            predict_phase_a<DREG, true>(P, G, c0, Ks, smem, mu_s);
+            phase_a<PNT, DREG, KS_TF32>(P, G, c0, Ks, smem, mu_s, 0ull, nullptr, nullptr, P.m, G.np);
             const int nb = G.np / PBM;
             const int nkt_row = G.np / tc::kTcK;  // images per row block in the A array
             const uint8_t* Bimg = reinterpret_cast<const uint8_t*>(Ks);
@@ -1071,11 +1094,7 @@ small_kstar_kernel(const SmallParams S, int g) {
     for (int idx = tid; idx < SMC * d; idx += 256) {
         const int c = idx / d, j = idx - c * d;
         double v = 0.0;
-        if (c < mc) {
-            v = candidate_coord(S.P, pc0 + c, j);
-            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-            v = v / G.ls[j];
-        }
+        if (c < mc) v = scale_input(candidate_coord(S.P, pc0 + c, j), G.xform, G.ls, j);
         xc_s[c][j] = v;
     }
     __syncthreads();
@@ -1290,11 +1309,7 @@ small_grad_kernel(const SmallParams S, int g) {
     for (int idx = tid; idx < SMC * d; idx += 256) {
         const int c = idx / d, j = idx - c * d;
         double v = 0.0;
-        if (c < mc) {
-            v = S.P.Xc[(pc0 + c) * d + j];
-            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) v = rint(v);
-            v = v / G.ls[j];
-        }
+        if (c < mc) v = scale_input(S.P.Xc[(pc0 + c) * d + j], G.xform, G.ls, j);
         xc_s[c][j] = v;
     }
     __syncthreads();
@@ -1433,7 +1448,7 @@ small_finish_grad_kernel(const SmallParams S) {
         double gr = 0.0;
         for (int g = 0; g < ng; ++g) {
             const GpDev& G = S.P.gp[g];
-            if (G.xform && G.xform[j] == B200BO_XFORM_ROUND) continue;
+            if (G.xform && xform_rounds(G.xform[j])) continue;
             const int nb = G.np / 128;
             if (NEI && g == 0) {  // sum_s wn_s (-y_std) sum_b list s, then the u list
                 const int nl = S.P.n_ystar + 1;
