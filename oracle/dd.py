@@ -292,6 +292,63 @@ def backward(Lh, Ll, zh, zl, n):
 
 
 @njit(parallel=True, cache=False)
+def backward_rows(Lh, Ll, Zh, Zl, n):
+    """X[t] = L[:n, :n]^-T Z[t, :n] for every row t of Z: backward() row by row (rows in parallel), bit-equal to it.
+    Reads L's columns through a transposed copy."""
+    Th = np.ascontiguousarray(Lh[:n, :n].T)
+    Tl = np.ascontiguousarray(Ll[:n, :n].T)
+    m = Zh.shape[0]
+    Xh = np.zeros((m, n))
+    Xl = np.zeros((m, n))
+    for t in prange(m):
+        for i in range(n - 1, -1, -1):
+            sh, sl = 0.0, 0.0
+            for k in range(i + 1, n):
+                ph, pl = dd_mul(Th[i, k], Tl[i, k], Xh[t, k], Xl[t, k])
+                sh, sl = dd_add(sh, sl, ph, pl)
+            sh, sl = dd_sub(Zh[t, i], Zl[t, i], sh, sl)
+            Xh[t, i], Xl[t, i] = dd_div(sh, sl, Th[i, i], Tl[i, i])
+    return Xh, Xl
+
+
+@njit(parallel=True, cache=False)
+def lower_rows(Lh, Ll, Bh, Bl, n):
+    """V[t] = L[:n, :n] B[t, :n] for every row t of B: one ordered dot product per entry (factor rows in parallel)."""
+    m = Bh.shape[0]
+    Vh = np.zeros((m, n))
+    Vl = np.zeros((m, n))
+    for i in prange(n):
+        for t in range(m):
+            Vh[t, i], Vl[t, i] = _dot(Lh[i], Ll[i], Bh[t], Bl[t], 0, i + 1)
+    return Vh, Vl
+
+
+@njit(parallel=True, cache=False)
+def cross_cov_grad(A, B, code, c, inv_ls, Wh, Wl):
+    """G[t, q, j] = sum_i W[t, q, i] d(c k(a_t, b_i)) / d x_j for scaled rows A (m, d) and B (n, d), the derivative in
+    unscaled input coordinates: d k / d x_j = -c g(r^2) (a_tj - b_ij) / l_j with g of grad_factor_dd (0 at r = 0 for
+    Matern 1/2) and inv_ls = 1 / l (powers of two: exact).  Sums over i in order; rows t in parallel."""
+    m, d = A.shape
+    n = B.shape[0]
+    nq = Wh.shape[1]
+    Gh = np.zeros((m, nq, d))
+    Gl = np.zeros((m, nq, d))
+    for t in prange(m):
+        for i in range(n):
+            rh, rl = _r2(A[t], B[i])
+            kh, kl = cov_dd(code, rh, rl)
+            gh, gl = grad_factor_dd(code, rh, rl, kh, kl)
+            for j in range(d):
+                dh, dl = two_sum(A[t, j], -B[i, j])
+                dh, dl = dd_mul(dh, dl, gh, gl)
+                dh, dl = -c * inv_ls[j] * dh, -c * inv_ls[j] * dl
+                for q in range(nq):
+                    ph, pl = dd_mul(Wh[t, q, i], Wl[t, q, i], dh, dl)
+                    Gh[t, q, j], Gl[t, q, j] = dd_add(Gh[t, q, j], Gl[t, q, j], ph, pl)
+    return Gh, Gl
+
+
+@njit(parallel=True, cache=False)
 def inverse_t(Lh, Ll, n):
     """Wt = (L^-1)^T: row j of Wt is column j of L^-1, zero before j (columns in parallel)."""
     Wh = np.zeros((n, n))

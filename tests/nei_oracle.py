@@ -62,6 +62,32 @@ def nei(Ks, A, best, sd, xi, y_mean=0.0, y_std=1.0, log=False):
     return logmeanexp(_log_ei(a, sd))
 
 
+def nei_value_grad(gp0, x, A, best, xi, log=False):
+    """NEI (or LogNEI) and its input gradient (m, d) at the rows x.  gp0 is a grad_oracle.GradGP of the noiseless GP
+    (K0 = c k(X, X) + tau I, the noisy GP's y statistics), A = K0^-1 F (n, S), best (S,) data units.  With
+    d mu_s = s_y sum_n A_ns d k*_n / dx and d sd from GradGP.predict_grad, NEI's gradient is the mean over the fantasies
+    of EI's, Phi(z_s) d mu_s + phi(z_s) d sd, and LogNEI's is NEI's over NEI."""
+    import grad_oracle as GO
+
+    xs = gp0.transform(x) / gp0.ls
+    diff = xs[:, None, :] - gp0.Xs[None, :, :]
+    r = np.sqrt((diff ** 2).sum(-1))
+    ks = gp0.const * GO.k_of_r(r, gp0.nu)
+    dks = -(gp0.const * GO.h_of_r(r, gp0.nu))[:, :, None] * diff / gp0.ls
+    _, sd, _, dsd = gp0.predict_grad(x)
+    mu = gp0.y_std * (ks @ A) + gp0.y_mean
+    dmu = gp0.y_std * np.einsum("ns,mnj->msj", A, dks)
+    a = mu - best[None, :] - xi
+    with np.errstate(all="ignore"):
+        z = a / sd[:, None]
+        cdf, pdf = ndtr(z), np.exp(-0.5 * z * z) / np.sqrt(2.0 * np.pi)
+    v = (a * cdf + sd[:, None] * pdf).mean(axis=1)
+    g = (cdf[:, :, None] * dmu + pdf[:, :, None] * dsd[:, None, :]).mean(axis=1)
+    if log:
+        return np.log(v), g / v[:, None]
+    return v, g
+
+
 def _log_ei(a, sd):
     return LO.log_acq_term(LO.LOGEI, a, sd)
 
