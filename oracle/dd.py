@@ -575,6 +575,28 @@ class Fit:
         return float(np.max(r)) / float(np.max(np.abs(self.yn[0])))
 
 
+def solve_rows(fit, Bh, Bl):
+    """K^-1 B[t] for every row t of B, through the factor of `fit`."""
+    n = fit.n
+    V = forward_rows(fit.L[0], fit.L[1], Bh, Bl, n)
+    return backward_rows(fit.L[0], fit.L[1], V[0], V[1], n)
+
+
+def posterior_grad(fit, xs, Kg, W):
+    """The input gradients of the posterior at the scaled rows xs, whose cross covariances to the n training rows are
+    Kg (pair of (m, n) arrays): U = K^-1 k* per row (pair), and G = cross_cov_grad with the weights [W; u_t] of each
+    row t, so that G[t, q, j] = sum_i W[q, i] dk*_ti / dx_j for the rows q of W (the same for every t) and
+    G[t, -1, j] = u_t . dk*_t / dx_j.  With W = alpha_: d mu / dx_j = s_y G[t, 0, j] and
+    d sigma^2 / dx_j = -2 s_y^2 G[t, -1, j]."""
+    n, m = fit.n, len(xs)
+    U = solve_rows(fit, *Kg)
+    q = len(W[0])
+    Wh = np.ascontiguousarray(np.concatenate([np.broadcast_to(W[0], (m, q, n)), U[0][:, None, :]], axis=1))
+    Wl = np.ascontiguousarray(np.concatenate([np.broadcast_to(W[1], (m, q, n)), U[1][:, None, :]], axis=1))
+    G = cross_cov_grad(np.ascontiguousarray(xs), fit.Xs, fit.code, fit.c, 1.0 / ls_vec(fit.case), Wh, Wl)
+    return U, G
+
+
 def acquisitions(mu, var, y_max, kappa, xi):
     """UCB, EI and PoI at 50 digits from mu and sigma^2 (mpmath lists); mpmath's Phi and phi."""
     mp.mp.dps = 50

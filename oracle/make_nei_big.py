@@ -140,11 +140,7 @@ def _combine(yh, yl, sqh, sql, E, dsh, dsl, KRh, KRl):
     return Fh, Fl
 
 
-def _solve(fit, Bh, Bl):
-    """K^-1 B[t] for every row t of B, through the factor of `fit`."""
-    n = fit.n
-    V = dd.forward_rows(fit.L[0], fit.L[1], Bh, Bl, n)
-    return dd.backward_rows(fit.L[0], fit.L[1], V[0], V[1], n)
+_solve = dd.solve_rows
 
 
 def _ei(a, sd):
@@ -208,17 +204,12 @@ class Truth:
         """d NEI / dx and d LogNEI / dx on the rows gi: d mu_s = s_y sum_i a_si dk*_i, d sigma0^2 = -2 s_y^2 u . dk*
         with u = K0^-1 k*, d sigma0 = d sigma0^2 / (2 sigma0); NEI's the mean of Phi(z_s) d mu_s + phi(z_s) d sigma0,
         LogNEI's that over NEI."""
-        fit0, gi, n = self.fit0, self.gi, self.n
+        fit0, gi = self.fit0, self.gi
         Kg = (np.ascontiguousarray(Ks[0][gi]), np.ascontiguousarray(Ks[1][gi]))
-        U = _solve(fit0, *Kg)
         order = list(self.runs)
-        Wh = np.concatenate([self.runs[r]["A"][0] for r in order])
-        Wl = np.concatenate([self.runs[r]["A"][1] for r in order])
-        q = len(Wh)
-        Wh = np.ascontiguousarray(np.concatenate([np.broadcast_to(Wh, (len(gi), q, n)), U[0][:, None, :]], axis=1))
-        Wl = np.ascontiguousarray(np.concatenate([np.broadcast_to(Wl, (len(gi), q, n)), U[1][:, None, :]], axis=1))
-        G = dd.cross_cov_grad(np.ascontiguousarray(self.xs[gi]), fit0.Xs, fit0.code, fit0.c,
-                              1.0 / dd.ls_vec(self.nl), Wh, Wl)
+        W = tuple(np.concatenate([self.runs[r]["A"][p] for r in order]) for p in (0, 1))
+        q = len(W[0])
+        U, G = dd.posterior_grad(fit0, self.xs[gi], Kg, W)
         d = G[0].shape[2]
         ys = fit0.y_std
         self.U = U

@@ -10,6 +10,7 @@ import math
 
 import numpy as np
 from scipy.linalg import cho_solve, cholesky, solve_triangular
+from scipy.spatial.distance import cdist
 from scipy.special import erfcx, log_ndtr, ndtr
 
 UCB, EI, POI, MES = 0, 1, 2, 4
@@ -63,7 +64,7 @@ class GradGP:
         y = np.asarray(y, dtype=float)
         self.y_mean, self.y_std = (float(y.mean()), float(y.std()) or 1.0) if normalize else (0.0, 1.0)
         self.y_norm = (y - self.y_mean) / self.y_std
-        r = np.sqrt(((self.Xs[:, None, :] - self.Xs[None, :, :]) ** 2).sum(-1))
+        r = cdist(self.Xs, self.Xs)  # no (n, n, d) temporary: N = 8192, d = 32 would need 17 GB
         K = self.const * k_of_r(r, nu)
         K[np.diag_indices(n)] = self.const + self.noise + alpha
         self.K = K

@@ -194,38 +194,45 @@ def mp_Phi(mp, x):
     return mp.erfc(-x / mp.sqrt(2)) / 2
 
 
-def mp_log_h(z):
+# Each mp_* takes an fp64 or an mpmath argument and returns fp64 values, or with exact=True the mpmath values themselves
+# (oracle/make_acq_big.py evaluates them on its unrounded double-double mu and sigma).
+def _out(exact, *v):
+    v = v if exact else tuple(float(x) for x in v)
+    return v[0] if len(v) == 1 else v
+
+
+def mp_log_h(z, exact=False):
     """log h, h = phi(z) + z Phi(z); for z < -1 from the Mills form so that the cancellation stays inside 60 digits."""
     mp = _mp()
-    z = mp.mpf(float(z))
+    z = mp.mpf(z)
     if z > -1:
-        return float(mp.log(mp.npdf(z) + z * mp_Phi(mp, z)))
+        return _out(exact, mp.log(mp.npdf(z) + z * mp_Phi(mp, z)))
     mp.mp.dps = 60 + int(2 * mp.log10(-z)) + 10
     h = mp.npdf(z) + z * mp_Phi(mp, z)
-    return float(mp.log(h))
+    return _out(exact, mp.log(h))
 
 
-def mp_log_h_ratios(z):
+def mp_log_h_ratios(z, exact=False):
     mp = _mp()
-    z = mp.mpf(float(z))
+    z = mp.mpf(z)
     if z < -1:
         mp.mp.dps = 60 + int(2 * mp.log10(-z)) + 10
     P, p = mp_Phi(mp, z), mp.npdf(z)
     h = p + z * P
-    return float(P / h), float(p / h)
+    return _out(exact, P / h, p / h)
 
 
-def mp_log_ndtr(g):
+def mp_log_ndtr(g, exact=False):
     mp = _mp()
-    x = mp.mpf(float(g))
-    return float(mp.log(mp_Phi(mp, x)) if x < 0 else mp.log1p(-mp.erfc(x / mp.sqrt(2)) / 2))  # 1 - Phi exactly
+    x = mp.mpf(g)
+    return _out(exact, mp.log(mp_Phi(mp, x)) if x < 0 else mp.log1p(-mp.erfc(x / mp.sqrt(2)) / 2))  # 1 - Phi exactly
 
 
-def mp_cfactor(l, u):
+def mp_cfactor(l, u, exact=False):
     """(log p, dlogp/dl, dlogp/du) for p = Phi(u) - Phi(l), standardised bounds (+-inf allowed)."""
     mp = _mp()
-    lm = -mp.inf if l == -np.inf else mp.mpf(float(l))
-    um = mp.inf if u == np.inf else mp.mpf(float(u))
+    lm = -mp.inf if l == -np.inf else mp.mpf(l)
+    um = mp.inf if u == np.inf else mp.mpf(u)
     # Phi(u) - Phi(l) = Phi(-l) - Phi(-u): take the form without cancellation
     if lm >= 0:
         p = mp.erfc(lm / mp.sqrt(2)) / 2 - mp.erfc(um / mp.sqrt(2)) / 2
@@ -233,4 +240,4 @@ def mp_cfactor(l, u):
         p = mp_Phi(mp, um) - mp_Phi(mp, lm)
     dl = mp.mpf(0) if lm == -mp.inf else -mp.npdf(lm) / p
     du = mp.mpf(0) if um == mp.inf else mp.npdf(um) / p
-    return float(mp.log(p)), float(dl), float(du)
+    return _out(exact, mp.log(p), dl, du)

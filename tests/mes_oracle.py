@@ -23,6 +23,18 @@ def mes_term(g):
     return g * np.exp(norm.logpdf(g) - ln) / 2.0 - ln
 
 
+def mp_mes_term(g, dps=50):
+    """(g psi(g) / (2 Psi(g)) - log Psi(g), its derivative in g) at `dps` digits (mpmath) for an fp64 or mpmath g:
+    with lambda = psi / Psi, d lambda / dg = -lambda (g + lambda), the derivative is -lambda/2 - g lambda (g + lambda)/2."""
+    import mpmath as mp
+
+    with mp.workdps(dps):
+        g = mp.mpf(g)
+        P = mp.ncdf(g)
+        lam = mp.npdf(g) / P
+        return g * lam / 2 - mp.log(P), -lam / 2 - g * lam * (g + lam) / 2
+
+
 def mes_alpha(mu, sd, ystar):
     mu = np.asarray(mu, dtype=np.float64)
     sd = np.asarray(sd, dtype=np.float64)
