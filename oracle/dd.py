@@ -40,6 +40,18 @@ SQRT3_H, SQRT3_L = _pair(mp.sqrt(3))
 SQRT5_H, SQRT5_L = _pair(mp.sqrt(5))
 EXP_HALVINGS = 10  # exp(r) = exp(r / 2^10)^(2^10) after the reduction by k ln 2
 EXP_TERMS = 12  # Taylor terms of expm1 at |r| <= ln2 / 2^11: the 12th is below 1e-50
+# pi/2 as the sum of three doubles (each the fp64 rounding of the rest): k (pi/2 - P1 - P2 - P3) stays below 1e-40
+# for any |k| < 2^40, far past every feature argument of the path fixtures (|omega . xs + b| < 1e8).
+_PIO2 = mp.pi / 2
+PIO2_1 = float(_PIO2)
+PIO2_2 = float(_PIO2 - PIO2_1)
+PIO2_3 = float(_PIO2 - PIO2_1 - PIO2_2)
+TWO_OVER_PI = float(2 / mp.pi)
+# Taylor coefficients (-1)^k / (2k)! of cos and (-1)^k / (2k+1)! of sin (k = 0 .. 14) as double-doubles: at |r| <= pi/4
+# the first omitted terms are below 3e-36.
+TRIG_TERMS = 15
+COS_C = np.array([_pair(mp.mpf(-1) ** k / mp.factorial(2 * k)) for k in range(TRIG_TERMS)])
+SIN_C = np.array([_pair(mp.mpf(-1) ** k / mp.factorial(2 * k + 1)) for k in range(TRIG_TERMS)])
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -151,6 +163,36 @@ def dd_exp(ah, al):
     sh, sl = dd_add(sh, sl, 1.0, 0.0)
     ki = int(k)
     return np.ldexp(sh, ki), np.ldexp(sl, ki)
+
+
+@njit(cache=False)
+def dd_cos_sin(ah, al):
+    """(cos a, sin a) as double-doubles: a = k pi/2 + r with pi/2 in three doubles (the products k P_i exact), then the
+    Taylor series of cos and sin on |r| <= pi/4 (Horner in r^2) and the quadrant k mod 4."""
+    k = np.floor(ah * TWO_OVER_PI + 0.5)
+    ph, pl = two_prod(k, PIO2_1)
+    rh, rl = dd_sub(ah, al, ph, pl)
+    ph, pl = two_prod(k, PIO2_2)
+    rh, rl = dd_sub(rh, rl, ph, pl)
+    ph, pl = two_prod(k, PIO2_3)
+    rh, rl = dd_sub(rh, rl, ph, pl)
+    zh, zl = dd_mul(rh, rl, rh, rl)
+    ch, cl = COS_C[TRIG_TERMS - 1, 0], COS_C[TRIG_TERMS - 1, 1]
+    sh, sl = SIN_C[TRIG_TERMS - 1, 0], SIN_C[TRIG_TERMS - 1, 1]
+    for i in range(TRIG_TERMS - 2, -1, -1):
+        ch, cl = dd_mul(ch, cl, zh, zl)
+        ch, cl = dd_add(ch, cl, COS_C[i, 0], COS_C[i, 1])
+        sh, sl = dd_mul(sh, sl, zh, zl)
+        sh, sl = dd_add(sh, sl, SIN_C[i, 0], SIN_C[i, 1])
+    sh, sl = dd_mul(sh, sl, rh, rl)
+    quad = int(k) % 4
+    if quad == 0:
+        return ch, cl, sh, sl
+    if quad == 1:
+        return -sh, -sl, ch, cl
+    if quad == 2:
+        return -ch, -cl, -sh, -sl
+    return sh, sl, -ch, -cl
 
 
 @njit(cache=False)
@@ -595,6 +637,140 @@ def posterior_grad(fit, xs, Kg, W):
     Wl = np.ascontiguousarray(np.concatenate([np.broadcast_to(W[1], (m, q, n)), U[1][:, None, :]], axis=1))
     G = cross_cov_grad(np.ascontiguousarray(xs), fit.Xs, fit.code, fit.c, 1.0 / ls_vec(fit.case), Wh, Wl)
     return U, G
+
+
+@njit(parallel=True, cache=False)
+def feature_sums(Xs, omega, b, W, grad):
+    """F[t, p] = sum_l W[l, p] cos(omega_l . xs_t + b_l) at the scaled rows Xs (m, d), and with `grad`
+    S[t, p, j] = sum_l W[l, p] sin(omega_l . xs_t + b_l) omega_lj (else an empty S).  The phase is sum_j omega_lj xs_tj
+    in order j, then + b_l; the sums over l run in order; rows t in parallel."""
+    m, d = Xs.shape
+    L, q = W.shape
+    Fh = np.zeros((m, q))
+    Fl = np.zeros((m, q))
+    ms = m if grad else 0
+    Sh = np.zeros((ms, q, d))
+    Sl = np.zeros((ms, q, d))
+    for t in prange(m):
+        for l in range(L):
+            ph, pl = 0.0, 0.0
+            for j in range(d):
+                xh, xl = two_prod(omega[l, j], Xs[t, j])
+                ph, pl = dd_add(ph, pl, xh, xl)
+            ph, pl = dd_add(ph, pl, b[l], 0.0)
+            ch, cl, sh, sl = dd_cos_sin(ph, pl)
+            for p in range(q):
+                xh, xl = dd_mul_d(ch, cl, W[l, p])
+                Fh[t, p], Fl[t, p] = dd_add(Fh[t, p], Fl[t, p], xh, xl)
+                if grad:
+                    uh, ul = dd_mul_d(sh, sl, W[l, p])
+                    for j in range(d):
+                        vh, vl = dd_mul_d(uh, ul, omega[l, j])
+                        Sh[t, p, j], Sl[t, p, j] = dd_add(Sh[t, p, j], Sl[t, p, j], vh, vl)
+    return Fh, Fl, Sh, Sl
+
+
+@njit(parallel=True, cache=False)
+def _rows_dot(Ah, Al, Bh, Bl):
+    """O[t, p] = sum_i A[t, i] B[p, i] in order i (rows t in parallel)."""
+    m, n = Ah.shape
+    q = Bh.shape[0]
+    Oh = np.zeros((m, q))
+    Ol = np.zeros((m, q))
+    for t in prange(m):
+        for p in range(q):
+            Oh[t, p], Ol[t, p] = _dot(Ah[t], Al[t], Bh[p], Bl[p], 0, n)
+    return Oh, Ol
+
+
+@njit(cache=False)
+def _abs_sums(Vh, Vl):
+    """sum_i |V[p, i]| per row p, in order i."""
+    q, n = Vh.shape
+    out = np.zeros((q, 2))
+    for p in range(q):
+        for i in range(n):
+            h, l = (Vh[p, i], Vl[p, i]) if Vh[p, i] >= 0.0 else (-Vh[p, i], -Vl[p, i])
+            out[p, 0], out[p, 1] = dd_add(out[p, 0], out[p, 1], h, l)
+    return out
+
+
+class Paths:
+    """Posterior sample paths of a Fit (DESIGN.md 4.7, bayesianoptimization_b200/paths.py) on the draws
+    (omega (L, d), b (L,), w (L, q), eps (n, q)) of paths.draw_path_inputs, in double-double:
+
+        Phi(xs) = sqrt(2c/L) cos(omega xs + b)             (no WhiteKernel term: a path is the latent function)
+        V       = K^-1 (y_n - Phi(Xs) w - eps)             (K's diagonal c + white + alpha, as the Fit's)
+        path(x) = s_y (Phi(xs) w + c k(xs, Xs) V) + y_mean
+
+    The cross covariances c k(xs, Xs) carry no WhiteKernel term either.  V is (q, n), a pair."""
+
+    def __init__(self, fit, omega, b, w, eps):
+        mp.mp.dps = 50
+        self.fit = fit
+        self.omega = np.ascontiguousarray(omega, dtype=float)
+        self.b = np.ascontiguousarray(b, dtype=float)
+        self.w = np.ascontiguousarray(w, dtype=float)
+        self.eps = np.asarray(eps, dtype=float)
+        self.fs = mp.sqrt(2 * mp.mpf(fit.c) / self.omega.shape[0])
+        fs = _pair(self.fs)
+        Fh, Fl, _, _ = feature_sums(fit.Xs, self.omega, self.b, self.w, False)
+        q, n = self.w.shape[1], fit.n
+        Rh, Rl = np.empty((q, n)), np.empty((q, n))
+        for p in range(q):
+            for i in range(n):
+                th, tl = dd_mul(Fh[i, p], Fl[i, p], fs[0], fs[1])
+                th, tl = dd_sub(fit.yn[0][i], fit.yn[1][i], th, tl)
+                Rh[p, i], Rl[p, i] = dd_sub(th, tl, self.eps[i, p], 0.0)
+        self.V = solve_rows(fit, Rh, Rl)
+
+    def normalised(self, xs, Ks=None):
+        """Phi(xs) w + c k(xs, Xs) V (mpmath, (m, q) nested lists) at the scaled rows xs; Ks their cross covariances to
+        the training rows when the caller has them."""
+        xs = np.ascontiguousarray(xs)
+        Ks = self.fit.cross(xs) if Ks is None else Ks
+        Fh, Fl, _, _ = feature_sums(xs, self.omega, self.b, self.w, False)
+        Uh, Ul = _rows_dot(Ks[0], Ks[1], self.V[0], self.V[1])
+        return [[to_mp(Fh[t, p], Fl[t, p]) * self.fs + to_mp(Uh[t, p], Ul[t, p]) for p in range(Fh.shape[1])]
+                for t in range(len(Fh))]
+
+    def values(self, xs, Ks=None):
+        """Path values (mpmath, (m, q) nested lists, data units) at the scaled rows xs."""
+        f = self.fit
+        return [[f.y_std * v + f.y_mean for v in row] for row in self.normalised(xs, Ks)]
+
+    def grads(self, xs):
+        """d path / dx (mpmath, (m, q, d) nested lists, unscaled input coordinates) at the scaled rows xs: the feature
+        term through sin, the update term through cross_cov_grad."""
+        f = self.fit
+        xs = np.ascontiguousarray(xs)
+        (m, d), (q, n) = xs.shape, self.V[0].shape
+        _, _, Sh, Sl = feature_sums(xs, self.omega, self.b, self.w, True)
+        Wh = np.ascontiguousarray(np.broadcast_to(self.V[0], (m, q, n)))
+        Wl = np.ascontiguousarray(np.broadcast_to(self.V[1], (m, q, n)))
+        inv_ls = 1.0 / ls_vec(f.case)
+        Gh, Gl = cross_cov_grad(xs, f.Xs, f.code, f.c, inv_ls, Wh, Wl)
+        return [[[f.y_std * (to_mp(Gh[t, p, j], Gl[t, p, j]) - self.fs * to_mp(Sh[t, p, j], Sl[t, p, j]) * inv_ls[j])
+                  for j in range(d)] for p in range(q)] for t in range(m)]
+
+    def v_abs_sums(self):
+        """sum_i |V[p, i]| per path (mpmath)."""
+        return [to_mp(a, b) for a, b in _abs_sums(self.V[0], self.V[1])]
+
+    def bounds(self):
+        """B_p = |y_mean| + s_y (sqrt(2c/L) sum_l |w_lp| + c sum_i |V_pi|) >= |path_p(x)| everywhere (mpmath)."""
+        f = self.fit
+        sv = self.v_abs_sums()
+        return [abs(f.y_mean) + f.y_std * (self.fs * mp.fsum(abs(mp.mpf(float(a))) for a in self.w[:, p])
+                                           + f.c * sv[p]) for p in range(len(sv))]
+
+    def train_identity(self, i, p):
+        """y_mean + s_y (y_n,i - eps_ip - (white + alpha) V_pi): the value of path p at training row i in exact
+        arithmetic (K V = r with K's diagonal c + white + alpha, and c k(X_i, X_i) = c)."""
+        f = self.fit
+        s2 = to_mp(*f.diag) - f.c
+        r = to_mp(f.yn[0][i], f.yn[1][i]) - mp.mpf(self.eps[i, p]) - s2 * to_mp(self.V[0][p, i], self.V[1][p, i])
+        return f.y_mean + f.y_std * r
 
 
 def acquisitions(mu, var, y_max, kappa, xi):
