@@ -281,12 +281,12 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
+    CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_units_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -1379,13 +1379,14 @@ static int predict_pair_grid(b200bo_gp* g0) {
     return B200BO_OK;
 }
 
-// predict_acq16_kernel's bulk-copy phase B flags an mbarrier wait that ran out of its budget (a protocol error)
+// predict_acq16_kernel's bulk-copy phase B and the Gram bound pass flag an mbarrier wait that ran out of its budget (a
+// protocol error)
 static int check_pipe_timeout(b200bo_gp* g0) {
     if (!g0->pipe_armed) return B200BO_OK;
     unsigned long long f = 0;
     CU(cudaSetDevice(g0->device));
     CU(cudaMemcpyFromSymbol(&f, g_pipe_timeout, sizeof(f)));
-    if (f != 0) return set_err(B200BO_ERR_CUDA, "predict_acq16_kernel: a phase B pipeline wait timed out");
+    if (f != 0) return set_err(B200BO_ERR_CUDA, "a bulk-copy pipeline wait (phase B or the Gram bound pass) timed out");
     return B200BO_OK;
 }
 
@@ -1513,33 +1514,40 @@ static int bound_pass_choice(const b200bo_gp* g0, const GpDev& G) {
 }
 
 template <bool F32>
-static void launch_bound_gram(const PredictParams& P, unsigned ntiles, size_t smem, unsigned long long* keys,
-                              int* idx, double* kmax, double2* mu, cudaStream_t stream) {
+static void launch_bound_gram(const PredictParams& P, unsigned long long* keys, int* idx, double* kmax, double2* mu,
+                              cudaStream_t stream) {
+    const unsigned ntiles = (unsigned)((P.m + kGramTile - 1) / kGramTile);
+    const size_t smem = gram_bound_smem(P.d);
     switch (cov_code(P.gp[0].family, P.gp[0].nu)) {
-        case 1: predict_bound_gram_kernel<1, F32><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
-        case 2: predict_bound_gram_kernel<2, F32><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
-        default: predict_bound_gram_kernel<3, F32><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        case 1: predict_bound_gram_kernel<1, F32><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        case 2: predict_bound_gram_kernel<2, F32><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        default: predict_bound_gram_kernel<3, F32><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
     }
 }
 
 // The bound pass of a pruned launch (kBound*; -1: bound_pass_choice): a Gram pass (distances on the fp64 tensor pipe)
 // for every covariance whose dk/d(r^2) is bounded, the direct pass for Matern-0.5 (DESIGN.md 4.9).  mu: [m] interval
-// (mu_lo, mu_hi); idx, kmax may be nullptr.
+// (mu_lo, mu_hi); idx, kmax may be nullptr.  resume: a later launch of a chunked batch, which keeps the timeout flag.
 static int launch_bound_pass(b200bo_gp* g0, PredictParams& P, int pass, unsigned long long* keys, int* idx,
-                             double* kmax, double2* mu, cudaStream_t stream) {
-    const unsigned ntiles = (unsigned)((P.m + PBN - 1) / PBN);
+                             double* kmax, double2* mu, bool resume, cudaStream_t stream) {
     if (cov_code(P.gp[0].family, P.gp[0].nu) == 0) pass = kBoundDirect;
     if (pass != kBoundDirect) {
         int rc;
         if ((rc = ensure_gram(g0, stream))) return rc;
         if (pass < 0) pass = bound_pass_choice(g0, P.gp[0]);
         P.gp[0].gram = g0->gram.as<double>();
-        const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * gram_stride(P.d) + 2 * PA_CHUNK);
+        if (!resume) {  // the operand ring's timeout flag, read by check_pipe_timeout
+            void* flag = nullptr;
+            CU(cudaGetSymbolAddress(&flag, g_pipe_timeout));
+            CU(cudaMemsetAsync(flag, 0, sizeof(unsigned long long), stream));
+            g0->pipe_armed = true;
+        }
         if (pass == kBoundGram32)
-            launch_bound_gram<true>(P, ntiles, smem, keys, idx, kmax, mu, stream);
+            launch_bound_gram<true>(P, keys, idx, kmax, mu, stream);
         else
-            launch_bound_gram<false>(P, ntiles, smem, keys, idx, kmax, mu, stream);
+            launch_bound_gram<false>(P, keys, idx, kmax, mu, stream);
     } else {
+        const unsigned ntiles = (unsigned)((P.m + PBN - 1) / PBN);
         const size_t smem = sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * P.d + 2 * PA_CHUNK);
         if (P.d <= kPredictMaxDimRegs)
             predict_bound_kernel<true><<<ntiles, P16_NT, smem, stream>>>(P, keys, idx, kmax, mu);
@@ -1568,7 +1576,7 @@ static int prune_prepare(b200bo_gp* g0, PredictParams& P, bool resume, cudaStrea
         if ((rc = ensure_gram(g0, stream))) return rc;
         CU(cudaEventRecord(g0->ev0, stream));  // exclude the one-off operand build from the kernel time
     }
-    if ((rc = launch_bound_pass(g0, P, -1, keys, idx, nullptr, g0->prune_mu.as<double2>(), stream))) return rc;
+    if ((rc = launch_bound_pass(g0, P, -1, keys, idx, nullptr, g0->prune_mu.as<double2>(), resume, stream))) return rc;
     CU(cudaEventRecord(g0->ev_stage[0], stream));
     cub::DoubleBuffer<unsigned long long> kb(keys, keys + m);
     cub::DoubleBuffer<int> ib(idx, idx + m);
@@ -2011,7 +2019,7 @@ static int prune_bound_entry(const b200bo_acq* spec, const double* d_Xc, int64_t
     int np_max = 0;
     if ((rc = fill_params(spec, src, m, 0, stream, P, np_max))) return rc;
     return launch_bound_pass(g0, P, pass, reinterpret_cast<unsigned long long*>(d_key), nullptr, d_kmax,
-                             reinterpret_cast<double2*>(d_mu), stream);
+                             reinterpret_cast<double2*>(d_mu), false, stream);
 }
 
 extern "C" int b200bo_acq_prune_bound_dev(const b200bo_acq* spec, const double* d_Xc, int64_t m, uint64_t* d_key,

@@ -20,6 +20,8 @@
 //     the fraction is a measured choice (DESIGN.md 6), not "keep it all".
 // Selected with B200BO_PREDICT_WARPS=16 (A/B measurements decide the default, see DESIGN.md).
 #pragma once
+#include <type_traits>
+
 #include "predict_kernels.cuh"
 
 namespace b200bo {
@@ -121,6 +123,13 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictPara
     }
 }
 
+// failed polls before a wait gives up: seconds, against microseconds for a stage to arrive from L2 or HBM
+constexpr uint32_t kPipeWaitBudget = 1u << 28;
+// set by a ring wait (the bulk-copy phase B, the Gram bound pass) that ran out of its budget; the host reports it as an
+// error and clears it before every launch.  A global, not a launch parameter, so that the k-loop holds no register for
+// it.
+__device__ unsigned long long g_pipe_timeout;
+
 // ---- selection-only pruning: the Gram bound pass (DESIGN.md 4.9) ----------------------------------------------------
 // The direct pass spends about 40 % (d = 16) to 55 % (d = 32) of its fp64 instructions per (candidate, training row)
 // pair on the distance.  Here the distance comes from the fp64 tensor pipe in the Gram form
@@ -167,13 +176,35 @@ __host__ __device__ inline int gram_stride(int d) {
 //   fp32 mu partial of the kernel (alpha_ rounded to fp32, four fused products: 6 u relative to sum |alpha_ k~|).
 //   tests/test_prune_f32_cpu.py restates this with rsqrtf and exp2f perturbed to their documented error and
 //   tests/test_gpu_prune_f32.py checks the device function exhaustively over its fp32 arguments.
+// sqrt and exp2 run as rsqrt.approx.ftz and ex2.approx.ftz: on the clamped domain their arguments and results are
+// normal fp32 numbers, where these return the same bits as rsqrtf / exp2f without the denormal guards around them.
 template <int COV>
 struct CovF32 {
     static constexpr float r2max = COV == 1 ? 2300.f : COV == 2 ? 1400.f : 166.f;
     static constexpr float rel = COV == 1 ? 24.f : COV == 2 ? 32.f : 12.f;  // R, the mu partial included
     static constexpr float qz = COV == 3 ? 4.f : 8.f;                       // Q
+    // the exp2 argument per unit s (RBF) or r (Matern): -log2e / 2, -sqrt3 log2e, -sqrt5 log2e
+    static constexpr float ex2c = COV == 1 ? -2.49882102012634277344f
+                                  : COV == 2 ? -3.22596406936645507812f
+                                             : -0.72134751081466674805f;
 };
+// Conditions for the ftz forms: s >= 2^-100 keeps rsqrt's argument and result normal, and at s = r2max the exp2
+// argument (-119.8, -120.7, -119.7 for Matern-1.5, Matern-2.5, RBF) stays above -126, so 2^(...) is normal too
+static_assert(CovF32<3>::r2max * CovF32<3>::ex2c > -126.f, "RBF: exp2 argument below the normal range");
+static_assert(CovF32<1>::r2max * CovF32<1>::ex2c * CovF32<1>::ex2c < 126.f * 126.f, "Matern-1.5: exp2 argument");
+static_assert(CovF32<2>::r2max * CovF32<2>::ex2c * CovF32<2>::ex2c < 126.f * 126.f, "Matern-2.5: exp2 argument");
 constexpr double kF32Abs = 1e-30;  // the clamps, per unit covariance
+
+__device__ __forceinline__ float rsqrt_ftz(float x) {
+    float y;
+    asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+__device__ __forceinline__ float ex2_ftz(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
 
 // k~ of one pair from r~^2 (fp64); z: the exp argument's magnitude (natural units)
 template <int COV>
@@ -181,16 +212,16 @@ __device__ __forceinline__ float cov_f32(double r2, float& z) {
     const float s = fminf(fmaxf(__double2float_rn(r2), 0x1p-100f), CovF32<COV>::r2max);
     if (COV == 3) {
         z = 0.5f * s;
-        return exp2f(s * -0.72134751081466674805f);  // -log2e / 2
+        return ex2_ftz(s * CovF32<COV>::ex2c);
     }
-    const float r = s * rsqrtf(s);
+    const float r = s * rsqrt_ftz(s);
     if (COV == 2) {
-        z = r * 2.23606801033020019531f;                  // sqrt5
-        const float e = exp2f(r * -3.22596406936645507812f);  // -sqrt5 log2e
+        z = r * 2.23606801033020019531f;  // sqrt5
+        const float e = ex2_ftz(r * CovF32<COV>::ex2c);
         return fmaf(fmaf(z, 0.33333334326744079590f, 1.f), z, 1.f) * e;
     }
-    z = r * 1.73205077648162841797f;                  // sqrt3
-    const float e = exp2f(r * -2.49882102012634277344f);  // -sqrt3 log2e
+    z = r * 1.73205077648162841797f;  // sqrt3
+    const float e = ex2_ftz(r * CovF32<COV>::ex2c);
     return (1.f + z) * e;
 }
 
@@ -242,11 +273,69 @@ __global__ void __launch_bounds__(1024) gram_stats_kernel(const double* __restri
     }
 }
 
-// One CTA per tile of PBN candidates.  Warp w owns candidates (w & 3) * 32 .. +32 and rows (w >> 2) * 16 .. +16 of
-// every PA_CHUNK-row chunk: 2 x 2 m16n8k4 tiles (m: candidates, n: training rows) over ceil(K / 4) k-steps.  Thread
-// (g, t4) accumulates candidates i * 8 + g (i < 4) of its warp over rows 2 t4, 2 t4 + 1 (+ 8) of its slab; the partials
-// are added over the quad, then over the four row slabs in a fixed order.  Outputs as predict_bound_kernel's;
-// mu_out gets (mu_lo, mu_hi) and kmax_out kmax_lb.
+// The chunks of the Gram operand reach shared memory through a ring of kGramSlots slots, each a bulk copy of the
+// chunk's PA_CHUNK operand rows and alpha_ words (fp32 for the fp32 pass, fp64 otherwise) completing on the slot's
+// mbarrier, as phase B's PIPE_BULK ring: every warp counts its consumption of a slot, and the last of the 8 refills it
+// with the chunk kGramSlots ahead.  No CTA barrier separates the chunks, so warps drift up to kGramSlots - 1 chunks
+// apart and one warp's DMMAs issue while another's covariances do.  A CTA is 8 warps over a tile of kGramTile
+// candidates, so that several CTAs (3 at d <= 16 in the fp32 pass, at most 80 registers) share an SM and hide each
+// other's latencies, prologue and epilogue.  4 slots fit at d = B200BO_MAX_DIM.
+constexpr int kGramSlots = 4, kGramTile = 64, kGramNT = 256;
+__host__ __device__ inline size_t gram_slot_doubles(int d) { return (size_t)PA_CHUNK * (gram_stride(d) + 1); }
+// dynamic shared memory of predict_bound_gram_kernel: the candidate operand [kGramTile][stride], then the ring
+__host__ __device__ inline size_t gram_bound_smem(int d) {
+    return sizeof(double) * ((size_t)kGramTile * gram_stride(d) + kGramSlots * gram_slot_doubles(d));
+}
+
+// The covariance, mu partial and |k| maximum of one thread's 16 pairs of a chunk (acc[mi][ni][e]: candidate
+// (2 mi + (e >> 1)) * 8 + g, row ni * 8 + 2 t4 + (e & 1) of the warp's slab).  MASK: the slab holds rows >= n, whose
+// covariance is taken as 0; only the last chunks can.
+template <int COV, bool F32, bool MASK>
+__device__ __forceinline__ void gram_chunk_cov(const double (&acc)[2][2][4], int nrow, const double* al,
+                                               const float* alf, double (&macc)[4], double (&kmx)[4],
+                                               float (&kmxf)[4], float (&wsum)[4]) {
+    if constexpr (F32) {
+        float mp[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
+                    float z;
+                    float k = cov_f32<COV>(acc[mi][ni][e], z);
+                    if (MASK && r >= nrow) k = 0.f;
+                    const float a = alf[r];
+                    const float w = fmaf(z, CovF32<COV>::qz, CovF32<COV>::rel);
+                    mp[i] = fmaf(a, k, mp[i]);
+                    wsum[i] = fmaf(fabsf(a) * k, w, wsum[i]);
+                    kmxf[i] = fmaxf(kmxf[i], fmaf(k * -0x1p-24f, w, k));
+                }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) macc[i] += (double)mp[i];
+    } else {
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
+                    double k = cov_eval<COV>(acc[mi][ni][e]);
+                    if (MASK && r >= nrow) k = 0.0;
+                    macc[i] = fma(al[r], k, macc[i]);
+                    kmx[i] = fmax(kmx[i], k);
+                }
+    }
+}
+
+// One CTA per tile of kGramTile candidates.  Warp w owns candidates (w & 1) * 32 .. +32 and rows (w >> 1) * 16 .. +16
+// of every PA_CHUNK-row chunk: 2 x 2 m16n8k4 tiles (m: candidates, n: training rows) over ceil(K / 4) k-steps.  Thread
+// (g, t4) accumulates candidates i * 8 + g (i < 4) of its warp over rows 2 t4, 2 t4 + 1 (+ 8) of its slab, chunks in
+// ascending order; the partials are added over the quad, then over the four row slabs in a fixed order.  Outputs as
+// predict_bound_kernel's; mu_out gets (mu_lo, mu_hi) and kmax_out kmax_lb.  A ring wait that runs out of its budget
+// sets g_pipe_timeout.
 // F32: the covariance in fp32 (cov_f32).  Per thread and chunk the four alpha_ k~ products of a candidate are summed in
 // fp32 and then added to the fp64 partial; W = sum_i |alpha_i| k~_i (R + Q z~_i) (fp32) carries the relative part of
 // the margin, and the |k| maximum is taken over k~_i (1 - u (R + Q z~_i)), a lower bound of the row's exact k:
@@ -254,51 +343,59 @@ __global__ void __launch_bounds__(1024) gram_stats_kernel(const double* __restri
 //   kmax_lb = constv (max_i k~_i (1 - u (R + Q z~_i))) (1 - 2^-22) - constv (Lip dr2 + 64 u53 + kF32Abs)
 // (every fp32 sum of positive terms is within (np + 16) 2^-23 of its value; 2^-22 covers the rounding of the product).
 template <int COV, bool F32>
-__global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const PredictParams P, unsigned long long* keys,
-                                                                    int* idx, double* kmax_out, double2* mu_out) {
+__global__ void __launch_bounds__(kGramNT, F32 ? 3 : 2)
+    predict_bound_gram_kernel(const PredictParams P, unsigned long long* keys, int* idx, double* kmax_out,
+                              double2* mu_out) {
     static_assert(COV != 0, "Matern-0.5 has no Lipschitz bound in r^2");
     constexpr double lip = COV == 1 ? 1.5 : COV == 2 ? 5.0 / 6.0 : 0.5;
     extern __shared__ __align__(16) double smem[];
-    __shared__ double mu_s[4][PBN];
-    __shared__ double kmax_s[4][PBN];
-    __shared__ double w_s[F32 ? 4 : 1][PBN];
+    __shared__ double mu_s[4][kGramTile];
+    __shared__ double kmax_s[4][kGramTile];
+    __shared__ double w_s[F32 ? 4 : 1][kGramTile];
+    __shared__ uint64_t full_bar[kGramSlots];
+    __shared__ unsigned done_cnt[kGramSlots];
     const GpDev& G = P.gp[0];
     const int tid = threadIdx.x, d = P.d, str = gram_stride(d), nks = (d + 2 + 3) / 4;
-    const long long c0 = (long long)blockIdx.x * PBN;
-    double* xa_s = smem;                          // [PBN][str]: [x | |x|^2 | 1 | 0 ...]
-    double* xb_s = smem + (size_t)PBN * str;      // [2][PA_CHUNK][str]
-    double* al_s = xb_s + (size_t)2 * PA_CHUNK * str;  // [2][PA_CHUNK] (fp64), or [2][PA_CHUNK] floats (F32)
-    for (int q = tid; q < PBN * str; q += P16_NT) {
+    const long long c0 = (long long)blockIdx.x * kGramTile;
+    double* xa_s = smem;                            // [kGramTile][str]: [x | |x|^2 | 1 | 0 ...]
+    double* ring = smem + (size_t)kGramTile * str;  // slot s: [PA_CHUNK][str] operand rows, then PA_CHUNK alpha_ words
+    const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax, then alpha_ in fp32
+    const int nch = G.np / PA_CHUNK;
+    // one thread: chunk ch into the free slot s
+    auto copy = [&](int ch, int s) {
+        constexpr uint32_t abytes = PA_CHUNK * (F32 ? sizeof(float) : sizeof(double));
+        const uint32_t obytes = PA_CHUNK * str * sizeof(double);
+        double* dst = ring + s * gram_slot_doubles(d);
+        tc::mbar_arrive_expect_tx(&full_bar[s], obytes + abytes);
+        tc::bulk_g2s(dst, G.gram + (size_t)ch * PA_CHUNK * str, obytes, &full_bar[s]);
+        const void* asrc = F32 ? (const void*)(reinterpret_cast<const float*>(stats + 2) + (size_t)ch * PA_CHUNK)
+                               : (const void*)(G.alphav + (size_t)ch * PA_CHUNK);
+        tc::bulk_g2s(dst + PA_CHUNK * str, asrc, abytes, &full_bar[s]);
+    };
+    if (tid == 0) {  // the first chunks load while the candidates are built
+        for (int s = 0; s < kGramSlots; ++s) {
+            tc::mbar_init(&full_bar[s], 1);
+            done_cnt[s] = 0;
+        }
+        tc::mbar_fence_init();
+        for (int s = 0; s < kGramSlots && s < nch; ++s) copy(s, s);
+    }
+    for (int q = tid; q < kGramTile * str; q += kGramNT) {
         const int c = q / str, j = q - c * str;
         const long long gi = c0 + c;
         double v = j == d + 1 ? 1.0 : 0.0;
         if (j < d && gi < P.m) v = scale_input(candidate_coord(P, gi, j), G.xform, G.ls, j);  // as phase A builds them
         xa_s[q] = v;
     }
-    const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax, then alpha_ in fp32
-    auto load_chunk = [&](int buf, int ch) {
-        const double* src = G.gram + (size_t)ch * PA_CHUNK * str;
-        double* dst = xb_s + (size_t)buf * PA_CHUNK * str;
-        for (int q = tid; q < PA_CHUNK * str / 2; q += P16_NT) cp_async16_cg(dst + 2 * q, src + 2 * q);
-        if (F32) {
-            if (tid < PA_CHUNK / 4)
-                cp_async16_cg(reinterpret_cast<float*>(al_s) + buf * PA_CHUNK + 4 * tid,
-                              reinterpret_cast<const float*>(stats + 2) + (size_t)ch * PA_CHUNK + 4 * tid);
-        } else if (tid < PA_CHUNK / 2) {
-            cp_async16_cg(al_s + buf * PA_CHUNK + 2 * tid, G.alphav + (size_t)ch * PA_CHUNK + 2 * tid);
-        }
-    };
-    const int nch = G.np / PA_CHUNK;
-    load_chunk(0, 0);
-    cp_async_commit();
     __syncthreads();  // coordinates visible
-    if (tid < PBN) {
+    if (tid < kGramTile) {
         double x2 = 0.0;
         for (int j = 0; j < d; ++j) x2 = fma(xa_s[tid * str + j], xa_s[tid * str + j], x2);
         xa_s[tid * str + d] = x2;
     }
+    __syncthreads();  // norms |x|^2 and the ring's barriers visible
     const int lane = tid & 31, warp = tid >> 5, g = lane >> 2, t4 = lane & 3;
-    const int cg = warp & 3, rg = warp >> 2;
+    const int cg = warp & 1, rg = warp >> 1;
     const double* xa = xa_s + (size_t)(cg * 32 + g) * str + t4;
     double macc[4], kmx[4];
     float kmxf[4], wsum[4];
@@ -307,14 +404,12 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
         macc[i] = kmx[i] = 0.0;
         kmxf[i] = wsum[i] = 0.f;
     }
-    for (int ch = 0; ch < nch; ++ch) {
-        if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
-        cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();  // chunk ch (and, at ch = 0, the norms |x|^2) visible
-        const double* xb = xb_s + (size_t)(ch & 1) * PA_CHUNK * str + (size_t)(rg * 16 + g) * str + t4;
-        const double* al = al_s + (ch & 1) * PA_CHUNK + rg * 16 + 2 * t4;
-        const float* alf = reinterpret_cast<const float*>(al_s) + (ch & 1) * PA_CHUNK + rg * 16 + 2 * t4;
+    // chunk ch through the DMMA Gram product and the covariance section; MASK: the chunk holds rows >= n
+    auto chunk = [&](int ch, auto mask) {
+        const int s = ch % kGramSlots;
+        tc::mbar_wait_budget(&full_bar[s], (uint32_t)(ch / kGramSlots) & 1u, &g_pipe_timeout, kPipeWaitBudget);
+        const double* buf = ring + s * gram_slot_doubles(d);
+        const double* xb = buf + (size_t)(rg * 16 + g) * str + t4;
         double acc[2][2][4];
 #pragma unroll
         for (int mi = 0; mi < 2; ++mi)
@@ -322,6 +417,7 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
             for (int ni = 0; ni < 2; ++ni)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) acc[mi][ni][e] = 0.0;
+#pragma unroll 1  // unrolled, the k-steps take the registers that a third CTA per SM needs
         for (int ks = 0; ks < nks; ++ks) {
             double a[4], b[2];
 #pragma unroll
@@ -335,45 +431,25 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
                     dmma1684(acc[mi][ni][0], acc[mi][ni][1], acc[mi][ni][2], acc[mi][ni][3], a[2 * mi],
                              a[2 * mi + 1], b[ni]);
         }
-        // acc[mi][ni][e]: candidate (2 mi + (e >> 1)) * 8 + g, row ni * 8 + 2 t4 + (e & 1) of the slab
-        const int row0 = ch * PA_CHUNK + rg * 16 + 2 * t4;
-        if constexpr (F32) {
-            float mp[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
-                        float z;
-                        float k = cov_f32<COV>(acc[mi][ni][e], z);
-                        if (row0 + r >= G.n) k = 0.f;
-                        const float a = alf[r];
-                        const float w = fmaf(z, CovF32<COV>::qz, CovF32<COV>::rel);
-                        mp[i] = fmaf(a, k, mp[i]);
-                        wsum[i] = fmaf(fabsf(a) * k, w, wsum[i]);
-                        kmxf[i] = fmaxf(kmxf[i], fmaf(k * -0x1p-24f, w, k));
-                    }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) macc[i] += (double)mp[i];
-        } else {
-#pragma unroll
-            for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int i = 2 * mi + (e >> 1), r = ni * 8 + (e & 1);
-                        double k = cov_eval<COV>(acc[mi][ni][e]);
-                        if (row0 + r >= G.n) k = 0.0;
-                        macc[i] = fma(al[r], k, macc[i]);
-                        kmx[i] = fmax(kmx[i], k);
-                    }
+        const double* al = buf + PA_CHUNK * str + rg * 16 + 2 * t4;
+        const float* alf = reinterpret_cast<const float*>(buf + PA_CHUNK * str) + rg * 16 + 2 * t4;
+        const int nrow = G.n - (ch * PA_CHUNK + rg * 16 + 2 * t4);  // slab rows r < nrow of this thread are < n
+        gram_chunk_cov<COV, F32, decltype(mask)::value>(acc, nrow, al, alf, macc, kmx, kmxf, wsum);
+        __syncwarp();
+        if (lane == 0) {
+            __threadfence_block();  // this warp's reads of slot s happen before its count
+            if ((atomicAdd(&done_cnt[s], 1u) & 7u) == 7u) {  // last of the 8 warps: refill with chunk ch + kGramSlots
+                __threadfence_block();
+                tc::fence_proxy_async_smem();
+                if (ch + kGramSlots < nch) copy(ch + kGramSlots, s);
+            }
         }
-        __syncthreads();  // chunk buffer free for the prefetch of chunk ch+2
-    }
-    cp_async_wait<0>();
+    };
+    // the chunks below n / PA_CHUNK hold no padded row; the mask stays out of their loop (and its code size)
+    const int nfull = G.n / PA_CHUNK;
+    int ch = 0;
+    for (; ch < nfull; ++ch) chunk(ch, std::false_type{});
+    for (; ch < nch; ++ch) chunk(ch, std::true_type{});
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         if (F32) {
@@ -393,7 +469,7 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_gram_kernel(const Predic
     }
     __syncthreads();
     const int c = tid;
-    if (c < PBN && c0 + c < P.m) {
+    if (c < kGramTile && c0 + c < P.m) {
         const double u = 0x1p-53;
         const double gk = (d + 2) * u / (1.0 - (d + 2) * u), gn = G.np * u / (1.0 - G.np * u);
         const double dr2 = __dmul_ru(kGramCg * gk, __dadd_ru(xa_s[c * str + d], stats[1]));
@@ -626,11 +702,6 @@ __global__ void __launch_bounds__(256) pad_linv_stages_kernel(const double* __re
 }
 
 enum { PIPE_CPASYNC = 0, PIPE_BULK = 1, PIPE_BULK_MC = 2 };
-// failed polls before a wait gives up: seconds, against microseconds for a stage to arrive from L2 or HBM
-constexpr uint32_t kPipeWaitBudget = 1u << 28;
-// set by a wait of the bulk-copy phase B that ran out of its budget; the host reports it as an error and clears it
-// before every launch.  A global, not a launch parameter, so that the k-loop holds no register for it.
-__device__ unsigned long long g_pipe_timeout;
 
 template <bool MC>
 __device__ __forceinline__ void pipe_barrier() {
