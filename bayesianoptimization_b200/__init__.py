@@ -11,8 +11,8 @@ Two layers:
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, LogExpectedImprovement,
     LogProbabilityOfImprovement, NoisyExpectedImprovement, LogNoisyExpectedImprovement, ThompsonSampling,
-    ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, KrigingBeliever, GPHedge, AcquisitionFunction,
-    ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
+    ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, KrigingBeliever, PendingNEI, GPHedge,
+    AcquisitionFunction, ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
 """
 from . import _lib
 from ._build import build_library
@@ -30,7 +30,7 @@ _PLUGIN = {
     "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
     "MaxValueEntropySearch": "acquisition", "suggest_batch": "acquisition", "KrigingBeliever": "acquisition",
     "NoisyExpectedImprovement": "acquisition", "LogNoisyExpectedImprovement": "acquisition",
-    "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
+    "PendingNEI": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
 }
 
 

@@ -36,7 +36,7 @@ EXPORTS = [
     "b200bo_paths_argmin_topk_philox", "b200bo_paths_bound", "b200bo_cpaths_eval", "b200bo_cpaths_argmin_topk",
     "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
     "b200bo_acq_value_grad", "b200bo_paths_grad_rows", "b200bo_gp_fork", "b200bo_gp_condition",
-    "b200bo_gp_set_fantasies",
+    "b200bo_gp_set_fantasies", "b200bo_gp_condition_fantasies",
 ]
 
 
@@ -128,6 +128,7 @@ def lib():
     L.b200bo_gp_replicate.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_void_p)]
     L.b200bo_gp_fork.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_void_p)]
     L.b200bo_gp_condition.argtypes = [C.c_void_p, dp, C.c_int64, dp]
+    L.b200bo_gp_condition_fantasies.argtypes = [C.c_void_p, dp, C.c_int64, dp, dp, dp]
     L.b200bo_multi_gpu_acq_argmin_topk.argtypes = [C.POINTER(AcqSpec), C.c_int, dp, C.c_int64, C.c_int, dp,
                                                    i64p, dp, i64p]
     L.b200bo_multi_gpu_acq_argmin_topk_philox.argtypes = [C.POINTER(AcqSpec), C.c_int, C.c_uint64, dp, dp,

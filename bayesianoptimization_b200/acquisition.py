@@ -21,7 +21,8 @@ ranked and refined through the same three hooks.  ``ConstrainedThompsonSampling`
 from q paths (batch Thompson sampling).  ``MaxValueEntropySearch`` is the
 information-based policy: samples of the maximum from posterior paths, then a fused-kernel epilogue of mu and sigma.
 ``KrigingBeliever`` gives UCB / EI / PoI / MES pending points and batches: the fitted GP is conditioned on the points in
-flight on the device, with its own mean as their targets.  ``LogExpectedImprovement`` and
+flight on the device, with its own mean as their targets; ``PendingNEI`` does the same for noisy EI by drawing the
+pending values jointly with its fantasies.  ``LogExpectedImprovement`` and
 ``LogProbabilityOfImprovement`` are EI and PoI in log space, finite and well scaled where EI and PoI underflow.
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
@@ -490,20 +491,20 @@ def distinct_picks(picks, tops):
 
 def suggest_batch(optimizer, q):
     """q parameter dicts to probe next from a ``bayes_opt.BayesianOptimization`` whose acquisition function is a
-    (Constrained)ThompsonSampling or a KrigingBeliever: ``BayesianOptimization.suggest`` for a batch
+    (Constrained)ThompsonSampling, a KrigingBeliever or a PendingNEI: ``BayesianOptimization.suggest`` for a batch
     (R/bayes_opt/bayesian_optimization.py:323-333).  With no registered point it returns ``optimizer.random_sample(q)``;
     otherwise the acquisition's ``suggest_batch`` with the optimizer's GP, target space and RandomState, each row
     converted with ``array_to_params``.  For Thompson sampling nothing new enters ``save_state`` (q is an argument, not
-    state); a KrigingBeliever records the q points as dummies, which ``save_state`` carries."""
+    state); a KrigingBeliever or PendingNEI records the q points as dummies, which ``save_state`` carries."""
     acq = optimizer._acquisition_function
-    if isinstance(acq, KrigingBeliever):
+    if isinstance(acq, _PendingBatch):
         q = _check_int("q", q, 1)
     elif isinstance(acq, ThompsonSampling):
         q = _check_int("q", q, 1, B.MAX_PATHS)
     else:
-        raise TypeError(f"suggest_batch needs a ThompsonSampling, ConstrainedThompsonSampling or KrigingBeliever "
-                        f"acquisition function, got {type(acq).__name__}; for a batch of other acquisition functions "
-                        f"use ConstantLiar")
+        raise TypeError(f"suggest_batch needs a ThompsonSampling, ConstrainedThompsonSampling, KrigingBeliever or "
+                        f"PendingNEI acquisition function, got {type(acq).__name__}; for a batch of other acquisition "
+                        f"functions use ConstantLiar")
     space = optimizer._space
     if len(space) == 0:
         return optimizer.random_sample(q)
@@ -606,7 +607,7 @@ class _NoisyEI(_SuggestStream, DeviceHooks, _ref.ExpectedImprovement):
     The incumbent of each fantasy is its largest value over ``target_space.mask`` (the rows ``_target_max`` uses).
     Parameters, y_max, the xi decay and saved state are ExpectedImprovement's, plus ``n_samples`` (S, 1..16) and
     ``jitter`` (tau = min(alpha, jitter) on the noiseless GP's diagonal).  Constraints enter as for EI / LogEI.
-    Not inside KrigingBeliever, ConstantLiar or GPHedge; one device."""
+    Not inside KrigingBeliever, ConstantLiar or GPHedge (pending points and batches: ``PendingNEI``); one device."""
 
     _nei_kind = None
 
@@ -633,9 +634,14 @@ class _NoisyEI(_SuggestStream, DeviceHooks, _ref.ExpectedImprovement):
         if space is None:
             raise RuntimeError(f"{type(self).__name__} draws its fantasies against the target space of suggest(): "
                                "build its closure through suggest()")
+        return self._closure(gp, constraint, space)
+
+    def _closure(self, gp, constraint, space, pending=None, extra_rows=0):
+        """The closure over fantasies drawn from the suggest() stream; ``pending`` / ``extra_rows`` as in
+        ``noiseless_fantasies`` (PendingNEI)."""
         self.fantasies = None  # the previous closure's fantasies are not needed past this point
         fant = gp.noiseless_fantasies(self.n_samples, self.jitter, incumbent=np.asarray(space.mask, dtype=bool),
-                                      random_state=self._suggest_rng())
+                                      random_state=self._suggest_rng(), pending=pending, extra_rows=extra_rows)
         self.fantasies = fant
         return FusedAcquisition(self._nei_kind, gp, constraint, owner=self, fantasies=fant)
 
@@ -689,7 +695,8 @@ def accelerate(acq, candidate_source=None, refine=None):
     if refine not in (None, "stencil", "analytic"):
         raise ValueError("refine must be 'stencil' or 'analytic'")
     if isinstance(acq, _ref.ConstantLiar):
-        _refuse_nei(acq.base_acquisition, type(acq).__name__)
+        if not isinstance(acq, PendingNEI):
+            _refuse_nei(acq.base_acquisition, type(acq).__name__)
         acq.base_acquisition = accelerate(acq.base_acquisition, candidate_source, refine)
         return acq
     if isinstance(acq, _ref.GPHedge):
@@ -728,52 +735,18 @@ class GPHedge(_ref.GPHedge):
         super().__init__([accelerate(a) for a in base_acquisitions], *args, **kwargs)
 
 
-class KrigingBeliever(_ref.ConstantLiar):
-    """Batches and asynchronous suggestions for UCB, EI, PoI and MES: the fixed-hyper-parameter counterpart of
-    ``ConstantLiar`` (Kriging believer: Ginsbourger, Le Riche & Carraro, "Kriging is well-suited to parallelize
-    optimization", 2010; DESIGN.md 4.11).
-
-    A pending point - suggested, not yet registered - is a dummy, with ConstantLiar's bookkeeping (inherited:
-    ``dummies``, their expiry once a registered point is within atol / rtol, and get/set_acquisition_params, so
-    ``save_state`` carries them).  Where ConstantLiar registers the dummies with a made-up target and refits the GP on
-    that space, this class fits the hyper-parameters on the registered data only and then conditions the fitted GP on
-    the dummies with the GP's own posterior mean as their targets (``condition_on_pending``: one O(N^2) row update per
-    point on the device).  The mean is unchanged; the standard deviation shrinks near the dummies, so the base
-    acquisition turns away from them.  ``strategy`` is accepted for ConstantLiar's parameter layout and not used.
-
-    ``suggest()``: the base acquisition's own ``suggest`` (its empty-space error, one ``i += 1``, its y_max, its
-    kappa / xi decay) with the GP conditioned on the unexpired dummies between the fit and the closure; the pick
-    becomes a dummy.  ``suggest_batch(..., q)``: q points from one call by greedy rounds on one candidate set.
-    Constraints raise ConstraintNotSupportedError, as ConstantLiar does."""
-
-    def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
-        _refuse_nei(base_acquisition, "KrigingBeliever")
-        if _device_kind(base_acquisition) is None and not isinstance(base_acquisition, MaxValueEntropySearch):
-            raise TypeError(f"KrigingBeliever needs an UpperConfidenceBound, ExpectedImprovement, "
-                            f"ProbabilityOfImprovement, LogExpectedImprovement, LogProbabilityOfImprovement or "
-                            f"MaxValueEntropySearch base acquisition, got {type(base_acquisition).__name__}")
-        super().__init__(accelerate(base_acquisition), strategy, random_state, atol, rtol)
+class _PendingBatch(_ref.ConstantLiar):
+    """ConstantLiar's dummy bookkeeping (``dummies``, their expiry within atol / rtol of a registered point, and
+    get/set_acquisition_params, so ``save_state`` carries them) with the base acquisition's own ``suggest`` and greedy
+    batch rounds on one candidate set.  Subclasses say how the dummies and the picks enter the closure
+    (``_round_closure``); KrigingBeliever conditions the GP, PendingNEI the NEI fantasies."""
 
     def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
         return self._believe(gp, target_space, None, n_random, n_smart, fit_gp, random_state)
 
-    def suggest_batch(self, gp, target_space, q, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
-        """q points to probe next, as a (q, dim) array.  In this order:
-          1. the base acquisition's ``suggest`` accounting, once for the batch (one ``i += 1``, one kappa / xi decay;
-             y_max is the registered data's for every round), the hyper-parameter fit on the registered data, then
-             the conditioning on the unexpired dummies, on a fork of the GP with room for the batch;
-          2. the base closure on that GP - MES draws its y* samples here, once per batch;
-          3. ONE candidate set shared by every round: ``space.random_sample(max(n_random, n_smart), rs)``, or one
-             Philox seed in device_philox mode;
-          4. per round j = 0..q-1: the fused selection over that set on round j's GP, the refinement of its top
-             n_smart (the L-BFGS-B runs in lockstep; mixed-integer spaces: the reference's DE branch), the reference's
-             random-vs-refined rule, the duplicate rule of ``distinct_picks`` against the earlier picks, then the GP
-             is conditioned in place on the pick;
-          5. the q picks become dummies.
-        q = 1 without dummies returns the base acquisition's ``suggest`` point and leaves the RandomState as it does.
-        q is an integer >= 1."""
-        q = _check_int("q", q, 1)
-        return self._believe(gp, target_space, q, n_random, n_smart, fit_gp, random_state)
+    def _round_closure(self, gp, constraint, pending, q):
+        """(closure of round 0 over the dummies ``pending``, callable that extends it in place by one pick (d,))."""
+        raise NotImplementedError
 
     def _believe(self, gp, target_space, q, n_random, n_smart, fit_gp, random_state):
         if len(target_space) == 0:
@@ -785,17 +758,15 @@ class KrigingBeliever(_ref.ConstantLiar):
         self._remove_expired_dummies(target_space)
         base = self.base_acquisition
         pending = np.asarray(self.dummies, dtype=np.float64).reshape(len(self.dummies), target_space.dim)
-        round_gp = []
+        extend = []
 
         def get_acq(gp, constraint=None):  # between the base's fit and its closure
-            gp = _as_b200_gp(gp)
-            if len(pending) or (q or 1) > 1:
-                gp = gp.condition_on_pending(pending, extra_rows=q or 0)
-            round_gp.append(gp)
-            return type(base)._get_acq(base, gp=gp, constraint=constraint)
+            acq, ext = self._round_closure(_as_b200_gp(gp), constraint, pending, q)
+            extend.append(ext)
+            return acq
 
         def acq_min(acq, space, random_state, n_random=10_000, n_smart=10):
-            return self._rounds(acq, round_gp[0], space, random_state, n_random, n_smart, q)
+            return self._rounds(acq, extend[0], space, random_state, n_random, n_smart, q)
 
         base._get_acq = get_acq
         if q is not None:
@@ -812,7 +783,7 @@ class KrigingBeliever(_ref.ConstantLiar):
             self.dummies.extend(np.array(r) for r in x)
         return x
 
-    def _rounds(self, acq, gp, space, random_state, n_random, n_smart, q):
+    def _rounds(self, acq, extend, space, random_state, n_random, n_smart, q):
         if n_random == 0 and n_smart == 0:
             raise ValueError("Either n_random or n_smart needs to be greater than 0.")
         base = self.base_acquisition
@@ -842,8 +813,95 @@ class KrigingBeliever(_ref.ConstantLiar):
             x = distinct_picks(picks + [x], [[]] * len(picks) + [tops])[-1]
             picks.append(np.asarray(x, dtype=np.float64))
             if j < q - 1:
-                gp.condition_on_pending(picks[-1][None])  # in place: the fork has room for the batch
+                extend(picks[-1])  # in place: the closure has room for the batch
         return np.asarray(picks, dtype=np.float64)
+
+
+class KrigingBeliever(_PendingBatch):
+    """Batches and asynchronous suggestions for UCB, EI, PoI and MES: the fixed-hyper-parameter counterpart of
+    ``ConstantLiar`` (Kriging believer: Ginsbourger, Le Riche & Carraro, "Kriging is well-suited to parallelize
+    optimization", 2010; DESIGN.md 4.11).
+
+    A pending point - suggested, not yet registered - is a dummy, with ConstantLiar's bookkeeping (inherited:
+    ``dummies``, their expiry once a registered point is within atol / rtol, and get/set_acquisition_params, so
+    ``save_state`` carries them).  Where ConstantLiar registers the dummies with a made-up target and refits the GP on
+    that space, this class fits the hyper-parameters on the registered data only and then conditions the fitted GP on
+    the dummies with the GP's own posterior mean as their targets (``condition_on_pending``: one O(N^2) row update per
+    point on the device).  The mean is unchanged; the standard deviation shrinks near the dummies, so the base
+    acquisition turns away from them.  ``strategy`` is accepted for ConstantLiar's parameter layout and not used.
+
+    ``suggest()``: the base acquisition's own ``suggest`` (its empty-space error, one ``i += 1``, its y_max, its
+    kappa / xi decay) with the GP conditioned on the unexpired dummies between the fit and the closure; the pick
+    becomes a dummy.  ``suggest_batch(..., q)``: q points from one call by greedy rounds on one candidate set.
+    Constraints raise ConstraintNotSupportedError, as ConstantLiar does.  Noisy EI: ``PendingNEI``."""
+
+    def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
+        _refuse_nei(base_acquisition, "KrigingBeliever")
+        if _device_kind(base_acquisition) is None and not isinstance(base_acquisition, MaxValueEntropySearch):
+            raise TypeError(f"KrigingBeliever needs an UpperConfidenceBound, ExpectedImprovement, "
+                            f"ProbabilityOfImprovement, LogExpectedImprovement, LogProbabilityOfImprovement or "
+                            f"MaxValueEntropySearch base acquisition, got {type(base_acquisition).__name__}")
+        super().__init__(accelerate(base_acquisition), strategy, random_state, atol, rtol)
+
+    def suggest_batch(self, gp, target_space, q, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        """q points to probe next, as a (q, dim) array.  In this order:
+          1. the base acquisition's ``suggest`` accounting, once for the batch (one ``i += 1``, one kappa / xi decay;
+             y_max is the registered data's for every round), the hyper-parameter fit on the registered data, then
+             the conditioning on the unexpired dummies, on a fork of the GP with room for the batch;
+          2. the base closure on that GP - MES draws its y* samples here, once per batch;
+          3. ONE candidate set shared by every round: ``space.random_sample(max(n_random, n_smart), rs)``, or one
+             Philox seed in device_philox mode;
+          4. per round j = 0..q-1: the fused selection over that set on round j's GP, the refinement of its top
+             n_smart (the L-BFGS-B runs in lockstep; mixed-integer spaces: the reference's DE branch), the reference's
+             random-vs-refined rule, the duplicate rule of ``distinct_picks`` against the earlier picks, then the GP
+             is conditioned in place on the pick;
+          5. the q picks become dummies.
+        q = 1 without dummies returns the base acquisition's ``suggest`` point and leaves the RandomState as it does.
+        q is an integer >= 1."""
+        q = _check_int("q", q, 1)
+        return self._believe(gp, target_space, q, n_random, n_smart, fit_gp, random_state)
+
+    def _round_closure(self, gp, constraint, pending, q):
+        if len(pending) or (q or 1) > 1:
+            gp = gp.condition_on_pending(pending, extra_rows=q or 0)
+        base = self.base_acquisition
+        return type(base)._get_acq(base, gp=gp, constraint=constraint), lambda x: gp.condition_on_pending(x[None])
+
+
+class PendingNEI(_PendingBatch):
+    """Pending points and batches for noisy EI (``NoisyExpectedImprovement`` / ``LogNoisyExpectedImprovement``): the
+    unknown values at the points in flight are drawn jointly with NEI's fantasies of the registered values (Letham et
+    al., Bayesian Analysis 2019, section 5; DESIGN.md 4.14), not believed as in ``KrigingBeliever``.  Each candidate is
+    scored by NEI on the noiseless GP conditioned on the pending points, against incumbents that count the pending
+    fantasies, so a batch built round by round is greedy sequential qNEI (qLogNEI with the log base).
+
+    Dummies, their expiry, ``save_state``, ``suggest()``, ``suggest_batch(..., q)``, one ``i += 1`` and one xi decay
+    per call, the shared candidate set and the rounds are KrigingBeliever's.  The differences: per call the base draws
+    its fantasies once (Z, E, then ``standard_normal((p + q - 1, S))`` for the p unexpired dummies and the q - 1 later
+    picks; ``noiseless_fantasies(pending=..., extra_rows=...)``) on a fork of the noiseless GP, and each round extends
+    those fantasies to the previous pick (``NoiselessFantasies.condition_on_pending``); the fitted GP is never
+    conditioned or modified.  q = 1 without dummies returns the base's ``suggest`` point and leaves the RandomState as
+    it does.  Constraints raise ConstraintNotSupportedError; multi-device GPs and host-side (categorical) transforms
+    raise NotImplementedError; a non-positive pivot raises np.linalg.LinAlgError naming jitter.  ``strategy`` is
+    accepted for ConstantLiar's parameter layout and not used."""
+
+    def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
+        if not isinstance(base_acquisition, _NoisyEI):
+            raise TypeError(f"PendingNEI needs a NoisyExpectedImprovement or LogNoisyExpectedImprovement base "
+                            f"acquisition, got {type(base_acquisition).__name__}")
+        super().__init__(base_acquisition, strategy, random_state, atol, rtol)
+
+    def suggest_batch(self, gp, target_space, q, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        """q points to probe next, as a (q, dim) array: KrigingBeliever.suggest_batch's steps, with the fantasies of
+        step 2 drawn for the dummies and q - 1 later picks, and each round extending them to the previous pick.
+        q is an integer >= 1."""
+        q = _check_int("q", q, 1)
+        return self._believe(gp, target_space, q, n_random, n_smart, fit_gp, random_state)
+
+    def _round_closure(self, gp, constraint, pending, q):
+        base = self.base_acquisition
+        acq = base._closure(gp, constraint, base._suggest_space, pending=pending, extra_rows=(q or 1) - 1)
+        return acq, base.fantasies.condition_on_pending
 
 
 # isinstance(x, b200.AcquisitionFunction) holds for every acquisition of this module, as
@@ -851,6 +909,7 @@ class KrigingBeliever(_ref.ConstantLiar):
 # the concrete classes keep the reference's MRO).
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, LogExpectedImprovement,
              LogProbabilityOfImprovement, ConstantLiar, GPHedge, ThompsonSampling, ConstrainedThompsonSampling,
-             MaxValueEntropySearch, KrigingBeliever, NoisyExpectedImprovement, LogNoisyExpectedImprovement):
+             MaxValueEntropySearch, KrigingBeliever, NoisyExpectedImprovement, LogNoisyExpectedImprovement,
+             PendingNEI):
     AcquisitionFunction.register(_cls)
 del _cls

@@ -139,6 +139,11 @@ struct b200bo_gp {
     // best_s (empty: no fantasies)
     DevBuf fant_a;
     std::vector<double> fant_best;
+    // what pending rows need (b200bo_gp_condition_fantasies), [S][np] per sample: F (normalised) and the prior draws
+    // Z of the rows; W = K^-1 R over the first fant_nreg (registered) rows, [S][fant_nreg]
+    DevBuf fant_f, fant_z, fant_w;
+    DevBuf fant_tmp;  // b200bo_gp_condition_fantasies: the S solves ([S][np]), then the z row (S)
+    int fant_nreg = 0;
     DevBuf X, Xs, y, K, L, W, WT, T, alphav, v1, v2, ls, xf, info, part;
     DevBuf tscratch;  // b200bo_gp_condition: t = W^T l of the row update (np), so that alpha_ survives it
     // predict-side scratch (used when this handle is gps[0] of a call)
@@ -850,11 +855,22 @@ extern "C" int b200bo_gp_set_fantasies(b200bo_gp* nl, const b200bo_gp* ny, const
     const double sq = std::sqrt(s2 - tau), ds = s2 - tau;
     const std::vector<double>& y = nl->y_norm;
     std::vector<double> col(np, 0.0), fp(n), kr(n), F((size_t)n * S), A((size_t)np * S, 0.0), a(n);
+    // the state pending rows need (b200bo_gp_condition_fantasies): F, Z and W = K^-1 R per sample.  With
+    // sigma_n^2 = tau, k^T K0^-1 (y_n - L0 Z) + l^T Z = k^T K0^-1 y_n for a new row [l^T, r] of L0, so Z is kept as
+    // zeros and W as alpha_ = K0^-1 y_n: the same values without a solve.
+    for (DevBuf* b : {&nl->fant_f, &nl->fant_z})
+        if ((rc = b->reserve(sizeof(double) * np * S))) return rc;
+    if ((rc = nl->fant_w.reserve(sizeof(double) * n * S))) return rc;
+    if (ds == 0.0) CU(cudaMemsetAsync(nl->fant_z.p, 0, sizeof(double) * np * S, g_st));
+    nl->fant_nreg = n;
     const int wpb = 8;
     const dim3 blk(32 * wpb), grd((np + wpb - 1) / wpb);
     for (int s = 0; s < S; ++s) {
+        double* fz = nl->fant_z.as<double>() + (size_t)s * np;
+        double* fw = nl->fant_w.as<double>() + (size_t)s * n;
         for (int i = 0; i < n; ++i) col[i] = z[(size_t)i * S + s];
         if ((rc = h2d(in.p, col.data(), sizeof(double) * np))) return rc;
+        if (ds > 0.0) CU(cudaMemcpyAsync(fz, in.p, sizeof(double) * np, cudaMemcpyDeviceToDevice, g_st));
         gemv_rows_kernel<<<grd, blk, 0, g_st>>>(nl->L.as<double>(), np, in.as<double>(), out.as<double>(), np, np, 1);
         LAUNCHED();
         CU(cudaGetLastError());
@@ -863,13 +879,17 @@ extern "C" int b200bo_gp_set_fantasies(b200bo_gp* nl, const b200bo_gp* ny, const
             for (int i = 0; i < n; ++i) col[i] = (y[i] - fp[i]) - sq * e[(size_t)i * S + s];  // R
             if ((rc = h2d(in.p, col.data(), sizeof(double) * np))) return rc;
             if ((rc = solve_spd(noisy, in.as<double>(), out.as<double>(), v1.as<double>(), v2.as<double>()))) return rc;
+            CU(cudaMemcpyAsync(fw, out.p, sizeof(double) * n, cudaMemcpyDeviceToDevice, g_st));
             if ((rc = d2h(kr.data(), out.p, sizeof(double) * n))) return rc;  // K^-1 R
             for (int i = 0; i < n; ++i) col[i] = (y[i] - sq * e[(size_t)i * S + s]) - ds * kr[i];
         } else {
+            CU(cudaMemcpyAsync(fw, nl->alphav.p, sizeof(double) * n, cudaMemcpyDeviceToDevice, g_st));
             for (int i = 0; i < n; ++i) col[i] = y[i];  // sigma_n^2 = tau: F = y_n exactly
         }
         for (int i = 0; i < n; ++i) F[(size_t)i * S + s] = col[i];
         if ((rc = h2d(in.p, col.data(), sizeof(double) * np))) return rc;
+        CU(cudaMemcpyAsync(nl->fant_f.as<double>() + (size_t)s * np, in.p, sizeof(double) * np,
+                           cudaMemcpyDeviceToDevice, g_st));
         if ((rc = solve_spd(nl, in.as<double>(), out.as<double>(), v1.as<double>(), v2.as<double>()))) return rc;
         if ((rc = d2h(a.data(), out.p, sizeof(double) * n))) return rc;  // a_s = K0^-1 f_s
         for (int i = 0; i < n; ++i) A[(size_t)i * S + s] = a[i];
@@ -966,6 +986,32 @@ extern "C" int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new
     return B200BO_OK;
 }
 
+// Row n of b200bo_gp_condition: the factor row update, the believer target mu_norm(x) in y's padding slot n and as
+// row n of the host targets, alpha_ = [alpha_; 0].  *mu (nullable) receives the target in data units.  A non-positive
+// pivot leaves the handle unfitted.  gp->tscratch holds np entries.
+static int condition_row(b200bo_gp* gp, const double* x, double* mu) {
+    const int n = (int)gp->n;
+    double* yn = gp->y.as<double>() + n;
+    int finfo = 0, rc;
+    if ((rc = append_factor_row(gp, x, gp->tscratch.as<double>(), yn, &finfo))) return rc;
+    if (finfo != 0) {
+        gp->fitted = false;  // row n of K/L is garbage now
+        return set_err(B200BO_ERR_NOT_PD, "%d-th leading minor of the array is not positive definite", finfo);
+    }
+    double mu_norm = 0.0;
+    CU(cudaMemcpy(&mu_norm, yn, sizeof(double), cudaMemcpyDeviceToHost));
+    CU(cudaMemset(gp->alphav.as<double>() + n, 0, sizeof(double)));  // alpha_ = [alpha_; 0]
+    const double m = gp->y_std * mu_norm + gp->y_mean;  // data units, as the predict kernels form the mean
+    gp->y_norm.push_back(mu_norm);
+    gp->y_raw.push_back(m);
+    if (mu) *mu = m;
+    gp->n = n + 1;
+    gp->tc_valid = false;
+    gp->pad_valid = false;
+    gp->gram_valid = false;
+    return B200BO_OK;
+}
+
 // Kriging believer (DESIGN.md 4.11): row n gets the target mu_norm(x) = k(x, X)^T alpha_, so K' [alpha_; 0] =
 // [y; mu_norm(x)] and alpha_ extends by a zero - no solve, the mean is unchanged everywhere, only K, L, L^-1 grow.
 extern "C" int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, double* mu_out) {
@@ -985,29 +1031,86 @@ extern "C" int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, d
     gp->fant_best.clear();
     int rc;
     if ((rc = gp->tscratch.reserve(sizeof(double) * gp->np))) return rc;
-    for (int64_t r = 0; r < p; ++r) {
-        const int n = (int)gp->n;
-        double* yn = gp->y.as<double>() + n;  // the believer target lands in y's padding slot n
-        int finfo = 0;
-        if ((rc = append_factor_row(gp, Xp + r * d, gp->tscratch.as<double>(), yn, &finfo))) return rc;
-        if (finfo != 0) {
-            gp->fitted = false;  // row n of K/L is garbage now
-            return set_err(B200BO_ERR_NOT_PD, "%d-th leading minor of the array is not positive definite", finfo);
-        }
-        double mu_norm = 0.0;
-        CU(cudaMemcpy(&mu_norm, yn, sizeof(double), cudaMemcpyDeviceToHost));
-        CU(cudaMemset(gp->alphav.as<double>() + n, 0, sizeof(double)));  // alpha_ = [alpha_; 0]
-        const double mu = gp->y_std * mu_norm + gp->y_mean;  // data units, as the predict kernels form the mean
-        gp->y_norm.push_back(mu_norm);
-        gp->y_raw.push_back(mu);
-        if (mu_out) mu_out[r] = mu;
-        gp->n = n + 1;
-        gp->tc_valid = false;
-        gp->pad_valid = false;
-        gp->gram_valid = false;
-    }
+    for (int64_t r = 0; r < p; ++r)
+        if ((rc = condition_row(gp, Xp + r * d, mu_out ? mu_out + r : nullptr))) return rc;
     CU(cudaDeviceSynchronize());
     return B200BO_OK;
+}
+
+// The work of b200bo_gp_condition_fantasies after its checks; on an error the caller drops the fantasies.
+static int extend_fantasies(b200bo_gp* gp, const double* Xp, int64_t p, const double* zp, double* f_out,
+                            double* best_out) {
+    const int d = gp->d, S = (int)gp->fant_best.size();
+    const int np = gp->np, n0 = (int)gp->n;
+    int rc;
+    if ((rc = gp->tscratch.reserve(sizeof(double) * np))) return rc;
+    if ((rc = gp->fant_tmp.reserve(sizeof(double) * ((size_t)np * S + S)))) return rc;
+    double* acol = gp->fant_tmp.as<double>();
+    double* zrow = acol + (size_t)np * S;
+    double* best = gp->fant_a.as<double>() + (size_t)np * S;
+    for (int64_t r = 0; r < p; ++r) {
+        const int n = (int)gp->n;
+        if ((rc = condition_row(gp, Xp + r * d, nullptr))) return rc;
+        CU(cudaMemcpy(zrow, zp + r * S, sizeof(double) * S, cudaMemcpyHostToDevice));
+        fantasy_row_kernel<<<1, 32 * S>>>(gp->K.as<double>(), gp->L.as<double>(), np, n, gp->fant_nreg,
+                                          gp->fant_w.as<double>(), zrow, gp->fant_z.as<double>(),
+                                          gp->fant_f.as<double>(), best, gp->y_std, gp->y_mean);
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    const int n = (int)gp->n;
+    for (int s = 0; s < S && p > 0; ++s)
+        if ((rc = solve_spd(gp, gp->fant_f.as<double>() + (size_t)s * np, acol + (size_t)s * np, gp->v1.as<double>(),
+                            gp->v2.as<double>())))
+            return rc;
+    if (p > 0) {
+        fantasy_pack_kernel<<<(np * S + 255) / 256, 256>>>(acol, np, n, S, gp->fant_a.as<double>());
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    std::vector<double> F((size_t)S * np), A((size_t)np * S), bst(S);
+    CU(cudaMemcpy(F.data(), gp->fant_f.p, sizeof(double) * F.size(), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(A.data(), gp->fant_a.p, sizeof(double) * A.size(), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(bst.data(), best, sizeof(double) * S, cudaMemcpyDeviceToHost));
+    for (int s = 0; s < S; ++s)
+        for (int i = 0; i < n; ++i)
+            if (!std::isfinite(F[(size_t)s * np + i]) || !std::isfinite(A[(size_t)i * S + s]))
+                return set_err(B200BO_ERR_NOT_PD, "the fantasies are not finite: K0 = c k(X, X) + tau I is too "
+                                                  "ill-conditioned (raise jitter)");
+    gp->fant_best = bst;
+    if (f_out)
+        for (int64_t r = 0; r < p; ++r)
+            for (int s = 0; s < S; ++s) f_out[r * S + s] = gp->y_std * F[(size_t)s * np + n0 + r] + gp->y_mean;
+    if (best_out)
+        for (int s = 0; s < S; ++s) best_out[s] = bst[s];
+    return B200BO_OK;
+}
+
+// NEI fantasies at pending rows (include/b200bo.h, DESIGN.md 4.14): per row the believer row update of
+// b200bo_gp_condition, then fantasy_row_kernel forms the S values F_js on the device; after the last row
+// A' = K0'^-1 F' per sample with solve_spd, as b200bo_gp_set_fantasies solves.
+extern "C" int b200bo_gp_condition_fantasies(b200bo_gp* gp, const double* Xp, int64_t p, const double* zp,
+                                             double* f_out, double* best_out) {
+    if (!gp || (p > 0 && (!Xp || !zp))) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (p < 0) return set_err(B200BO_ERR_ARG, "p=%lld must be >= 0", (long long)p);
+    if (!gp->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
+    if (gp->replica)
+        return set_err(B200BO_ERR_STATE, "handle is a predict-only replica: condition the source or a fork of it");
+    if (p > gp->np - gp->n)
+        return set_err(B200BO_ERR_STATE, "no padding slack for %lld rows (n=%lld, np=%d): fork with extra_rows",
+                       (long long)p, gp->n, gp->np);
+    if (gp->fant_best.empty())
+        return set_err(B200BO_ERR_STATE, "the handle holds no fantasies (b200bo_gp_set_fantasies)");
+    const int d = gp->d, S = (int)gp->fant_best.size();
+    for (int64_t i = 0; i < p * d; ++i)
+        if (!std::isfinite(Xp[i])) return set_err(B200BO_ERR_ARG, "Input X contains NaN or infinity.");
+    for (int64_t i = 0; i < p * S; ++i)
+        if (!std::isfinite(zp[i])) return set_err(B200BO_ERR_ARG, "non-finite draw at %lld", (long long)i);
+    CU(cudaSetDevice(gp->device));
+    NvtxRange nvtx_range("b200bo:condition_fantasies");
+    const int rc = extend_fantasies(gp, Xp, p, zp, f_out, best_out);
+    if (rc != B200BO_OK) gp->fant_best.clear();  // A no longer matches the factor and F
+    return rc;
 }
 
 // the fitted model's shape, hyper-parameters and target statistics: what a fork and a replica both take from the source
@@ -1060,6 +1163,24 @@ static int fork_into(const b200bo_gp* src, int64_t extra_rows, b200bo_gp* dst) {
         repitch_identity_kernel<<<grd, blk>>>(m.from->as<double>(), (int)np0, m.to->as<double>(), (int)np);
         LAUNCHED();
         CU(cudaGetLastError());
+    }
+    if (!src->fant_best.empty()) {  // NEI fantasies: A ([np'][S], best_s behind it), F and Z ([S][np']), W as it is
+        const size_t S = src->fant_best.size(), nreg = src->fant_nreg;
+        if ((rc = dst->fant_a.reserve(sizeof(double) * (np * S + S)))) return rc;
+        CU(cudaMemset(dst->fant_a.p, 0, sizeof(double) * np * S));
+        CU(cudaMemcpy(dst->fant_a.p, src->fant_a.p, sizeof(double) * n * S, cudaMemcpyDeviceToDevice));
+        CU(cudaMemcpy(dst->fant_a.as<double>() + np * S, src->fant_a.as<double>() + np0 * S, sizeof(double) * S,
+                      cudaMemcpyDeviceToDevice));
+        for (const Mat& m : {Mat{&dst->fant_f, &src->fant_f}, Mat{&dst->fant_z, &src->fant_z}}) {
+            if ((rc = m.to->reserve(sizeof(double) * np * S))) return rc;
+            CU(cudaMemset(m.to->p, 0, sizeof(double) * np * S));
+            CU(cudaMemcpy2D(m.to->p, sizeof(double) * np, m.from->p, sizeof(double) * np0, sizeof(double) * n, S,
+                            cudaMemcpyDeviceToDevice));
+        }
+        if ((rc = dst->fant_w.reserve(sizeof(double) * nreg * S))) return rc;
+        CU(cudaMemcpy(dst->fant_w.p, src->fant_w.p, sizeof(double) * nreg * S, cudaMemcpyDeviceToDevice));
+        dst->fant_nreg = src->fant_nreg;
+        dst->fant_best = src->fant_best;
     }
     CU(cudaDeviceSynchronize());
     dst->fitted = true;

@@ -785,6 +785,39 @@ __global__ void append_winv_kernel(double* __restrict__ W, double* __restrict__ 
     }
 }
 
+// NEI fantasies at a pending row n just appended to the noiseless factor (b200bo_gp_condition_fantasies): one warp per
+// sample s,  F[s][n] = sum_{i<n} L[n][i] Z[s][i] + sum_{i<nreg} K[n][i] W[s][i] + L[n][n] z_s  in a fixed order (lane
+// strides, then a butterfly), the joint prior draw from the grown factor plus the Matheron update over the registered
+// rows.  Stores F[s][n] and Z[s][n] = z_s and raises best_s (data units) behind A: best[s] = max(best[s], y_std F + y_mean).
+__global__ void fantasy_row_kernel(const double* __restrict__ K, const double* __restrict__ L, int np, int n, int nreg,
+                                   const double* __restrict__ W, const double* __restrict__ zrow, double* __restrict__ Z,
+                                   double* __restrict__ F, double* __restrict__ best, double y_std, double y_mean) {
+    const int s = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const double* lrow = L + (size_t)n * np;
+    const double* krow = K + (size_t)n * np;
+    const double* zs = Z + (size_t)s * np;
+    const double* ws = W + (size_t)s * nreg;
+    double acc = 0.0;
+    for (int i = lane; i < n; i += 32) acc = fma(lrow[i], zs[i], acc);
+    for (int i = lane; i < nreg; i += 32) acc = fma(krow[i], ws[i], acc);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) {
+        const double z = zrow[s];
+        const double f = fma(lrow[n], z, acc);
+        Z[(size_t)s * np + n] = z;
+        F[(size_t)s * np + n] = f;
+        best[s] = fmax(best[s], y_std * f + y_mean);
+    }
+}
+// A[i][s] = Acol[s][i] for i < n, zero for n <= i < np: the [np][S] layout the NEI kernels read
+__global__ void fantasy_pack_kernel(const double* __restrict__ Acol, int np, int n, int S, double* __restrict__ A) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= np * S) return;
+    const int i = idx / S, s = idx % S;
+    A[idx] = i < n ? Acol[(size_t)s * np + i] : 0.0;
+}
+
 // Re-pitch of an np_src x np_src matrix into an np_dst x np_dst one (np_dst >= np_src, both multiples of 32), in one
 // pass: dst[i][j] = src[i][j] inside the source block, the identity outside it - the padding invariant of K, L, L^-1
 // and its transpose.  32x8 threads per 32x32 tile, 4 rows each; every store is a coalesced 256-byte row segment.

@@ -302,6 +302,14 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
                 self.__dict__["_b200_handle"] = self._fork_handle(pending.shape[0])
             B.check(B.lib().b200bo_gp_condition(self._handle().ptr, B.as_dp(pending), pending.shape[0], None))
 
+    def _bare_copy(self):
+        """A new regressor with this one's fitted attributes and none of its device state (handles, replicas, cached
+        factor reads, the noiseless regressor of NEI)."""
+        out = type(self).__new__(type(self))
+        skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha", "_b200_noiseless")
+        out.__dict__.update({k: v for k, v in self.__dict__.items() if k not in skip})
+        return out
+
     def _fork_handle(self, extra_rows):
         h = _Handle.__new__(_Handle)
         h.ptr = C.c_void_p()
@@ -748,10 +756,7 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         # in place on a conditioned GP; B200BO_ERR_STATE (checked before any work) means no slack left: fork
         rc = L.b200bo_gp_condition(self._handle().ptr, B.as_dp(Xc), p, B.as_dp(mu)) if n_reg is not None else B.ERR_STATE
         if rc == B.ERR_STATE:
-            out = type(self).__new__(type(self))
-            skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha",
-                    "_b200_noiseless")
-            out.__dict__.update({k: v for k, v in self.__dict__.items() if k not in skip})
+            out = self._bare_copy()
             out.__dict__["_b200_handle"] = self._fork_handle(p + int(extra_rows))
             out.__dict__["_b200_conditioned"] = n if n_reg is None else n_reg
             rc = L.b200bo_gp_condition(out._handle().ptr, B.as_dp(Xc), p, B.as_dp(mu))
@@ -784,7 +789,8 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
 
         return PosteriorPaths(self, n_paths, n_features, random_state)
 
-    def noiseless_fantasies(self, n_samples, jitter=1e-6, incumbent=None, random_state=None):
+    def noiseless_fantasies(self, n_samples, jitter=1e-6, incumbent=None, random_state=None, pending=None,
+                            extra_rows=0):
         """S = ``n_samples`` (1..16) joint samples of the noise-free function values at the training inputs, for noisy
         expected improvement (DESIGN.md 4.13, ``b200bo_gp_set_fantasies``).
 
@@ -794,7 +800,14 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         regressor on a device handle of its own, always in fp64.  From ``random_state`` (``check_random_state``) it
         draws Z = standard_normal((n, S)), then E = standard_normal((n, S)).  ``incumbent`` is the (n,) mask of the
         rows whose fantasy values may be the incumbent best_s (all rows when None).  Returns a ``NoiselessFantasies``.
-        One device, no pending-point conditioning; a non-PD K0 raises np.linalg.LinAlgError naming ``jitter``."""
+
+        ``pending`` ((p, d), points suggested and not yet registered) and ``extra_rows`` (room for that many later
+        ``NoiselessFantasies.condition_on_pending`` rows) draw the values at pending points jointly with the fantasies
+        (DESIGN.md 4.14, ``b200bo_gp_condition_fantasies``): after Z and E, ``standard_normal((p + extra_rows, S))``;
+        then the noiseless regressor is forked with that capacity and the fork is conditioned on ``pending``.  This GP
+        and the noiseless regressor are never modified.  With neither argument nothing is forked or drawn beyond Z, E.
+        One device (multi-device GPs raise NotImplementedError, and with pending rows so do host-side, categorical,
+        input transforms); a non-PD K0 or pending pivot raises np.linalg.LinAlgError naming ``jitter``."""
         S = int(n_samples)
         if isinstance(n_samples, bool) or S != n_samples or not 1 <= S <= B.MAX_PATHS:
             raise ValueError(f"n_samples must be an integer in [1, {B.MAX_PATHS}], got {n_samples!r}")
@@ -807,6 +820,19 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
             raise NotImplementedError("noisy expected improvement runs on one device: the GP is multi-device")
         if self.__dict__.get("_b200_conditioned") is not None:
             raise NotImplementedError("noisy expected improvement on a GP conditioned on pending points")
+        if isinstance(extra_rows, bool) or not isinstance(extra_rows, (int, np.integer)) or extra_rows < 0:
+            raise ValueError(f"extra_rows must be an integer >= 0, got {extra_rows!r}")
+        d = self.X_train_.shape[1]
+        P = np.empty((0, d)) if pending is None else np.array(pending, dtype=np.float64)
+        if P.ndim == 1 and P.size == d:
+            P = P.reshape(1, d)
+        if P.size == 0:
+            P = P.reshape(0, d)
+        if P.ndim != 2 or P.shape[1] != d:
+            raise ValueError("pending must be (n_pending, d) with the d of the fitted GP")
+        if not np.all(np.isfinite(P)):
+            raise ValueError("Input contains NaN or infinity.")
+        rows = P.shape[0] + int(extra_rows)
         n = self.X_train_.shape[0]
         mask = np.ones(n, dtype=np.uint8) if incumbent is None else np.asarray(incumbent, dtype=bool).astype(np.uint8)
         if mask.shape != (n,):
@@ -814,12 +840,16 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         if not mask.any():
             raise ValueError("the incumbent mask selects no training row")
         self._ensure_device_fit()
+        if rows and self.__dict__.get("_b200_xform", ("device", None))[0] == "host":
+            raise NotImplementedError("pending points for noisy expected improvement with a host-side (categorical) "
+                                      "kernel transform")
         ek = parse_kernel(self.kernel_)
         alpha = float(self.alpha)
         tau = min(alpha, jitter)
         rs = check_random_state(random_state)
         Z = B.c_f64(rs.standard_normal((n, S)))
         E = B.c_f64(rs.standard_normal((n, S)))
+        Zp = B.c_f64(rs.standard_normal((rows, S))) if rows else None
         if ek.noise == 0.0 and tau == alpha:
             nl = self
         else:
@@ -827,10 +857,7 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
             # buffers, so at most two N^2 handles (this GP's and the noiseless one) are ever live for NEI
             nl = self.__dict__.get("_b200_noiseless")
             handle = nl._handle() if nl is not None and nl.device == self.device else _Handle(self.device)
-            nl = type(self).__new__(type(self))
-            skip = ("_b200_handle", "_b200_restart_handles", "_b200_replicas", "_b200_L", "_b200_alpha",
-                    "_b200_noiseless")
-            nl.__dict__.update({k: v for k, v in self.__dict__.items() if k not in skip})
+            nl = self._bare_copy()
             nl.__dict__["_b200_handle"] = handle
             self.__dict__["_b200_noiseless"] = nl
             nl.alpha = tau
@@ -846,19 +873,58 @@ class B200GaussianProcessRegressor(GaussianProcessRegressor):
         best = np.empty(S)
         B.check(B.lib().b200bo_gp_set_fantasies(nl._handle().ptr, self._handle().ptr, B.as_dp(Z), B.as_dp(E), S,
                                                 mask.ctypes.data_as(C.POINTER(C.c_uint8)), B.as_dp(F), B.as_dp(best)))
-        return NoiselessFantasies(nl, F, best, tau)
+        fant = NoiselessFantasies(nl, F, best, tau)
+        if rows:
+            # the fork's X_train_ grows with the pending rows (NoiselessFantasies.condition_on_pending) while its
+            # targets stay the registered ones: it holds fantasies for NEI and is never refitted
+            fork = nl._bare_copy()
+            fork.__dict__["_b200_handle"] = nl._fork_handle(rows)
+            fork.__dict__["_b200_conditioned"] = n
+            fant.gp, fant._zp, fant._next = fork, Zp, 0
+            fant.condition_on_pending(P)
+        return fant
 
 
 class NoiselessFantasies:
     """S joint samples of the noise-free function values at the training inputs (``noiseless_fantasies``).
 
-    gp    the noiseless regressor holding A = K0^-1 F on its device handle (the fitted GP itself when tau = sigma_n^2)
-    F     (n, S) fantasy values, data units
+    gp    the noiseless regressor holding A = K0^-1 F on its device handle (the fitted GP itself when tau = sigma_n^2);
+          with pending points a fork of it whose ``X_train_`` ends with the pending rows
+    F     (n, S) fantasy values, data units ((n + p, S) with p pending rows)
     best  (S,) best_s, the largest fantasy value over the incumbent rows
     tau   the noiseless GP's diagonal term"""
 
     def __init__(self, gp, F, best, tau):
         self.gp, self.F, self.best, self.tau = gp, F, best, tau
+        self._zp, self._next = None, 0  # pre-drawn z rows of pending points, and the next one to use
+
+    def condition_on_pending(self, X):
+        """Extends the fantasies in place to the pending points ``X`` ((p, d) or (d,)): their values are drawn jointly
+        with the fantasies from the next p of the z rows ``noiseless_fantasies(pending=..., extra_rows=...)`` drew
+        (``b200bo_gp_condition_fantasies``).  F gains p rows and best may rise: pending rows count toward the incumbent.
+        More rows than were drawn raise ValueError; a non-positive pivot raises np.linalg.LinAlgError naming jitter."""
+        X = B.c_f64(np.asarray(X, dtype=np.float64).reshape(-1, self.gp.X_train_.shape[1]))
+        p = X.shape[0]
+        if self._zp is None or self._next + p > self._zp.shape[0]:
+            left = 0 if self._zp is None else self._zp.shape[0] - self._next
+            raise ValueError(f"{p} pending rows, {left} pre-drawn z rows left: pass pending / extra_rows to "
+                             "noiseless_fantasies")
+        if not np.all(np.isfinite(X)):
+            raise ValueError("Input contains NaN or infinity.")
+        zp = B.c_f64(self._zp[self._next:self._next + p])
+        f = np.empty((p, self.n_samples))
+        best = np.empty(self.n_samples)
+        rc = B.lib().b200bo_gp_condition_fantasies(self.handle.ptr, B.as_dp(X), p, B.as_dp(zp), B.as_dp(f),
+                                                   B.as_dp(best))
+        if rc == B.ERR_NOT_PD:
+            msg = B.lib().b200bo_last_error().decode("utf-8", "replace")
+            raise np.linalg.LinAlgError(f"{msg} (noiseless GP with tau = {self.tau!r} at a pending point: raise "
+                                        "jitter)")
+        B.check(rc)
+        self._next += p
+        self.gp.X_train_ = np.vstack([self.gp.X_train_, X])
+        self.F = np.vstack([self.F, f])
+        self.best = best
 
     @property
     def n_samples(self):

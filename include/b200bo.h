@@ -219,7 +219,7 @@ int b200bo_gp_append(b200bo_gp* gp, const double* x_new, double y_new, int64_t* 
  *
  * b200bo_gp_fork: a new, full and appendable handle on src's device (not a predict-only replica) holding src's fitted
  * state - X / Xs, K, L, L^-1 and its transpose, alpha_, y, the y statistics, the transform, the hyper-parameters, the
- * precision and the MES samples - with capacity np' = ceil((n + extra_rows)/128)*128 rows.  The N^2 matrices are
+ * precision, the MES samples and the NEI fantasies (A re-pitched, best_s, F, Z, W) - with capacity np' = ceil((n + extra_rows)/128)*128 rows.  The N^2 matrices are
  * re-pitched from np to np' with identity padding.  Extra device memory: about 4 * 8 * np'^2 bytes, plus the stage
  * images of L^-1 the predict kernels build on first use.  np' == np: predictions, acquisitions and selections are
  * bit-equal to src's; np' > np: equal to round-off.  The fork's training set is for conditioning / appending:
@@ -235,6 +235,26 @@ int b200bo_gp_fork(const b200bo_gp* src, int64_t extra_rows, b200bo_gp** out);
  * non-finite Xp -> B200BO_ERR_ARG; a non-positive pivot -> B200BO_ERR_NOT_PD with the 1-based index of the failing
  * row in the message (LAPACK dpotrf convention), and the handle is left unfitted. */
 int b200bo_gp_condition(b200bo_gp* gp, const double* Xp, int64_t p, double* mu_out);
+
+/* ---- NEI with pending points (DESIGN.md 4.14) -------------------------------------------------
+ * (Letham et al. 2019: the values at pending points are drawn jointly with the fantasies.)  `noiseless` holds S
+ * fantasies (b200bo_gp_set_fantasies, or a fork of such a handle: b200bo_gp_fork carries A, best_s, F, the prior draws Z
+ * and W = K^-1 R of the registered rows).  Conditions it in place on the p rows of Xp ((p,d) host) as
+ * b200bo_gp_condition does (same row update, believer targets, y statistics), and per row j, with the new row
+ * [l^T, r] of L0 and zp[j] (the (p,S) host array, row-major) its fresh standard-normal draws:
+ *   F_js = l^T [Z_s; z_1s .. z_(j-1)s] + r z_js + const_value k(x_j, X_reg)^T W_s      (normalised units)
+ * - the joint prior draw at x_j from the grown factor plus the Matheron update over the registered rows - then
+ * best_s = max(best_s, y_std F_js + y_mean): pending rows always count toward the incumbent.  After the last row
+ * A' = K0'^-1 F' per sample with the explicit-inverse solve and one refinement step of b200bo_gp_set_fantasies.  With
+ * sigma_n^2 = tau, F_js = mu(x_j) + (the l^T z terms of the pending rows) + r z_js.  The handle is then an ordinary NEI
+ * handle over X u P.  p single-row calls give bit-equal results to one p-row call; p = 0 changes nothing.  f_out
+ * (nullable, (p,S) host) receives F_j. in data units, best_out (nullable, (S,) host) best_s.  Errors, in this order:
+ * NULL arguments or p < 0 -> B200BO_ERR_ARG; not fitted or a replica, p > np - n (no slack: fork first), no fantasies ->
+ * B200BO_ERR_STATE; non-finite Xp or zp -> B200BO_ERR_ARG; a non-positive pivot -> B200BO_ERR_NOT_PD with the 1-based
+ * index of the failing row in the message, or non-finite fantasies -> B200BO_ERR_NOT_PD; after either the handle holds
+ * no fantasies (and after a pivot failure it is unfitted).  b200bo_gp_condition on the handle drops the fantasies. */
+int b200bo_gp_condition_fantasies(b200bo_gp* noiseless, const double* Xp, int64_t p, const double* zp, double* f_out,
+                                  double* best_out);
 
 /* Replaces GaussianProcessRegressor.log_marginal_likelihood(theta, eval_gradient)
  * (SK/gaussian_process/_gpr.py:541-656) on the training set of the last b200bo_gp_set_data /
