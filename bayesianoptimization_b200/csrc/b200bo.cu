@@ -171,9 +171,10 @@ struct b200bo_gp {
     // selection-only pruning: bound keys / local indices (two buffers each for the radix sort), its temp storage and
     // the control words of predict_acq16_kernel's prune mode
     DevBuf prune_key, prune_idx, prune_tmp, prune_ctl;
-    // its refine stages: the interval of K* alpha_ per candidate from the bound pass, the survivor list, the
-    // per-row-block partials, K* alpha_ of the tiles and the arrival counters of predict_units_kernel
-    DevBuf prune_mu, prune_surv, prune_part, prune_mu_unit, prune_arrive;
+    // its refine stages: the interval of K* alpha_ per candidate from the bound pass, the survivor list and its keys
+    // (two buffers each for the sort of the final rounds), the per-row-block partials, K* alpha_ of the tiles and the
+    // arrival counters of predict_units_kernel
+    DevBuf prune_mu, prune_surv, prune_surv_key, prune_part, prune_mu_unit, prune_arrive;
     // candidates of the last call (chunked: all chunks) and those of them evaluated outside the prune mode; the
     // prune mode counts its own in prune_ctl[2] (prune_counted)
     long long stat_total = 0, stat_direct = 0;
@@ -294,8 +295,11 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_units_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_units_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_units_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_units_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_units_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(ks_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(ks_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
@@ -1544,6 +1548,18 @@ static int prune_refine_blocks(int np, long long ntiles) {
     return b < nb / 8 ? b : nb / 8;
 }
 
+// A/B switches of the refine stages (DESIGN.md 4.9, 6.1), read per call.  B200BO_PRUNE_ROUNDS=0: no merged k-th key
+// and one final stage over the survivors in arrival order.  B200BO_PRUNE_SHARED_KS=0: every unit builds K* for its
+// rows itself.
+static bool prune_rounds() {
+    const char* e = getenv("B200BO_PRUNE_ROUNDS");
+    return !(e && e[0] == '0');
+}
+static bool prune_shared_ks() {
+    const char* e = getenv("B200BO_PRUNE_SHARED_KS");
+    return !(e && e[0] == '0');
+}
+
 // control words of a launch with refine stages: the tile kernel starts behind the lead tiles, and the lead stage sees
 // the k-th key carried into the launch
 __global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
@@ -1552,32 +1568,71 @@ __global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
     ctl[kCtlKthLead] = ctl[kCtlKth];
 }
 
+// Tiles of the final rounds: 8, 16, 32, then the rest of the kRefineMaxTiles, at most `grid` each (a round's K* slots).
+// One round over all survivors without rounds.
+static int final_round_tiles(bool rounds, int r, int t0, int grid) {
+    const int t = rounds && r < 3 ? 8 << r : kRefineMaxTiles - t0;
+    return t < grid ? t : grid;
+}
+
 // The lead, refine and final stages of a pruned launch (predict16.cuh), between prune_prepare and the tile kernel.
+// With rounds (prune_rounds) merge_kth_kernel tightens the k-th key after the lead stage and after every final round,
+// and the final rounds take the survivors sorted by key, skipping the tiles above the key.  With shared K*
+// (prune_shared_ks) ks_build_kernel builds the K* of a stage's or round's tiles once, before its units.
 static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg, int blocks, bool resume,
                                cudaStream_t stream) {
     const int nb = P.gp[0].np / PBM, grid = g0->sm_count;
+    const int nsurv = kRefineMaxTiles * PBN;
+    const bool rounds = prune_rounds(), shared_ks = prune_shared_ks();
     int rc;
-    if ((rc = g0->prune_surv.reserve(sizeof(int) * (size_t)kRefineMaxTiles * PBN))) return rc;
+    if ((rc = g0->prune_surv.reserve(sizeof(int) * 2 * (size_t)nsurv))) return rc;
+    if ((rc = g0->prune_surv_key.reserve(sizeof(unsigned long long) * 2 * (size_t)nsurv))) return rc;
     if ((rc = g0->prune_part.reserve(sizeof(double) * (size_t)kUnitSlots * nb * 32 * PBN))) return rc;
     if ((rc = g0->prune_mu_unit.reserve(sizeof(double) * (size_t)kUnitSlots * PBN))) return rc;
     if ((rc = g0->prune_arrive.reserve(sizeof(unsigned) * kUnitSlots))) return rc;
+    unsigned long long* skey = g0->prune_surv_key.as<unsigned long long>();
+    int* sidx = g0->prune_surv.as<int>();
+    cub::DoubleBuffer<unsigned long long> kb(skey, skey + nsurv);
+    cub::DoubleBuffer<int> ib(sidx, sidx + nsurv);
+    size_t tmp = 0;
+    if (rounds) {
+        CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, kb, ib, nsurv, 0, 64, stream));
+        if ((rc = g0->prune_tmp.reserve(tmp))) return rc;
+    }
     unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
     if (!resume) CU(cudaMemsetAsync(ctl + kCtlRefined, 0, sizeof(unsigned long long), stream));
     CU(cudaMemsetAsync(g0->prune_arrive.p, 0, sizeof(unsigned) * kUnitSlots, stream));
+    if (rounds) CU(cudaMemsetAsync(skey, 0xFF, sizeof(unsigned long long) * nsurv, stream));  // unused slots sort last
     prune_ctl_refine_kernel<<<1, 1, 0, stream>>>(ctl);
     LAUNCHED();
     RefineParams R;
     R.mu = g0->prune_mu.as<double2>();
     R.mu_unit = g0->prune_mu_unit.as<double>();
-    R.surv = g0->prune_surv.as<int>();
+    R.surv = sidx;
+    R.surv_key = skey;
     R.part = g0->prune_part.as<double>();
     R.arrive = g0->prune_arrive.as<unsigned>();
     R.blocks = blocks;
     R.groups_max = nb / 2 < 32 ? nb / 2 : 32;
     R.final_stage = 0;
-    auto units = dreg ? predict_units_kernel<true> : predict_units_kernel<false>;
+    R.t0 = 0;
+    R.t1 = kRefineMaxTiles;
+    R.round_skip = 0;
+    // with shared K* the units run no phase A, so the candidates' coordinates never sit in registers
+    auto units = shared_ks ? predict_units_kernel<false, true>
+                           : (dreg ? predict_units_kernel<true, false> : predict_units_kernel<false, false>);
+    auto build = dreg ? ks_build_kernel<true> : ks_build_kernel<false>;
+    const SelList* lists = g0->sel_cta.as<SelList>();
+    if (shared_ks) {
+        build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
+        LAUNCHED();
+    }
     units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
     LAUNCHED();
+    if (rounds) {
+        merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
+        LAUNCHED();
+    }
     CU(cudaEventRecord(g0->ev_stage[2], stream));
     PredictParams Q = P;  // the lead stage has begun the per-CTA lists
     Q.sel_resume = 1;
@@ -1588,8 +1643,29 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     LAUNCHED();
     CU(cudaEventRecord(g0->ev_stage[3], stream));
     R.final_stage = 1;
-    units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-    LAUNCHED();
+    R.round_skip = rounds;
+    if (rounds) {  // survivors ascending by key; the sentinels of the unused slots last
+        CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, kb, ib, nsurv, 0, 64, stream));
+        LAUNCHED();
+        R.surv = ib.Current();
+        R.surv_key = kb.Current();
+    }
+    for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r) {
+        R.t0 = t0;
+        R.t1 = t0 + final_round_tiles(rounds, r, t0, grid);
+        if (r > 0) CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+        if (shared_ks) {
+            build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+            LAUNCHED();
+        }
+        units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+        LAUNCHED();
+        if (rounds) {
+            merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
+            LAUNCHED();
+        }
+        t0 = R.t1;
+    }
     CU(cudaGetLastError());
     CU(cudaEventRecord(g0->ev_stage[4], stream));
     return B200BO_OK;

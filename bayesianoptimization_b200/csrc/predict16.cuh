@@ -506,8 +506,9 @@ enum {
     kCtlRefined = 5,  // candidates the refine stage looked at
     kCtlUnit = 6,     // next unit of predict_units_kernel in the lead stage
     kCtlKthLead = 7,  // the k-th key as it was before the lead stage
-    kCtlUnitFinal = 8,  // the same for the final stage
-    kCtlWords = 9
+    kCtlUnitFinal = 8,  // the same for the current final round
+    kCtlKthRound = 9,   // the k-th key as it was before the current final round (written by merge_kth_kernel)
+    kCtlWords = 10
 };
 
 // Prune mode of predict_acq16_kernel: thread 0 claims the next tile in bound order and stops the CTA (returns ntiles)
@@ -963,13 +964,94 @@ constexpr long long kCtlClosed = 1ll << 40;  // value of kCtlTile no batch reach
 struct RefineParams {
     const double2* mu;       // [m] interval (mu_lo, mu_hi) of K* alpha_ per candidate (local index), from the bound pass
     double* mu_unit;         // [kUnitSlots][PBN] K* alpha_ of a tile's candidates, from its last group's phase A
-    int* surv;               // [kRefineMaxTiles * PBN] local indices the refine stage let through
+    int* surv;               // [kRefineMaxTiles * PBN] local indices the refine stage let through (final: sorted)
+    unsigned long long* surv_key;  // [kRefineMaxTiles * PBN] their keys (max of single-point and refined key)
     double* part;            // [kUnitSlots][np / PBM][4][8][PBN] per-row-block partial sums of squares
     unsigned* arrive;        // [kUnitSlots] units that have delivered their part of a tile
     int blocks;              // leading row blocks of the refined bound
     int groups_max;          // most units a tile is split into
     int final_stage;         // predict_units_kernel: 0 lead, 1 final
+    int t0, t1;              // final stage: the round's tiles [t0, t1) of the survivor list
+    int round_skip;          // final stage: skip a tile whose first key is above kCtlKthRound
 };
+
+// The tiles of a lead stage or final round, the same in every CTA: candidates list[0, n), tiles [tbeg, tend) of
+// PBN columns, partial-sum slots from slot0.  Final stage: too many survivors leave n = 0 (the tile kernel takes over
+// in bound order); otherwise the stage closes the tile kernel's counter.
+struct UnitRound {
+    const int* list;
+    long long n, tbeg, tend;
+    int slot0;
+};
+__device__ __forceinline__ UnitRound unit_round(const PredictParams& P, const RefineParams& R) {
+    UnitRound U;
+    U.list = P.perm;
+    U.n = min(P.m, (long long)kLeadTiles * PBN);
+    U.slot0 = 0;
+    U.tbeg = 0;
+    if (R.final_stage) {
+        U.n = (long long)P.prune_ctl[kCtlSurv];
+        if (U.n > (long long)kRefineMaxTiles * PBN) U.n = 0;
+        else if (blockIdx.x == 0 && threadIdx.x == 0) atomicExch(P.prune_ctl + kCtlTile, (unsigned long long)kCtlClosed);
+        U.list = R.surv;
+        U.slot0 = kLeadTiles;
+        U.tbeg = R.t0;
+    }
+    U.tend = (U.n + PBN - 1) / PBN;
+    if (R.final_stage && U.tend > R.t1) U.tend = R.t1;
+    return U;
+}
+
+// whether every unit of tile `tile` skips it: its best bound key is above the k-th key copied before the stage / round
+__device__ __forceinline__ bool unit_skip(const PredictParams& P, const RefineParams& R, long long tile) {
+    if (!R.final_stage) return P.perm_key[tile * PBN] > P.prune_ctl[kCtlKthLead];
+    return R.round_skip && R.surv_key[tile * PBN] > P.prune_ctl[kCtlKthRound];
+}
+
+// The k-th smallest key over the union of the per-CTA lists (sel_cta, lists carried in by a continued batch included)
+// into kCtlKth, when there are k entries, and a copy of that word into kCtlKthRound for the next final round.  It is
+// the k-th smallest of values already produced, so the final k-th key is <= it.  One warp: k rounds of a merge of the
+// list heads.
+__global__ void __launch_bounds__(32) merge_kth_kernel(const SelList* __restrict__ lists, int nlists, int k,
+                                                        unsigned long long* ctl) {
+    __shared__ int head[1024];
+    const int lane = threadIdx.x;
+    for (int l = lane; l < nlists; l += 32) head[l] = 0;
+    __syncwarp();
+    unsigned long long kth = 0xFFFFFFFFFFFFFFFFull;
+    bool full = true;
+    for (int r = 0; r < k; ++r) {
+        unsigned long long bk = 0xFFFFFFFFFFFFFFFFull;
+        int bl = 0x7FFFFFFF;
+        for (int l = lane; l < nlists; l += 32) {
+            const int h = head[l];
+            if (h < k && lists[l].idx[h] != SEL_NOIDX && (lists[l].key[h] < bk || bl == 0x7FFFFFFF)) {
+                bk = lists[l].key[h];
+                bl = l;
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const unsigned long long ok = __shfl_xor_sync(0xffffffffu, bk, o);
+            const int ol = __shfl_xor_sync(0xffffffffu, bl, o);
+            if (ol != 0x7FFFFFFF && (bl == 0x7FFFFFFF || ok < bk || (ok == bk && ol < bl))) {
+                bk = ok;
+                bl = ol;
+            }
+        }
+        if (bl == 0x7FFFFFFF) {  // fewer than k entries
+            full = false;
+            break;
+        }
+        kth = bk;
+        if (lane == 0) head[bl] += 1;
+        __syncwarp();
+    }
+    if (lane == 0) {
+        if (full && kth < ctl[kCtlKth]) ctl[kCtlKth] = kth;
+        ctl[kCtlKthRound] = ctl[kCtlKth];
+    }
+}
 
 // first row block of group j of G over nb row blocks, cut so that the groups' k-tile counts (row block ib: ib + 1) are
 // about equal; j = G gives nb.  Groups may be empty.
@@ -1030,21 +1112,64 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
             const double r = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
             const double2 mu = R.mu[li];
             const unsigned long long key = prune_bound_key(P, G, mu.x, mu.y, prune_var_ub(G, r));
-            if (key <= kth && P.perm_key[c0 + c] <= kth) {
+            const unsigned long long key1 = P.perm_key[c0 + c];
+            if (key <= kth && key1 <= kth) {
                 const unsigned long long pos = atomicAdd(P.prune_ctl + kCtlSurv, 1ull);
-                if (pos < (unsigned long long)kRefineMaxTiles * PBN) R.surv[pos] = li;
+                if (pos < (unsigned long long)kRefineMaxTiles * PBN) {
+                    R.surv[pos] = li;
+                    R.surv_key[pos] = key > key1 ? key : key1;  // both are lower bounds
+                }
             }
         }
         __syncthreads();
     }
 }
 
+// K* of the tiles of a lead stage or final round (unit_round, unit_skip), each into its own scratch slot
+// (tile - tbeg; a round has at most gridDim.x tiles), with phase_a's arithmetic: items (tile, chunks [ch0, ch1)), the
+// chunks of a tile cut so that there are about gridDim.x items.  Plain stores: every unit of the tile reads the slot.
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT, 1) ks_build_kernel(const PredictParams P, const RefineParams R) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    const GpDev& G = P.gp[0];
+    const UnitRound U = unit_round(P, R);
+    const long long nt = U.tend - U.tbeg;
+    if (nt <= 0) return;
+    const int nch = G.np / PA_CHUNK;
+    const int per = (int)max(1ll, (nch * nt + gridDim.x - 1) / gridDim.x), items = (nch + per - 1) / per;
+    for (long long it = blockIdx.x; it < nt * items; it += gridDim.x) {
+        const long long tile = U.tbeg + it / items;
+        const int ch0 = (int)(it % items) * per, ch1 = min(nch, ch0 + per);
+        if (unit_skip(P, R, tile)) continue;
+        double* Ks = P.scratch + (tile - U.tbeg) * P.scratch_stride;
+        phase_a<P16_NT, DREG, KS_F64>(P, G, tile * PBN, Ks, smem, mu_s, 0ull, nullptr, U.list, U.n, ch1 * PA_CHUNK,
+                                      ch0 * PA_CHUNK);
+    }
+}
+
+// K* alpha_ of a tile from its K* slot, in phase_a's order: thread (part, column) runs one fma chain over the chunks in
+// ascending order, rows part * 16 .. part * 16 + 15 of each, so mu_s[part][c] is phase A's bit for bit.
+__device__ __forceinline__ void unit_mu_from_ks(const GpDev& G, const double* __restrict__ Ks,
+                                                double (*mu_s)[PBN]) {
+    constexpr int ROWS = PA_CHUNK / P16_SPLIT;
+    const int c = threadIdx.x & (PBN - 1), part = threadIdx.x >> 7;
+    double mu = 0.0;
+    for (int n0 = part * ROWS; n0 < G.np; n0 += PA_CHUNK) {
+#pragma unroll
+        for (int q = 0; q < ROWS; ++q) mu = fma(__ldg(G.alphav + n0 + q), __ldcg(Ks + (size_t)(n0 + q) * PBN + c), mu);
+    }
+    mu_s[part][c] = mu;
+}
+
 // Exact evaluation in units of (tile, group of consecutive row blocks).  Lead stage: the tiles are the first
 // kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this launch (a
 // continued batch; read from kCtlKthLead, which does not move, so that all units of a tile decide alike).  Final
-// stage: the tiles are the survivor list.  A unit builds K* for the rows its row blocks need in its CTA's scratch,
-// runs phase B over its row blocks, and the last unit to arrive finishes the tile as the tile kernel's epilogue does.
-template <bool DREG>
+// stage: the tiles [t0, t1) of the survivor list, with round_skip each skipped when its first key is above
+// kCtlKthRound.  A unit builds K* for the rows its row blocks need in its CTA's scratch (SHARED_KS: reads the tile's
+// slot that ks_build_kernel filled, and the unit of the last group computes mu from it), runs phase B over its row
+// blocks, and the last unit to arrive finishes the tile as the tile kernel's epilogue does.
+template <bool DREG, bool SHARED_KS>
 __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictParams P, const RefineParams R) {
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
@@ -1054,50 +1179,47 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
     const int tid = threadIdx.x;
     const GpDev& G = P.gp[0];
     const int nb = G.np / PBM;
-    double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
     const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last), pol_first = l2_policy_evict_first();
     if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
     __syncthreads();
-    // candidates of this stage, their tiles and the units per tile: the same in every CTA
-    const int* list = P.perm;
-    long long n = min(P.m, (long long)kLeadTiles * PBN);
-    int groups = R.groups_max, slot0 = 0;
-    unsigned long long* claim = P.prune_ctl + kCtlUnit;
-    if (R.final_stage) {
-        n = (long long)P.prune_ctl[kCtlSurv];
-        if (n > (long long)kRefineMaxTiles * PBN) n = 0;  // too many: the tile kernel takes over in bound order
-        else if (blockIdx.x == 0 && tid == 0) atomicExch(P.prune_ctl + kCtlTile, (unsigned long long)kCtlClosed);
-        list = R.surv;
-        slot0 = kLeadTiles;
-        claim = P.prune_ctl + kCtlUnitFinal;
-    }
-    const long long ntiles = (n + PBN - 1) / PBN;
-    if (R.final_stage && ntiles > 0)
-        groups = (int)max(1ll, min((long long)R.groups_max, 2ll * gridDim.x / ntiles));
+    const UnitRound U = unit_round(P, R);
+    const int* list = U.list;
+    const long long n = U.n;
+    unsigned long long* claim = P.prune_ctl + (R.final_stage ? kCtlUnitFinal : kCtlUnit);
+    int groups = R.groups_max;
+    if (R.final_stage && U.tend > U.tbeg)
+        groups = (int)max(1ll, min((long long)R.groups_max, 2ll * gridDim.x / (U.tend - U.tbeg)));
     for (;;) {
         if (tid == 0) unit_s = (long long)atomicAdd(claim, 1ull);
         __syncthreads();
         const long long unit = unit_s;
-        const long long tile = unit / groups;
-        if (tile >= ntiles) break;
+        const long long tile = U.tbeg + unit / groups;
+        if (tile >= U.tend) break;
         const long long c0 = tile * PBN;
-        if (!R.final_stage && P.perm_key[c0] > P.prune_ctl[kCtlKthLead]) {
+        if (unit_skip(P, R, tile)) {
             __syncthreads();
             continue;
         }
-        const int grp = (int)(unit - tile * groups);
+        const int grp = (int)(unit - (tile - U.tbeg) * groups);
         const int ib0 = unit_cut(nb, groups, grp), ib1 = unit_cut(nb, groups, grp + 1);
-        double* part = R.part + (size_t)(slot0 + tile) * nb * 32 * PBN;
+        const int slot = U.slot0 + (int)tile;
+        double* part = R.part + (size_t)slot * nb * 32 * PBN;
         if (ib1 > ib0) {
-            phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
-            predict16_phase_b<1684, true>(G, Ks, smem, pol_last, pol_first, ib0, ib1, part);
-            if (ib1 == nb && tid < PBN)  // phase A ran over all np rows: mu_s holds the tile kernel's K* alpha_ sums
-                R.mu_unit[(size_t)(slot0 + tile) * PBN + tid] =
-                    ((mu_s[0][tid] + mu_s[1][tid]) + mu_s[2][tid]) + mu_s[3][tid];
+            if constexpr (SHARED_KS) {
+                const double* Ks = P.scratch + (tile - U.tbeg) * P.scratch_stride;
+                if (ib1 == nb) unit_mu_from_ks(G, Ks, mu_s);
+                predict16_phase_b<1684, true>(G, Ks, smem, pol_last, l2_policy_evict_last(0.f), ib0, ib1, part);
+            } else {
+                double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
+                phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
+                predict16_phase_b<1684, true>(G, Ks, smem, pol_last, pol_first, ib0, ib1, part);
+            }
+            if (ib1 == nb && tid < PBN)  // mu_s holds the tile kernel's K* alpha_ parts (phase A over all np rows)
+                R.mu_unit[(size_t)slot * PBN + tid] = ((mu_s[0][tid] + mu_s[1][tid]) + mu_s[2][tid]) + mu_s[3][tid];
         }
         __threadfence();  // this unit's partials and mu before its arrival
         __syncthreads();
-        if (tid == 0) last_s = atomicAdd(R.arrive + slot0 + tile, 1u) == (unsigned)groups - 1;
+        if (tid == 0) last_s = atomicAdd(R.arrive + slot, 1u) == (unsigned)groups - 1;
         __syncthreads();
         if (last_s) {
             __threadfence();
@@ -1110,7 +1232,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
                 const long long gi = valid ? (long long)list[c0 + c] : P.m;
                 const double colsq = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
                 double val = 0.0, base, prod;
-                const double mu_n = valid ? __ldcg(R.mu_unit + (size_t)(slot0 + tile) * PBN + c) : 0.0;
+                const double mu_n = valid ? __ldcg(R.mu_unit + (size_t)slot * PBN + c) : 0.0;
                 candidate_epilogue(P, G, 0, mu_n, colsq, gi, base, prod, &val);
                 runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, valid);
                 if (tid == 0) {

@@ -457,7 +457,8 @@ constexpr int PA_CHUNK = 64;  // training rows per staged chunk
 //   KS_KMAX    nowhere: each thread keeps the largest |K*_i| of its rows in kmax_s[part][c] (the bound pass of pruning)
 // mu_s[part][c] is the part's share of K* alpha_; each caller adds the NT / PBN parts in its fixed order.
 // Column c is candidate c0 + c of the first mlim, or perm[c0 + c] when perm is set (tiles in bound order); rows: the
-// leading training rows to build (a multiple of PA_CHUNK; G.np for all of them - mu_s is K* alpha_ only then).
+// leading training rows to build (a multiple of PA_CHUNK; G.np for all of them - mu_s is K* alpha_ only then); row0
+// (a multiple of PA_CHUNK, 0 but in ks_build_kernel): the rows before it are skipped, mu_s is then meaningless.
 enum { KS_F64, KS_F64_EF, KS_TF32, KS_KMAX };
 
 __device__ __forceinline__ void st_global_hint(double* p, double v, unsigned long long pol) {
@@ -468,7 +469,7 @@ template <int NT, bool DREG, int KS, int KSTR, int COV>
 __device__ __forceinline__ void phase_a_impl(const PredictParams& P, const GpDev& G, long long c0,
                                              double* __restrict__ Ks, double* smem, double (*mu_s)[PBN],
                                              unsigned long long pol_first, double (*kmax_s)[PBN], const int* perm,
-                                             long long mlim, int rows) {
+                                             long long mlim, int rows, int row0) {
     constexpr int ROWS = PA_CHUNK / (NT / PBN);  // rows of every chunk per thread
     const int tid = threadIdx.x;
     const int d = P.d, np = G.np;
@@ -493,8 +494,8 @@ __device__ __forceinline__ void phase_a_impl(const PredictParams& P, const GpDev
     // The 256-thread kernels always build all np rows; they take np from G here rather than rows from the call site,
     // because where that load sits steers their instruction schedule (read at the call, fp32 mode ran 0.2 % slower on an
     // H100 80GB HBM3 at 700 W).
-    const int nch = (NT == PNT ? np : rows) / PA_CHUNK;
-    load_chunk(0, 0);
+    const int nch = (NT == PNT ? np : rows) / PA_CHUNK, ch0 = row0 / PA_CHUNK;
+    load_chunk(ch0 & 1, ch0);
     cp_async_commit();
     __syncthreads();  // xc_s visible
     const int c = tid & (PBN - 1), part = tid >> 7;  // part in [0, NT / PBN)
@@ -505,7 +506,7 @@ __device__ __forceinline__ void phase_a_impl(const PredictParams& P, const GpDev
     }
     double mu_acc = 0.0, kmax = 0.0;
     constexpr int R = 8;
-    for (int ch = 0; ch < nch; ++ch) {
+    for (int ch = ch0; ch < nch; ++ch) {
         if (ch + 1 < nch) load_chunk((ch + 1) & 1, ch + 1);
         cp_async_commit();
         cp_async_wait<1>();
@@ -597,12 +598,21 @@ __device__ __forceinline__ void phase_a_impl(const PredictParams& P, const GpDev
 template <int NT, bool DREG, int KS, int KSTR = PBN>
 __device__ __forceinline__ void phase_a(const PredictParams& P, const GpDev& G, long long c0, double* __restrict__ Ks,
                                         double* smem, double (*mu_s)[PBN], unsigned long long pol_first,
-                                        double (*kmax_s)[PBN], const int* perm, long long mlim, int rows) {
+                                        double (*kmax_s)[PBN], const int* perm, long long mlim, int rows,
+                                        int row0 = 0) {
     switch (cov_code(G.family, G.nu)) {
-        case 0: phase_a_impl<NT, DREG, KS, KSTR, 0>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-        case 1: phase_a_impl<NT, DREG, KS, KSTR, 1>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-        case 2: phase_a_impl<NT, DREG, KS, KSTR, 2>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
-        default: phase_a_impl<NT, DREG, KS, KSTR, 3>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows); break;
+        case 0:
+            phase_a_impl<NT, DREG, KS, KSTR, 0>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows, row0);
+            break;
+        case 1:
+            phase_a_impl<NT, DREG, KS, KSTR, 1>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows, row0);
+            break;
+        case 2:
+            phase_a_impl<NT, DREG, KS, KSTR, 2>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows, row0);
+            break;
+        default:
+            phase_a_impl<NT, DREG, KS, KSTR, 3>(P, G, c0, Ks, smem, mu_s, pol_first, kmax_s, perm, mlim, rows, row0);
+            break;
     }
 }
 

@@ -1,7 +1,10 @@
 """Where the kernel time of a pruned selection call goes, stage by stage (DESIGN.md 4.9, 6), and the A/B of the refine
-stages (B200BO_PRUNE_REFINE=0/1) in one process, then bench.py per setting, alternated.
+stages' switches in one process, then bench.py per setting, alternated.
 
   python tools/prune_stages.py [--settings 0,1] [--reps 3] [--calls 3] [--legs c3,c2,c5,philox,worst] [--bench-runs 2]
+
+A setting is a value of B200BO_PRUNE_REFINE, or switches joined by '+', e.g. the stages without and with their
+rounds and shared K*:  --settings ROUNDS=0+SHARED_KS=0,ROUNDS=1+SHARED_KS=1  (names without B200BO_PRUNE_).
 
 Legs as in tools/prune_ab.py (argmin + top-10; Matern-2.5, alpha 1e-6, normalize_y).  Per leg and setting:
 b200bo_last_kernel_ms mean (min-max), the stage split of b200bo_last_prune_stage_ms (bound pass, sort, lead, refine,
@@ -26,6 +29,20 @@ from predict_pipe_ab import Sampler, card  # noqa: E402
 from prune_ab import ALPHA, K, LEGS, XI  # noqa: E402
 
 STAGES = ("bound", "sort", "lead", "refine", "final", "tiles")
+SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_ROUNDS", "B200BO_PRUNE_SHARED_KS")
+
+
+def setting_env(s):
+    """environment variables of a setting: a bare value of B200BO_PRUNE_REFINE, or NAME=V joined by '+'"""
+    if "=" not in s:
+        return {"B200BO_PRUNE_REFINE": s}
+    return {"B200BO_PRUNE_" + k: v for k, v in (kv.split("=", 1) for kv in s.split("+"))}
+
+
+def apply_setting(s):
+    for v in SWITCHES:
+        os.environ.pop(v, None)
+    os.environ.update(setting_env(s))
 
 
 def leg(name, settings, reps, calls, exact):
@@ -73,7 +90,7 @@ def leg(name, settings, reps, calls, exact):
     res = {s: {"ms": [], "st": [], "clocks": []} for s in settings}
     for _ in range(reps):
         for s in settings:
-            os.environ["B200BO_PRUNE_REFINE"] = s
+            apply_setting(s)
             call()  # warm-up of this setting
             with Sampler() as smp:
                 for _ in range(calls):
@@ -82,12 +99,13 @@ def leg(name, settings, reps, calls, exact):
                     res[s]["st"].append(st)
             res[s]["clocks"].extend(smp.samples)
             res[s].update(evaluated=ev, refined=ref, total=tot, sel=rec)
-    os.environ.pop("B200BO_PRUNE_REFINE", None)
+    apply_setting("1")
+    os.environ.pop("B200BO_PRUNE_REFINE")
     base = float(np.mean(res[settings[0]]["ms"]))
     for s in settings:
         t, c, st = np.array(res[s]["ms"]), np.array(res[s]["clocks"]), np.array(res[s]["st"]).mean(0)
         print(json.dumps({
-            "leg": name, "B200BO_PRUNE_REFINE": int(s), "kernel_ms_mean": round(float(t.mean()), 3),
+            "leg": name, "setting": s, "kernel_ms_mean": round(float(t.mean()), 3),
             "kernel_ms_min_max": [round(float(t.min()), 3), round(float(t.max()), 3)],
             "speedup_vs_first_setting": round(base / float(t.mean()), 3),
             "stage_ms": {k: round(float(v), 3) for k, v in zip(STAGES, st)},
@@ -105,7 +123,8 @@ def leg(name, settings, reps, calls, exact):
 def bench_ab(args, settings):
     for run in range(args.bench_runs):
         for s in settings:
-            env = dict(os.environ, B200BO_PRUNE_REFINE=s)
+            env = {k: v for k, v in os.environ.items() if k not in SWITCHES}
+            env.update(setting_env(s))
             cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(args.bench_steps),
                    "--warmup", str(args.bench_warmup), "--no-cpu-baseline"]
             with Sampler() as smp:
@@ -115,7 +134,7 @@ def bench_ab(args, settings):
                 if ln.startswith("{"):
                     line = json.loads(ln)
                     break
-            rec = {"leg": "bench", "run": run, "B200BO_PRUNE_REFINE": int(s), "rc": r.returncode, **smp.medians()}
+            rec = {"leg": "bench", "run": run, "setting": s, "rc": r.returncode, **smp.medians()}
             if line is not None:
                 rec["line"] = line
             else:
@@ -125,7 +144,7 @@ def bench_ab(args, settings):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--settings", default="0,1", help="values of B200BO_PRUNE_REFINE, alternated")
+    ap.add_argument("--settings", default="0,1", help="settings of the switches (see above), alternated")
     ap.add_argument("--reps", type=int, default=3, help="alternations of the settings at c3")
     ap.add_argument("--calls", type=int, default=3, help="timed launches per setting and alternation at c3")
     ap.add_argument("--legs", default="c3,c2,c5,philox,worst")
