@@ -1,8 +1,8 @@
 """bayesianoptimization_b200 - a H100-native GP-surrogate + acquisition engine that drops in
 behind ``bayes_opt.BayesianOptimization.suggest()`` and the ``bayes_opt.acquisition`` classes.
 
-Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI/MES/LogEI/LogPoI/NEI/LogNEI (x constraint probability) ->
-argmin/top-k, in hand-written sm_90a CUDA behind the C ABI declared in include/b200bo.h.
+Hot path: GP fit -> batched posterior predict -> UCB/EI/PoI/MES/LogEI/LogPoI/NEI/LogNEI (x constraint probability)
+or CNEI/LogCNEI -> argmin/top-k, in hand-written sm_90a CUDA behind the C ABI declared in include/b200bo.h.
 No CPU fallback: importing the compute classes without the built library raises ImportError.
 
 Two layers:
@@ -10,7 +10,8 @@ Two layers:
     PosteriorPaths, ConstrainedPaths (posterior sample paths, resolved lazily)
   * acquisition seam (a plug-in for the ``bayes_opt`` package, which must be importable):
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, LogExpectedImprovement,
-    LogProbabilityOfImprovement, NoisyExpectedImprovement, LogNoisyExpectedImprovement, ThompsonSampling,
+    LogProbabilityOfImprovement, NoisyExpectedImprovement, LogNoisyExpectedImprovement,
+    ConstrainedNoisyExpectedImprovement, LogConstrainedNoisyExpectedImprovement, ThompsonSampling,
     ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, KrigingBeliever, PendingNEI, GPHedge,
     AcquisitionFunction, ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
 """
@@ -30,7 +31,9 @@ _PLUGIN = {
     "ThompsonSampling": "acquisition", "ConstrainedThompsonSampling": "acquisition",
     "MaxValueEntropySearch": "acquisition", "suggest_batch": "acquisition", "KrigingBeliever": "acquisition",
     "NoisyExpectedImprovement": "acquisition", "LogNoisyExpectedImprovement": "acquisition",
-    "PendingNEI": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths", "ConstrainedPaths": "paths",
+    "PendingNEI": "acquisition", "ConstrainedNoisyExpectedImprovement": "acquisition",
+    "LogConstrainedNoisyExpectedImprovement": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths",
+    "ConstrainedPaths": "paths",
 }
 
 

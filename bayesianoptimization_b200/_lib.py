@@ -14,6 +14,7 @@ OK, ERR_CUDA, ERR_ARG, ERR_NOT_PD, ERR_UNSUPPORTED, ERR_STATE = 0, -1, -2, -3, -
 KERNEL_MATERN, KERNEL_RBF = 0, 1
 NU_05, NU_15, NU_25, NU_INF = 0, 1, 2, 3
 ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE, ACQ_MES, ACQ_LOGEI, ACQ_LOGPOI, ACQ_NEI, ACQ_LOGNEI = 0, 1, 2, 3, 4, 6, 7, 8, 9
+ACQ_CNEI, ACQ_LOGCNEI = 10, 11
 MAX_GPS, MAX_DIM, MAX_TOPK, MAX_PATHS = 8, 64, 64, 16
 XFORM_IDENTITY, XFORM_ROUND = 0, 1
 GET_L, GET_ALPHA, GET_YSTATS, GET_K, GET_LINV = 0, 1, 2, 3, 4
@@ -36,7 +37,7 @@ EXPORTS = [
     "b200bo_paths_argmin_topk_philox", "b200bo_paths_bound", "b200bo_cpaths_eval", "b200bo_cpaths_argmin_topk",
     "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
     "b200bo_acq_value_grad", "b200bo_paths_grad_rows", "b200bo_gp_fork", "b200bo_gp_condition",
-    "b200bo_gp_set_fantasies", "b200bo_gp_condition_fantasies",
+    "b200bo_gp_set_fantasies", "b200bo_gp_condition_fantasies", "b200bo_gp_set_fantasy_incumbent",
 ]
 
 
@@ -129,6 +130,7 @@ def lib():
     L.b200bo_gp_fork.argtypes = [C.c_void_p, C.c_int64, C.POINTER(C.c_void_p)]
     L.b200bo_gp_condition.argtypes = [C.c_void_p, dp, C.c_int64, dp]
     L.b200bo_gp_condition_fantasies.argtypes = [C.c_void_p, dp, C.c_int64, dp, dp, dp]
+    L.b200bo_gp_set_fantasy_incumbent.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), dp]
     L.b200bo_multi_gpu_acq_argmin_topk.argtypes = [C.POINTER(AcqSpec), C.c_int, dp, C.c_int64, C.c_int, dp,
                                                    i64p, dp, i64p]
     L.b200bo_multi_gpu_acq_argmin_topk_philox.argtypes = [C.POINTER(AcqSpec), C.c_int, C.c_uint64, dp, dp,

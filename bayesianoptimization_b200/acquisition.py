@@ -22,7 +22,8 @@ from q paths (batch Thompson sampling).  ``MaxValueEntropySearch`` is the
 information-based policy: samples of the maximum from posterior paths, then a fused-kernel epilogue of mu and sigma.
 ``KrigingBeliever`` gives UCB / EI / PoI / MES pending points and batches: the fitted GP is conditioned on the points in
 flight on the device, with its own mean as their targets; ``PendingNEI`` does the same for noisy EI by drawing the
-pending values jointly with its fantasies.  ``LogExpectedImprovement`` and
+pending values jointly with its fantasies; ``ConstrainedNoisyExpectedImprovement`` adds fantasies of noisy constraints
+and a sampled-feasibility incumbent.  ``LogExpectedImprovement`` and
 ``LogProbabilityOfImprovement`` are EI and PoI in log space, finite and well scaled where EI and PoI underflow.
 
 ``bayes_opt`` must be importable (this package is a plug-in for it).  The GP seam
@@ -31,6 +32,7 @@ pending values jointly with its fantasies.  ``LogExpectedImprovement`` and
 from __future__ import annotations
 
 import abc
+import ctypes as C
 import warnings
 
 import numpy as np
@@ -673,6 +675,105 @@ class LogNoisyExpectedImprovement(_NoisyEI):
     _nei_kind = B.ACQ_LOGNEI
 
 
+def cnei_eligible(space_in_bounds, constraint_fantasies, lb, ub):
+    """The (n, S) incumbent mask of constrained NEI (DESIGN.md 4.15): row i may be sample s's incumbent when it lies
+    within the bounds (``space_in_bounds``, (n,)) and lb_j <= F_j[i, s] <= ub_j for every constraint j."""
+    ok = np.asarray(space_in_bounds, dtype=bool)[:, None]
+    for j, F in enumerate(constraint_fantasies):
+        ok = ok & (lb[j] <= F) & (F <= ub[j])
+    return ok
+
+
+def _in_bounds(space):
+    """The bounds part of ``target_space.mask``: the registered rows inside the parameter bounds."""
+    p, b = np.asarray(space.params), np.asarray(space.bounds)
+    return np.all((b[:, 0] <= p) & (p <= b[:, 1]), axis=1)
+
+
+class _ConstrainedNoisyEI(_NoisyEI):
+    """Constrained noisy expected improvement (Letham, Karrer, Ottoni & Bakshy, "Constrained Bayesian Optimization with
+    Noisy Experiments", Bayesian Analysis 2019; DESIGN.md 4.15): NEI whose constraints are noisy too.  Each constraint
+    GP gets fantasies of its own, and per sample s
+
+        CNEI(x) = (1/S) sum_s EI(mu_s(x) - best_s - xi, sigma0(x)) * prod_j P_js(x),
+
+    with P_js the probability that constraint j lies in [lb_j, ub_j] under its noiseless GP conditioned on sample s of
+    its fantasies, and best_s the largest target fantasy over the rows that lie within the bounds and that sample s
+    calls feasible.  A sample with no such row takes the smallest target fantasy over all registered rows as its
+    incumbent: a floor, against which EI still rewards objective value and feasibility together.  So the class ranks
+    candidates before any feasible point is registered and never raises NoValidPointRegisteredError (it still raises
+    TargetSpaceEmptyError on an empty space).
+
+    Every ``suggest()`` refuses before any draw (more than 7 constraints, multi-device GPs, a GP conditioned on pending
+    points), then draws from the RandomState it receives: the target's Z, E, then per constraint j in order its Z_j,
+    E_j (``noiseless_fantasies``), then the reference's random stage and refinement (refine="analytic": the device
+    gradient of CNEI).  Parameters, get/set_acquisition_params and saved state are NoisyExpectedImprovement's.
+    Without a constraint it is NoisyExpectedImprovement (LogNoisyExpectedImprovement), the same draws and values.  With
+    constraint GPs fitted as the reference fits them (alpha = 1e-6, no WhiteKernel term) the constraint fantasies are
+    the observed values and the value is NEI times the probability of feasibility; make the constraint GPs noisy, for
+    example ``m.set_params(kernel=Matern(nu=2.5) + WhiteKernel())`` for each ``m`` in ``optimizer.constraint.model``,
+    to model constraint noise.  ``PendingNEI`` accepts it and refuses constraints."""
+
+    _cnei_kind = None
+
+    def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        # ExpectedImprovement.suggest without its NoValidPointRegisteredError: y_max is not used by (C)NEI
+        self._path_rng = _ensure_rng(random_state)
+        self._suggest_space = target_space
+        try:
+            self.y_max = target_space._target_max()
+            x = _ref.AcquisitionFunction.suggest(self, gp, target_space, n_random=n_random, n_smart=n_smart,
+                                                 fit_gp=fit_gp, random_state=self._path_rng)
+            self.decay_exploration()
+            return x
+        finally:
+            self._path_rng = None
+            self._suggest_space = None
+
+    def _closure(self, gp, constraint, space, pending=None, extra_rows=0):
+        if constraint is None:
+            return super()._closure(gp, constraint, space, pending=pending, extra_rows=extra_rows)
+        models = [_as_b200_gp(m) for m in constraint.model]
+        for g in [gp, *models]:  # before any draw: a refusal consumes no random numbers
+            if len(g.device_list()) > 1:
+                raise NotImplementedError("constrained noisy expected improvement runs on one device: a GP is "
+                                          "multi-device")
+            if g.__dict__.get("_b200_conditioned") is not None:
+                raise NotImplementedError("constrained noisy expected improvement on a GP conditioned on pending "
+                                          "points")
+        if (pending is not None and len(pending)) or extra_rows:
+            raise _ConstraintNotSupportedError("pending points with constraints are not supported")
+        self.fantasies = self.constraint_fantasies = None
+        rs = self._suggest_rng()
+        fant = gp.noiseless_fantasies(self.n_samples, self.jitter, random_state=rs)
+        cfant = [m.noiseless_fantasies(self.n_samples, self.jitter, random_state=rs) for m in models]
+        ok = cnei_eligible(_in_bounds(space), [f.F for f in cfant], np.atleast_1d(constraint.lb),
+                           np.atleast_1d(constraint.ub))
+        eligible = np.ascontiguousarray(ok, dtype=np.uint8)
+        best = np.empty(self.n_samples)
+        B.check(B.lib().b200bo_gp_set_fantasy_incumbent(fant.handle.ptr, eligible.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                        B.as_dp(best)))
+        fant.best = best
+        self.fantasies, self.constraint_fantasies = fant, cfant
+        return FusedAcquisition(self._cnei_kind, gp, constraint, owner=self, fantasies=fant,
+                                constraint_fantasies=cfant)
+
+
+class ConstrainedNoisyExpectedImprovement(_ConstrainedNoisyEI):
+    __doc__ = _ConstrainedNoisyEI.__doc__
+    _nei_kind = B.ACQ_NEI
+    _cnei_kind = B.ACQ_CNEI
+
+
+class LogConstrainedNoisyExpectedImprovement(_ConstrainedNoisyEI):
+    """Log constrained noisy expected improvement: log CNEI(x) = log of the mean over the samples of
+    EI_s * prod_j P_js, formed from LogEI's tail-safe terms plus sum_j log P_js (Ament et al. 2023), finite where CNEI
+    underflows.  Otherwise ConstrainedNoisyExpectedImprovement; without a constraint it is LogNoisyExpectedImprovement."""
+
+    _nei_kind = B.ACQ_LOGNEI
+    _cnei_kind = B.ACQ_LOGCNEI
+
+
 def _refuse_nei(acq, where):
     if isinstance(acq, _NoisyEI):
         raise TypeError(f"{where} does not support {type(acq).__name__}: its fantasies are drawn per suggest() against "
@@ -910,6 +1011,6 @@ class PendingNEI(_PendingBatch):
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, LogExpectedImprovement,
              LogProbabilityOfImprovement, ConstantLiar, GPHedge, ThompsonSampling, ConstrainedThompsonSampling,
              MaxValueEntropySearch, KrigingBeliever, NoisyExpectedImprovement, LogNoisyExpectedImprovement,
-             PendingNEI):
+             ConstrainedNoisyExpectedImprovement, LogConstrainedNoisyExpectedImprovement, PendingNEI):
     AcquisitionFunction.register(_cls)
 del _cls

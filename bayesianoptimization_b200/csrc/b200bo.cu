@@ -285,6 +285,11 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    // the CNEI / LogCNEI instantiations
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<true, 1684, PIPE_BULK_MC, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
@@ -918,6 +923,44 @@ extern "C" int b200bo_gp_set_fantasies(b200bo_gp* nl, const b200bo_gp* ny, const
     return B200BO_OK;
 }
 
+// Per-sample incumbents of CNEI (include/b200bo.h, DESIGN.md 4.15): best_s from the fantasies F the handle keeps
+// ([S][np], normalised), in data units as b200bo_gp_set_fantasies forms them, with the empty-sample floor.
+extern "C" int b200bo_gp_set_fantasy_incumbent(b200bo_gp* nl, const uint8_t* eligible, double* best_out) {
+    if (!nl || !eligible) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!nl->fitted) return set_err(B200BO_ERR_STATE, "GP handle is not fitted");
+    if (nl->replica) return set_err(B200BO_ERR_STATE, "handle is a predict-only replica");
+    if (nl->fant_best.empty())
+        return set_err(B200BO_ERR_STATE, "the handle holds no fantasies (b200bo_gp_set_fantasies)");
+    if (nl->fant_nreg != nl->n)
+        return set_err(B200BO_ERR_STATE, "the fantasies are conditioned on pending rows");
+    const int n = (int)nl->n, np = nl->np, S = (int)nl->fant_best.size();
+    CU(cudaSetDevice(nl->device));
+    StreamScope scope(nl);
+    int rc;
+    std::vector<double> F((size_t)S * np);
+    if ((rc = d2h(F.data(), nl->fant_f.p, sizeof(double) * F.size()))) return rc;
+    std::vector<double> best(S);
+    for (int s = 0; s < S; ++s) {
+        double hi = -std::numeric_limits<double>::infinity(), lo = std::numeric_limits<double>::infinity();
+        bool any = false;
+        for (int i = 0; i < n; ++i) {
+            const double v = nl->y_std * F[(size_t)s * np + i] + nl->y_mean;
+            lo = std::fmin(lo, v);
+            if (eligible[(size_t)i * S + s]) {
+                hi = std::fmax(hi, v);
+                any = true;
+            }
+        }
+        best[s] = any ? hi : lo;
+    }
+    if ((rc = h2d(nl->fant_a.as<double>() + (size_t)np * S, best.data(), sizeof(double) * S))) return rc;
+    if ((rc = sync_fit_stream())) return rc;
+    nl->fant_best = best;
+    if (best_out)
+        for (int s = 0; s < S; ++s) best_out[s] = best[s];
+    return B200BO_OK;
+}
+
 // Row n of the O(N^2) factor update at the hyper-parameters of the last fit, shared by b200bo_gp_append and
 // b200bo_gp_condition: row n of X / Xs, row and column n of K, row n of L (pivot checked) and of L^-1 (W and WT).
 // tvec: n-entry device scratch.  believer (nullable, device): receives k(x, X) . alpha_ in normalised units, computed
@@ -1477,9 +1520,12 @@ static void predict16_config(int grid, cudaStream_t stream, bool pair, cudaLaunc
 template <int MMA, int PIPE>
 static int launch_predict16(bool dreg, int grid, cudaStream_t stream, const PredictParams& P) {
     auto fn = dreg ? predict_acq16_kernel<true, MMA, PIPE> : predict_acq16_kernel<false, MMA, PIPE>;
-    if constexpr (PIPE != PIPE_CPASYNC) {  // NEI / LogNEI: bulk-copy pipes only (DESIGN.md 4.13)
+    if constexpr (PIPE != PIPE_CPASYNC) {  // NEI / LogNEI, CNEI / LogCNEI: bulk-copy pipes only (DESIGN.md 4.13, 4.15)
         if (acq_is_nei(P.acq_kind))
             fn = dreg ? predict_acq16_kernel<true, MMA, PIPE, true> : predict_acq16_kernel<false, MMA, PIPE, true>;
+        else if (acq_is_cnei(P.acq_kind))
+            fn = dreg ? predict_acq16_kernel<true, MMA, PIPE, false, true>
+                      : predict_acq16_kernel<false, MMA, PIPE, false, true>;
     }
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
@@ -1844,6 +1890,19 @@ static int check_spec(const b200bo_acq* spec) {
         return set_err(B200BO_ERR_STATE, "MES: gps[0] holds no samples of the maximum (b200bo_gp_set_max_values)");
     if (acq_is_nei(spec->kind) && spec->gps[0]->fant_best.empty())
         return set_err(B200BO_ERR_STATE, "NEI: gps[0] holds no fantasies (b200bo_gp_set_fantasies)");
+    if (acq_is_cnei(spec->kind)) {  // every GP a noiseless handle with fantasies of the same S and n
+        const b200bo_gp* g0 = spec->gps[0];
+        for (int g = 0; g < spec->n_gps; ++g) {
+            const b200bo_gp* gp = spec->gps[g];
+            if (gp->fant_best.empty())
+                return set_err(B200BO_ERR_STATE, "CNEI: gps[%d] holds no fantasies (b200bo_gp_set_fantasies)", g);
+            if (gp->fant_best.size() != g0->fant_best.size())
+                return set_err(B200BO_ERR_ARG, "CNEI: gps[%d] holds %d fantasies, gps[0] %d", g,
+                               (int)gp->fant_best.size(), (int)g0->fant_best.size());
+            if (gp->n != g0->n || gp->np != g0->np)
+                return set_err(B200BO_ERR_ARG, "CNEI: gps[%d] has a different training set size", g);
+        }
+    }
     return B200BO_OK;
 }
 
@@ -1913,9 +1972,11 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
     if (spec->kind == B200BO_ACQ_MES) {
         P.n_ystar = (int)g0->ystar.size();
         for (int k = 0; k < P.n_ystar; ++k) P.ystar[k] = g0->ystar[k];
-    } else if (acq_is_nei(spec->kind)) {  // A and best_s on the device
+    } else if (acq_uses_fantasies(spec->kind)) {  // A and best_s on the device
         P.n_ystar = (int)g0->fant_best.size();
         P.fant_a = g0->fant_a.as<double>();
+        if (acq_is_cnei(spec->kind))
+            for (int g = 0; g < spec->n_gps; ++g) P.fant_a_gp[g] = spec->gps[g]->fant_a.as<double>();
     }
     P.Xc = src.philox ? nullptr : src.d_Xc;
     P.index_base = index_base;
@@ -1936,7 +1997,7 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
 // finish for every GP.
 static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool grad, cudaStream_t stream) {
     b200bo_gp* g0 = spec->gps[0];
-    const bool nei = acq_is_nei(spec->kind);
+    const bool nei = acq_is_nei(spec->kind), cnei = acq_is_cnei(spec->kind);
     int rc;
     for (int g = 0; g < spec->n_gps; ++g) {
         b200bo_gp* gp = spec->gps[g];
@@ -1950,7 +2011,8 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
         Q.unit_tab = gp->s_unit.as<int2>();
         Q.rb_tab = gp->s_rb.as<int2>();
         S.nunits[g] = gp->s_nunits;
-        if (grad && g == 0 && nei) {  // S mean lists + the u list per block (small_grad_kernel<true>)
+        // S mean lists + the u list per block (small_grad_kernel<true>): gps[0] of NEI, every GP of CNEI
+        if (grad && ((g == 0 && nei) || cnei)) {
             const size_t lists = g0->fant_best.size() + 1;
             if ((rc = gp->s_gpart.reserve(sizeof(double) * (size_t)SMAXP * (gp->np / 128) * lists * gp->d * SMC)))
                 return rc;
@@ -1980,7 +2042,10 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
                 small_reduce_kernel<1><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
                 small_trsv_kernel<true><<<dim3(gp->s_nunits_u, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
                 small_reduce_kernel<2><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
-                if (nei && g == 0)
+                if (cnei)
+                    small_grad_kernel<true, true><<<dim3(gp->np / 128, npass, (unsigned)g0->fant_best.size()), 256,
+                                                    0, stream>>>(S, g);
+                else if (nei && g == 0)
                     small_grad_kernel<true><<<dim3(gp->np / 128, npass, (unsigned)g0->fant_best.size()), 256, 0,
                                               stream>>>(S, g);
                 else
@@ -1990,10 +2055,14 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
             }
             for (int i = 0; i < (grad ? 6 : 3); ++i) LAUNCHED();
         }
-        if (grad)
+        if (grad && cnei)
+            small_finish_grad_cnei_kernel<<<npass, 256, 0, stream>>>(S);
+        else if (grad)
             (nei ? small_finish_grad_kernel<true> : small_finish_grad_kernel<false>)<<<npass, 256, 0, stream>>>(S);
         else if (nei)
             small_finish_kernel<true><<<npass, 256, 0, stream>>>(S);
+        else if (cnei)
+            small_finish_kernel<false, true><<<npass, 256, 0, stream>>>(S);
         else
             small_finish_kernel<false><<<npass, 256, 0, stream>>>(S);
         LAUNCHED();
@@ -2040,8 +2109,9 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
     if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
     if (k > 0 && !d_sel) return set_err(B200BO_ERR_ARG, "d_sel is NULL");
     b200bo_gp* g0 = spec->gps[0];
-    // NEI / LogNEI: no single mean to report; always fp64 (the 16-warp kernel or the small-batch kernels)
-    const bool nei = acq_is_nei(spec->kind);
+    // NEI / LogNEI, CNEI / LogCNEI: no single mean to report; always fp64 (the 16-warp kernel or the small-batch
+    // kernels)
+    const bool nei = acq_uses_fantasies(spec->kind);
     if (nei && (d_mu || d_sd))
         return set_err(B200BO_ERR_ARG, "NEI averages over fantasies and has no single posterior mean: mu / sd outputs "
                                        "are not available");
@@ -2090,6 +2160,10 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             return set_err(B200BO_ERR_UNSUPPORTED, "NEI runs on the bulk-copy phase-B pipes only (B200BO_PREDICT_PIPE="
                                                    "cpasync / B200BO_PREDICT_MMA=884 select a pipe without it)");
         P.scratch_stride = (long long)np_max * (pipe == PIPE_CPASYNC ? PBN : PSTR_DMMA);
+        if (acq_is_cnei(spec->kind)) {  // the per-sample carry of CNEI behind K*, one column per candidate
+            P.carry_off = P.scratch_stride;
+            P.scratch_stride += (long long)P.n_ystar * PSTR_DMMA;
+        }
         if ((rc = g0->pscratch.reserve(sizeof(double) * (size_t)P.scratch_stride * g0->sm_count))) return rc;
         P.scratch = g0->pscratch.as<double>();
         CU(cudaEventRecord(g0->ev0, stream));

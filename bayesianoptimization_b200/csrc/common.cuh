@@ -14,9 +14,16 @@ constexpr int kPad = 128;  // training-set size is padded to a multiple of this
 __host__ __device__ constexpr bool acq_is_nei(int kind) {
     return kind == B200BO_ACQ_NEI || kind == B200BO_ACQ_LOGNEI;
 }
+// CNEI / LogCNEI (DESIGN.md 4.15): every GP of the call holds fantasies; served by their own kernel instantiations
+__host__ __device__ constexpr bool acq_is_cnei(int kind) {
+    return kind == B200BO_ACQ_CNEI || kind == B200BO_ACQ_LOGCNEI;
+}
+// the kinds that average over fantasies: no single mean, fp64 on the 16-warp bulk pipes and the small-batch kernels
+__host__ __device__ constexpr bool acq_uses_fantasies(int kind) { return acq_is_nei(kind) || acq_is_cnei(kind); }
 __host__ __device__ constexpr bool acq_kind_valid(int kind) {
     return kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_EI || kind == B200BO_ACQ_POI || kind == B200BO_ACQ_NONE ||
-           kind == B200BO_ACQ_MES || kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI || acq_is_nei(kind);
+           kind == B200BO_ACQ_MES || kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI ||
+           acq_uses_fantasies(kind);
 }
 // The log-space kinds: the value is -(alpha + sum_j log p_j), the constraint factors summed as logs.  NEI = false in
 // the kernels built without NEI / LogNEI (DESIGN.md 4.13), which then test for LogEI and LogPoI only.

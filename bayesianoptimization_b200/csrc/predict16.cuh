@@ -871,8 +871,10 @@ __device__ __forceinline__ void predict16_phase_b_bulk(const PredictParams& P, c
 // PIPE: phase B data path; PIPE_BULK_MC is launched in clusters of 2 CTAs, and the two CTAs of a cluster run the
 // same number of tiles: when the pair's second tile lies past the batch (odd tile count), the second CTA runs it
 // with every column masked (c0 >= m: zero coordinates, no output, no selection entry).
-// NEI: the instantiation that serves B200BO_ACQ_NEI / LOGNEI (candidate_epilogue<true>).
-template <bool DREG, int MMA, int PIPE, bool NEI = false>
+// NEI: the instantiation that serves B200BO_ACQ_NEI / LOGNEI (candidate_epilogue<true>).  CNEI: the one that serves
+// B200BO_ACQ_CNEI / LOGCNEI: each GP's pass hands cnei_term that GP's K* column, and the S running terms of a
+// candidate wait between the passes in the CTA's scratch slot behind K* (P.carry_off, the column's stride).
+template <bool DREG, int MMA, int PIPE, bool NEI = false, bool CNEI = false>
 __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictParams P) {
     static_assert(PIPE == PIPE_CPASYNC || MMA == 1684, "the bulk-copy phase B runs on m16n8k4");
     extern __shared__ __align__(16) double smem[];
@@ -926,8 +928,12 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
                 const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
                 const long long gi = (P.perm && c0 + c < P.m) ? (long long)P.perm[c0 + c] : c0 + c;
                 double val = 0.0;
-                candidate_epilogue<NEI>(P, G, g, mu_n, colsq, gi, base_s[c], prod_s[c], &val, Ks + c,
-                                        PIPE == PIPE_CPASYNC ? PBN : PSTR_DMMA);
+                if constexpr (CNEI)
+                    candidate_epilogue<false, false, true>(P, G, g, mu_n, colsq, gi, base_s[c], prod_s[c], &val,
+                                                           Ks + c, PSTR_DMMA, nullptr, Ks + P.carry_off + c);
+                else
+                    candidate_epilogue<NEI>(P, G, g, mu_n, colsq, gi, base_s[c], prod_s[c], &val, Ks + c,
+                                            PIPE == PIPE_CPASYNC ? PBN : PSTR_DMMA);
                 if (P.sel_cta && g == P.n_gps - 1) {
                     runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, c0 + c < P.m);
                     if (P.perm && tid == 0 && sel_s.list.idx[P.sel_k - 1] != SEL_NOIDX)

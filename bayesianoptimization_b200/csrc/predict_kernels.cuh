@@ -71,6 +71,11 @@ struct PredictParams {
     unsigned long long* prune_ctl;  // [0] next tile to claim, [1] least k-th key of a full CTA list, [2] evaluated
     // NEI / LogNEI (DESIGN.md 4.13): A = K0^-1 F of gps[0], [np][n_ystar] row-major, then best_0 .. best_{n_ystar-1}
     const double* fant_a;
+    // CNEI / LogCNEI (DESIGN.md 4.15): A_g = K0_g^-1 F_g of every GP g ([np][n_ystar]); fant_a is gps[0]'s, best_s
+    // behind it.  Here rather than in GpDev, so that the struct every other kernel reads keeps its layout.
+    const double* fant_a_gp[B200BO_MAX_GPS];
+    // predict_acq16_kernel: offset (doubles) of each CTA's per-sample carry [n_ystar][PSTR_DMMA] in its scratch slot
+    long long carry_off;
 };
 
 // coordinate j of candidate gi (local index) as the reference's x_tries[gi, j]
@@ -314,6 +319,72 @@ __device__ __noinline__ double nei_term(int kind, const double* __restrict__ kco
     return mx + log(e) - log((double)S);
 }
 
+// CNEI / LogCNEI (DESIGN.md 4.15) of one candidate, GP g of n_gps, out of line like nei_term.  The S fantasy means
+// y_std k*^T a_gs + y_mean of GP g come from its K* column kcol (kcol[i * kstr]) and A_g, summed as in nei_term.  g = 0
+// forms the per-sample target terms EI_s (LogEI_s), each constraint GP multiplies in P_gs (adds log P_gs), and the
+// running terms wait in carry[s * kstr] between the GP passes of a candidate.  At the last GP the terms are reduced
+// over s exactly as nei_term reduces them (returned value alpha); before it the return value is unused.
+__device__ __noinline__ double cnei_term(int kind, int g, int n_gps, const double* __restrict__ kcol, int kstr, int n,
+                                         const double* __restrict__ A, const double* __restrict__ best, int S,
+                                         double y_std, double y_mean, double xi, double lb, double ub, double sd,
+                                         double* __restrict__ carry) {
+    double t[B200BO_MAX_PATHS];
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s) t[s] = 0.0;
+    for (int i = 0; i < n; ++i) {
+        const double k = kcol[(size_t)i * kstr];
+        const double* a = A + (size_t)i * S;
+#pragma unroll
+        for (int s = 0; s < B200BO_MAX_PATHS; ++s)
+            if (s < S) t[s] = fma(a[s], k, t[s]);
+    }
+    const bool lg = kind == B200BO_ACQ_LOGCNEI, last = g == n_gps - 1;
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s) {
+        if (s < S) {
+            const double mean = y_std * t[s] + y_mean;
+            double v;
+            if (g == 0) {
+                v = lg ? log_acq_term(B200BO_ACQ_LOGEI, mean - best[s] - xi, sd) : nei_ei_term(mean - best[s] - xi, sd);
+            } else if (lg) {
+                v = carry[s * kstr] + log_cfactor(lb, ub, mean, sd);
+            } else {
+                const double p_lo = (lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(lb, mean, sd);
+                const double p_hi = (ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(ub, mean, sd);
+                v = carry[s * kstr] * (p_hi - p_lo);
+            }
+            if (last)
+                t[s] = v;
+            else
+                carry[s * kstr] = v;
+        }
+    }
+    if (!last) return 0.0;
+    if (!lg) {
+        double sum = 0.0;
+#pragma unroll
+        for (int s = 0; s < B200BO_MAX_PATHS; ++s)
+            if (s < S) sum += t[s];
+        return sum / (double)S;
+    }
+    double mx = -CUDART_INF;
+    bool nan = false;
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s) {
+        if (s < S) {
+            nan = nan || isnan(t[s]);
+            mx = fmax(mx, t[s]);
+        }
+    }
+    if (nan) return CUDART_NAN;
+    if (mx == -CUDART_INF) return -CUDART_INF;
+    double e = 0.0;
+#pragma unroll
+    for (int s = 0; s < B200BO_MAX_PATHS; ++s)
+        if (s < S) e += exp(t[s] - mx);
+    return mx + log(e) - log((double)S);
+}
+
 // ---- per-candidate epilogue shared by the tiled and the small-batch kernels ---------------------
 // mu_n: K* alpha_ (normalised units); colsq: sum_i V_i^2.  g = 0: target GP -> base acquisition;
 // g >= 1: constraint GP -> probability factor.  The last GP writes -base * prod.
@@ -332,12 +403,14 @@ struct EpilogueGrad {
     double* cms;  // NEI: the coefficients of d mu_s, cms[s * kstr] (nei_term); cm is 0
 };
 
-template <bool NEI = false, bool GRAD = false>
+// CNEI (template flag of the instantiations that serve CNEI / LogCNEI only, value form): every GP's pass goes to
+// cnei_term over GP g's K* column kcol, with the per-sample carry at carry[s * kstr]; the last GP writes -alpha.
+template <bool NEI = false, bool GRAD = false, bool CNEI = false>
 __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const GpDev& G, int g,
                                                    double mu_n, double colsq, long long gi,
                                                    double& base_neg, double& prod, double* final_val = nullptr,
                                                    const double* kcol = nullptr, int kstr = 0,
-                                                   EpilogueGrad* gr = nullptr) {
+                                                   EpilogueGrad* gr = nullptr, double* carry = nullptr) {
     const bool logk = acq_constraints_in_log<NEI>(P.acq_kind);
     const double mean = G.y_std * mu_n + G.y_mean;
     double var = G.prior - colsq;
@@ -346,6 +419,18 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
         if (P.clamp_count && gi < P.m) atomicAdd(P.clamp_count, 1ull);
     }
     const double sd = sqrt(var * (G.y_std * G.y_std));
+    if constexpr (CNEI) {
+        static_assert(!GRAD && !NEI, "CNEI has a value form only");
+        const double a = cnei_term(P.acq_kind, g, P.n_gps, kcol, kstr, G.n, P.fant_a_gp[g],
+                                   P.fant_a + (size_t)P.gp[0].np * P.n_ystar, P.n_ystar, G.y_std, G.y_mean, P.xi,
+                                   G.lb, G.ub, sd, carry);
+        if (g == P.n_gps - 1) {
+            const double val = -1.0 * a;
+            if (final_val) *final_val = val;
+            if (P.acq_out && gi < P.m) P.acq_out[gi] = val;
+        }
+        return;
+    }
     double term = 0.0, cm = 0.0, cs = 0.0;
     if (g == 0) {
         if (P.acq_kind == B200BO_ACQ_UCB) {
@@ -1275,13 +1360,15 @@ __device__ __forceinline__ void small_finish_sums(const SmallParams& S, int pass
     }
 }
 
-// Per pass (blockIdx.x): the sums above, then the per-candidate epilogue of every GP (NEI: the NEI / LogNEI kinds).
-template <bool NEI>
+// Per pass (blockIdx.x): the sums above, then the per-candidate epilogue of every GP (NEI: the NEI / LogNEI kinds;
+// CNEI: the CNEI / LogCNEI kinds, each GP with its own K* column and the per-sample carry in shared memory).
+template <bool NEI, bool CNEI = false>
 __global__ void __launch_bounds__(256)
 small_finish_kernel(const SmallParams S) {
     __shared__ double red[8][SMC];
     __shared__ double colsq_s[B200BO_MAX_GPS][SMC];
     __shared__ double mu_s[B200BO_MAX_GPS][SMC];
+    __shared__ double carry_s[CNEI ? B200BO_MAX_PATHS : 1][SMC];
     const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
     const int pass = blockIdx.x, mc = small_pass_mc(S, pass);
     const long long pc0 = small_pass_c0(S, pass);
@@ -1289,9 +1376,12 @@ small_finish_kernel(const SmallParams S) {
     if (sl == 0 && c < mc) {
         double base_neg = 0.0, prod = 1.0;
         const double* kcol = S.sg[0].ksm + (size_t)pass * S.P.gp[0].np * SMC + c;  // gps[0]'s K* column (NEI)
-        for (int g = 0; g < S.P.n_gps; ++g)
-            candidate_epilogue<NEI>(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg, prod, nullptr,
-                                    kcol, SMC);
+        for (int g = 0; g < S.P.n_gps; ++g) {
+            if constexpr (CNEI)
+                kcol = S.sg[g].ksm + (size_t)pass * S.P.gp[g].np * SMC + c;
+            candidate_epilogue<NEI, false, CNEI>(S.P, S.P.gp[g], g, mu_s[g][c], colsq_s[g][c], pc0 + c, base_neg,
+                                                 prod, nullptr, kcol, SMC, nullptr, CNEI ? &carry_s[0][c] : nullptr);
+        }
     }
 }
 
@@ -1305,8 +1395,9 @@ small_finish_kernel(const SmallParams S) {
 // coefficients of each row, then thread = (candidate, dimensions j = jg, jg + 8, ..) adds the 32 rows in order.
 // NEI (gps[0] of an NEI / LogNEI call): blockIdx.z = fantasy s, the first list takes a_s = column s of A instead of
 // alpha_, and gpart holds S + 1 lists per block: [b][s][j][c] for s < S, then the u list (written by s = 0).
+// CNEI (every GP of a CNEI / LogCNEI call, with NEI): the same lists from GP g's own A_g (PredictParams::fant_a_gp).
 constexpr int SGR = 32;  // rows per sub-chunk
-template <bool NEI>
+template <bool NEI, bool CNEI = false>
 __global__ void __launch_bounds__(256)
 small_grad_kernel(const SmallParams S, int g) {
     const GpDev& G = S.P.gp[g];
@@ -1342,7 +1433,9 @@ small_grad_kernel(const SmallParams S, int g) {
                     r2 = fma(df, df, r2);
                 }
                 const double ch = G.constv * cov_dh_from_r2(r2, G.family, G.nu);
-                if constexpr (NEI)
+                if constexpr (CNEI)
+                    ca = S.P.fant_a_gp[g][(size_t)n * S.P.n_ystar + blockIdx.z] * ch;
+                else if constexpr (NEI)
                     ca = S.P.fant_a[(size_t)n * S.P.n_ystar + blockIdx.z] * ch;
                 else
                     ca = G.alphav[n] * ch;
@@ -1483,6 +1576,174 @@ small_finish_grad_kernel(const SmallParams S) {
             }
             const double wa = wa_s[g][cc], wu = wu_s[g][cc];
             gr += ((wa == 0.0 ? 0.0 : wa * a) + (wu == 0.0 ? 0.0 : wu * u)) / G.ls[j];
+        }
+        S.grad_out[(pc0 + cc) * d + j] = isnan(val_s[cc]) ? CUDART_NAN : gr;
+    }
+}
+
+// CNEI / LogCNEI gradient coefficients of one candidate (b200bo_acq_value_grad, DESIGN.md 4.15), out of line: the
+// value as cnei_term forms it (same means, same products in j order, same sums in s order), and
+//   wn[(g * B200BO_MAX_PATHS + s) * SMC] = the coefficient of d mu_gs,   wsig[g] = that of d sigma0_g   (data units).
+// CNEI = -(1/S) sum_s T_s, T_s = EI_s prod_j P_js: by the product rule per sample, without dividing by a P,
+//   d T_s = prod_j P_js dEI_s + EI_s sum_j (prod_{k != j} P_ks) dP_js     (prefix and suffix products over j);
+// LogCNEI = -logmeanexp_s l_s, l_s = LogEI_s + sum_j log P_js: d = -sum_s p_s d l_s, p_s = exp(l_s - M) / sum exp(l - M).
+// EI_s / LogEI_s give Phi / phi (LogEI's r / sd, q / sd), the factors EI's (log_cfactor's) coefficients; sd = 0 makes a
+// GP's coefficients 0.  kcol[g]: GP g's K* column (stride SMC).
+__device__ __noinline__ double cnei_grad_term(const PredictParams& P, const double* const* kcol, const double* sdv,
+                                              double* wn, double* wsig) {
+    const int S = P.n_ystar, ng = P.n_gps;
+    const bool lg = P.acq_kind == B200BO_ACQ_LOGCNEI;
+    const double* best = P.fant_a + (size_t)P.gp[0].np * S;
+    double T[B200BO_MAX_PATHS], cm0[B200BO_MAX_PATHS], cs0[B200BO_MAX_PATHS];
+    double pf[B200BO_MAX_GPS][B200BO_MAX_PATHS], pcm[B200BO_MAX_GPS][B200BO_MAX_PATHS],
+        pcs[B200BO_MAX_GPS][B200BO_MAX_PATHS];
+    for (int g = 0; g < ng; ++g) {
+        const GpDev& G = P.gp[g];
+        const double* A = P.fant_a_gp[g];
+        const double sd = sdv[g];
+        wsig[g] = 0.0;
+        for (int s = 0; s < S; ++s) {
+            double t = 0.0;
+            for (int i = 0; i < G.n; ++i) t = fma(A[(size_t)i * S + s], kcol[g][(size_t)i * SMC], t);
+            const double mean = G.y_std * t + G.y_mean;
+            if (g == 0) {
+                T[s] = lg ? log_acq_term<true>(B200BO_ACQ_LOGEI, mean - best[s] - P.xi, sd, &cm0[s], &cs0[s])
+                          : nei_ei_term<true>(mean - best[s] - P.xi, sd, &cm0[s], &cs0[s]);
+                continue;
+            }
+            double cm = 0.0, cs = 0.0, v;
+            if (lg) {
+                v = log_cfactor<true>(G.lb, G.ub, mean, sd, &cm, &cs);
+            } else {
+                const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
+                const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
+                v = p_hi - p_lo;
+                if (sd > 0.0) {
+                    if (G.lb != -CUDART_INF) {
+                        const double z = (G.lb - mean) / sd, pz = norm_pdf(z);
+                        cm += pz / sd;
+                        cs += pz == 0.0 ? 0.0 : z * pz / sd;
+                    }
+                    if (G.ub != CUDART_INF) {
+                        const double z = (G.ub - mean) / sd, pz = norm_pdf(z);
+                        cm -= pz / sd;
+                        cs -= pz == 0.0 ? 0.0 : z * pz / sd;
+                    }
+                }
+            }
+            pf[g][s] = v;
+            pcm[g][s] = cm;
+            pcs[g][s] = cs;
+        }
+    }
+    double val;
+    if (!lg) {
+        double sum = 0.0;
+        for (int s = 0; s < S; ++s) {
+            double t = T[s];
+            for (int g = 1; g < ng; ++g) t = t * pf[g][s];
+            sum += t;
+        }
+        val = -1.0 * (sum / (double)S);
+        const double w = -1.0 / (double)S;
+        for (int s = 0; s < S; ++s) {
+            double suf[B200BO_MAX_GPS + 1];  // suf[g] = prod_{k >= g} P_ks
+            suf[ng] = 1.0;
+            for (int g = ng - 1; g >= 1; --g) suf[g] = pf[g][s] * suf[g + 1];
+            wn[s * SMC] = w * suf[1] * cm0[s];
+            wsig[0] += w * suf[1] * cs0[s];
+            double pre = T[s];  // EI_s prod_{k < g} P_ks
+            for (int g = 1; g < ng; ++g) {
+                const double o = w * pre * suf[g + 1];
+                wn[(g * B200BO_MAX_PATHS + s) * SMC] = o * pcm[g][s];
+                wsig[g] += o * pcs[g][s];
+                pre = pre * pf[g][s];
+            }
+        }
+        return val;
+    }
+    double mx = -CUDART_INF;
+    bool nan = false;
+    for (int s = 0; s < S; ++s) {
+        for (int g = 1; g < ng; ++g) T[s] = T[s] + pf[g][s];
+        nan = nan || isnan(T[s]);
+        mx = fmax(mx, T[s]);
+    }
+    for (int g = 0; g < ng; ++g)
+        for (int s = 0; s < S; ++s) wn[(g * B200BO_MAX_PATHS + s) * SMC] = 0.0;
+    if (nan) return CUDART_NAN;
+    if (mx == -CUDART_INF) return CUDART_INF;
+    double e = 0.0;
+    for (int s = 0; s < S; ++s) e += exp(T[s] - mx);
+    for (int s = 0; s < S; ++s) {
+        const double w = -exp(T[s] - mx) / e;
+        wn[s * SMC] = w * cm0[s];
+        wsig[0] += w * cs0[s];
+        for (int g = 1; g < ng; ++g) {
+            wn[(g * B200BO_MAX_PATHS + s) * SMC] = w * pcm[g][s];
+            wsig[g] += w * pcs[g][s];
+        }
+    }
+    return -1.0 * (mx + log(e) - log((double)S));
+}
+
+// Gradient finish of CNEI / LogCNEI, per pass (blockIdx.x): per candidate cnei_grad_term, then per dimension
+//   grad_j = sum_g ( sum_s wn_gs (-y_std_g) sum_b list_gs[b][j] + wu_g sum_b u_g[b][j] ) / ls_gj,
+//   wu_g = wsig_g y_std_g / sqrt(var_g)  (0 where var_g <= 0),
+// over the S + 1 lists per block small_grad_kernel<true, true> wrote for every GP.
+__global__ void __launch_bounds__(256)
+small_finish_grad_cnei_kernel(const SmallParams S) {
+    __shared__ double red[8][SMC];
+    __shared__ double colsq_s[B200BO_MAX_GPS][SMC];
+    __shared__ double mu_s[B200BO_MAX_GPS][SMC];
+    __shared__ double wu_s[B200BO_MAX_GPS][SMC];
+    __shared__ double val_s[SMC];
+    __shared__ double wn_s[B200BO_MAX_GPS * B200BO_MAX_PATHS][SMC];
+    const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
+    const int pass = blockIdx.x, mc = small_pass_mc(S, pass), d = S.P.d, ng = S.P.n_gps, nl = S.P.n_ystar + 1;
+    const long long pc0 = small_pass_c0(S, pass);
+    small_finish_sums(S, pass, red, colsq_s, mu_s);
+    if (sl == 0 && c < mc) {
+        const double* kcol[B200BO_MAX_GPS];
+        double sdv[B200BO_MAX_GPS], var[B200BO_MAX_GPS], wsig[B200BO_MAX_GPS];
+        for (int g = 0; g < ng; ++g) {
+            const GpDev& G = S.P.gp[g];
+            kcol[g] = S.sg[g].ksm + (size_t)pass * G.np * SMC + c;
+            double v = G.prior - colsq_s[g][c];
+            if (v < 0.0) {
+                v = 0.0;
+                if (S.P.clamp_count) atomicAdd(S.P.clamp_count, 1ull);
+            }
+            var[g] = v;
+            sdv[g] = sqrt(v * (G.y_std * G.y_std));
+        }
+        const double val = cnei_grad_term(S.P, kcol, sdv, &wn_s[0][c], wsig);
+        for (int g = 0; g < ng; ++g)
+            wu_s[g][c] = var[g] > 0.0 && wsig[g] != 0.0 ? wsig[g] * S.P.gp[g].y_std / sqrt(var[g]) : 0.0;
+        val_s[c] = val;
+        if (S.P.acq_out) S.P.acq_out[pc0 + c] = val;
+    }
+    __syncthreads();
+    for (int idx = tid; idx < SMC * d; idx += 256) {
+        const int cc = idx & 31, j = idx >> 5;
+        if (cc >= mc) continue;
+        double gr = 0.0;
+        for (int g = 0; g < ng; ++g) {
+            const GpDev& G = S.P.gp[g];
+            if (G.xform && xform_rounds(G.xform[j])) continue;
+            const int nb = G.np / 128;
+            const double* gp = S.sg[g].gpart + (size_t)pass * nb * nl * d * SMC;
+            double an = 0.0, u = 0.0;
+            for (int s = 0; s < nl - 1; ++s) {
+                const double wn = wn_s[g * B200BO_MAX_PATHS + s][cc];
+                if (wn == 0.0) continue;
+                double a = 0.0;
+                for (int b = 0; b < nb; ++b) a += gp[(((size_t)b * nl + s) * d + j) * SMC + cc];
+                an += -G.y_std * wn * a;
+            }
+            for (int b = 0; b < nb; ++b) u += gp[(((size_t)b * nl + nl - 1) * d + j) * SMC + cc];
+            const double wu = wu_s[g][cc];
+            gr += (an + (wu == 0.0 ? 0.0 : wu * u)) / G.ls[j];
         }
         S.grad_out[(pc0 + cc) * d + j] = isnan(val_s[cc]) ? CUDART_NAN : gr;
     }

@@ -43,7 +43,8 @@ _NEEDS_Y_MAX = (B.ACQ_EI, B.ACQ_POI, B.ACQ_LOGEI, B.ACQ_LOGPOI)
 class FusedAcquisition:
     """Callable closure over fitted device GPs.
 
-    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES / ACQ_LOGEI / ACQ_LOGPOI / ACQ_NEI / ACQ_LOGNEI
+    kind      B.ACQ_UCB / ACQ_EI / ACQ_POI / ACQ_MES / ACQ_LOGEI / ACQ_LOGPOI / ACQ_NEI / ACQ_LOGNEI / ACQ_CNEI /
+              ACQ_LOGCNEI
     gp        fitted B200GaussianProcessRegressor (target)
     constraint  object with .model (list of device GPs), .lb, .ub  (bayes_opt ConstraintModel) or None
     params    either fixed ``kappa``/``xi``/``y_max`` values or ``owner``: an acquisition object whose
@@ -54,22 +55,39 @@ class FusedAcquisition:
               over one GP, called alternately, each see their own samples.
     fantasies   ACQ_NEI / ACQ_LOGNEI only: ``gp.noiseless_fantasies(...)``.  The spec's gps[0] is its noiseless handle;
               candidate transforms and the device come from ``gp``.  One device; always fp64 (DESIGN.md 4.13).
+              ACQ_CNEI / ACQ_LOGCNEI: the target's, as for NEI.
+    constraint_fantasies  ACQ_CNEI / ACQ_LOGCNEI only: one ``noiseless_fantasies`` per constraint GP, in
+              ``constraint.model`` order, each with the S of ``fantasies``.  The spec's gps[j] are their noiseless handles
+              (DESIGN.md 4.15).
     """
 
     def __init__(self, kind, gp, constraint=None, kappa=0.0, xi=0.0, y_max=None, owner=None, max_values=None,
-                 fantasies=None):
+                 fantasies=None, constraint_fantasies=None):
         gp = _as_b200_gp(gp)
         self.kind = int(kind)
         self._ystar = None
         self._fant = None
-        if self.kind in (B.ACQ_NEI, B.ACQ_LOGNEI):
+        self._cfant = None
+        if self.kind in (B.ACQ_CNEI, B.ACQ_LOGCNEI):
+            n_con = 0 if constraint is None else len(constraint.model)
+            cf = list(constraint_fantasies or [])
+            if fantasies is None or len(cf) != n_con:
+                raise ValueError("CNEI needs the target's fantasies and one per constraint GP "
+                                 "(B200GaussianProcessRegressor.noiseless_fantasies)")
+            if any(len(g.device_list()) > 1 for g in [gp, *(constraint.model if n_con else [])]):
+                raise NotImplementedError("constrained noisy expected improvement runs on one device: a GP is "
+                                          "multi-device")
+            self._fant, self._cfant = fantasies, cf
+        elif constraint_fantasies is not None:
+            raise ValueError("constraint_fantasies belong to ACQ_CNEI / ACQ_LOGCNEI only")
+        elif self.kind in (B.ACQ_NEI, B.ACQ_LOGNEI):
             if fantasies is None:
                 raise ValueError("NEI needs fantasies (B200GaussianProcessRegressor.noiseless_fantasies)")
             if len(gp.device_list()) > 1:
                 raise NotImplementedError("noisy expected improvement runs on one device: the GP is multi-device")
             self._fant = fantasies
         elif fantasies is not None:
-            raise ValueError("fantasies belong to ACQ_NEI / ACQ_LOGNEI only")
+            raise ValueError("fantasies belong to ACQ_NEI / ACQ_LOGNEI / ACQ_CNEI / ACQ_LOGCNEI only")
         if self.kind == B.ACQ_MES:
             ys = B.c_f64(np.asarray(max_values if max_values is not None else [], dtype=np.float64).reshape(-1))
             if not 1 <= ys.size <= B.MAX_PATHS or not np.all(np.isfinite(ys)):
@@ -113,6 +131,8 @@ class FusedAcquisition:
         handles = [g._device_handles() for g in self._gps]  # [gp][device]
         if self._fant is not None:
             handles[0] = [self._fant.handle]  # the noiseless handle holding the fantasies
+        for j, f in enumerate(self._cfant or []):
+            handles[1 + j] = [f.handle]
         sig = tuple(h.ptr.value for hs in handles for h in hs)
         kappa, xi, y_max = self._params()
         if self.kind in _NEEDS_Y_MAX and y_max is None:

@@ -93,6 +93,24 @@ extern "C" {
  * p_s = exp(l_s - M) / sum exp(l - M) (LogEI's per-fantasy derivative, softmax-weighted). */
 #define B200BO_ACQ_NEI 8
 #define B200BO_ACQ_LOGNEI 9
+/* Constrained noisy expected improvement and its log (Letham et al. 2019, with noisy constraints; DESIGN.md 4.15).
+ * No counterpart in the reference.  Every GP of the call is a NOISELESS handle holding fantasies with the same S and
+ * n: gps[0] the target's (b200bo_gp_set_fantasies, then usually b200bo_gp_set_fantasy_incumbent for best_s), gps[j],
+ * j >= 1, constraint j's (A_j = K0_j^-1 F_j; its best_s are not used).  With mu_s and sigma0 from gps[0] as for NEI,
+ * mu_js = y_std_j k_j*^T a_js + y_mean_j and sigma0_j the posterior sd of gps[j] (data units):
+ *   P_js = Phi((ub_j - mu_js)/sigma0_j) - Phi((lb_j - mu_js)/sigma0_j)   (the factor rules of EI's constraints)
+ *   CNEI:    alpha = (1/S) sum_{s=0..S-1}, in s order, EI(a_s, sigma0) * P_1s * .. * P_Js       (products in j order)
+ *   LOGCNEI: alpha = M + log sum_s exp(l_s - M) - log S,  l_s = LogEI(a_s, sigma0) + sum_j log P_js  (log_cfactor)
+ *            (-inf when every l_s is -inf; NaN when any l_s is NaN)
+ *   acq_neg = -alpha.
+ * Without constraint GPs (n_gps = 1) the value is NEI / LOGNEI.  Served where NEI is (the 16-warp fp64 kernel on its
+ * bulk-copy pipes with host, device and Philox candidates, and the small-batch kernels); everything NEI refuses returns
+ * B200BO_ERR_UNSUPPORTED.  b200bo_acq_value_grad serves both kinds (small-batch path), by the product rule per sample:
+ * d CNEI = (1/S) sum_s [prod_j P_js dEI_s + EI_s sum_j (prod_{k != j} P_ks) dP_js]; d LOGCNEI = sum_s p_s d l_s with
+ * p_s = exp(l_s - M) / sum exp(l - M).  Never pruned.  mu / sd outputs: B200BO_ERR_ARG.  A GP
+ * without fantasies: B200BO_ERR_STATE; handles with different S or n: B200BO_ERR_ARG. */
+#define B200BO_ACQ_CNEI 10
+#define B200BO_ACQ_LOGCNEI 11
 
 #define B200BO_MAX_GPS 8   /* 1 target GP + up to 7 constraint GPs per call */
 #define B200BO_MAX_DIM 64  /* max input dimension d */
@@ -197,6 +215,16 @@ int b200bo_gp_set_max_values(b200bo_gp* gp, const double* ystar, int K);
  * or set_transform on `noiseless` drops the fantasies; an NEI call on it then returns B200BO_ERR_STATE. */
 int b200bo_gp_set_fantasies(b200bo_gp* noiseless, const b200bo_gp* noisy, const double* z, const double* e, int S,
                             const uint8_t* incumbent, double* f_out, double* best_out);
+
+/* Per-sample incumbents for B200BO_ACQ_CNEI / B200BO_ACQ_LOGCNEI (DESIGN.md 4.15).  eligible: (n, S) host mask,
+ * row-major: eligible[i*S + s] != 0 when row i may be sample s's incumbent (in the caller's rule: within the bounds
+ * and feasible under sample s's constraint fantasies).  Recomputes, on the device copy and the host copy,
+ *   best_s = max over eligible rows i of (y_std F_is + y_mean),
+ *   or, when no row is eligible in sample s, min over all n rows of (y_std F_is + y_mean)
+ * (a floor: EI against it still rewards objective value and feasibility together).  best_out (nullable, (S,) host)
+ * receives best_s.  NULL handle or mask -> B200BO_ERR_ARG; not fitted, a replica, no fantasies, or fantasies
+ * conditioned on pending rows -> B200BO_ERR_STATE.  A later fit, append or condition drops them with the fantasies. */
+int b200bo_gp_set_fantasy_incumbent(b200bo_gp* noiseless, const uint8_t* eligible, double* best_out);
 
 /* Replaces the tail of GaussianProcessRegressor.fit (SK/gaussian_process/_gpr.py:275-285,
  * :349-367): y normalisation, K = k(X,X), K_ii += alpha, L = chol(K), alpha_ = K^-1 y, plus
