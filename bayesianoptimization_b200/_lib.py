@@ -38,6 +38,7 @@ EXPORTS = [
     "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
     "b200bo_acq_value_grad", "b200bo_paths_grad_rows", "b200bo_gp_fork", "b200bo_gp_condition",
     "b200bo_gp_set_fantasies", "b200bo_gp_condition_fantasies", "b200bo_gp_set_fantasy_incumbent",
+    "b200bo_gp_set_constrained_incumbent",
 ]
 
 
@@ -131,6 +132,8 @@ def lib():
     L.b200bo_gp_condition.argtypes = [C.c_void_p, dp, C.c_int64, dp]
     L.b200bo_gp_condition_fantasies.argtypes = [C.c_void_p, dp, C.c_int64, dp, dp, dp]
     L.b200bo_gp_set_fantasy_incumbent.argtypes = [C.c_void_p, C.POINTER(C.c_uint8), dp]
+    L.b200bo_gp_set_constrained_incumbent.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, dp, dp,
+                                                      C.POINTER(C.c_uint8), dp]
     L.b200bo_multi_gpu_acq_argmin_topk.argtypes = [C.POINTER(AcqSpec), C.c_int, dp, C.c_int64, C.c_int, dp,
                                                    i64p, dp, i64p]
     L.b200bo_multi_gpu_acq_argmin_topk_philox.argtypes = [C.POINTER(AcqSpec), C.c_int, C.c_uint64, dp, dp,

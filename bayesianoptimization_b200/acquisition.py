@@ -647,6 +647,10 @@ class _NoisyEI(_SuggestStream, DeviceHooks, _ref.ExpectedImprovement):
         self.fantasies = fant
         return FusedAcquisition(self._nei_kind, gp, constraint, owner=self, fantasies=fant)
 
+    def _extender(self, constraint):
+        """PendingNEI's round step for the latest closure: extends its fantasies in place to a pick (d,)."""
+        return self.fantasies.condition_on_pending
+
     def get_acquisition_params(self):
         return {**super().get_acquisition_params(), "n_samples": self.n_samples, "jitter": self.jitter}
 
@@ -686,8 +690,16 @@ def cnei_eligible(space_in_bounds, constraint_fantasies, lb, ub):
 
 def _in_bounds(space):
     """The bounds part of ``target_space.mask``: the registered rows inside the parameter bounds."""
-    p, b = np.asarray(space.params), np.asarray(space.bounds)
+    return _rows_in_bounds(space.params, space.bounds)
+
+
+def _rows_in_bounds(rows, bounds):
+    p, b = np.asarray(rows), np.asarray(bounds)
     return np.all((b[:, 0] <= p) & (p <= b[:, 1]), axis=1)
+
+
+def _which_gp(j):
+    return "the target GP" if j == 0 else f"constraint GP {j - 1} (constraint.model[{j - 1}])"
 
 
 class _ConstrainedNoisyEI(_NoisyEI):
@@ -712,7 +724,13 @@ class _ConstrainedNoisyEI(_NoisyEI):
     constraint GPs fitted as the reference fits them (alpha = 1e-6, no WhiteKernel term) the constraint fantasies are
     the observed values and the value is NEI times the probability of feasibility; make the constraint GPs noisy, for
     example ``m.set_params(kernel=Matern(nu=2.5) + WhiteKernel())`` for each ``m`` in ``optimizer.constraint.model``,
-    to model constraint noise.  ``PendingNEI`` accepts it and refuses constraints."""
+    to model constraint noise.  The incumbents are formed on the device (``b200bo_gp_set_constrained_incumbent``).
+
+    ``PendingNEI`` gives it pending points and batches with constraints (DESIGN.md 4.16): the target's and every
+    constraint's fantasies are drawn jointly with their values at the pending points (per GP in order: Z, E, then
+    ``standard_normal((p + q - 1, S))``), a pending row counts toward sample s's incumbent only where sample s's
+    constraint fantasies call it feasible (and it lies within the bounds), and each round extends every GP to the pick
+    (``condition_on_pending``).  A batch built round by round is greedy sequential constrained qNEI."""
 
     _cnei_kind = None
 
@@ -731,32 +749,75 @@ class _ConstrainedNoisyEI(_NoisyEI):
             self._suggest_space = None
 
     def _closure(self, gp, constraint, space, pending=None, extra_rows=0):
+        """The closure over the fantasies of the target and of every constraint GP; ``pending`` ((p, d)) and
+        ``extra_rows`` as in ``noiseless_fantasies``, for every GP (PendingNEI, DESIGN.md 4.16)."""
         if constraint is None:
             return super()._closure(gp, constraint, space, pending=pending, extra_rows=extra_rows)
         models = [_as_b200_gp(m) for m in constraint.model]
-        for g in [gp, *models]:  # before any draw: a refusal consumes no random numbers
+        box = np.asarray(space.bounds, dtype=np.float64)
+        P = np.empty((0, box.shape[0])) if pending is None else np.asarray(pending, dtype=np.float64)
+        P = P.reshape(-1, box.shape[0])
+        rows = P.shape[0] + int(extra_rows)
+        # before any draw: a refusal consumes no random numbers
+        if len(models) + 1 > B.MAX_GPS:
+            raise NotImplementedError(f"at most {B.MAX_GPS - 1} constraint GPs are supported")
+        for g in [gp, *models]:
             if len(g.device_list()) > 1:
                 raise NotImplementedError("constrained noisy expected improvement runs on one device: a GP is "
                                           "multi-device")
             if g.__dict__.get("_b200_conditioned") is not None:
                 raise NotImplementedError("constrained noisy expected improvement on a GP conditioned on pending "
                                           "points")
-        if (pending is not None and len(pending)) or extra_rows:
-            raise _ConstraintNotSupportedError("pending points with constraints are not supported")
+        for g in [gp, *models] if rows else []:
+            g._ensure_device_fit()
+            if g.__dict__.get("_b200_xform", ("device", None))[0] == "host":
+                raise NotImplementedError("pending points for constrained noisy expected improvement with a host-side "
+                                          "(categorical) kernel transform")
         self.fantasies = self.constraint_fantasies = None
         rs = self._suggest_rng()
-        fant = gp.noiseless_fantasies(self.n_samples, self.jitter, random_state=rs)
-        cfant = [m.noiseless_fantasies(self.n_samples, self.jitter, random_state=rs) for m in models]
-        ok = cnei_eligible(_in_bounds(space), [f.F for f in cfant], np.atleast_1d(constraint.lb),
-                           np.atleast_1d(constraint.ub))
-        eligible = np.ascontiguousarray(ok, dtype=np.uint8)
+        kw = {"pending": P, "extra_rows": extra_rows} if rows else {}
+        fants = []
+        for j, g in enumerate([gp, *models]):  # the target's draws, then each constraint's, in order
+            try:
+                fants.append(g.noiseless_fantasies(self.n_samples, self.jitter, random_state=rs, **kw))
+            except np.linalg.LinAlgError as e:
+                raise np.linalg.LinAlgError(f"{e} [{_which_gp(j)}]") from None
+        self.fantasies, self.constraint_fantasies = fants[0], fants[1:]
+        self._bounds_box = box
+        self._in_bounds_mask = np.concatenate([_in_bounds(space), _rows_in_bounds(P, box)])
+        self._lb = B.c_f64(np.atleast_1d(constraint.lb))
+        self._ub = B.c_f64(np.atleast_1d(constraint.ub))
+        self._set_incumbent()
+        return FusedAcquisition(self._cnei_kind, gp, constraint, owner=self, fantasies=self.fantasies,
+                                constraint_fantasies=self.constraint_fantasies)
+
+    def _set_incumbent(self):
+        """best_s over the rows the fantasies hold, on the device (``b200bo_gp_set_constrained_incumbent``)."""
+        fant, cfant = self.fantasies, self.constraint_fantasies
+        handles = (C.c_void_p * len(cfant))(*[f.handle.ptr.value for f in cfant])
+        inb = np.ascontiguousarray(self._in_bounds_mask, dtype=np.uint8)
         best = np.empty(self.n_samples)
-        B.check(B.lib().b200bo_gp_set_fantasy_incumbent(fant.handle.ptr, eligible.ctypes.data_as(C.POINTER(C.c_uint8)),
-                                                        B.as_dp(best)))
+        B.check(B.lib().b200bo_gp_set_constrained_incumbent(
+            fant.handle.ptr, handles, len(cfant), B.as_dp(self._lb), B.as_dp(self._ub),
+            inb.ctypes.data_as(C.POINTER(C.c_uint8)), B.as_dp(best)))
         fant.best = best
-        self.fantasies, self.constraint_fantasies = fant, cfant
-        return FusedAcquisition(self._cnei_kind, gp, constraint, owner=self, fantasies=fant,
-                                constraint_fantasies=cfant)
+
+    def condition_on_pending(self, X):
+        """Extends the latest closure in place to the pending points ``X`` ((p, d) or (d,)): the target's fantasies,
+        then each constraint's in ``constraint.model`` order (``NoiselessFantasies.condition_on_pending``, each from
+        its own pre-drawn z rows), then the incumbents over the grown rows.  A non-positive pivot raises
+        np.linalg.LinAlgError naming jitter and the GP."""
+        X = np.asarray(X, dtype=np.float64).reshape(-1, self._bounds_box.shape[0])
+        for j, f in enumerate([self.fantasies, *self.constraint_fantasies]):
+            try:
+                f.condition_on_pending(X)
+            except np.linalg.LinAlgError as e:
+                raise np.linalg.LinAlgError(f"{e} [{_which_gp(j)}]") from None
+        self._in_bounds_mask = np.concatenate([self._in_bounds_mask, _rows_in_bounds(X, self._bounds_box)])
+        self._set_incumbent()
+
+    def _extender(self, constraint):
+        return super()._extender(constraint) if constraint is None else self.condition_on_pending
 
 
 class ConstrainedNoisyExpectedImprovement(_ConstrainedNoisyEI):
@@ -849,11 +910,14 @@ class _PendingBatch(_ref.ConstantLiar):
         """(closure of round 0 over the dummies ``pending``, callable that extends it in place by one pick (d,))."""
         raise NotImplementedError
 
+    def _serves_constraints(self):
+        return False
+
     def _believe(self, gp, target_space, q, n_random, n_smart, fit_gp, random_state):
         if len(target_space) == 0:
             raise _TargetSpaceEmptyError("Cannot suggest a point without previous samples: register a point first "
                                          "(target_space.random_sample() / target_space.probe()).")
-        if target_space.constraint is not None:
+        if target_space.constraint is not None and not self._serves_constraints():
             raise _ConstraintNotSupportedError(f"{type(self).__name__} does not support constrained optimization: "
                                                "the target space has a constraint")
         self._remove_expired_dummies(target_space)
@@ -982,9 +1046,12 @@ class PendingNEI(_PendingBatch):
     picks; ``noiseless_fantasies(pending=..., extra_rows=...)``) on a fork of the noiseless GP, and each round extends
     those fantasies to the previous pick (``NoiselessFantasies.condition_on_pending``); the fitted GP is never
     conditioned or modified.  q = 1 without dummies returns the base's ``suggest`` point and leaves the RandomState as
-    it does.  Constraints raise ConstraintNotSupportedError; multi-device GPs and host-side (categorical) transforms
-    raise NotImplementedError; a non-positive pivot raises np.linalg.LinAlgError naming jitter.  ``strategy`` is
-    accepted for ConstantLiar's parameter layout and not used."""
+    it does.  With a ``ConstrainedNoisyExpectedImprovement`` / ``LogConstrainedNoisyExpectedImprovement`` base it
+    serves constrained target spaces (DESIGN.md 4.16): every constraint GP gets fantasies at the pending points too,
+    after the target's, and a pending row counts toward a sample's incumbent only where that sample calls it feasible;
+    with an NEI / LogNEI base a constraint raises ConstraintNotSupportedError.  Multi-device GPs and host-side
+    (categorical) transforms raise NotImplementedError; a non-positive pivot raises np.linalg.LinAlgError naming jitter
+    (and, with constraints, the GP).  ``strategy`` is accepted for ConstantLiar's parameter layout and not used."""
 
     def __init__(self, base_acquisition, strategy="max", random_state=None, atol=1e-5, rtol=1e-8):
         if not isinstance(base_acquisition, _NoisyEI):
@@ -999,10 +1066,13 @@ class PendingNEI(_PendingBatch):
         q = _check_int("q", q, 1)
         return self._believe(gp, target_space, q, n_random, n_smart, fit_gp, random_state)
 
+    def _serves_constraints(self):
+        return isinstance(self.base_acquisition, _ConstrainedNoisyEI)
+
     def _round_closure(self, gp, constraint, pending, q):
         base = self.base_acquisition
         acq = base._closure(gp, constraint, base._suggest_space, pending=pending, extra_rows=(q or 1) - 1)
-        return acq, base.fantasies.condition_on_pending
+        return acq, base._extender(constraint)
 
 
 # isinstance(x, b200.AcquisitionFunction) holds for every acquisition of this module, as

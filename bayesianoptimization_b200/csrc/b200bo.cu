@@ -143,6 +143,7 @@ struct b200bo_gp {
     // Z of the rows; W = K^-1 R over the first fant_nreg (registered) rows, [S][fant_nreg]
     DevBuf fant_f, fant_z, fant_w;
     DevBuf fant_tmp;  // b200bo_gp_condition_fantasies: the S solves ([S][np]), then the z row (S)
+    DevBuf fant_mask;  // b200bo_gp_set_constrained_incumbent: the in-bounds mask of the rows (n bytes)
     int fant_nreg = 0;
     DevBuf X, Xs, y, K, L, W, WT, T, alphav, v1, v2, ls, xf, info, part;
     DevBuf tscratch;  // b200bo_gp_condition: t = W^T l of the row update (np), so that alpha_ survives it
@@ -958,6 +959,54 @@ extern "C" int b200bo_gp_set_fantasy_incumbent(b200bo_gp* nl, const uint8_t* eli
     nl->fant_best = best;
     if (best_out)
         for (int s = 0; s < S; ++s) best_out[s] = best[s];
+    return B200BO_OK;
+}
+
+// CNEI's incumbents on the device (include/b200bo.h, DESIGN.md 4.16): eligibility and best_s from the F of the target and
+// constraint handles, over registered and pending rows alike; only the S incumbents come back to the host.
+extern "C" int b200bo_gp_set_constrained_incumbent(b200bo_gp* target, b200bo_gp* const* constraints, int n_constraints,
+                                                   const double* lb, const double* ub, const uint8_t* in_bounds,
+                                                   double* best_out) {
+    if (!target || !in_bounds || (n_constraints > 0 && (!constraints || !lb || !ub)))
+        return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (n_constraints < 0 || n_constraints > B200BO_MAX_GPS - 1)
+        return set_err(B200BO_ERR_ARG, "n_constraints=%d out of range [0,%d]", n_constraints, B200BO_MAX_GPS - 1);
+    IncumbentGPs G{};
+    G.n_gps = n_constraints + 1;
+    for (int g = 0; g < G.n_gps; ++g) {
+        const b200bo_gp* h = g == 0 ? target : constraints[g - 1];
+        if (!h) return set_err(B200BO_ERR_ARG, "NULL argument");
+        if (!h->fitted) return set_err(B200BO_ERR_STATE, "GP handle %d is not fitted", g);
+        if (h->replica) return set_err(B200BO_ERR_STATE, "handle %d is a predict-only replica", g);
+        if (h->fant_best.empty())
+            return set_err(B200BO_ERR_STATE, "handle %d holds no fantasies (b200bo_gp_set_fantasies)", g);
+        if (h->device != target->device || h->n != target->n || h->np != target->np ||
+            h->fant_best.size() != target->fant_best.size())
+            return set_err(B200BO_ERR_ARG, "handle %d differs from the target in device, n, np or S", g);
+        if (g > 0 && !(lb[g - 1] < ub[g - 1]))
+            return set_err(B200BO_ERR_ARG, "constraint %d: lb=%.17g is not below ub=%.17g", g - 1, lb[g - 1], ub[g - 1]);
+        G.f[g] = h->fant_f.as<double>();
+        G.y_std[g] = h->y_std;
+        G.y_mean[g] = h->y_mean;
+        G.lb[g] = g > 0 ? lb[g - 1] : 0.0;
+        G.ub[g] = g > 0 ? ub[g - 1] : 0.0;
+    }
+    const int n = (int)target->n, np = target->np, S = (int)target->fant_best.size();
+    CU(cudaSetDevice(target->device));
+    StreamScope scope(target);
+    NvtxRange nvtx_range("b200bo:set_constrained_incumbent");
+    int rc;
+    if ((rc = target->fant_mask.reserve(n))) return rc;
+    if ((rc = h2d(target->fant_mask.p, in_bounds, n))) return rc;
+    double* best = target->fant_a.as<double>() + (size_t)np * S;  // the kernels read best_s behind A
+    fantasy_incumbent_kernel<<<1, 32 * S, 0, g_st>>>(G, target->fant_mask.as<uint8_t>(), n, np, best);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    std::vector<double> bst(S);
+    if ((rc = d2h(bst.data(), best, sizeof(double) * S))) return rc;
+    target->fant_best = bst;
+    if (best_out)
+        for (int s = 0; s < S; ++s) best_out[s] = bst[s];
     return B200BO_OK;
 }
 

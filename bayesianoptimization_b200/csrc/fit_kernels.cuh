@@ -810,6 +810,45 @@ __global__ void fantasy_row_kernel(const double* __restrict__ K, const double* _
         best[s] = fmax(best[s], y_std * f + y_mean);
     }
 }
+// The GPs of a constrained incumbent (b200bo_gp_set_constrained_incumbent): F ([S][np], normalised) and the y statistics
+// of the target (index 0) and of each constraint, with the constraint's bounds (data units; index 0 unused).
+struct IncumbentGPs {
+    const double* f[B200BO_MAX_GPS];
+    double y_std[B200BO_MAX_GPS], y_mean[B200BO_MAX_GPS];
+    double lb[B200BO_MAX_GPS], ub[B200BO_MAX_GPS];
+    int n_gps;
+};
+// CNEI's incumbents over the n rows of the handles (DESIGN.md 4.16): one warp per sample s.  Each value is taken to data
+// units as v = y_std F + y_mean with separate roundings (the host's arithmetic, no FMA contraction); row i is eligible
+// when in_bounds[i] != 0 and every constraint's v lies in [lb, ub].  best[s] = max of the target's v over the eligible
+// rows, or min over all rows when none is.  max / min are exact, so the lane order does not change the result.
+__global__ void fantasy_incumbent_kernel(const IncumbentGPs G, const uint8_t* __restrict__ in_bounds, int n, int np,
+                                         double* __restrict__ best) {
+    const int s = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double hi = -CUDART_INF, lo = CUDART_INF;
+    bool any = false;
+    for (int i = lane; i < n; i += 32) {
+        const size_t k = (size_t)s * np + i;
+        const double v = __dadd_rn(__dmul_rn(G.y_std[0], G.f[0][k]), G.y_mean[0]);
+        lo = fmin(lo, v);
+        bool ok = in_bounds[i] != 0;
+        for (int g = 1; g < G.n_gps && ok; ++g) {
+            const double c = __dadd_rn(__dmul_rn(G.y_std[g], G.f[g][k]), G.y_mean[g]);
+            ok = G.lb[g] <= c && c <= G.ub[g];
+        }
+        if (ok) {
+            hi = fmax(hi, v);
+            any = true;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    }
+    any = __any_sync(0xffffffffu, any);
+    if (lane == 0) best[s] = any ? hi : lo;
+}
 // A[i][s] = Acol[s][i] for i < n, zero for n <= i < np: the [np][S] layout the NEI kernels read
 __global__ void fantasy_pack_kernel(const double* __restrict__ Acol, int np, int n, int S, double* __restrict__ A) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;

@@ -226,6 +226,22 @@ int b200bo_gp_set_fantasies(b200bo_gp* noiseless, const b200bo_gp* noisy, const 
  * conditioned on pending rows -> B200BO_ERR_STATE.  A later fit, append or condition drops them with the fantasies. */
 int b200bo_gp_set_fantasy_incumbent(b200bo_gp* noiseless, const uint8_t* eligible, double* best_out);
 
+/* Per-sample incumbents of CNEI / LogCNEI formed on the device (DESIGN.md 4.16), on unconditioned handles and on
+ * handles conditioned on pending rows (b200bo_gp_condition_fantasies) alike.  target: the target's noiseless handle;
+ * constraints[j], j < n_constraints (0..7): constraint j's noiseless handle, all with the target's S, n (registered plus
+ * pending rows), np and device.  in_bounds: (n,) host mask, nonzero when row i lies within the parameter bounds.  From
+ * the F every handle keeps, in data units v = y_std F + y_mean formed without FMA contraction (so v equals the host
+ * copies b200bo_gp_set_fantasies and b200bo_gp_condition_fantasies return, bit for bit), row i is eligible in sample s
+ * when in_bounds[i] != 0 and lb[j] <= v_j[i, s] <= ub[j] for every j, and
+ *   best_s = max over eligible rows of v_target[i, s],  or, with no eligible row, min over all n rows of v_target[i, s]
+ * - b200bo_gp_set_fantasy_incumbent's rule with that mask, bit for bit.  Writes best_s behind the target's A and into
+ * its host copy; best_out (nullable, (S,) host) receives it.  No fantasy matrix is copied to the host.  NULL handles,
+ * in_bounds, or lb / ub with n_constraints > 0, n_constraints outside [0, 7], a different S, n, np or device, or
+ * !(lb[j] < ub[j]) -> B200BO_ERR_ARG; a handle not fitted, a replica, or without fantasies -> B200BO_ERR_STATE. */
+int b200bo_gp_set_constrained_incumbent(b200bo_gp* target, b200bo_gp* const* constraints, int n_constraints,
+                                        const double* lb, const double* ub, const uint8_t* in_bounds,
+                                        double* best_out);
+
 /* Replaces the tail of GaussianProcessRegressor.fit (SK/gaussian_process/_gpr.py:275-285,
  * :349-367): y normalisation, K = k(X,X), K_ii += alpha, L = chol(K), alpha_ = K^-1 y, plus
  * the triangular inverse L^-1 the predict kernel streams.  X: (n,d) host, y: (n,) host.
