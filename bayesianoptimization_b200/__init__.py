@@ -12,14 +12,16 @@ Two layers:
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, LogExpectedImprovement,
     LogProbabilityOfImprovement, NoisyExpectedImprovement, LogNoisyExpectedImprovement,
     ConstrainedNoisyExpectedImprovement, LogConstrainedNoisyExpectedImprovement, ThompsonSampling,
-    ConstrainedThompsonSampling, MaxValueEntropySearch, ConstantLiar, KrigingBeliever, PendingNEI, GPHedge,
+    ConstrainedThompsonSampling, MaxValueEntropySearch, PosteriorMean, ConstantLiar, KrigingBeliever, PendingNEI, GPHedge,
     AcquisitionFunction, ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
+  * recommend(optimizer): the point a run should report, by the posterior mean (bayes_opt is imported when called).
 """
 from . import _lib
 from ._build import build_library
 from .dropin import accelerate_acquisition, enable
 from .fused import FusedAcquisition
 from .gpr import B200GaussianProcessRegressor, to_b200_gp
+from .recommend import recommend
 
 __version__ = "0.2.0"
 
@@ -33,7 +35,7 @@ _PLUGIN = {
     "NoisyExpectedImprovement": "acquisition", "LogNoisyExpectedImprovement": "acquisition",
     "PendingNEI": "acquisition", "ConstrainedNoisyExpectedImprovement": "acquisition",
     "LogConstrainedNoisyExpectedImprovement": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths",
-    "ConstrainedPaths": "paths",
+    "ConstrainedPaths": "paths", "PosteriorMean": "acquisition",
 }
 
 
@@ -48,5 +50,5 @@ def __getattr__(name):
 
 __all__ = [
     "B200GaussianProcessRegressor", "FusedAcquisition", "enable", "accelerate_acquisition", "to_b200_gp",
-    "build_library", "__version__", *_PLUGIN,
+    "build_library", "recommend", "__version__", *_PLUGIN,
 ]

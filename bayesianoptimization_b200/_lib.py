@@ -14,7 +14,7 @@ OK, ERR_CUDA, ERR_ARG, ERR_NOT_PD, ERR_UNSUPPORTED, ERR_STATE = 0, -1, -2, -3, -
 KERNEL_MATERN, KERNEL_RBF = 0, 1
 NU_05, NU_15, NU_25, NU_INF = 0, 1, 2, 3
 ACQ_UCB, ACQ_EI, ACQ_POI, ACQ_NONE, ACQ_MES, ACQ_LOGEI, ACQ_LOGPOI, ACQ_NEI, ACQ_LOGNEI = 0, 1, 2, 3, 4, 6, 7, 8, 9
-ACQ_CNEI, ACQ_LOGCNEI = 10, 11
+ACQ_CNEI, ACQ_LOGCNEI, ACQ_MEAN = 10, 11, 12
 MAX_GPS, MAX_DIM, MAX_TOPK, MAX_PATHS = 8, 64, 64, 16
 XFORM_IDENTITY, XFORM_ROUND = 0, 1
 GET_L, GET_ALPHA, GET_YSTATS, GET_K, GET_LINV = 0, 1, 2, 3, 4

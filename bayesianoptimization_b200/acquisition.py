@@ -175,6 +175,39 @@ class ExpectedImprovement(DeviceHooks, _ref.ExpectedImprovement):
     """bayes_opt.acquisition.ExpectedImprovement with the device hooks."""
 
 
+class PosteriorMean(DeviceHooks, _ref.AcquisitionFunction):
+    """Maximise the posterior mean: the point a noisy run should recommend (Letham et al., Bayesian Analysis 2019),
+    not a rule for what to evaluate next.  ``recommend(optimizer)`` uses it; it also works as an acquisition function.
+
+    The closure is ``FusedAcquisition(ACQ_MEAN, gp, constraint)`` (include/b200bo.h, DESIGN.md 4.17): -mu of the target
+    GP, and with constraints the merit "mu where every constraint's mean lies within its bounds, else -T (1 + the
+    summed violation of the means)", so every mean-feasible point ranks above every infeasible one.  It is not a product
+    of probabilities and needs no sigma: one mean-only kernel, without the L^-1 product the other kinds run.
+
+    ``suggest`` is the reference's base ``suggest`` (random stage plus L-BFGS-B, the RandomState used as UCB uses it);
+    it suggests before any feasible point is registered and never raises NoValidPointRegisteredError.  The acquisition
+    params are empty, so ``save_state`` carries nothing extra.  A subclass that overrides ``base_acq(mean, std)`` gets
+    the reference's closure on the device predict, as for the other classes.  ConstantLiar, GPHedge, KrigingBeliever and
+    PendingNEI refuse it (TypeError)."""
+
+    def base_acq(self, mean, std):
+        return mean
+
+    def _get_acq(self, gp, constraint=None):
+        _as_b200_gp(gp)
+        if type(self).base_acq is not PosteriorMean.base_acq:  # a host formula: the reference's closure
+            acq = _ref.AcquisitionFunction._get_acq(self, gp=gp, constraint=constraint)
+            acq.b200_vectorized = True
+            return acq
+        return FusedAcquisition(B.ACQ_MEAN, gp, constraint)
+
+    def get_acquisition_params(self):
+        return {}
+
+    def set_acquisition_params(self, params):
+        pass
+
+
 # ---- log-space acquisitions (DESIGN.md 4.12) ------------------------------------------------------------------
 # numpy forms of the device epilogue (csrc/common.cuh log_h, csrc/predict_kernels.cuh log_acq_term / log_cfactor),
 # for user subclasses that override base_acq and for calls outside the fused kernel.
@@ -839,6 +872,9 @@ def _refuse_nei(acq, where):
     if isinstance(acq, _NoisyEI):
         raise TypeError(f"{where} does not support {type(acq).__name__}: its fantasies are drawn per suggest() against "
                         "the registered data")
+    if isinstance(acq, PosteriorMean):
+        raise TypeError(f"{where} does not support {type(acq).__name__}: it recommends the best posterior mean and "
+                        "does not choose points to evaluate")
 
 
 _HOOKED = {
@@ -1081,6 +1117,6 @@ class PendingNEI(_PendingBatch):
 for _cls in (UpperConfidenceBound, ProbabilityOfImprovement, ExpectedImprovement, LogExpectedImprovement,
              LogProbabilityOfImprovement, ConstantLiar, GPHedge, ThompsonSampling, ConstrainedThompsonSampling,
              MaxValueEntropySearch, KrigingBeliever, NoisyExpectedImprovement, LogNoisyExpectedImprovement,
-             ConstrainedNoisyExpectedImprovement, LogConstrainedNoisyExpectedImprovement, PendingNEI):
+             ConstrainedNoisyExpectedImprovement, LogConstrainedNoisyExpectedImprovement, PendingNEI, PosteriorMean):
     AcquisitionFunction.register(_cls)
 del _cls

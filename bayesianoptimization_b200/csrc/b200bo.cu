@@ -293,6 +293,8 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_acq16_kernel<false, 1684, PIPE_BULK_MC, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
+    CU(cudaFuncSetAttribute(predict_mean_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
+    CU(cudaFuncSetAttribute(predict_mean_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDfma));
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
@@ -1917,6 +1919,18 @@ static int ensure_tc(b200bo_gp* gp, cudaStream_t stream) {
     return B200BO_OK;
 }
 
+// B200BO_ACQ_MEAN: T = 2 B + 1 with B = |y_mean| + y_std const_value A1 of gps[0] (include/b200bo.h).  A1 = sum |alpha_|
+// comes with the Gram operand of pruning (once per fit; the first call after a fit synchronises `stream`).
+static int mean_merit_T(b200bo_gp* g0, cudaStream_t stream, double& T) {
+    const int rc = ensure_gram(g0, stream);
+    if (rc) return rc;
+    T = 2.0 * (fabs(g0->y_mean) + g0->y_std * g0->constv * g0->gram_a1) + 1.0;
+    return B200BO_OK;
+}
+
+// dynamic shared memory of predict_mean_kernel: phase A's staged candidates, training rows and alpha_
+static size_t mean_smem_bytes(int d) { return sizeof(double) * ((size_t)(PBN + 2 * PA_CHUNK) * d + 2 * PA_CHUNK); }
+
 static int check_spec(const b200bo_acq* spec) {
     if (!spec) return set_err(B200BO_ERR_ARG, "spec is NULL");
     if (spec->n_gps < 1 || spec->n_gps > B200BO_MAX_GPS)
@@ -2046,7 +2060,7 @@ static int fill_params(const b200bo_acq* spec, const CandSrc& src, int64_t m, in
 // finish for every GP.
 static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool grad, cudaStream_t stream) {
     b200bo_gp* g0 = spec->gps[0];
-    const bool nei = acq_is_nei(spec->kind), cnei = acq_is_cnei(spec->kind);
+    const bool nei = acq_is_nei(spec->kind), cnei = acq_is_cnei(spec->kind), mean = spec->kind == B200BO_ACQ_MEAN;
     int rc;
     for (int g = 0; g < spec->n_gps; ++g) {
         b200bo_gp* gp = spec->gps[g];
@@ -2086,6 +2100,14 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
         for (int g = 0; g < spec->n_gps; ++g) {
             const b200bo_gp* gp = spec->gps[g];
             small_kstar_kernel<<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+            LAUNCHED();
+            if (mean) {  // K* alpha_ only: no triangular product, no sums of squares
+                if (grad) {
+                    small_grad_kernel<false, false, true><<<dim3(gp->np / 128, npass), 256, 0, stream>>>(S, g);
+                    LAUNCHED();
+                }
+                continue;
+            }
             small_trsv_kernel<false><<<dim3(gp->s_nunits, ngrp), 256, kSmallTrsvSmemBytes, stream>>>(S, g, npass);
             if (grad) {
                 small_reduce_kernel<1><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
@@ -2102,9 +2124,11 @@ static int small_launch(const b200bo_acq* spec, SmallParams& S, int64_t m, bool 
             } else {
                 small_reduce_kernel<0><<<dim3(gp->np / SROWS, npass), 256, 0, stream>>>(S, g);
             }
-            for (int i = 0; i < (grad ? 6 : 3); ++i) LAUNCHED();
+            for (int i = 0; i < (grad ? 5 : 2); ++i) LAUNCHED();
         }
-        if (grad && cnei)
+        if (mean)
+            (grad ? small_finish_mean_kernel<true> : small_finish_mean_kernel<false>)<<<npass, 256, 0, stream>>>(S);
+        else if (grad && cnei)
             small_finish_grad_cnei_kernel<<<npass, 256, 0, stream>>>(S);
         else if (grad)
             (nei ? small_finish_grad_kernel<true> : small_finish_grad_kernel<false>)<<<npass, 256, 0, stream>>>(S);
@@ -2133,7 +2157,7 @@ static int eval_core(const b200bo_acq* spec, const CandSrc& src, int64_t m, doub
                      double* d_sd, int k, void* d_sel, int64_t index_base, cudaStream_t stream,
                      SelMode sm = SelMode()) {
     const bool split = k > 0 && !d_acq_neg && !d_mu && !d_sd && m > kPruneMaxBatch && prune_enabled() && spec &&
-                       spec->gps[0];
+                       spec->gps[0] && spec->kind != B200BO_ACQ_MEAN;
     if (!split) return eval_launch(spec, src, m, d_acq_neg, d_mu, d_sd, k, d_sel, index_base, stream, sm);
     // consecutive launches continue the per-CTA selection lists (and the pruning's k-th key), one merge at the end
     for (long long c0 = 0; c0 < m; c0 += kPruneMaxBatch) {
@@ -2164,12 +2188,17 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
     if (nei && (d_mu || d_sd))
         return set_err(B200BO_ERR_ARG, "NEI averages over fantasies and has no single posterior mean: mu / sd outputs "
                                        "are not available");
+    const bool mean = spec->kind == B200BO_ACQ_MEAN;
+    if (mean && d_sd)
+        return set_err(B200BO_ERR_ARG, "the posterior-mean merit needs no sigma and does not form it: the sd output is "
+                                       "not available");
     const int precision = nei ? B200BO_PRECISION_FP64 : g0->precision;
     CU(cudaSetDevice(g0->device));
     NvtxRange nvtx_range("b200bo:predict_acq");
     PredictParams P;
     int np_max = 0;
     if ((rc = fill_params(spec, src, m, index_base, stream, P, np_max))) return rc;
+    if (mean && spec->n_gps > 1 && (rc = mean_merit_T(g0, stream, P.mean_T))) return rc;
     P.acq_out = d_acq_neg;
     P.mu_out = d_mu;
     P.sd_out = d_sd;
@@ -2191,6 +2220,28 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
         memset(&S, 0, sizeof(S));
         S.P = P;
         if ((rc = small_launch(spec, S, m, false, stream))) return rc;
+    } else if (grid > 0 && mean) {
+        // fp64 whatever the handle's precision, never pruned; chunked batches keep one list per CTA across launches
+        const bool dreg = P.d <= kPredictMaxDimRegs;
+        const size_t smem = mean_smem_bytes(P.d);
+        int per_sm = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+            &per_sm, dreg ? predict_mean_kernel<true> : predict_mean_kernel<false>, P16_NT, smem));
+        const int full = g0->sm_count * (per_sm > 0 ? per_sm : 1);
+        grid = (sm.resume || !sm.finish || ntiles >= full) ? full : (int)ntiles;
+        if (k > 0) {
+            if ((rc = g0->sel_cta.reserve(sizeof(SelList) * (size_t)full))) return rc;
+            P.sel_cta = g0->sel_cta.as<SelList>();
+            P.sel_k = k;
+            P.sel_resume = sm.resume;
+            fused_sel = true;
+        }
+        CU(cudaEventRecord(g0->ev0, stream));
+        (dreg ? predict_mean_kernel<true> : predict_mean_kernel<false>)<<<grid, P16_NT, smem, stream>>>(P);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(g0->ev1, stream));
+        g_last_timed = g0;
     } else if (grid > 0) {
         if (k > 0) {  // selection fused into the epilogue: no acq[M] needed
             if ((rc = g0->sel_cta.reserve(sizeof(SelList) * (size_t)g0->sm_count))) return rc;
@@ -2657,6 +2708,7 @@ extern "C" int b200bo_acq_value_grad(const b200bo_acq* spec, const double* Xc, i
     int np_max = 0;
     cudaStream_t stream = nullptr;
     if ((rc = fill_params(spec, src, m, 0, stream, S.P, np_max))) return rc;
+    if (spec->kind == B200BO_ACQ_MEAN && spec->n_gps > 1 && (rc = mean_merit_T(g0, stream, S.P.mean_T))) return rc;
     S.P.acq_out = g0->out_acq.as<double>();
     if ((rc = g0->clamp.reserve(2 * sizeof(unsigned long long)))) return rc;
     S.P.clamp_count = g0->clamp.as<unsigned long long>();

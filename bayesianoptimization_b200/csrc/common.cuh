@@ -23,7 +23,7 @@ __host__ __device__ constexpr bool acq_uses_fantasies(int kind) { return acq_is_
 __host__ __device__ constexpr bool acq_kind_valid(int kind) {
     return kind == B200BO_ACQ_UCB || kind == B200BO_ACQ_EI || kind == B200BO_ACQ_POI || kind == B200BO_ACQ_NONE ||
            kind == B200BO_ACQ_MES || kind == B200BO_ACQ_LOGEI || kind == B200BO_ACQ_LOGPOI ||
-           acq_uses_fantasies(kind);
+           acq_uses_fantasies(kind) || kind == B200BO_ACQ_MEAN;
 }
 // The log-space kinds: the value is -(alpha + sum_j log p_j), the constraint factors summed as logs.  NEI = false in
 // the kernels built without NEI / LogNEI (DESIGN.md 4.13), which then test for LogEI and LogPoI only.

@@ -123,6 +123,52 @@ __global__ void __launch_bounds__(P16_NT) predict_bound_kernel(const PredictPara
     }
 }
 
+// B200BO_ACQ_MEAN (include/b200bo.h, DESIGN.md 4.17): the mean-only tile kernel.  A persistent grid of CTAs shaped as
+// the direct bound pass (P16_NT threads, the same phase A without K* stores), each folding its tiles of PBN candidates
+// into one running selection list.  Per tile, phase A of every GP in j order; mu = K* alpha_ in the tile kernel's order
+// of the four parts and de-normalised with candidate_epilogue's expression, so mu_0 is bit-equal to the mean
+// predict_acq16_kernel (b200bo_gp_predict) gives the batch; then the merit.  No K* scratch, no L^-1, no phase B.
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT) predict_mean_kernel(const PredictParams P) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    __shared__ double mu0_s[PBN], viol_s[PBN];
+    __shared__ SelShared sel_s;
+    const int tid = threadIdx.x;
+    if (P.sel_cta) {
+        if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
+        __syncthreads();
+    }
+    const long long ntiles = (P.m + PBN - 1) / PBN;
+    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        const long long c0 = tile * PBN;
+        for (int g = 0; g < P.n_gps; ++g) {
+            const GpDev& G = P.gp[g];
+            phase_a<P16_NT, DREG, KS_NONE>(P, G, c0, nullptr, smem, mu_s, 0ull, nullptr, nullptr, P.m, G.np);
+            if (tid < PBN) {
+                const int c = tid;
+                const long long gi = c0 + c;
+                const double mu_n = ((mu_s[0][c] + mu_s[1][c]) + mu_s[2][c]) + mu_s[3][c];
+                const double mean = G.y_std * mu_n + G.y_mean;
+                if (g == 0) {
+                    mu0_s[c] = mean;
+                    viol_s[c] = 0.0;
+                    if (P.mu_out && gi < P.m) P.mu_out[gi] = mean;
+                } else {
+                    viol_s[c] = __dadd_rn(viol_s[c], mean_viol(G, mean));
+                }
+                if (g == P.n_gps - 1) {
+                    const double val = mean_merit_neg(mu0_s[c], viol_s[c], P.mean_T);
+                    if (P.acq_out && gi < P.m) P.acq_out[gi] = val;
+                    if (P.sel_cta) runsel_update<1>(sel_s, P.sel_k, tid, val, gi + P.index_base, gi < P.m);
+                }
+            }
+            __syncthreads();
+        }
+    }
+    if (P.sel_cta && tid < PBN) runsel_store(sel_s, P.sel_cta + blockIdx.x, tid);
+}
+
 // failed polls before a wait gives up: seconds, against microseconds for a stage to arrive from L2 or HBM
 constexpr uint32_t kPipeWaitBudget = 1u << 28;
 // set by a ring wait (the bulk-copy phase B, the Gram bound pass) that ran out of its budget; the host reports it as an

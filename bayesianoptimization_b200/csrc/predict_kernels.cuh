@@ -76,6 +76,8 @@ struct PredictParams {
     const double* fant_a_gp[B200BO_MAX_GPS];
     // predict_acq16_kernel: offset (doubles) of each CTA's per-sample carry [n_ystar][PSTR_DMMA] in its scratch slot
     long long carry_off;
+    // B200BO_ACQ_MEAN (DESIGN.md 4.17): T = 2 B + 1 of the merit, B >= |mu_0| (0 without constraint GPs: unused)
+    double mean_T;
 };
 
 // coordinate j of candidate gi (local index) as the reference's x_tries[gi, j]
@@ -523,6 +525,21 @@ __device__ __forceinline__ void candidate_epilogue(const PredictParams& P, const
     }
 }
 
+// ---- B200BO_ACQ_MEAN: the posterior-mean merit (include/b200bo.h, DESIGN.md 4.17) -----------------------------
+// Constraint GP G's violation at its posterior mean (data units): an infinite bound contributes 0 (the short-circuits
+// of the constraint factors), max(0, .) propagates NaN as np.maximum does, and the explicit _rn intrinsics keep FMA
+// contraction out, so that the numpy restatement reproduces the value bit for bit.
+__device__ __forceinline__ double mean_pos(double x) { return (x > 0.0 || x != x) ? x : 0.0; }
+__device__ __forceinline__ double mean_viol(const GpDev& G, double mean) {
+    const double lo = G.lb == -CUDART_INF ? 0.0 : mean_pos(__dsub_rn(G.lb, mean));
+    const double hi = G.ub == CUDART_INF ? 0.0 : mean_pos(__dsub_rn(mean, G.ub));
+    return __dadd_rn(lo, hi);
+}
+// -merit: -mu_0 where viol = 0, else T (1 + viol) (= -(-T (1 + viol)) exactly)
+__device__ __forceinline__ double mean_merit_neg(double mu0, double viol, double T) {
+    return viol == 0.0 ? -mu0 : __dmul_rn(T, __dadd_rn(1.0, viol));
+}
+
 // ---- phase A: the tile's K*^T (np x PBN) + K* alpha_ -----------------------------------------------
 // Every fused predict kernel builds its tile's covariances with this one function, so the tile kernels, the bound pass
 // and the refine / units stages get the same K* entries and the same mu = K* alpha_, bit for bit (DESIGN.md 4.9).
@@ -540,11 +557,12 @@ constexpr int PA_CHUNK = 64;  // training rows per staged chunk
 //   KS_TF32    tf32 (hi, lo) pairs in the wgmma operand-image layout of tc_common.cuh ([np/32][hi|lo][16 KiB],
 //              candidate = operand row, training index = K), fenced for the bulk copies that read them (fp32 mode)
 //   KS_KMAX    nowhere: each thread keeps the largest |K*_i| of its rows in kmax_s[part][c] (the bound pass of pruning)
+//   KS_NONE    nowhere, and no kmax: mu_s only (the mean-only kernel of B200BO_ACQ_MEAN)
 // mu_s[part][c] is the part's share of K* alpha_; each caller adds the NT / PBN parts in its fixed order.
 // Column c is candidate c0 + c of the first mlim, or perm[c0 + c] when perm is set (tiles in bound order); rows: the
 // leading training rows to build (a multiple of PA_CHUNK; G.np for all of them - mu_s is K* alpha_ only then); row0
 // (a multiple of PA_CHUNK, 0 but in ks_build_kernel): the rows before it are skipped, mu_s is then meaningless.
-enum { KS_F64, KS_F64_EF, KS_TF32, KS_KMAX };
+enum { KS_F64, KS_F64_EF, KS_TF32, KS_KMAX, KS_NONE };
 
 __device__ __forceinline__ void st_global_hint(double* p, double v, unsigned long long pol) {
     asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;\n" ::"l"(p), "d"(v), "l"(pol) : "memory");
@@ -649,7 +667,7 @@ __device__ __forceinline__ void phase_a_impl(const PredictParams& P, const GpDev
                 } else if constexpr (KS == KS_TF32) {
                     hi[q] = tc::to_tf32((float)kv);
                     lo[q] = tc::to_tf32((float)(kv - (double)hi[q]));
-                } else {
+                } else if constexpr (KS == KS_KMAX) {
                     kmax = fmax(kmax, fabs(kv));
                 }
                 mu_acc = fma(al[r0 + q], kv, mu_acc);
@@ -1325,6 +1343,8 @@ small_reduce_kernel(const SmallParams S, int g) {
 
 // Per pass: the row-block and K* alpha_ partials of every GP summed in index order into colsq_s / mu_s.  256 threads
 // = 32 candidates x 8 slices of the partial lists (fixed-order two-level sum).
+// COLSQ = false (B200BO_ACQ_MEAN): the K* alpha_ sums only - no triangular product ran.
+template <bool COLSQ = true>
 __device__ __forceinline__ void small_finish_sums(const SmallParams& S, int pass, double (*red)[SMC],
                                                   double (*colsq_s)[SMC], double (*mu_s)[SMC]) {
     const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
@@ -1332,20 +1352,23 @@ __device__ __forceinline__ void small_finish_sums(const SmallParams& S, int pass
         const GpDev& G = S.P.gp[g];
         const SmallGp& Q = S.sg[g];
         const int nrb = G.np / SROWS, nb = G.np / 128;
-        const double* crb = Q.colsq_rb + (size_t)pass * nrb * SMC;
         const double* mu_part = Q.mu_part + (size_t)pass * nb * SMC;
         // slice sl sums a contiguous range of the lists; the 8 slice sums are then added in order
         double s = 0.0;
-        for (int b = sl * ((nrb + 7) / 8); b < min(nrb, (sl + 1) * ((nrb + 7) / 8)); ++b) s += crb[(size_t)b * SMC + c];
-        red[sl][c] = s;
-        __syncthreads();
-        if (sl == 0) {
-            double t = 0.0;
+        if constexpr (COLSQ) {
+            const double* crb = Q.colsq_rb + (size_t)pass * nrb * SMC;
+            for (int b = sl * ((nrb + 7) / 8); b < min(nrb, (sl + 1) * ((nrb + 7) / 8)); ++b)
+                s += crb[(size_t)b * SMC + c];
+            red[sl][c] = s;
+            __syncthreads();
+            if (sl == 0) {
+                double t = 0.0;
 #pragma unroll
-            for (int r = 0; r < 8; ++r) t += red[r][c];
-            colsq_s[g][c] = t;
+                for (int r = 0; r < 8; ++r) t += red[r][c];
+                colsq_s[g][c] = t;
+            }
+            __syncthreads();
         }
-        __syncthreads();
         s = 0.0;
         for (int b = sl * ((nb + 7) / 8); b < min(nb, (sl + 1) * ((nb + 7) / 8)); ++b) s += mu_part[(size_t)b * SMC + c];
         red[sl][c] = s;
@@ -1396,8 +1419,9 @@ small_finish_kernel(const SmallParams S) {
 // NEI (gps[0] of an NEI / LogNEI call): blockIdx.z = fantasy s, the first list takes a_s = column s of A instead of
 // alpha_, and gpart holds S + 1 lists per block: [b][s][j][c] for s < S, then the u list (written by s = 0).
 // CNEI (every GP of a CNEI / LogCNEI call, with NEI): the same lists from GP g's own A_g (PredictParams::fant_a_gp).
+// MEAN (B200BO_ACQ_MEAN, without NEI): the alpha_ list only; u = L^-T v was not formed and its slots stay unwritten.
 constexpr int SGR = 32;  // rows per sub-chunk
-template <bool NEI, bool CNEI = false>
+template <bool NEI, bool CNEI = false, bool MEAN = false>
 __global__ void __launch_bounds__(256)
 small_grad_kernel(const SmallParams S, int g) {
     const GpDev& G = S.P.gp[g];
@@ -1439,7 +1463,7 @@ small_grad_kernel(const SmallParams S, int g) {
                     ca = S.P.fant_a[(size_t)n * S.P.n_ystar + blockIdx.z] * ch;
                 else
                     ca = G.alphav[n] * ch;
-                cu = usum[(size_t)n * SMC + c] * ch;
+                if constexpr (!MEAN) cu = usum[(size_t)n * SMC + c] * ch;
             }
             coef[0][rl][c] = ca;
             coef[1][rl][c] = cu;
@@ -1478,7 +1502,7 @@ small_grad_kernel(const SmallParams S, int g) {
             const int j = rg + 8 * t;
             if (j < d) {
                 out[(size_t)j * SMC + c] = sa[t];
-                out[(size_t)(d + j) * SMC + c] = su[t];
+                if constexpr (!MEAN) out[(size_t)(d + j) * SMC + c] = su[t];
             }
         }
     }
@@ -1578,6 +1602,78 @@ small_finish_grad_kernel(const SmallParams S) {
             gr += ((wa == 0.0 ? 0.0 : wa * a) + (wu == 0.0 ? 0.0 : wu * u)) / G.ls[j];
         }
         S.grad_out[(pc0 + cc) * d + j] = isnan(val_s[cc]) ? CUDART_NAN : gr;
+    }
+}
+
+// B200BO_ACQ_MEAN on the small-batch path, per pass (blockIdx.x): the K* alpha_ sums of small_finish_sums (the order
+// b200bo_gp_predict's small path adds them in), mu_g = y_std mu_n + y_mean as candidate_epilogue forms it, then the
+// merit.  GRAD (b200bo_acq_value_grad): d acq_neg = sum_g w_g d mu_g, with d mu_g / d x_j = -y_std_g (sum_b gpart_g
+// [b][0][j]) / ls_gj (small_grad_kernel<false, false, true>) and
+//   w_0 = -1 where viol = 0 (the boundary included), else w_0 = 0 and w_g = -T below lb_g, +T above ub_g, 0 within.
+// A rounded dimension has gradient 0; a NaN value gives a NaN row.
+template <bool GRAD>
+__global__ void __launch_bounds__(256)
+small_finish_mean_kernel(const SmallParams S) {
+    __shared__ double red[8][SMC];
+    __shared__ double mu_s[B200BO_MAX_GPS][SMC];
+    __shared__ double w_s[B200BO_MAX_GPS][SMC];
+    __shared__ double val_s[SMC];
+    const int tid = threadIdx.x, c = tid & 31, sl = tid >> 5;
+    const int pass = blockIdx.x, mc = small_pass_mc(S, pass), ng = S.P.n_gps;
+    const long long pc0 = small_pass_c0(S, pass);
+    small_finish_sums<false>(S, pass, red, nullptr, mu_s);
+    if (sl == 0 && c < mc) {
+        const long long gi = pc0 + c;
+        double mu0 = 0.0, viol = 0.0;
+        for (int g = 0; g < ng; ++g) {
+            const GpDev& G = S.P.gp[g];
+            const double mean = G.y_std * mu_s[g][c] + G.y_mean;
+            mu_s[g][c] = mean;
+            if (g == 0) {
+                mu0 = mean;
+                if (S.P.mu_out) S.P.mu_out[gi] = mean;
+            } else {
+                viol = __dadd_rn(viol, mean_viol(G, mean));
+            }
+        }
+        const double val = mean_merit_neg(mu0, viol, S.P.mean_T);
+        if (S.P.acq_out) S.P.acq_out[gi] = val;
+        if constexpr (GRAD) {
+            val_s[c] = val;
+            const bool feasible = viol == 0.0;
+            for (int g = 0; g < ng; ++g) {
+                const GpDev& G = S.P.gp[g];
+                const double mean = mu_s[g][c];
+                double w = 0.0;
+                if (g == 0)
+                    w = feasible ? -1.0 : 0.0;
+                else if (!feasible && G.lb != -CUDART_INF && mean < G.lb)
+                    w = -S.P.mean_T;
+                else if (!feasible && G.ub != CUDART_INF && mean > G.ub)
+                    w = S.P.mean_T;
+                w_s[g][c] = w;
+            }
+        }
+    }
+    if constexpr (GRAD) {
+        __syncthreads();
+        const int d = S.P.d;
+        for (int idx = tid; idx < SMC * d; idx += 256) {
+            const int cc = idx & 31, j = idx >> 5;
+            if (cc >= mc) continue;
+            double gr = 0.0;
+            for (int g = 0; g < ng; ++g) {
+                const GpDev& G = S.P.gp[g];
+                const double w = w_s[g][cc];
+                if (w == 0.0 || (G.xform && xform_rounds(G.xform[j]))) continue;
+                const int nb = G.np / 128;
+                const double* gp = S.sg[g].gpart + (size_t)pass * nb * 2 * d * SMC;
+                double a = 0.0;
+                for (int b = 0; b < nb; ++b) a += gp[((size_t)b * 2 * d + j) * SMC + cc];
+                gr += w * (-G.y_std * a) / G.ls[j];
+            }
+            S.grad_out[(pc0 + cc) * d + j] = isnan(val_s[cc]) ? CUDART_NAN : gr;
+        }
     }
 }
 

@@ -111,6 +111,24 @@ extern "C" {
  * without fantasies: B200BO_ERR_STATE; handles with different S or n: B200BO_ERR_ARG. */
 #define B200BO_ACQ_CNEI 10
 #define B200BO_ACQ_LOGCNEI 11
+/* Posterior-mean merit, for recommending a point at the end of a noisy run (Letham et al. 2019 recommend the best
+ * posterior mean; DESIGN.md 4.17).  No counterpart in the reference, whose TargetSpace.max() is the largest noisy
+ * observation.  With mu_j the posterior mean of gps[j] (data units) and A1 = sum_i |alpha_i| of gps[0] (normalised
+ * units):
+ *   viol(x)  = sum_{j=1..J}, in j order, (max(0, lb_j - mu_j) + max(0, mu_j - ub_j))
+ *   merit(x) = mu_0                     if viol(x) = 0
+ *            = -T (1 + viol(x))         otherwise,   T = 2 B + 1,  B = |y_mean| + y_std const_value A1 >= |mu_0|
+ *   acq_neg  = -merit(x)                (-mu_0 without constraint GPs)
+ * so every mean-feasible candidate ranks above every infeasible one.  This is the rule: it is not a product of
+ * probabilities, and it needs no sigma.  For a one-sided bound, viol_j = 0 is a marginal probability of feasibility of
+ * at least 1/2.  An infinite bound contributes 0 (the short-circuits of the constraint factors); the sums, max (NaN-
+ * propagating), add and multiply are evaluated without FMA contraction, as for b200bo_cpaths_eval.  Served by the
+ * host, device and Philox entry points, the multi-GPU entry points and b200bo_acq_value_grad, always in fp64 and
+ * never pruned: one mean-only tile kernel (no L^-1 product) or the small-batch kernels.  mu_0 of a batch served by
+ * the tile kernel is bit-equal to the mean b200bo_gp_predict returns for it on an fp64 handle.  d_mu is allowed;
+ * d_sd -> B200BO_ERR_ARG.  The A/B switches B200BO_PREDICT_* and B200BO_PRUNE* do not apply.  Gradient: -d mu_0 on a
+ * feasible row (viol = 0), T sum_j d viol_j on an infeasible one (d viol_j = -d mu_j below lb_j, +d mu_j above ub_j). */
+#define B200BO_ACQ_MEAN 12
 
 #define B200BO_MAX_GPS 8   /* 1 target GP + up to 7 constraint GPs per call */
 #define B200BO_MAX_DIM 64  /* max input dimension d */
