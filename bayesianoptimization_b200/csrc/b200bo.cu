@@ -249,6 +249,19 @@ extern "C" int b200bo_device_count(void) {
     return n;
 }
 
+// dynamic shared memory of the register-fragment fp32 Gram pass, every k-step count of d <= kGramRegMaxDim
+template <int COV>
+static cudaError_t gram_reg_attrs() {
+    constexpr int attr = cudaFuncAttributeMaxDynamicSharedMemorySize;
+    const int smem = (int)gram_reg_bound_smem(kGramRegMaxDim);
+    cudaError_t e;
+    if ((e = cudaFuncSetAttribute(predict_bound_gram_reg_kernel<COV, 1>, (cudaFuncAttribute)attr, smem))) return e;
+    if ((e = cudaFuncSetAttribute(predict_bound_gram_reg_kernel<COV, 2>, (cudaFuncAttribute)attr, smem))) return e;
+    if ((e = cudaFuncSetAttribute(predict_bound_gram_reg_kernel<COV, 3>, (cudaFuncAttribute)attr, smem))) return e;
+    if ((e = cudaFuncSetAttribute(predict_bound_gram_reg_kernel<COV, 4>, (cudaFuncAttribute)attr, smem))) return e;
+    return cudaFuncSetAttribute(predict_bound_gram_reg_kernel<COV, 5>, (cudaFuncAttribute)attr, smem);
+}
+
 // device properties, timing events and the opt-in shared-memory sizes of the big kernels
 static int init_handle(b200bo_gp* gp) {
     CU(cudaDeviceGetAttribute(&gp->sm_count, cudaDevAttrMultiProcessorCount, gp->device));
@@ -301,6 +314,9 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
     CU(cudaFuncSetAttribute(predict_bound_gram_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gram_bound_smem(B200BO_MAX_DIM)));
+    CU(gram_reg_attrs<1>());
+    CU(gram_reg_attrs<2>());
+    CU(gram_reg_attrs<3>());
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_units_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
@@ -1768,16 +1784,18 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     return B200BO_OK;
 }
 
-// Gram bound pass operand of pruning (once per fit): [np][stride] doubles, A1, Ymax, then np floats (alpha_).  A1 is
-// read back (one synchronisation per fit) for the choice of pass.
+// Gram bound pass operand of pruning (once per fit): [np][stride] doubles, A1, Ymax, then np floats (alpha_) and np
+// float pairs (the margin weights of predict_bound_gram_reg_kernel).  A1 is read back (one synchronisation per fit) for
+// the choice of pass.
 static int ensure_gram(b200bo_gp* gp, cudaStream_t stream) {
     if (gp->gram_valid) return B200BO_OK;
     const int np = gp->np, d = gp->d;
     int rc;
-    if ((rc = gp->gram.reserve(sizeof(double) * ((size_t)np * gram_stride(d) + 2) + sizeof(float) * np))) return rc;
+    if ((rc = gp->gram.reserve(sizeof(double) * ((size_t)np * gram_stride(d) + 2) + 3 * sizeof(float) * np)))
+        return rc;
     double* img = gp->gram.as<double>();
     gram_operand_kernel<<<(np + 255) / 256, 256, 0, stream>>>(gp->Xs.as<double>(), gp->alphav.as<double>(),
-                                                              (int)gp->n, np, d, img);
+                                                              (int)gp->n, np, d, cov_code(gp->family, gp->nu), img);
     LAUNCHED();
     gram_stats_kernel<<<1, 1024, 0, stream>>>(gp->alphav.as<double>(), (int)gp->n, d, img,
                                               img + (size_t)np * gram_stride(d));
@@ -1807,10 +1825,40 @@ static int bound_pass_choice(const b200bo_gp* g0, const GpDev& G) {
     return g0->gram_a1 * G.constv * 0x1p-24 <= kPruneF32MaxMargin ? kBoundGram32 : kBoundGram64;
 }
 
+// The fp32 Gram pass at d <= kGramRegMaxDim runs predict_bound_gram_reg_kernel (candidate fragments in registers, the
+// default) unless B200BO_PRUNE_GRAM_KERNEL=ring (read per call, for A/B measurements) picks predict_bound_gram_kernel,
+// which every other d, and the fp64 Gram pass, runs.
+static bool gram_reg_kernel(int d) {
+    if (d > kGramRegMaxDim) return false;
+    const char* e = getenv("B200BO_PRUNE_GRAM_KERNEL");
+    return !(e && !strcmp(e, "ring"));
+}
+
+template <int COV>
+static void launch_bound_gram_reg(const PredictParams& P, unsigned ntiles, unsigned long long* keys, int* idx,
+                                  double* kmax, double2* mu, cudaStream_t stream) {
+    const size_t smem = gram_reg_bound_smem(P.d);
+    switch ((P.d + 2 + 3) / 4) {
+        case 1: predict_bound_gram_reg_kernel<COV, 1><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        case 2: predict_bound_gram_reg_kernel<COV, 2><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        case 3: predict_bound_gram_reg_kernel<COV, 3><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        case 4: predict_bound_gram_reg_kernel<COV, 4><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+        default: predict_bound_gram_reg_kernel<COV, 5><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;
+    }
+}
+
 template <bool F32>
 static void launch_bound_gram(const PredictParams& P, unsigned long long* keys, int* idx, double* kmax, double2* mu,
                               cudaStream_t stream) {
     const unsigned ntiles = (unsigned)((P.m + kGramTile - 1) / kGramTile);
+    if (F32 && gram_reg_kernel(P.d)) {
+        switch (cov_code(P.gp[0].family, P.gp[0].nu)) {
+            case 1: launch_bound_gram_reg<1>(P, ntiles, keys, idx, kmax, mu, stream); break;
+            case 2: launch_bound_gram_reg<2>(P, ntiles, keys, idx, kmax, mu, stream); break;
+            default: launch_bound_gram_reg<3>(P, ntiles, keys, idx, kmax, mu, stream); break;
+        }
+        return;
+    }
     const size_t smem = gram_bound_smem(P.d);
     switch (cov_code(P.gp[0].family, P.gp[0].nu)) {
         case 1: predict_bound_gram_kernel<1, F32><<<ntiles, kGramNT, smem, stream>>>(P, keys, idx, kmax, mu); break;

@@ -252,10 +252,15 @@ __device__ __forceinline__ float ex2_ftz(float x) {
     return y;
 }
 
-// k~ of one pair from r~^2 (fp64); z: the exp argument's magnitude (natural units)
+// s: r~^2 (fp64) rounded to fp32 and clamped to [2^-100, r2max]
 template <int COV>
-__device__ __forceinline__ float cov_f32(double r2, float& z) {
-    const float s = fminf(fmaxf(__double2float_rn(r2), 0x1p-100f), CovF32<COV>::r2max);
+__device__ __forceinline__ float cov_f32_arg(double r2) {
+    return fminf(fmaxf(__double2float_rn(r2), 0x1p-100f), CovF32<COV>::r2max);
+}
+
+// k~ of one pair from its clamped fp32 argument s; z: the exp argument's magnitude (natural units)
+template <int COV>
+__device__ __forceinline__ float cov_f32_s(float s, float& z) {
     if (COV == 3) {
         z = 0.5f * s;
         return ex2_ftz(s * CovF32<COV>::ex2c);
@@ -271,14 +276,34 @@ __device__ __forceinline__ float cov_f32(double r2, float& z) {
     return (1.f + z) * e;
 }
 
-// training-side operand, once per fit: row i < n = [-2 Xs_i | 1 | |Xs_i|^2 | 0 ...], zero rows for i >= n; alpha_ in
-// fp32 (0 for i >= n) behind A1 and Ymax, for the fp32 pass
+// k~ of one pair from r~^2 (fp64)
+template <int COV>
+__device__ __forceinline__ float cov_f32(double r2, float& z) {
+    return cov_f32_s<COV>(cov_f32_arg<COV>(r2), z);
+}
+
+// the per-row margin weights of the register-fragment fp32 pass (predict_bound_gram_reg_kernel): (|a| R, |a| Q) in
+// fp32, a = alpha_i in fp32
+template <int COV>
+__device__ __forceinline__ float2 gram_row_weights(float a) {
+    return make_float2(fabsf(a) * CovF32<COV>::rel, fabsf(a) * CovF32<COV>::qz);
+}
+
+// training-side operand, once per fit: row i < n = [-2 Xs_i | 1 | |Xs_i|^2 | 0 ...], zero rows for i >= n; behind A1
+// and Ymax, alpha_ in fp32 (0 for i >= n) for the fp32 passes, then the margin weights of the covariance cov
+// (gram_row_weights; zero for Matern-0.5, which has no Gram pass)
 __global__ void __launch_bounds__(256) gram_operand_kernel(const double* __restrict__ Xs, const double* __restrict__ alphav,
-                                                           int n, int np, int d, double* __restrict__ img) {
+                                                           int n, int np, int d, int cov, double* __restrict__ img) {
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= np) return;
     const int str = gram_stride(d);
-    reinterpret_cast<float*>(img + (size_t)np * str + 2)[i] = i < n ? (float)alphav[i] : 0.f;
+    float* af = reinterpret_cast<float*>(img + (size_t)np * str + 2);
+    const float a = i < n ? (float)alphav[i] : 0.f;
+    af[i] = a;
+    reinterpret_cast<float2*>(af + np)[i] = cov == 1   ? gram_row_weights<1>(a)
+                                            : cov == 2 ? gram_row_weights<2>(a)
+                                            : cov == 3 ? gram_row_weights<3>(a)
+                                                       : make_float2(0.f, 0.f);
     double* row = img + (size_t)i * str;
     double y2 = 0.0;
     for (int j = 0; j < d; ++j) {
@@ -534,6 +559,222 @@ __global__ void __launch_bounds__(kGramNT, F32 ? 3 : 2)
             dmu = __dmul_ru(__dmul_ru(stats[0], 1.0 + 0x1p-20), __fma_ru(3.0 * gn, G.constv, dk));
             kmax_lb = fmax(0.0, __dsub_rd(__dmul_rd(G.constv, kt), dk));
         }
+        const double mu_lo = __dsub_rd(mu, dmu), mu_hi = __dadd_ru(mu, dmu);
+        keys[c0 + c] = prune_bound_key(P, G, mu_lo, mu_hi, prune_var_ub(G, kmax_lb * kmax_lb / G.kdiag));
+        if (idx) idx[c0 + c] = (int)(c0 + c);
+        if (mu_out) mu_out[c0 + c] = make_double2(mu_lo, mu_hi);
+        if (kmax_out) kmax_out[c0 + c] = kmax_lb;
+    }
+}
+
+// ---- the fp32 Gram bound pass with the candidate operand in registers (d <= 16; DESIGN.md 4.9) -----------------------
+// predict_bound_gram_kernel<COV, true> keeps the candidate fragments in shared memory and runs each chunk as a DMMA
+// phase and then a covariance phase, so a warp never has tensor and XU / FMA work ready at once.  Here, with the same
+// launch contract, outputs, ring and candidate build:
+//   * warp w owns candidates (w & 3) * 16 .. +16 and rows (w >> 2) * 32 .. +32 of every chunk: one m16 slab, whose
+//     NKS k-step fragments (2 doubles each, NKS = ceil((d + 2) / 4) <= 5) are loaded into registers once; per chunk
+//     4 n8 tiles x NKS DMMAs read only the training operand from the ring;
+//   * the DMMAs of the next n8 tile (the first tile of the next chunk after the fourth) issue before the covariances of
+//     the current one, so every warp has both kinds of work in flight.  Two tiles of accumulators are live (16
+//     registers): with two halves of 2 tiles (32) beside the 20 fragment registers the kernel spills at 80;
+//   * per pair, one FMNMX keeps the least s~ (cov_f32_arg) per candidate instead of the max of k~ (1 - u (R + Q z~));
+//     the epilogue evaluates that lower bound once, at the least s~: cov_f32_s is a function of s~ alone, so it is the
+//     row's own lower bound, no larger than the row's exact k and so than max_i k_i;
+//   * W takes the per-row weights (|alpha_i| R, |alpha_i| Q) of the operand image: W += k~ fma(z~, |a| Q, |a| R), two
+//     roundings per term before the sum as before (|a| k~ and fma(z~, Q, R)), so (np + 16) 2^-23 still covers the sum.
+// The mu partial still spans four rows in fp32 (2 n8 tiles x 2 rows per thread and candidate), so R and Q are
+// CovF32's.  Thread (g, t4) accumulates candidates g, g + 8 of its slab; partials are added over the quad, then over the
+// two row slabs.  dmu and kmax_lb as predict_bound_gram_kernel<COV, true>'s.  A slot is counted as consumed after the
+// warp's covariances of its fourth tile, its last read of the slot's operand rows, alpha_ words and weights.
+constexpr int kGramRegMaxDim = 16;
+// slot of the register-fragment pass: [PA_CHUNK][str] operand rows, PA_CHUNK alpha_ (fp32), PA_CHUNK weight pairs
+__host__ __device__ inline size_t gram_reg_slot_doubles(int d) { return (size_t)PA_CHUNK * gram_stride(d) + PA_CHUNK * 3 / 2; }
+__host__ __device__ inline size_t gram_reg_bound_smem(int d) {
+    return sizeof(double) * ((size_t)kGramTile * gram_stride(d) + kGramSlots * gram_reg_slot_doubles(d));
+}
+
+// covariances of one thread's 4 pairs of an n8 tile (acc[e]: candidate g + 8 (e >> 1), row 2 t4 + (e & 1) of the tile;
+// al / wt: alpha_ and weights of those two rows), into the fp32 mu partials mp; rows r >= nrow are >= n (MASK) and
+// stay out of the least s~ (their alpha_ and weights are 0)
+template <int COV, bool MASK>
+__device__ __forceinline__ void gram_reg_tile_cov(const double (&acc)[4], const float* al, const float* wt, int nrow,
+                                                  float (&mp)[2], float (&wsum)[2], float (&smin)[2]) {
+    const float2 a = *reinterpret_cast<const float2*>(al);
+    const float4 w = *reinterpret_cast<const float4*>(wt);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const int i = e >> 1, j = e & 1;
+        const float s = cov_f32_arg<COV>(acc[e]);
+        float z;
+        const float k = cov_f32_s<COV>(s, z);
+        smin[i] = fminf(smin[i], MASK && j >= nrow ? INFINITY : s);
+        mp[i] = fmaf(j ? a.y : a.x, k, mp[i]);
+        wsum[i] = fmaf(k, fmaf(z, j ? w.w : w.y, j ? w.z : w.x), wsum[i]);
+    }
+}
+
+template <int COV, int NKS>
+__global__ void __launch_bounds__(kGramNT, 3)
+    predict_bound_gram_reg_kernel(const PredictParams P, unsigned long long* keys, int* idx, double* kmax_out,
+                                  double2* mu_out) {
+    static_assert(COV != 0, "Matern-0.5 has no Lipschitz bound in r^2");
+    static_assert(NKS >= 1 && 4 * NKS <= (kGramRegMaxDim + 2 + 3) / 4 * 4, "k-steps of d <= 16");
+    constexpr double lip = COV == 1 ? 1.5 : COV == 2 ? 5.0 / 6.0 : 0.5;
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[2][kGramTile];
+    __shared__ float w_s[2][kGramTile], s_s[2][kGramTile];
+    __shared__ uint64_t full_bar[kGramSlots];
+    __shared__ unsigned done_cnt[kGramSlots];
+    const GpDev& G = P.gp[0];
+    // gram_stride(d) of every d with NKS k-steps: the operand addresses fold into immediates
+    constexpr int str = NKS & 1 ? 4 * NKS : 4 * NKS + 4;
+    constexpr size_t slot_doubles = (size_t)PA_CHUNK * str + PA_CHUNK * 3 / 2;  // gram_reg_slot_doubles(d)
+    const int tid = threadIdx.x, d = P.d;
+    const long long c0 = (long long)blockIdx.x * kGramTile;
+    double* xa_s = smem;                            // [kGramTile][str]: [x | |x|^2 | 1 | 0 ...]
+    double* ring = smem + (size_t)kGramTile * str;  // slot s: gram_reg_slot_doubles
+    const double* stats = G.gram + (size_t)G.np * str;  // A1, Ymax, alpha_ in fp32, then the weight pairs
+    const float* alpha32 = reinterpret_cast<const float*>(stats + 2);
+    const int nch = G.np / PA_CHUNK;
+    // one thread: chunk ch into the free slot s
+    auto copy = [&](int ch, int s) {
+        constexpr uint32_t abytes = PA_CHUNK * sizeof(float), wbytes = PA_CHUNK * sizeof(float2);
+        constexpr uint32_t obytes = PA_CHUNK * str * sizeof(double);
+        double* dst = ring + s * slot_doubles;
+        tc::mbar_arrive_expect_tx(&full_bar[s], obytes + abytes + wbytes);
+        tc::bulk_g2s(dst, G.gram + (size_t)ch * PA_CHUNK * str, obytes, &full_bar[s]);
+        tc::bulk_g2s(dst + PA_CHUNK * str, alpha32 + (size_t)ch * PA_CHUNK, abytes, &full_bar[s]);
+        tc::bulk_g2s(dst + PA_CHUNK * str + PA_CHUNK / 2, alpha32 + G.np + (size_t)ch * PA_CHUNK * 2, wbytes,
+                     &full_bar[s]);
+    };
+    if (tid == 0) {  // the first chunks load while the candidates are built
+        for (int s = 0; s < kGramSlots; ++s) {
+            tc::mbar_init(&full_bar[s], 1);
+            done_cnt[s] = 0;
+        }
+        tc::mbar_fence_init();
+        for (int s = 0; s < kGramSlots && s < nch; ++s) copy(s, s);
+    }
+    for (int q = tid; q < kGramTile * str; q += kGramNT) {
+        const int c = q / str, j = q - c * str;
+        const long long gi = c0 + c;
+        double v = j == d + 1 ? 1.0 : 0.0;
+        if (j < d && gi < P.m) v = scale_input(candidate_coord(P, gi, j), G.xform, G.ls, j);  // as phase A builds them
+        xa_s[q] = v;
+    }
+    __syncthreads();  // coordinates visible
+    if (tid < kGramTile) {
+        double x2 = 0.0;
+        for (int j = 0; j < d; ++j) x2 = fma(xa_s[tid * str + j], xa_s[tid * str + j], x2);
+        xa_s[tid * str + d] = x2;
+    }
+    __syncthreads();  // norms |x|^2 and the ring's barriers visible
+    const int lane = tid & 31, warp = tid >> 5, g = lane >> 2, t4 = lane & 3;
+    const int cs = warp & 3, rs = warp >> 2;
+    // the thread's place in a slot: operand row rs * 32 + g, column t4 (b fragments); alpha_ / weight rows
+    // rs * 32 + 2 t4 (+ 1)
+    const int boff = (rs * 32 + g) * str + t4, roff = rs * 32 + 2 * t4;
+    double fa[NKS][2];  // a0 / a1 of k-step ks: candidates cs * 16 + g (+ 8), column 4 ks + t4
+#pragma unroll
+    for (int ks = 0; ks < NKS; ++ks) {
+        fa[ks][0] = xa_s[(size_t)(cs * 16 + g) * str + 4 * ks + t4];
+        fa[ks][1] = xa_s[(size_t)(cs * 16 + g + 8) * str + 4 * ks + t4];
+    }
+    double macc[2] = {0.0, 0.0};
+    float wsum[2] = {0.f, 0.f}, smin[2] = {INFINITY, INFINITY};
+    // DMMAs of n8 tile t (rows rs * 32 + t * 8 .. +8) of the chunk in slot buffer buf
+    auto mma = [&](double (&acc)[4], const double* buf, int t) {
+        const double* xb = buf + boff + t * 8 * str;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[e] = 0.0;
+#pragma unroll
+        for (int ks = 0; ks < NKS; ++ks) dmma1684(acc[0], acc[1], acc[2], acc[3], fa[ks][0], fa[ks][1], xb[4 * ks]);
+    };
+    auto slot = [&](int ch) { return ring + (ch % kGramSlots) * slot_doubles; };
+    auto wait = [&](int ch) {
+        tc::mbar_wait_budget(&full_bar[ch % kGramSlots], (uint32_t)(ch / kGramSlots) & 1u, &g_pipe_timeout,
+                             kPipeWaitBudget);
+    };
+    double acc0[4], acc1[4];
+    // chunk ch, whose tile 0 DMMAs are in acc0: per tile t the DMMAs of tile t + 1 (of the next chunk's tile 0 for
+    // t = 3), then tile t's covariances; the mu partial is added to macc after tiles 1 and 3, and the slot released
+    // after tile 3.  MASK: the chunk holds rows >= n
+    auto chunk = [&](int ch, auto mask) {
+        constexpr bool M = decltype(mask)::value;
+        const int s = ch % kGramSlots;
+        const double* buf = slot(ch);
+        const float* al = reinterpret_cast<const float*>(buf + PA_CHUNK * str) + roff;
+        const float* wt = reinterpret_cast<const float*>(buf + PA_CHUNK * str + PA_CHUNK / 2) + 2 * roff;
+        const int nrow = G.n - (ch * PA_CHUNK + roff);  // tile 0 rows r < nrow are < n
+        float mp[2] = {0.f, 0.f};
+        auto flush = [&]() {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                macc[i] += (double)mp[i];
+                mp[i] = 0.f;
+            }
+        };
+        mma(acc1, buf, 1);
+        gram_reg_tile_cov<COV, M>(acc0, al, wt, nrow, mp, wsum, smin);
+        mma(acc0, buf, 2);
+        gram_reg_tile_cov<COV, M>(acc1, al + 8, wt + 16, nrow - 8, mp, wsum, smin);
+        flush();
+        mma(acc1, buf, 3);
+        gram_reg_tile_cov<COV, M>(acc0, al + 16, wt + 32, nrow - 16, mp, wsum, smin);
+        if (ch + 1 < nch) {
+            wait(ch + 1);
+            mma(acc0, slot(ch + 1), 0);
+        }
+        gram_reg_tile_cov<COV, M>(acc1, al + 24, wt + 48, nrow - 24, mp, wsum, smin);
+        flush();
+        __syncwarp();
+        if (lane == 0) {
+            __threadfence_block();  // this warp's reads of slot s happen before its count
+            if ((atomicAdd(&done_cnt[s], 1u) & 7u) == 7u) {  // last of the 8 warps: refill with chunk ch + kGramSlots
+                __threadfence_block();
+                tc::fence_proxy_async_smem();
+                if (ch + kGramSlots < nch) copy(ch + kGramSlots, s);
+            }
+        }
+    };
+    wait(0);
+    mma(acc0, slot(0), 0);
+    // the chunks below n / PA_CHUNK hold no padded row; the mask stays out of their loop (and its code size)
+    const int nfull = G.n / PA_CHUNK;
+    int ch = 0;
+    for (; ch < nfull; ++ch) chunk(ch, std::false_type{});
+    for (; ch < nch; ++ch) chunk(ch, std::true_type{});
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        macc[i] += __shfl_xor_sync(0xffffffffu, macc[i], 1);
+        macc[i] += __shfl_xor_sync(0xffffffffu, macc[i], 2);
+        wsum[i] += __shfl_xor_sync(0xffffffffu, wsum[i], 1);
+        wsum[i] += __shfl_xor_sync(0xffffffffu, wsum[i], 2);
+        smin[i] = fminf(smin[i], __shfl_xor_sync(0xffffffffu, smin[i], 1));
+        smin[i] = fminf(smin[i], __shfl_xor_sync(0xffffffffu, smin[i], 2));
+        if (t4 == 0) {
+            mu_s[rs][cs * 16 + i * 8 + g] = macc[i];
+            w_s[rs][cs * 16 + i * 8 + g] = wsum[i];
+            s_s[rs][cs * 16 + i * 8 + g] = smin[i];
+        }
+    }
+    __syncthreads();
+    const int c = tid;
+    if (c < kGramTile && c0 + c < P.m) {
+        const double u = 0x1p-53;
+        const double gk = (d + 2) * u / (1.0 - (d + 2) * u), gn = G.np * u / (1.0 - G.np * u);
+        const double dr2 = __dmul_ru(kGramCg * gk, __dadd_ru(xa_s[c * str + d], stats[1]));
+        const double mu = G.constv * (mu_s[0][c] + mu_s[1][c]);
+        float z;
+        const float k = cov_f32_s<COV>(fminf(s_s[0][c], s_s[1][c]), z);
+        const double kt = (double)fmaf(k * -0x1p-24f, fmaf(z, CovF32<COV>::qz, CovF32<COV>::rel), k);
+        const double dk1 = __fma_ru(lip, dr2, kGramCcov * u + kF32Abs);  // per unit covariance and row
+        const double w = __dadd_ru((double)w_s[0][c], (double)w_s[1][c]);
+        const double wr = __dmul_ru(__dmul_ru(w, 0x1p-24), 1.0 + (G.np + 16) * 0x1p-23);
+        const double dmu =
+            __dmul_ru(__dmul_ru(G.constv, 1.0 + 0x1p-20), __fma_ru(stats[0], __dadd_ru(dk1, 3.0 * gn), wr));
+        const double kmax_lb =
+            fmax(0.0, __dsub_rd(__dmul_rd(__dmul_rd(G.constv, kt), 1.0 - 0x1p-22), __dmul_ru(G.constv, dk1)));
         const double mu_lo = __dsub_rd(mu, dmu), mu_hi = __dadd_ru(mu, dmu);
         keys[c0 + c] = prune_bound_key(P, G, mu_lo, mu_hi, prune_var_ub(G, kmax_lb * kmax_lb / G.kdiag));
         if (idx) idx[c0 + c] = (int)(c0 + c);

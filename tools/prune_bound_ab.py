@@ -1,5 +1,6 @@
-"""A/B of the two Gram bound passes of pruning (B200BO_PRUNE_BOUND=f64/f32, DESIGN.md 4.9, 6) in one process, on
-both sides of the rule that picks between them (A1 constv 2^-24 <= 1e-3).
+"""A/B of the Gram bound passes of pruning (B200BO_PRUNE_BOUND=f64/f32, DESIGN.md 4.9, 6) in one process, on both
+sides of the rule that picks between them (A1 constv 2^-24 <= 1e-3); the fp32 pass with both of its kernels (f32: the
+default, predict_bound_gram_reg_kernel at d <= 16; f32-ring: B200BO_PRUNE_GRAM_KERNEL=ring).
 
   python tools/prune_bound_ab.py [--reps 3] [--calls 3] [--legs c3,b_m25_c3,b_rbf_long]
 
@@ -24,7 +25,17 @@ from predict_pipe_ab import Sampler, card  # noqa: E402
 from prune_ab import ALPHA, K, LEGS, XI  # noqa: E402
 
 STAGES = ("bound", "sort", "lead", "refine", "final", "tiles")
-PASSES = ("f64", "f32")
+PASSES = ("f64", "f32", "f32-ring")
+SWITCHES = ("B200BO_PRUNE_BOUND", "B200BO_PRUNE_GRAM_KERNEL")
+
+
+def apply_pass(p):
+    for v in SWITCHES:
+        os.environ.pop(v, None)
+    if p:
+        os.environ["B200BO_PRUNE_BOUND"] = p.split("-")[0]
+        if p.endswith("-ring"):
+            os.environ["B200BO_PRUNE_GRAM_KERNEL"] = "ring"
 
 
 def problem(name):
@@ -64,7 +75,7 @@ def leg(name, reps, calls):
     m = x.shape[0]
     xc = torch.from_numpy(np.ascontiguousarray(x)).to(dev)
     sel = torch.zeros((K + 1, 2), dtype=torch.int64, device=dev)
-    os.environ.pop("B200BO_PRUNE_BOUND", None)
+    apply_pass(None)
     auto = C.c_int()
     B.check(L.b200bo_acq_prune_bound_pass(C.byref(spec), C.byref(auto), stream.cuda_stream))
 
@@ -81,7 +92,7 @@ def leg(name, reps, calls):
     res = {p: {"ms": [], "st": [], "clocks": []} for p in PASSES}
     for _ in range(reps):
         for p in PASSES:
-            os.environ["B200BO_PRUNE_BOUND"] = p
+            apply_pass(p)
             call()
             with Sampler() as smp:
                 for _ in range(calls):
@@ -90,7 +101,7 @@ def leg(name, reps, calls):
                     res[p]["st"].append(st)
             res[p]["clocks"].extend(smp.samples)
             res[p].update(evaluated=ev, refined=ref, total=tot, sel=rec)
-    os.environ.pop("B200BO_PRUNE_BOUND", None)
+    apply_pass(None)
     for p in PASSES:
         t, c, st = np.array(res[p]["ms"]), np.array(res[p]["clocks"]), np.array(res[p]["st"]).mean(0)
         print(json.dumps({
