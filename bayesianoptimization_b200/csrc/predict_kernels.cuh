@@ -247,6 +247,19 @@ __device__ __noinline__ double log_cfactor(double lb, double ub, double mean, do
     return lpb + log1mexp(d);
 }
 
+// p = Phi(u) - Phi(l) of one CNEI constraint factor, u = (ub - mean)/sd, l = (lb - mean)/sd: an infinite bound
+// contributes 0 / 1 and a finite bound with sd <= 0 (or a NaN mean) is the frozen-norm NaN, as EI's factor.  A pair
+// with l > 0 (the mean below the lower bound) is reflected, Phi(-l) - Phi(-u), so that a factor far in a constraint's
+// tail keeps its digits instead of cancelling to 0 (EI's factor keeps the reference's unreflected form).
+__device__ __forceinline__ double cnei_factor(double lb, double ub, double mean, double sd) {
+    const bool has_l = lb != -CUDART_INF, has_u = ub != CUDART_INF;
+    if (has_l && lb > mean && sd > 0.0)
+        return ndtr((mean - lb) / sd) - (has_u ? ndtr((mean - ub) / sd) : 0.0);
+    const double p_lo = has_l ? norm_cdf_loc_scale(lb, mean, sd) : 0.0;
+    const double p_hi = has_u ? norm_cdf_loc_scale(ub, mean, sd) : 1.0;
+    return p_hi - p_lo;
+}
+
 // NEI / LogNEI (DESIGN.md 4.13) of one candidate, out of line like mes_term and with scalar arguments only, so that
 // the kernels that inline candidate_epilogue keep their register allocation.  The S fantasy means k*^T a_s
 // (normalised units) come from the candidate's column of the K* tile the kernel already holds (kcol[i * kstr] =
@@ -351,9 +364,7 @@ __device__ __noinline__ double cnei_term(int kind, int g, int n_gps, const doubl
             } else if (lg) {
                 v = carry[s * kstr] + log_cfactor(lb, ub, mean, sd);
             } else {
-                const double p_lo = (lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(lb, mean, sd);
-                const double p_hi = (ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(ub, mean, sd);
-                v = carry[s * kstr] * (p_hi - p_lo);
+                v = carry[s * kstr] * cnei_factor(lb, ub, mean, sd);
             }
             if (last)
                 t[s] = v;
@@ -1711,9 +1722,7 @@ __device__ __noinline__ double cnei_grad_term(const PredictParams& P, const doub
             if (lg) {
                 v = log_cfactor<true>(G.lb, G.ub, mean, sd, &cm, &cs);
             } else {
-                const double p_lo = (G.lb == -CUDART_INF) ? 0.0 : norm_cdf_loc_scale(G.lb, mean, sd);
-                const double p_hi = (G.ub == CUDART_INF) ? 1.0 : norm_cdf_loc_scale(G.ub, mean, sd);
-                v = p_hi - p_lo;
+                v = cnei_factor(G.lb, G.ub, mean, sd);
                 if (sd > 0.0) {
                     if (G.lb != -CUDART_INF) {
                         const double z = (G.lb - mean) / sd, pz = norm_pdf(z);

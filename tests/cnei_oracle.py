@@ -33,14 +33,19 @@ def incumbents(F, ok):
 
 
 def factor(mean, sd, lb, ub):
-    """P = Phi((ub - mean)/sd) - Phi((lb - mean)/sd) with the device's rules: an infinite bound contributes 0 / 1,
-    a finite bound with sd <= 0 gives NaN (scipy's frozen norm)."""
+    """P = Phi((ub - mean)/sd) - Phi((lb - mean)/sd) with the device's rules (cnei_factor): an infinite bound
+    contributes 0 / 1, a finite bound with sd <= 0 gives NaN (scipy's frozen norm), and where the mean lies below a
+    finite lb the pair is reflected, Phi((mean - lb)/sd) - Phi((mean - ub)/sd), so that the upper tail does not
+    cancel."""
     with np.errstate(all="ignore"):
         def cdf(b):
             return np.where(sd > 0.0, ndtr((b - mean) / sd), np.nan)
         p_lo = 0.0 if lb == -np.inf else cdf(lb)
         p_hi = 1.0 if ub == np.inf else cdf(ub)
-        return p_hi - p_lo
+        if lb == -np.inf:
+            return p_hi - p_lo
+        refl = ndtr((mean - lb) / sd) - (0.0 if ub == np.inf else ndtr((mean - ub) / sd))
+        return np.where((lb > mean) & (sd > 0.0), refl, p_hi - p_lo)
 
 
 def cnei(Ks, A, best, sd, xi, Kc_list, Ac_list, sdc_list, lb, ub, y_mean=0.0, y_std=1.0, cy_mean=None, cy_std=None,
