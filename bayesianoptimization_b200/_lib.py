@@ -27,7 +27,8 @@ EXPORTS = [
     "b200bo_gp_set_transform", "b200bo_gp_set_max_values", "b200bo_gp_fit",
     "b200bo_gp_set_data", "b200bo_gp_append", "b200bo_gp_lml", "b200bo_gp_get", "b200bo_gp_n", "b200bo_gp_dim",
     "b200bo_gp_predict", "b200bo_gp_predict_cov", "b200bo_acq_eval", "b200bo_acq_argmin_topk", "b200bo_acq_eval_dev",
-    "b200bo_last_kernel_ms", "b200bo_last_prune_stats", "b200bo_last_prune_stage_ms", "b200bo_acq_prune_bound_dev",
+    "b200bo_last_kernel_ms", "b200bo_last_prune_stats", "b200bo_last_prune_stage_ms",
+    "b200bo_last_prune_levels", "b200bo_acq_prune_bound_dev",
     "b200bo_acq_prune_bound_gram_dev", "b200bo_acq_prune_bound_gram32_dev", "b200bo_acq_prune_bound_pass",
     "b200bo_cov_f32_dev",
     "b200bo_acq_argmin_topk_philox", "b200bo_acq_select_philox_dev", "b200bo_philox_rows",
@@ -113,6 +114,7 @@ def lib():
     L.b200bo_last_kernel_ms.argtypes = [C.POINTER(C.c_float)]
     L.b200bo_last_prune_stats.argtypes = [i64p, i64p]
     L.b200bo_last_prune_stage_ms.argtypes = [C.POINTER(C.c_float), i64p]
+    L.b200bo_last_prune_levels.argtypes = [C.POINTER(C.c_float), i64p, C.POINTER(C.c_int)]
     L.b200bo_acq_prune_bound_dev.argtypes = [C.POINTER(AcqSpec), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                              C.c_void_p]
     L.b200bo_acq_prune_bound_gram_dev.argtypes = [C.POINTER(AcqSpec), C.c_void_p, C.c_int64, C.c_void_p,

@@ -173,17 +173,20 @@ struct b200bo_gp {
     // the control words of predict_acq16_kernel's prune mode
     DevBuf prune_key, prune_idx, prune_tmp, prune_ctl;
     // its refine stages: the interval of K* alpha_ per candidate from the bound pass, the survivor list and its keys
-    // (two buffers each for the sort of the final rounds), the per-row-block partials, K* alpha_ of the tiles and the
-    // arrival counters of predict_units_kernel
-    DevBuf prune_mu, prune_surv, prune_surv_key, prune_part, prune_mu_unit, prune_arrive;
+    // (two buffers each for the sort of the final rounds; with levels, the lists of the levels too), the survivors'
+    // carried prefixes, the per-row-block partials, K* alpha_ of the tiles and the arrival counters of
+    // predict_units_kernel
+    DevBuf prune_mu, prune_surv, prune_surv_key, prune_prefix, prune_part, prune_mu_unit, prune_arrive;
     // candidates of the last call (chunked: all chunks) and those of them evaluated outside the prune mode; the
     // prune mode counts its own in prune_ctl[2] (prune_counted)
     long long stat_total = 0, stat_direct = 0;
     bool prune_counted = false;
     // stage boundaries of the last pruned launch on its stream: after the bound pass, the sort, the lead, refine and
-    // final stages (b200bo_last_prune_stage_ms; the stages start at ev0 and the tile kernel ends at ev1)
-    cudaEvent_t ev_stage[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    // final stages, and after the refine levels (b200bo_last_prune_stage_ms, b200bo_last_prune_levels; the stages start
+    // at ev0 and the tile kernel ends at ev1)
+    cudaEvent_t ev_stage[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool stage_timed = false, stage_refined = false;
+    int stage_levels = 0;  // refine levels of the last pruned launch
     DevBuf pbounds, prow;   // throughput mode: Philox bounds (lo, span) / regenerated winner rows
     bool replica = false;   // predict-only copy made by b200bo_gp_replicate
     // look-ahead Cholesky: bulk stream, chain/bulk events, copy of the next diagonal step's panel block
@@ -1672,39 +1675,80 @@ static bool prune_shared_ks() {
     const char* e = getenv("B200BO_PRUNE_SHARED_KS");
     return !(e && e[0] == '0');
 }
+// B200BO_PRUNE_LEVELS=0: no refine levels; the final stage starts from row block 0 in rounds of 8, 16, 32, the rest.
+static bool prune_levels() {
+    const char* e = getenv("B200BO_PRUNE_LEVELS");
+    return !(e && e[0] == '0');
+}
+
+// Row blocks at which the refine levels end, after the refine stage's b: one level to 2b.  At C3 (DESIGN.md 4.9) the
+// refine stage lets 12.1 tiles through at b = 4, 1.6 at b = 8; a further level cannot shorten the final round,
+// whose latency is that of its last row block.
+static int prune_level_ends(int b, int nb, int* ends) {
+    ends[0] = 2 * b < nb ? 2 * b : nb;
+    return ends[0] < nb ? 1 : 0;
+}
+
+// survivors of the last level in key order (sorted slots pos): their local indices and carried prefixes
+__global__ void level_gather_kernel(const unsigned long long* __restrict__ ctl, int n_word, const int* __restrict__ pos,
+                                    const int* __restrict__ idx, const double* __restrict__ pre, int* __restrict__ idx_out,
+                                    double* __restrict__ pre_out) {
+    const long long n = (long long)ctl[n_word] * 32;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long sl = i >> 5;
+        const int q = (int)(i & 31), p = pos[sl];
+        if (q == 0) idx_out[sl] = idx[p];
+        pre_out[i] = pre[(size_t)p * 32 + q];
+    }
+}
 
 // control words of a launch with refine stages: the tile kernel starts behind the lead tiles, and the lead stage sees
 // the k-th key carried into the launch
 __global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
     ctl[kCtlTile] = ctl[kCtlRefTile] = kLeadTiles;
     ctl[kCtlSurv] = ctl[kCtlUnit] = ctl[kCtlUnitFinal] = 0ull;
+    for (int l = 0; l < kPruneMaxLevels; ++l) ctl[kCtlLevel + l] = 0ull;
     ctl[kCtlKthLead] = ctl[kCtlKth];
 }
 
-// Tiles of the final rounds: 8, 16, 32, then the rest of the kRefineMaxTiles, at most `grid` each (a round's K* slots).
-// One round over all survivors without rounds.
-static int final_round_tiles(bool rounds, int r, int t0, int grid) {
-    const int t = rounds && r < 3 ? 8 << r : kRefineMaxTiles - t0;
+// Tiles of the final rounds: 8, 16, 32, then the rest of the kRefineMaxTiles, at most `grid` each (a round's K* slots);
+// after refine levels 8, then the rest (at C3 the level leaves 1.6 tiles).  One round over all survivors without rounds.
+static int final_round_tiles(bool rounds, bool levels, int r, int t0, int grid) {
+    const int t = rounds && r < (levels ? 1 : 3) ? 8 << r : kRefineMaxTiles - t0;
     return t < grid ? t : grid;
 }
 
 // The lead, refine and final stages of a pruned launch (predict16.cuh), between prune_prepare and the tile kernel.
 // With rounds (prune_rounds) merge_kth_kernel tightens the k-th key after the lead stage and after every final round,
 // and the final rounds take the survivors sorted by key, skipping the tiles above the key.  With shared K*
-// (prune_shared_ks) ks_build_kernel builds the K* of a stage's or round's tiles once, before its units.
+// (prune_shared_ks) ks_build_kernel builds the K* of a stage's or round's tiles once, before its units.  With levels
+// (prune_levels) the refine stage stores every survivor's prefix, each level carries it on over its row blocks and
+// passes its survivors on, and the final stage starts from the last level's row block.
 static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg, int blocks, bool resume,
                                cudaStream_t stream) {
     const int nb = P.gp[0].np / PBM, grid = g0->sm_count;
     const int nsurv = kRefineMaxTiles * PBN;
     const bool rounds = prune_rounds(), shared_ks = prune_shared_ks();
+    int ends[kPruneMaxLevels];
+    const int nlev = prune_levels() ? prune_level_ends(blocks, nb, ends) : 0;
     int rc;
-    if ((rc = g0->prune_surv.reserve(sizeof(int) * 2 * (size_t)nsurv))) return rc;
-    if ((rc = g0->prune_surv_key.reserve(sizeof(unsigned long long) * 2 * (size_t)nsurv))) return rc;
+    if ((rc = g0->prune_surv.reserve(sizeof(int) * 4 * (size_t)nsurv))) return rc;
+    if ((rc = g0->prune_surv_key.reserve(sizeof(unsigned long long) * 3 * (size_t)nsurv))) return rc;
+    if (nlev && (rc = g0->prune_prefix.reserve(sizeof(double) * 2 * 32 * (size_t)nsurv))) return rc;
     if ((rc = g0->prune_part.reserve(sizeof(double) * (size_t)kUnitSlots * nb * 32 * PBN))) return rc;
     if ((rc = g0->prune_mu_unit.reserve(sizeof(double) * (size_t)kUnitSlots * PBN))) return rc;
     if ((rc = g0->prune_arrive.reserve(sizeof(unsigned) * kUnitSlots))) return rc;
     unsigned long long* skey = g0->prune_surv_key.as<unsigned long long>();
     int* sidx = g0->prune_surv.as<int>();
+    // lists A and B (the refine stage writes A, the levels alternate), the slots of the last level for the sort
+    unsigned long long* lkey[2] = {skey, skey + nsurv};
+    int* lidx[2] = {sidx, sidx + nsurv};
+    int* spos = sidx + 2 * nsurv;
+    double* lpre[2] = {nullptr, nullptr};
+    if (nlev) {
+        lpre[0] = g0->prune_prefix.as<double>();
+        lpre[1] = lpre[0] + (size_t)32 * nsurv;
+    }
     cub::DoubleBuffer<unsigned long long> kb(skey, skey + nsurv);
     cub::DoubleBuffer<int> ib(sidx, sidx + nsurv);
     size_t tmp = 0;
@@ -1715,19 +1759,23 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
     if (!resume) CU(cudaMemsetAsync(ctl + kCtlRefined, 0, sizeof(unsigned long long), stream));
     CU(cudaMemsetAsync(g0->prune_arrive.p, 0, sizeof(unsigned) * kUnitSlots, stream));
-    if (rounds) CU(cudaMemsetAsync(skey, 0xFF, sizeof(unsigned long long) * nsurv, stream));  // unused slots sort last
+    if (rounds && !nlev) CU(cudaMemsetAsync(skey, 0xFF, sizeof(unsigned long long) * nsurv, stream));  // unused slots sort last
     prune_ctl_refine_kernel<<<1, 1, 0, stream>>>(ctl);
     LAUNCHED();
-    RefineParams R;
+    RefineParams R = {};
     R.mu = g0->prune_mu.as<double2>();
     R.mu_unit = g0->prune_mu_unit.as<double>();
     R.surv = sidx;
     R.surv_key = skey;
+    R.prefix = nullptr;
     R.part = g0->prune_part.as<double>();
     R.arrive = g0->prune_arrive.as<unsigned>();
     R.blocks = blocks;
     R.groups_max = nb / 2 < 32 ? nb / 2 : 32;
-    R.final_stage = 0;
+    R.final_stage = kStageLead;
+    R.b0 = 0;
+    R.b1 = nb;
+    R.n_word = kCtlSurv;
     R.t0 = 0;
     R.t1 = kRefineMaxTiles;
     R.round_skip = 0;
@@ -1749,24 +1797,77 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     CU(cudaEventRecord(g0->ev_stage[2], stream));
     PredictParams Q = P;  // the lead stage has begun the per-CTA lists
     Q.sel_resume = 1;
+    R.prefix = lpre[0];
     if (dreg)
         predict_refine_kernel<true><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
     else
         predict_refine_kernel<false><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
     LAUNCHED();
     CU(cudaEventRecord(g0->ev_stage[3], stream));
-    R.final_stage = 1;
+    // levels: the survivors of list `in`, counted in word n_word, over row blocks [b0, ends[l]) into the other list
+    int in = 0;
+    R.final_stage = kStageLevel;
+    R.b1 = blocks;
+    for (int l = 0; l < nlev; ++l) {
+        const int out = 1 - in;
+        R.b0 = R.b1;
+        R.b1 = ends[l];
+        R.surv = lidx[in];
+        R.surv_key = lkey[in];
+        R.prefix = lpre[in];
+        R.surv_out = lidx[out];
+        R.surv_key_out = lkey[out];
+        R.prefix_out = lpre[out];
+        R.pos_out = spos;
+        R.out_word = kCtlLevel + l;
+        if (rounds && l == nlev - 1)  // unused slots sort last
+            CU(cudaMemsetAsync(lkey[out], 0xFF, sizeof(unsigned long long) * nsurv, stream));
+        for (int t0 = 0; t0 < kRefineMaxTiles; t0 = R.t1) {
+            R.t0 = t0;
+            R.t1 = t0 + grid < kRefineMaxTiles ? t0 + grid : kRefineMaxTiles;
+            CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+            if (shared_ks) {
+                build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+                LAUNCHED();
+            }
+            units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+            LAUNCHED();
+        }
+        R.n_word = R.out_word;
+        in = out;
+    }
+    g0->stage_levels = nlev;
+    CU(cudaEventRecord(g0->ev_stage[5], stream));
+    R.final_stage = kStageFinal;
+    R.b0 = nlev ? R.b1 : 0;
+    R.b1 = nb;
     R.round_skip = rounds;
+    R.surv = lidx[in];
+    R.surv_key = lkey[in];
+    R.prefix = lpre[in];
     if (rounds) {  // survivors ascending by key; the sentinels of the unused slots last
-        CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, kb, ib, nsurv, 0, 64, stream));
-        LAUNCHED();
-        R.surv = ib.Current();
-        R.surv_key = kb.Current();
+        if (nlev) {  // sorted with their slots, then their indices and prefixes gathered into the other list
+            cub::DoubleBuffer<unsigned long long> lk(lkey[in], skey + 2 * nsurv);
+            cub::DoubleBuffer<int> lp(spos, sidx + 3 * nsurv);
+            CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, lk, lp, nsurv, 0, 64, stream));
+            LAUNCHED();
+            level_gather_kernel<<<2 * grid, 256, 0, stream>>>(ctl, R.n_word, lp.Current(), lidx[in], lpre[in],
+                                                               lidx[1 - in], lpre[1 - in]);
+            LAUNCHED();
+            R.surv = lidx[1 - in];
+            R.surv_key = lk.Current();
+            R.prefix = lpre[1 - in];
+        } else {
+            CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, kb, ib, nsurv, 0, 64, stream));
+            LAUNCHED();
+            R.surv = ib.Current();
+            R.surv_key = kb.Current();
+        }
     }
     for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r) {
         R.t0 = t0;
-        R.t1 = t0 + final_round_tiles(rounds, r, t0, grid);
-        if (r > 0) CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+        R.t1 = t0 + final_round_tiles(rounds, nlev > 0, r, t0, grid);
+        if (r > 0 || nlev) CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
         if (shared_ks) {
             build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
             LAUNCHED();
@@ -2347,6 +2448,7 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             if (prune && (rc = prune_prepare(g0, P, sm.resume, stream))) return rc;
             const int refine = prune && predict_mma() == 1684 ? prune_refine_blocks(P.gp[0].np, ntiles) : 0;
             g0->stage_refined = refine > 0;
+            g0->stage_levels = 0;
             if (refine) {
                 // every SM keeps a list, begun by the lead stage and continued by the final stage and the tile kernel
                 grid = g0->sm_count;
@@ -2544,14 +2646,35 @@ extern "C" int b200bo_last_prune_stage_ms(float* ms, int64_t* refined) {
     CU(cudaEventElapsedTime(&ms[0], g0->ev0, g0->ev_stage[0]));
     CU(cudaEventElapsedTime(&ms[1], g0->ev_stage[0], g0->ev_stage[1]));
     cudaEvent_t last = g0->ev_stage[1];
-    if (g0->stage_refined) {
-        for (int i = 2; i < 5; ++i) CU(cudaEventElapsedTime(&ms[i], g0->ev_stage[i - 1], g0->ev_stage[i]));
+    if (g0->stage_refined) {  // the refine levels are counted with the refine stage
+        CU(cudaEventElapsedTime(&ms[2], g0->ev_stage[1], g0->ev_stage[2]));
+        CU(cudaEventElapsedTime(&ms[3], g0->ev_stage[2], g0->ev_stage[5]));
+        CU(cudaEventElapsedTime(&ms[4], g0->ev_stage[5], g0->ev_stage[4]));
         last = g0->ev_stage[4];
         unsigned long long n = 0;
         CU(cudaMemcpy(&n, g0->prune_ctl.as<unsigned long long>() + kCtlRefined, sizeof(n), cudaMemcpyDeviceToHost));
         *refined = (int64_t)n;
     }
     CU(cudaEventElapsedTime(&ms[5], last, g0->ev1));
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_last_prune_levels(float* ms, int64_t* passed, int* levels) {
+    if (!ms || !passed || !levels) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!g_last_timed) return set_err(B200BO_ERR_STATE, "no timed kernel on this thread");
+    b200bo_gp* g0 = g_last_timed;
+    if (!g0->stage_timed) return set_err(B200BO_ERR_STATE, "the last launch on this thread was not pruned");
+    CU(cudaSetDevice(g0->device));
+    CU(cudaEventSynchronize(g0->ev1));
+    *ms = 0.f;
+    *levels = g0->stage_refined ? g0->stage_levels : 0;
+    for (int l = 0; l <= kPruneMaxLevels; ++l) passed[l] = 0;
+    if (!g0->stage_refined) return B200BO_OK;
+    CU(cudaEventElapsedTime(ms, g0->ev_stage[3], g0->ev_stage[5]));
+    unsigned long long w[kCtlWords];
+    CU(cudaMemcpy(w, g0->prune_ctl.as<unsigned long long>(), sizeof(w), cudaMemcpyDeviceToHost));
+    passed[0] = (int64_t)w[kCtlSurv];
+    for (int l = 0; l < *levels; ++l) passed[l + 1] = (int64_t)w[kCtlLevel + l];
     return B200BO_OK;
 }
 

@@ -795,7 +795,9 @@ enum {
     kCtlKthLead = 7,  // the k-th key as it was before the lead stage
     kCtlUnitFinal = 8,  // the same for the current final round
     kCtlKthRound = 9,   // the k-th key as it was before the current final round (written by merge_kth_kernel)
-    kCtlWords = 10
+    kCtlLevel = 10,     // [kPruneMaxLevels] candidates each refine level let through
+    kPruneMaxLevels = 4,
+    kCtlWords = kCtlLevel + kPruneMaxLevels
 };
 
 // Prune mode of predict_acq16_kernel: thread 0 claims the next tile in bound order and stops the CTA (returns ntiles)
@@ -837,11 +839,12 @@ __device__ __forceinline__ void predict16_load_stage(double* as, double* bs, con
 // Row blocks [ib0, ib1) of L^-1.  PART = false: red = the sums over those blocks (the whole product: 0, np / PBM).
 // PART = true (predict_units_kernel): nothing is summed across row blocks; every thread stores its s(ib) (the sum of
 // squares of its 4 rows, per column) to part[ib][wm][g][column], and the tile's finisher adds them in this function's
-// order (unit_finish_colsq).
+// order (unit_finish_colsq).  PART = false with `pre` (predict_refine_kernel): every thread also stores its running
+// sums before the xor tree to pre[wm * 8 + g][column], the prefix a later pass carries on from row block ib1.
 template <int MMA, bool PART>
 __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* __restrict__ Ks, double* smem,
                                                   unsigned long long pol_last, unsigned long long pol_first, int ib0,
-                                                  int ib1, double* __restrict__ part) {
+                                                  int ib1, double* __restrict__ part, double* pre = nullptr) {
     static_assert(MMA == 884 || MMA == 1684, "phase B shape");
     constexpr int STR = PSTR_DMMA, BK = PBK_DMMA;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -935,6 +938,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             double v = csq[j][e];
+            if (pre) pre[(wm * 8 + g) * PBN + wn * 32 + j * 8 + t4 * 2 + e] = v;
             v += __shfl_xor_sync(0xffffffffu, v, 4);
             v += __shfl_xor_sync(0xffffffffu, v, 8);
             v += __shfl_xor_sync(0xffffffffu, v, 16);
@@ -1242,8 +1246,12 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
 //           with the leading b row blocks of L^-1 only.  r_b = sum of V_i^2 over those rows is k*^T K^-1 k* of the GP
 //           conditioned on the first b * PBM training points alone, and the remaining terms are squares, so
 //           r_b <= k*^T K^-1 k* and prune_var_ub(r_b) bounds the variance as the single-point r does.  Candidates whose
-//           refined key and single-point key are both <= the k-th key are appended to the survivor list;
-//   final   the survivors through predict_units_kernel.
+//           refined key and single-point key are both <= the k-th key are appended to the survivor list, with the
+//           running sums of their first b row blocks (the prefix);
+//   levels  predict_units_kernel over row blocks [b_l, b_l+1) of the survivors only: the last unit of a tile carries
+//           each survivor's prefix on to b_l+1, keys it as the refine stage does and appends the survivors whose
+//           keys are all <= the k-th key, with the new prefix, to the next level's list;
+//   final   the survivors through predict_units_kernel, from the carried prefix on.
 // When more than kRefineMaxTiles tiles of survivors come up (little prunes: the refine stage stops claiming tiles as
 // soon as it sees that), the final stage does nothing and the tile kernel goes on in bound order behind the lead
 // tiles as it would have without these stages; otherwise the final stage closes the tile kernel's counter.
@@ -1254,23 +1262,35 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
 constexpr int kLeadTiles = 8, kRefineMaxTiles = 128, kUnitSlots = kLeadTiles + kRefineMaxTiles;
 constexpr long long kCtlClosed = 1ll << 40;  // value of kCtlTile no batch reaches
 
+enum { kStageLead = 0, kStageFinal = 1, kStageLevel = 2 };
+
 struct RefineParams {
     const double2* mu;       // [m] interval (mu_lo, mu_hi) of K* alpha_ per candidate (local index), from the bound pass
     double* mu_unit;         // [kUnitSlots][PBN] K* alpha_ of a tile's candidates, from its last group's phase A
     int* surv;               // [kRefineMaxTiles * PBN] local indices the refine stage let through (final: sorted)
     unsigned long long* surv_key;  // [kRefineMaxTiles * PBN] their keys (max of single-point and refined key)
+    // [kRefineMaxTiles * PBN][32] per survivor, the running sums over row blocks [0, b0) per (row slab wm, lane group
+    // g), index wm * 8 + g, before the xor tree; nullptr: none (the lead, and every stage without levels)
+    double* prefix;
+    int* surv_out;           // a level: the survivors it lets through, their keys, prefixes and slots (the values of
+    unsigned long long* surv_key_out;  // the final sort)
+    double* prefix_out;
+    int* pos_out;
     double* part;            // [kUnitSlots][np / PBM][4][8][PBN] per-row-block partial sums of squares
     unsigned* arrive;        // [kUnitSlots] units that have delivered their part of a tile
     int blocks;              // leading row blocks of the refined bound
     int groups_max;          // most units a tile is split into
-    int final_stage;         // predict_units_kernel: 0 lead, 1 final
-    int t0, t1;              // final stage: the round's tiles [t0, t1) of the survivor list
+    int final_stage;         // predict_units_kernel: kStageLead, kStageFinal or kStageLevel
+    int b0, b1;              // the units' row blocks [b0, b1): the lead and the final stage end at np / PBM
+    int n_word;              // final stage and levels: the prune_ctl word counting their candidates
+    int out_word;            // a level: the prune_ctl word counting the candidates it lets through
+    int t0, t1;              // final stage and levels: the round's tiles [t0, t1) of the survivor list
     int round_skip;          // final stage: skip a tile whose first key is above kCtlKthRound
 };
 
-// The tiles of a lead stage or final round, the same in every CTA: candidates list[0, n), tiles [tbeg, tend) of
-// PBN columns, partial-sum slots from slot0.  Final stage: too many survivors leave n = 0 (the tile kernel takes over
-// in bound order); otherwise the stage closes the tile kernel's counter.
+// The tiles of a lead stage, level or final round, the same in every CTA: candidates list[0, n), tiles [tbeg, tend)
+// of PBN columns, partial-sum slots from slot0.  Levels and final stage: too many refine survivors leave n = 0 (the
+// tile kernel takes over in bound order); otherwise the final stage closes the tile kernel's counter.
 struct UnitRound {
     const int* list;
     long long n, tbeg, tend;
@@ -1282,10 +1302,13 @@ __device__ __forceinline__ UnitRound unit_round(const PredictParams& P, const Re
     U.n = min(P.m, (long long)kLeadTiles * PBN);
     U.slot0 = 0;
     U.tbeg = 0;
-    if (R.final_stage) {
-        U.n = (long long)P.prune_ctl[kCtlSurv];
-        if (U.n > (long long)kRefineMaxTiles * PBN) U.n = 0;
-        else if (blockIdx.x == 0 && threadIdx.x == 0) atomicExch(P.prune_ctl + kCtlTile, (unsigned long long)kCtlClosed);
+    if (R.final_stage != kStageLead) {
+        U.n = 0;
+        if (P.prune_ctl[kCtlSurv] <= (unsigned long long)kRefineMaxTiles * PBN) {
+            U.n = (long long)P.prune_ctl[R.n_word];
+            if (R.final_stage == kStageFinal && blockIdx.x == 0 && threadIdx.x == 0)
+                atomicExch(P.prune_ctl + kCtlTile, (unsigned long long)kCtlClosed);
+        }
         U.list = R.surv;
         U.slot0 = kLeadTiles;
         U.tbeg = R.t0;
@@ -1297,7 +1320,8 @@ __device__ __forceinline__ UnitRound unit_round(const PredictParams& P, const Re
 
 // whether every unit of tile `tile` skips it: its best bound key is above the k-th key copied before the stage / round
 __device__ __forceinline__ bool unit_skip(const PredictParams& P, const RefineParams& R, long long tile) {
-    if (!R.final_stage) return P.perm_key[tile * PBN] > P.prune_ctl[kCtlKthLead];
+    if (R.final_stage == kStageLead) return P.perm_key[tile * PBN] > P.prune_ctl[kCtlKthLead];
+    if (R.final_stage == kStageLevel) return false;  // no exact value moves the k-th key between levels
     return R.round_skip && R.surv_key[tile * PBN] > P.prune_ctl[kCtlKthRound];
 }
 
@@ -1346,26 +1370,33 @@ __global__ void __launch_bounds__(32) merge_kth_kernel(const SelList* __restrict
     }
 }
 
-// first row block of group j of G over nb row blocks, cut so that the groups' k-tile counts (row block ib: ib + 1) are
-// about equal; j = G gives nb.  Groups may be empty.
-__host__ __device__ inline int unit_cut(int nb, int G, int j) {
-    const long long total = (long long)nb * (nb + 1) / 2;
-    int ib = 0;
-    while (ib < nb && (long long)ib * (ib + 1) / 2 * G < total * j) ++ib;
+// first row block of group j of G over the row blocks [b0, nb), cut so that the groups' k-tile counts (row block ib:
+// ib + 1) are about equal; j = G gives nb.  Groups may be empty.
+__host__ __device__ inline int unit_cut(int b0, int nb, int G, int j) {
+    const long long base = (long long)b0 * (b0 + 1) / 2, total = (long long)nb * (nb + 1) / 2 - base;
+    int ib = b0;
+    while (ib < nb && ((long long)ib * (ib + 1) / 2 - base) * G < total * j) ++ib;
     return j >= G ? nb : ib;
 }
 
-// sum over the row blocks [0, nb) of a tile's partials, in the order of predict16_phase_b: per (row slab wm, lane
-// group g) over ib, then the xor-shuffle tree over g (4, 8, 16: ((0+1)+(2+3))+((4+5)+(6+7))), written to red[wm][c];
-// the caller adds the slabs.  512 threads: thread = (wm, column).
-__device__ __forceinline__ void unit_finish_colsq(const double* __restrict__ part, int nb, double* red) {
+// sum over the row blocks [ib0, nb) of a tile's partials, in the order of predict16_phase_b: per (row slab wm, lane
+// group g) over ib, starting from the carried prefix of row blocks [0, ib0) (pre_in[column][wm * 8 + g]; nullptr:
+// ib0 = 0, from 0), then the xor-shuffle tree over g (4, 8, 16: ((0+1)+(2+3))+((4+5)+(6+7))), written to red[wm][c];
+// the caller adds the slabs.  pre_out (nullable): the sums before the tree, [wm * 8 + g][c].  Columns from ncols on
+// read no prefix.  512 threads: thread = (wm, column).
+__device__ __forceinline__ void unit_finish_colsq(const double* __restrict__ part, const double* __restrict__ pre_in,
+                                                  long long ncols, int ib0, int nb, double* red, double* pre_out) {
     const int c = threadIdx.x & (PBN - 1), wm = threadIdx.x >> 7;
     double v[8];
 #pragma unroll
-    for (int g = 0; g < 8; ++g) v[g] = 0.0;
-    for (int ib = 0; ib < nb; ++ib) {
+    for (int g = 0; g < 8; ++g) v[g] = pre_in && c < ncols ? __ldcg(pre_in + (size_t)c * 32 + wm * 8 + g) : 0.0;
+    for (int ib = ib0; ib < nb; ++ib) {
 #pragma unroll
         for (int g = 0; g < 8; ++g) v[g] += __ldcg(part + ((size_t)(ib * 4 + wm) * 8 + g) * PBN + c);
+    }
+    if (pre_out) {
+#pragma unroll
+        for (int g = 0; g < 8; ++g) pre_out[(wm * 8 + g) * PBN + c] = v[g];
     }
     red[wm * PBN + c] = ((v[0] + v[1]) + (v[2] + v[3])) + ((v[4] + v[5]) + (v[6] + v[7]));
 }
@@ -1398,7 +1429,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
         if (tile >= ntiles) break;
         const long long c0 = tile * PBN;
         phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, R.blocks * PBM);
-        predict16_phase_b<1684, false>(G, Ks, smem, pol_last, pol_first, 0, R.blocks, nullptr);
+        double* pre = R.prefix ? smem + 4 * PBN : nullptr;  // [32][PBN] behind red
+        predict16_phase_b<1684, false>(G, Ks, smem, pol_last, pol_first, 0, R.blocks, nullptr, pre);
         const double* red = smem;
         if (tid < PBN && c0 + tid < P.m) {
             const int c = tid, li = P.perm[c0 + c];
@@ -1411,6 +1443,10 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
                 if (pos < (unsigned long long)kRefineMaxTiles * PBN) {
                     R.surv[pos] = li;
                     R.surv_key[pos] = key > key1 ? key : key1;  // both are lower bounds
+                    if (pre) {
+#pragma unroll 4
+                        for (int q = 0; q < 32; ++q) R.prefix[pos * 32 + q] = pre[q * PBN + c];
+                    }
                 }
             }
         }
@@ -1418,8 +1454,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
     }
 }
 
-// K* of the tiles of a lead stage or final round (unit_round, unit_skip), each into its own scratch slot
-// (tile - tbeg; a round has at most gridDim.x tiles), with phase_a's arithmetic: items (tile, chunks [ch0, ch1)), the
+// K* rows [0, PBM * b1) of the tiles of a lead stage, level or final round (unit_round, unit_skip), each into its own
+// scratch slot (tile - tbeg; a round has at most gridDim.x tiles), with phase_a's arithmetic: items (tile, chunks [ch0, ch1)), the
 // chunks of a tile cut so that there are about gridDim.x items.  Plain stores: every unit of the tile reads the slot.
 template <bool DREG>
 __global__ void __launch_bounds__(P16_NT, 1) ks_build_kernel(const PredictParams P, const RefineParams R) {
@@ -1429,7 +1465,7 @@ __global__ void __launch_bounds__(P16_NT, 1) ks_build_kernel(const PredictParams
     const UnitRound U = unit_round(P, R);
     const long long nt = U.tend - U.tbeg;
     if (nt <= 0) return;
-    const int nch = G.np / PA_CHUNK;
+    const int nch = R.b1 * PBM / PA_CHUNK;
     const int per = (int)max(1ll, (nch * nt + gridDim.x - 1) / gridDim.x), items = (nch + per - 1) / per;
     for (long long it = blockIdx.x; it < nt * items; it += gridDim.x) {
         const long long tile = U.tbeg + it / items;
@@ -1455,13 +1491,15 @@ __device__ __forceinline__ void unit_mu_from_ks(const GpDev& G, const double* __
     mu_s[part][c] = mu;
 }
 
-// Exact evaluation in units of (tile, group of consecutive row blocks).  Lead stage: the tiles are the first
-// kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this launch (a
+// Exact evaluation in units of (tile, group of consecutive row blocks of [b0, b1)).  Lead stage: the tiles are the
+// first kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this launch (a
 // continued batch; read from kCtlKthLead, which does not move, so that all units of a tile decide alike).  Final
 // stage: the tiles [t0, t1) of the survivor list, with round_skip each skipped when its first key is above
-// kCtlKthRound.  A unit builds K* for the rows its row blocks need in its CTA's scratch (SHARED_KS: reads the tile's
-// slot that ks_build_kernel filled, and the unit of the last group computes mu from it), runs phase B over its row
-// blocks, and the last unit to arrive finishes the tile as the tile kernel's epilogue does.
+// kCtlKthRound.  A level: the tiles [t0, t1) of its survivor list, none skipped.  A unit builds K* for the rows its
+// row blocks need in its CTA's scratch (SHARED_KS: reads the tile's slot that ks_build_kernel filled, and the unit of
+// the last group computes mu from it), runs phase B over its row blocks, and the last unit to arrive finishes the
+// tile: from the survivors' carried prefix on, as the tile kernel's epilogue does (lead, final), or as the refine
+// stage keys its candidates at b1 row blocks (a level).
 template <bool DREG, bool SHARED_KS>
 __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictParams P, const RefineParams R) {
     extern __shared__ __align__(16) double smem[];
@@ -1479,9 +1517,10 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
     const int* list = U.list;
     const long long n = U.n;
     unsigned long long* claim = P.prune_ctl + (R.final_stage ? kCtlUnitFinal : kCtlUnit);
+    const int b0 = R.b0, b1 = R.b1;
     int groups = R.groups_max;
-    if (R.final_stage && U.tend > U.tbeg)
-        groups = (int)max(1ll, min((long long)R.groups_max, 2ll * gridDim.x / (U.tend - U.tbeg)));
+    if (R.final_stage != kStageLead && U.tend > U.tbeg)
+        groups = (int)max(1ll, min((long long)min(R.groups_max, b1 - b0), 2ll * gridDim.x / (U.tend - U.tbeg)));
     for (;;) {
         if (tid == 0) unit_s = (long long)atomicAdd(claim, 1ull);
         __syncthreads();
@@ -1494,7 +1533,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
             continue;
         }
         const int grp = (int)(unit - (tile - U.tbeg) * groups);
-        const int ib0 = unit_cut(nb, groups, grp), ib1 = unit_cut(nb, groups, grp + 1);
+        const int ib0 = unit_cut(b0, b1, groups, grp), ib1 = unit_cut(b0, b1, groups, grp + 1);
         const int slot = U.slot0 + (int)tile;
         double* part = R.part + (size_t)slot * nb * 32 * PBN;
         if (ib1 > ib0) {
@@ -1516,10 +1555,28 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
         __syncthreads();
         if (last_s) {
             __threadfence();
+            if (tid == 0) R.arrive[slot] = 0u;  // every unit of the tile has arrived: the slot's next level starts at 0
             double* red = smem;
-            unit_finish_colsq(part, nb, red);
+            double* pre = R.final_stage == kStageLevel ? smem + 4 * PBN : nullptr;  // [32][PBN] behind red
+            unit_finish_colsq(part, R.prefix ? R.prefix + c0 * 32 : nullptr, n - c0, b0, b1, red, pre);
             __syncthreads();
-            if (tid < PBN) {
+            if (R.final_stage == kStageLevel) {
+                if (tid < PBN && c0 + tid < n) {
+                    const int c = tid, li = list[c0 + c];
+                    const double r = ((red[c] + red[PBN + c]) + red[2 * PBN + c]) + red[3 * PBN + c];
+                    const double2 mu = R.mu[li];
+                    const unsigned long long key = prune_bound_key(P, G, mu.x, mu.y, prune_var_ub(G, r));
+                    const unsigned long long key1 = R.surv_key[c0 + c], kth = P.prune_ctl[kCtlKth];
+                    if (key <= kth && key1 <= kth) {
+                        const unsigned long long pos = atomicAdd(P.prune_ctl + R.out_word, 1ull);
+                        R.surv_out[pos] = li;
+                        R.surv_key_out[pos] = key > key1 ? key : key1;  // every key is a lower bound
+                        R.pos_out[pos] = (int)pos;
+#pragma unroll 4
+                        for (int q = 0; q < 32; ++q) R.prefix_out[pos * 32 + q] = pre[q * PBN + c];
+                    }
+                }
+            } else if (tid < PBN) {
                 const int c = tid;
                 const bool valid = c0 + c < n;
                 const long long gi = valid ? (long long)list[c0 + c] : P.m;

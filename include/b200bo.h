@@ -519,12 +519,20 @@ int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total);
 
 /* Where the kernel time of the most recent pruned launch on this thread went (a streamed or split batch: its last
  * launch), from CUDA events recorded between the stages on the call's stream: ms[0] bound pass, ms[1] sort,
- * ms[2] lead (the first tiles in bound order, split across SMs), ms[3] refine (leading-row-block bound), ms[4] final
- * (exact evaluation of the refine survivors, split across SMs), ms[5] the whole-tile kernel in bound order.  ms[2..4]
+ * ms[2] lead (the first tiles in bound order, split across SMs), ms[3] refine (leading-row-block bound, and its
+ * levels), ms[4] final (exact evaluation of the refine survivors, split across SMs), ms[5] the whole-tile kernel in
+ * bound order.  ms[2..4]
  * are 0 when the refine stages did not run (B200BO_PRUNE_REFINE=0, DESIGN.md 4.9).  *refined = candidates that went
  * through the refine stage (all launches of the call).  B200BO_ERR_STATE when the launch was not pruned.  Synchronises
  * on the stop event; nothing is read back unless this is called. */
 int b200bo_last_prune_stage_ms(float ms[6], int64_t* refined);
+
+/* The refine levels of the most recent pruned launch on this thread (DESIGN.md 4.9): *ms = their time (part of
+ * ms[3] of b200bo_last_prune_stage_ms), *levels = how many ran (0 with B200BO_PRUNE_LEVELS=0 or without refine
+ * stages), passed[0] = candidates the refine stage let through (more than 16384: the tile kernel took over and no
+ * level ran), passed[1 + l] = those level l let through; passed has room for 5.  B200BO_ERR_STATE when the launch was
+ * not pruned.  Synchronises on the stop event. */
+int b200bo_last_prune_levels(float* ms, int64_t passed[5], int* levels);
 
 /* The direct bound pass of selection-only pruning alone (the one the selection runs for Matern-0.5; EI, UCB, PoI,
  * LogEI or LogPoI on one GP; 1 <= m <= INT_MAX device rows d_Xc):

@@ -8,8 +8,9 @@ rounds and shared K*:  --settings ROUNDS=0+SHARED_KS=0,ROUNDS=1+SHARED_KS=1  (na
 fp32 Gram bound kernels:  --settings GRAM_KERNEL=ring,GRAM_KERNEL=reg
 
 Legs as in tools/prune_ab.py (argmin + top-10; Matern-2.5, alpha 1e-6, normalize_y).  Per leg and setting:
-b200bo_last_kernel_ms mean (min-max), the stage split of b200bo_last_prune_stage_ms (bound pass, sort, lead, refine,
-final, whole-tile kernel; mean over the timed calls), the candidates that went through the full N^2 term and through
+b200bo_last_kernel_ms mean (min-max), the stage split of b200bo_last_prune_stage_ms (bound pass, sort, lead, refine
+with its levels, final, whole-tile kernel; mean over the timed calls), the levels' part of the refine stage and the
+candidates the refine stage and each level let through (b200bo_last_prune_levels), the candidates that went through the full N^2 term and through
 the refine stage, the median SM clock and power draw sampled read-only by nvidia-smi, and whether the records (value
 bits and indices) equal those of B200BO_PRUNE=0 (one extra call; --no-exact skips it: at c5 it takes seconds).
 """
@@ -30,7 +31,8 @@ from predict_pipe_ab import Sampler, card  # noqa: E402
 from prune_ab import ALPHA, K, LEGS, XI  # noqa: E402
 
 STAGES = ("bound", "sort", "lead", "refine", "final", "tiles")
-SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_ROUNDS", "B200BO_PRUNE_SHARED_KS", "B200BO_PRUNE_GRAM_KERNEL")
+SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_ROUNDS", "B200BO_PRUNE_SHARED_KS", "B200BO_PRUNE_GRAM_KERNEL",
+            "B200BO_PRUNE_LEVELS")
 
 
 def setting_env(s):
@@ -76,30 +78,33 @@ def leg(name, settings, reps, calls, exact):
             B.check(L.b200bo_acq_eval_dev(C.byref(spec), xc.data_ptr(), m, None, None, None, K, sel.data_ptr(), 0,
                                           stream.cuda_stream))
         ms, ev, tot, ref = C.c_float(), C.c_int64(), C.c_int64(), C.c_int64()
-        st = (C.c_float * 6)()
+        st, lms, passed, nlev = (C.c_float * 6)(), C.c_float(), (C.c_int64 * 5)(), C.c_int()
         B.check(L.b200bo_last_kernel_ms(C.byref(ms)))
         B.check(L.b200bo_last_prune_stats(C.byref(ev), C.byref(tot)))
         if stages:
             B.check(L.b200bo_last_prune_stage_ms(st, C.byref(ref)))
-        return ms.value, list(st), ev.value, ref.value, tot.value, sel.cpu().numpy().copy()
+            B.check(L.b200bo_last_prune_levels(C.byref(lms), passed, C.byref(nlev)))
+        lev = (lms.value, list(passed)[:nlev.value + 1])
+        return ms.value, list(st), ev.value, ref.value, tot.value, sel.cpu().numpy().copy(), lev
 
     ref_sel = None
     if exact:
         os.environ["B200BO_PRUNE"] = "0"
         ref_sel = call(stages=False)[5]
         os.environ.pop("B200BO_PRUNE")
-    res = {s: {"ms": [], "st": [], "clocks": []} for s in settings}
+    res = {s: {"ms": [], "st": [], "lev_ms": [], "clocks": []} for s in settings}
     for _ in range(reps):
         for s in settings:
             apply_setting(s)
             call()  # warm-up of this setting
             with Sampler() as smp:
                 for _ in range(calls):
-                    ms, st, ev, ref, tot, rec = call()
+                    ms, st, ev, ref, tot, rec, (lev_ms, passed) = call()
                     res[s]["ms"].append(ms)
                     res[s]["st"].append(st)
+                    res[s]["lev_ms"].append(lev_ms)
             res[s]["clocks"].extend(smp.samples)
-            res[s].update(evaluated=ev, refined=ref, total=tot, sel=rec)
+            res[s].update(evaluated=ev, refined=ref, total=tot, sel=rec, passed=passed)
     apply_setting("1")
     os.environ.pop("B200BO_PRUNE_REFINE")
     base = float(np.mean(res[settings[0]]["ms"]))
@@ -110,6 +115,7 @@ def leg(name, settings, reps, calls, exact):
             "kernel_ms_min_max": [round(float(t.min()), 3), round(float(t.max()), 3)],
             "speedup_vs_first_setting": round(base / float(t.mean()), 3),
             "stage_ms": {k: round(float(v), 3) for k, v in zip(STAGES, st)},
+            "levels_ms": round(float(np.mean(res[s]["lev_ms"])), 3), "passed_refine_then_levels": res[s]["passed"],
             "evaluated": res[s]["evaluated"], "refined": res[s]["refined"], "total": res[s]["total"],
             "evaluated_frac": res[s]["evaluated"] / res[s]["total"],
             "refined_frac": res[s]["refined"] / res[s]["total"],
