@@ -4,17 +4,20 @@ predict_bound_kernel (csrc/predict16.cuh) keys every candidate by v_lb, a lower 
 from the posterior mean and the largest cross-covariance alone:
     var_ub = min(prior, prior - max_i k*_i^2 / K_ii + eps * prior) >= sigma^2
 and EI / UCB (as max(mu, mu + kappa sigma)) / PoI (while a < 0) at sigma_ub, lowered by a relative and an absolute
-margin.  Candidates whose mean or bound is not finite, or whose a = mu - y_max - xi is within a few ulps of 0, are never
+margin (LogEI / LogPoI: the logs of EI / PoI, LogPoI 0 for a >= 0, lowered by 1e-9 |v| + 1e-9).  Candidates whose mean or bound is not finite, or whose a = mu - y_max - xi is within a few ulps of 0, are never
 pruned (key 0).  Here: the bound lies below sklearn's exact closure value on small problems, training points and
 near-duplicates included, for every acquisition kind and kappa of either sign.
 """
 import numpy as np
 import pytest
 from scipy.stats import norm
+
+import logei_oracle as LO
 from sklearn.gaussian_process import GaussianProcessRegressor
 from sklearn.gaussian_process.kernels import RBF, ConstantKernel, Matern, WhiteKernel
 
 VAR_EPS, REL_MARGIN, ABS_MARGIN = 1e-8, 1e-9, 1e-300  # kPruneVarEps, kPruneRelMargin, kPruneAbsMargin
+LOG_ABS_MARGIN = 1e-9  # kPruneLogAbsMargin
 
 
 def bound_value(kind, mu, kmax, prior, kdiag, y_std, y_max, kappa, xi):
@@ -30,6 +33,10 @@ def bound_value(kind, mu, kmax, prior, kdiag, y_std, y_max, kappa, xi):
             z = a / sd
             base = a * norm.cdf(z) + sd * norm.pdf(z)
             scale = np.abs(base)
+        elif kind in ("logei", "logpoi"):
+            code = LO.LOGEI if kind == "logei" else LO.LOGPOI
+            base = np.where((kind == "logpoi") & (a >= 0), 0.0, LO.log_acq_term(code, a, sd))
+            scale = np.abs(base) + LOG_ABS_MARGIN / REL_MARGIN
         else:
             base = np.where(a < 0, norm.cdf(a / sd), 1.0)
             scale = np.abs(base)
@@ -50,6 +57,8 @@ def exact_value(kind, mu, sd, y_max, kappa, xi):
         z = a / sd
         if kind == "ei":
             return -(a * norm.cdf(z) + sd * norm.pdf(z))
+        if kind in ("logei", "logpoi"):
+            return -LO.log_acq_term(LO.LOGEI if kind == "logei" else LO.LOGPOI, a, sd)
         return -norm.cdf(z)
 
 
@@ -62,7 +71,8 @@ KERNELS = {
 
 
 @pytest.mark.parametrize("kname", sorted(KERNELS))
-@pytest.mark.parametrize("kind,kappa", [("ei", 0.0), ("poi", 0.0), ("ucb", 2.576), ("ucb", -1.0)])
+@pytest.mark.parametrize("kind,kappa", [("ei", 0.0), ("poi", 0.0), ("ucb", 2.576), ("ucb", -1.0), ("logei", 0.0),
+                                        ("logpoi", 0.0)])
 def test_bound_below_sklearn(kname, kind, kappa):
     rs = np.random.RandomState(3)
     n, d, alpha, xi = 120, 4, 1e-6, 0.01
