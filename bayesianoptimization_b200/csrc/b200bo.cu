@@ -173,7 +173,7 @@ struct b200bo_gp {
     // the control words of predict_acq16_kernel's prune mode
     DevBuf prune_key, prune_idx, prune_tmp, prune_ctl;
     // its refine stages: the interval of K* alpha_ per candidate from the bound pass, the survivor list and its keys
-    // (two buffers each for the sort of the final rounds; with levels, the lists of the levels too), the survivors'
+    // (the refine stage's and the level's, the level's slots and the second buffers of their sort), the survivors'
     // carried prefixes, the per-row-block partials, K* alpha_ of the tiles and the arrival counters of
     // predict_units_kernel
     DevBuf prune_mu, prune_surv, prune_surv_key, prune_prefix, prune_part, prune_mu_unit, prune_arrive;
@@ -182,7 +182,7 @@ struct b200bo_gp {
     long long stat_total = 0, stat_direct = 0;
     bool prune_counted = false;
     // stage boundaries of the last pruned launch on its stream: after the bound pass, the sort, the lead, refine and
-    // final stages, and after the refine levels (b200bo_last_prune_stage_ms, b200bo_last_prune_levels; the stages start
+    // final stages, and after the refine level (b200bo_last_prune_stage_ms, b200bo_last_prune_levels; the stages start
     // at ev0 and the tile kernel ends at ev1)
     cudaEvent_t ev_stage[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool stage_timed = false, stage_refined = false;
@@ -322,9 +322,7 @@ static int init_handle(b200bo_gp* gp) {
     CU(gram_reg_attrs<3>());
     CU(cudaFuncSetAttribute(predict_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(predict_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_units_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_units_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
-    CU(cudaFuncSetAttribute(predict_units_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(predict_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(ks_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(ks_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
@@ -1664,32 +1662,7 @@ static int prune_refine_blocks(int np, long long ntiles) {
     return b < nb / 8 ? b : nb / 8;
 }
 
-// A/B switches of the refine stages (DESIGN.md 4.9, 6.1), read per call.  B200BO_PRUNE_ROUNDS=0: no merged k-th key
-// and one final stage over the survivors in arrival order.  B200BO_PRUNE_SHARED_KS=0: every unit builds K* for its
-// rows itself.
-static bool prune_rounds() {
-    const char* e = getenv("B200BO_PRUNE_ROUNDS");
-    return !(e && e[0] == '0');
-}
-static bool prune_shared_ks() {
-    const char* e = getenv("B200BO_PRUNE_SHARED_KS");
-    return !(e && e[0] == '0');
-}
-// B200BO_PRUNE_LEVELS=0: no refine levels; the final stage starts from row block 0 in rounds of 8, 16, 32, the rest.
-static bool prune_levels() {
-    const char* e = getenv("B200BO_PRUNE_LEVELS");
-    return !(e && e[0] == '0');
-}
-
-// Row blocks at which the refine levels end, after the refine stage's b: one level to 2b.  At C3 (DESIGN.md 4.9) the
-// refine stage lets 12.1 tiles through at b = 4, 1.6 at b = 8; a further level cannot shorten the final round,
-// whose latency is that of its last row block.
-static int prune_level_ends(int b, int nb, int* ends) {
-    ends[0] = 2 * b < nb ? 2 * b : nb;
-    return ends[0] < nb ? 1 : 0;
-}
-
-// survivors of the last level in key order (sorted slots pos): their local indices and carried prefixes
+// survivors of the level in key order (sorted slots pos): their local indices and carried prefixes
 __global__ void level_gather_kernel(const unsigned long long* __restrict__ ctl, int n_word, const int* __restrict__ pos,
                                     const int* __restrict__ idx, const double* __restrict__ pre, int* __restrict__ idx_out,
                                     double* __restrict__ pre_out) {
@@ -1711,55 +1684,45 @@ __global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
     ctl[kCtlKthLead] = ctl[kCtlKth];
 }
 
-// Tiles of the final rounds: 8, 16, 32, then the rest of the kRefineMaxTiles, at most `grid` each (a round's K* slots);
-// after refine levels 8, then the rest (at C3 the level leaves 1.6 tiles).  One round over all survivors without rounds.
-static int final_round_tiles(bool rounds, bool levels, int r, int t0, int grid) {
-    const int t = rounds && r < (levels ? 1 : 3) ? 8 << r : kRefineMaxTiles - t0;
+// Tiles of the final rounds: 8, then the rest of the kRefineMaxTiles (at C3 the level leaves 1.6 tiles), at most
+// `grid` each (a round's K* slots)
+static int final_round_tiles(int r, int t0, int grid) {
+    const int t = r == 0 ? 8 : kRefineMaxTiles - t0;
     return t < grid ? t : grid;
 }
 
-// The lead, refine and final stages of a pruned launch (predict16.cuh), between prune_prepare and the tile kernel.
-// With rounds (prune_rounds) merge_kth_kernel tightens the k-th key after the lead stage and after every final round,
-// and the final rounds take the survivors sorted by key, skipping the tiles above the key.  With shared K*
-// (prune_shared_ks) ks_build_kernel builds the K* of a stage's or round's tiles once, before its units.  With levels
-// (prune_levels) the refine stage stores every survivor's prefix, each level carries it on over its row blocks and
-// passes its survivors on, and the final stage starts from the last level's row block.
+// The lead, refine, level and final stages of a pruned launch (predict16.cuh), between prune_prepare and the tile
+// kernel.  ks_build_kernel builds the K* of a stage's or round's tiles once, before its units.  The refine stage
+// stores every survivor's prefix, the level carries it on over row blocks [b, 2b) and passes its survivors on, and
+// the final stage starts from row block 2b in rounds over those survivors sorted by key, skipping the tiles above the
+// key.  merge_kth_kernel tightens the k-th key after the lead stage and after every final round.
 static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg, int blocks, bool resume,
                                cudaStream_t stream) {
     const int nb = P.gp[0].np / PBM, grid = g0->sm_count;
     const int nsurv = kRefineMaxTiles * PBN;
-    const bool rounds = prune_rounds(), shared_ks = prune_shared_ks();
-    int ends[kPruneMaxLevels];
-    const int nlev = prune_levels() ? prune_level_ends(blocks, nb, ends) : 0;
     int rc;
     if ((rc = g0->prune_surv.reserve(sizeof(int) * 4 * (size_t)nsurv))) return rc;
     if ((rc = g0->prune_surv_key.reserve(sizeof(unsigned long long) * 3 * (size_t)nsurv))) return rc;
-    if (nlev && (rc = g0->prune_prefix.reserve(sizeof(double) * 2 * 32 * (size_t)nsurv))) return rc;
+    if ((rc = g0->prune_prefix.reserve(sizeof(double) * 2 * 32 * (size_t)nsurv))) return rc;
     if ((rc = g0->prune_part.reserve(sizeof(double) * (size_t)kUnitSlots * nb * 32 * PBN))) return rc;
     if ((rc = g0->prune_mu_unit.reserve(sizeof(double) * (size_t)kUnitSlots * PBN))) return rc;
     if ((rc = g0->prune_arrive.reserve(sizeof(unsigned) * kUnitSlots))) return rc;
     unsigned long long* skey = g0->prune_surv_key.as<unsigned long long>();
     int* sidx = g0->prune_surv.as<int>();
-    // lists A and B (the refine stage writes A, the levels alternate), the slots of the last level for the sort
+    // lists A (the refine stage's survivors) and B (the level's), the level's slots and the second key and slot buffers
+    // of their sort; the sorted survivors are gathered back into list A
     unsigned long long* lkey[2] = {skey, skey + nsurv};
     int* lidx[2] = {sidx, sidx + nsurv};
     int* spos = sidx + 2 * nsurv;
-    double* lpre[2] = {nullptr, nullptr};
-    if (nlev) {
-        lpre[0] = g0->prune_prefix.as<double>();
-        lpre[1] = lpre[0] + (size_t)32 * nsurv;
-    }
-    cub::DoubleBuffer<unsigned long long> kb(skey, skey + nsurv);
-    cub::DoubleBuffer<int> ib(sidx, sidx + nsurv);
+    double* lpre[2] = {g0->prune_prefix.as<double>(), g0->prune_prefix.as<double>() + (size_t)32 * nsurv};
+    cub::DoubleBuffer<unsigned long long> lk(lkey[1], skey + 2 * nsurv);
+    cub::DoubleBuffer<int> lp(spos, sidx + 3 * nsurv);
     size_t tmp = 0;
-    if (rounds) {
-        CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, kb, ib, nsurv, 0, 64, stream));
-        if ((rc = g0->prune_tmp.reserve(tmp))) return rc;
-    }
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, lk, lp, nsurv, 0, 64, stream));
+    if ((rc = g0->prune_tmp.reserve(tmp))) return rc;
     unsigned long long* ctl = g0->prune_ctl.as<unsigned long long>();
     if (!resume) CU(cudaMemsetAsync(ctl + kCtlRefined, 0, sizeof(unsigned long long), stream));
     CU(cudaMemsetAsync(g0->prune_arrive.p, 0, sizeof(unsigned) * kUnitSlots, stream));
-    if (rounds && !nlev) CU(cudaMemsetAsync(skey, 0xFF, sizeof(unsigned long long) * nsurv, stream));  // unused slots sort last
     prune_ctl_refine_kernel<<<1, 1, 0, stream>>>(ctl);
     LAUNCHED();
     RefineParams R = {};
@@ -1778,22 +1741,14 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     R.n_word = kCtlSurv;
     R.t0 = 0;
     R.t1 = kRefineMaxTiles;
-    R.round_skip = 0;
-    // with shared K* the units run no phase A, so the candidates' coordinates never sit in registers
-    auto units = shared_ks ? predict_units_kernel<false, true>
-                           : (dreg ? predict_units_kernel<true, false> : predict_units_kernel<false, false>);
     auto build = dreg ? ks_build_kernel<true> : ks_build_kernel<false>;
     const SelList* lists = g0->sel_cta.as<SelList>();
-    if (shared_ks) {
-        build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
-        LAUNCHED();
-    }
-    units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
+    build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
     LAUNCHED();
-    if (rounds) {
-        merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
-        LAUNCHED();
-    }
+    predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(P, R);
+    LAUNCHED();
+    merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
+    LAUNCHED();
     CU(cudaEventRecord(g0->ev_stage[2], stream));
     PredictParams Q = P;  // the lead stage has begun the per-CTA lists
     Q.sel_resume = 1;
@@ -1804,80 +1759,54 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
         predict_refine_kernel<false><<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
     LAUNCHED();
     CU(cudaEventRecord(g0->ev_stage[3], stream));
-    // levels: the survivors of list `in`, counted in word n_word, over row blocks [b0, ends[l]) into the other list
-    int in = 0;
+    // The level: the survivors of list A, counted in kCtlSurv, over row blocks [b, 2b) into list B.  It always exists:
+    // prune_refine_blocks clamps b to nb / 8 with nb >= 8, so 2b <= nb / 4 < nb.  One level is enough: at C3 (DESIGN.md
+    // 4.9) it leaves 1.6 tiles of the refine stage's 12.1, and a further level cannot shorten the final round, whose
+    // latency is that of its last row block.
     R.final_stage = kStageLevel;
-    R.b1 = blocks;
-    for (int l = 0; l < nlev; ++l) {
-        const int out = 1 - in;
-        R.b0 = R.b1;
-        R.b1 = ends[l];
-        R.surv = lidx[in];
-        R.surv_key = lkey[in];
-        R.prefix = lpre[in];
-        R.surv_out = lidx[out];
-        R.surv_key_out = lkey[out];
-        R.prefix_out = lpre[out];
-        R.pos_out = spos;
-        R.out_word = kCtlLevel + l;
-        if (rounds && l == nlev - 1)  // unused slots sort last
-            CU(cudaMemsetAsync(lkey[out], 0xFF, sizeof(unsigned long long) * nsurv, stream));
-        for (int t0 = 0; t0 < kRefineMaxTiles; t0 = R.t1) {
-            R.t0 = t0;
-            R.t1 = t0 + grid < kRefineMaxTiles ? t0 + grid : kRefineMaxTiles;
-            CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
-            if (shared_ks) {
-                build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-                LAUNCHED();
-            }
-            units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-            LAUNCHED();
-        }
-        R.n_word = R.out_word;
-        in = out;
+    R.b0 = blocks;
+    R.b1 = 2 * blocks;
+    R.surv_out = lidx[1];
+    R.surv_key_out = lkey[1];
+    R.prefix_out = lpre[1];
+    R.pos_out = spos;
+    R.out_word = kCtlLevel;
+    CU(cudaMemsetAsync(lkey[1], 0xFF, sizeof(unsigned long long) * nsurv, stream));  // unused slots sort last
+    for (int t0 = 0; t0 < kRefineMaxTiles; t0 = R.t1) {
+        R.t0 = t0;
+        R.t1 = t0 + grid < kRefineMaxTiles ? t0 + grid : kRefineMaxTiles;
+        CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+        build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+        LAUNCHED();
+        predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+        LAUNCHED();
     }
-    g0->stage_levels = nlev;
+    g0->stage_levels = 1;
     CU(cudaEventRecord(g0->ev_stage[5], stream));
+    // the level's survivors ascending by key (the sentinels of the unused slots last), sorted with their slots, then
+    // their indices and prefixes gathered into list A in that order
+    CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, lk, lp, nsurv, 0, 64, stream));
+    LAUNCHED();
+    level_gather_kernel<<<2 * grid, 256, 0, stream>>>(ctl, kCtlLevel, lp.Current(), lidx[1], lpre[1], lidx[0],
+                                                       lpre[0]);
+    LAUNCHED();
     R.final_stage = kStageFinal;
-    R.b0 = nlev ? R.b1 : 0;
+    R.b0 = 2 * blocks;
     R.b1 = nb;
-    R.round_skip = rounds;
-    R.surv = lidx[in];
-    R.surv_key = lkey[in];
-    R.prefix = lpre[in];
-    if (rounds) {  // survivors ascending by key; the sentinels of the unused slots last
-        if (nlev) {  // sorted with their slots, then their indices and prefixes gathered into the other list
-            cub::DoubleBuffer<unsigned long long> lk(lkey[in], skey + 2 * nsurv);
-            cub::DoubleBuffer<int> lp(spos, sidx + 3 * nsurv);
-            CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, lk, lp, nsurv, 0, 64, stream));
-            LAUNCHED();
-            level_gather_kernel<<<2 * grid, 256, 0, stream>>>(ctl, R.n_word, lp.Current(), lidx[in], lpre[in],
-                                                               lidx[1 - in], lpre[1 - in]);
-            LAUNCHED();
-            R.surv = lidx[1 - in];
-            R.surv_key = lk.Current();
-            R.prefix = lpre[1 - in];
-        } else {
-            CU(cub::DeviceRadixSort::SortPairs(g0->prune_tmp.p, tmp, kb, ib, nsurv, 0, 64, stream));
-            LAUNCHED();
-            R.surv = ib.Current();
-            R.surv_key = kb.Current();
-        }
-    }
+    R.n_word = kCtlLevel;
+    R.surv = lidx[0];
+    R.surv_key = lk.Current();
+    R.prefix = lpre[0];
     for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r) {
         R.t0 = t0;
-        R.t1 = t0 + final_round_tiles(rounds, nlev > 0, r, t0, grid);
-        if (r > 0 || nlev) CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
-        if (shared_ks) {
-            build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-            LAUNCHED();
-        }
-        units<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+        R.t1 = t0 + final_round_tiles(r, t0, grid);
+        CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+        build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
         LAUNCHED();
-        if (rounds) {
-            merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
-            LAUNCHED();
-        }
+        predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+        LAUNCHED();
+        merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
+        LAUNCHED();
         t0 = R.t1;
     }
     CU(cudaGetLastError());

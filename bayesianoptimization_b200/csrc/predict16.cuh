@@ -1242,16 +1242,18 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
 // k-th key, and another for whatever the single-point bound leaves.  The refine stages replace both:
 //   lead    the first kLeadTiles tiles in bound order, evaluated exactly by predict_units_kernel, which splits the row
 //           blocks of every tile across CTAs, so the k-th key exists after a fraction of a tile latency;
+//           merge_kth_kernel then sets the k-th key from the union of the per-CTA lists;
 //   refine  predict_refine_kernel: for the following tiles in bound order (same stop rule as prune_claim) the product
 //           with the leading b row blocks of L^-1 only.  r_b = sum of V_i^2 over those rows is k*^T K^-1 k* of the GP
 //           conditioned on the first b * PBM training points alone, and the remaining terms are squares, so
 //           r_b <= k*^T K^-1 k* and prune_var_ub(r_b) bounds the variance as the single-point r does.  Candidates whose
 //           refined key and single-point key are both <= the k-th key are appended to the survivor list, with the
 //           running sums of their first b row blocks (the prefix);
-//   levels  predict_units_kernel over row blocks [b_l, b_l+1) of the survivors only: the last unit of a tile carries
-//           each survivor's prefix on to b_l+1, keys it as the refine stage does and appends the survivors whose
-//           keys are all <= the k-th key, with the new prefix, to the next level's list;
-//   final   the survivors through predict_units_kernel, from the carried prefix on.
+//   level   predict_units_kernel over row blocks [b, 2b) of the survivors only: the last unit of a tile carries each
+//           survivor's prefix on to 2b, keys it as the refine stage does and appends the survivors whose keys are all
+//           <= the k-th key, with the new prefix, to the level's list;
+//   final   the level's survivors sorted by key through predict_units_kernel, from the carried prefix on, in rounds
+//           that each skip the tiles above the k-th key merged before them.
 // When more than kRefineMaxTiles tiles of survivors come up (little prunes: the refine stage stops claiming tiles as
 // soon as it sees that), the final stage does nothing and the tile kernel goes on in bound order behind the lead
 // tiles as it would have without these stages; otherwise the final stage closes the tile kernel's counter.
@@ -1270,7 +1272,7 @@ struct RefineParams {
     int* surv;               // [kRefineMaxTiles * PBN] local indices the refine stage let through (final: sorted)
     unsigned long long* surv_key;  // [kRefineMaxTiles * PBN] their keys (max of single-point and refined key)
     // [kRefineMaxTiles * PBN][32] per survivor, the running sums over row blocks [0, b0) per (row slab wm, lane group
-    // g), index wm * 8 + g, before the xor tree; nullptr: none (the lead, and every stage without levels)
+    // g), index wm * 8 + g, before the xor tree; nullptr in the lead stage (b0 = 0)
     double* prefix;
     int* surv_out;           // a level: the survivors it lets through, their keys, prefixes and slots (the values of
     unsigned long long* surv_key_out;  // the final sort)
@@ -1282,15 +1284,14 @@ struct RefineParams {
     int groups_max;          // most units a tile is split into
     int final_stage;         // predict_units_kernel: kStageLead, kStageFinal or kStageLevel
     int b0, b1;              // the units' row blocks [b0, b1): the lead and the final stage end at np / PBM
-    int n_word;              // final stage and levels: the prune_ctl word counting their candidates
-    int out_word;            // a level: the prune_ctl word counting the candidates it lets through
-    int t0, t1;              // final stage and levels: the round's tiles [t0, t1) of the survivor list
-    int round_skip;          // final stage: skip a tile whose first key is above kCtlKthRound
+    int n_word;              // final stage and level: the prune_ctl word counting their candidates
+    int out_word;            // the level: the prune_ctl word counting the candidates it lets through
+    int t0, t1;              // final stage and level: the round's tiles [t0, t1) of the survivor list
 };
 
-// The tiles of a lead stage, level or final round, the same in every CTA: candidates list[0, n), tiles [tbeg, tend)
-// of PBN columns, partial-sum slots from slot0.  Levels and final stage: too many refine survivors leave n = 0 (the
-// tile kernel takes over in bound order); otherwise the final stage closes the tile kernel's counter.
+// The tiles of a lead stage, level launch or final round, the same in every CTA: candidates list[0, n), tiles
+// [tbeg, tend) of PBN columns, partial-sum slots from slot0.  Level and final stage: too many refine survivors leave
+// n = 0 (the tile kernel takes over in bound order); otherwise the final stage closes the tile kernel's counter.
 struct UnitRound {
     const int* list;
     long long n, tbeg, tend;
@@ -1321,8 +1322,8 @@ __device__ __forceinline__ UnitRound unit_round(const PredictParams& P, const Re
 // whether every unit of tile `tile` skips it: its best bound key is above the k-th key copied before the stage / round
 __device__ __forceinline__ bool unit_skip(const PredictParams& P, const RefineParams& R, long long tile) {
     if (R.final_stage == kStageLead) return P.perm_key[tile * PBN] > P.prune_ctl[kCtlKthLead];
-    if (R.final_stage == kStageLevel) return false;  // no exact value moves the k-th key between levels
-    return R.round_skip && R.surv_key[tile * PBN] > P.prune_ctl[kCtlKthRound];
+    if (R.final_stage == kStageLevel) return false;  // no exact value moves the k-th key during the level
+    return R.surv_key[tile * PBN] > P.prune_ctl[kCtlKthRound];
 }
 
 // The k-th smallest key over the union of the per-CTA lists (sel_cta, lists carried in by a continued batch included)
@@ -1429,7 +1430,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
         if (tile >= ntiles) break;
         const long long c0 = tile * PBN;
         phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, P.perm, P.m, R.blocks * PBM);
-        double* pre = R.prefix ? smem + 4 * PBN : nullptr;  // [32][PBN] behind red
+        double* pre = smem + 4 * PBN;  // [32][PBN] behind red
         predict16_phase_b<1684, false>(G, Ks, smem, pol_last, pol_first, 0, R.blocks, nullptr, pre);
         const double* red = smem;
         if (tid < PBN && c0 + tid < P.m) {
@@ -1443,10 +1444,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
                 if (pos < (unsigned long long)kRefineMaxTiles * PBN) {
                     R.surv[pos] = li;
                     R.surv_key[pos] = key > key1 ? key : key1;  // both are lower bounds
-                    if (pre) {
 #pragma unroll 4
-                        for (int q = 0; q < 32; ++q) R.prefix[pos * 32 + q] = pre[q * PBN + c];
-                    }
+                    for (int q = 0; q < 32; ++q) R.prefix[pos * 32 + q] = pre[q * PBN + c];
                 }
             }
         }
@@ -1494,13 +1493,11 @@ __device__ __forceinline__ void unit_mu_from_ks(const GpDev& G, const double* __
 // Exact evaluation in units of (tile, group of consecutive row blocks of [b0, b1)).  Lead stage: the tiles are the
 // first kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this launch (a
 // continued batch; read from kCtlKthLead, which does not move, so that all units of a tile decide alike).  Final
-// stage: the tiles [t0, t1) of the survivor list, with round_skip each skipped when its first key is above
-// kCtlKthRound.  A level: the tiles [t0, t1) of its survivor list, none skipped.  A unit builds K* for the rows its
-// row blocks need in its CTA's scratch (SHARED_KS: reads the tile's slot that ks_build_kernel filled, and the unit of
-// the last group computes mu from it), runs phase B over its row blocks, and the last unit to arrive finishes the
-// tile: from the survivors' carried prefix on, as the tile kernel's epilogue does (lead, final), or as the refine
-// stage keys its candidates at b1 row blocks (a level).
-template <bool DREG, bool SHARED_KS>
+// stage: the tiles [t0, t1) of the survivor list, each skipped when its first key is above kCtlKthRound.  The level:
+// the tiles [t0, t1) of its survivor list, none skipped.  A unit reads the tile's K* from the slot that
+// ks_build_kernel filled (the unit of the last group computes mu from it), runs phase B over its row blocks, and the
+// last unit to arrive finishes the tile: from the survivors' carried prefix on, as the tile kernel's epilogue does
+// (lead, final), or as the refine stage keys its candidates at b1 row blocks (the level).
 __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictParams P, const RefineParams R) {
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
@@ -1510,7 +1507,7 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
     const int tid = threadIdx.x;
     const GpDev& G = P.gp[0];
     const int nb = G.np / PBM;
-    const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last), pol_first = l2_policy_evict_first();
+    const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last);
     if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
     __syncthreads();
     const UnitRound U = unit_round(P, R);
@@ -1537,15 +1534,9 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
         const int slot = U.slot0 + (int)tile;
         double* part = R.part + (size_t)slot * nb * 32 * PBN;
         if (ib1 > ib0) {
-            if constexpr (SHARED_KS) {
-                const double* Ks = P.scratch + (tile - U.tbeg) * P.scratch_stride;
-                if (ib1 == nb) unit_mu_from_ks(G, Ks, mu_s);
-                predict16_phase_b<1684, true>(G, Ks, smem, pol_last, l2_policy_evict_last(0.f), ib0, ib1, part);
-            } else {
-                double* Ks = P.scratch + (long long)blockIdx.x * P.scratch_stride;
-                phase_a<P16_NT, DREG, KS_F64_EF>(P, G, c0, Ks, smem, mu_s, pol_first, nullptr, list, n, ib1 * PBM);
-                predict16_phase_b<1684, true>(G, Ks, smem, pol_last, pol_first, ib0, ib1, part);
-            }
+            const double* Ks = P.scratch + (tile - U.tbeg) * P.scratch_stride;
+            if (ib1 == nb) unit_mu_from_ks(G, Ks, mu_s);
+            predict16_phase_b<1684, true>(G, Ks, smem, pol_last, l2_policy_evict_last(0.f), ib0, ib1, part);
             if (ib1 == nb && tid < PBN)  // mu_s holds the tile kernel's K* alpha_ parts (phase A over all np rows)
                 R.mu_unit[(size_t)slot * PBN + tid] = ((mu_s[0][tid] + mu_s[1][tid]) + mu_s[2][tid]) + mu_s[3][tid];
         }

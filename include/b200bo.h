@@ -528,10 +528,10 @@ int b200bo_last_prune_stats(int64_t* evaluated, int64_t* total);
 int b200bo_last_prune_stage_ms(float ms[6], int64_t* refined);
 
 /* The refine levels of the most recent pruned launch on this thread (DESIGN.md 4.9): *ms = their time (part of
- * ms[3] of b200bo_last_prune_stage_ms), *levels = how many ran (0 with B200BO_PRUNE_LEVELS=0 or without refine
- * stages), passed[0] = candidates the refine stage let through (more than 16384: the tile kernel took over and no
- * level ran), passed[1 + l] = those level l let through; passed has room for 5.  B200BO_ERR_STATE when the launch was
- * not pruned.  Synchronises on the stop event. */
+ * ms[3] of b200bo_last_prune_stage_ms), *levels = how many ran (1 whenever the refine stages ran, else 0),
+ * passed[0] = candidates the refine stage let through (more than 16384: the tile kernel took over and the level
+ * evaluated nothing), passed[1 + l] = those level l let through; passed has room for 5.  B200BO_ERR_STATE when the
+ * launch was not pruned.  Synchronises on the stop event. */
 int b200bo_last_prune_levels(float* ms, int64_t passed[5], int* levels);
 
 /* The direct bound pass of selection-only pruning alone (the one the selection runs for Matern-0.5; EI, UCB, PoI,

@@ -1,11 +1,12 @@
-"""The refine levels of pruning (B200BO_PRUNE_LEVELS, DESIGN.md 4.9): the refine stage's survivors carry their running
-sums of squares into a level over the next row blocks, which keys them again, and into the final stage.
+"""The refine level of pruning (DESIGN.md 4.9): the refine stage's survivors carry their running sums of squares into
+a level over the next row blocks, which keys them again, and into the final stage.
 
-The records (value bits and indices) must equal those without levels, with the rounds and the shared K* on and off,
-and those of the unpruned call: at the C3 shape, on the ill-conditioned production-size fixtures, for a streamed
-(continued) host batch, for the Philox source and at N = 1024 (one leading row block, a level to two).  Repeat calls are
-bit-identical, and where the refine stage lets candidates through but the level lets none (illbig_b_m25_c3, EI), the
-final stage evaluates nothing and the records still hold.
+The records (value bits and indices) must equal those of the unpruned call: at the C3 shape, on the ill-conditioned
+production-size fixtures, for a streamed (continued) host batch, for the Philox source and at N = 1024 (one leading row
+block, a level to two).  At C3 the level lets fewer candidates through than the refine stage, and no candidate goes
+through the full N^2 term but the lead tiles' and the level's survivors.  Repeat calls are bit-identical, and where the
+refine stage lets candidates through but the level lets none (illbig_b_m25_c3, EI), the final stage evaluates nothing
+and the records still hold.
 """
 import ctypes as C
 
@@ -18,9 +19,8 @@ from oracle import make_illcond_big as MB
 
 pytestmark = pytest.mark.gpu
 
-# (B200BO_PRUNE, B200BO_PRUNE_LEVELS, B200BO_PRUNE_ROUNDS, B200BO_PRUNE_SHARED_KS)
-SETTINGS = (("0", "1", "1", "1"), ("1", "0", "1", "1"), ("1", "1", "1", "1"), ("1", "1", "0", "1"),
-            ("1", "1", "1", "0"), ("1", "1", "0", "0"), ("1", "0", "0", "0"))
+SETTINGS = ("0", "1")  # B200BO_PRUNE
+LEAD_TILES, PBN = 8, 128  # kLeadTiles, candidates per tile
 
 
 @pytest.fixture(scope="module")
@@ -53,11 +53,8 @@ def _all(monkeypatch, fn):
     from bayesianoptimization_b200 import _lib as B
 
     out, stats = [], []
-    for prune, levels, rounds, shared in SETTINGS:
+    for prune in SETTINGS:
         monkeypatch.setenv("B200BO_PRUNE", prune)
-        monkeypatch.setenv("B200BO_PRUNE_LEVELS", levels)
-        monkeypatch.setenv("B200BO_PRUNE_ROUNDS", rounds)
-        monkeypatch.setenv("B200BO_PRUNE_SHARED_KS", shared)
         out.append(fn())
         ev, tot = C.c_int64(), C.c_int64()
         B.check(B.lib().b200bo_last_prune_stats(C.byref(ev), C.byref(tot)))
@@ -98,7 +95,7 @@ def _c3(bo):
     return bo.FusedAcquisition(B.ACQ_EI, gp, xi=0.01, y_max=float(y.max()))
 
 
-def test_c3_levels_equal_and_fewer_evaluated(bo, monkeypatch):
+def test_c3_one_level_and_evaluated_bound(bo, monkeypatch):
     import torch
 
     acq = _c3(bo)
@@ -106,14 +103,12 @@ def test_c3_levels_equal_and_fewer_evaluated(bo, monkeypatch):
     out, stats = _all(monkeypatch, lambda: _dev(acq, xd, 10))
     print(f"\nc3 (evaluated, levels, passed) per setting: {stats}")
     assert _equal(out)
-    assert stats[1][1] == 0 and stats[2][1] == 1, stats  # LEVELS=0 / 1
-    passed = stats[2][2]
-    assert 0 < passed[1] < passed[0] <= 128 * 128, stats
-    assert stats[2][0] < stats[1][0], stats  # fewer candidates through the full N^2 term
+    ev, nlev, passed = stats[1]
+    assert nlev == 1 and 0 < passed[1] < passed[0] <= 128 * 128, stats
+    # the lead tiles and the final rounds over the level's survivors; the tile kernel evaluates nothing
+    assert ev <= LEAD_TILES * PBN + passed[1], stats
     # repeat calls: bit-identical records
     monkeypatch.setenv("B200BO_PRUNE", "1")
-    for v in ("B200BO_PRUNE_LEVELS", "B200BO_PRUNE_ROUNDS", "B200BO_PRUNE_SHARED_KS"):
-        monkeypatch.delenv(v, raising=False)
     for _ in range(3):
         assert np.array_equal(_dev(acq, xd, 10), out[0])
 
@@ -144,7 +139,7 @@ def test_c3_philox(bo, monkeypatch):
 
     out, stats = _all(monkeypatch, run)
     assert _equal(out)
-    assert stats[2][1] == 1 and stats[2][2][1] < stats[2][2][0], stats
+    assert stats[1][1] == 1 and stats[1][2][1] < stats[1][2][0], stats
 
 
 @pytest.mark.parametrize("kind", ("ucb", "ei"))
@@ -165,7 +160,7 @@ def test_illcond_big(bo, monkeypatch, name, kind):
     print(f"\n{name} {kind}: {stats}")
     assert _equal(out), (name, kind)
     if (name, kind) == ("b_m25_c3", "ei"):  # nothing survives the level: only the lead tiles are evaluated
-        ev, nlev, passed = stats[2]
+        ev, nlev, passed = stats[1]
         assert nlev == 1 and passed[0] > 0 and passed[1] == 0 and ev == 1024, stats
 
 
@@ -185,4 +180,4 @@ def test_n1024(bo, monkeypatch):
     out, stats = _all(monkeypatch, lambda: _dev(acq, xd, 10))
     print(f"\nn1024: {stats}")
     assert _equal(out)
-    assert stats[2][1] == 1 and 0 < stats[2][2][1] <= stats[2][2][0], stats
+    assert stats[1][1] == 1 and 0 < stats[1][2][1] <= stats[1][2][0], stats

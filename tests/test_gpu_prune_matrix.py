@@ -6,7 +6,7 @@ a 1e6 target offset with y_std 5e-4; ConstantKernel 2^-13 and 2^13 with a WhiteK
 every kind (UCB, EI, PoI, LogEI, LogPoI) and every parameter point of the fixture (kappa -1, 0, 2.576, 100; y_max below
 every mu, max y, max y + 4 s_y, each with xi 0, 0.01, 10 s_y):
   1. the records (argmin and top-k: value bits and indices) of every switch combination of SETTINGS (every pair of
-     values of the seven B200BO_PRUNE_* switches, and the defaults) equal those with B200BO_PRUNE=0, at k = 1 and
+     values of the four B200BO_PRUNE_* switches, and the defaults) equal those with B200BO_PRUNE=0, at k = 1 and
      k = 64 (B200BO_MAX_TOPK), on host candidates, on device candidates and on eight copies of the candidates (35 tiles,
      where the lead, refine, level and final stages run).  Each problem must have calls where the refine stage
      evaluated candidates and where the level let some through;
@@ -35,10 +35,14 @@ from test_prune_cpu import VAR_EPS
 
 pytestmark = pytest.mark.gpu
 
-SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_REFINE_BLOCKS", "B200BO_PRUNE_ROUNDS", "B200BO_PRUNE_SHARED_KS",
-            "B200BO_PRUNE_LEVELS", "B200BO_PRUNE_BOUND", "B200BO_PRUNE_GRAM_KERNEL")
-VALUES = (("1", "0"), ("4", "1", "64"), ("1", "0"), ("1", "0"), ("1", "0"), ("auto", "f64", "f32"), ("reg", "ring"))
+SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_REFINE_BLOCKS", "B200BO_PRUNE_BOUND", "B200BO_PRUNE_GRAM_KERNEL")
+VALUES = (("1", "0"), ("4", "1", "64"), ("auto", "f64", "f32"), ("reg", "ring"))
 DEFAULTS = tuple(v[0] for v in VALUES)
+
+
+def switch(setting, name):
+    """the value of switch B200BO_PRUNE_<name> in a setting"""
+    return setting[SWITCHES.index("B200BO_PRUNE_" + name)]
 
 
 def pairwise(values):
@@ -185,7 +189,7 @@ def _sources(r):
 
 
 @pytest.mark.parametrize("name", PM.PROBLEMS)
-def test_records_every_switch_pair(bo, monkeypatch, name):
+def test_records_every_switch_pair_one_level(bo, monkeypatch, name):
     r = fixture(name)
     gp = _gp(bo, name)
     src = _sources(r)
@@ -196,10 +200,10 @@ def test_records_every_switch_pair(bo, monkeypatch, name):
             stats = _records_equal(monkeypatch, _acq(bo, gp, kind, p), src, SETTINGS)
             for st, (ev, tot, ref, nlev, passed) in stats["x8"]:
                 assert ev <= tot == 8 * len(r["xt"])
-                if st[0] == "1":
+                if switch(st, "REFINE") == "1":
                     staged += 1
                     refined += ref > 0
-                    assert nlev == (1 if st[4] == "1" else 0), (kind, j, st, nlev)
+                    assert nlev == 1, (kind, j, st, nlev)
                     level_passed += nlev == 1 and len(passed) == 2 and passed[1] > 0
     print(f"\n{name}: {len(SETTINGS)} settings; of {staged} staged x8 calls the refine stage evaluated in {refined}, "
           f"the level let candidates through in {level_passed} ({time.perf_counter() - t0:.1f} s)")
@@ -351,7 +355,7 @@ def test_conditioned_and_forked_handles(bo, monkeypatch, name):
         for kind in PM.KINDS:
             for p in _points(r, kind)[::2]:
                 stats = _records_equal(monkeypatch, _acq(bo, g, kind, p), src, SINGLE)
-                pruned += sum(s[0] == "1" and ev < tot for s, (ev, tot, *_) in stats["x8"])
+                pruned += sum(switch(s, "REFINE") == "1" and ev < tot for s, (ev, tot, *_) in stats["x8"])
         assert pruned > 0, p_rows
 
 

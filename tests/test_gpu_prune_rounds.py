@@ -1,11 +1,10 @@
-"""The merged k-th key, the final rounds and the shared K* of pruning's refine stages (B200BO_PRUNE_ROUNDS,
-B200BO_PRUNE_SHARED_KS, DESIGN.md 4.9).
+"""The merged k-th key, the final rounds and the shared K* of pruning's refine stages (DESIGN.md 4.9).
 
-The records (value bits and indices) must equal those of the unpruned call and of the stages without either switch,
-with each switch alone and with both: for EI, UCB, PoI and LogEI, k = 1 / 10 / 64, every covariance code with and
-without candidate registers, ragged batch and training sizes, streamed host batches, the Philox source, a batch split
-into launches of kPruneMaxBatch, a batch with a NaN value and UCB with kappa = 100 (the tile kernel takes over).  At the
-C3 shape the rounds must send strictly fewer candidates through the full N^2 term than the stages without them.
+The records (value bits and indices) must equal those of the unpruned call: for EI, UCB, PoI and LogEI, k = 1 / 10 /
+64, every covariance code with and without candidate registers, ragged batch and training sizes, streamed host batches,
+the Philox source, a batch split into launches of kPruneMaxBatch, a batch with a NaN value and UCB with kappa = 100
+(the tile kernel takes over).  At the C3 shape the refine stage runs, and no candidate goes through the full N^2 term
+but the lead tiles' and the level's survivors: the final stage closes the tile kernel's counter.
 """
 import ctypes as C
 
@@ -17,8 +16,8 @@ import kernel_matrix_cases as KM
 
 pytestmark = pytest.mark.gpu
 
-# (B200BO_PRUNE, B200BO_PRUNE_ROUNDS, B200BO_PRUNE_SHARED_KS); the second is the stages without the switches
-SETTINGS = (("0", "1", "1"), ("1", "0", "0"), ("1", "1", "0"), ("1", "0", "1"), ("1", "1", "1"))
+SETTINGS = ("0", "1")  # B200BO_PRUNE
+LEAD_TILES, PBN = 8, 128  # kLeadTiles, candidates per tile
 
 
 @pytest.fixture(scope="module")
@@ -48,10 +47,8 @@ def _all(monkeypatch, fn):
     from bayesianoptimization_b200 import _lib as B
 
     out, stats = [], []
-    for prune, rounds, shared in SETTINGS:
+    for prune in SETTINGS:
         monkeypatch.setenv("B200BO_PRUNE", prune)
-        monkeypatch.setenv("B200BO_PRUNE_ROUNDS", rounds)
-        monkeypatch.setenv("B200BO_PRUNE_SHARED_KS", shared)
         out.append(fn())
         ev, tot, ref = C.c_int64(), C.c_int64(), C.c_int64()
         B.check(B.lib().b200bo_last_prune_stats(C.byref(ev), C.byref(tot)))
@@ -109,19 +106,25 @@ def _gp(bo, X, y, kernel):
     return bo.B200GaussianProcessRegressor(kernel=kernel, alpha=1e-6, normalize_y=True, optimizer=None).fit(X, y)
 
 
-def test_c3_shape_fewer_evaluated(bo, monkeypatch):
+def test_c3_shape_evaluates_lead_and_level_survivors(bo, monkeypatch):
     import torch
+
+    from bayesianoptimization_b200 import _lib as B
 
     X, y = _problem(4096, 16, 0)
     gp = _gp(bo, X, y, Matern(nu=2.5, length_scale=0.7))
     acq = _acq(bo, gp, "ei", y)
     xd = torch.from_numpy(np.random.RandomState(1000).uniform(size=(1 << 20, 16))).cuda()
     out, stats = _all(monkeypatch, lambda: _dev(acq, xd, 10))
+    ms, passed, nlev = C.c_float(), (C.c_int64 * 5)(), C.c_int()
+    B.check(B.lib().b200bo_last_prune_levels(C.byref(ms), passed, C.byref(nlev)))
     assert _equal(out)
-    assert all(s[1] > 0 for s in stats[1:]), stats  # the stages ran
-    assert stats[2][0] < stats[1][0] and stats[4][0] < stats[1][0], stats
-    print(f"c3: evaluated old {stats[1][0]}, rounds {stats[2][0]}, both {stats[4][0]}; "
-          f"refined {stats[1][1]} -> {stats[4][1]}")
+    evaluated, refined = stats[1]
+    assert refined > 0, stats  # the stages ran
+    assert nlev.value == 1 and 0 < passed[1] < passed[0], (nlev.value, list(passed))
+    # the lead tiles and the final rounds over the level's survivors; the tile kernel evaluates nothing
+    assert evaluated <= LEAD_TILES * PBN + passed[1], (stats, list(passed))
+    print(f"c3: evaluated {evaluated}, refined {refined}, passed {list(passed)[:2]}")
 
 
 @pytest.mark.parametrize("kind", ("ei", "ucb", "poi", "logei"))

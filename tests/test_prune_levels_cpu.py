@@ -7,9 +7,9 @@ on to the last row block.  Here:
       running sum per level, added afterwards, does not;
   (b) every level's key is a lower bound of the exact closure value, on the well- and ill-conditioned sets of
       tests/test_prune_refine_cpu.py;
-  (c) the schedule: unit_cut with a start block tiles [b0, nb) with balanced k-tile counts, the level ends at 2b, and
-      the final rounds (8, then the rest after a level; 8, 16, 32, the rest without) cover the survivor tiles, at most
-      one tile per SM each (the rounds' stop rule is tests/test_prune_rounds_cpu.py's).
+  (c) the schedule: unit_cut with a start block tiles [b0, nb) with balanced k-tile counts, the one level ends at 2b,
+      and the final rounds (8, then the rest) cover the survivor tiles, at most one tile per SM each (the rounds'
+      stop rule is tests/test_prune_rounds_cpu.py's).
 """
 import numpy as np
 import pytest
@@ -34,15 +34,19 @@ def unit_cut(b0, nb, groups, j):
     return ib
 
 
+def refine_blocks(nb, blocks=4):
+    """prune_refine_blocks of b200bo.cu: B200BO_PRUNE_REFINE_BLOCKS (default 4), at least 1, clamped to nb / 8"""
+    return min(max(blocks, 1), nb // 8)
+
+
 def level_ends(b, nb):
-    """prune_level_ends of b200bo.cu: one level, to 2b (none when that reaches nb)"""
-    e = min(2 * b, nb)
-    return [e] if e < nb else []
+    """the level of prune_refine_stages in b200bo.cu: one, to 2b"""
+    return [2 * b]
 
 
-def final_round_tiles(rounds, levels, r, t0, grid):
-    t = 8 << r if rounds and r < (1 if levels else 3) else K_REFINE_MAX_TILES - t0
-    return min(t, grid)
+def final_round_tiles(r, t0, grid):
+    """final_round_tiles of b200bo.cu: 8, then the rest, at most grid each"""
+    return min(8 if r == 0 else K_REFINE_MAX_TILES - t0, grid)
 
 
 def carried(s, cuts):
@@ -108,7 +112,7 @@ def test_cuts_with_start_block(nb, groups):
         cost = [sum(ib + 1 for ib in range(a, b)) for a, b in zip(cuts, cuts[1:])]
         # no group exceeds the mean by more than one row block's k-tiles
         assert max(cost) <= sum(cost) / groups + nb, (b0, cost)
-    # b0 = 0 is the cut of the lead and of the final stage without levels
+    # b0 = 0 is the cut of the lead stage
     for j in range(groups + 1):
         total = nb * (nb + 1) // 2
         ib = 0
@@ -119,24 +123,26 @@ def test_cuts_with_start_block(nb, groups):
 
 @pytest.mark.parametrize("nb", [8, 16, 32, 64, 128])
 def test_level_schedule(nb):
-    b = min(4, nb // 8)  # prune_refine_blocks' default, clamped to an eighth of the row blocks
-    ends = level_ends(b, nb)
-    assert ends == [2 * b] and b < ends[0] < nb
+    # the default and the B200BO_PRUNE_REFINE_BLOCKS values of tests/test_gpu_prune_matrix.py, clamped
+    for blocks in (4, 1, 64):
+        b = refine_blocks(nb, blocks)
+        ends = level_ends(b, nb)
+        assert ends == [2 * b] and b < ends[0] < nb, (blocks, b, ends)
 
 
-@pytest.mark.parametrize("levels", [False, True])
-@pytest.mark.parametrize("rounds", [False, True])
-@pytest.mark.parametrize("grid", [132, 114, 64])
-def test_round_schedule(levels, rounds, grid):
+# SM counts: below, at and around the first round of 8 and the 120 tiles after it, the H100 PCIe (114) and SXM (132)
+@pytest.mark.parametrize("grid", [1, 7, 8, 9, 64, 114, 119, 120, 121, 127, 128, 132])
+def test_round_schedule(grid):
     t0, sizes = 0, []
     while t0 < K_REFINE_MAX_TILES:
-        t = final_round_tiles(rounds, levels, len(sizes), t0, grid)
+        t = final_round_tiles(len(sizes), t0, grid)
         assert 0 < t <= grid
         sizes.append(t)
         t0 += t
     assert t0 == K_REFINE_MAX_TILES
-    if rounds and grid >= K_REFINE_MAX_TILES:
-        assert sizes == ([8, 120] if levels else [8, 16, 32, 72])
-    if not rounds:
-        assert sizes[0] == min(grid, K_REFINE_MAX_TILES)
+    assert sizes[0] == min(8, grid)
+    if grid >= K_REFINE_MAX_TILES - 8:
+        assert sizes == [8, 120]
+    else:
+        assert sizes[1:-1] == [grid] * (len(sizes) - 2) and 0 < sizes[-1] <= grid
 

@@ -3,10 +3,10 @@ numpy.
 
   (a) merge_kth_kernel: the k-th smallest value over the union of the per-CTA lists is >= the final k-th value (it is
       the k-th of values already produced) and <= the least k-th value of any single list (the key before it);
-  (b) the stages with rounds: lead tiles in bound order, the refine stage against the merged key, the survivors sorted
-      by max(single-point key, refined key) and evaluated in rounds of 8, 16, 32 and the rest of the tiles, a round
-      skipping the tiles whose first key is above the key merged before it, return the records of a full argsort,
-      on well-conditioned, clustered and ill-conditioned (tests/golden) training sets;
+  (b) the stages: lead tiles in bound order, the refine stage against the merged key, the survivors sorted by
+      max(single-point key, refined key) and evaluated in rounds of 8 tiles and then the rest (final_round_tiles), a
+      round skipping the tiles whose first key is above the key merged before it, return the records of a full
+      argsort, on well-conditioned, clustered and ill-conditioned (tests/golden) training sets;
   (c) unit_mu_from_ks: mu = K* alpha_ recomputed from the stored K* by one fma chain per (part, column), chunks
       ascending and rows part * 16 .. part * 16 + 15 of each, is phase A's mu bit for bit on IEEE doubles, and a
       chain in plain row order is not.
@@ -27,7 +27,7 @@ GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 TILE = 8  # candidates per tile here (PBN = 128 on the device)
 LEAD = 8  # kLeadTiles
 MAX_TILES = 24  # kRefineMaxTiles, scaled down with the tile
-ROUND_TILES = (8, 16, 32)  # then the rest
+FIRST_ROUND = 8  # tiles of the first final round, then the rest
 
 
 def kth(values, k):
@@ -38,7 +38,7 @@ def kth(values, k):
 
 def stages(lb1, lbr, value, k):
     """(evaluated candidates, merged key after the lead, per-list key after the lead, keys before each round):
-    the lead, refine and final stages with rounds over candidates keyed by lb1 (single point) and lbr (refined)."""
+    the lead, refine and final stages over candidates keyed by lb1 (single point) and lbr (refined)."""
     m = len(value)
     perm = np.argsort(lb1, kind="stable")
     ntiles = -(-m // TILE)
@@ -66,7 +66,7 @@ def stages(lb1, lbr, value, k):
     stiles = [surv[t * TILE:(t + 1) * TILE] for t in range(-(-len(surv) // TILE))]
     t0, r, before = 0, 0, []
     while t0 < MAX_TILES:
-        t1 = t0 + (ROUND_TILES[r] if r < len(ROUND_TILES) else MAX_TILES - t0)
+        t1 = t0 + (FIRST_ROUND if r == 0 else MAX_TILES - t0)
         before.append(key)
         for t in stiles[t0:t1]:
             if skey[t[0]] > key:  # sorted: every later tile of the round is skipped too

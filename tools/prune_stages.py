@@ -3,8 +3,7 @@ stages' switches in one process, then bench.py per setting, alternated.
 
   python tools/prune_stages.py [--settings 0,1] [--reps 3] [--calls 3] [--legs c3,c2,c5,philox,worst] [--bench-runs 2]
 
-A setting is a value of B200BO_PRUNE_REFINE, or switches joined by '+', e.g. the stages without and with their
-rounds and shared K*:  --settings ROUNDS=0+SHARED_KS=0,ROUNDS=1+SHARED_KS=1  (names without B200BO_PRUNE_), or the two
+A setting is a value of B200BO_PRUNE_REFINE, or switches joined by '+' (names without B200BO_PRUNE_), e.g. the two
 fp32 Gram bound kernels:  --settings GRAM_KERNEL=ring,GRAM_KERNEL=reg
 
 Legs as in tools/prune_ab.py (argmin + top-10; Matern-2.5, alpha 1e-6, normalize_y).  Per leg and setting:
@@ -31,8 +30,7 @@ from predict_pipe_ab import Sampler, card  # noqa: E402
 from prune_ab import ALPHA, K, LEGS, XI  # noqa: E402
 
 STAGES = ("bound", "sort", "lead", "refine", "final", "tiles")
-SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_ROUNDS", "B200BO_PRUNE_SHARED_KS", "B200BO_PRUNE_GRAM_KERNEL",
-            "B200BO_PRUNE_LEVELS")
+SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_GRAM_KERNEL")
 
 
 def setting_env(s):
