@@ -12,7 +12,8 @@ Two layers:
     UpperConfidenceBound, ExpectedImprovement, ProbabilityOfImprovement, LogExpectedImprovement,
     LogProbabilityOfImprovement, NoisyExpectedImprovement, LogNoisyExpectedImprovement,
     ConstrainedNoisyExpectedImprovement, LogConstrainedNoisyExpectedImprovement, ThompsonSampling,
-    ConstrainedThompsonSampling, MaxValueEntropySearch, PosteriorMean, ConstantLiar, KrigingBeliever, PendingNEI, GPHedge,
+    ConstrainedThompsonSampling, TrustRegionThompsonSampling, MaxValueEntropySearch, PosteriorMean, ConstantLiar,
+    KrigingBeliever, PendingNEI, GPHedge,
     AcquisitionFunction, ConstraintModel, enable(optimizer), suggest_batch(optimizer, q) - resolved lazily on first access.
   * recommend(optimizer): the point a run should report, by the posterior mean (bayes_opt is imported when called).
 """
@@ -35,7 +36,7 @@ _PLUGIN = {
     "NoisyExpectedImprovement": "acquisition", "LogNoisyExpectedImprovement": "acquisition",
     "PendingNEI": "acquisition", "ConstrainedNoisyExpectedImprovement": "acquisition",
     "LogConstrainedNoisyExpectedImprovement": "acquisition", "ConstraintModel": "constraint", "PosteriorPaths": "paths",
-    "ConstrainedPaths": "paths", "PosteriorMean": "acquisition",
+    "ConstrainedPaths": "paths", "PosteriorMean": "acquisition", "TrustRegionThompsonSampling": "acquisition",
 }
 
 

@@ -39,7 +39,8 @@ EXPORTS = [
     "b200bo_cpaths_argmin_topk_philox", "b200bo_paths_eval_rows", "b200bo_cpaths_eval_rows",
     "b200bo_acq_value_grad", "b200bo_paths_grad_rows", "b200bo_gp_fork", "b200bo_gp_condition",
     "b200bo_gp_set_fantasies", "b200bo_gp_condition_fantasies", "b200bo_gp_set_fantasy_incumbent",
-    "b200bo_gp_set_constrained_incumbent",
+    "b200bo_gp_set_constrained_incumbent", "b200bo_paths_argmin_topk_philox_tr", "b200bo_cpaths_argmin_topk_philox_tr",
+    "b200bo_philox_tr_rows",
 ]
 
 
@@ -157,6 +158,10 @@ def lib():
     L.b200bo_cpaths_argmin_topk.argtypes = [*sets, dp, C.c_int64, C.c_int, dp, i64p, dp, i64p]
     L.b200bo_cpaths_argmin_topk_philox.argtypes = [*sets, C.c_uint64, dp, dp, C.c_int64, C.c_int64, C.c_int,
                                                    *philox_outs]
+    tr = [C.c_uint64, dp, dp, dp, C.c_double, C.c_int64, C.c_int64, C.c_int]  # seed, lo, hi, center, p, m, base, k
+    L.b200bo_paths_argmin_topk_philox_tr.argtypes = [C.c_void_p, *tr, *philox_outs]
+    L.b200bo_cpaths_argmin_topk_philox_tr.argtypes = [*sets, *tr, *philox_outs]
+    L.b200bo_philox_tr_rows.argtypes = [C.c_int, C.c_uint64, dp, dp, dp, C.c_double, C.c_int, i64p, C.c_int64, dp]
     _lib = L
     return L
 

@@ -119,36 +119,56 @@ class DeviceHooks(abc.ABC):
     def _refine_grad(self, acq, space):
         return self.b200_refine == "analytic" and all(space.continuous_dimensions) and _offers_grad(acq)
 
+    def _candidate_rows(self, space, n, random_state):
+        """The host_rng candidates of the random stage: the reference's RNG stream (TrustRegionThompsonSampling: its
+        trust-region source)."""
+        return space.random_sample(n, random_state=random_state)
+
+    def _select_philox(self, sel, seed, space, n, k):
+        """The device_philox random stage of a closure or of q paths: ``argmin_topk_philox`` over the space's bounds
+        (TrustRegionThompsonSampling: over its trust-region source)."""
+        return sel.argmin_topk_philox(seed, space.bounds, n, k)
+
     def _random_sample_minimize(self, acq, space, random_state, n_random, n_x_seeds=0):
-        if n_random == 0 or not _device_closure(acq) or n_x_seeds > B.MAX_TOPK:
-            # (n_smart beyond the device's top-k capacity: evaluate on the device, select with numpy)
+        if n_random == 0 or not _device_closure(acq):
             return super()._random_sample_minimize(acq, space, random_state, n_random, n_x_seeds)
-        if self.b200_candidate_source == "device_philox" and all(space.continuous_dimensions):
+        if (n_x_seeds <= B.MAX_TOPK and self.b200_candidate_source == "device_philox"
+                and all(space.continuous_dimensions)):
             seed = _philox_seed(random_state)
-            _, min_acq, x_min, _, x_seeds = acq.argmin_topk_philox(seed, space.bounds, n_random, n_x_seeds)
+            _, min_acq, x_min, _, x_seeds = self._select_philox(acq, seed, space, n_random, n_x_seeds)
             return x_min, min_acq, (x_seeds if n_x_seeds != 0 else [])
-        x_tries = space.random_sample(n_random, random_state=random_state)  # the reference's RNG stream
+        x_tries = self._candidate_rows(space, n_random, random_state)
+        if n_x_seeds > B.MAX_TOPK:
+            # n_smart beyond the device's top-k capacity: evaluate on the device, select with numpy as the reference
+            ys = acq(x_tries)
+            return x_tries[ys.argmin()], ys.min(), x_tries[np.argsort(ys)[:n_x_seeds]]
         idx, min_acq, top = acq.argmin_topk(x_tries, n_x_seeds)
         return x_tries[idx], min_acq, (x_tries[top] if n_x_seeds != 0 else [])
 
+    def _refine_bounds(self, space):
+        """(d, 2) bounds of the L-BFGS-B refinement and of its clip: the space's (TrustRegionThompsonSampling: its
+        trust region)."""
+        return space.bounds
+
     def _smart_minimize(self, acq, space, x_seeds, random_state):
+        bounds = self._refine_bounds(space)
         if len(x_seeds) != 0 and self._refine_grad(acq, space):
-            runs = [r for r in lockstep_lbfgsb(acq, x_seeds, space.bounds, grad=True) if r.success]
-            return self._best_run(runs, space)
+            runs = [r for r in lockstep_lbfgsb(acq, x_seeds, bounds, grad=True) if r.success]
+            return self._best_run(runs, bounds)
         batched = _device_closure(acq) or getattr(acq, "b200_vectorized", False)
         refine = acq.refine_mode() if _device_closure(acq) and hasattr(acq, "refine_mode") else _null()
         with refine:
             if not batched or len(x_seeds) == 0 or not all(space.continuous_dimensions):
                 return super()._smart_minimize(acq, space, x_seeds, random_state)
-            runs = [r for r in lockstep_lbfgsb(acq, x_seeds, space.bounds) if r.success]
-        return self._best_run(runs, space)
+            runs = [r for r in lockstep_lbfgsb(acq, x_seeds, bounds) if r.success]
+        return self._best_run(runs, bounds)
 
     @staticmethod
-    def _best_run(runs, space):
+    def _best_run(runs, bounds):
         if not runs:
-            return np.full(space.bounds.shape[0], np.nan), np.inf
+            return np.full(bounds.shape[0], np.nan), np.inf
         best = min(runs, key=lambda r: float(np.squeeze(r.fun)))  # first of equal minima, like the loop
-        return np.clip(best.x, space.bounds[:, 0], space.bounds[:, 1]), np.squeeze(best.fun)
+        return np.clip(best.x, bounds[:, 0], bounds[:, 1]), np.squeeze(best.fun)
 
 
 class _null:
@@ -440,9 +460,9 @@ class ThompsonSampling(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
         Returns (q, d) random-stage winners, (q,) their -path values, and per path its top-k rows, best first."""
         q = paths.n_paths
         if self.b200_candidate_source == "device_philox" and all(space.continuous_dimensions) and k <= B.MAX_TOPK:
-            _, vals, x_r, _, tx = paths.argmin_topk_philox(_philox_seed(random_state), space.bounds, n, k)
+            _, vals, x_r, _, tx = self._select_philox(paths, _philox_seed(random_state), space, n, k)
             return x_r, vals, (tx if k else [[]] * q)
-        x_tries = space.random_sample(n, random_state=random_state)  # the reference's RNG stream
+        x_tries = self._candidate_rows(space, n, random_state)
         if k <= B.MAX_TOPK:
             idx, vals, ti = paths.argmin_topk(x_tries, k)
             tops = [x_tries[t] for t in ti]
@@ -460,17 +480,10 @@ class ThompsonSampling(_SuggestStream, DeviceHooks, _ref.AcquisitionFunction):
             return [self._smart_minimize(acq.path(p), space, tops[p], random_state) for p in range(q)]
         seeds = [s for p in range(q) for s in tops[p]]
         owner = [p for p in range(q) for _ in tops[p]]
-        runs = lockstep_lbfgsb(acq, seeds, space.bounds, run_paths=owner,
+        bounds = self._refine_bounds(space)
+        runs = lockstep_lbfgsb(acq, seeds, bounds, run_paths=owner,
                                grad=self._refine_grad(acq, space)) if seeds else []
-        out = []
-        for p in range(q):
-            ok = [r for r, o in zip(runs, owner) if o == p and r.success]
-            if not ok:
-                out.append((np.full(space.bounds.shape[0], np.nan), np.inf))
-                continue
-            best = min(ok, key=lambda r: float(np.squeeze(r.fun)))  # first of equal minima, like the loop
-            out.append((np.clip(best.x, space.bounds[:, 0], space.bounds[:, 1]), np.squeeze(best.fun)))
-        return out
+        return [self._best_run([r for r, o in zip(runs, owner) if o == p and r.success], bounds) for p in range(q)]
 
     def get_acquisition_params(self):
         return {"n_features": self.n_features}
@@ -506,6 +519,120 @@ class ConstrainedThompsonSampling(ThompsonSampling):
         return self._closure(ConstrainedPaths(target, paths, constraint.lb, constraint.ub))
 
 
+class TrustRegionThompsonSampling(ConstrainedThompsonSampling):
+    """Thompson sampling inside a trust region: TuRBO-1 (Eriksson et al., NeurIPS 2019) over the global GP, and with a
+    ConstraintModel SCBO (Eriksson & Poloczek, AISTATS 2021).  DESIGN.md 4.18.
+
+    A box around the best registered row of the current run, shaped by the fitted GP's length scales, grows after
+    ``success_tolerance`` successful batches, shrinks after ``failure_tolerance`` failed ones (None:
+    ceil(max(4, d) / q), q the size of the batch just evaluated) and restarts when its length falls below ``length_min``
+    (``trust_region.TrustRegionState``).  Each ``suggest`` / ``suggest_batch(q <= 16)``:
+      1. folds the rows registered since the last call into the state and picks the centre: the best row of the run
+         inside the space's current bounds (with none inside, the run's best clipped into them);
+      2. when the current run has no row yet (after a restart) returns ``space.random_sample(q, rs)`` and draws nothing
+         else;
+      3. otherwise runs (Constrained)ThompsonSampling's suggest with three changes: the random-stage candidates are the
+         centre with a random subset of coordinates redrawn in the box (about min(d, 20) of them;
+         ``trust_region.host_candidates`` from the RandomState in host_rng mode, ``argmin_topk_philox_tr`` from one
+         Philox seed in device_philox mode), the L-BFGS-B refinement runs inside the box, and the result is clipped to
+         it.
+    Continuous spaces only (NotImplementedError otherwise).  ConstantLiar, GPHedge and KrigingBeliever refuse it
+    (TypeError): their dummy rows would count as observations.  The state travels in get/set_acquisition_params, so
+    ``save_state`` / ``load_state`` resume the run.  ``last_box`` is the (lo, hi) of the latest call, None after a
+    random call."""
+
+    def __init__(self, n_features=4096, length_init=0.8, length_min=2**-7, length_max=1.6, success_tolerance=3,
+                 failure_tolerance=None, random_state=None):
+        from .trust_region import TrustRegionConfig, TrustRegionState
+
+        super().__init__(n_features=n_features, random_state=random_state)
+        self.tr_config = TrustRegionConfig(length_init, length_min, length_max, success_tolerance, failure_tolerance)
+        self.tr_state = TrustRegionState(length=self.tr_config.length_init)
+        self.last_box = None
+        self._tr_center = None  # inside suggest: the centre row, then (lo, hi, center, p) once the GP is fitted
+        self._tr_box = None
+
+    @staticmethod
+    def _tr_rows(space):
+        """(targets, total violations or None) of every registered row."""
+        from .trust_region import total_violation
+
+        if space.constraint is None:
+            return space.target, None
+        return space.target, total_violation(space.constraint_values, space.constraint.lb, space.constraint.ub)
+
+    def suggest(self, gp, target_space, n_random=10_000, n_smart=10, fit_gp=True, random_state=None):
+        if len(target_space) == 0:  # the reference's TargetSpaceEmptyError
+            return super().suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
+                                   random_state=random_state)
+        if not all(target_space.continuous_dimensions):
+            raise NotImplementedError(f"{type(self).__name__} supports continuous spaces only: its trust region is a "
+                                      "box of the continuous coordinates")
+        y, viol = self._tr_rows(target_space)
+        self.tr_state = self.tr_state.update(y, viol, target_space.dim, self.tr_config)
+        if self.tr_state.run_empty:  # a restart: the new run begins at random points
+            self.i += 1
+            self.last_box = None
+            X = target_space.random_sample(self._batch_q or 1, random_state=_ensure_rng(random_state))
+            return X if self._batch_q is not None else X[0]
+        # the best row of the run inside the current bounds; with none inside, the run's best (box() clips it in)
+        idx = self.tr_state.center_index(y, viol, target_space.params, target_space.bounds)
+        if idx is None:
+            idx = self.tr_state.center_index(y, viol)
+        self._tr_center = np.array(target_space.params[idx], dtype=np.float64)
+        try:
+            x = super().suggest(gp, target_space, n_random=n_random, n_smart=n_smart, fit_gp=fit_gp,
+                                random_state=random_state)
+            lo, hi = self.last_box
+            return np.clip(x, lo, hi)
+        finally:
+            self._tr_center = self._tr_box = None
+
+    def _get_acq(self, gp, constraint=None):
+        if self._tr_center is not None:  # the fitted GP's length scales shape this call's box
+            from .gpr import parse_kernel
+            from .trust_region import box, perturb_probability
+
+            space = self._suggest_space
+            ls = parse_kernel(_as_b200_gp(gp).kernel_).length_scale
+            lo, hi, center = box(self._tr_center, self.tr_state.length, ls, space.bounds)
+            self._tr_box = (lo, hi, center, perturb_probability(space.dim))
+            self.last_box = (lo, hi)
+        return super()._get_acq(gp, constraint=constraint)
+
+    def _refine_bounds(self, space):
+        if self._tr_box is None:
+            return space.bounds
+        return np.stack(self._tr_box[:2], axis=1)
+
+    def _candidate_rows(self, space, n, random_state):
+        if self._tr_box is None:
+            return super()._candidate_rows(space, n, random_state)
+        from .trust_region import host_candidates
+
+        lo, hi, center, p = self._tr_box
+        return host_candidates(random_state, n, lo, hi, center, p)
+
+    def _select_philox(self, sel, seed, space, n, k):
+        if self._tr_box is None:
+            return super()._select_philox(sel, seed, space, n, k)
+        lo, hi, center, p = self._tr_box
+        return sel.argmin_topk_philox_tr(seed, lo, hi, center, p, n, k)
+
+    def get_acquisition_params(self):
+        from dataclasses import asdict
+
+        return {**super().get_acquisition_params(), "trust_region_config": asdict(self.tr_config),
+                "trust_region": self.tr_state.to_dict()}
+
+    def set_acquisition_params(self, params):
+        from .trust_region import TrustRegionConfig, TrustRegionState
+
+        super().set_acquisition_params(params)
+        self.tr_config = TrustRegionConfig(**params["trust_region_config"])
+        self.tr_state = TrustRegionState.from_dict(params["trust_region"])
+
+
 def distinct_picks(picks, tops):
     """The duplicate rule of batch Thompson sampling: in path order p = 0..q-1, a pick bit-equal to an earlier pick is
     replaced by the first row of tops[p] (path p's top-k, best first) that is bit-equal to no pick so far; with none
@@ -526,11 +653,12 @@ def distinct_picks(picks, tops):
 
 def suggest_batch(optimizer, q):
     """q parameter dicts to probe next from a ``bayes_opt.BayesianOptimization`` whose acquisition function is a
-    (Constrained)ThompsonSampling, a KrigingBeliever or a PendingNEI: ``BayesianOptimization.suggest`` for a batch
-    (R/bayes_opt/bayesian_optimization.py:323-333).  With no registered point it returns ``optimizer.random_sample(q)``;
-    otherwise the acquisition's ``suggest_batch`` with the optimizer's GP, target space and RandomState, each row
-    converted with ``array_to_params``.  For Thompson sampling nothing new enters ``save_state`` (q is an argument, not
-    state); a KrigingBeliever or PendingNEI records the q points as dummies, which ``save_state`` carries."""
+    (Constrained)ThompsonSampling, a TrustRegionThompsonSampling, a KrigingBeliever or a PendingNEI:
+    ``BayesianOptimization.suggest`` for a batch (R/bayes_opt/bayesian_optimization.py:323-333).  With no registered
+    point it returns ``optimizer.random_sample(q)``; otherwise the acquisition's ``suggest_batch`` with the optimizer's
+    GP, target space and RandomState, each row converted with ``array_to_params``.  For Thompson sampling nothing new
+    enters ``save_state`` (q is an argument, not state); a KrigingBeliever or PendingNEI records the q points as
+    dummies, which ``save_state`` carries."""
     acq = optimizer._acquisition_function
     if isinstance(acq, _PendingBatch):
         q = _check_int("q", q, 1)
@@ -875,6 +1003,9 @@ def _refuse_nei(acq, where):
     if isinstance(acq, PosteriorMean):
         raise TypeError(f"{where} does not support {type(acq).__name__}: it recommends the best posterior mean and "
                         "does not choose points to evaluate")
+    if isinstance(acq, TrustRegionThompsonSampling):
+        raise TypeError(f"{where} does not support {type(acq).__name__}: its trust region would count the dummy rows "
+                        "as observations")
 
 
 _HOOKED = {

@@ -2867,13 +2867,19 @@ extern "C" int b200bo_acq_argmin_topk(const b200bo_acq* spec, const double* Xc, 
 // ---------------------------------------------------------------------------------------
 // The Philox rows of q sets of (kk+1) merged records at d_rec (kk = max(k, 1)), regenerated on stream into prow from
 // the device bounds pbounds: best_x (q,d), topk_x (q,k,d) host, either nullable
+// tr: the trust-region source, pbounds [3][d] with the centre last, perturbation probability tr_p.
 static int philox_winner_rows(DevBuf& prow, const DevBuf& pbounds, uint64_t seed, const SelRecord* d_rec, int q, int k,
-                              int d, double* best_x, double* topk_x, cudaStream_t stream) {
+                              int d, double* best_x, double* topk_x, cudaStream_t stream, bool tr = false,
+                              double tr_p = 1.0) {
     if (!best_x && !(topk_x && k > 0)) return B200BO_OK;
     const int kk = k > 0 ? k : 1, nrec = q * (kk + 1);
     int rc;
     if ((rc = prow.reserve(sizeof(double) * (size_t)nrec * d))) return rc;
-    philox_rows_kernel<<<nrec, 64, 0, stream>>>(seed, pbounds.as<double>(), d, d_rec, nrec, prow.as<double>());
+    if (tr)
+        philox_tr_rows_kernel<<<nrec, 64, 0, stream>>>(seed, pbounds.as<double>(), tr_p, d, d_rec, nrec,
+                                                       prow.as<double>());
+    else
+        philox_rows_kernel<<<nrec, 64, 0, stream>>>(seed, pbounds.as<double>(), d, d_rec, nrec, prow.as<double>());
     LAUNCHED();
     CU(cudaGetLastError());
     std::vector<double> rows((size_t)nrec * d);
@@ -2933,6 +2939,51 @@ extern "C" int b200bo_philox_rows(int device, uint64_t seed, const double* lo, c
     LAUNCHED();
     cudaError_t e = cudaMemcpy(out, d_out.p, sizeof(double) * n_idx * d, cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) return set_err(B200BO_ERR_CUDA, "philox_rows: %s", cudaGetErrorString(e));
+    return B200BO_OK;
+}
+
+// trust-region source (select.cuh philox_tr_coord): lo <= center <= hi, all finite, 0 <= p <= 1 -> pb [3][d]
+static int pack_tr_bounds(const double* lo, const double* hi, const double* center, double p, int d, double* pb) {
+    if (!lo || !hi || !center) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (!(p >= 0.0 && p <= 1.0)) return set_err(B200BO_ERR_ARG, "trust region: p=%g out of [0,1]", p);
+    for (int j = 0; j < d; ++j) {
+        if (!(std::isfinite(lo[j]) && std::isfinite(hi[j]) && std::isfinite(center[j])))
+            return set_err(B200BO_ERR_ARG, "trust region: non-finite bound or centre in column %d", j);
+        if (!(lo[j] <= center[j] && center[j] <= hi[j]))
+            return set_err(B200BO_ERR_ARG, "trust region: lo <= center <= hi fails in column %d", j);
+        pb[j] = lo[j];
+        pb[d + j] = hi[j] - lo[j];
+        pb[2 * d + j] = center[j];
+    }
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_philox_tr_rows(int device, uint64_t seed, const double* lo, const double* hi,
+                                     const double* center, double p, int d, const int64_t* idx, int64_t n_idx,
+                                     double* out) {
+    if (!idx || !out) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (d <= 0 || d > B200BO_MAX_DIM || n_idx < 0) return set_err(B200BO_ERR_ARG, "bad shape");
+    std::vector<double> pb(3 * d);
+    int rc;
+    if ((rc = pack_tr_bounds(lo, hi, center, p, d, pb.data()))) return rc;
+    if (n_idx == 0) return B200BO_OK;
+    CU(cudaSetDevice(device));
+    std::vector<SelRecord> rec((size_t)n_idx);
+    for (int64_t i = 0; i < n_idx; ++i) {
+        rec[i].value = 0.0;
+        rec[i].index = idx[i];
+    }
+    DevBuf d_rec, d_pb, d_out;
+    if ((rc = d_rec.reserve(sizeof(SelRecord) * n_idx))) return rc;
+    if ((rc = d_pb.reserve(sizeof(double) * 3 * d))) return rc;
+    if ((rc = d_out.reserve(sizeof(double) * n_idx * d))) return rc;
+    CU(cudaMemcpy(d_rec.p, rec.data(), sizeof(SelRecord) * n_idx, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d_pb.p, pb.data(), sizeof(double) * 3 * d, cudaMemcpyHostToDevice));
+    philox_tr_rows_kernel<<<(unsigned)n_idx, 64>>>(seed, d_pb.as<double>(), p, d, d_rec.as<SelRecord>(), (int)n_idx,
+                                                   d_out.as<double>());
+    LAUNCHED();
+    cudaError_t e = cudaMemcpy(out, d_out.p, sizeof(double) * n_idx * d, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) return set_err(B200BO_ERR_CUDA, "philox_tr_rows: %s", cudaGetErrorString(e));
     return B200BO_OK;
 }
 
@@ -3278,13 +3329,14 @@ extern "C" int b200bo_paths_argmin_topk(b200bo_paths* ps, const double* Xc, int6
     return read_records(ps->sel.p, q, k, best_val, best_idx, topk_val, topk_idx);
 }
 
-// Philox bounds into ps->pbounds, on the device when this returns (the selection may run on a non-blocking stream)
-static int paths_set_pbounds(b200bo_paths* ps, const double* lo, const double* hi) {
+// Philox bounds into ps->pbounds, in the order of `stream`: the kernels that read them run on it (a host-to-device copy
+// from pageable memory returns once staged, so on the legacy stream alone it would not order a non-blocking stream)
+static int paths_set_pbounds(b200bo_paths* ps, const double* lo, const double* hi, cudaStream_t stream = nullptr) {
     double pb[2 * B200BO_MAX_DIM];
     int rc;
     if ((rc = pack_pbounds(lo, hi, ps->d, pb))) return rc;
     if ((rc = ps->pbounds.reserve(sizeof(double) * 2 * B200BO_MAX_DIM))) return rc;
-    CU(cudaMemcpy(ps->pbounds.p, pb, sizeof(double) * 2 * ps->d, cudaMemcpyHostToDevice));
+    CU(cudaMemcpyAsync(ps->pbounds.p, pb, sizeof(double) * 2 * ps->d, cudaMemcpyHostToDevice, stream));
     return B200BO_OK;
 }
 
@@ -3314,6 +3366,48 @@ extern "C" int b200bo_paths_argmin_topk_philox(b200bo_paths* ps, uint64_t seed, 
     if ((rc = paths_merge(ps, grid, kk, nullptr))) return rc;
     if ((rc = read_records(ps->sel.p, q, k, best_val, best_idx, topk_val, topk_idx))) return rc;
     return philox_winner_rows(ps->prow, ps->pbounds, seed, ps->sel.as<SelRecord>(), q, k, ps->d, best_x, topk_x, nullptr);
+}
+
+// trust-region bounds and centre into ps->pbounds ([3][d]), in the order of `stream` (as paths_set_pbounds)
+static int paths_set_tr_bounds(b200bo_paths* ps, const double* lo, const double* hi, const double* center, double p,
+                               cudaStream_t stream = nullptr) {
+    double pb[3 * B200BO_MAX_DIM];
+    int rc;
+    if ((rc = pack_tr_bounds(lo, hi, center, p, ps->d, pb))) return rc;
+    if ((rc = ps->pbounds.reserve(sizeof(double) * 3 * B200BO_MAX_DIM))) return rc;
+    CU(cudaMemcpyAsync(ps->pbounds.p, pb, sizeof(double) * 3 * ps->d, cudaMemcpyHostToDevice, stream));
+    return B200BO_OK;
+}
+
+extern "C" int b200bo_paths_argmin_topk_philox_tr(b200bo_paths* ps, uint64_t seed, const double* lo, const double* hi,
+                                                  const double* center, double p, int64_t m, int64_t index_base, int k,
+                                                  double* best_val, int64_t* best_idx, double* best_x,
+                                                  double* topk_val, int64_t* topk_idx, double* topk_x) {
+    if (!ps) return set_err(B200BO_ERR_ARG, "NULL argument");
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (m <= 0) return set_err(B200BO_ERR_ARG, "m must be > 0");
+    CU(cudaSetDevice(ps->device));
+    NvtxRange nvtx_range("b200bo:paths_select");
+    int rc;
+    if ((rc = paths_set_tr_bounds(ps, lo, hi, center, p))) return rc;
+    const int kk = k > 0 ? k : 1, q = ps->q, d = ps->d;
+    const int grid = paths_grid(ps, m);
+    if ((rc = ps->sel_cta.reserve(sizeof(SelList) * (size_t)q * grid))) return rc;
+    if ((rc = ps->sel.reserve(sizeof(SelRecord) * (size_t)q * (kk + 1)))) return rc;
+    PathsParams P = paths_params(ps);
+    P.pbounds = ps->pbounds.as<double>();
+    P.tr_center = ps->pbounds.as<double>() + 2 * d;
+    P.tr_p = p;
+    P.seed = seed;
+    P.index_base = index_base;
+    P.m = m;
+    P.sel_cta = ps->sel_cta.as<SelList>();
+    P.sel_k = kk;
+    if ((rc = paths_launch(ps, P, grid, nullptr))) return rc;
+    if ((rc = paths_merge(ps, grid, kk, nullptr))) return rc;
+    if ((rc = read_records(ps->sel.p, q, k, best_val, best_idx, topk_val, topk_idx))) return rc;
+    return philox_winner_rows(ps->prow, ps->pbounds, seed, ps->sel.as<SelRecord>(), q, k, d, best_x, topk_x, nullptr,
+                              true, p);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -3355,9 +3449,11 @@ static int cpaths_check(b200bo_paths* const* sets, int G, const double* lb, cons
 // Xc: host rows, streamed through set 0's ChunkedUpload; nullptr: the Philox source of set 0's pbounds and `seed`,
 // generated chunk by chunk.  k > 0: -g folded into the per-path lists (merged into set 0's sel); merit / raw (host,
 // nullable): the (m,q) merit and the (m,G,q) values.  pidx (device, (m,), nullable): row mode - merit is (m,), row i
-// on path pidx[i] only (host rows, k = 0, no raw).  Returns with the work finished and the inputs checked.
+// on path pidx[i] only (host rows, k = 0, no raw).  tr (Philox only): the trust-region source, set 0's pbounds [3][d]
+// with the centre last, perturbation probability tr_p.  Returns with the work finished and the inputs checked.
 static int cpaths_run(b200bo_paths* const* sets, CPathsParams& C, const double* Xc, uint64_t seed, int64_t m,
-                      int64_t index_base, int k, double* merit, double* raw, const int* pidx = nullptr) {
+                      int64_t index_base, int k, double* merit, double* raw, const int* pidx = nullptr,
+                      bool tr = false, double tr_p = 1.0) {
     b200bo_paths* s0 = sets[0];
     const int G = C.G, q = pidx ? 1 : C.q, d = s0->d;  // q: values per row
     const long long chunk = kChunkTilesPerSm * PBN * s0->sm_count;
@@ -3387,6 +3483,10 @@ static int cpaths_run(b200bo_paths* const* sets, CPathsParams& C, const double* 
             PathsParams P = paths_params(sets[g]);
             P.Xc = dx;
             P.pbounds = s0->pbounds.as<double>();
+            if (tr) {
+                P.tr_center = s0->pbounds.as<double>() + 2 * d;
+                P.tr_p = tr_p;
+            }
             P.seed = seed;
             P.index_base = index_base + c0;
             P.m = mc;
@@ -3487,11 +3587,34 @@ extern "C" int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G
     CU(cudaSetDevice(s0->device));
     NvtxRange nvtx_range("b200bo:cpaths_select");
     const int kk = k > 0 ? k : 1;
-    if ((rc = paths_set_pbounds(s0, lo, hi))) return rc;
+    if ((rc = s0->upload.ensure())) return rc;
+    if ((rc = paths_set_pbounds(s0, lo, hi, s0->upload.exec))) return rc;
     if ((rc = cpaths_run(sets, C, nullptr, seed, m, index_base, kk, nullptr, nullptr))) return rc;
     if ((rc = read_records(s0->sel.p, C.q, k, best_val, best_idx, topk_val, topk_idx))) return rc;
     return philox_winner_rows(s0->prow, s0->pbounds, seed, s0->sel.as<SelRecord>(), C.q, k, s0->d, best_x, topk_x,
                               nullptr);
+}
+
+extern "C" int b200bo_cpaths_argmin_topk_philox_tr(b200bo_paths* const* sets, int G, const double* lb,
+                                                   const double* ub, uint64_t seed, const double* lo, const double* hi,
+                                                   const double* center, double p, int64_t m, int64_t index_base,
+                                                   int k, double* best_val, int64_t* best_idx, double* best_x,
+                                                   double* topk_val, int64_t* topk_idx, double* topk_x) {
+    CPathsParams C;
+    int rc;
+    if ((rc = cpaths_check(sets, G, lb, ub, C))) return rc;
+    if (k < 0 || k > B200BO_MAX_TOPK) return set_err(B200BO_ERR_ARG, "k=%d out of range", k);
+    if (m <= 0) return set_err(B200BO_ERR_ARG, "m must be > 0");
+    b200bo_paths* s0 = sets[0];
+    CU(cudaSetDevice(s0->device));
+    NvtxRange nvtx_range("b200bo:cpaths_select");
+    const int kk = k > 0 ? k : 1;
+    if ((rc = s0->upload.ensure())) return rc;
+    if ((rc = paths_set_tr_bounds(s0, lo, hi, center, p, s0->upload.exec))) return rc;
+    if ((rc = cpaths_run(sets, C, nullptr, seed, m, index_base, kk, nullptr, nullptr, nullptr, true, p))) return rc;
+    if ((rc = read_records(s0->sel.p, C.q, k, best_val, best_idx, topk_val, topk_idx))) return rc;
+    return philox_winner_rows(s0->prow, s0->pbounds, seed, s0->sel.as<SelRecord>(), C.q, k, s0->d, best_x, topk_x,
+                              nullptr, true, p);
 }
 
 // ---------------------------------------------------------------------------------------

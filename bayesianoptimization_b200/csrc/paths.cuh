@@ -46,7 +46,18 @@ struct PathsParams {
     double* out;              // [m][q] ([m] with path_idx) or nullptr
     SelList* sel_cta;         // [q][gridDim.x] per-CTA running selections, or nullptr
     const int* path_idx;      // [m]: row mode (ROWS instantiation) - row i on path path_idx[i] only
+    // trust-region source (select.cuh philox_tr_coord), Philox only: [d] centre in the pbounds buffer, or nullptr
+    const double* tr_center;
+    double tr_p;              // probability that a coordinate other than the forced one is perturbed
 };
+
+// coordinate j of candidate gi: host rows, the Philox box, or the trust-region source around tr_center
+__device__ __forceinline__ double paths_coord(const PathsParams& P, long long gi, int j) {
+    if (!P.Xc && P.tr_center)
+        return philox_tr_coord(P.seed, gi + P.index_base, j, P.d, P.pbounds[j], P.pbounds[P.d + j], P.tr_center[j],
+                               P.tr_p);
+    return candidate_coord(P, gi, j);
+}
 
 // dynamic shared memory: 2 stage buffers [64][d + q + 1] | xc [d][128] | red [2][q][128] | SelShared [q]
 __host__ __device__ inline size_t paths_smem_bytes(int d, int q, bool sel) {
@@ -87,7 +98,7 @@ __global__ void __launch_bounds__(PT_NT, QT == 16 ? 1 : 2) paths_eval_kernel(con
             const int cc = idx / d, j = idx - cc * d;
             const long long gi = c0 + cc;
             double v = 0.0;
-            if (gi < P.m) v = scale_input(candidate_coord(P, gi, j), P.xform, P.ls, j);
+            if (gi < P.m) v = scale_input(paths_coord(P, gi, j), P.xform, P.ls, j);
             xc_s[j * PBN + cc] = v;
         }
         int pc = 0;  // ROWS: the column of V / W this thread's candidate reads

@@ -288,6 +288,44 @@ __device__ __forceinline__ double philox_coord(unsigned long long seed, long lon
     return __dadd_rn(lo, __dmul_rn(span, u));
 }
 
+// ---------------------------------------------------------------------------------------
+// Trust-region source of the sample-path kernels (TuRBO / SCBO, DESIGN.md 4.18): the centre with a random subset of
+// its coordinates redrawn in the box [lo, hi].  Counter-based like philox_coord, per (seed, global row r, column j):
+//   u_j  = philox_coord over [lo_j, hi_j]                      (counter lane 3 = 0: the plain source over the box)
+//   v_j  = the same 53-bit uniform from counter (r_lo, r_hi, j/2, 1)
+//   f(r) = (o0 * d) >> 32,  o0 of counter (r_lo, r_hi, 0, 2)   (the column every row perturbs)
+//   x_j  = (j == f(r) || v_j < p) ? u_j : center_j
+// p >= 1 skips the mask draws: x_j = u_j, bit-equal to philox_coord.  oracle restatement: tests/trust_region_oracle.py
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ double philox_tr_coord(unsigned long long seed, long long row, int col, int d, double lo,
+                                                  double span, double center, double p) {
+    if (p < 1.0) {
+        const unsigned r0 = (unsigned)row, r1 = (unsigned)((unsigned long long)row >> 32);
+        const unsigned k0 = (unsigned)seed, k1 = (unsigned)(seed >> 32);
+        unsigned o[4];
+        philox4x32_10(r0, r1, 0u, 2u, k0, k1, o);
+        const int f = (int)(((unsigned long long)o[0] * (unsigned)d) >> 32);
+        if (col != f) {
+            philox4x32_10(r0, r1, (unsigned)(col >> 1), 1u, k0, k1, o);
+            const unsigned long long w = (col & 1) ? ((unsigned long long)o[2] | ((unsigned long long)o[3] << 32))
+                                                   : ((unsigned long long)o[0] | ((unsigned long long)o[1] << 32));
+            if (!((double)(w >> 11) * 1.1102230246251565e-16 < p)) return center;
+        }
+    }
+    return philox_coord(seed, row, col, lo, span);
+}
+
+// rows of the trust-region source for a list of global indices; bounds: [3][d] = lo_j, hi_j - lo_j, center_j
+__global__ void philox_tr_rows_kernel(unsigned long long seed, const double* __restrict__ bounds, double p, int d,
+                                      const SelRecord* __restrict__ rec, int nrec, double* __restrict__ out) {
+    const int r = blockIdx.x;
+    if (r >= nrec) return;
+    const long long row = rec[r].index;
+    for (int j = threadIdx.x; j < d; j += blockDim.x)
+        out[(size_t)r * d + j] =
+            (row >= 0) ? philox_tr_coord(seed, row, j, d, bounds[j], bounds[d + j], bounds[2 * d + j], p) : CUDART_NAN;
+}
+
 // rows of the Philox candidate matrix for a list of global indices (the winners' coordinates)
 __global__ void philox_rows_kernel(unsigned long long seed, const double* __restrict__ bounds, int d,
                                    const SelRecord* __restrict__ rec, int nrec, double* __restrict__ out) {

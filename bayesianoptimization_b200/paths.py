@@ -175,20 +175,34 @@ class PosteriorPaths:
         Returns (idx (q,), values (q,), x_best (q, d), [top-k indices], [top-k rows])."""
         if self._xform[0] == "host":
             raise NotImplementedError("device candidate generation with a host-side kernel transform")
-        bounds = B.c_f64(np.asarray(bounds, dtype=np.float64).reshape(self.dim, 2))
+        bounds = np.asarray(bounds, dtype=np.float64).reshape(self.dim, 2)
         lo, hi = B.c_f64(bounds[:, 0]), B.c_f64(bounds[:, 1])
+        return self._select_philox("_philox", (B.as_dp(lo), B.as_dp(hi)), seed, m, k, index_base)
+
+    def argmin_topk_philox_tr(self, seed, lo, hi, center, p, m, k, index_base=0):
+        """``argmin_topk_philox`` over the trust-region source (``b200bo_*_argmin_topk_philox_tr``): the centre with a
+        random subset of its coordinates redrawn in the box [lo, hi], each perturbed with probability p besides one
+        forced column per row (DESIGN.md 4.18).  Same returns."""
+        if self._xform[0] == "host":
+            raise NotImplementedError("device candidate generation with a host-side kernel transform")
+        lo, hi, center = (B.c_f64(np.asarray(a, dtype=np.float64).reshape(self.dim)) for a in (lo, hi, center))
+        return self._select_philox("_philox_tr", (B.as_dp(lo), B.as_dp(hi), B.as_dp(center), float(p)), seed, m, k,
+                                   index_base)
+
+    def _select_philox(self, suffix, source, seed, m, k, index_base):
+        """The selection entry _c_select + suffix over a device candidate source: its arguments `source` go between
+        the seed and m."""
         k, q, d = int(k), self.n_paths, self.dim
         kk = max(k, 1)
         bv, bi, bx = np.empty(q), np.empty(q, dtype=np.int64), np.empty((q, d))
         tv, ti, tx = np.empty(q * kk), np.empty(q * kk, dtype=np.int64), np.empty((q * kk, d))
-        B.check(getattr(B.lib(), self._c_select + "_philox")(
-            *self._args(), int(seed) & 0xFFFFFFFFFFFFFFFF, B.as_dp(lo), B.as_dp(hi), int(m), int(index_base), k,
+        B.check(getattr(B.lib(), self._c_select + suffix)(
+            *self._args(), int(seed) & 0xFFFFFFFFFFFFFFFF, *source, int(m), int(index_base), k,
             B.as_dp(bv), bi.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(bx), B.as_dp(tv),
             ti.ctypes.data_as(C.POINTER(C.c_int64)), B.as_dp(tx)))
         ti, tx = ti[:q * k].reshape(q, k), tx[:q * k].reshape(q, k, d)
         keep = ti >= 0
-        return bi, bv, bx, [ti[p][keep[p]] for p in range(q)], [tx[p][keep[p]] for p in range(q)]
-
+        return bi, bv, bx, [ti[r][keep[r]] for r in range(q)], [tx[r][keep[r]] for r in range(q)]
 
     def bound(self):
         """(q,) B_p >= |path_p(x)| for every x (computed at creation from the path's own weights)."""
@@ -281,6 +295,8 @@ class ConstrainedPaths:
     _c_select = "b200bo_cpaths_argmin_topk"
     argmin_topk = PosteriorPaths.argmin_topk
     argmin_topk_philox = PosteriorPaths.argmin_topk_philox
+    argmin_topk_philox_tr = PosteriorPaths.argmin_topk_philox_tr
+    _select_philox = PosteriorPaths._select_philox
 
 
 class PathAcquisition:
@@ -310,6 +326,10 @@ class PathAcquisition:
 
     def argmin_topk_philox(self, seed, bounds, m, k, index_base=0):
         idx, val, bx, ti, tx = self.paths.argmin_topk_philox(seed, bounds, m, k, index_base)
+        return int(idx[0]), float(val[0]), bx[0], ti[0], tx[0]
+
+    def argmin_topk_philox_tr(self, seed, lo, hi, center, p, m, k, index_base=0):
+        idx, val, bx, ti, tx = self.paths.argmin_topk_philox_tr(seed, lo, hi, center, p, m, k, index_base)
         return int(idx[0]), float(val[0]), bx[0], ti[0], tx[0]
 
 

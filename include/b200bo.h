@@ -475,6 +475,21 @@ int b200bo_paths_argmin_topk(b200bo_paths* paths, const double* Xc, int64_t m, i
 int b200bo_paths_argmin_topk_philox(b200bo_paths* paths, uint64_t seed, const double* lo, const double* hi, int64_t m,
                                     int64_t index_base, int k, double* best_val, int64_t* best_idx, double* best_x,
                                     double* topk_val, int64_t* topk_idx, double* topk_x);
+/* Trust-region source (TuRBO / SCBO, DESIGN.md 4.18): the centre with a random subset of coordinates redrawn in the box
+ * [lo, hi].  Per (seed, global row r, column j):
+ *   u_j  = the b200bo_paths_argmin_topk_philox coordinate over [lo_j, hi_j]   (counter (r_lo, r_hi, j/2, 0))
+ *   v_j  = the same 53-bit uniform from counter (r_lo, r_hi, j/2, 1)
+ *   f(r) = (o0 * d) >> 32, o0 the first word of counter (r_lo, r_hi, 0, 2)
+ *   x_j  = (j == f(r) || v_j < p) ? u_j : center_j
+ * p = 1 draws no mask: the candidates are bit-equal to b200bo_paths_argmin_topk_philox over [lo, hi].  lo, hi, center:
+ * (d,) host, lo <= center <= hi and all finite; 0 <= p <= 1; else B200BO_ERR_ARG.  Outputs as the plain entry. */
+int b200bo_paths_argmin_topk_philox_tr(b200bo_paths* paths, uint64_t seed, const double* lo, const double* hi,
+                                       const double* center, double p, int64_t m, int64_t index_base, int k,
+                                       double* best_val, int64_t* best_idx, double* best_x, double* topk_val,
+                                       int64_t* topk_idx, double* topk_x);
+/* Rows of the trust-region source for given global indices (idx < 0 -> NaN row).  out: (n_idx, d) host. */
+int b200bo_philox_tr_rows(int device, uint64_t seed, const double* lo, const double* hi, const double* center,
+                          double p, int d, const int64_t* idx, int64_t n_idx, double* out);
 /* bound: (q,) host.  B_p = |y_mean| + y_std (sqrt(2 const_value / L) sum_l |w[l][p]| + const_value sum_i |v[i][p]|),
  * computed at creation: |path_p(x)| <= B_p for every x, since |cos| <= 1 and 0 <= const_value k <= const_value. */
 int b200bo_paths_bound(const b200bo_paths* paths, double* bound);
@@ -505,6 +520,12 @@ int b200bo_cpaths_argmin_topk_philox(b200bo_paths* const* sets, int G, const dou
                                      uint64_t seed, const double* lo, const double* hi, int64_t m, int64_t index_base,
                                      int k, double* best_val, int64_t* best_idx, double* best_x, double* topk_val,
                                      int64_t* topk_idx, double* topk_x);
+/* The same over the trust-region source of b200bo_paths_argmin_topk_philox_tr (SCBO). */
+int b200bo_cpaths_argmin_topk_philox_tr(b200bo_paths* const* sets, int G, const double* lb, const double* ub,
+                                        uint64_t seed, const double* lo, const double* hi, const double* center,
+                                        double p, int64_t m, int64_t index_base, int k, double* best_val,
+                                        int64_t* best_idx, double* best_x, double* topk_val, int64_t* topk_idx,
+                                        double* topk_x);
 
 /* Duration (ms) of the most recent fused predict+acquisition kernel launched through a
  * device or host entry point on this thread, measured with CUDA events on its stream.  With selection-only pruning
