@@ -187,6 +187,7 @@ struct b200bo_gp {
     cudaEvent_t ev_stage[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool stage_timed = false, stage_refined = false;
     int stage_levels = 0;  // refine levels of the last pruned launch
+    int coop_final[2] = {-1, -1};  // final_rounds_coop per DREG: -1 not yet checked, 0 launch by launch, 1 cooperative
     DevBuf pbounds, prow;   // throughput mode: Philox bounds (lo, span) / regenerated winner rows
     bool replica = false;   // predict-only copy made by b200bo_gp_replicate
     // look-ahead Cholesky: bulk stream, chain/bulk events, copy of the next diagonal step's panel block
@@ -325,6 +326,8 @@ static int init_handle(b200bo_gp* gp) {
     CU(cudaFuncSetAttribute(predict_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(ks_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(ks_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(final_rounds_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
+    CU(cudaFuncSetAttribute(final_rounds_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPredictSmemBytesDmma));
     CU(cudaFuncSetAttribute(trailing_update64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTrailSmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
     CU(cudaFuncSetAttribute(dgemm128_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemm128SmemBytes));
@@ -1662,6 +1665,13 @@ static int prune_refine_blocks(int np, long long ntiles) {
     return b < nb / 8 ? b : nb / 8;
 }
 
+// Column groups per row-block group of the level's and the final rounds' units (DESIGN.md 4.9): 4 (32 columns each)
+// unless B200BO_PRUNE_COLSPLIT=0 (read per call, for A/B measurements) keeps every unit on all 128 columns
+static int prune_colgroups() {
+    const char* e = getenv("B200BO_PRUNE_COLSPLIT");
+    return e && e[0] == '0' ? 1 : 4;
+}
+
 // survivors of the level in key order (sorted slots pos): their local indices and carried prefixes
 __global__ void level_gather_kernel(const unsigned long long* __restrict__ ctl, int n_word, const int* __restrict__ pos,
                                     const int* __restrict__ idx, const double* __restrict__ pre, int* __restrict__ idx_out,
@@ -1689,6 +1699,23 @@ __global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
 static int final_round_tiles(int r, int t0, int grid) {
     const int t = r == 0 ? 8 : kRefineMaxTiles - t0;
     return t < grid ? t : grid;
+}
+
+// Whether the final rounds run as one cooperative launch (final_rounds_kernel): the device supports it and `grid`
+// CTAs of 512 threads with the phase B shared memory are co-resident (one per SM).  Checked once per handle.
+static bool final_rounds_coop(b200bo_gp* g0, bool dreg, int grid) {
+    int& ok = g0->coop_final[dreg ? 1 : 0];
+    if (ok < 0) {
+        int dev = 0, coop = 0, per_sm = 0;
+        ok = cudaGetDevice(&dev) == cudaSuccess &&
+             cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) == cudaSuccess && coop &&
+             cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+                 &per_sm, dreg ? final_rounds_kernel<true> : final_rounds_kernel<false>, P16_NT,
+                 kPredictSmemBytesDmma) == cudaSuccess &&
+             per_sm * g0->sm_count >= grid;
+        cudaGetLastError();
+    }
+    return ok == 1;
 }
 
 // The lead, refine, level and final stages of a pruned launch (predict16.cuh), between prune_prepare and the tile
@@ -1735,6 +1762,7 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     R.arrive = g0->prune_arrive.as<unsigned>();
     R.blocks = blocks;
     R.groups_max = nb / 2 < 32 ? nb / 2 : 32;
+    R.colgroups = prune_colgroups();
     R.final_stage = kStageLead;
     R.b0 = 0;
     R.b1 = nb;
@@ -1797,17 +1825,34 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     R.surv = lidx[0];
     R.surv_key = lk.Current();
     R.prefix = lpre[0];
-    for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r) {
-        R.t0 = t0;
-        R.t1 = t0 + final_round_tiles(r, t0, grid);
-        CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
-        build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+    FinalRounds F = {};  // the rounds' tiles; more than kMax rounds (a grid under 18 SMs) launch by launch
+    bool few = true;
+    for (int t0 = 0; t0 < kRefineMaxTiles && few; ++F.nr) {
+        few = F.nr < FinalRounds::kMax;
+        if (!few) break;
+        F.rt[F.nr] = t0;
+        t0 += final_round_tiles(F.nr, t0, grid);
+        F.rt[F.nr + 1] = t0;
+    }
+    CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+    if (few && final_rounds_coop(g0, dreg, grid)) {
+        void* args[] = {(void*)&Q, (void*)&R, (void*)&F};
+        CU(cudaLaunchCooperativeKernel(dreg ? (const void*)final_rounds_kernel<true> : (const void*)final_rounds_kernel<false>,
+                                       dim3(grid), dim3(P16_NT), args, kPredictSmemBytesDmma, stream));
         LAUNCHED();
-        predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-        LAUNCHED();
-        merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
-        LAUNCHED();
-        t0 = R.t1;
+    } else {  // the grid cannot be co-resident (or too many rounds): the rounds launch by launch
+        for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r) {
+            R.t0 = t0;
+            R.t1 = t0 + final_round_tiles(r, t0, grid);
+            if (r > 0) CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+            build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+            LAUNCHED();
+            predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
+            LAUNCHED();
+            merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
+            LAUNCHED();
+            t0 = R.t1;
+        }
     }
     CU(cudaGetLastError());
     CU(cudaEventRecord(g0->ev_stage[4], stream));

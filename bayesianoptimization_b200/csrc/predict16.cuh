@@ -22,6 +22,8 @@
 #pragma once
 #include <type_traits>
 
+#include <cooperative_groups.h>
+
 #include "predict_kernels.cuh"
 
 namespace b200bo {
@@ -815,17 +817,24 @@ __device__ __forceinline__ long long prune_claim(const PredictParams& P, long lo
     return tile_s;
 }
 
-// stage loader: BK k-rows x 128 doubles of LinvT (evict_last) and of K* (evict_first), 512 threads
+// stage loader: BK k-rows x 128 doubles of LinvT (evict_last) and of K* (evict_first), 512 threads.  NJ = 1: of K*
+// only the 32 columns cb .. cb + 31 of a column group (one 16-byte copy per thread)
+template <int NJ = 4>
 __device__ __forceinline__ void predict16_load_stage(double* as, double* bs, const double* Ag, const double* Bg,
                                                      int np, unsigned long long pol_last,
-                                                     unsigned long long pol_first) {
+                                                     unsigned long long pol_first, int cb = 0) {
     constexpr int STR = PSTR_DMMA, BK = PBK_DMMA;
+    static_assert(NJ == 4 || BK * 16 == P16_NT, "one column-group copy per thread");
     const int tid = threadIdx.x;
 #pragma unroll
     for (int t = 0; t < BK * 64 / P16_NT; ++t) {
         const int q = tid + t * P16_NT;
         const int kk = q >> 6, m2 = (q & 63) * 2;
         cp_async16_cg_hint(as + kk * STR + m2, Ag + (size_t)kk * np + m2, pol_last);
+        if constexpr (NJ == 4) cp_async16_cg_hint(bs + kk * STR + m2, Bg + kk * PBN + m2, pol_first);
+    }
+    if constexpr (NJ == 1) {
+        const int kk = tid >> 4, m2 = cb + (tid & 15) * 2;
         cp_async16_cg_hint(bs + kk * STR + m2, Bg + kk * PBN + m2, pol_first);
     }
 }
@@ -841,11 +850,17 @@ __device__ __forceinline__ void predict16_load_stage(double* as, double* bs, con
 // squares of its 4 rows, per column) to part[ib][wm][g][column], and the tile's finisher adds them in this function's
 // order (unit_finish_colsq).  PART = false with `pre` (predict_refine_kernel): every thread also stores its running
 // sums before the xor tree to pre[wm * 8 + g][column], the prefix a later pass carries on from row block ib1.
-template <int MMA, bool PART>
+// NJ = 1 (PART only): the column group cg, columns cg * 32 .. cg * 32 + 31, alone.  Warp (wn, wm) then takes the n8 tile
+// wn of the group (the tile j = wn of the unsplit warp wn' = cg) over the same row slab wm: the same fragments, the same
+// MMAs in the same k order and the same s(ib) for every (wm, g, column) it covers, so the group's part entries are
+// the unsplit ones bit for bit; four such units make up the whole part image.
+template <int MMA, bool PART, int NJ = 4>
 __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* __restrict__ Ks, double* smem,
                                                   unsigned long long pol_last, unsigned long long pol_first, int ib0,
-                                                  int ib1, double* __restrict__ part, double* pre = nullptr) {
+                                                  int ib1, double* __restrict__ part, double* pre = nullptr,
+                                                  int cg = 0) {
     static_assert(MMA == 884 || MMA == 1684, "phase B shape");
+    static_assert(NJ == 4 || (NJ == 1 && PART && MMA == 1684), "column groups: the units' m16n8k4 phase B");
     constexpr int STR = PSTR_DMMA, BK = PBK_DMMA;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // the four warps of an SM sub-partition (equal warp & 3) own the four different row slabs, so skipping the
@@ -853,25 +868,26 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
     const int wn = warp >> 2;
     const int wm = (warp + wn) & 3;
     const int g = lane >> 2, t4 = lane & 3;
+    const int wc = NJ == 4 ? wn * 32 : cg * 32 + wn * 8;  // first column of the warp's NJ n8 tiles
     const int np = G.np;
     double* As = smem;
     double* Bs = smem + PSTAGES * BK * STR;
-    double csq[4][2];
+    double csq[NJ][2];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) csq[j][0] = csq[j][1] = 0.0;
+    for (int j = 0; j < NJ; ++j) csq[j][0] = csq[j][1] = 0.0;
     for (int ib = ib0; ib < ib1; ++ib) {
-        double acc[4][4][2];
+        double acc[4][NJ][2];
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
-            for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
+            for (int j = 0; j < NJ; ++j) acc[i][j][0] = acc[i][j][1] = 0.0;
         const int nks = (ib + 1) * (PBM / BK);
         const double* Abase = G.linvT + (size_t)ib * PBM;
 #pragma unroll
         for (int s = 0; s < PSTAGES - 1; ++s) {
             if (s < nks)
-                predict16_load_stage(As + s * BK * STR, Bs + s * BK * STR, Abase + (size_t)(s * BK) * np,
-                                     Ks + (size_t)(s * BK) * PBN, np, pol_last, pol_first);
+                predict16_load_stage<NJ>(As + s * BK * STR, Bs + s * BK * STR, Abase + (size_t)(s * BK) * np,
+                                         Ks + (size_t)(s * BK) * PBN, np, pol_last, pol_first, cg * 32);
             cp_async_commit();
         }
         for (int ks = 0; ks < nks; ++ks) {
@@ -880,35 +896,35 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
             const int nxt = ks + PSTAGES - 1;
             const bool live = ks * BK < ib * PBM + (wm + 1) * 32;
             const double* as = As + (ks % PSTAGES) * BK * STR + wm * 32 + g;
-            const double* bs = Bs + (ks % PSTAGES) * BK * STR + wn * 32 + g;
+            const double* bs = Bs + (ks % PSTAGES) * BK * STR + wc + g;
 #pragma unroll
             for (int k4 = 0; k4 < BK / 4; ++k4) {
                 if (k4 == 1) {
                     if (nxt < nks)
-                        predict16_load_stage(As + (nxt % PSTAGES) * BK * STR, Bs + (nxt % PSTAGES) * BK * STR,
-                                             Abase + (size_t)(nxt * BK) * np, Ks + (size_t)(nxt * BK) * PBN, np,
-                                             pol_last, pol_first);
+                        predict16_load_stage<NJ>(As + (nxt % PSTAGES) * BK * STR, Bs + (nxt % PSTAGES) * BK * STR,
+                                                 Abase + (size_t)(nxt * BK) * np, Ks + (size_t)(nxt * BK) * PBN, np,
+                                                 pol_last, pol_first, cg * 32);
                     cp_async_commit();
                 }
                 if (live) {
-                    double a[4], b[4];
+                    double a[4], b[NJ];
                     const int krow = (k4 * 4 + t4) * STR;
 #pragma unroll
                     for (int i = 0; i < 4; ++i) a[i] = as[krow + i * 8];
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) b[j] = bs[krow + j * 8];
+                    for (int j = 0; j < NJ; ++j) b[j] = bs[krow + j * 8];
                     if constexpr (MMA == 1684) {
 #pragma unroll
                         for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
-                            for (int j = 0; j < 4; ++j)
+                            for (int j = 0; j < NJ; ++j)
                                 dmma1684(acc[2 * mi][j][0], acc[2 * mi][j][1], acc[2 * mi + 1][j][0],
                                          acc[2 * mi + 1][j][1], a[2 * mi], a[2 * mi + 1], b[j]);
                     } else {
 #pragma unroll
                         for (int i = 0; i < 4; ++i)
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
+                            for (int j = 0; j < NJ; ++j) dmma884(acc[i][j][0], acc[i][j][1], a[i], b[j]);
                     }
                 }
             }
@@ -916,7 +932,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
         cp_async_wait<0>();
         __syncthreads();
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < NJ; ++j) {
             double s0 = 0.0, s1 = 0.0;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
@@ -924,7 +940,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
                 s1 = fma(acc[i][j][1], acc[i][j][1], s1);
             }
             if constexpr (PART) {
-                double* q = part + ((size_t)(ib * 4 + wm) * 8 + g) * PBN + wn * 32 + j * 8 + t4 * 2;
+                double* q = part + ((size_t)(ib * 4 + wm) * 8 + g) * PBN + wc + j * 8 + t4 * 2;
                 *reinterpret_cast<double2*>(q) = make_double2(s0, s1);
             } else {
                 csq[j][0] += s0;
@@ -934,7 +950,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
     }
     if constexpr (PART) return;
 #pragma unroll
-    for (int j = 0; j < 4; ++j)
+    for (int j = 0; j < NJ; ++j)
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             double v = csq[j][e];
@@ -947,7 +963,7 @@ __device__ __forceinline__ void predict16_phase_b(const GpDev& G, const double* 
     double* red = smem;  // [4][PBN]: row slab wm, every column produced by exactly one warp
     if (g == 0) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < NJ; ++j) {
             red[wm * PBN + wn * 32 + j * 8 + t4 * 2] = csq[j][0];
             red[wm * PBN + wn * 32 + j * 8 + t4 * 2 + 1] = csq[j][1];
         }
@@ -1257,8 +1273,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
 // When more than kRefineMaxTiles tiles of survivors come up (little prunes: the refine stage stops claiming tiles as
 // soon as it sees that), the final stage does nothing and the tile kernel goes on in bound order behind the lead
 // tiles as it would have without these stages; otherwise the final stage closes the tile kernel's counter.
-// Exact values are bit-equal to the tile kernel's: K* entries carry no order, mu comes from the unit that runs phase A
-// over all np rows (the last group of a tile; the same function and order of sums as the tile kernel), and the sum of
+// Exact values are bit-equal to the tile kernel's: K* entries carry no order, mu comes from the one unit of a tile that
+// recomputes it from the K* slot over all np rows (the same function and order of sums as phase A), and the sum of
 // squares is added up by unit_finish_colsq in the order of predict16_phase_b.  No CTA waits for another: the
 // stages are kernel boundaries, and within predict_units_kernel the last unit to arrive at a tile's counter finishes it.
 constexpr int kLeadTiles = 8, kRefineMaxTiles = 128, kUnitSlots = kLeadTiles + kRefineMaxTiles;
@@ -1281,7 +1297,9 @@ struct RefineParams {
     double* part;            // [kUnitSlots][np / PBM][4][8][PBN] per-row-block partial sums of squares
     unsigned* arrive;        // [kUnitSlots] units that have delivered their part of a tile
     int blocks;              // leading row blocks of the refined bound
-    int groups_max;          // most units a tile is split into
+    int groups_max;          // most row-block groups a tile is split into
+    int colgroups;           // level and final stage: column groups per row-block group when the row-block groups of
+                             // the round's tiles cannot fill the grid (1: no column split)
     int final_stage;         // predict_units_kernel: kStageLead, kStageFinal or kStageLevel
     int b0, b1;              // the units' row blocks [b0, b1): the lead and the final stage end at np / PBM
     int n_word;              // final stage and level: the prune_ctl word counting their candidates
@@ -1330,10 +1348,10 @@ __device__ __forceinline__ bool unit_skip(const PredictParams& P, const RefinePa
 // into kCtlKth, when there are k entries, and a copy of that word into kCtlKthRound for the next final round.  It is
 // the k-th smallest of values already produced, so the final k-th key is <= it.  One warp: k rounds of a merge of the
 // list heads.
-__global__ void __launch_bounds__(32) merge_kth_kernel(const SelList* __restrict__ lists, int nlists, int k,
-                                                        unsigned long long* ctl) {
-    __shared__ int head[1024];
-    const int lane = threadIdx.x;
+// One warp (lane = threadIdx.x & 31); head: nlists ints of shared memory.
+__device__ __forceinline__ void merge_kth_run(const SelList* __restrict__ lists, int nlists, int k,
+                                              unsigned long long* ctl, int* head) {
+    const int lane = threadIdx.x & 31;
     for (int l = lane; l < nlists; l += 32) head[l] = 0;
     __syncwarp();
     unsigned long long kth = 0xFFFFFFFFFFFFFFFFull;
@@ -1369,6 +1387,12 @@ __global__ void __launch_bounds__(32) merge_kth_kernel(const SelList* __restrict
         if (full && kth < ctl[kCtlKth]) ctl[kCtlKth] = kth;
         ctl[kCtlKthRound] = ctl[kCtlKth];
     }
+}
+
+__global__ void __launch_bounds__(32) merge_kth_kernel(const SelList* __restrict__ lists, int nlists, int k,
+                                                        unsigned long long* ctl) {
+    __shared__ int head[1024];
+    merge_kth_run(lists, nlists, k, ctl, head);
 }
 
 // first row block of group j of G over the row blocks [b0, nb), cut so that the groups' k-tile counts (row block ib:
@@ -1457,9 +1481,8 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_refine_kernel(const Predict
 // scratch slot (tile - tbeg; a round has at most gridDim.x tiles), with phase_a's arithmetic: items (tile, chunks [ch0, ch1)), the
 // chunks of a tile cut so that there are about gridDim.x items.  Plain stores: every unit of the tile reads the slot.
 template <bool DREG>
-__global__ void __launch_bounds__(P16_NT, 1) ks_build_kernel(const PredictParams P, const RefineParams R) {
-    extern __shared__ __align__(16) double smem[];
-    __shared__ double mu_s[P16_SPLIT][PBN];
+__device__ __forceinline__ void ks_build_run(const PredictParams& P, const RefineParams& R, double* smem,
+                                             double (*mu_s)[PBN]) {
     const GpDev& G = P.gp[0];
     const UnitRound U = unit_round(P, R);
     const long long nt = U.tend - U.tbeg;
@@ -1476,6 +1499,13 @@ __global__ void __launch_bounds__(P16_NT, 1) ks_build_kernel(const PredictParams
     }
 }
 
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT, 1) ks_build_kernel(const PredictParams P, const RefineParams R) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    ks_build_run<DREG>(P, R, smem, mu_s);
+}
+
 // K* alpha_ of a tile from its K* slot, in phase_a's order: thread (part, column) runs one fma chain over the chunks in
 // ascending order, rows part * 16 .. part * 16 + 15 of each, so mu_s[part][c] is phase A's bit for bit.
 __device__ __forceinline__ void unit_mu_from_ks(const GpDev& G, const double* __restrict__ Ks,
@@ -1490,59 +1520,97 @@ __device__ __forceinline__ void unit_mu_from_ks(const GpDev& G, const double* __
     mu_s[part][c] = mu;
 }
 
-// Exact evaluation in units of (tile, group of consecutive row blocks of [b0, b1)).  Lead stage: the tiles are the
-// first kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this launch (a
-// continued batch; read from kCtlKthLead, which does not move, so that all units of a tile decide alike).  Final
-// stage: the tiles [t0, t1) of the survivor list, each skipped when its first key is above kCtlKthRound.  The level:
-// the tiles [t0, t1) of its survivor list, none skipped.  A unit reads the tile's K* from the slot that
-// ks_build_kernel filled (the unit of the last group computes mu from it), runs phase B over its row blocks, and the
-// last unit to arrive finishes the tile: from the survivors' carried prefix on, as the tile kernel's epilogue does
-// (lead, final), or as the refine stage keys its candidates at b1 row blocks (the level).
-__global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictParams P, const RefineParams R) {
-    extern __shared__ __align__(16) double smem[];
-    __shared__ double mu_s[P16_SPLIT][PBN];
-    __shared__ SelShared sel_s;
+// k-tile groups of row-block group j of G over [b0, nb) (unit_cut): sum of ib + 1 over its row blocks
+__host__ __device__ inline long long unit_cost(int b0, int nb, int G, int j) {
+    const long long a = unit_cut(b0, nb, G, j), b = unit_cut(b0, nb, G, j + 1);
+    return (b * (b + 1) - a * (a + 1)) / 2;
+}
+
+// Exact evaluation in units of (tile, group of consecutive row blocks of [b0, b1), column group).  Lead stage: the
+// tiles are the first kLeadTiles of P.perm, each skipped when its best bound key is above the k-th key carried into this
+// launch (a continued batch; read from kCtlKthLead, which does not move, so that all units of a tile decide alike).
+// Final stage: the tiles [t0, t1) of the survivor list, each skipped when its first key is above kCtlKthRound.  The
+// level: the tiles [t0, t1) of its survivor list, none skipped.  The level and the final rounds cut [b0, b1) into up to
+// one row block per group (at most 32 groups, about 2 * gridDim.x units) and split every row-block group into
+// R.colgroups column groups of 32 columns when their tiles' row-block groups alone cannot fill the grid.  At C3 the
+// final round has 2 tiles over row blocks [8, 32): 24 groups of 4 column groups, the heaviest unit a quarter of the
+// last row block (8 of its 32 k-tiles) where 16 whole-column groups made a group of two row blocks, 59 k-tiles, the
+// round's latency.  The part image and the arrival count are the same either way.  Units are claimed row-block
+// group descending (the single large row blocks first), tiles innermost.  A unit reads the tile's K* from the
+// slot that ks_build_kernel filled, runs phase B over its row blocks and columns, and the last unit to arrive finishes
+// the tile: from the survivors' carried prefix on, as the tile kernel's epilogue does (lead, final), or as the refine
+// stage keys its candidates at b1 row blocks (the level).  In the lead and the final stage the first column group of the
+// row-block group with the fewest k-tiles (an empty one if any) also computes the tile's mu from the slot.
+// The units of one launch or round, between the CTA's runsel_begin and runsel_store (sel_s: its running list).
+__device__ __forceinline__ void units_run(const PredictParams& P, const RefineParams& R, double* smem,
+                                          double (*mu_s)[PBN], SelShared& sel_s) {
     __shared__ long long unit_s;
-    __shared__ int last_s;
+    __shared__ int last_s, mu_grp_s;
     const int tid = threadIdx.x;
     const GpDev& G = P.gp[0];
     const int nb = G.np / PBM;
     const unsigned long long pol_last = l2_policy_evict_last(P.linv_l2_last);
-    if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
-    __syncthreads();
     const UnitRound U = unit_round(P, R);
     const int* list = U.list;
-    const long long n = U.n;
+    const long long n = U.n, nt = U.tend - U.tbeg;
     unsigned long long* claim = P.prune_ctl + (R.final_stage ? kCtlUnitFinal : kCtlUnit);
     const int b0 = R.b0, b1 = R.b1;
-    int groups = R.groups_max;
-    if (R.final_stage != kStageLead && U.tend > U.tbeg)
-        groups = (int)max(1ll, min((long long)min(R.groups_max, b1 - b0), 2ll * gridDim.x / (U.tend - U.tbeg)));
+    int groups = R.groups_max, cgs = 1;
+    if (R.final_stage != kStageLead && nt > 0) {
+        const int gmax = min(32, b1 - b0);  // up to one row block per group
+        if (nt * gmax < 2ll * gridDim.x) cgs = R.colgroups;
+        groups = (int)max(1ll, min((long long)gmax, 2ll * gridDim.x / (nt * cgs)));
+    }
+    if (tid < 32) {  // the row-block group with the fewest k-tiles, the lowest such on ties
+        long long c = tid < groups ? unit_cost(b0, b1, groups, tid) : 0x7FFFFFFFFFFFFFFFll;
+        int j = tid;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const long long oc = __shfl_xor_sync(0xffffffffu, c, o);
+            const int oj = __shfl_xor_sync(0xffffffffu, j, o);
+            if (oc < c || (oc == c && oj < j)) {
+                c = oc;
+                j = oj;
+            }
+        }
+        if (tid == 0) mu_grp_s = j;
+    }
+    __syncthreads();
+    const int mu_grp = R.final_stage == kStageLevel ? -1 : mu_grp_s;  // the level keys from the stored mu interval
+    const long long units = nt * groups * cgs;
     for (;;) {
         if (tid == 0) unit_s = (long long)atomicAdd(claim, 1ull);
         __syncthreads();
         const long long unit = unit_s;
-        const long long tile = U.tbeg + unit / groups;
-        if (tile >= U.tend) break;
+        if (unit >= units) break;
+        const long long tile = U.tbeg + unit % nt, r = unit / nt;
         const long long c0 = tile * PBN;
         if (unit_skip(P, R, tile)) {
             __syncthreads();
             continue;
         }
-        const int grp = (int)(unit - (tile - U.tbeg) * groups);
+        const int grp = groups - 1 - (int)(r / cgs), cg = (int)(r % cgs);
         const int ib0 = unit_cut(b0, b1, groups, grp), ib1 = unit_cut(b0, b1, groups, grp + 1);
         const int slot = U.slot0 + (int)tile;
         double* part = R.part + (size_t)slot * nb * 32 * PBN;
+        const double* Ks = P.scratch + (tile - U.tbeg) * P.scratch_stride;
+        const bool mu_unit = grp == mu_grp && cg == 0;
+        if (mu_unit) unit_mu_from_ks(G, Ks, mu_s);
         if (ib1 > ib0) {
-            const double* Ks = P.scratch + (tile - U.tbeg) * P.scratch_stride;
-            if (ib1 == nb) unit_mu_from_ks(G, Ks, mu_s);
-            predict16_phase_b<1684, true>(G, Ks, smem, pol_last, l2_policy_evict_last(0.f), ib0, ib1, part);
-            if (ib1 == nb && tid < PBN)  // mu_s holds the tile kernel's K* alpha_ parts (phase A over all np rows)
+            if (cgs == 1)
+                predict16_phase_b<1684, true>(G, Ks, smem, pol_last, l2_policy_evict_last(0.f), ib0, ib1, part);
+            else
+                predict16_phase_b<1684, true, 1>(G, Ks, smem, pol_last, l2_policy_evict_last(0.f), ib0, ib1, part,
+                                                 nullptr, cg);
+        }
+        if (mu_unit) {  // mu_s holds the tile kernel's K* alpha_ parts (phase A over all np rows)
+            __syncthreads();
+            if (tid < PBN)
                 R.mu_unit[(size_t)slot * PBN + tid] = ((mu_s[0][tid] + mu_s[1][tid]) + mu_s[2][tid]) + mu_s[3][tid];
         }
         __threadfence();  // this unit's partials and mu before its arrival
         __syncthreads();
-        if (tid == 0) last_s = atomicAdd(R.arrive + slot, 1u) == (unsigned)groups - 1;
+        if (tid == 0) last_s = atomicAdd(R.arrive + slot, 1u) == (unsigned)(groups * cgs) - 1;
         __syncthreads();
         if (last_s) {
             __threadfence();
@@ -1585,7 +1653,60 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
         }
         __syncthreads();
     }
+}
+
+__global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictParams P, const RefineParams R) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    __shared__ SelShared sel_s;
+    const int tid = threadIdx.x;
+    if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
+    units_run(P, R, smem, mu_s, sel_s);
     if (tid < PBN) runsel_store(sel_s, P.sel_cta + blockIdx.x, tid);
+}
+
+// The rounds of the final stage in one cooperative launch (one CTA per SM, every CTA resident): per round the K*
+// build, a grid barrier, the units, a grid barrier, the merge of the k-th key by CTA 0 (which also resets the units'
+// claim counter), and a grid barrier.  The same work and arithmetic as ks_build_kernel, predict_units_kernel and
+// merge_kth_kernel launched round by round, without their launches: a round with no tiles left (at C3 the second)
+// costs its barriers only, and once the rounds are past the survivors every CTA leaves together (the survivor count
+// does not move during the stage, so all CTAs decide alike).  rt[0 .. nr]: the rounds' first tiles, then the end.
+struct FinalRounds {
+    static constexpr int kMax = 8;
+    int nr;
+    int rt[kMax + 1];
+};
+
+template <bool DREG>
+__global__ void __launch_bounds__(P16_NT, 1) final_rounds_kernel(const PredictParams P, RefineParams R,
+                                                                 const FinalRounds F) {
+    extern __shared__ __align__(16) double smem[];
+    __shared__ double mu_s[P16_SPLIT][PBN];
+    __shared__ SelShared sel_s;
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    const int tid = threadIdx.x;
+    if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
+    __syncthreads();
+    for (int r = 0; r < F.nr; ++r) {
+        R.t0 = F.rt[r];
+        R.t1 = F.rt[r + 1];
+        const UnitRound U = unit_round(P, R);
+        if (U.tbeg >= (U.n + PBN - 1) / PBN) break;  // this and every later round has no tile
+        ks_build_run<DREG>(P, R, smem, mu_s);
+        __threadfence();
+        grid.sync();
+        units_run(P, R, smem, mu_s, sel_s);
+        if (tid < PBN) runsel_store(sel_s, P.sel_cta + blockIdx.x, tid);
+        __threadfence();
+        grid.sync();
+        if (blockIdx.x == 0 && tid < 32) {
+            merge_kth_run(P.sel_cta, gridDim.x, P.sel_k, P.prune_ctl, reinterpret_cast<int*>(smem));
+            if (tid == 0) P.prune_ctl[kCtlUnitFinal] = 0ull;
+            __threadfence();
+        }
+        grid.sync();
+    }
 }
 
 }  // namespace b200bo
