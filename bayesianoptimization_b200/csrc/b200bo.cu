@@ -186,8 +186,7 @@ struct b200bo_gp {
     // at ev0 and the tile kernel ends at ev1)
     cudaEvent_t ev_stage[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool stage_timed = false, stage_refined = false;
-    int stage_levels = 0;  // refine levels of the last pruned launch
-    int coop_final[2] = {-1, -1};  // final_rounds_coop per DREG: -1 not yet checked, 0 launch by launch, 1 cooperative
+    int coop_final[2] = {-1, -1};  // final_rounds_coop per DREG: -1 not yet checked, 0 no, 1 yes
     DevBuf pbounds, prow;   // throughput mode: Philox bounds (lo, span) / regenerated winner rows
     bool replica = false;   // predict-only copy made by b200bo_gp_replicate
     // look-ahead Cholesky: bulk stream, chain/bulk events, copy of the next diagonal step's panel block
@@ -1665,13 +1664,6 @@ static int prune_refine_blocks(int np, long long ntiles) {
     return b < nb / 8 ? b : nb / 8;
 }
 
-// Column groups per row-block group of the level's and the final rounds' units (DESIGN.md 4.9): 4 (32 columns each)
-// unless B200BO_PRUNE_COLSPLIT=0 (read per call, for A/B measurements) keeps every unit on all 128 columns
-static int prune_colgroups() {
-    const char* e = getenv("B200BO_PRUNE_COLSPLIT");
-    return e && e[0] == '0' ? 1 : 4;
-}
-
 // survivors of the level in key order (sorted slots pos): their local indices and carried prefixes
 __global__ void level_gather_kernel(const unsigned long long* __restrict__ ctl, int n_word, const int* __restrict__ pos,
                                     const int* __restrict__ idx, const double* __restrict__ pre, int* __restrict__ idx_out,
@@ -1689,20 +1681,13 @@ __global__ void level_gather_kernel(const unsigned long long* __restrict__ ctl, 
 // the k-th key carried into the launch
 __global__ void prune_ctl_refine_kernel(unsigned long long* ctl) {
     ctl[kCtlTile] = ctl[kCtlRefTile] = kLeadTiles;
-    ctl[kCtlSurv] = ctl[kCtlUnit] = ctl[kCtlUnitFinal] = 0ull;
-    for (int l = 0; l < kPruneMaxLevels; ++l) ctl[kCtlLevel + l] = 0ull;
+    ctl[kCtlSurv] = ctl[kCtlUnit] = ctl[kCtlLevel] = 0ull;
     ctl[kCtlKthLead] = ctl[kCtlKth];
 }
 
-// Tiles of the final rounds: 8, then the rest of the kRefineMaxTiles (at C3 the level leaves 1.6 tiles), at most
-// `grid` each (a round's K* slots)
-static int final_round_tiles(int r, int t0, int grid) {
-    const int t = r == 0 ? 8 : kRefineMaxTiles - t0;
-    return t < grid ? t : grid;
-}
-
-// Whether the final rounds run as one cooperative launch (final_rounds_kernel): the device supports it and `grid`
-// CTAs of 512 threads with the phase B shared memory are co-resident (one per SM).  Checked once per handle.
+// Whether the final rounds can run (final_rounds_kernel, a cooperative launch): the device supports cooperative
+// launches and `grid` CTAs of 512 threads with the phase B shared memory are co-resident (one per SM).  Checked once
+// per handle; without it a call takes no refine stages.
 static bool final_rounds_coop(b200bo_gp* g0, bool dreg, int grid) {
     int& ok = g0->coop_final[dreg ? 1 : 0];
     if (ok < 0) {
@@ -1722,7 +1707,8 @@ static bool final_rounds_coop(b200bo_gp* g0, bool dreg, int grid) {
 // kernel.  ks_build_kernel builds the K* of a stage's or round's tiles once, before its units.  The refine stage
 // stores every survivor's prefix, the level carries it on over row blocks [b, 2b) and passes its survivors on, and
 // the final stage starts from row block 2b in rounds over those survivors sorted by key, skipping the tiles above the
-// key.  merge_kth_kernel tightens the k-th key after the lead stage and after every final round.
+// key, in one cooperative launch (the caller has checked final_rounds_coop).  The k-th key is merged after the lead
+// stage and after every final round.
 static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg, int blocks, bool resume,
                                cudaStream_t stream) {
     const int nb = P.gp[0].np / PBM, grid = g0->sm_count;
@@ -1762,7 +1748,6 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     R.arrive = g0->prune_arrive.as<unsigned>();
     R.blocks = blocks;
     R.groups_max = nb / 2 < 32 ? nb / 2 : 32;
-    R.colgroups = prune_colgroups();
     R.final_stage = kStageLead;
     R.b0 = 0;
     R.b1 = nb;
@@ -1803,13 +1788,12 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     for (int t0 = 0; t0 < kRefineMaxTiles; t0 = R.t1) {
         R.t0 = t0;
         R.t1 = t0 + grid < kRefineMaxTiles ? t0 + grid : kRefineMaxTiles;
-        CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
+        CU(cudaMemsetAsync(ctl + kCtlUnit, 0, sizeof(unsigned long long), stream));
         build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
         LAUNCHED();
         predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
         LAUNCHED();
     }
-    g0->stage_levels = 1;
     CU(cudaEventRecord(g0->ev_stage[5], stream));
     // the level's survivors ascending by key (the sentinels of the unused slots last), sorted with their slots, then
     // their indices and prefixes gathered into list A in that order
@@ -1825,35 +1809,11 @@ static int prune_refine_stages(b200bo_gp* g0, const PredictParams& P, bool dreg,
     R.surv = lidx[0];
     R.surv_key = lk.Current();
     R.prefix = lpre[0];
-    FinalRounds F = {};  // the rounds' tiles; more than kMax rounds (a grid under 18 SMs) launch by launch
-    bool few = true;
-    for (int t0 = 0; t0 < kRefineMaxTiles && few; ++F.nr) {
-        few = F.nr < FinalRounds::kMax;
-        if (!few) break;
-        F.rt[F.nr] = t0;
-        t0 += final_round_tiles(F.nr, t0, grid);
-        F.rt[F.nr + 1] = t0;
-    }
-    CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
-    if (few && final_rounds_coop(g0, dreg, grid)) {
-        void* args[] = {(void*)&Q, (void*)&R, (void*)&F};
-        CU(cudaLaunchCooperativeKernel(dreg ? (const void*)final_rounds_kernel<true> : (const void*)final_rounds_kernel<false>,
-                                       dim3(grid), dim3(P16_NT), args, kPredictSmemBytesDmma, stream));
-        LAUNCHED();
-    } else {  // the grid cannot be co-resident (or too many rounds): the rounds launch by launch
-        for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r) {
-            R.t0 = t0;
-            R.t1 = t0 + final_round_tiles(r, t0, grid);
-            if (r > 0) CU(cudaMemsetAsync(ctl + kCtlUnitFinal, 0, sizeof(unsigned long long), stream));
-            build<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-            LAUNCHED();
-            predict_units_kernel<<<grid, P16_NT, kPredictSmemBytesDmma, stream>>>(Q, R);
-            LAUNCHED();
-            merge_kth_kernel<<<1, 32, 0, stream>>>(lists, grid, P.sel_k, ctl);
-            LAUNCHED();
-            t0 = R.t1;
-        }
-    }
+    CU(cudaMemsetAsync(ctl + kCtlUnit, 0, sizeof(unsigned long long), stream));
+    void* args[] = {(void*)&Q, (void*)&R};
+    CU(cudaLaunchCooperativeKernel(dreg ? (const void*)final_rounds_kernel<true> : (const void*)final_rounds_kernel<false>,
+                                   dim3(grid), dim3(P16_NT), args, kPredictSmemBytesDmma, stream));
+    LAUNCHED();
     CU(cudaGetLastError());
     CU(cudaEventRecord(g0->ev_stage[4], stream));
     return B200BO_OK;
@@ -2420,9 +2380,10 @@ static int eval_launch(const b200bo_acq* spec, const CandSrc& src, int64_t m, do
             prune = fused_sel && !P.acq_out && !P.mu_out && !P.sd_out && P.n_gps == 1 && pipe != PIPE_BULK_MC &&
                     acq_prunable(spec->kind) && m <= std::numeric_limits<int>::max() && prune_enabled();
             if (prune && (rc = prune_prepare(g0, P, sm.resume, stream))) return rc;
-            const int refine = prune && predict_mma() == 1684 ? prune_refine_blocks(P.gp[0].np, ntiles) : 0;
+            const int refine = prune && predict_mma() == 1684 && final_rounds_coop(g0, dreg, g0->sm_count)
+                                   ? prune_refine_blocks(P.gp[0].np, ntiles)
+                                   : 0;
             g0->stage_refined = refine > 0;
-            g0->stage_levels = 0;
             if (refine) {
                 // every SM keeps a list, begun by the lead stage and continued by the final stage and the tile kernel
                 grid = g0->sm_count;
@@ -2641,14 +2602,14 @@ extern "C" int b200bo_last_prune_levels(float* ms, int64_t* passed, int* levels)
     CU(cudaSetDevice(g0->device));
     CU(cudaEventSynchronize(g0->ev1));
     *ms = 0.f;
-    *levels = g0->stage_refined ? g0->stage_levels : 0;
-    for (int l = 0; l <= kPruneMaxLevels; ++l) passed[l] = 0;
+    *levels = g0->stage_refined ? 1 : 0;
+    for (int l = 0; l < 5; ++l) passed[l] = 0;
     if (!g0->stage_refined) return B200BO_OK;
     CU(cudaEventElapsedTime(ms, g0->ev_stage[3], g0->ev_stage[5]));
     unsigned long long w[kCtlWords];
     CU(cudaMemcpy(w, g0->prune_ctl.as<unsigned long long>(), sizeof(w), cudaMemcpyDeviceToHost));
     passed[0] = (int64_t)w[kCtlSurv];
-    for (int l = 0; l < *levels; ++l) passed[l + 1] = (int64_t)w[kCtlLevel + l];
+    passed[1] = (int64_t)w[kCtlLevel];
     return B200BO_OK;
 }
 

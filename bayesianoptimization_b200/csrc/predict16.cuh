@@ -793,13 +793,11 @@ enum {
     kCtlRefTile = 3,  // next tile of the refine stage, in bound order
     kCtlSurv = 4,     // candidates the refine stage let through
     kCtlRefined = 5,  // candidates the refine stage looked at
-    kCtlUnit = 6,     // next unit of predict_units_kernel in the lead stage
-    kCtlKthLead = 7,  // the k-th key as it was before the lead stage
-    kCtlUnitFinal = 8,  // the same for the current final round
-    kCtlKthRound = 9,   // the k-th key as it was before the current final round (written by merge_kth_kernel)
-    kCtlLevel = 10,     // [kPruneMaxLevels] candidates each refine level let through
-    kPruneMaxLevels = 4,
-    kCtlWords = kCtlLevel + kPruneMaxLevels
+    kCtlUnit = 6,      // next unit of the lead stage, the current level launch or the current final round
+    kCtlKthLead = 7,   // the k-th key as it was before the lead stage
+    kCtlKthRound = 8,  // the k-th key as it was before the current final round (written by merge_kth_run)
+    kCtlLevel = 9,     // candidates the refine level let through
+    kCtlWords = 10
 };
 
 // Prune mode of predict_acq16_kernel: thread 0 claims the next tile in bound order and stops the CTA (returns ntiles)
@@ -1268,16 +1266,24 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_acq16_kernel(const PredictP
 //   level   predict_units_kernel over row blocks [b, 2b) of the survivors only: the last unit of a tile carries each
 //           survivor's prefix on to 2b, keys it as the refine stage does and appends the survivors whose keys are all
 //           <= the k-th key, with the new prefix, to the level's list;
-//   final   the level's survivors sorted by key through predict_units_kernel, from the carried prefix on, in rounds
-//           that each skip the tiles above the k-th key merged before them.
+//   final   the level's survivors sorted by key through the same units (final_rounds_kernel), from the carried prefix
+//           on, in rounds that each skip the tiles above the k-th key merged before them.
 // When more than kRefineMaxTiles tiles of survivors come up (little prunes: the refine stage stops claiming tiles as
 // soon as it sees that), the final stage does nothing and the tile kernel goes on in bound order behind the lead
 // tiles as it would have without these stages; otherwise the final stage closes the tile kernel's counter.
 // Exact values are bit-equal to the tile kernel's: K* entries carry no order, mu comes from the one unit of a tile that
 // recomputes it from the K* slot over all np rows (the same function and order of sums as phase A), and the sum of
-// squares is added up by unit_finish_colsq in the order of predict16_phase_b.  No CTA waits for another: the
-// stages are kernel boundaries, and within predict_units_kernel the last unit to arrive at a tile's counter finishes it.
+// squares is added up by unit_finish_colsq in the order of predict16_phase_b.  The stages are kernel boundaries, the
+// steps of a final round grid barriers, and within the units the last unit to arrive at a tile's counter finishes it.
 constexpr int kLeadTiles = 8, kRefineMaxTiles = 128, kUnitSlots = kLeadTiles + kRefineMaxTiles;
+
+// Tiles of final round r from tile t0 on: 8, then the rest of the kRefineMaxTiles (at C3 the level leaves 1.6 tiles),
+// at most `grid` each (a round's K* slots)
+__host__ __device__ inline int final_round_tiles(int r, int t0, int grid) {
+    const int t = r == 0 ? 8 : kRefineMaxTiles - t0;
+    return t < grid ? t : grid;
+}
+
 constexpr long long kCtlClosed = 1ll << 40;  // value of kCtlTile no batch reaches
 
 enum { kStageLead = 0, kStageFinal = 1, kStageLevel = 2 };
@@ -1298,14 +1304,16 @@ struct RefineParams {
     unsigned* arrive;        // [kUnitSlots] units that have delivered their part of a tile
     int blocks;              // leading row blocks of the refined bound
     int groups_max;          // most row-block groups a tile is split into
-    int colgroups;           // level and final stage: column groups per row-block group when the row-block groups of
-                             // the round's tiles cannot fill the grid (1: no column split)
     int final_stage;         // predict_units_kernel: kStageLead, kStageFinal or kStageLevel
     int b0, b1;              // the units' row blocks [b0, b1): the lead and the final stage end at np / PBM
     int n_word;              // final stage and level: the prune_ctl word counting their candidates
     int out_word;            // the level: the prune_ctl word counting the candidates it lets through
     int t0, t1;              // final stage and level: the round's tiles [t0, t1) of the survivor list
 };
+
+// column groups of 32 columns per row-block group of a level or final round whose row-block groups alone cannot fill
+// the grid
+constexpr int kUnitColGroups = 4;
 
 // The tiles of a lead stage, level launch or final round, the same in every CTA: candidates list[0, n), tiles
 // [tbeg, tend) of PBN columns, partial-sum slots from slot0.  Level and final stage: too many refine survivors leave
@@ -1532,7 +1540,7 @@ __host__ __device__ inline long long unit_cost(int b0, int nb, int G, int j) {
 // Final stage: the tiles [t0, t1) of the survivor list, each skipped when its first key is above kCtlKthRound.  The
 // level: the tiles [t0, t1) of its survivor list, none skipped.  The level and the final rounds cut [b0, b1) into up to
 // one row block per group (at most 32 groups, about 2 * gridDim.x units) and split every row-block group into
-// R.colgroups column groups of 32 columns when their tiles' row-block groups alone cannot fill the grid.  At C3 the
+// kUnitColGroups column groups of 32 columns when their tiles' row-block groups alone cannot fill the grid.  At C3 the
 // final round has 2 tiles over row blocks [8, 32): 24 groups of 4 column groups, the heaviest unit a quarter of the
 // last row block (8 of its 32 k-tiles) where 16 whole-column groups made a group of two row blocks, 59 k-tiles, the
 // round's latency.  The part image and the arrival count are the same either way.  Units are claimed row-block
@@ -1553,12 +1561,12 @@ __device__ __forceinline__ void units_run(const PredictParams& P, const RefinePa
     const UnitRound U = unit_round(P, R);
     const int* list = U.list;
     const long long n = U.n, nt = U.tend - U.tbeg;
-    unsigned long long* claim = P.prune_ctl + (R.final_stage ? kCtlUnitFinal : kCtlUnit);
+    unsigned long long* claim = P.prune_ctl + kCtlUnit;
     const int b0 = R.b0, b1 = R.b1;
     int groups = R.groups_max, cgs = 1;
     if (R.final_stage != kStageLead && nt > 0) {
         const int gmax = min(32, b1 - b0);  // up to one row block per group
-        if (nt * gmax < 2ll * gridDim.x) cgs = R.colgroups;
+        if (nt * gmax < 2ll * gridDim.x) cgs = kUnitColGroups;
         groups = (int)max(1ll, min((long long)gmax, 2ll * gridDim.x / (nt * cgs)));
     }
     if (tid < 32) {  // the row-block group with the fewest k-tiles, the lowest such on ties
@@ -1670,16 +1678,10 @@ __global__ void __launch_bounds__(P16_NT, 1) predict_units_kernel(const PredictP
 // claim counter), and a grid barrier.  The same work and arithmetic as ks_build_kernel, predict_units_kernel and
 // merge_kth_kernel launched round by round, without their launches: a round with no tiles left (at C3 the second)
 // costs its barriers only, and once the rounds are past the survivors every CTA leaves together (the survivor count
-// does not move during the stage, so all CTAs decide alike).  rt[0 .. nr]: the rounds' first tiles, then the end.
-struct FinalRounds {
-    static constexpr int kMax = 8;
-    int nr;
-    int rt[kMax + 1];
-};
-
+// does not move during the stage, so all CTAs decide alike).  The rounds' tiles come from final_round_tiles, so any
+// grid size runs in this one launch.
 template <bool DREG>
-__global__ void __launch_bounds__(P16_NT, 1) final_rounds_kernel(const PredictParams P, RefineParams R,
-                                                                 const FinalRounds F) {
+__global__ void __launch_bounds__(P16_NT, 1) final_rounds_kernel(const PredictParams P, RefineParams R) {
     extern __shared__ __align__(16) double smem[];
     __shared__ double mu_s[P16_SPLIT][PBN];
     __shared__ SelShared sel_s;
@@ -1688,9 +1690,9 @@ __global__ void __launch_bounds__(P16_NT, 1) final_rounds_kernel(const PredictPa
     const int tid = threadIdx.x;
     if (tid < PBN) runsel_begin(sel_s, P.sel_cta + blockIdx.x, P.sel_resume, tid);
     __syncthreads();
-    for (int r = 0; r < F.nr; ++r) {
-        R.t0 = F.rt[r];
-        R.t1 = F.rt[r + 1];
+    for (int r = 0, t0 = 0; t0 < kRefineMaxTiles; ++r, t0 = R.t1) {
+        R.t0 = t0;
+        R.t1 = t0 + final_round_tiles(r, t0, gridDim.x);
         const UnitRound U = unit_round(P, R);
         if (U.tbeg >= (U.n + PBN - 1) / PBN) break;  // this and every later round has no tile
         ks_build_run<DREG>(P, R, smem, mu_s);
@@ -1702,7 +1704,7 @@ __global__ void __launch_bounds__(P16_NT, 1) final_rounds_kernel(const PredictPa
         grid.sync();
         if (blockIdx.x == 0 && tid < 32) {
             merge_kth_run(P.sel_cta, gridDim.x, P.sel_k, P.prune_ctl, reinterpret_cast<int*>(smem));
-            if (tid == 0) P.prune_ctl[kCtlUnitFinal] = 0ull;
+            if (tid == 0) P.prune_ctl[kCtlUnit] = 0ull;
             __threadfence();
         }
         grid.sync();

@@ -45,7 +45,7 @@ def level_ends(b, nb):
 
 
 def final_round_tiles(r, t0, grid):
-    """final_round_tiles of b200bo.cu: 8, then the rest, at most grid each"""
+    """final_round_tiles of predict16.cuh: 8, then the rest, at most grid each"""
     return min(8 if r == 0 else K_REFINE_MAX_TILES - t0, grid)
 
 
@@ -133,6 +133,9 @@ def test_level_schedule(nb):
 # SM counts: below, at and around the first round of 8 and the 120 tiles after it, the H100 PCIe (114) and SXM (132)
 @pytest.mark.parametrize("grid", [1, 7, 8, 9, 64, 114, 119, 120, 121, 127, 128, 132])
 def test_round_schedule(grid):
+    """The final stage's rounds as final_rounds_kernel (predict16.cuh) loops over them: t0 from 0 while t0 <
+    kRefineMaxTiles, t1 = t0 + final_round_tiles(r, t0, gridDim.x), with no cap on the round count (grid 1: 128 rounds
+    of one tile)."""
     t0, sizes = 0, []
     while t0 < K_REFINE_MAX_TILES:
         t = final_round_tiles(len(sizes), t0, grid)

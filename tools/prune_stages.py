@@ -5,8 +5,6 @@ stages' switches in one process, then bench.py per setting, alternated.
 
 A setting is a value of B200BO_PRUNE_REFINE, or switches joined by '+' (names without B200BO_PRUNE_), e.g. the two
 fp32 Gram bound kernels:  --settings GRAM_KERNEL=ring,GRAM_KERNEL=reg
-or the units of the level and the final rounds on all 128 columns against column groups of 32:
---settings COLSPLIT=0,COLSPLIT=1
 
 Legs as in tools/prune_ab.py (argmin + top-10; Matern-2.5, alpha 1e-6, normalize_y).  Per leg and setting:
 b200bo_last_kernel_ms mean (min-max), the stage split of b200bo_last_prune_stage_ms (bound pass, sort, lead, refine
@@ -32,7 +30,7 @@ from predict_pipe_ab import Sampler, card  # noqa: E402
 from prune_ab import ALPHA, K, LEGS, XI  # noqa: E402
 
 STAGES = ("bound", "sort", "lead", "refine", "final", "tiles")
-SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_GRAM_KERNEL", "B200BO_PRUNE_COLSPLIT")
+SWITCHES = ("B200BO_PRUNE_REFINE", "B200BO_PRUNE_GRAM_KERNEL")
 
 
 def setting_env(s):
